@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """Benchmark of the distributed sigmoid (SigLIP) loss hot path (BASELINE.json metric).
 
-    python bench.py --gpus 1 --steps 20 --warmup 5                 # this repo's sm_100a path
-    torchrun --nproc-per-node N ... bench.py --gpus N ...          # one rank per GPU (driver launches this)
+    python bench.py --gpus 1 --steps 20 --warmup 5                 # this repo's sm_90a path
+    torchrun --nproc-per-node N ... bench.py --gpus N ...          # one rank per GPU
+    python bench.py --gpus 1 --steps 20 --warmup 5 --dump-outputs DIR   # also save what the last timed step computed
     python bench.py --impl reference --gpus 1 --steps 20 --warmup 5  # the UNMODIFIED reference on the host cores
     python bench.py --batch 4096 --dim 768                         # another BASELINE.json config (configs[1])
 
@@ -32,7 +33,8 @@ if ROOT not in sys.path:
 
 METRIC = "image-text pairs/sec"
 UNIT = "pairs/s"
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
+DUMP_MATRIX_BYTES = 24 << 20   # per [B, D] output in --dump-outputs: larger ones are saved as a seeded row sample
 
 
 def _peaks():
@@ -42,11 +44,11 @@ def _peaks():
             p = json.load(f)
         return float(p["bf16_tflops_sustained"]), "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)"
     except Exception:
-        return 1400.0, "B200_PROFILING.md fallback, sustained ~1.4 PFLOP/s (of fallback)"
+        return 989.0, "H100 SXM data sheet, dense BF16 at 700 W (of data sheet)"
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md) through NVML from a Python
+    """SM clock / throttle reasons sampled DURING the timed region through NVML from a Python
     thread every ~5 ms (the C calls release the GIL)."""
 
     def __init__(self, gpu_index: int, period_s: float = 0.005):
@@ -107,8 +109,8 @@ class ClockSampler:
         reasons = sorted(k for k, bit in names.items() if (mask & bit) and k != "gpu_idle")
         return {"sm_mhz": clocks[len(clocks) // 2] if clocks else None, "sm_max_mhz": self.max_mhz,
                 "reasons": reasons, "reasons_mask": hex(mask), "samples": len(sel),
-                "note": "sustained state by construction (warm-up until the step time is stable): a power-capped B200 "
-                        "runs tensor work at 1.2-1.4 GHz; sw_power_cap is the expected reason"}
+                "note": "sustained state by construction (warm-up until the step time is stable): under sustained "
+                        "tensor load a power-capped GPU lowers its clocks; sw_power_cap is the expected reason"}
 
 
 def _nvlink_counters(gpu_index: int):
@@ -168,10 +170,10 @@ def synth(rank: int, B: int, D: int):
 
 
 # ------------------------------------------------------------------------------------------------------
-# Reference arm: the UNMODIFIED reference (baseline/_ref, placed by tools/fetch_ref.py) on the host cores
+# Reference arm: the UNMODIFIED reference (oracle/_ref, placed by oracle/fetch_ref.py) on the host cores
 # ------------------------------------------------------------------------------------------------------
 def _load_reference_module():
-    """(DDPSigmoidLoss class of the unmodified reference, "reference") or (None, "port") when baseline/_ref is absent."""
+    """(DDPSigmoidLoss class of the unmodified reference, "reference") or (None, "port") when oracle/_ref is absent."""
     if os.path.exists(os.path.join(REF_DIR, "distributed_sigmoid_loss.py")):
         if REF_DIR not in sys.path:
             sys.path.insert(0, REF_DIR)
@@ -185,7 +187,7 @@ def cpu_reference_times(B: int, D: int, steps: int, warmup: int):
     """Times `DDPSigmoidLoss(B).forward(img, txt)` + `.backward()` of the unmodified reference
     (distributed_sigmoid_loss.py:17-48) under a world_size-1 gloo group, fp32 on the bf16-rounded bench inputs, all
     host threads, FULL per-rank chunk (B x B logits). Falls back to the oracle's op-for-op port (kind "port") only if
-    baseline/_ref is missing. Returns (seconds per step, threads, kind)."""
+    oracle/_ref is missing. Returns (seconds per step, threads, kind)."""
     import torch
     import torch.distributed as dist
 
@@ -256,9 +258,9 @@ def run_reference(args):
     # At N>1 the job is W ranks x W chunks of that unit on this one host (W x 8 GiB of B x B intermediates per rank do
     # not fit and per-chunk cost is linear in W, BASELINE.md §4): whole-job rate = W*B / (W*W * t_chunk), extrapolated.
     value = W * B / (W * W * sec)
-    what = ("unmodified reference DDPSigmoidLoss.forward + .backward() (baseline/_ref/distributed_sigmoid_loss.py:8-48, "
+    what = ("unmodified reference DDPSigmoidLoss.forward + .backward() (oracle/_ref/distributed_sigmoid_loss.py:8-48, "
             "world_size-1 gloo group)" if kind == "reference" else
-            "oracle.port_step, the reference's op sequence (baseline/_ref missing: run tools/fetch_ref.py)")
+            "oracle.port_step, the reference's op sequence (oracle/_ref missing: run oracle/fetch_ref.py)")
     sample = (f"{what}; fp32 on the bf16-rounded bench inputs; every timed step scores the FULL {B} x {B} chunk of rank 0 "
               f"(D={D}): {sec:.3f} s per step on {threads} host threads")
     if W > 1:
@@ -374,6 +376,23 @@ def parity_pass(rank, world, dev, cta_group, B=2048, D=768):
 # ------------------------------------------------------------------------------------------------------
 # this repo's path
 # ------------------------------------------------------------------------------------------------------
+def dump_outputs(outdir: str, arrays: dict) -> None:
+    """Writes each output as outdir/<name>.npy in float32. A [B, D] output larger than DUMP_MATRIX_BYTES is saved as
+    the rows of a fixed seeded sample (same rows for the same B, in ascending order), so that two builds can be compared
+    output for output on the same inputs within a bounded size."""
+    import numpy as np
+    import torch
+
+    os.makedirs(outdir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().float().reshape(t.shape if t.dim() > 0 else (1,))
+        if a.dim() == 2 and a.numel() * 4 > DUMP_MATRIX_BYTES:
+            k = max(1, DUMP_MATRIX_BYTES // (4 * a.shape[1]))
+            rows = torch.randperm(a.shape[0], generator=torch.Generator().manual_seed(0))[:k].sort().values
+            a = a[rows.to(a.device)]
+        np.save(os.path.join(outdir, name + ".npy"), a.cpu().numpy().astype(np.float32))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -388,7 +407,7 @@ def run_ours(args):
             raise SystemExit("--gpus N > 1 must be launched with torch.distributed.run (one rank per GPU)")
         args.gpus = world
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: the product path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs an H100: the product path has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     numa = _bind_to_gpu_numa_node(local_rank)   # pinned host buffers next to the GPU's PCIe root (matters for e2e)
@@ -427,9 +446,17 @@ def run_ours(args):
             loss = mod(img, txt)
             loss.backward()
             return loss
+        def outputs(loss):
+            return dict(loss=loss, dimg=img.grad, dtxt=txt.grad, dt_prime=mod.t_prime.grad, dbias=mod.bias.grad)
     elif args.api == "fused":   # the fused C-ABI entry siglip_fwd_bwd (BASELINE.json configs[1] "fused fwd+bwd"), bf16 gradients
+        last = [None]
+
         def step():
-            return eng.fwd_bwd(img_d, txt_d, tpt, bt, torch.bfloat16)[0]
+            last[0] = eng.fwd_bwd(img_d, txt_d, tpt, bt, torch.bfloat16)
+            return last[0][0]
+
+        def outputs(loss):
+            return dict(zip(("loss", "dimg", "dtxt", "dt_prime", "dbias"), last[0]))
     else:   # the same fused C-ABI step captured once into a CUDA graph and replayed (single rank only: the cross-rank
             # flag values of a multi-rank step are kernel parameters that advance every step)
         if world > 1:
@@ -448,6 +475,9 @@ def run_ours(args):
         def step():
             graph.replay()
             return graph_out[0]
+
+        def outputs(loss):
+            return dict(zip(("loss", "dimg", "dtxt", "dt_prime", "dbias"), graph_out))
 
     def barrier():
         if world > 1:
@@ -475,9 +505,8 @@ def run_ours(args):
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return float(t)
 
-    # Sustained power state at every N. A B200 under tensor load drops from its burst clocks to the power-capped state
-    # after ~50-100 ms (1.16 -> 1.33 ms per step at the headline shape; MEASURED_PEAKS.json: cuBLAS 1701.7 burst vs
-    # 1432 sustained). The first steps after the requested warm-up are reported as "burst"; the warm-up then continues
+    # Sustained power state at every N. A power-capped GPU under tensor load drops from its burst clocks to a lower
+    # sustained clock after tens of milliseconds. The first steps after the requested warm-up are reported as "burst"; the warm-up then continues
     # in ~25 ms batches until (a) at least --sustain-ms of GPU time have passed AND (b) the step time of three
     # consecutive batches agrees within 1.5 % (the clocks have settled), at most 4 s.
     burst_ms = timed_batch(args.steps) / args.steps
@@ -507,6 +536,8 @@ def run_ours(args):
     e1.record()
     barrier()
     last_sample = sampler.mark()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, outputs(loss))   # after the timed region: the copies are not timed
     nvl1 = _nvlink_counters(local_rank) if (rank == 0 and world > 1) else None
     my_clock = sampler.median_since(first_sample)
     ms_mine = e0.elapsed_time(e1)
@@ -645,16 +676,7 @@ def run_ours(args):
         grad_avg_ms = grad_ms / max(grad_n, 1)
         loss_avg_ms = loss_ms / max(loss_n, 1)
         achieved = flops_grad / (grad_avg_ms * 1e-3) / 1e12 if grad_n else None
-        traffic, traffic_src = None, None
-        prof = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-        if os.path.exists(prof) and (B, D) == (16384, 1024):
-            try:
-                with open(prof) as f:
-                    tj = json.load(f)
-                traffic = tj.get("grad_kernel_dram_bytes_per_launch")
-                traffic_src = tj.get("source", "profiles/roofline_traffic.json (one ncu --set full capture, not measured in this run)")
-            except Exception:
-                traffic = None
+        traffic, traffic_src = None, "not measured (DRAM bytes per launch need a profiler capture)"
 
         def stats(col):
             v = sorted(r[col] for r in per_rank)
@@ -674,8 +696,8 @@ def run_ours(args):
                                        "tflops_per_gpu across N (FLOP-normalised efficiency = W*t(1)/t(W))",
                        "power_state": f"sustained: warm-up extended to {n_warm} steps ({warm_ms:.0f} ms of measured GPU time, "
                                       "until three consecutive ~25 ms batches agree within 1.5 %) before the timed steps, at every N",
-                       "l2": "no explicit flush: each step streams >1 GiB (16-bit sigma operand) through the 126 MB L2"
-                             if B >= 8192 else "no explicit flush: inputs + sigma operand of a step fit the 126 MB L2 at this "
+                       "l2": "no explicit flush: each step streams >1 GiB (16-bit sigma operand) through the 50 MB L2"
+                             if B >= 8192 else "no explicit flush: inputs + sigma operand of a step fit the 50 MB L2 at this "
                                                "shape (as they do in a training loop that calls the loss every step)",
                        "api": "DDPSigmoidLoss.forward + loss.backward() (torch autograd over the C ABI)"
                               if args.api == "module" else ("siglip_fwd_bwd (C ABI, one fused call, bf16 gradients)"
@@ -778,7 +800,7 @@ def run_ours(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20, help="timed steps of the reported value")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--batch", type=int, default=16384)
@@ -792,12 +814,17 @@ def main():
     ap.add_argument("--cta-group", type=int, default=int(os.environ.get("SIGLIP_CTA_GROUP", "2")))
     ap.add_argument("--cpu-steps", type=int, default=3, help="timed steps of the cpu_baseline leg inside the N=1 run")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (loss, dimg, dtxt, dt_prime, dbias of rank 0) as "
+                         "DIR/<name>.npy in float32; the [B, D] gradients as a seeded row sample when large")
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--no-scaling-diag", action="store_true")
     ap.add_argument("--clock-period-ms", type=float, default=5.0, help="NVML clock / throttle-reason sampling period")
     ap.add_argument("--sustain-ms", type=float, default=600.0,
                     help="minimum GPU time of the warm-up (power-capped sustained clocks at every N)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs saves what this repo's timed path computed; it does not apply to --impl reference")
     if args.impl == "reference":
         return run_reference(args)
     return run_ours(args)

@@ -2,7 +2,7 @@
 
 The shared library is built in-tree (``make -C distributed_sigmoid_loss_b200/csrc`` or
 ``__graft_entry__.build()``) and loaded from the package directory. There is no fallback: if the
-library is missing or no sm_100 device is visible, the product path raises.
+library is missing or no sm_90 device is visible, the product path raises.
 """
 from __future__ import annotations
 
@@ -92,7 +92,7 @@ class SiglipError(RuntimeError):
 
 
 def build(force: bool = False) -> str:
-    """Compile the CUDA extension for sm_100a with nvcc (cross-compiles without a GPU)."""
+    """Compile the CUDA extension for sm_90a with nvcc (cross-compiles without a GPU)."""
     if force and os.path.exists(LIB_PATH):
         os.remove(LIB_PATH)
     subprocess.run(["make", "-C", CSRC_DIR], check=True, capture_output=True, text=True)

@@ -1,5 +1,4 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM),
-// cluster addressing. Nothing here is library code; every wrapper is one PTX instruction (or a bounded
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma, cluster addressing. Nothing here is library code; every wrapper is one PTX instruction (or a bounded
 // spin around one) so that the kernels in siglip_kernels.cu read as the hardware sequence they are.
 #pragma once
 #include <cuda.h>
@@ -73,16 +72,10 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t byt
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// arrive on a barrier that lives in another CTA of the cluster (address from mapa_shared)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
-}
-// Hand-back of a TMEM accumulator stage: the arrive only has to follow this warp's tcgen05.ld's (tcgen05.wait::ld +
-// tcgen05.fence::before_thread_sync make that so), it publishes no memory writes — a relaxed arrive avoids the
-// MEMBAR / ERRBAR sequence a release at cluster scope costs per warp and tile (ncu: 9 % of the loss kernel's stalls).
-__device__ __forceinline__ void mbar_arrive_relaxed(uint32_t bar) {
-  asm volatile("mbarrier.arrive.relaxed.cta.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
+// Arrive on a barrier that lives in another CTA of the cluster (address from mapa_shared).
+// Hand-back of a shared-memory stage that was read only by wgmma (async proxy, complete after wgmma.wait_group): the
+// arrive has to follow that wait in program order and publishes no memory writes, so it needs no release fence — a
+// release at cluster scope costs two full fences (MEMBAR.ALL.CTA + MEMBAR.ALL.GPU) per warp and k block.
 __device__ __forceinline__ void mbar_arrive_cluster_relaxed(uint32_t cluster_bar) {
   asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
 }
@@ -177,22 +170,12 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
 }
 
 // 2-D tiled load global -> shared, completion (bytes) signalled on `bar`.
-// kCG == 2: the barrier may live in the peer CTA of the pair (shared::cluster address).
-template <int kCG>
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint32_t bar, uint32_t dst, int c0, int c1) {
-  if constexpr (kCG == 1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
-        : "memory");
-  } else {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
-        : "memory");
-  }
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
+      : "memory");
 }
 
 // L2 eviction-priority policies for streamed vs re-used operands (createpolicy; whole line range, fraction 1.0).
@@ -213,22 +196,13 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last() {
 }
 
 // tma_load_2d with an L2 cache policy for the lines it touches.
-template <int kCG>
 __device__ __forceinline__ void tma_load_2d_hint(const CUtensorMap* m, uint32_t bar, uint32_t dst, int c0, int c1,
                                                  uint64_t policy) {
-  if constexpr (kCG == 1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "l"(policy)
-        : "memory");
-  } else {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "l"(policy)
-        : "memory");
-  }
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "l"(policy)
+      : "memory");
 }
 
 // Same load, delivered to the same shared-memory offset of every CTA in `cta_mask` of the cluster; each
@@ -242,203 +216,78 @@ __device__ __forceinline__ void tma_load_2d_mcast(const CUtensorMap* m, uint32_t
       : "memory");
 }
 
-// cta_group::2 flavour of the multicast load (2x2 clusters: two MMA pairs share an operand tile). `bar` is THIS CTA's
-// barrier offset with the pair bit cleared (bit 24 of a shared::cluster address selects the CTA within an MMA pair):
-// in every destination CTA the complete_tx lands on the barrier of that destination's pair LEADER.
-__device__ __forceinline__ void tma_load_2d_mcast_2sm(const CUtensorMap* m, uint32_t bar, uint32_t dst, int c0, int c1,
-                                                      uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%4, %5}], [%2], %3;" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & 0xFEFFFFFFu), "h"(cta_mask), "r"(c0), "r"(c1)
-      : "memory");
+// ---------------------------------------------------------------------------------------------
+// wgmma (sm_90a warpgroup MMA): D[64 x 128, fp32 registers] (+)= A[smem desc] * B[smem desc]
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kN>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kN) : "memory");
 }
+// Keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs.
+__device__ __forceinline__ void acc_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+
+#define SIGLIP_WGMMA_ACC64                                                                                         \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
+  "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "    \
+  "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define SIGLIP_WGMMA_OUT64(d)                                                                                      \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),        \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),         \
+      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),        \
+      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),        \
+      "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),        \
+      "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),        \
+      "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),        \
+      "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+
+// Operand type of the MMA: 0 bf16 x bf16, 1 fp16 x fp16 (K = 16 per instruction), 2 e4m3 x e4m3 (K = 32, K-major only).
+// kTA / kTB: 1 = the operand is MN-major in shared memory (transposed), 0 = K-major.
+template <int kType, int kTA, int kTB>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  if constexpr (kType == 0) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " SIGLIP_WGMMA_ACC64 ", %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : SIGLIP_WGMMA_OUT64(d)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTA), "n"(kTB));
+  } else if constexpr (kType == 1) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " SIGLIP_WGMMA_ACC64 ", %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : SIGLIP_WGMMA_OUT64(d)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTA), "n"(kTB));
+  } else {
+    static_assert(kType != 2 || (kTA == 0 && kTB == 0), "8-bit wgmma operands are K-major");
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 " SIGLIP_WGMMA_ACC64 ", %64, %65, p, 1, 1;\n\t}"
+        : SIGLIP_WGMMA_OUT64(d)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+  }
+}
+#undef SIGLIP_WGMMA_ACC64
+#undef SIGLIP_WGMMA_OUT64
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, TMEM loads
-// ---------------------------------------------------------------------------------------------
-template <int kCG>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  if constexpr (kCG == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int kCG>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (kCG == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  } else {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  }
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread.
-template <int kCG>
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  if constexpr (kCG == 1) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-
-// Same with 8-bit operands (kind::f8f6f4; here e4m3 x e4m3 -> fp32): K = 32 per instruction. Measurement path only.
-template <int kCG>
-__device__ __forceinline__ void umma_f8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  if constexpr (kCG == 1) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-
-// All previously issued MMAs of this thread -> arrive(1) on `bar` when they retire.
-// kCG == 2: arrive on the same barrier offset in both CTAs of the pair.
-template <int kCG>
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if constexpr (kCG == 1) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-                 : "memory");
-  } else {
-    const uint16_t mask = 0x3;
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            bar),
-        "h"(mask)
-        : "memory");
-  }
-}
-
-// cta_group::1 commit whose arrive is delivered to the same barrier offset in every CTA of `cta_mask`
-// (frees a multicast-fed smem stage in all CTAs that write into it).
-__device__ __forceinline__ void umma_commit_mcast(uint32_t bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// cta_group::2 commit with an explicit cluster CTA mask (2x2 clusters: a stage is released in all four CTAs, an
-// accumulator is published to the two CTAs of one pair)
-__device__ __forceinline__ void umma_commit_2sm_mask(uint32_t bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (one row per thread).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------------------------------------
-// Descriptors (bit layouts: PTX ISA "tcgen05 shared memory descriptor" / "instruction descriptor")
-// ---------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128-byte swizzle, sm_100 version field = 1.
+// Shared-memory matrix descriptor of wgmma (PTX ISA "Matrix Descriptor Format", sm_90), 128-byte swizzle:
 //   [0,14)  start address >> 4      [16,30) leading byte offset >> 4
-//   [32,46) stride byte offset >> 4 [46,48) version = 1           [61,64) layout type (2 = SWIZZLE_128B)
+//   [32,46) stride byte offset >> 4 [62,64) swizzle mode (1 = 128B)
+// K-major: 8-row groups SBO = 1024 B apart (LBO unused). MN-major: 64-element MN blocks LBO apart, 8-k groups SBO apart.
+// ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 accumulate.
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt (1 = bf16)  [10,13) B fmt (1 = bf16)
-//   [15] A major (1 = MN)  [16] B major (1 = MN)    [17,23) N >> 3          [24,29) M >> 4
-//   ab_f16: both operands hold IEEE fp16 instead of bf16 (mixing fp16 with bf16 in one MMA faults on sm_100a)
-//   ab_f16 == 2: kind::f8f6f4 with e4m3 operands (format code 0 in both fields)
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int m, int n, int a_mn_major, int b_mn_major,
-                                                       int ab_f16 = 0) {
-  return (1u << 4) | ((ab_f16 ? 0u : 1u) << 7) | ((ab_f16 ? 0u : 1u) << 10) |
-         (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
-}
-
-// ---------------------------------------------------------------------------------------------
-// Packed fp32x2 arithmetic (sm_100: FFMA2 / FMUL2 / FADD2 — two fp32 lanes per instruction on the FMA pipe)
-// ---------------------------------------------------------------------------------------------
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pack2(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(f32x2 v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
 // ---------------------------------------------------------------------------------------------
 // MUFU approximations (each one SFU instruction)
 // ---------------------------------------------------------------------------------------------
-// three-input maximum (FMNMX3 on sm_100)
-__device__ __forceinline__ float max3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

@@ -1,4 +1,4 @@
-// C ABI (include/siglip_b200.h) over the sm_100a kernels: context + workspaces, TMA descriptor encoding,
+// C ABI (include/siglip_b200.h) over the sm_90a kernels: context + workspaces, TMA descriptor encoding,
 // the per-step chunk schedule, CUDA-IPC peer bootstrap. Host-side only; no torch types anywhere.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -107,10 +107,12 @@ int encode_u8_kmajor(CUtensorMap* m, const void* base, int rows, int K, long lon
   return 0;
 }
 
-// Operand tensor map for the mainloop. mn == 0: stored [rows][K]; mn == 1: stored [K][rows].
-int encode_operand(CUtensorMap* m, const void* base, int rows, int K, long long ld, int mn, int box_rows_kmajor) {
+// Operand tensor map for the mainloop. mn == 0: stored [rows][K], box {64 k, box_rows_kmajor rows};
+// mn == 1: stored [K][rows], box {64 rows, box_k_mnmajor k}.
+int encode_operand(CUtensorMap* m, const void* base, int rows, int K, long long ld, int mn, int box_rows_kmajor,
+                   int box_k_mnmajor = 64) {
   if (!mn) return encode_bf16_2d(m, base, (uint64_t)K, (uint64_t)rows, (uint64_t)ld, 64, (uint32_t)box_rows_kmajor);
-  return encode_bf16_2d(m, base, (uint64_t)rows, (uint64_t)K, (uint64_t)ld, 64, 64);
+  return encode_bf16_2d(m, base, (uint64_t)rows, (uint64_t)K, (uint64_t)ld, 64, (uint32_t)box_k_mnmajor);
 }
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
@@ -165,17 +167,14 @@ struct siglip_ctx {
   int stages_loss = 0, stages_grad = 0;  // 0 = kernel default
   int mcast = 1;                         // 2: vertically adjacent tiles share the B tile by TMA multicast
   int grad_bf16 = 0;                     // dimg / dtxt outputs are bf16 instead of fp32
-  int epi_sleep_grad_ns = 0;             // back-off of the gradient kernel's epilogue warps while a K loop runs
-  int epi_sleep_loss_ns = 0;
   int sync_scalar_grads = 0;             // backward returns the mean over ranks of dt' / dbias
   int bidir = 0;                         // visiting order of the text chunks: r, r+1, r-1, r+2, r-2, ...
-  int grad_tile_n = 0;                   // column-tile width of the gradient kernel: 0 = choose, 128, 256
   int input_f16 = 0;                     // img / txt are fp16(x * kXScale) instead of bf16 (fp32-input path)
   int saved_f16 = 0;                     // format of the embeddings of the forward saved for backward
   int tprime_f64 = 0;                    // t_prime / dt_prime pointers of forward / backward / fwd_bwd are fp64 device scalars
-  int pdl = 1;                           // programmatic dependent launch of the tcgen05 kernels (set-up overlaps the previous tail)
-  int inkernel_sync = 1;                 // fused step: flags waited for / raised inside the tcgen05 kernels (0: helper launches)
-  int split_k = 0;                       // gradient kernel: 0 = off (default: measured no gain, profiles/r02_notes.md), -1 = split a
+  int pdl = 1;                           // programmatic dependent launch of the wgmma kernels (set-up overlaps the previous tail)
+  int inkernel_sync = 1;                 // fused step: flags waited for / raised inside the wgmma kernels (0: helper launches)
+  int split_k = 0;                       // gradient kernel: 0 = off (default), -1 = split a
                                          // ragged last wave automatically, S >= 2 = at most S slices
   long long peer_timeout_ms = 600000;    // bound of every wait on a peer (10 min: a peer may be saving a checkpoint)
   int aux_trace_on = 0;
@@ -295,11 +294,11 @@ int ensure_g(siglip_ctx* c, int i) {
 }
 
 // Workspace of the gradient kernel's split-K (fp32 partial accumulators of the tiles of a ragged last wave): fewer than
-// one 256 KiB partial per SM pair can ever be outstanding.
+// one 64 KiB partial per SM can ever be outstanding.
 constexpr int kSplitKMaxTiles = 160;
 int ensure_splitk(siglip_ctx* c) {
   if (c->splitk_ws != nullptr) return 0;
-  const size_t bytes = static_cast<size_t>(c->num_sms + 2) * 128 * 256 * sizeof(float);
+  const size_t bytes = static_cast<size_t>(c->num_sms + 2) * 128 * siglip::kTileCols * sizeof(float);
   CK(cudaMalloc(reinterpret_cast<void**>(&c->splitk_ws), bytes));
   CK(cudaMalloc(reinterpret_cast<void**>(&c->splitk_counters), 2 * kSplitKMaxTiles * sizeof(unsigned int)));
   CK(cudaMemset(c->splitk_counters, 0, 2 * kSplitKMaxTiles * sizeof(unsigned int)));
@@ -353,23 +352,23 @@ struct FinJob {   // last chunk of a forward: the loss kernel's last CTA writes 
   float* dbias = nullptr;
 };
 
-// The loss kernel over one text chunk (Bn rows, owner's batch): S = img @ txt_c^T on tcgen05, fused
+// The loss kernel over one text chunk (Bn rows, owner's batch): S = img @ txt_c^T on wgmma, fused
 // scale/bias/log-sigmoid/reduce. save: also write the sigma operand G[gi] (+ g_diag on the own chunk); the fp16 copies
 // the gradient kernel needs are auxiliary jobs built by the caller.
 int run_loss_chunk(siglip_ctx* c, int gi, bool own, bool first, const void* img, const __nv_bfloat16* txt_c, int Bn,
                    const float* t_prime, const float* bias, bool save, const AuxList& aux, const FinJob* fin,
                    const EndSignal& end, cudaStream_t st) {
   const int cg = c->cta_group;
-  const int tile_m = 128 * cg;
   int rc;
   if ((rc = ensure_g(c, save ? gi : 0))) return rc;
   __nv_bfloat16* G = c->G[save ? gi : 0];
   CUtensorMap tmA, tmB, tmG;
   if ((rc = encode_operand(&tmA, img, c->B, c->D, c->D, 0, 128))) return rc;
   const int mc = c->mcast;
-  if ((rc = encode_operand(&tmB, txt_c, Bn, c->D, c->D, 0, 256 / (cg * mc)))) return rc;
-  // store map of the sigma operand: [B, Bn] inside the padded [Bp, Bp] buffer, one 32x32 slab per TMA store
-  if ((rc = encode_bf16_2d(&tmG, G, (uint64_t)Bn, (uint64_t)c->B, (uint64_t)c->Bp, 32, 32,
+  if ((rc = encode_operand(&tmB, txt_c, Bn, c->D, c->D, 0, siglip::b_box_rows_kmajor(siglip::cluster_size(cg, mc)))))
+    return rc;
+  // store map of the sigma operand: [B, Bn] inside the padded [Bp, Bp] buffer, one 16-row x 32-column slab per TMA store
+  if ((rc = encode_bf16_2d(&tmG, G, (uint64_t)Bn, (uint64_t)c->B, (uint64_t)c->Bp, 32, 16,
                            CU_TENSOR_MAP_SWIZZLE_64B)))
     return rc;
   KernelParams p;
@@ -381,8 +380,6 @@ int run_loss_chunk(siglip_ctx* c, int gi, bool own, bool first, const void* img,
   p.prob[0].M = c->B;
   p.prob[0].N = Bn;
   p.prob[0].K = c->D;
-  p.prob[0].tiles_m = ceil_div(c->B, tile_m);
-  p.prob[0].tiles_n = ceil_div(Bn, 256);
   p.t_prime = t_prime;
   p.bias = bias;
   p.inv_b = 1.0f / static_cast<float>(c->B);
@@ -401,7 +398,6 @@ int run_loss_chunk(siglip_ctx* c, int gi, bool own, bool first, const void* img,
     p.fin_dbias = fin->dbias;
   }
   p.dbg = c->dbg_dev;
-  p.epi_sleep_ns = static_cast<unsigned int>(c->epi_sleep_loss_ns);
   if (save && c->dbg_no_gstore) p.store_g = 0;  // timing experiments only (wrong gradients)
   apply_aux(c, p, aux, end);
   unsigned long long* wstats = nullptr;
@@ -418,17 +414,16 @@ int run_loss_chunk(siglip_ctx* c, int gi, bool own, bool first, const void* img,
     CK(cudaStreamSynchronize(st));
     std::vector<unsigned long long> h(8 * 256);
     CK(cudaMemcpy(h.data(), wstats, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    double s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    int nmma = 0, nall = 0;
+    // slots written by the kernel: [0] producer empty-wait, [1] consumer thread 0 full-wait, [3] its loop cycles
+    double s[4] = {0, 0, 0, 0};
+    int nall = 0;
     for (int b = 0; b < 256; ++b) {
-      if (h[8 * b + 7]) nall++;
-      if (h[8 * b + 3]) nmma++;
-      for (int j = 0; j < 8; ++j) s[j] += static_cast<double>(h[8 * b + j]);
+      if (h[8 * b + 3]) nall++;
+      for (int j = 0; j < 4; ++j) s[j] += static_cast<double>(h[8 * b + j]);
     }
-    printf("[loss waitstats] producer empty-wait %.0f cyc/CTA | MMA (%d issuers): loop %.0f cyc, full-wait %.1f%%, "
-           "tmem-wait (epilogue not done) %.1f%% | epilogue warp 0 (%d CTAs): loop %.0f cyc, waiting for an accumulator %.1f%%\n",
-           s[0] / (nall ? nall : 1), nmma, s[3] / (nmma ? nmma : 1), 100.0 * s[1] / (s[3] > 0 ? s[3] : 1),
-           100.0 * s[2] / (s[3] > 0 ? s[3] : 1), nall, s[7] / (nall ? nall : 1), 100.0 * s[6] / (s[7] > 0 ? s[7] : 1));
+    printf("[loss waitstats] %d CTAs: producer empty-wait %.0f cyc/CTA | consumer thread 0: loop %.0f cyc/CTA, "
+           "waiting for operands %.1f%%\n",
+           nall, s[0] / (nall ? nall : 1), s[3] / (nall ? nall : 1), 100.0 * s[1] / (s[3] > 0 ? s[3] : 1));
     fflush(stdout);
     cudaFree(wstats);
   }
@@ -474,41 +469,20 @@ int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_
                    const float* t_prime, const float* grad_out, const GradOut& o, const AuxList& aux,
                    const EndSignal& end, cudaStream_t st) {
   const int cg = c->cta_group;
-  const int tile_m = 128 * cg;
+  const int bk = siglip::b_box_k_mnmajor(siglip::cluster_size(cg, c->mcast));
   CUtensorMap tmA0, tmB0, tmA1, tmB1;
   int rc;
   if (c->G[gi] == nullptr) return fail(SIGLIP_ERR_STATE, "gradient kernel without a saved sigma operand");
   if ((rc = encode_operand(&tmA0, c->G[gi], c->B, Bn, c->Bp, 0, 128))) return rc;
-  if ((rc = encode_operand(&tmB0, c->txt16[gi], c->D, Bn, c->D, 1, 0))) return rc;
+  if ((rc = encode_operand(&tmB0, c->txt16[gi], c->D, Bn, c->D, 1, 0, bk))) return rc;
   if ((rc = encode_operand(&tmA1, c->G[gi], Bn, c->B, c->Bp, 1, 0))) return rc;
-  if ((rc = encode_operand(&tmB1, c->img16, c->D, c->B, c->D, 1, 0))) return rc;
+  if ((rc = encode_operand(&tmB1, c->img16, c->D, c->B, c->D, 1, 0, bk))) return rc;
   KernelParams p;
   memset(&p, 0, sizeof(p));
   p.nprob = 2;
-  const int tiles_m0 = ceil_div(c->B, tile_m), tiles_m1 = ceil_div(Bn, tile_m);
-  // Column-tile width: 256, or 128 when that fills the waves of the persistent grid better (small B: B = 4096, D = 768
-  // is 96 tiles of 256 columns on 74 SM pairs = 2 waves for 1.3 waves of work, but 3 half-waves with 128 columns).
-  // A narrow tile streams the same sigma panel for half the flops and becomes L2->SM bound: it costs 0.66-0.70 of a
-  // full tile, measured (tools/tile_width_ab.py), so it pays only when the 256-wide grid leaves most of a wave empty.
-  int tile_n = c->grad_tile_n;
-  const long long units = c->num_sms / cg;
-  if (tile_n == 0) {
-    auto cost = [&](int tn) {   // waves x average tile cost (a 256-wide grid already runs a short last column as 128)
-      const long long cols = ceil_div(c->D, tn);
-      const int rem = c->D - static_cast<int>(cols - 1) * tn;
-      const double row_cost = (tn == 128) ? 0.70 * cols : (cols - 1) + (rem <= 128 ? 0.70 : 1.0);
-      const long long tiles = static_cast<long long>(tiles_m0 + tiles_m1) * cols;
-      return static_cast<double>((tiles + units - 1) / units) * row_cost / static_cast<double>(cols);
-    };
-    tile_n = (c->mcast == 1 && cost(128) < 0.97 * cost(256)) ? 128 : 256;
-    if (c->split_k != 0 && c->mcast == 1) tile_n = 256;   // split-K (when asked for) evens out the last wave instead
-  }
-  if (c->mcast != 1) tile_n = 256;
   for (int i = 0; i < 2; ++i) {
     Problem& pr = p.prob[i];
     pr.N = c->D;
-    pr.tile_n = tile_n;
-    pr.tiles_n = ceil_div(c->D, tile_n);
     pr.b_mn = 1;
     pr.ab_f16 = 1;
     pr.acc_scale = 1.0f / (kGScale * kXScale);
@@ -520,7 +494,6 @@ int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_
   }
   p.prob[0].M = c->B;
   p.prob[0].K = Bn;
-  p.prob[0].tiles_m = tiles_m0;
   p.prob[0].a_mn = 0;
   p.prob[0].out = o.dimg_out;
   p.prob[0].out_bf16 = o.dimg_bf16 ? 1 : 0;
@@ -529,7 +502,6 @@ int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_
   p.prob[0].fix_mat = own ? txt_own : nullptr;
   p.prob[1].M = Bn;
   p.prob[1].K = c->B;
-  p.prob[1].tiles_m = tiles_m1;
   p.prob[1].a_mn = 1;
   p.prob[1].out = o.dtxt_out;
   p.prob[1].out_bf16 = o.dtxt_bf16 ? 1 : 0;
@@ -538,7 +510,6 @@ int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_
   p.prob[1].fix_mat = own ? reinterpret_cast<const __nv_bfloat16*>(img) : nullptr;
   p.p1_wait_flag = o.dtxt_add_flag;
   p.p1_wait_value = o.dtxt_add_value;
-  p.epi_sleep_ns = static_cast<unsigned int>(c->epi_sleep_grad_ns);
   if (o.sc_dt_prime != nullptr || o.sc_dbias != nullptr) {
     p.sc_saved = c->scalars + kSavedScalars;
     p.sc_dt_prime = o.sc_dt_prime;
@@ -955,7 +926,7 @@ void free_ctx(siglip_ctx* c);
 
 extern "C" {
 
-const char* siglip_version(void) { return "siglip_b200 0.4.0 sm_100a"; }
+const char* siglip_version(void) { return "siglip_b200 0.5.0 sm_90a"; }
 
 const char* siglip_last_error(void) { return g_last_error.c_str(); }
 
@@ -968,7 +939,7 @@ int siglip_device_count(void) {
   int ok = 0;
   for (int i = 0; i < n; ++i) {
     int major = 0;
-    if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 10) ok++;
+    if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 9) ok++;
   }
   return ok;
 }
@@ -992,7 +963,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   if (device < 0 || device >= ndev) return fail(SIGLIP_ERR_INVALID, "device ordinal out of range");
   int major = 0;
   CK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-  if (major != 10) return fail(SIGLIP_ERR_NO_DEVICE, "device is not compute capability 10.x (B200, sm_100a required)");
+  if (major != 9) return fail(SIGLIP_ERR_NO_DEVICE, "device is not compute capability 9.x (H100, sm_90a required)");
   CK(cudaSetDevice(device));
   siglip_ctx* c = new siglip_ctx();
   // every failure below releases what was allocated so far (the caller never sees a half-built context)
@@ -1098,15 +1069,11 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
       if (value != 1 && value != 2) return fail(SIGLIP_ERR_INVALID, "mcast must be 1 or 2");
       c->mcast = value;
       return 0;
-    case SIGLIP_OPT_EPI_SLEEP_GRAD_NS:
-      c->epi_sleep_grad_ns = value < 0 ? 0 : value;
-      return 0;
+    case SIGLIP_OPT_EPI_SLEEP_GRAD_NS:   // accepted for existing callers; no effect on sm_90a (see the header)
     case SIGLIP_OPT_EPI_SLEEP_LOSS_NS:
-      c->epi_sleep_loss_ns = value < 0 ? 0 : value;
       return 0;
-    case SIGLIP_OPT_GRAD_TILE_N:
+    case SIGLIP_OPT_GRAD_TILE_N:         // accepted for existing callers; every column tile is 128 wide on sm_90a
       if (value != 0 && value != 128 && value != 256) return fail(SIGLIP_ERR_INVALID, "grad_tile_n must be 0, 128 or 256");
-      c->grad_tile_n = value;
       return 0;
     case SIGLIP_OPT_INPUT_F16:
       c->input_f16 = value ? 1 : 0;
@@ -1119,10 +1086,9 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
       c->sync_scalar_grads = value ? 1 : 0;
       return 0;
     case SIGLIP_OPT_STAGES_LOSS:
-      c->stages_loss = value;
-      return 0;
     case SIGLIP_OPT_STAGES_GRAD:
-      c->stages_grad = value;
+      if (value != 0 && value != 4 && value != 6) return fail(SIGLIP_ERR_INVALID, "pipeline stages must be 0 (default), 4 or 6");
+      (option == SIGLIP_OPT_STAGES_LOSS ? c->stages_loss : c->stages_grad) = value;
       return 0;
     case SIGLIP_OPT_KERNEL_TIMING:
       c->kernel_timing = value ? 1 : 0;
@@ -1585,23 +1551,26 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
   if (A == nullptr || Bm == nullptr || C == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (cta_group != 1 && cta_group != 2) return fail(SIGLIP_ERR_INVALID, "cta_group must be 1 or 2");
   if (M < 1 || N < 8 || K < 1 || (N % 8) != 0) return fail(SIGLIP_ERR_INVALID, "need N % 8 == 0");
-  if (siglip_device_count() == 0) return fail(SIGLIP_ERR_NO_DEVICE, "no sm_100 device; no CPU fallback");
+  if (siglip_device_count() == 0) return fail(SIGLIP_ERR_NO_DEVICE, "no sm_90 device; no CPU fallback");
   CK(cudaSetDevice(device));
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   int num_sms = 0;
   CK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
   CUtensorMap tmA, tmB;
   int rc;
-  const bool fp8 = getenv("SIGLIP_DEBUG_AB_FP8") != nullptr;   // A, B hold e4m3 bytes, K-major (kind::f8f6f4)
+  const bool fp8 = getenv("SIGLIP_DEBUG_AB_FP8") != nullptr;   // A, B hold e4m3 bytes, K-major
   const char* env_mc = getenv("SIGLIP_DEBUG_MCAST");
   const int mcast = env_mc ? atoi(env_mc) : 1;
+  if (mcast != 1 && mcast != 2) return fail(SIGLIP_ERR_INVALID, "SIGLIP_DEBUG_MCAST must be 1 or 2");
   if (fp8) {
     if (a_mn || b_mn || mcast != 1) return fail(SIGLIP_ERR_INVALID, "the fp8 measurement path is K-major, no multicast");
     if ((rc = encode_u8_kmajor(&tmA, A, M, K, lda, 128))) return rc;
-    if ((rc = encode_u8_kmajor(&tmB, Bm, N, K, ldb, 256 / cta_group))) return rc;
+    if ((rc = encode_u8_kmajor(&tmB, Bm, N, K, ldb, siglip::b_box_rows_kmajor(cta_group)))) return rc;
   } else {
+    const int cs = siglip::cluster_size(cta_group, mcast);
     if ((rc = encode_operand(&tmA, A, M, K, lda, a_mn, 128))) return rc;
-    if ((rc = encode_operand(&tmB, Bm, N, K, ldb, b_mn, 256 / (cta_group * mcast)))) return rc;
+    if ((rc = encode_operand(&tmB, Bm, N, K, ldb, b_mn, siglip::b_box_rows_kmajor(cs), siglip::b_box_k_mnmajor(cs))))
+      return rc;
   }
   float* zero = nullptr;  // t' = 0 -> scale exp(0) * 1 = 1
   CK(cudaMalloc(reinterpret_cast<void**>(&zero), sizeof(float)));
@@ -1617,8 +1586,6 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
   p.prob[0].M = M;
   p.prob[0].N = N;
   p.prob[0].K = K;
-  p.prob[0].tiles_m = ceil_div(M, 128 * cta_group);
-  p.prob[0].tiles_n = ceil_div(N, 256);
   p.prob[0].a_mn = a_mn ? 1 : 0;
   p.prob[0].b_mn = b_mn ? 1 : 0;
   p.prob[0].ab_f16 = fp8 ? 2 : (getenv("SIGLIP_DEBUG_AB_F16") ? 1 : 0);
@@ -1635,15 +1602,14 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
   unsigned long long* wstats = nullptr;
   if (getenv("SIGLIP_DEBUG_WAITSTATS")) {
     printf("[waitstats cg=%d] max co-resident clusters: %d (SMs %d)\n", cta_group,
-           siglip::query_max_active_clusters(cta_group), num_sms);
+           siglip::query_max_active_clusters(siglip::cluster_size(cta_group, mcast)), num_sms);
     CK(cudaMalloc(reinterpret_cast<void**>(&wstats), 8 * 256 * sizeof(unsigned long long)));
     CK(cudaMemsetAsync(wstats, 0, 8 * 256 * sizeof(unsigned long long), st));
     p.wait_stats = wstats;
   }
-  const char* env_sl = getenv("SIGLIP_DEBUG_EPI_SLEEP");
-  p.epi_sleep_ns = env_sl ? static_cast<unsigned int>(atoi(env_sl)) : 0u;
   const char* env_st = getenv("SIGLIP_DEBUG_STAGES");
   const int stages = env_st ? atoi(env_st) : 0;
+  if (stages != 0 && stages != 4 && stages != 6) return fail(SIGLIP_ERR_INVALID, "SIGLIP_DEBUG_STAGES must be 4 or 6");
   if (iters > 1)  // warm-up
     lrc = siglip::launch_gemm(cta_group, siglip::kModeOut, stages, mcast, &tmA, &tmB, &tmA, &tmB, &tmA, p, num_sms, st);
   cudaEventRecord(e0, st);
@@ -1661,22 +1627,16 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
   if (wstats != nullptr) {
     std::vector<unsigned long long> h(8 * 256);
     cudaMemcpy(h.data(), wstats, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-    double s[6] = {0, 0, 0, 0, 0, 0};
-    int nlead = 0, nall = 0;
+    // slots written by the kernel: [0] producer empty-wait, [1] consumer thread 0 full-wait, [3] its loop cycles
+    double s[4] = {0, 0, 0, 0};
+    int nall = 0;
     for (int b = 0; b < 256; ++b) {
-      if (h[8 * b + 0] || h[8 * b + 3]) nall++;
-      s[0] += static_cast<double>(h[8 * b + 0]);
-      if (h[8 * b + 3]) {
-        nlead++;
-        for (int j = 1; j < 6; ++j) s[j] += static_cast<double>(h[8 * b + j]);
-      }
+      if (h[8 * b + 3]) nall++;
+      for (int j = 0; j < 4; ++j) s[j] += static_cast<double>(h[8 * b + j]);
     }
-    const double tot = s[3] > 0 ? s[3] : 1;
-    printf("[waitstats cg=%d] producer empty-wait avg %.0f cyc (%d CTAs); MMA thread (%d issuers): loop %.0f cyc = "
-           "full-wait %.1f%% + tmem-wait %.1f%% + mma-issue %.1f%% + commit %.1f%% + other %.1f%%\n",
-           cta_group, s[0] / (nall ? nall : 1), nall, nlead, s[3] / (nlead ? nlead : 1), 100.0 * s[1] / tot,
-           100.0 * s[2] / tot, 100.0 * s[4] / tot, 100.0 * s[5] / tot,
-           100.0 * (s[3] - s[1] - s[2] - s[4] - s[5]) / tot);
+    printf("[waitstats cg=%d] %d CTAs: producer empty-wait %.0f cyc/CTA | consumer thread 0: loop %.0f cyc/CTA, "
+           "waiting for operands %.1f%%\n",
+           cta_group, nall, s[0] / (nall ? nall : 1), s[3] / (nall ? nall : 1), 100.0 * s[1] / (s[3] > 0 ? s[3] : 1));
     fflush(stdout);
     cudaFree(wstats);
   }

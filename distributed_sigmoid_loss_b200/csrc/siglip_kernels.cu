@@ -1,61 +1,52 @@
-// sm_100a kernels of the distributed sigmoid (SigLIP) loss hot path.
+// sm_90a kernels of the distributed sigmoid (SigLIP) loss hot path.
 //
 // What the reference does per text chunk (distributed_sigmoid_loss.py:22-33, rwightman_sigmoid_loss.py:49-66):
 //     logits = img @ txt_chunk.T * exp(t') + b ; loss = -logsigmoid(labels * logits).sum()
 // and, through autograd, two more contractions (G @ txt, G.T @ img) for the gradients.
 //
-// Here every contraction is a tile loop on the tcgen05 tensor pipe, one persistent warp-specialised kernel template:
-//   * 20 warps: 16 epilogue warps (4 per TMEM lane quarter), a TMA producer warp and an MMA warp (warp-uniform loops,
-//     one elected lane issues), 2 auxiliary warps (TMEM allocation, NVSwitch peer pulls / folds, operand conversion);
-//   * operands staged by TMA into a 128B-swizzled shared-memory ring, 2 x 256-column fp32 accumulators in TMEM so the
-//     MMA of tile n+1 overlaps the epilogue of tile n;
+// Here every contraction is a tile loop on the Hopper tensor cores (wgmma), one persistent warp-specialised kernel:
+//   * 12 warps: two consumer warpgroups (each owns 64 rows of the 128 x 128 fp32 accumulator tile in registers: it
+//     issues the wgmma's of its half and then runs the epilogue on those registers), a TMA producer warp, an idle
+//     warp that initialises the barriers, and 2 auxiliary warps (NVSwitch peer pulls / folds, operand conversion);
+//   * operands staged by TMA into a 128B-swizzled shared-memory ring guarded by full / empty mbarriers;
 //   * kModeLoss: the epilogue turns the S tile into softplus / sigma terms, reduces the three scalar sums and
 //     (training) writes the sigma tile as the scaled-fp16 operand of the gradient contractions through TMA stores —
 //     the logits never exist in HBM;
 //   * kModeOut: the epilogue scales the accumulator by grad_out * exp(t') / B, adds the fp32 positive-pair rank-1
 //     term and writes fp32 or bf16 gradients. Two problems (dimg and dtxt) share one launch so that the tile count
-//     fills the 148 SMs evenly.
-// Instantiated for cta_group::1 (128x256 tiles) and cta_group::2 (256x256 tiles per SM pair, the default), each
-// optionally with the B tile TMA-multicast across two vertically adjacent tiles of a cluster.
+//     fills the 132 SMs evenly.
+// Instantiated for clusters of 1, 2 or 4 CTAs on vertically adjacent 128-row blocks: the CTAs of a cluster compute the
+// same column tile, each fetches 1 / cluster of the common B tile and TMA-multicasts it to all of them.
 #include "siglip_kernels.cuh"
 
 #include <stdio.h>
 #include <stdlib.h>
 
-#include <type_traits>
-
 namespace siglip {
 
 namespace {
 
-constexpr int kBlockM = 128;   // accumulator rows per CTA (= TMEM lanes)
-constexpr int kTileN = 256;    // accumulator columns per tile (= UMMA N)
-constexpr int kBlockK = 64;    // 64 bf16 = one 128-byte swizzle row
-constexpr int kUmmaK = 16;
-constexpr int kNumEpiWarps = 16;                       // 4 per TMEM lane quarter -> 4 resident per SM sub-partition
-constexpr int kEpiColGroups = kNumEpiWarps / 4;        // column groups of the 256-column accumulator
-constexpr int kEpiCols = 256 / kEpiColGroups;          // columns per epilogue warp (64)
-constexpr int kSlabsPerWarp = kEpiCols / 32;           // 32-column TMEM loads per warp per tile (2)
+constexpr int kBlockM = 128;   // accumulator rows per CTA (two consumer warpgroups x 64)
+constexpr int kTileN = 128;    // accumulator columns per tile (= wgmma N)
+constexpr int kBlockK = 64;    // 64 16-bit values = one 128-byte swizzle row
+constexpr int kMmaK = 16;
+constexpr int kNumEpiWarps = 8;                        // the two consumer warpgroups
 constexpr int kProducerWarp = kNumEpiWarps;
-constexpr int kMmaWarp = kNumEpiWarps + 1;
-constexpr int kAllocWarp = kNumEpiWarps + 2;           // this warp and the next also run the optional peer pull
+constexpr int kInitWarp = kNumEpiWarps + 1;
+constexpr int kAuxWarp = kNumEpiWarps + 2;             // this warp and the next run the auxiliary jobs
 constexpr int kNumThreads = (kNumEpiWarps + 4) * 32;
-constexpr int kAccStages = 2;
-constexpr int kTmemCols = 512;
 
-constexpr int kStagingBytesPerWarp = 2048;  // one 32x32 16-bit slab, 64-byte rows, 64B-swizzled (TMA store source)
+constexpr int kStagingBytesPerWarp = 1024;  // one 16x32 16-bit slab, 64-byte rows, 64B-swizzled (TMA store source)
 
-template <int kCG, int kMode, int kStagesT>
+template <int kMode, int kStagesT>
 struct Cfg {
-  static constexpr int kTileM = kBlockM * kCG;
-  static constexpr int kBRows = kTileN / kCG;                      // B-operand rows held by each CTA
   static constexpr int kABytes = kBlockM * kBlockK * 2;            // 16 KiB
-  static constexpr int kBBytes = kBRows * kBlockK * 2;             // 32 / 16 KiB
+  static constexpr int kBBytes = kTileN * kBlockK * 2;             // 16 KiB
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = kStagesT;
   static constexpr int kStagingBytes = (kMode == kModeLoss) ? kNumEpiWarps * kStagingBytesPerWarp : 0;
   static constexpr int kSmemBytes =
-      kStages * kStageBytes + kStagingBytes + 1024 /*barriers*/ + 1024 /*alignment slack*/;
+      kStages * kStageBytes + kStagingBytes + 1024 /*barriers, reduction*/ + 1024 /*alignment slack*/;
   static_assert(kSmemBytes <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
 };
 
@@ -113,7 +104,7 @@ __device__ __forceinline__ double warp_sum(double v) {
 // legitimately be late by a checkpoint save or an evaluation pass).
 __device__ __forceinline__ void wait_peer_flags(const volatile unsigned int* flags, int n, unsigned int value,
                                                 unsigned long long timeout_ns, DebugRecord* dbg, unsigned int site) {
-  if (threadIdx.x == kAllocWarp * 32) {
+  if (threadIdx.x == kAuxWarp * 32) {
     uint64_t t0 = 0;
     uint32_t spins = 0;
     for (int f = 0; f < n; ++f) {
@@ -183,55 +174,30 @@ struct TileCoord {
   int slot;    // split tiles only: index into the partial-accumulator workspace / arrival counters
 };
 
-// Work unit of a cluster: kMC vertically adjacent tiles (same n block, consecutive m blocks) — one per CTA (pair)
-// of the cluster, so that the B operand tile is common and can be TMA-multicast.
-template <int kMC>
-__device__ __forceinline__ int cluster_tiles(const Problem& pr) {
-  return ((pr.tiles_m + kMC - 1) / kMC) * pr.tiles_n;
-}
+// Work unit of a cluster: kCS vertically adjacent 128-row blocks (same n block, consecutive m blocks) — one per CTA of
+// the cluster, so that the B operand tile is common and can be TMA-multicast. tiles_m counts such row panels.
+__device__ __forceinline__ int cluster_tiles(const Problem& pr) { return pr.tiles_m * pr.tiles_n; }
 
-// Column tiles of the out kernel (N-major B operand, no multicast) may be 128 wide instead of 256 (Problem::tile_n):
-// twice the tiles of half the work each, for shapes whose 256-wide tiles fill the last wave badly.
-template <int kMode, int kMC>
-__device__ __forceinline__ int tile_stride_n(const Problem& pr) {
-  if constexpr (kMode == kModeOut && kMC == 1) {
-    return (pr.tile_n == kTileN / 2 && pr.b_mn) ? kTileN / 2 : kTileN;
-  } else {
-    return kTileN;
-  }
-}
-
-// Columns the MMA of column tile n_blk computes: 256, or 128 for narrow tiles / a short last tile of the out kernel.
-template <int kMode, int kMC>
-__device__ __forceinline__ int tile_cols(const Problem& pr, int n_blk) {
-  if constexpr (kMode == kModeOut && kMC == 1) {
-    if (tile_stride_n<kMode, kMC>(pr) == kTileN / 2) return kTileN / 2;
-    return (pr.b_mn && pr.N - n_blk * kTileN <= kTileN / 2) ? kTileN / 2 : kTileN;
-  } else {
-    return kTileN;
-  }
-}
-
-// Work item -> tile. Items 0 .. sk_first-1 are whole tiles in schedule order; with split-K (out kernel, kMC == 1) the
-// remaining sk_tiles tiles — the ragged last wave — appear sk_parts times, slice-major, so that the slices of one tile
-// run on different clusters at the same time.
-template <int kMC>
-__device__ __forceinline__ TileCoord decode_tile(const KernelParams& p, int t, int mc_rank) {
+// Work item -> tile. Items 0 .. sk_first-1 are whole tiles in schedule order; with split-K (out kernel) the remaining
+// sk_tiles tiles — the ragged last wave — appear sk_parts times, slice-major, so that the slices of one tile run on
+// different clusters at the same time.
+template <int kCS>
+__device__ __forceinline__ TileCoord decode_tile(const KernelParams& p, int t, int crank) {
   TileCoord c;
   c.part = -1;
   c.slot = 0;
-  if (kMC == 1 && p.sk_parts > 1 && t >= p.sk_first) {
+  if (p.sk_parts > 1 && t >= p.sk_first) {
     const int q = t - p.sk_first;
     c.part = q / p.sk_tiles;
     c.slot = q - c.part * p.sk_tiles;
     t = p.sk_first + c.slot;
   }
-  const int t0 = cluster_tiles<kMC>(p.prob[0]);
+  const int t0 = cluster_tiles(p.prob[0]);
   c.prob = (t >= t0) ? 1 : 0;
   const int tt = c.prob ? t - t0 : t;
   const int tn = p.prob[c.prob].tiles_n;
   const int mrow = tt / tn;
-  c.m_blk = mrow * kMC + mc_rank;   // may be >= tiles_m for the last row when tiles_m is odd: fully masked tile
+  c.m_blk = mrow * kCS + crank;   // may lie beyond M in the last row panel: fully masked block
   c.n_blk = tt - mrow * tn;
   return c;
 }
@@ -249,40 +215,45 @@ __device__ __forceinline__ void item_k_range(const KernelParams& p, const TileCo
 }
 
 // -------------------------------------------------------------------------------------------------
-// Epilogue of the loss kernel: one 32-column slab of one accumulator row per thread.
+// Accumulator fragment of a consumer thread (wgmma m64n128 f32): acc[4 i + e] holds row r_lo + 8 (e >> 1) and column
+// 8 i + c_lo + (e & 1) of its warpgroup's 64 x 128 block, with r_lo = 16 (warp % 4) + lane / 4, c_lo = 2 (lane % 4).
+// The epilogues walk it in slabs of 32 columns (acc[16 c .. 16 c + 15]): per warp a 16-row x 32-column block.
 //
-// Per element (s = <img_i, txt_j>, z = t*s + b, reference distributed_sigmoid_loss.py:24-33):
+// Epilogue of the loss kernel. Per element (s = <img_i, txt_j>, z = t*s + b, reference distributed_sigmoid_loss.py:24-33):
 //   negative pair: term = softplus(z),  g = dterm/dz = sigma(z)
 //   positive pair: term = softplus(-z), g = -sigma(-z)            (own chunk diagonal only)
 // Sums kept per thread: sum term, sum g, sum g*s (-> loss, dbias, dt').
 //
 // Fast path (whole warp slab has z < kFastZ, i.e. e = exp(z) < 2^-6, which is where a SigLIP batch lives:
-// bias ~ -10): 1 MUFU (ex2) + ~6 packed FMA-pipe instructions per element, sigma and log1p by their series.
+// bias ~ -10): 1 MUFU (ex2) + ~8 FMA-pipe instructions per element, sigma and log1p by their series.
 // General path: any z, exp(-|z|) + degree-7 log1p polynomial + rcp.
 // -------------------------------------------------------------------------------------------------
 constexpr float kFastZ = -4.2f;  // e < 0.015 < 2^-6: series truncated after e^2, relative error < e^3 = 3.4e-6
 
-// The sigma slab goes to HBM through shared memory + one TMA store per warp: 4 conflict-free 16-byte
-// st.shared per thread instead of 4 strided 16-byte global stores (32 cache lines per instruction).
+// The sigma slab goes to HBM through shared memory + one TMA store per warp: 8 conflict-free 4-byte st.shared per
+// thread (64B swizzle) instead of 8 scattered 4-byte global stores.
 struct GStore {
-  const CUtensorMap* tmap;  // 16-bit [B, B] tensor, box {32 cols, 32 rows}, SWIZZLE_64B
-  uint32_t stage;           // this warp's 2 KiB staging buffer (shared::cta address, 512-byte aligned)
-  int row0;                 // first row of this warp's 32-row block
+  const CUtensorMap* tmap;  // 16-bit [B, B] tensor, box {32 cols, 16 rows}, SWIZZLE_64B
+  uint32_t stage;           // this warp's 1 KiB staging buffer (shared::cta address, 512-byte aligned)
+  int row0;                 // first row of this warp's 16-row band
   int lane;
   uint64_t policy;          // L2 evict_first: the sigma lines are not read again before they have left the L2
 };
 
-__device__ __forceinline__ void store_g_slab(const GStore& gs, int col0, const uint32_t (&packed)[16]) {
+// packed[2 j + h]: the two sigma values of column pair j (columns 8 j + c_lo, + 1) in row r_lo + 8 h of the band
+__device__ __forceinline__ void store_g_slab(const GStore& gs, int col0, const uint32_t (&packed)[8]) {
   // the previous TMA store of this warp must have finished READING the staging buffer
   if (gs.lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
   __syncwarp();
-  const uint32_t row_addr = gs.stage + static_cast<uint32_t>(gs.lane) * 64u;
-  const uint32_t sw = (static_cast<uint32_t>(gs.lane) >> 1) & 3u;   // 64B swizzle: 16-byte chunk ^= (row / 2) % 4
 #pragma unroll
-  for (uint32_t c = 0; c < 4; ++c) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(row_addr + ((c ^ sw) << 4)), "r"(packed[4 * c + 0]),
-                 "r"(packed[4 * c + 1]), "r"(packed[4 * c + 2]), "r"(packed[4 * c + 3])
-                 : "memory");
+  for (uint32_t h = 0; h < 2; ++h) {
+    const uint32_t r = (static_cast<uint32_t>(gs.lane) >> 2) + 8u * h;
+    const uint32_t sw = (r >> 1) & 3u;   // 64B swizzle: 16-byte chunk ^= (row / 2) % 4
+#pragma unroll
+    for (uint32_t j = 0; j < 4; ++j) {
+      const uint32_t addr = gs.stage + r * 64u + ((j ^ sw) << 4) + 4u * (static_cast<uint32_t>(gs.lane) & 3u);
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(packed[2 * j + h]) : "memory");
+    }
   }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the TMA engine
   __syncwarp();
@@ -297,59 +268,53 @@ __device__ __forceinline__ void store_g_slab(const GStore& gs, int col0, const u
 
 // Fast path: every z of the slab is < kFastZ, so e = exp(z) < 2^-6 and both sigma(z) = e / (1 + e) and log1p(e) are
 // evaluated by their alternating series on the FMA pipe (truncation < 3.4e-6 relative at the edge of the path, < 1e-8
-// for the z ~ -10 of a SigLIP batch; the tolerance is 1e-3), two elements per instruction
-// (FFMA2 / FMUL2 / FADD2). One MUFU (ex2) per element instead of two: the epilogue of this kernel is bound by the
-// MUFU and FMA pipes, not by the tensor pipe it has to keep up with.
-template <bool kF16>
-__device__ __forceinline__ void loss_slab_fast(const uint32_t (&v)[32], float tl, float bl, int col0, bool store_g,
+// for the z ~ -10 of a SigLIP batch; the tolerance is 1e-3). One MUFU (ex2) per element instead of two: the epilogue
+// is bound by the MUFU and FMA pipes.
+__device__ __forceinline__ void loss_slab_fast(const float* v, float tl, float bl, int col0, bool store_g,
                                                const GStore& gst, float gscale, float& acc_sp, float& acc_g,
                                                float& acc_gs) {
-  uint32_t packed[16];
-  const f32x2 tl2 = pack2(tl, tl), bl2 = pack2(bl, bl);
-  // sigma is produced already multiplied by the power-of-two scale of the 16-bit operand (exact), and the two sums
-  // that use it are un-scaled once per slab
-  const f32x2 gs_p = pack2(gscale, gscale), gs_n = pack2(-gscale, -gscale), one = pack2(1.0f, 1.0f);
-  const f32x2 c2 = pack2(0.33333334f, 0.33333334f), c1 = pack2(-0.5f, -0.5f);
-  f32x2 a_sp = pack2(0.f, 0.f), a_g = pack2(0.f, 0.f), a_gs = pack2(0.f, 0.f);
+  uint32_t packed[8];
+  float a_sp = 0.f, a_g = 0.f, a_gs = 0.f;
+  float g_prev = 0.f;
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const f32x2 s = pack2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-    const f32x2 t1 = fma2(s, tl2, bl2);                   // z * log2(e)
-    float t1a, t1b;
-    unpack2(t1, t1a, t1b);
-    const f32x2 e = pack2(ex2_approx(t1a), ex2_approx(t1b));   // exp(z), z < kFastZ
-    f32x2 q = fma2(e, gs_p, gs_n);                         // S sigma(z) / e = S (1 - e + e^2)   [- e^3 < 3.8e-6 dropped]
-    q = fma2(e, q, gs_p);
-    const f32x2 g = mul2(e, q);                            // S sigma(z)
-    f32x2 l = fma2(e, c2, c1);                             // log1p(e) / e = 1 - e/2 + e^2/3     [- e^3/4 < 1e-6 dropped]
-    l = fma2(e, l, one);
-    a_sp = fma2(e, l, a_sp);
-    a_g = add2(a_g, g);
-    a_gs = fma2(g, s, a_gs);
-    float g0, g1;
-    unpack2(g, g0, g1);
-    packed[j] = pack_16x2<kF16>(g0, g1);
+  for (int i = 0; i < 16; ++i) {
+    const float s = v[i];
+    const float e = ex2_approx(fmaf(s, tl, bl));        // exp(z), z < kFastZ
+    // sigma is produced already multiplied by the power-of-two scale of the 16-bit operand (exact), and the two sums
+    // that use it are un-scaled once per slab
+    float q = fmaf(e, gscale, -gscale);                  // S sigma(z) / e = S (1 - e + e^2)  [- e^3 < 3.8e-6 dropped]
+    q = fmaf(e, q, gscale);
+    const float g = e * q;                               // S sigma(z)
+    float l = fmaf(e, 0.33333334f, -0.5f);               // log1p(e) / e = 1 - e/2 + e^2/3    [- e^3/4 < 1e-6 dropped]
+    l = fmaf(e, l, 1.0f);
+    a_sp = fmaf(e, l, a_sp);
+    a_g += g;
+    a_gs = fmaf(g, s, a_gs);
+    // element i = 4 j + e': row half e' >> 1, column e' & 1 -> packed[2 j + (e' >> 1)]
+    if (i & 1)
+      packed[2 * (i >> 2) + ((i >> 1) & 1)] = pack_16x2<true>(g_prev, g);
+    else
+      g_prev = g;
   }
   const float inv_s = 1.0f / gscale;
-  float x0, x1;
-  unpack2(a_sp, x0, x1);
-  acc_sp += x0 + x1;
-  unpack2(a_g, x0, x1);
-  acc_g = fmaf(x0 + x1, inv_s, acc_g);
-  unpack2(a_gs, x0, x1);
-  acc_gs = fmaf(x0 + x1, inv_s, acc_gs);
+  acc_sp += a_sp;
+  acc_g = fmaf(a_g, inv_s, acc_g);
+  acc_gs = fmaf(a_gs, inv_s, acc_gs);
   if (store_g) store_g_slab(gst, col0, packed);
 }
 
-template <bool kEdge, bool kDiag, bool kF16>
-__device__ __forceinline__ void loss_slab(const uint32_t (&v)[32], float t, float b, int row, int col0, int nrows,
+// General path. row_lo: global row of this thread's first fragment row; col0: global column of the slab; c_lo as above.
+template <bool kMask>
+__device__ __forceinline__ void loss_slab(const float* v, float t, float b, int row_lo, int col0, int c_lo, int nrows,
                                           int ncols, bool store_g, const GStore& gst, float gscale, float* g_diag,
-                                          float& acc_sp, float& acc_g, float& acc_gs, bool on_diag = true) {
-  uint32_t packed[16];
+                                          bool on_diag, float& acc_sp, float& acc_g, float& acc_gs) {
+  uint32_t packed[8];
   float g_prev = 0.f;
 #pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    const float s = __uint_as_float(v[j]);
+  for (int i = 0; i < 16; ++i) {
+    const int row = row_lo + 8 * ((i >> 1) & 1);
+    const int col = col0 + 8 * (i >> 2) + c_lo + (i & 1);
+    const float s = v[i];
     const float z = fmaf(s, t, b);
     const float e = ex2_approx(-fabsf(z) * kLog2e);    // exp(-|z|) in (0, 1]
     const float l = e * log1p_over_e(e);               // log1p(exp(-|z|))
@@ -359,16 +324,14 @@ __device__ __forceinline__ void loss_slab(const uint32_t (&v)[32], float t, floa
     float g = sig_z;                                   // d softplus(z) / dz
     float g_store = sig_z;
     bool valid = true;
-    if constexpr (kEdge) valid = (row < nrows) && (col0 + j < ncols);
-    if constexpr (kDiag) {
-      if (on_diag && row == col0 + j) {                // positive pair (label +1): softplus(-z), -sigma(-z)
+    if constexpr (kMask) {
+      valid = (row < nrows) && (col < ncols);
+      if (on_diag && row == col) {                     // positive pair (label +1): softplus(-z), -sigma(-z)
         sp = fmaxf(-z, 0.f) + l;
         g = -((z >= 0.f) ? e * r : r);                 // sigma(-z) without the 1 - sigma(z) cancellation
         g_store = 0.f;                                 // the 16-bit operand carries negatives only
         if (store_g && valid) g_diag[row] = g;
       }
-    }
-    if constexpr (kEdge) {
       sp = valid ? sp : 0.f;
       g = valid ? g : 0.f;
       g_store = valid ? g_store : 0.f;
@@ -376,22 +339,24 @@ __device__ __forceinline__ void loss_slab(const uint32_t (&v)[32], float t, floa
     acc_sp += sp;
     acc_g += g;
     acc_gs = fmaf(g, s, acc_gs);
-    if (j & 1) {
-      packed[j >> 1] = pack_16x2<kF16>(g_prev, g_store * gscale);
-    } else {
+    if (i & 1)
+      packed[2 * (i >> 2) + ((i >> 1) & 1)] = pack_16x2<true>(g_prev, g_store * gscale);
+    else
       g_prev = g_store * gscale;
-    }
   }
   if (store_g) store_g_slab(gst, col0, packed);
 }
 
-// Epilogue of the out kernel: one 32-column slab.
+// Epilogue of the out kernel: one row of the fragment (h = 0: row_lo, 1: row_lo + 8), 16 column pairs.
 //   val = scale * (acc * acc_scale + fix * x[row, col]) (+ add_src[row, col]);  written as fp32 or bf16
-// Every global load of the slab is issued before the first store: the stores may alias the loads as far as the compiler
-// knows, and a load -> store -> load -> store chain (8 exposed L2 round trips per warp and tile) was most of the 15 us
-// between the last MMA and the end of the kernel.
-__device__ __forceinline__ void out_slab(const uint32_t (&v)[32], float scale, int row, int col0, const Problem& pr,
-                                         float fix) {
+// parts / nparts: owner of a split tile — the other K-slices' fp32 partials (float4 j of this thread's fragment at
+// parts[j * 256], slices part_stride apart) are added to acc first, in slice order. (Read here instead of being added
+// into the accumulator registers: a non-wgmma write to them makes ptxas serialise every wgmma of the kernel.)
+// All global loads of a group of four column pairs are issued before its stores: the stores may alias the loads as far
+// as the compiler knows, and a load -> store -> load chain exposes one L2 round trip per pair.
+__device__ __forceinline__ void out_row(const float (&acc)[64], int h, float scale, int row, int col0, int c_lo,
+                                       const Problem& pr, float fix, const float4* parts = nullptr, int nparts = 0,
+                                       size_t part_stride = 0) {
   if (row >= pr.M) return;
   const float as = pr.acc_scale;   // undoes the power-of-two scaling of the fp16 operands (1 for bf16)
   const float xs = (pr.fix_mat_scale != 0.f) ? pr.fix_mat_scale : 1.0f;
@@ -399,57 +364,50 @@ __device__ __forceinline__ void out_slab(const uint32_t (&v)[32], float scale, i
   const __nv_bfloat16* xrow = pr.fix_mat ? pr.fix_mat + static_cast<long long>(row) * pr.ldx : nullptr;
   const float* arow = pr.add_src ? pr.add_src + static_cast<long long>(row) * pr.ld_add : nullptr;
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {         // two halves of 16 columns: all loads of a half are in flight before its stores
-    uint4 xb[2];
-    float4 ad[4];
+  for (int jb = 0; jb < 4; ++jb) {
+    uint32_t xw[4];
+    float2 ad[4];
 #pragma unroll
-    for (int qq = 0; qq < 2; ++qq) {
-      const int c = col0 + 16 * h + 8 * qq;
-      const bool in = c < pr.N;
-      xb[qq] = (xrow != nullptr && in) ? __ldg(reinterpret_cast<const uint4*>(xrow + c)) : make_uint4(0u, 0u, 0u, 0u);
-      ad[2 * qq] = (arow != nullptr && in) ? *reinterpret_cast<const float4*>(arow + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-      ad[2 * qq + 1] =
-          (arow != nullptr && in) ? *reinterpret_cast<const float4*>(arow + c + 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int jj = 0; jj < 4; ++jj) {
+      const int c = col0 + 8 * (4 * jb + jj) + c_lo;
+      const bool in = c < pr.N;   // N % 8 == 0 (host): a column pair is wholly inside or outside
+      xw[jj] = (xrow != nullptr && in) ? __ldg(reinterpret_cast<const unsigned int*>(xrow + c)) : 0u;
+      ad[jj] = (arow != nullptr && in) ? *reinterpret_cast<const float2*>(arow + c) : make_float2(0.f, 0.f);
     }
 #pragma unroll
-    for (int qq = 0; qq < 2; ++qq) {    // 8 columns at a time (N % 8 == 0 is enforced by the host)
-      const int q = 2 * h + qq;
-      const int c = col0 + 8 * q;
+    for (int jj = 0; jj < 4; ++jj) {
+      const int j = 4 * jb + jj;
+      const int c = col0 + 8 * j + c_lo;
       if (c < pr.N) {
-        float o[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) o[e] = __uint_as_float(v[8 * q + e]) * as;
-        if (xrow != nullptr) {
-          const uint32_t xw[4] = {xb[qq].x, xb[qq].y, xb[qq].z, xb[qq].w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            float x0, x1;
-            if (pr.fix_f16) {
-              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&xw[e]));
-              x0 = f.x;
-              x1 = f.y;
-            } else {
-              x0 = __uint_as_float(xw[e] << 16);
-              x1 = __uint_as_float(xw[e] & 0xffff0000u);
-            }
-            o[2 * e + 0] = fmaf(fixs, x0, o[2 * e + 0]);
-            o[2 * e + 1] = fmaf(fixs, x1, o[2 * e + 1]);
-          }
+        float o0 = acc[4 * j + 2 * h], o1 = acc[4 * j + 2 * h + 1];
+        for (int sp = 0; sp < nparts; ++sp) {     // fixed order: slice 0 (mine) + 1 + 2 + ...
+          const float4 a = __ldcg(parts + static_cast<size_t>(sp) * part_stride + j * (kNumEpiWarps * 32));
+          o0 += h ? a.z : a.x;
+          o1 += h ? a.w : a.y;
         }
-        const float4 a0 = ad[2 * qq], a1 = ad[2 * qq + 1];   // zeros without a running sum
-        o[0] = fmaf(o[0], scale, a0.x); o[1] = fmaf(o[1], scale, a0.y);
-        o[2] = fmaf(o[2], scale, a0.z); o[3] = fmaf(o[3], scale, a0.w);
-        o[4] = fmaf(o[4], scale, a1.x); o[5] = fmaf(o[5], scale, a1.y);
-        o[6] = fmaf(o[6], scale, a1.z); o[7] = fmaf(o[7], scale, a1.w);
+        o0 *= as;
+        o1 *= as;
+        if (xrow != nullptr) {
+          float x0, x1;
+          if (pr.fix_f16) {
+            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&xw[jj]));
+            x0 = f.x;
+            x1 = f.y;
+          } else {
+            x0 = __uint_as_float(xw[jj] << 16);
+            x1 = __uint_as_float(xw[jj] & 0xffff0000u);
+          }
+          o0 = fmaf(fixs, x0, o0);
+          o1 = fmaf(fixs, x1, o1);
+        }
+        o0 = fmaf(o0, scale, ad[jj].x);   // zeros without a running sum
+        o1 = fmaf(o1, scale, ad[jj].y);
         if (pr.out_bf16) {
           __nv_bfloat16* orow = reinterpret_cast<__nv_bfloat16*>(pr.out) + static_cast<long long>(row) * pr.ldo;
-          *reinterpret_cast<uint4*>(orow + c) =
-              make_uint4(pack_16x2<false>(o[0], o[1]), pack_16x2<false>(o[2], o[3]), pack_16x2<false>(o[4], o[5]),
-                         pack_16x2<false>(o[6], o[7]));
+          *reinterpret_cast<uint32_t*>(orow + c) = pack_16x2<false>(o0, o1);
         } else {
           float* orow = reinterpret_cast<float*>(pr.out) + static_cast<long long>(row) * pr.ldo;
-          *reinterpret_cast<float4*>(orow + c) = make_float4(o[0], o[1], o[2], o[3]);
-          *reinterpret_cast<float4*>(orow + c + 4) = make_float4(o[4], o[5], o[6], o[7]);
+          *reinterpret_cast<float2*>(orow + c) = make_float2(o0, o1);
         }
       }
     }
@@ -457,26 +415,120 @@ __device__ __forceinline__ void out_slab(const uint32_t (&v)[32], float scale, i
 }
 
 // -------------------------------------------------------------------------------------------------
+// Mainloop of one consumer warpgroup: acc (+)= A[its 64 rows] * B[128 columns]^T over k-blocks [kb0, kb1), operands
+// from the shared-memory ring. One k block = 4 wgmma's; the stage of the previous k block is handed back (to every CTA
+// of the cluster that multicasts into it) once wgmma.wait_group says its MMAs have finished reading it.
+// -------------------------------------------------------------------------------------------------
+template <int kType, int kTA, int kTB, int kCS, int kStageBytes>
+__device__ __forceinline__ void mma_loop(float (&acc)[64], int kb0, int kb1, int& stage, uint32_t& phase, int nstages,
+                                         uint64_t adesc0, uint64_t bdesc0, uint32_t a_adv, uint32_t b_adv,
+                                         uint32_t full0, uint32_t empty0, int lane, DebugRecord* dbg, int t,
+                                         long long* waited) {
+  auto release = [&](int s) {
+    if (lane == 0) {
+      const uint32_t eb = empty0 + 8u * static_cast<uint32_t>(s);
+      if constexpr (kCS == 1) {
+        mbar_arrive(eb);
+      } else {
+#pragma unroll
+        for (uint32_t r = 0; r < static_cast<uint32_t>(kCS); ++r) mbar_arrive_cluster_relaxed(mapa_shared(eb, r));
+      }
+    }
+  };
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc_fence(acc[i]);
+  int prev = -1;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(full0 + 8u * static_cast<uint32_t>(stage), phase, dbg, 3, t, kb, 0, waited);
+    const uint64_t so = static_cast<uint64_t>(stage) * static_cast<uint64_t>(kStageBytes >> 4);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBlockK / kMmaK; ++k) {
+      wgmma_m64n128<kType, kTA, kTB>(acc, adesc0 + so + static_cast<uint64_t>(k * a_adv),
+                                     bdesc0 + so + static_cast<uint64_t>(k * b_adv), (kb != kb0 || k != 0) ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();   // the MMAs of the previous k block are done: its stage may be refilled
+    if (prev >= 0) release(prev);
+    prev = stage;
+    if (++stage == nstages) {
+      stage = 0;
+      phase ^= 1u;
+    }
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc_fence(acc[i]);
+  if (prev >= 0) release(prev);
+}
+
+// The same loop for e4m3 operands (K-major, 32 values per wgmma). Hopper's fp8 wgmma keeps its accumulator at reduced
+// precision (~14 significant bits), so a chain of them drifts from the fp32 sum by ~1e-3 relative. Each instruction
+// here starts from zero (scale-d = 0) and its result is added into the fp32 `sum` on the CUDA cores: the products of
+// e4m3 values are exact, and only the sum of the 32 products of one instruction passes through the narrow accumulator.
+// `acc` is only ever written by wgmma (a non-wgmma write to a wgmma accumulator makes ptxas serialise every wgmma of
+// the kernel); `sum` is the result.
+template <int kCS, int kStageBytes>
+__device__ __forceinline__ void mma_loop_f8(float (&sum)[64], float (&acc)[64], int kb0, int kb1, int& stage,
+                                            uint32_t& phase, int nstages, uint64_t adesc0, uint64_t bdesc0,
+                                            uint32_t full0, uint32_t empty0, int lane, DebugRecord* dbg, int t,
+                                            long long* waited) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) sum[i] = 0.f;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(full0 + 8u * static_cast<uint32_t>(stage), phase, dbg, 3, t, kb, 0, waited);
+    const uint64_t so = static_cast<uint64_t>(stage) * static_cast<uint64_t>(kStageBytes >> 4);
+#pragma unroll 1
+    for (int k = 0; k < kBlockK / kMmaK; ++k) {   // 4 x 32 bytes of the 128-byte swizzle row
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc_fence(acc[i]);
+      wgmma_fence();
+      wgmma_m64n128<2, 0, 0>(acc, adesc0 + so + static_cast<uint64_t>(k * 2), bdesc0 + so + static_cast<uint64_t>(k * 2),
+                             0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < 64; ++i) {
+        acc_fence(acc[i]);
+        sum[i] += acc[i];
+      }
+    }
+    if (lane == 0) {   // this k block's MMAs are complete: hand the stage back
+      const uint32_t eb = empty0 + 8u * static_cast<uint32_t>(stage);
+      if constexpr (kCS == 1) {
+        mbar_arrive(eb);
+      } else {
+#pragma unroll
+        for (uint32_t r = 0; r < static_cast<uint32_t>(kCS); ++r) mbar_arrive_cluster_relaxed(mapa_shared(eb, r));
+      }
+    }
+    if (++stage == nstages) {
+      stage = 0;
+      phase ^= 1u;
+    }
+  }
+}
+
+// -------------------------------------------------------------------------------------------------
 // The kernel
 // -------------------------------------------------------------------------------------------------
-template <int kCG, int kMode, int kStagesT, int kMC>
+// kF8: the out kernel of the 8-bit measurement path (its own instantiation: the extra fp32 result registers of
+// mma_loop_f8 would otherwise cost the production kernels spills).
+template <int kMode, int kStagesT, int kCS, bool kF8 = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
                    const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1,
                    const __grid_constant__ CUtensorMap tmG, const __grid_constant__ KernelParams p) {
-  using C = Cfg<kCG, kMode, kStagesT>;
+  using C = Cfg<kMode, kStagesT>;
+  static_assert(kCS == 1 || kCS == 2 || kCS == 4, "clusters of 1, 2 or 4 CTAs");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t staging_base = smem_base + C::kStages * C::kStageBytes;
   const uint32_t bar_base = staging_base + C::kStagingBytes;
-  // barrier map (8 bytes each)
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (C::kStages + s); };
-  auto tmem_full_bar = [&](int a) { return bar_base + 8u * (2 * C::kStages + a); };
-  auto tmem_empty_bar = [&](int a) { return bar_base + 8u * (2 * C::kStages + kAccStages + a); };
-  const uint32_t tmem_ptr_smem = bar_base + 8u * (2 * C::kStages + 2 * kAccStages);
-  const uint32_t red_smem = tmem_ptr_smem + 16;  // 8 warps x 3 doubles
+  // barrier map (8 bytes each): full[kStages], empty[kStages], then the loss kernel's reduction slots
+  const uint32_t full0 = bar_base, empty0 = bar_base + 8u * C::kStages;
+  const uint32_t red_smem = bar_base + 16u * C::kStages;  // 8 warps x 3 doubles
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -486,19 +538,12 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
     atomicMax(p.aux_trace + 12, now);                                                // ... of the last CTA to start
     atomicMin(p.aux_trace + 13, now);                                                // ... of the first
   }
-  static_assert(kMC == 1 || kMC == 2, "operand multicast across 1 or 2 tiles");
-  // Cluster layout: kCG consecutive CTAs form one MMA pair; kMC pairs (or single CTAs) on vertically adjacent tiles
-  // share the B operand tile by TMA multicast. cg=2, mc=2 is the 2x2 cluster cuBLAS' nvjet kernels use.
-  constexpr int kClusterSize = kCG * kMC;
-  const uint32_t crank = (kClusterSize > 1) ? cluster_ctarank() : 0u;
-  const uint32_t cta_rank = (kCG == 2) ? (crank & 1u) : 0u;                 // rank inside the MMA pair
-  const int mc_rank = (kMC > 1) ? static_cast<int>(crank / kCG) : 0;         // which of the cluster's tiles
-  const uint32_t leader_rank = crank - cta_rank;                             // cluster rank of this pair's leader
-  constexpr uint16_t kMcMask = static_cast<uint16_t>((1u << kClusterSize) - 1u);  // every CTA of the cluster
-  const int cluster_id = blockIdx.x / kClusterSize;
-  const int num_clusters = gridDim.x / kClusterSize;
-  const int whole_tiles = cluster_tiles<kMC>(p.prob[0]) + (p.nprob > 1 ? cluster_tiles<kMC>(p.prob[1]) : 0);
-  const int total_tiles = (kMC == 1 && p.sk_parts > 1) ? p.sk_first + p.sk_tiles * p.sk_parts : whole_tiles;
+  const uint32_t crank = (kCS > 1) ? cluster_ctarank() : 0u;
+  constexpr uint16_t kMcMask = static_cast<uint16_t>((1u << kCS) - 1u);  // every CTA of the cluster
+  const int cluster_id = blockIdx.x / kCS;
+  const int num_clusters = gridDim.x / kCS;
+  const int whole_tiles = cluster_tiles(p.prob[0]) + (p.nprob > 1 ? cluster_tiles(p.prob[1]) : 0);
+  const int total_tiles = (p.sk_parts > 1) ? p.sk_first + p.sk_tiles * p.sk_parts : whole_tiles;
 
   if (warp == kProducerWarp && lane == 0) {
     prefetch_tmap(&tmA0);
@@ -508,30 +553,20 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       prefetch_tmap(&tmB1);
     }
   }
-  if (warp == kMmaWarp && lane == 0) {
+  if (warp == kInitWarp && lane == 0) {
     for (int s = 0; s < C::kStages; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), kMC);   // every CTA that multicasts into this stage must see it released by all readers
-    }
-    for (int a = 0; a < kAccStages; ++a) {
-      mbar_init(tmem_full_bar(a), 1);
-      mbar_init(tmem_empty_bar(a), kNumEpiWarps * kCG);
+      mbar_init(full0 + 8u * s, 1);
+      // every consumer warp of every CTA that multicasts into this stage must have released it
+      mbar_init(empty0 + 8u * s, kNumEpiWarps * kCS);
     }
     fence_mbar_init();
   }
-  if (warp == kAllocWarp) {
-    tmem_alloc<kCG>(tmem_ptr_smem, kTmemCols);
-  }
-  tc_fence_before();
-  if constexpr (kClusterSize > 1) {
+  if constexpr (kCS > 1) {
     cluster_sync_all();
   } else {
     __syncthreads();
   }
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_ptr_smem));
-  // Programmatic dependent launch: everything above (barriers, TMEM, descriptor prefetch) touched no global memory and
+  // Programmatic dependent launch: everything above (barriers, descriptor prefetch) touched no global memory and
   // may run while the previous kernel of the stream drains its last tiles; from here on its results are needed (and the
   // buffers it read are overwritten). The next kernel of the stream may start ITS set-up as soon as SMs free up.
   if (p.pdl) {
@@ -546,219 +581,88 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
 
   if (warp == kProducerWarp) {
     // ===================================== TMA producer =====================================
-    // The whole warp runs the loop (warp-uniform control flow keeps descriptors and barrier addresses in uniform
-    // registers); one elected lane issues the TMA instructions.
-    {
-      int stage = 0;
-      uint32_t phase = 0;
-      long long w_empty = 0;
-      // L2 priorities: the embeddings (A and B of the loss kernel, B of the gradient kernel: 32 MiB each) are re-read
-      // by every tile wave and must survive the 512 MiB sigma operand streaming through the 126 MB L2 once per pass.
-      // The sigma operand itself keeps normal priority: the four column tiles of a row panel (and both CTAs of a pair)
-      // read the same lines a little apart in time and rely on finding them in L2 (evict_first there: 2.6 GB of DRAM
-      // reads per launch instead of 1.5).
-      const uint64_t pol_b = l2_policy_evict_last();
-      const uint64_t pol_a = (kMode == kModeLoss) ? pol_b : l2_policy_evict_normal();
-      for (int t = cluster_id; t < total_tiles; t += num_clusters) {
-        const TileCoord tc = decode_tile<kMC>(p, t, mc_rank);
-        const Problem& pr = p.prob[tc.prob];
-        const CUtensorMap* tmA = tc.prob ? &tmA1 : &tmA0;
-        const CUtensorMap* tmB = tc.prob ? &tmB1 : &tmB0;
-        const int m_idx = tc.m_blk * C::kTileM + static_cast<int>(cta_rank) * kBlockM;
-        // a last column tile with <= 128 columns left runs as a 128-wide MMA (out mode, N-major B, no multicast):
-        // D = 1152 is 4.5 tiles of 256 — without this 10 % of the gradient MMA work would be padding
-        const int n_cur = tile_cols<kMode, kMC>(pr, tc.n_blk);
-        const int b_rows = n_cur / kCG;                               // B rows this CTA holds for the tile
-        const int n_idx = tc.n_blk * tile_stride_n<kMode, kMC>(pr) + static_cast<int>(cta_rank) * b_rows;
-        const uint32_t stage_tx = static_cast<uint32_t>(C::kABytes + b_rows * kBlockK * 2) * kCG;
-        // elements per 128-byte swizzle row: 64 16-bit values, or 128 8-bit ones (fp8 experiment, K-major only)
-        const int kblk = (pr.ab_f16 == 2) ? 2 * kBlockK : kBlockK;
-        const int num_kb = (pr.K + kblk - 1) / kblk;
-        const int a_mn = pr.a_mn, b_mn = pr.b_mn;
-        int kb0, kb1;
-        item_k_range(p, tc, num_kb, kb0, kb1);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u, p.dbg, 1, t, kb, 0, p.wait_stats ? &w_empty : nullptr);
-          if (elect_one_sync()) {
-            const uint32_t sA = smem_base + stage * C::kStageBytes;
-            const uint32_t sB = sA + C::kABytes;
-            uint32_t fb = full_bar(stage);
-            if (cta_rank == 0) mbar_arrive_expect_tx(fb, stage_tx);
-            const uint32_t fb_local = fb;
-            if constexpr (kCG == 2) fb = mapa_shared(fb, leader_rank);   // the pair's leader owns the full barriers
-            const int k_idx = kb * kblk;
-            if (!a_mn) {
-              tma_load_2d_hint<kCG>(tmA, fb, sA, k_idx, m_idx, pol_a);  // box {64 k, 128 rows}
+    // The whole warp runs the loop (warp-uniform control flow); one elected lane issues the TMA instructions.
+    int stage = 0;
+    uint32_t phase = 0;
+    long long w_empty = 0;
+    // L2 priorities: the embeddings (A and B of the loss kernel, B of the gradient kernel) are re-read by every tile
+    // wave and must survive the sigma operand streaming through the 50 MB L2 once per pass. The sigma operand itself
+    // keeps normal priority: the column tiles of a row panel read the same lines a little apart in time.
+    const uint64_t pol_b = l2_policy_evict_last();
+    const uint64_t pol_a = (kMode == kModeLoss) ? pol_b : l2_policy_evict_normal();
+    for (int t = cluster_id; t < total_tiles; t += num_clusters) {
+      const TileCoord tc = decode_tile<kCS>(p, t, static_cast<int>(crank));
+      const Problem& pr = p.prob[tc.prob];
+      const CUtensorMap* tmA = tc.prob ? &tmA1 : &tmA0;
+      const CUtensorMap* tmB = tc.prob ? &tmB1 : &tmB0;
+      const int m_idx = tc.m_blk * kBlockM;
+      const int n_idx = tc.n_blk * kTileN;
+      // elements per 128-byte swizzle row: 64 16-bit values, or 128 8-bit ones (fp8 measurement path, K-major only)
+      const int kblk = (pr.ab_f16 == 2) ? 2 * kBlockK : kBlockK;
+      const int num_kb = (pr.K + kblk - 1) / kblk;
+      const int a_mn = pr.a_mn, b_mn = pr.b_mn;
+      int kb0, kb1;
+      item_k_range(p, tc, num_kb, kb0, kb1);
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(empty0 + 8u * stage, phase ^ 1u, p.dbg, 1, t, kb, 0, p.wait_stats ? &w_empty : nullptr);
+        if (elect_one_sync()) {
+          const uint32_t sA = smem_base + stage * C::kStageBytes;
+          const uint32_t sB = sA + C::kABytes;
+          const uint32_t fb = full0 + 8u * stage;
+          // A of this CTA plus the WHOLE B tile: the other CTAs of the cluster multicast their shares into it
+          mbar_arrive_expect_tx(fb, C::kStageBytes);
+          const int k_idx = kb * kblk;
+          if (!a_mn) {
+            tma_load_2d_hint(tmA, fb, sA, k_idx, m_idx, pol_a);    // box {64 k, 128 rows}
+          } else {
+#pragma unroll
+            for (int h = 0; h < kBlockM / 64; ++h)                  // boxes {64 rows, 64 k}
+              tma_load_2d_hint(tmA, fb, sA + h * 8192, m_idx + 64 * h, k_idx, pol_a);
+          }
+          // this CTA's 1 / kCS of the B tile, delivered to every CTA of the cluster
+          auto load_b = [&](uint32_t dst, int c0, int c1) {
+            if constexpr (kCS == 1) {
+              tma_load_2d_hint(tmB, fb, dst, c0, c1, pol_b);
             } else {
-#pragma unroll
-              for (int h = 0; h < kBlockM / 64; ++h)        // boxes {64 rows, 64 k}
-                tma_load_2d_hint<kCG>(tmA, fb, sA + h * 8192, m_idx + 64 * h, k_idx, pol_a);
+              tma_load_2d_mcast(tmB, fb, dst, c0, c1, kMcMask);
             }
-            if constexpr (kMC == 1) {
-              if (!b_mn) {
-                tma_load_2d_hint<kCG>(tmB, fb, sB, k_idx, n_idx, pol_b);  // box {64 k, kBRows rows}
-              } else {
+          };
+          if (!b_mn) {
+            constexpr int kRows = kTileN / kCS;                     // box {64 k, kRows rows}
+            load_b(sB + crank * (kRows * 128), k_idx, n_idx + static_cast<int>(crank) * kRows);
+          } else if constexpr (kCS == 4) {
+            // boxes {64 columns, 32 k}: CTA r fetches k half (r & 1) of the 64-column block (r >> 1)
+            const int h = static_cast<int>(crank >> 1), kh = static_cast<int>(crank & 1u);
+            load_b(sB + h * 8192 + kh * 4096, n_idx + 64 * h, k_idx + 32 * kh);
+          } else {
 #pragma unroll
-                for (int h = 0; h < C::kBRows / 64; ++h)
-                  if (h * 64 < b_rows) tma_load_2d_hint<kCG>(tmB, fb, sB + h * 8192, n_idx + 64 * h, k_idx, pol_b);
-              }
-            } else if constexpr (kCG == 1) {
-              // this CTA fetches 1/kMC of the common B tile and multicasts it to every CTA of the cluster
-              constexpr int kPart = C::kBRows / kMC;  // rows of B per CTA
-              if (!b_mn) {
-                tma_load_2d_mcast(tmB, fb, sB + mc_rank * (kPart * kBlockK * 2), k_idx, n_idx + mc_rank * kPart,
-                                  kMcMask);         // box {64 k, kPart rows}
-              } else {
-#pragma unroll
-                for (int h = 0; h < kPart / 64; ++h) {
-                  const int hh = mc_rank * (kPart / 64) + h;
-                  tma_load_2d_mcast(tmB, fb, sB + hh * 8192, n_idx + 64 * hh, k_idx, kMcMask);
-                }
-              }
-            } else {
-              // 2x2 cluster: the CTAs with the same rank-in-pair of both pairs hold the same 128 B rows; each of them
-              // fetches 64 of those rows and multicasts them to both. The bytes are counted on each pair leader's
-              // full barrier (pair bit cleared in the barrier address).
-              constexpr int kPart = C::kBRows / kMC;  // 64 rows
-              const uint16_t mask = static_cast<uint16_t>(0x5u << cta_rank);   // CTAs {cta_rank, cta_rank + 2}
-              if (!b_mn) {
-                tma_load_2d_mcast_2sm(tmB, fb_local, sB + mc_rank * (kPart * kBlockK * 2), k_idx,
-                                      n_idx + mc_rank * kPart, mask);          // box {64 k, 64 rows}
-              } else {
-                tma_load_2d_mcast_2sm(tmB, fb_local, sB + mc_rank * 8192, n_idx + 64 * mc_rank, k_idx, mask);
-              }
-            }
-          }
-          __syncwarp();
-          if (++stage == C::kStages) {
-            stage = 0;
-            phase ^= 1u;
+            for (int h = static_cast<int>(crank) * (2 / kCS); h < (static_cast<int>(crank) + 1) * (2 / kCS); ++h)
+              load_b(sB + h * 8192, n_idx + 64 * h, k_idx);         // boxes {64 columns, 64 k}
           }
         }
-      }
-      if (p.wait_stats && lane == 0) p.wait_stats[8ll * blockIdx.x + 0] = static_cast<unsigned long long>(w_empty);
-    }
-  } else if (warp == kMmaWarp) {
-    // ===================================== MMA issuer =====================================
-    // Warp-uniform loop; one elected lane issues tcgen05.mma / tcgen05.commit.
-    if (cta_rank == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      long long w_full = 0, w_tmem = 0;
-      const bool prof = p.wait_stats != nullptr;
-      const long long c_start = clock_cycles();
-      for (int t = cluster_id; t < total_tiles; t += num_clusters) {
-        const TileCoord tc = decode_tile<kMC>(p, t, mc_rank);
-        const Problem& pr = p.prob[tc.prob];
-        const uint32_t idesc = make_idesc_bf16(C::kTileM, tile_cols<kMode, kMC>(pr, tc.n_blk), pr.a_mn, pr.b_mn, pr.ab_f16);
-        // K-major: 8-row groups 1024 B apart (SBO), K advance 32 B inside the swizzle row.
-        // MN-major: 64-element MN blocks 8192 B apart (LBO), 8-k groups 1024 B apart (SBO), K advance 16 rows.
-        const uint32_t a_lbo = pr.a_mn ? 8192u : 16u, b_lbo = pr.b_mn ? 8192u : 16u;
-        const uint32_t a_adv = pr.a_mn ? (kUmmaK * 128u) >> 4 : (kUmmaK * 2u) >> 4;
-        const uint32_t b_adv = pr.b_mn ? (kUmmaK * 128u) >> 4 : (kUmmaK * 2u) >> 4;
-        // descriptors of stage 0; later stages add stage * kStageBytes >> 4 to the start-address field
-        const uint64_t adesc0 = make_smem_desc_sw128(smem_base, a_lbo, 1024u);
-        const uint64_t bdesc0 = make_smem_desc_sw128(smem_base + C::kABytes, b_lbo, 1024u);
-        const bool fp8 = (pr.ab_f16 == 2);
-        const int num_kb = (pr.K + (fp8 ? 2 * kBlockK : kBlockK) - 1) / (fp8 ? 2 * kBlockK : kBlockK);
-        int kb0, kb1;
-        item_k_range(p, tc, num_kb, kb0, kb1);
-        mbar_wait(tmem_empty_bar(as), aphase ^ 1u, p.dbg, 2, t, as, 0, prof ? &w_tmem : nullptr);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(as * kTileN);
-        if (p.aux_trace != nullptr && blockIdx.x == 0 && t == cluster_id) {     // diagnostic, first tile only
-          mbar_wait(full_bar(stage), phase, p.dbg, 3, t, kb0, 0, nullptr);
-          if (lane == 0) p.aux_trace[6] = globaltimer_ns();                      // first operands have landed
+        __syncwarp();
+        if (++stage == C::kStages) {
+          stage = 0;
+          phase ^= 1u;
         }
-        // The k loop is the critical path of the kernel (one elected lane feeds the tensor pipe): keep it free of
-        // anything that is not the four MMAs and the two commits. The 8-bit measurement variant gets its own copy.
-        // Everything the four MMAs of a k block need is computed here, in warp-uniform code (uniform registers), from
-        // 32-bit arithmetic on the low descriptor word (the start-address field cannot carry out of it: shared memory
-        // addresses >> 4 stay below 2^14); the elected branch holds nothing but the issue. This warp shares its
-        // scheduler with four epilogue warps: in the loss kernel (busy epilogue) every instruction of this loop shows
-        // up as tensor-pipe idle time (138 instead of 128 cycles per MMA with the ~96-instruction loop this replaces).
-        const uint32_t a_hi = static_cast<uint32_t>(adesc0 >> 32), b_hi = static_cast<uint32_t>(bdesc0 >> 32);
-        const uint32_t a_lo0 = static_cast<uint32_t>(adesc0), b_lo0 = static_cast<uint32_t>(bdesc0);
-        auto desc64 = [](uint32_t hi, uint32_t lo) { return (static_cast<uint64_t>(hi) << 32) | lo; };
-        auto issue_tile = [&](auto is_fp8) {
-          for (int kb = kb0; kb < kb1; ++kb) {
-            mbar_wait_warp(full_bar(stage), phase, p.dbg, 3, t, kb, prof ? &w_full : nullptr);
-            tc_fence_after();
-            const uint32_t so = static_cast<uint32_t>(stage) * static_cast<uint32_t>(C::kStageBytes >> 4);
-            const uint32_t al = a_lo0 + so, bl = b_lo0 + so;
-            const uint32_t acc0 = static_cast<uint32_t>(kb != kb0);
-            const bool last = (kb == kb1 - 1);
-            const uint32_t ebar = empty_bar(stage);
-            if (elect_one_sync()) {
-#pragma unroll
-              for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-                const uint64_t ad = desc64(a_hi, al + static_cast<uint32_t>(k) * a_adv);
-                const uint64_t bd = desc64(b_hi, bl + static_cast<uint32_t>(k) * b_adv);
-                if constexpr (decltype(is_fp8)::value) {   // kind::f8f6f4: 32 e4m3 values (32 bytes) per instruction
-                  umma_f8<kCG>(tmem_d, ad, bd, idesc, k == 0 ? acc0 : 1u);
-                } else {
-                  umma_bf16<kCG>(tmem_d, ad, bd, idesc, k == 0 ? acc0 : 1u);
-                }
-              }
-              if constexpr (kMC > 1 && kCG == 1) {
-                umma_commit_mcast(ebar, kMcMask);  // stage is free in every CTA that writes into it
-              } else if constexpr (kMC > 1) {
-                umma_commit_2sm_mask(ebar, kMcMask);   // all four CTAs of the 2x2 cluster
-              } else {
-                umma_commit<kCG>(ebar);  // frees the smem stage (both CTAs) when the MMAs retire
-              }
-              if (last) {                            // accumulator ready for the epilogue warps of this pair
-                if constexpr (kMC > 1 && kCG == 2) {
-                  umma_commit_2sm_mask(tmem_full_bar(as), static_cast<uint16_t>(0x3u << leader_rank));
-                } else {
-                  umma_commit<kCG>(tmem_full_bar(as));
-                }
-              }
-            }
-            if (++stage == C::kStages) {
-              stage = 0;
-              phase ^= 1u;
-            }
-          }
-        };
-        if (fp8)
-          issue_tile(std::true_type{});
-        else
-          issue_tile(std::false_type{});
-        if (++as == kAccStages) {
-          as = 0;
-          aphase ^= 1u;
-        }
-      }
-      if (p.aux_trace != nullptr && lane == 0) {
-        const unsigned long long now = globaltimer_ns();
-        if (blockIdx.x == 0) p.aux_trace[7] = now;                    // last MMA issued (CTA 0)
-        atomicMax(p.aux_trace + 9, now);                              // ... latest / earliest over the issuing CTAs
-        atomicMin(p.aux_trace + 10, now);
-      }
-      if (prof && lane == 0) {
-        p.wait_stats[8ll * blockIdx.x + 1] = static_cast<unsigned long long>(w_full);
-        p.wait_stats[8ll * blockIdx.x + 2] = static_cast<unsigned long long>(w_tmem);
-        p.wait_stats[8ll * blockIdx.x + 3] = static_cast<unsigned long long>(clock_cycles() - c_start);
       }
     }
+    if (p.wait_stats && lane == 0) p.wait_stats[8ll * blockIdx.x + 0] = static_cast<unsigned long long>(w_empty);
   } else if (warp < kNumEpiWarps) {
-    // ===================================== epilogue =====================================
-    const int q = warp & 3;        // TMEM lane quarter this warp may touch
-    const int cgrp = warp >> 2;    // which kEpiCols columns of the 256-column accumulator
-    const int row_in_cta = q * 32 + lane;
+    // ===================================== consumers: MMA + epilogue =====================================
+    const int wg = warp >> 2;                       // warpgroup: rows [64 wg, 64 wg + 64) of the CTA's block
+    const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // first fragment row (the second is r_lo + 8)
+    const int c_lo = 2 * (lane & 3);                // first fragment column of every 8-column group
     const float t_exact = expf(load_t_prime(p));
     const float bias = (kMode == kModeLoss) ? *p.bias : 0.f;
     // loss kernel: z = t_eff * acc + b with t_eff = t * s_scale (the accumulator is 2^8 <img, txt> for fp16 x 16 operands)
     const float s_scale = (kMode == kModeLoss && p.s_scale != 0.f) ? p.s_scale : 1.0f;
     const float t_eff = t_exact * s_scale;
     const float tl = t_eff * kLog2e, bl = bias * kLog2e;
-    // per-thread running sums over the tiles of this CTA: compensated fp32 (Kahan) — a DADD per sum, thread and tile
-    // was 11 % of the loss kernel's stall samples (the fp64 pipe of this part is narrow); fp64 only at the very end
+    // per-thread running sums over the tiles of this CTA: compensated fp32 (Kahan); fp64 only at the very end
     float s_sp = 0.f, s_g = 0.f, s_gs = 0.f, c_sp = 0.f, c_g = 0.f, c_gs = 0.f;
-    long long w_epi = 0;
+    long long w_full = 0;
+    long long* w_full_p = (p.wait_stats != nullptr && threadIdx.x == 0) ? &w_full : nullptr;
     if constexpr (kMode == kModeOut) {
       // backward of the two scalars: saved (upstream gradient 1) * grad_out, by one thread of the launch
       if (blockIdx.x == 0 && threadIdx.x == 0 && p.sc_saved != nullptr) {
@@ -773,42 +677,104 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       }
     }
     const uint64_t g_store_policy = l2_policy_evict_first();
-    const long long epi_start = clock_cycles();
-    int as = 0;
-    uint32_t aphase = 0;
+    const long long c_start = clock_cycles();
+    int stage = 0;
+    uint32_t phase = 0;
     bool p1_ready = false;
-    uint32_t empty_remote[kAccStages];
-#pragma unroll
-    for (int a = 0; a < kAccStages; ++a) {
-      empty_remote[a] = (kCG == 2) ? mapa_shared(tmem_empty_bar(a), leader_rank) : tmem_empty_bar(a);
-    }
+    float acc[64];
+    float acc8[kF8 ? 64 : 1];   // result of the 8-bit mainloop (see mma_loop_f8)
     for (int t = cluster_id; t < total_tiles; t += num_clusters) {
-      const TileCoord tc = decode_tile<kMC>(p, t, mc_rank);
+      const TileCoord tc = decode_tile<kCS>(p, t, static_cast<int>(crank));
       const Problem& pr = p.prob[tc.prob];
-      const int row = tc.m_blk * C::kTileM + static_cast<int>(cta_rank) * kBlockM + row_in_cta;
-      const int col_base = tc.n_blk * tile_stride_n<kMode, kMC>(pr) + cgrp * kEpiCols;
-      mbar_wait(tmem_full_bar(as), aphase, p.dbg, 4, t, as, p.epi_sleep_ns,
-                (p.wait_stats != nullptr && warp == 0) ? &w_epi : nullptr);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + static_cast<uint32_t>(as * kTileN + cgrp * kEpiCols) +
-                             (static_cast<uint32_t>(q * 32) << 16);
-      float acc_sp = 0.f, acc_g = 0.f, acc_gs = 0.f;
+      const int row0 = tc.m_blk * kBlockM;            // first row of this CTA's block
+      const int col_base = tc.n_blk * kTileN;
+      const int row_lo = row0 + r_lo;                 // global rows of this thread: row_lo, row_lo + 8
+      const bool fp8 = (pr.ab_f16 == 2);
+      const int num_kb = (pr.K + (fp8 ? 2 * kBlockK : kBlockK) - 1) / (fp8 ? 2 * kBlockK : kBlockK);
+      int kb0, kb1;
+      item_k_range(p, tc, num_kb, kb0, kb1);
+      {
+        // K-major: 8-row groups 1024 B apart (SBO), K advance 32 B inside the swizzle row (16 16-bit or 32 8-bit values).
+        // MN-major: 64-element MN blocks 8192 B apart (LBO), 8-k groups 1024 B apart (SBO), K advance 16 rows.
+        // This warpgroup's 64 A rows start 8192 B into the A tile in both layouts.
+        const uint32_t a_lbo = pr.a_mn ? 8192u : 16u, b_lbo = pr.b_mn ? 8192u : 16u;
+        const uint32_t a_adv = pr.a_mn ? (kMmaK * 128u) >> 4 : 32u >> 4;
+        const uint32_t b_adv = pr.b_mn ? (kMmaK * 128u) >> 4 : 32u >> 4;
+        const uint64_t adesc0 = make_smem_desc_sw128(smem_base + static_cast<uint32_t>(wg) * 8192u, a_lbo, 1024u);
+        const uint64_t bdesc0 = make_smem_desc_sw128(smem_base + C::kABytes, b_lbo, 1024u);
+#define SIGLIP_MMA_LOOP(T, TA, TB)                                                                                  \
+  mma_loop<T, TA, TB, kCS, C::kStageBytes>(acc, kb0, kb1, stage, phase, C::kStages, adesc0, bdesc0, a_adv, b_adv, \
+                                           full0, empty0, lane, p.dbg, t, w_full_p)
+        const int sel = pr.a_mn * 2 + pr.b_mn;
+        if (fp8) {
+          // kF8 instantiation only (launch_gemm routes 8-bit operands there): the result lands in acc8
+          if constexpr (kF8)
+            mma_loop_f8<kCS, C::kStageBytes>(acc8, acc, kb0, kb1, stage, phase, C::kStages, adesc0, bdesc0, full0,
+                                             empty0, lane, p.dbg, t, w_full_p);
+        } else if (pr.ab_f16) {
+          switch (sel) {
+            case 0: SIGLIP_MMA_LOOP(1, 0, 0); break;
+            case 1: SIGLIP_MMA_LOOP(1, 0, 1); break;
+            case 2: SIGLIP_MMA_LOOP(1, 1, 0); break;
+            default: SIGLIP_MMA_LOOP(1, 1, 1); break;
+          }
+        } else {
+          switch (sel) {
+            case 0: SIGLIP_MMA_LOOP(0, 0, 0); break;
+            case 1: SIGLIP_MMA_LOOP(0, 0, 1); break;
+            case 2: SIGLIP_MMA_LOOP(0, 1, 0); break;
+            default: SIGLIP_MMA_LOOP(0, 1, 1); break;
+          }
+        }
+#undef SIGLIP_MMA_LOOP
+      }
+      if (p.aux_trace != nullptr && threadIdx.x == 0 && t == cluster_id && blockIdx.x == 0)
+        p.aux_trace[6] = globaltimer_ns();                                   // first tile's MMAs done (CTA 0)
 
-      bool edge = false, diag = false;
-      GStore gst;
-      gst.tmap = &tmG;
-      gst.stage = staging_base + static_cast<uint32_t>(warp) * kStagingBytesPerWarp;
-      gst.row0 = tc.m_blk * C::kTileM + static_cast<int>(cta_rank) * kBlockM + q * 32;
-      gst.lane = lane;
-      gst.policy = g_store_policy;
-      float scale = 0.f, fix = 0.f;
       if constexpr (kMode == kModeLoss) {
-        const int tile_m0 = tc.m_blk * C::kTileM, tile_n0 = tc.n_blk * kTileN;
-        edge = (tile_m0 + C::kTileM > pr.M) || (tile_n0 + kTileN > pr.N);
-        diag = p.own_chunk && (tile_m0 < tile_n0 + kTileN) && (tile_n0 < tile_m0 + C::kTileM);
+        float acc_sp = 0.f, acc_g = 0.f, acc_gs = 0.f;
+        const bool edge = (row0 + kBlockM > pr.M) || (col_base + kTileN > pr.N);
+        // 128-aligned row and column blocks: only a block on the diagonal holds positive pairs
+        const bool diag = p.own_chunk && (row0 == col_base);
+        const bool sg = p.store_g != 0;
+        GStore gst;
+        gst.tmap = &tmG;
+        gst.stage = staging_base + static_cast<uint32_t>(warp) * kStagingBytesPerWarp;
+        gst.row0 = row0 + wg * 64 + (warp & 3) * 16;
+        gst.lane = lane;
+        gst.policy = g_store_policy;
+#pragma unroll
+        for (int c = 0; c < kTileN / 32; ++c) {
+          const float* v = acc + 16 * c;
+          const int col0 = col_base + 32 * c;
+          // Only the 16x32 slabs that touch the diagonal of a diagonal block hold positive pairs, and only the slabs
+          // that cross the matrix border of an edge block need masking; every other slab takes the fast path like
+          // the rest of the matrix.
+          const bool slab_diag = diag && (gst.row0 < col0 + 32) && (col0 < gst.row0 + 16);
+          const bool slab_edge = edge && ((gst.row0 + 16 > pr.M) || (col0 + 32 > pr.N));
+          if (!slab_edge && !slab_diag) {
+            // z is monotone in s (t > 0): the slab is "all very negative" iff max s is
+            float smax = v[0];
+#pragma unroll
+            for (int j = 1; j < 16; ++j) smax = fmaxf(smax, v[j]);
+            const bool fast = __all_sync(0xffffffffu, fmaf(smax, t_eff, bias) < kFastZ);
+            if (fast)
+              loss_slab_fast(v, tl, bl, col0, sg, gst, p.g_scale, acc_sp, acc_g, acc_gs);
+            else
+              loss_slab<false>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag, false,
+                               acc_sp, acc_g, acc_gs);
+          } else {
+            loss_slab<true>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag, slab_diag,
+                            acc_sp, acc_g, acc_gs);
+          }
+        }
+        kahan_add(s_sp, c_sp, acc_sp);
+        kahan_add(s_g, c_g, acc_g);
+        kahan_add(s_gs, c_gs, acc_gs);
       } else {
-        scale = t_exact * p.inv_b * (p.grad_out != nullptr ? *p.grad_out : 1.0f);
-        fix = (pr.fix_vec != nullptr && row < pr.M) ? pr.fix_vec[row] : 0.f;
+        const float scale = t_exact * p.inv_b * (p.grad_out != nullptr ? *p.grad_out : 1.0f);
+        const float fix0 = (pr.fix_vec != nullptr && row_lo < pr.M) ? pr.fix_vec[row_lo] : 0.f;
+        const float fix1 = (pr.fix_vec != nullptr && row_lo + 8 < pr.M) ? pr.fix_vec[row_lo + 8] : 0.f;
         if (tc.prob == 1 && p.p1_wait_flag != nullptr && !p1_ready) {
           // the dtxt tiles of the LAST gradient launch add the folded sum of the peers' contributions: the fold that
           // completes it runs in this very launch (auxiliary warps of all CTAs) and must have finished everywhere
@@ -840,166 +806,88 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
           __syncwarp();
           p1_ready = true;
         }
-      }
-
-      auto slab = [&](uint32_t(&v)[32], int c) {
-        const int col0 = col_base + c * 32;
-        if constexpr (kMode == kModeLoss) {
-          const bool sg = p.store_g != 0;
-          // Only the 32x32 slabs that touch the diagonal of a diagonal tile (rows and columns are 32-aligned: row0 ==
-          // col0) hold positive pairs, and only the slabs that cross the matrix border of an edge tile need masking:
-          // 8 of the 64 slabs of a diagonal 256x256 tile. Every other slab of such a tile takes the fast path like the
-          // rest of the matrix — a whole diagonal tile on the general path had a 3-4x longer epilogue, which ended up
-          // on the critical path of the clusters that own one (most visible at small B: 16 of 256 tiles at B = 4096).
-          const bool slab_diag = diag && (gst.row0 == col0);
-          const bool slab_edge = edge && ((gst.row0 + 32 > pr.M) || (col0 + 32 > pr.N));
-          if (!slab_edge && !slab_diag) {
-            // z is monotone in s (t > 0): the slab is "all very negative" iff max s is
-            float smax = fmaxf(__uint_as_float(v[0]), __uint_as_float(v[1]));
-#pragma unroll
-            for (int j = 2; j < 32; j += 2) smax = max3(smax, __uint_as_float(v[j]), __uint_as_float(v[j + 1]));
-            const bool fast = __all_sync(0xffffffffu, fmaf(smax, t_eff, bias) < kFastZ);
-            if (fast)
-              loss_slab_fast<true>(v, tl, bl, col0, sg, gst, p.g_scale, acc_sp, acc_g, acc_gs);
-            else
-              loss_slab<false, false, true>(v, t_eff, bias, row, col0, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag, acc_sp, acc_g, acc_gs);
-          } else {
-            // border and / or diagonal slabs (a few per chunk): ONE masked variant — two more copies of the unrolled
-            // general path only made the kernel's code larger (the loss and gradient kernels alternate and share the
-            // instruction caches)
-            loss_slab<true, true, true>(v, t_eff, bias, row, col0, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag, acc_sp, acc_g, acc_gs, slab_diag);
-          }
+        if constexpr (kF8) {   // whole tiles only: split-K is never requested for 8-bit operands
+          out_row(acc8, 0, scale, row_lo, col_base, c_lo, pr, fix0);
+          out_row(acc8, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1);
+        } else if (tc.part < 0) {
+          out_row(acc, 0, scale, row_lo, col_base, c_lo, pr, fix0);
+          out_row(acc, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1);
         } else {
-          if (tc.part < 0) {
-            out_slab(v, scale, row, col0, pr, fix);
+          // split tile: this CTA's 128 x 128 fp32 partial in fragment order, thread-contiguous float4's
+          const size_t kPartF4 = static_cast<size_t>(kBlockM) * kTileN / 4;
+          float4* ws = reinterpret_cast<float4*>(p.sk_ws) +
+                       (static_cast<size_t>(tc.slot) * (p.sk_parts - 1) * kCS + crank) * kPartF4 + threadIdx.x;
+          const size_t part_stride = static_cast<size_t>(kCS) * kPartF4;   // float4 per slice
+          if (tc.part > 0) {
+            float4* dst = ws + static_cast<size_t>(tc.part - 1) * part_stride;
+#pragma unroll
+            for (int j4 = 0; j4 < 16; ++j4)
+              dst[j4 * (kNumEpiWarps * 32)] = make_float4(acc[4 * j4], acc[4 * j4 + 1], acc[4 * j4 + 2], acc[4 * j4 + 3]);
+            // my share of the partial accumulator is written: arrive (release) on the tile's counter
+            __threadfence();
+            __syncwarp();
+            if (lane == 0) atomicAdd(p.sk_counters + 2 * tc.slot, 1u);
           } else {
-            // split tile: 32x32 fp32 slab of this thread's row <-> workspace, lanes contiguous (512 B per warp access)
-            const int slab_id = cgrp * kSlabsPerWarp + c;
-            float4* ws = reinterpret_cast<float4*>(p.sk_ws) +
-                         ((static_cast<size_t>(tc.slot) * (p.sk_parts - 1)) * kCG + cta_rank) * (8 * 8 * kBlockM) +
-                         static_cast<size_t>(slab_id) * (8 * kBlockM) + row_in_cta;
-            const size_t part_stride = static_cast<size_t>(kCG) * (8 * 8 * kBlockM);   // float4 per slice
-            if (tc.part > 0) {
-              float4* dst = ws + static_cast<size_t>(tc.part - 1) * part_stride;
-#pragma unroll
-              for (int j4 = 0; j4 < 8; ++j4)
-                dst[j4 * kBlockM] = make_float4(__uint_as_float(v[4 * j4]), __uint_as_float(v[4 * j4 + 1]),
-                                                __uint_as_float(v[4 * j4 + 2]), __uint_as_float(v[4 * j4 + 3]));
-            } else {
-#pragma unroll 1
-              for (int sp = 0; sp < p.sk_parts - 1; ++sp) {     // fixed order: slice 0 (mine) + 1 + 2 + ...
-                const float4* src = ws + static_cast<size_t>(sp) * part_stride;
-#pragma unroll
-                for (int j4 = 0; j4 < 8; ++j4) {
-                  const float4 a = __ldcg(src + j4 * kBlockM);
-                  v[4 * j4] = __float_as_uint(__uint_as_float(v[4 * j4]) + a.x);
-                  v[4 * j4 + 1] = __float_as_uint(__uint_as_float(v[4 * j4 + 1]) + a.y);
-                  v[4 * j4 + 2] = __float_as_uint(__uint_as_float(v[4 * j4 + 2]) + a.z);
-                  v[4 * j4 + 3] = __float_as_uint(__uint_as_float(v[4 * j4 + 3]) + a.w);
-                }
-              }
-              out_slab(v, scale, row, col0, pr, fix);
-            }
-          }
-        }
-      };
-      if constexpr (kMode == kModeOut) {
-        if (tc.part == 0) {
-          // owner slice: the other slices' partial accumulators must be in the workspace (they run at the same time
-          // on other clusters and wait for nothing, so this cannot deadlock on a co-resident persistent grid)
-          if (lane == 0) {
-            const unsigned int need = static_cast<unsigned int>((p.sk_parts - 1) * kCG * kNumEpiWarps);
-            const unsigned int* ctr = p.sk_counters + 2 * tc.slot;
-            uint64_t t0 = 0;
-            uint32_t spins = 0;
-            while (true) {
-              unsigned int cv;
-              asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(cv) : "l"(ctr) : "memory");
-              if (cv >= need) break;
-              __nanosleep(100);
-              if ((++spins & 0x3ffu) == 0) {
-                const uint64_t now = globaltimer_ns();
-                if (t0 == 0) t0 = now;
-                if (now - t0 > SIGLIP_WAIT_TIMEOUT_NS) {
-                  if (p.dbg != nullptr) {
-                    p.dbg->block = blockIdx.x;
-                    p.dbg->thread = threadIdx.x;
-                    p.dbg->aux0 = cv;
-                    p.dbg->aux1 = need;
-                    p.dbg->code = 4;
-                    __threadfence_system();
+            // owner slice: the other slices' partial accumulators must be in the workspace (they run at the same time
+            // on other clusters and wait for nothing, so this cannot deadlock on a co-resident persistent grid)
+            if (lane == 0) {
+              const unsigned int need = static_cast<unsigned int>((p.sk_parts - 1) * kCS * kNumEpiWarps);
+              const unsigned int* ctr = p.sk_counters + 2 * tc.slot;
+              uint64_t t0 = 0;
+              uint32_t spins = 0;
+              while (true) {
+                unsigned int cv;
+                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(cv) : "l"(ctr) : "memory");
+                if (cv >= need) break;
+                __nanosleep(100);
+                if ((++spins & 0x3ffu) == 0) {
+                  const uint64_t now = globaltimer_ns();
+                  if (t0 == 0) t0 = now;
+                  if (now - t0 > SIGLIP_WAIT_TIMEOUT_NS) {
+                    if (p.dbg != nullptr) {
+                      p.dbg->block = blockIdx.x;
+                      p.dbg->thread = threadIdx.x;
+                      p.dbg->aux0 = cv;
+                      p.dbg->aux1 = need;
+                      p.dbg->code = 4;
+                      __threadfence_system();
+                    }
+                    __trap();
                   }
-                  __trap();
                 }
               }
             }
-          }
-          __syncwarp();
-        }
-      }
-
-      // kSlabsPerWarp slabs of 32 columns. With four epilogue warps per SM sub-partition the TMEM load latency
-      // of one warp is covered by the arithmetic of the others.
-      uint32_t v[32];
-      // column groups beyond a short (128-column) tile have nothing to read (warp-uniform)
-      const bool cols_active = cgrp * kEpiCols < tile_cols<kMode, kMC>(pr, tc.n_blk);
-#pragma unroll
-      for (int c = 0; c < kSlabsPerWarp; ++c) {
-        if (cols_active) {
-          tmem_ld_32x32(taddr + 32 * c, v);
-          tmem_ld_wait();
-        }
-        if (c == kSlabsPerWarp - 1) {
-          // every TMEM read of this warp for this accumulator stage has landed: hand the stage back
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if (kCG == 2 && cta_rank != 0) {
-              mbar_arrive_cluster_relaxed(empty_remote[as]);
-            } else {
-              mbar_arrive_relaxed(tmem_empty_bar(as));
+            __syncwarp();
+            out_row(acc, 0, scale, row_lo, col_base, c_lo, pr, fix0, ws, p.sk_parts - 1, part_stride);
+            out_row(acc, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1, ws, p.sk_parts - 1, part_stride);
+            // every owner warp has consumed the partials: the last one re-arms the counters for the next launch
+            __syncwarp();
+            if (lane == 0) {
+              const unsigned int seen = atomicAdd(p.sk_counters + 2 * tc.slot + 1, 1u);
+              if (seen == static_cast<unsigned int>(kCS * kNumEpiWarps) - 1u) {
+                p.sk_counters[2 * tc.slot] = 0u;
+                p.sk_counters[2 * tc.slot + 1] = 0u;
+              }
             }
           }
         }
-        if (cols_active) slab(v, c);
-      }
-
-      if constexpr (kMode == kModeLoss) {
-        kahan_add(s_sp, c_sp, acc_sp);
-        kahan_add(s_g, c_g, acc_g);
-        kahan_add(s_gs, c_gs, acc_gs);
-      } else {
-        if (tc.part > 0) {
-          // my slabs of the partial accumulator are written: arrive (release) on the tile's counter
-          __threadfence();
-          __syncwarp();
-          if (lane == 0) atomicAdd(p.sk_counters + 2 * tc.slot, 1u);
-        } else if (tc.part == 0) {
-          // every owner warp has consumed the partials: the last one re-arms the counters for the next launch
-          __syncwarp();
-          if (lane == 0) {
-            const unsigned int seen = atomicAdd(p.sk_counters + 2 * tc.slot + 1, 1u);
-            if (seen == static_cast<unsigned int>(kCG * kNumEpiWarps) - 1u) {
-              p.sk_counters[2 * tc.slot] = 0u;
-              p.sk_counters[2 * tc.slot + 1] = 0u;
-            }
-          }
-        }
-      }
-      if (++as == kAccStages) {
-        as = 0;
-        aphase ^= 1u;
       }
     }
-    if (p.aux_trace != nullptr && threadIdx.x == 0) atomicMax(p.aux_trace + 11, globaltimer_ns());   // tiles done
+    if (p.aux_trace != nullptr && threadIdx.x == 0) {
+      const unsigned long long now = globaltimer_ns();
+      if (blockIdx.x == 0) p.aux_trace[7] = now;                    // last tile done (CTA 0)
+      atomicMax(p.aux_trace + 9, now);                              // ... latest / earliest over the CTAs
+      atomicMin(p.aux_trace + 10, now);
+      atomicMax(p.aux_trace + 11, now);
+    }
     if (p.wait_stats != nullptr && threadIdx.x == 0) {
-      p.wait_stats[8ll * blockIdx.x + 6] = static_cast<unsigned long long>(w_epi);
-      p.wait_stats[8ll * blockIdx.x + 7] = static_cast<unsigned long long>(clock_cycles() - epi_start);
+      p.wait_stats[8ll * blockIdx.x + 1] = static_cast<unsigned long long>(w_full);
+      p.wait_stats[8ll * blockIdx.x + 3] = static_cast<unsigned long long>(clock_cycles() - c_start);
     }
     if constexpr (kMode == kModeLoss) {
       // all sigma slabs of this warp must be in global memory before the kernel ends
       if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-      // fixed-order reduction: lanes -> warp -> epilogue warps -> one slot per CTA (summed later in slot order)
+      // fixed-order reduction: lanes -> warp -> consumer warps -> one slot per CTA (summed later in slot order)
       double d_sp = warp_sum(static_cast<double>(s_sp) - static_cast<double>(c_sp));
       double d_g = warp_sum(static_cast<double>(s_g) - static_cast<double>(c_g));
       // sum g * acc -> sum g * <img, txt>
@@ -1013,7 +901,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       named_barrier_sync(1, kNumEpiWarps * 32);
       if (warp == 0) {
         unsigned int ticket = 0;
-        // 16 warps x 3 sums: lanes 0..15 take one warp's triple each, fixed shuffle tree (same order every run)
+        // 8 warps x 3 sums: lanes 0..7 take one warp's triple each, fixed shuffle tree (same order every run)
         double s0 = (lane < kNumEpiWarps) ? red[lane * 3 + 0] : 0.0;
         double s1 = (lane < kNumEpiWarps) ? red[lane * 3 + 1] : 0.0;
         double s2 = (lane < kNumEpiWarps) ? red[lane * 3 + 2] : 0.0;
@@ -1039,7 +927,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
           ticket = __shfl_sync(0xffffffffu, ticket, 0);
           if (ticket == gridDim.x - 1) {
             // last CTA of the forward's last loss kernel: every slot is final. One warp, slot order and a fixed
-            // shuffle tree => bitwise reproducible for a fixed grid (the former finalize kernel, without its launch)
+            // shuffle tree => bitwise reproducible for a fixed grid
             __threadfence();
             double f0 = 0.0, f1 = 0.0, f2 = 0.0;
             for (unsigned int i = lane; i < gridDim.x; i += 32) {
@@ -1062,7 +950,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
         }
       }
     }
-  } else {
+  } else if (warp >= kAuxWarp) {
     // ===================== the two auxiliary warps: NVSwitch peer pull, conversions, fold =====================
     // A text chunk is read ONCE from its owner's buffer (P2P over NVLink) into local HBM while the previous chunk's
     // tiles compute (replaces distributed_utils.py:10-27 neighbour_exchange / the all_gather at
@@ -1070,7 +958,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
     // contributions are folded into a local fp32 accumulator the same way (the reduce-scatter of all_gather's backward,
     // torch functional.py:343-354, spread over the steps instead of exposed at the end). Buffer hand-over between the
     // ranks is by flags: waits before a job, release-stores once every CTA has finished its share of it.
-    const int aux_tid = static_cast<int>(threadIdx.x) - kAllocWarp * 32;
+    const int aux_tid = static_cast<int>(threadIdx.x) - kAuxWarp * 32;
     const unsigned long long nthreads = static_cast<unsigned long long>(gridDim.x) * 64ull;
     const unsigned long long tid0 = static_cast<unsigned long long>(blockIdx.x) * 64ull + aux_tid;
     const bool tracer = (p.aux_trace != nullptr && blockIdx.x == 0 && aux_tid == 0);
@@ -1169,15 +1057,10 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
   }
 
   // ===================================== teardown =====================================
-  tc_fence_before();
-  if constexpr (kClusterSize > 1) {
+  if constexpr (kCS > 1) {
     cluster_sync_all();   // peers may still multicast into this CTA's smem / arrive on its barriers
   } else {
     __syncthreads();
-  }
-  if (warp == kAllocWarp) {
-    tc_fence_after();
-    tmem_dealloc<kCG>(tmem_base, kTmemCols);
   }
   // every warp of this CTA is past its last global write (barrier above): the last CTA of the launch tells the peers
   if (threadIdx.x == 0 && p.aux_trace != nullptr) atomicMin(p.aux_trace + 8, globaltimer_ns());   // first CTA to finish
@@ -1476,12 +1359,11 @@ __global__ void normalize_bwd_kernel(const void* __restrict__ x, const float* __
   }
 }
 
-template <int kCG, int kMode, int kStages, int kMC>
+template <int kMode, int kStages, int kCS, bool kF8 = false>
 int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensorMap* tmA1, const CUtensorMap* tmB1,
                 const CUtensorMap* tmG, const KernelParams& p, int num_sms, cudaStream_t stream) {
-  using C = Cfg<kCG, kMode, kStages>;
-  constexpr int kClusterSize = kCG * kMC;
-  auto kern = siglip_gemm_kernel<kCG, kMode, kStages, kMC>;
+  using C = Cfg<kMode, kStages>;
+  auto kern = siglip_gemm_kernel<kMode, kStages, kCS, kF8>;
   static bool attr_set = false;
   cudaError_t e = cudaSuccess;
   if (!attr_set) {
@@ -1489,15 +1371,21 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
     if (e != cudaSuccess) return static_cast<int>(e);
     attr_set = true;
   }
-  int total_tiles = ((p.prob[0].tiles_m + kMC - 1) / kMC) * p.prob[0].tiles_n;
-  if (p.nprob > 1) total_tiles += ((p.prob[1].tiles_m + kMC - 1) / kMC) * p.prob[1].tiles_n;
+  KernelParams pl = p;
+  int total_tiles = 0;
+  for (int i = 0; i < pl.nprob; ++i) {
+    Problem& pr = pl.prob[i];
+    pr.tiles_m = (pr.M + kBlockM * kCS - 1) / (kBlockM * kCS);
+    pr.tiles_n = (pr.N + kTileN - 1) / kTileN;
+    total_tiles += pr.tiles_m * pr.tiles_n;
+  }
   cudaLaunchConfig_t cfg{};
   cfg.blockDim = dim3(kNumThreads);
   cfg.dynamicSmemBytes = C::kSmemBytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = kClusterSize;
+  attr[0].val.clusterDim.x = kCS;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -1508,19 +1396,18 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
   // how many fit (once per instantiation) instead of assuming num_sms / cluster size.
   static int max_clusters = -1;
   if (max_clusters < 0) {
-    cfg.gridDim = dim3((num_sms / kClusterSize) * kClusterSize);
+    cfg.gridDim = dim3((num_sms / kCS) * kCS);
     int n = 0;
     if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) {
       cudaGetLastError();
-      n = num_sms / kClusterSize;
+      n = num_sms / kCS;
     }
     max_clusters = n;
-    if (getenv("SIGLIP_DEBUG_WAITSTATS")) printf("[launch] cluster size %d: %d co-resident clusters\n", kClusterSize, n);
+    if (getenv("SIGLIP_DEBUG_WAITSTATS")) printf("[launch] cluster size %d: %d co-resident clusters\n", kCS, n);
   }
-  int clusters = max_clusters < num_sms / kClusterSize ? max_clusters : num_sms / kClusterSize;
-  KernelParams pl = p;
+  int clusters = max_clusters < num_sms / kCS ? max_clusters : num_sms / kCS;
   pl.sk_parts = 0;
-  if (kMode == kModeOut && kMC == 1 && p.sk_request != 0 && p.sk_ws != nullptr && clusters > 1) {
+  if (kMode == kModeOut && p.sk_request != 0 && p.sk_ws != nullptr && clusters > 1) {
     // Split-K of the ragged last wave: `rem` tiles left after the full waves would occupy rem of `clusters` units for
     // a whole tile time. Cut each of them into S = floor(clusters / rem) K-slices (S * rem <= clusters work items, one
     // per unit): the last wave then lasts ~1/S of a tile. Not worth it when the last wave is more than half full
@@ -1533,7 +1420,7 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
       if (p.sk_request > 1 && S > p.sk_request) S = p.sk_request;
       if (p.sk_request < 0 && S > 4) S = 4;
       while (S > 1 && num_kb / S < 8) --S;
-      const size_t need = static_cast<size_t>(rem) * (S - 1) * kCG * (8 * 8 * kBlockM) * sizeof(float4);
+      const size_t need = static_cast<size_t>(rem) * (S - 1) * kCS * kBlockM * kTileN * sizeof(float);
       if (S >= 2 && rem <= p.sk_max_tiles && need <= p.sk_ws_bytes) {
         pl.sk_parts = S;
         pl.sk_tiles = rem;
@@ -1544,7 +1431,7 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
   }
   if (clusters > total_tiles) clusters = total_tiles;
   if (clusters < 1) clusters = 1;
-  cfg.gridDim = dim3(clusters * kClusterSize);
+  cfg.gridDim = dim3(clusters * kCS);
   cfg.numAttrs = pl.pdl ? 2 : 1;
   e = cudaLaunchKernelEx(&cfg, kern, *tmA0, *tmB0, *tmA1, *tmB1, *tmG, pl);
   return static_cast<int>(e);
@@ -1552,99 +1439,73 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
 
 }  // namespace
 
-int query_max_active_clusters(int cta_group) {
-  int n = -1;
+int query_max_active_clusters(int cluster) {
+  int n = -1, dev = 0, num_sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return n;
   cudaLaunchConfig_t cfg{};
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.x = cluster;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   cfg.blockDim = dim3(kNumThreads);
-  cfg.gridDim = dim3(148);
-  if (cta_group == 2) {
-    auto kern = siglip_gemm_kernel<2, kModeOut, 7, 1>;
-    cfg.dynamicSmemBytes = Cfg<2, kModeOut, 7>::kSmemBytes;
+  cfg.gridDim = dim3((num_sms / cluster) * cluster);
+  cfg.dynamicSmemBytes = Cfg<kModeOut, 6>::kSmemBytes;
+  auto query = [&](auto kern) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cfg.dynamicSmemBytes);
     cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
-  } else {
-    auto kern = siglip_gemm_kernel<1, kModeOut, 4, 2>;
-    cfg.dynamicSmemBytes = Cfg<1, kModeOut, 4>::kSmemBytes;
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cfg.dynamicSmemBytes);
-    cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
-  }
+  };
+  if (cluster == 4)
+    query(siglip_gemm_kernel<kModeOut, 6, 4>);
+  else if (cluster == 2)
+    query(siglip_gemm_kernel<kModeOut, 6, 2>);
+  else
+    query(siglip_gemm_kernel<kModeOut, 6, 1>);
   return n;
 }
 
-int default_stages(int cta_group, int mode) {
-  if (mode == kModeLoss) return cta_group == 2 ? 6 : 4;
-  return cta_group == 2 ? 7 : 4;
+int default_stages(int /*mode*/) { return 6; }
+
+size_t gemm_smem_bytes(int mode) {
+  return mode == kModeLoss ? static_cast<size_t>(Cfg<kModeLoss, 6>::kSmemBytes)
+                           : static_cast<size_t>(Cfg<kModeOut, 6>::kSmemBytes);
 }
 
-size_t gemm_smem_bytes(int cta_group, int mode) {
-  if (mode == kModeLoss)
-    return cta_group == 2 ? static_cast<size_t>(Cfg<2, kModeLoss, 6>::kSmemBytes)
-                          : static_cast<size_t>(Cfg<1, kModeLoss, 4>::kSmemBytes);
-  return cta_group == 2 ? static_cast<size_t>(Cfg<2, kModeOut, 7>::kSmemBytes)
-                        : static_cast<size_t>(Cfg<1, kModeOut, 4>::kSmemBytes);
-}
+#define SIGLIP_LAUNCH(MODE, ST, CS) \
+  return launch_impl<MODE, ST, CS>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
 
-#define SIGLIP_LAUNCH(CG, MODE, ST, MC) \
-  return launch_impl<CG, MODE, ST, MC>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+#define SIGLIP_LAUNCH_STAGES(MODE, CS)   \
+  do {                                   \
+    if (stages == 4) SIGLIP_LAUNCH(MODE, 4, CS); \
+    SIGLIP_LAUNCH(MODE, 6, CS);          \
+  } while (0)
 
 int launch_gemm(int cta_group, int mode, int stages, int mcast, const CUtensorMap* tmA0, const CUtensorMap* tmB0,
                 const CUtensorMap* tmA1, const CUtensorMap* tmB1, const CUtensorMap* tmG, const KernelParams& p,
                 int num_sms, cudaStream_t stream) {
-  if (stages <= 0) stages = default_stages(cta_group, mode);
-  if (cta_group == 2 && mcast == 2) {  // 2x2 clusters: two MMA pairs share the B tile by TMA multicast
-    if (mode == kModeLoss) {
-      switch (stages) {
-        case 4: SIGLIP_LAUNCH(2, kModeLoss, 4, 2);
-        default: SIGLIP_LAUNCH(2, kModeLoss, 6, 2);
-      }
-    }
-    switch (stages) {
-      case 4: SIGLIP_LAUNCH(2, kModeOut, 4, 2);
-      default: SIGLIP_LAUNCH(2, kModeOut, 7, 2);
-    }
+  if (stages <= 0) stages = default_stages(mode);
+  if (mode == kModeOut && p.prob[0].ab_f16 == 2) {   // 8-bit measurement path: K-major, no multicast, no split-K
+    if (cluster_size(cta_group, mcast) == 2)
+      return launch_impl<kModeOut, 6, 2, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+    return launch_impl<kModeOut, 6, 1, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
   }
-  if (cta_group == 2) {  // 2-CTA MMA pairs, no operand multicast
-    if (mode == kModeLoss) {
-      switch (stages) {
-        case 4: SIGLIP_LAUNCH(2, kModeLoss, 4, 1);
-        default: SIGLIP_LAUNCH(2, kModeLoss, 6, 1);
-      }
-    }
-    switch (stages) {
-      case 4: SIGLIP_LAUNCH(2, kModeOut, 4, 1);
-      default: SIGLIP_LAUNCH(2, kModeOut, 7, 1);
-    }
-  }
-  if (mcast == 2) {  // 1-CTA MMA, clusters of 2 sharing the B tile by TMA multicast
-    if (mode == kModeLoss) {
-      switch (stages) {
-        case 3: SIGLIP_LAUNCH(1, kModeLoss, 3, 2);
-        default: SIGLIP_LAUNCH(1, kModeLoss, 4, 2);
-      }
-    }
-    switch (stages) {
-      case 3: SIGLIP_LAUNCH(1, kModeOut, 3, 2);
-      default: SIGLIP_LAUNCH(1, kModeOut, 4, 2);
-    }
-  }
-  if (mode == kModeLoss) {
-    switch (stages) {
-      case 3: SIGLIP_LAUNCH(1, kModeLoss, 3, 1);
-      default: SIGLIP_LAUNCH(1, kModeLoss, 4, 1);
-    }
-  }
-  switch (stages) {
-    case 3: SIGLIP_LAUNCH(1, kModeOut, 3, 1);
-    default: SIGLIP_LAUNCH(1, kModeOut, 4, 1);
+  switch (cluster_size(cta_group, mcast)) {
+    case 4:
+      if (mode == kModeLoss) SIGLIP_LAUNCH_STAGES(kModeLoss, 4);
+      SIGLIP_LAUNCH_STAGES(kModeOut, 4);
+    case 2:
+      if (mode == kModeLoss) SIGLIP_LAUNCH_STAGES(kModeLoss, 2);
+      SIGLIP_LAUNCH_STAGES(kModeOut, 2);
+    default:
+      if (mode == kModeLoss) SIGLIP_LAUNCH_STAGES(kModeLoss, 1);
+      SIGLIP_LAUNCH_STAGES(kModeOut, 1);
   }
 }
+#undef SIGLIP_LAUNCH_STAGES
 #undef SIGLIP_LAUNCH
 
 int launch_reduce_slots(void* out, int out_bf16, const float* const* slots_dev, int nslots, size_t n, int num_sms,

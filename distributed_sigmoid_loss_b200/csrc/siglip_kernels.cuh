@@ -1,4 +1,4 @@
-// Host-visible declarations of the sm_100a kernels (definitions in siglip_kernels.cu).
+// Host-visible declarations of the sm_90a kernels (definitions in siglip_kernels.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -9,17 +9,16 @@
 
 namespace siglip {
 
-// One dense contraction C[M,N] = A[M,K] * B[N,K]^T on the tcgen05 pipe.
+// One dense contraction C[M,N] = A[M,K] * B[N,K]^T on the wgmma tensor cores, in 128 x 128 tiles (one per CTA).
 // `a_mn` / `b_mn` say how the operand sits in memory:
-//   0: K-major  — global tensor is [rows][K], K contiguous      (TMA box {64 k, rows})
-//   1: MN-major — global tensor is [K][rows], rows contiguous   (TMA boxes {64 rows, 64 k})
+//   0: K-major  — global tensor is [rows][K], K contiguous      (TMA box {64 k, rows}: A 128 rows, B kTileN / cluster)
+//   1: MN-major — global tensor is [K][rows], rows contiguous   (TMA boxes {64 rows, 64 k}; B of a 4-CTA cluster {64, 32})
 struct Problem {
   int M, N, K;
-  int tiles_m, tiles_n;
-  int tile_n;       // out kernel, N-major B: 128 = narrow column tiles (tiles_n = ceil(N / 128)); 0 / 256 = default
+  int tiles_m, tiles_n;   // filled in by launch_gemm: row panels of one cluster, 128-column tiles
   int a_mn, b_mn;
   int ab_f16;       // 0: bf16 operands; 1: both IEEE fp16 (gradient contractions: scaled sigma x scaled embeddings);
-                    // 2: both fp8 e4m3, K-major only (kind::f8f6f4 — the SURVEY.md §8f-4 measurement, siglip_debug_gemm)
+                    // 2: both fp8 e4m3, K-major only (the SURVEY.md §8f-4 measurement, siglip_debug_gemm)
   float acc_scale;  // multiplies the accumulator in the out epilogue (2^-k for a 2^k-scaled fp16 A operand)
   // epilogue of the "out" kernel:
   //   out = scale * (acc * acc_scale + fix_vec[row] * fix_mat[row, col]) (+ add_src[row, col]); fp32 or bf16 output
@@ -91,7 +90,6 @@ struct KernelParams {
   float* sc_dbias;
   DebugRecord* dbg;
   unsigned long long* wait_stats;  // optional [gridDim.x][4]: producer empty-wait, MMA full-wait, MMA tmem-wait, MMA loop cycles
-  unsigned int epi_sleep_ns;  // back-off of the epilogue warps while they wait for an accumulator (0 = spin)
   // Work of the two auxiliary warps of every CTA while the tiles compute: up to kMaxAuxJobs jobs executed in order,
   // each spread over all CTAs of the launch (grid-stride over 16-byte vectors). This is where the cross-rank exchange
   // lives: peer pulls of text chunks and folds of the peers' dtxt contributions over NVSwitch P2P, ordered by flags.
@@ -114,7 +112,7 @@ struct KernelParams {
   int sk_first;
   int sk_tiles;
   int sk_request;              // host request to launch_gemm: -1 choose, 0 off, S >= 2
-  float* sk_ws;                // [sk_tiles][sk_parts - 1][cta_group][8 slabs][8][128] float4
+  float* sk_ws;                // [sk_tiles][sk_parts - 1][cluster CTA][128 x 128 fp32 in fragment order]
   size_t sk_ws_bytes;
   unsigned int* sk_counters;   // [sk_tiles][2]: arrivals of the non-owner warps, owner warps that consumed them
   int sk_max_tiles;            // capacity of sk_counters
@@ -125,17 +123,26 @@ struct KernelParams {
 
 enum KernelMode { kModeLoss = 0, kModeOut = 1 };
 
-// Dynamic shared memory needed by the default configuration of (cta_group, mode).
-size_t gemm_smem_bytes(int cta_group, int mode);
-int default_stages(int cta_group, int mode);
-int query_max_active_clusters(int cta_group);  // co-resident clusters of the out kernel (diagnostic)
+constexpr int kTileCols = 128;   // columns of a tile (wgmma N); a CTA computes 128 rows of it
 
-// Launch the warp-specialised persistent kernel. `stages` <= 0 selects the default pipeline depth.
-// tmG: store map of the sigma operand (loss mode; 16-bit [B, B], box {32, 32}, 64B swizzle) — any valid map in out mode.
+// CTAs per cluster: cta_group (1 or 2) CTAs compute one 128- or 256-row tile, mcast (1 or 2) such tiles share their B
+// tile as well; either way a cluster is a column of vertically adjacent 128-row blocks sharing B through TMA multicast.
+inline int cluster_size(int cta_group, int mcast) { return cta_group * mcast; }
+// Box of the B operand's tensor map for a cluster of `cs` CTAs (each CTA fetches 1 / cs of the B tile):
+// K-major rows, MN-major k extent.
+inline int b_box_rows_kmajor(int cs) { return kTileCols / cs; }
+inline int b_box_k_mnmajor(int cs) { return cs == 4 ? 32 : 64; }
+
+// Dynamic shared memory needed by the default configuration of `mode`.
+size_t gemm_smem_bytes(int mode);
+int default_stages(int mode);
+int query_max_active_clusters(int cluster);  // co-resident clusters of the out kernel (diagnostic)
+
+// Launch the warp-specialised persistent kernel. `stages` <= 0 selects the default pipeline depth (4 or 6).
+// tmG: store map of the sigma operand (loss mode; 16-bit [B, B], box {32, 16}, 64B swizzle) — any valid map in out mode.
 // Returns cudaError_t as int.
-// mcast: 1 = every CTA (pair) loads its own operands; 2 = clusters of two CTAs (cta_group 1) or two MMA pairs
-// (cta_group 2: a 2x2 cluster) on vertically adjacent tiles share the B tile through TMA multicast; the K-major B map
-// must then have box rows 256 / (cta_group * mcast).
+// cta_group x mcast = CTAs per cluster (1, 2 or 4); the B maps must have the boxes b_box_rows_kmajor /
+// b_box_k_mnmajor give for that cluster size.
 int launch_gemm(int cta_group, int mode, int stages, int mcast, const CUtensorMap* tmA0, const CUtensorMap* tmB0,
                 const CUtensorMap* tmA1, const CUtensorMap* tmB1, const CUtensorMap* tmG, const KernelParams& p,
                 int num_sms, cudaStream_t stream);

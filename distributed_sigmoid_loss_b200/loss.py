@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's module surface over the sm_100a C-ABI library.
+"""Host-side mirror of the reference's module surface over the sm_90a C-ABI library.
 
 Reference interface (ahmdtaha/distributed_sigmoid_loss):
   * ``DDPSigmoidLoss(gpu_batch_size).forward(image_embeddings, text_embeddings)``
@@ -51,7 +51,7 @@ class SigmoidLossEngine:
                  batch_per_rank=None):
         self._L = _capi.lib()
         if not torch.cuda.is_available() or self._L.siglip_device_count() == 0:
-            raise RuntimeError("distributed_sigmoid_loss_b200 needs an sm_100 (B200) device; there is no CPU fallback")
+            raise RuntimeError("distributed_sigmoid_loss_b200 needs an sm_90 (H100) device; there is no CPU fallback")
         self.batch, self.dim, self.device, self.group = batch, dim, torch.device(device), group
         self.rank, self.world = rank_world if rank_world is not None else _group_rank_world(group)
         h = ctypes.c_void_p()
@@ -502,7 +502,7 @@ def _validate(image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, exp
             f"The size of tensor a ({image_embeddings.shape[0]}) must match the size of tensor b ({expect_batch}): "
             "batch does not equal gpu_batch_size")
     if image_embeddings.device.type != "cuda" or text_embeddings.device != image_embeddings.device:
-        raise RuntimeError("distributed_sigmoid_loss_b200 runs on CUDA (sm_100a) tensors only; there is no CPU path")
+        raise RuntimeError("distributed_sigmoid_loss_b200 runs on CUDA (sm_90a) tensors only; there is no CPU path")
 
 
 def _pad_dim(x: torch.Tensor) -> torch.Tensor:

@@ -48,9 +48,9 @@ static double softplus(double x) { return x > 0 ? x + log1p(exp(-x)) : log1p(exp
 int main(void) {
   const int B = 384, D = 128;
   const float t_prime = logf(10.0f), bias = -10.0f;
-  printf("%s, %d sm_100 device(s)\n", siglip_version(), siglip_device_count());
+  printf("%s, %d sm_90 device(s)\n", siglip_version(), siglip_device_count());
   if (siglip_device_count() == 0) {
-    fprintf(stderr, "no B200: this library has no CPU fallback\n");
+    fprintf(stderr, "no H100: this library has no CPU fallback\n");
     return 1;
   }
   const size_t n = (size_t)B * D;

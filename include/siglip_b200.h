@@ -1,5 +1,5 @@
 /*
- * siglip_b200.h — C ABI of the B200-native distributed sigmoid (SigLIP) loss hot path.
+ * siglip_b200.h — C ABI of the H100-native (sm_90a) distributed sigmoid (SigLIP) loss hot path.
  *
  * The reference (ahmdtaha/distributed_sigmoid_loss) has no FFI layer: its boundary is the Python
  * nn.Module `DDPSigmoidLoss.forward(image_embeddings, text_embeddings)` (distributed_sigmoid_loss.py:8-48)
@@ -28,7 +28,7 @@ enum {
   SIGLIP_OK = 0,
   SIGLIP_ERR_INVALID = 1,   /* bad argument / shape (reference: broadcast RuntimeError when B != gpu_batch_size) */
   SIGLIP_ERR_CUDA = 2,      /* a CUDA runtime / driver call failed */
-  SIGLIP_ERR_NO_DEVICE = 3, /* no sm_100 device: there is NO CPU fallback */
+  SIGLIP_ERR_NO_DEVICE = 3, /* no sm_90 device: there is NO CPU fallback */
   SIGLIP_ERR_STATE = 4      /* call sequence error (e.g. world > 1 without imported peer handles) */
 };
 
@@ -38,20 +38,23 @@ enum {
  *   SIGLIP_DEBUG_NO_GSTORE, SIGLIP_DEBUG_NO_CVT   timing experiments: skip the sigma store / the fp16 operand copies
  *                                (the gradients are then WRONG)
  *   SIGLIP_DEBUG_PRINT_TIMES     print the per-launch CUDA-event times collected under SIGLIP_OPT_KERNEL_TIMING
- *   SIGLIP_DEBUG_MCAST, _AB_F16, _WAITSTATS, _EPI_SLEEP, _STAGES   variants of siglip_debug_gemm(_timed) only
+ *   SIGLIP_DEBUG_MCAST, _AB_F16, _AB_FP8, _WAITSTATS, _STAGES   variants of siglip_debug_gemm(_timed) only
  */
 
 /* tuning knobs (siglip_ctx_set_option) */
 enum {
-  SIGLIP_OPT_CTA_GROUP = 1, /* 1: cta_group::1 128x256 tiles; 2: cta_group::2 256x256 tiles per SM pair (default) */
+  SIGLIP_OPT_CTA_GROUP = 1, /* 1: every CTA computes its own 128-row tile; 2 (default): clusters of two CTAs on adjacent
+                               128-row blocks share the B tile by TMA multicast. Tiles are 128 columns wide */
   SIGLIP_OPT_OVERLAP_PULL = 2, /* 1 (default): pull the next text chunk inside the loss kernel; 0: separate copy */
   SIGLIP_OPT_KERNEL_TIMING = 3, /* 1: bracket every loss / gradient kernel launch with CUDA events on the caller's stream */
-  SIGLIP_OPT_STAGES_LOSS = 4,  /* TMA->MMA pipeline depth of the loss kernel (0 = default) */
+  SIGLIP_OPT_STAGES_LOSS = 4,  /* TMA->MMA pipeline depth of the loss kernel: 0 (default, = 6), 4 or 6 */
   SIGLIP_OPT_STAGES_GRAD = 5,  /* ... of the gradient kernel */
-  SIGLIP_OPT_MCAST = 6,        /* 2: vertically adjacent tiles share the B tile by TMA multicast (cta_group 2: 2x2 clusters); default 1 */
+  SIGLIP_OPT_MCAST = 6,        /* 2: twice as many vertically adjacent CTAs share the B tile by TMA multicast (cta_group 2:
+                                  clusters of 4); default 1 */
   SIGLIP_OPT_GRAD_BF16 = 7,     /* 1: siglip_fwd_bwd writes dimg / dtxt as bf16 [B, D] (the dtype autograd returns for bf16 inputs); default 0 = fp32 */
   SIGLIP_OPT_OVERLAP_REDUCE = 8, /* 1 (default): fold the peers' dtxt contributions in step by step inside the gradient kernels; 0: one reduction at the end */
-  SIGLIP_OPT_EPI_SLEEP_GRAD_NS = 9, /* nanosleep back-off of the epilogue warps while they wait for an accumulator (gradient kernel) */
+  SIGLIP_OPT_EPI_SLEEP_GRAD_NS = 9, /* accepted, no effect on sm_90a: the warps that run the epilogue also issue the MMAs
+                                       and never wait idle for an accumulator (gradient kernel) */
   SIGLIP_OPT_EPI_SLEEP_LOSS_NS = 10, /* ... (loss kernel) */
   SIGLIP_OPT_SYNC_SCALAR_GRADS = 11, /* 1: siglip_backward returns the MEAN over ranks of dt_prime / dbias (what DDP's
                                         all-reduce of the two parameters does, README.md:20,
@@ -65,7 +68,8 @@ enum {
                                 bf16: 11 significant bits for callers with fp32 embeddings (the reference's own test feeds fp32,
                                 test_distributed_sigmoid_loss.py:57-68; bf16 rounding of such inputs costs 1.7e-3 in the
                                 gradients, this format 2e-4). Same on all ranks. Default 0 */
-  SIGLIP_OPT_GRAD_TILE_N = 14, /* column-tile width of the gradient kernel: 0 (default) = choose by wave fill, 128, 256 */
+  SIGLIP_OPT_GRAD_TILE_N = 14, /* 0, 128 or 256; accepted, no effect on sm_90a: every column tile is 128 wide (the wgmma
+                                  accumulator lives in registers) */
   SIGLIP_OPT_PEER_TIMEOUT_MS = 15, /* bound of every in-kernel wait on a PEER rank (text-ready / contribution-ready /
                                       buffer-free flags, scalar exchange). Default 600000 (10 min, the order of a process
                                       group's collective timeout: a peer may be late by a checkpoint save or an evaluation
@@ -73,7 +77,7 @@ enum {
                                       creation. On expiry the kernel records the wait site and traps: the next call
                                       returns SIGLIP_ERR_CUDA naming it. Waits on the kernel's own mbarriers keep their
                                       4 s bound. */
-  SIGLIP_OPT_INKERNEL_SYNC = 16, /* 1 (default): siglip_fwd_bwd waits for / raises every cross-rank flag inside its tcgen05
+  SIGLIP_OPT_INKERNEL_SYNC = 16, /* 1 (default): siglip_fwd_bwd waits for / raises every cross-rank flag inside its wgmma
                                     kernels (a W-rank step is exactly 2W launches); 0: separate one-block wait / signal
                                     kernels and a copy around them (A/B measurements) */
   SIGLIP_OPT_SPLIT_K = 17, /* gradient kernel, tiles of a ragged last wave: 0 (default) never split; -1 split them
@@ -81,8 +85,8 @@ enum {
                               through a workspace, fixed-order sum: bitwise independent of which CTA finishes first).
                               Measured: no gain at the shapes tried (the last wave is not what a short launch waits for),
                               so it stays opt-in */
-  SIGLIP_OPT_PDL = 19, /* 1 (default): the tcgen05 kernels are launched with programmatic stream serialization: their
-                          set-up (barriers, TMEM allocation, descriptor prefetch) overlaps the tail of the previous kernel
+  SIGLIP_OPT_PDL = 19, /* 1 (default): the wgmma kernels are launched with programmatic stream serialization: their
+                          set-up (barrier initialisation, descriptor prefetch) overlaps the tail of the previous kernel
                           of the stream; griddepcontrol.wait orders every global access behind it. 0: plain launches */
   SIGLIP_OPT_TPRIME_F64 = 20, /* 1: the t_prime pointer given to siglip_forward / siglip_backward / siglip_fwd_bwd(_scaled)
                                  is an fp64 device scalar — the dtype of the reference's parameter
@@ -92,13 +96,13 @@ enum {
                                last peer flag seen, jobs done, end of launch); read with siglip_ctx_aux_trace */
 };
 
-/* Library / build identification: "siglip_b200 <version> sm_100a". */
+/* Library / build identification: "siglip_b200 <version> sm_90a". */
 const char* siglip_version(void);
 
 /* Text of the last error on the calling thread ("" if none). */
 const char* siglip_last_error(void);
 
-/* Number of CUDA devices with compute capability 10.x visible to the process (0 on a CPU-only box). */
+/* Number of CUDA devices with compute capability 9.x visible to the process (0 on a CPU-only box). */
 int siglip_device_count(void);
 
 /*
@@ -240,7 +244,7 @@ int siglip_ctx_kernel_times(siglip_ctx* ctx, double* loss_ms, int* loss_launches
 unsigned long long siglip_ctx_launch_count(const siglip_ctx* ctx);
 
 /*
- * Test hook: plain contraction C[M,N] (fp32) = A * B^T on the same tcgen05 mainloop, to pin the operand
+ * Test hook: plain contraction C[M,N] (fp32) = A * B^T on the same wgmma mainloop, to pin the operand
  * layouts independently of the loss epilogue. a_mn / b_mn: 0 = operand stored [rows][K] (K contiguous),
  * 1 = stored [K][rows] (rows contiguous). lda/ldb/ldc in elements. cta_group 1 or 2.
  */
@@ -268,8 +272,8 @@ int siglip_debug_get_slot(siglip_ctx* ctx, int chunk, float* out_dev, void* cuda
 int siglip_debug_set_mailbox(siglip_ctx* ctx, int peer, float dt_prime, float dbias);
 /* With SIGLIP_OPT_AUX_TRACE: device-synchronise and copy out 16 globaltimer stamps (ns) per launch since the last call:
  * [0..2] auxiliary warps of CTA 0: start, last peer flag observed (0 = no wait), jobs done; [3] launch end as seen by
- * the last CTA; [4] kernel entry (CTA 0); [5] set-up done (barriers, TMEM); [6] first operands landed (MMA warp of CTA 0);
- * [7] last MMA issued (CTA 0); [8] first CTA finished; [9] / [10] latest / earliest "last MMA issued" over the CTAs;
+ * the last CTA; [4] kernel entry (CTA 0); [5] set-up done (barriers); [6] MMAs of the first tile done (CTA 0);
+ * [7] last tile done (CTA 0); [8] first CTA finished; [9] / [10] latest / earliest "last tile done" over the CTAs;
  * [11] last CTA through the epilogue of its tiles; [12] / [13] last / first CTA to enter the kernel; [14] last CTA through
  * its set-up; [15] unused. `out` holds 16 * max_launches values. */
 int siglip_ctx_aux_trace(siglip_ctx* ctx, unsigned long long* out, int max_launches, int* n_launches);

@@ -15,23 +15,23 @@ os.environ.setdefault("SIGLIP_PEER_TIMEOUT_MS", "30000")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (sm_100a) device; run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (sm_90a) device; run with -m gpu on the GPU box")
 
 
 def _cuda_ok() -> bool:
     try:
         import torch
 
-        return torch.cuda.is_available() and torch.cuda.get_device_capability(0)[0] == 10
+        return torch.cuda.is_available() and torch.cuda.get_device_capability(0)[0] == 9
     except Exception:
         return False
 
 
 def pytest_collection_modifyitems(config, items):
-    # `-m gpu` on a box without a B200 should skip, not error (the driver never does that, developers might)
+    # `-m gpu` on a machine without an H100 skips instead of erroring
     if _cuda_ok():
         return
-    skip = pytest.mark.skip(reason="no sm_100 device visible")
+    skip = pytest.mark.skip(reason="no sm_90 device visible")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -1,5 +1,5 @@
-"""bench.py's output contract (one JSON line, the keys the driver reads). The reference arm runs anywhere (CPU);
-this repo's arm needs a B200."""
+"""bench.py's output contract (one JSON line and its keys). The reference arm runs anywhere (CPU); this repo's arm
+needs an H100."""
 import json
 import os
 import subprocess
@@ -22,10 +22,10 @@ def _run(args, timeout=900):
 
 
 def test_reference_arm_line():
-    """`--impl reference` runs the UNMODIFIED reference module from baseline/_ref (tools/fetch_ref.py) when it is there
-    (it is in the build container, and it ships to the GPU box), the oracle port otherwise; a timed step is the full
-    per-rank chunk, so steps x ms_per_step is the time the arm really spent."""
-    have_ref = os.path.exists(os.path.join(ROOT, "baseline", "_ref", "distributed_sigmoid_loss.py"))
+    """`--impl reference` runs the UNMODIFIED reference module from oracle/_ref (oracle/fetch_ref.py, run by build())
+    when it is there, the oracle port otherwise; a timed step is the full per-rank chunk, so steps x ms_per_step is the
+    time the arm really spent."""
+    have_ref = os.path.exists(os.path.join(ROOT, "oracle", "_ref", "distributed_sigmoid_loss.py"))
     d = _run(["--impl", "reference", "--gpus", "1", "--steps", "2", "--warmup", "1", "--batch", "256", "--dim", "64"])
     assert d["impl"] == "reference" and BASE_KEYS <= set(d)
     assert d["metric"] == "image-text pairs/sec" and d["unit"] == "pairs/s" and d["higher_is_better"] is True
@@ -69,3 +69,30 @@ def test_product_arm_line():
     par = d["parity"]
     assert par["pass"] is True and par["shape"] == [2048, 768]
     assert all(v <= 1e-3 for v in par["fused_fp32"].values())
+
+
+@pytest.mark.gpu
+def test_dump_outputs_of_the_timed_path(tmp_path):
+    """--dump-outputs writes the last timed step's five outputs as float32 .npy files, at most 64 MB in all; the inputs
+    are fixed by the arguments, so a second run computes the same outputs."""
+    import numpy as np
+
+    names = ("loss", "dimg", "dtxt", "dt_prime", "dbias")
+    runs = []
+    for i in range(2):
+        out = tmp_path / f"run{i}"
+        d = _run(["--gpus", "1", "--steps", "2", "--warmup", "1", "--batch", "2048", "--dim", "256", "--sustain-ms", "20",
+                  "--no-cpu-baseline", "--no-parity", "--dump-outputs", str(out)])
+        assert d["steps"] == 2
+        assert sorted(p.name for p in out.iterdir()) == sorted(n + ".npy" for n in names)
+        assert sum(p.stat().st_size for p in out.iterdir()) <= 64 << 20
+        arrays = {n: np.load(out / (n + ".npy")) for n in names}
+        assert all(a.dtype == np.float32 for a in arrays.values())
+        assert arrays["dimg"].shape == arrays["dtxt"].shape == (2048, 256) and arrays["loss"].shape == (1,)
+        assert np.isfinite(arrays["loss"]).all() and abs(float(arrays["loss"][0]) - d["loss"]) <= 1e-6 * abs(d["loss"])
+        runs.append(arrays)
+    for n in names:
+        np.testing.assert_allclose(runs[1][n], runs[0][n], rtol=1e-6, atol=0)
+    with pytest.raises(AssertionError):
+        _run(["--impl", "reference", "--steps", "1", "--warmup", "0", "--batch", "64", "--dim", "64",
+              "--dump-outputs", str(tmp_path / "ref")])

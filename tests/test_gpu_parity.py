@@ -1,4 +1,4 @@
-"""Parity of the sm_100a path against the reference (golden fixtures from the unmodified reference, and the pinned
+"""Parity of the sm_90a path against the reference (golden fixtures from the unmodified reference, and the pinned
 oracle at sizes the fixtures do not reach). Everything here goes through the C ABI (ctypes) or the module mirror.
 
 Tolerances (BASELINE.json north_star: "within 1e-3 relative of the reference"):
@@ -61,7 +61,7 @@ def _contribution(eng, k, dtxt):
 
 
 # ---------------------------------------------------------------------------------------------------------
-# operand layouts of the tcgen05 mainloop
+# operand layouts of the wgmma mainloop
 # ---------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("cg", [1, 2])
 @pytest.mark.parametrize("a_f16", [0, 1])
@@ -827,7 +827,7 @@ def test_config2_shape_single_chunk_and_two_chunk_loopback():
 
 def test_config4_shape_single_chunk():
     """BASELINE.json configs[4] per-rank shape (B=32768, D=1152): one full chunk against fp32 autograd on the GPU
-    (a 32768 x 32768 fp32 logits matrix is 4 GiB; autograd keeps a handful of them: fits the 180 GB), plus the
+    (a 32768 x 32768 fp32 logits matrix is 4 GiB; autograd keeps a handful of them: fits the 80 GB), plus the
     size-independent identities."""
     from oracle.siglip_oracle import torch_reference_fp32
 
@@ -1061,7 +1061,7 @@ def test_peer_timeout_option_and_trace_hook():
 
 
 # ---------------------------------------------------------------------------------------------------------
-# split-K of the gradient kernel's ragged last wave; fp8 (kind::f8f6f4) measurement path
+# split-K of the gradient kernel's ragged last wave; fp8 (wgmma e4m3) measurement path
 # ---------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("shape", [(4096, 768), (1000, 136), (2048, 1152), (520, 264), (8192, 768)])
 @pytest.mark.parametrize("cg", [1, 2])
@@ -1094,8 +1094,9 @@ def test_split_k_is_deterministic_and_matches_unsplit(shape, cg):
 
 @pytest.mark.parametrize("cg", [1, 2])
 def test_fp8_measurement_path_computes_the_e4m3_product(cg, monkeypatch):
-    """siglip_debug_gemm under SIGLIP_DEBUG_AB_FP8: e4m3 x e4m3 -> fp32 on the same mainloop (tcgen05 kind::f8f6f4).
-    Products of e4m3 values are exact in fp32, so the result equals the fp32 product of the dequantised operands."""
+    """siglip_debug_gemm under SIGLIP_DEBUG_AB_FP8: e4m3 x e4m3 -> fp32 on the same mainloop (wgmma e4m3, each
+    instruction's result summed in fp32). Products of e4m3 values are exact in fp32, so the result equals the fp32
+    product of the dequantised operands."""
     from distributed_sigmoid_loss_b200 import _capi
     L = _capi.lib()
     monkeypatch.setenv("SIGLIP_DEBUG_AB_FP8", "1")

@@ -1,4 +1,4 @@
-"""Real-peer check under pytest: on a box with two or more B200s, run tools/multi_gpu_check.py (one rank per GPU, NCCL
+"""Real-peer check under pytest: on a machine with two or more H100s, run tools/multi_gpu_check.py (one rank per GPU, NCCL
 process group, CUDA-IPC peer mappings, in-kernel flags over NVSwitch) on two ranks and require every comparison to pass —
 the float64 closed form over the global batch, fp32 autograd with the text gradient all-reduced (the reduce-scatter of
 all_gather's backward, torch distributed/nn/functional.py:343-354), the reference's own acceptance test

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Where does a launch of the tcgen05 kernels spend its time? globaltimer stamps of CTA 0 (SIGLIP_OPT_AUX_TRACE) for
+"""Where does a launch of the wgmma kernels spend its time? globaltimer stamps of CTA 0 (SIGLIP_OPT_AUX_TRACE) for
 back-to-back fused steps at one shape: gap since the previous launch ended, set-up, first operands, MMA issue span, tail
 (last MMA issued -> last CTA done)."""
 import argparse
