@@ -33,6 +33,7 @@ EXPORTED_SYMBOLS = (
     "siglip_fwd_bwd",
     "siglip_fwd_bwd_scaled",
     "siglip_fwd",
+    "siglip_set_sample_ids",
     "siglip_fwd_bwd_host",
     "siglip_convert_f32",
     "siglip_host_submit",
@@ -48,6 +49,7 @@ EXPORTED_SYMBOLS = (
     "siglip_debug_loopback",
     "siglip_debug_set_text_chunk",
     "siglip_debug_get_slot",
+    "siglip_debug_set_chunk_ids",
     "siglip_debug_set_mailbox",
     "siglip_ctx_aux_trace",
     "siglip_ctx_destroy",
@@ -79,6 +81,7 @@ SIGLIP_OPT_SPLIT_K = 17
 SIGLIP_OPT_AUX_TRACE = 18
 SIGLIP_OPT_PDL = 19
 SIGLIP_OPT_TPRIME_F64 = 20
+SIGLIP_OPT_SAMPLE_IDS = 21
 
 _lib: Optional[ctypes.CDLL] = None
 
@@ -172,6 +175,10 @@ def lib() -> ctypes.CDLL:
     L.siglip_debug_set_text_chunk.restype = ci
     L.siglip_debug_get_slot.argtypes = [vp, ci, vp, vp]
     L.siglip_debug_get_slot.restype = ci
+    L.siglip_set_sample_ids.argtypes = [vp, vp, vp]
+    L.siglip_set_sample_ids.restype = ci
+    L.siglip_debug_set_chunk_ids.argtypes = [vp, ci, vp, vp]
+    L.siglip_debug_set_chunk_ids.restype = ci
     L.siglip_ctx_launch_count.argtypes = [vp]
     L.siglip_ctx_launch_count.restype = ctypes.c_ulonglong
     L.siglip_debug_gemm.argtypes = [ci, ci, ci, ci, ci, vp, ctypes.c_longlong, ci, vp, ctypes.c_longlong, ci, vp,

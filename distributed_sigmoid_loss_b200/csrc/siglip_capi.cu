@@ -178,10 +178,16 @@ struct siglip_ctx {
                                          // ragged last wave automatically, S >= 2 = at most S slices
   long long peer_timeout_ms = 600000;    // bound of every wait on a peer (10 min: a peer may be saving a checkpoint)
   int aux_trace_on = 0;
+  int sample_ids = 0;                    // SIGLIP_OPT_SAMPLE_IDS: labels from per-sample ids (collective)
+  bool ids_set = false;                  // siglip_set_sample_ids was called since the previous step
   // diagnostics, read from the environment once at context creation (see include/siglip_b200.h)
   bool dbg_no_gstore = false, dbg_no_cvt = false, dbg_loss_waitstats = false;
   // workspaces
-  __nv_bfloat16* txt_all = nullptr;      // [world][Bmax, D] bf16; slot `rank` is what the peers pull (world > 1)
+  __nv_bfloat16* txt_all = nullptr;      // [world][Bmax, D] bf16; slot `rank` is what the peers pull (world > 1),
+                                         // followed by ids_all in the same (IPC-exported) allocation
+  int64_t* ids_all = nullptr;            // [world][ids_stride] sample ids of every text chunk (world > 1)
+  int64_t* ids_in = nullptr;             // [ids_stride] this rank's ids for the next step (siglip_set_sample_ids)
+  int ids_stride = 0;                    // Bmax rounded up to even: every slot is a whole number of 16-byte vectors
   __nv_bfloat16* G[kMaxWorld] = {};      // [Bp, Bp] sigma operands (fp16 bits x kGScale), diagonal zeroed, allocated on
                                          // first use: fused step 2 (own chunk + the chunk in flight), split API one per chunk
   __nv_bfloat16* img16 = nullptr;        // [B, D] fp16 (x kXScale) images: B operand of the dtxt contraction
@@ -265,6 +271,28 @@ int timing_mark(siglip_ctx* c, std::vector<cudaEvent_t>& evs, size_t& used, cuda
 }
 
 inline size_t chunk_stride(const siglip_ctx* c) { return static_cast<size_t>(c->Bmax) * c->D; }
+
+// Sample ids of text chunk `cidx` as the loss kernel reads them (null outside SIGLIP_OPT_SAMPLE_IDS): the caller's ids
+// for the own chunk, the gathered copy for the others.
+inline const int64_t* chunk_ids(const siglip_ctx* c, int cidx) {
+  if (!c->sample_ids) return nullptr;
+  return (cidx == c->rank) ? c->ids_in : c->ids_all + static_cast<size_t>(cidx) * c->ids_stride;
+}
+// Rank o's published ids slot, seen through its exported text allocation (they sit behind its [world][Bmax, D] text)
+inline const int64_t* peer_ids(const siglip_ctx* c, int o) {
+  return reinterpret_cast<const int64_t*>(c->peer_txt[o] + c->world * chunk_stride(c)) +
+         static_cast<size_t>(o) * c->ids_stride;
+}
+inline size_t ids_bytes(const siglip_ctx* c, int rank) { return static_cast<size_t>(c->Bs[rank]) * sizeof(int64_t); }
+// ids of step s are given once: a step in ids mode consumes them (checked before anything is launched)
+int take_ids(siglip_ctx* c) {
+  if (!c->sample_ids) return 0;
+  if (!c->ids_set)
+    return fail(SIGLIP_ERR_STATE,
+                "SIGLIP_OPT_SAMPLE_IDS is on but siglip_set_sample_ids was not called since the previous step");
+  c->ids_set = false;
+  return 0;
+}
 inline unsigned long long peer_timeout_ns(const siglip_ctx* c) {
   return static_cast<unsigned long long>(c->peer_timeout_ms) * 1000000ull;
 }
@@ -355,9 +383,10 @@ struct FinJob {   // last chunk of a forward: the loss kernel's last CTA writes 
 // The loss kernel over one text chunk (Bn rows, owner's batch): S = img @ txt_c^T on wgmma, fused
 // scale/bias/log-sigmoid/reduce. save: also write the sigma operand G[gi] (+ g_diag on the own chunk); the fp16 copies
 // the gradient kernel needs are auxiliary jobs built by the caller.
+// col_ids: sample ids of the chunk (null = positional labels).
 int run_loss_chunk(siglip_ctx* c, int gi, bool own, bool first, const void* img, const __nv_bfloat16* txt_c, int Bn,
-                   const float* t_prime, const float* bias, bool save, const AuxList& aux, const FinJob* fin,
-                   const EndSignal& end, cudaStream_t st) {
+                   const int64_t* col_ids, const float* t_prime, const float* bias, bool save, const AuxList& aux,
+                   const FinJob* fin, const EndSignal& end, cudaStream_t st) {
   const int cg = c->cta_group;
   int rc;
   if ((rc = ensure_g(c, save ? gi : 0))) return rc;
@@ -389,6 +418,10 @@ int run_loss_chunk(siglip_ctx* c, int gi, bool own, bool first, const void* img,
   p.own_chunk = own ? 1 : 0;
   p.store_g = save ? 1 : 0;
   p.g_scale = kGScale;
+  if (col_ids != nullptr) {
+    p.row_ids = c->ids_in;
+    p.col_ids = col_ids;
+  }
   p.partials = c->partials;
   p.accumulate_partials = first ? 0 : 1;  // the first chunk of a forward overwrites every slot of the grid
   if (fin != nullptr) {
@@ -599,6 +632,35 @@ void add_pull_job(siglip_ctx* c, AuxList& aux, int o, unsigned int s) {
   j.wait_n = 1;
   j.wait_value = s;
   j.site = 5;
+  if (c->sample_ids) {
+    // the chunk's ids ride the same flag: the owner published them before its text signal, and every CTA has
+    // observed that flag in the job above before it runs this one
+    siglip::AuxJob& ji = aux.add(siglip::kAuxCopy);
+    ji.src = reinterpret_cast<const uint4*>(peer_ids(c, o));
+    ji.dst = reinterpret_cast<uint4*>(c->ids_all + static_cast<size_t>(o) * c->ids_stride);
+    ji.n16 = (ids_bytes(c, o) + 15) / 16;   // within the slot: ids_stride is even
+  }
+}
+
+// publish job of my ids (L0 of the fused step): same flag-2 wait as the text publish job that must follow it in the
+// same launch, whose end-of-job signal then covers both copies
+void add_ids_publish_job(siglip_ctx* c, AuxList& aux, unsigned int s) {
+  siglip::AuxJob& j = aux.add(siglip::kAuxCopy);
+  j.src = reinterpret_cast<const uint4*>(c->ids_in);
+  j.dst = reinterpret_cast<uint4*>(c->ids_all + static_cast<size_t>(c->rank) * c->ids_stride);
+  j.n16 = (ids_bytes(c, c->rank) + 15) / 16;
+  j.wait_flags = c->flags + 2 * kMaxWorld;
+  j.wait_n = c->world;
+  j.wait_value = s - 1;
+  j.site = 11;
+}
+
+// the same publish as a stream copy (split forward, helper-kernel variant of the fused step)
+int copy_own_ids(siglip_ctx* c, cudaStream_t st) {
+  if (!c->sample_ids) return 0;
+  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(c->rank) * c->ids_stride, c->ids_in, ids_bytes(c, c->rank),
+                     cudaMemcpyDeviceToDevice, st));
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -613,6 +675,7 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
   if ((rc = check_call(c, img, txt, t_prime, st))) return rc;
   if (bias == nullptr || loss == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if ((rc = check_dbg(c, "siglip forward (previous launch)"))) return rc;
+  if ((rc = take_ids(c))) return rc;
   CK(cudaSetDevice(c->device));
   const int W = c->world, r = c->rank;
   const size_t stride = chunk_stride(c);
@@ -627,6 +690,7 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
     if ((rc = wait_peers(c, 2, s - 1, st))) return rc;
     CK(cudaMemcpyAsync(c->txt_all + r * stride, txt, static_cast<size_t>(c->B) * c->D * sizeof(__nv_bfloat16),
                        cudaMemcpyDeviceToDevice, st));
+    if ((rc = copy_own_ids(c, st))) return rc;   // before the signal, which covers it
     if ((rc = signal_peers(c, 0, s, st))) return rc;
     own_txt = c->txt_all + r * stride;
   }
@@ -650,10 +714,13 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
         if ((rc = wait_one(c, 0, nxt, s, st))) return rc;
         CK(cudaMemcpyAsync(c->txt_all + nxt * stride, c->peer_txt[nxt] + nxt * stride,
                            static_cast<size_t>(c->Bs[nxt]) * c->D * sizeof(__nv_bfloat16), cudaMemcpyDefault, st));
+        if (c->sample_ids)
+          CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(nxt) * c->ids_stride, peer_ids(c, nxt),
+                             ids_bytes(c, nxt), cudaMemcpyDefault, st));
       }
     }
-    if ((rc = run_loss_chunk(c, k, k == 0, k == 0, img, txt_c, c->Bs[cidx], t_prime, bias, save, aux,
-                             (k == W - 1) ? &fin : nullptr, EndSignal(), st)))
+    if ((rc = run_loss_chunk(c, k, k == 0, k == 0, img, txt_c, c->Bs[cidx], chunk_ids(c, cidx), t_prime, bias, save,
+                             aux, (k == W - 1) ? &fin : nullptr, EndSignal(), st)))
       return rc;
   }
   if (W > 1) {
@@ -776,6 +843,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   if (bias == nullptr || loss == nullptr || dimg == nullptr || dtxt == nullptr)
     return fail(SIGLIP_ERR_INVALID, "null argument");
   if ((rc = check_dbg(c, "siglip_fwd_bwd (previous launch)"))) return rc;
+  if ((rc = take_ids(c))) return rc;
   CK(cudaSetDevice(c->device));
   const int W = c->world, r = c->rank;
   const size_t stride = chunk_stride(c);
@@ -800,7 +868,10 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
     if (W > 1) {
       if (ik) {
         // my gathered slot is what the peers pull: they must be done with the previous forward's copy (flag 2),
-        // then "text of forward s in place" (flag 0) goes to every rank once all CTAs have copied their share
+        // then "text of forward s in place" (flag 0) goes to every rank once all CTAs have copied their share. My
+        // ids (sample-id mode) are copied by a job before it: each CTA finishes both before the text job's ticket, so
+        // the same signal covers them.
+        if (c->sample_ids) add_ids_publish_job(c, aux, s);
         siglip::AuxJob& cp = aux.add(siglip::kAuxCopy);
         cp.src = reinterpret_cast<const uint4*>(txt);
         cp.dst = reinterpret_cast<uint4*>(c->txt_all + r * stride);
@@ -815,6 +886,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       } else {
         if ((rc = wait_peers(c, 2, s - 1, st))) return rc;
         CK(cudaMemcpyAsync(c->txt_all + r * stride, txt, own_bytes, cudaMemcpyDeviceToDevice, st));
+        if ((rc = copy_own_ids(c, st))) return rc;
         if ((rc = signal_peers(c, 0, s, st))) return rc;
       }
     }
@@ -834,8 +906,8 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       c->prewait3 = n - 1;
       add_pull_job(c, aux, step_owner(c, r, 1), s);
     }
-    if ((rc = run_loss_chunk(c, 0, true, true, img, own_txt, c->B, t_prime, bias, true, aux, (W == 1) ? &fin : nullptr,
-                             EndSignal(), st)))
+    if ((rc = run_loss_chunk(c, 0, true, true, img, own_txt, c->B, chunk_ids(c, r), t_prime, bias, true, aux,
+                             (W == 1) ? &fin : nullptr, EndSignal(), st)))
       return rc;
   }
   if (W > 1) own_txt = c->txt_all + r * stride;   // the copy the peers see (same bytes)
@@ -849,8 +921,8 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       if (k + 1 < W) add_pull_job(c, aux, step_owner(c, r, k + 1), s);
       const bool lastL = (k == W - 1);
       EndSignal end = (lastL && ik) ? end_signal(c, 2, s) : EndSignal();   // "I have pulled everyone's text"
-      if ((rc = run_loss_chunk(c, 1, false, false, img, txt_c, c->Bs[cidx], t_prime, bias, true, aux,
-                               lastL ? &fin : nullptr, end, st)))
+      if ((rc = run_loss_chunk(c, 1, false, false, img, txt_c, c->Bs[cidx], chunk_ids(c, cidx), t_prime, bias, true,
+                               aux, lastL ? &fin : nullptr, end, st)))
         return rc;
       if (lastL && !ik && (rc = signal_peers(c, 2, s, st))) return rc;
     }
@@ -1009,8 +1081,13 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   CK(alloc(reinterpret_cast<void**>(&c->flags), kFlagBytes));
   CK(alloc(reinterpret_cast<void**>(&c->sync_words), kSyncWords * sizeof(unsigned int)));
   CK(alloc(reinterpret_cast<void**>(&c->scalars), 24 * sizeof(float)));
+  c->ids_stride = round_up(Bmax, 2);
+  const size_t ids_slot_bytes = static_cast<size_t>(c->ids_stride) * sizeof(int64_t);
+  CK(alloc(reinterpret_cast<void**>(&c->ids_in), ids_slot_bytes));
   if (world > 1) {
-    CK(alloc(reinterpret_cast<void**>(&c->txt_all), stride * world * sizeof(__nv_bfloat16)));
+    // the gathered ids live behind the gathered text, so that one exported handle covers both
+    CK(alloc(reinterpret_cast<void**>(&c->txt_all), stride * world * sizeof(__nv_bfloat16) + world * ids_slot_bytes));
+    c->ids_all = reinterpret_cast<int64_t*>(c->txt_all + stride * world);   // 16-byte aligned: D % 8 == 0
     CK(alloc(reinterpret_cast<void**>(&c->slots), stride * world * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dimg_acc), static_cast<size_t>(c->B) * D * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dtxt_acc), static_cast<size_t>(c->B) * D * sizeof(float)));
@@ -1084,6 +1161,10 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
       return 0;
     case SIGLIP_OPT_SYNC_SCALAR_GRADS:
       c->sync_scalar_grads = value ? 1 : 0;
+      return 0;
+    case SIGLIP_OPT_SAMPLE_IDS:
+      c->sample_ids = value ? 1 : 0;
+      c->ids_set = false;
       return 0;
     case SIGLIP_OPT_STAGES_LOSS:
     case SIGLIP_OPT_STAGES_GRAD:
@@ -1221,6 +1302,16 @@ int siglip_ctx_import_handles(siglip_ctx* c, const void* all_ranks_bytes, size_t
   return publish_peer_tables(c);
 }
 
+int siglip_set_sample_ids(siglip_ctx* c, const int64_t* ids_dev, void* cuda_stream) {
+  if (c == nullptr || ids_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->sample_ids) return fail(SIGLIP_ERR_STATE, "siglip_set_sample_ids needs SIGLIP_OPT_SAMPLE_IDS = 1");
+  CK(cudaSetDevice(c->device));
+  CK(cudaMemcpyAsync(c->ids_in, ids_dev, ids_bytes(c, c->rank), cudaMemcpyDeviceToDevice,
+                     static_cast<cudaStream_t>(cuda_stream)));
+  c->ids_set = true;
+  return 0;
+}
+
 int siglip_forward(siglip_ctx* c, const void* img, const void* txt, const float* t_prime, const float* bias,
                    float* loss, int save_for_backward, void* cuda_stream) {
   return forward_impl(c, img, txt, t_prime, bias, loss, save_for_backward != 0, static_cast<cudaStream_t>(cuda_stream));
@@ -1297,6 +1388,8 @@ int siglip_host_submit_grads(siglip_ctx* c, const void* img_host, const void* tx
     return fail(SIGLIP_ERR_INVALID, "null argument");
   if ((dimg_host_bf16 == nullptr) != (dtxt_host_bf16 == nullptr))
     return fail(SIGLIP_ERR_INVALID, "give both gradient host buffers or neither");
+  if (c->sample_ids)
+    return fail(SIGLIP_ERR_STATE, "the host-buffer entries take no sample ids: unavailable under SIGLIP_OPT_SAMPLE_IDS");
   const bool with_grads = dimg_host_bf16 != nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   CK(cudaSetDevice(c->device));
@@ -1453,6 +1546,14 @@ int siglip_debug_set_text_chunk(siglip_ctx* c, int chunk, const void* txt_dev, v
   CK(cudaMemcpyAsync(c->txt_all + chunk * chunk_stride(c), txt_dev,
                      static_cast<size_t>(c->Bs[chunk]) * c->D * sizeof(__nv_bfloat16), cudaMemcpyDeviceToDevice,
                      static_cast<cudaStream_t>(cuda_stream)));
+  return 0;
+}
+
+int siglip_debug_set_chunk_ids(siglip_ctx* c, int chunk, const int64_t* ids_dev, void* cuda_stream) {
+  if (c == nullptr || ids_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
+  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * c->ids_stride, ids_dev, ids_bytes(c, chunk),
+                     cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
 
@@ -1683,6 +1784,7 @@ void free_ctx(siglip_ctx* c) {
     cudaFree(c->txt16[k]);
   }
   cudaFree(c->g_diag);
+  cudaFree(c->ids_in);
   cudaFree(c->img16);
   cudaFree(c->slots);
   cudaFree(c->dimg_acc);

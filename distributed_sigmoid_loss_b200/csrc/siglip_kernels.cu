@@ -304,10 +304,11 @@ __device__ __forceinline__ void loss_slab_fast(const float* v, float tl, float b
 }
 
 // General path. row_lo: global row of this thread's first fragment row; col0: global column of the slab; c_lo as above.
+// pos (kMask only): bit i set = element i is a positive pair by sample id (SIGLIP_OPT_SAMPLE_IDS); 0 without ids.
 template <bool kMask>
 __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int row_lo, int col0, int c_lo, int nrows,
                                           int ncols, bool store_g, const GStore& gst, float gscale, float* g_diag,
-                                          bool on_diag, float& acc_sp, float& acc_g, float& acc_gs) {
+                                          bool on_diag, uint32_t pos, float& acc_sp, float& acc_g, float& acc_gs) {
   uint32_t packed[8];
   float g_prev = 0.f;
 #pragma unroll
@@ -329,8 +330,12 @@ __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int 
       if (on_diag && row == col) {                     // positive pair (label +1): softplus(-z), -sigma(-z)
         sp = fmaxf(-z, 0.f) + l;
         g = -((z >= 0.f) ? e * r : r);                 // sigma(-z) without the 1 - sigma(z) cancellation
-        g_store = 0.f;                                 // the 16-bit operand carries negatives only
+        g_store = 0.f;                                 // the own diagonal stays out of the 16-bit operand
         if (store_g && valid) g_diag[row] = g;
+      } else if ((pos >> i) & 1u) {                    // any other positive (same sample id): same terms, and its
+        sp = fmaxf(-z, 0.f) + l;                       // g * 2^14 in [-16384, 0) goes into the fp16 operand
+        g = -((z >= 0.f) ? e * r : r);
+        g_store = g;
       }
       sp = valid ? sp : 0.f;
       g = valid ? g : 0.f;
@@ -514,13 +519,16 @@ __device__ __forceinline__ void mma_loop_f8(float (&sum)[64], float (&acc)[64], 
 // -------------------------------------------------------------------------------------------------
 // kF8: the out kernel of the 8-bit measurement path (its own instantiation: the extra fp32 result registers of
 // mma_loop_f8 would otherwise cost the production kernels spills).
-template <int kMode, int kStagesT, int kCS, bool kF8 = false>
+// kIds: the loss kernel with labels from sample ids (SIGLIP_OPT_SAMPLE_IDS); its own instantiation, so that the default
+// loss kernel is exactly the code it was without the option.
+template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
                    const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1,
                    const __grid_constant__ CUtensorMap tmG, const __grid_constant__ KernelParams p) {
   using C = Cfg<kMode, kStagesT>;
   static_assert(kCS == 1 || kCS == 2 || kCS == 4, "clusters of 1, 2 or 4 CTAs");
+  static_assert(!kIds || kMode == kModeLoss, "sample ids are a loss-kernel option");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -743,6 +751,13 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
         gst.row0 = row0 + wg * 64 + (warp & 3) * 16;
         gst.lane = lane;
         gst.policy = g_store_policy;
+        // Sample-id labels (kIds): the ids of this thread's two fragment rows, loaded once per tile (a row beyond M takes
+        // row M - 1's id: it only lies in edge slabs, which mask it).
+        int64_t rid0 = 0, rid1 = 0;
+        if constexpr (kIds) {
+          rid0 = p.row_ids[min(row_lo, pr.M - 1)];
+          rid1 = p.row_ids[min(row_lo + 8, pr.M - 1)];
+        }
 #pragma unroll
         for (int c = 0; c < kTileN / 32; ++c) {
           const float* v = acc + 16 * c;
@@ -752,7 +767,26 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
           // the rest of the matrix.
           const bool slab_diag = diag && (gst.row0 < col0 + 32) && (col0 < gst.row0 + 16);
           const bool slab_edge = edge && ((gst.row0 + 16 > pr.M) || (col0 + 32 > pr.N));
-          if (!slab_edge && !slab_diag) {
+          // With sample ids, a slab in which any element's ids match (slab_pos) also takes the label-applying path.
+          // pos bit i <-> fragment element i (row r_lo + 8 ((i >> 1) & 1), column 8 (i >> 2) + c_lo + (i & 1)).
+          uint32_t pos = 0;
+          bool slab_pos = false;
+          if constexpr (kIds) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+#pragma unroll
+              for (int e1 = 0; e1 < 2; ++e1) {
+                const int col = col0 + 8 * j + c_lo + e1;
+                if (col < pr.N) {
+                  const int64_t cid = p.col_ids[col];
+                  pos |= static_cast<uint32_t>(cid == rid0) << (4 * j + e1);
+                  pos |= static_cast<uint32_t>(cid == rid1) << (4 * j + 2 + e1);
+                }
+              }
+            }
+            slab_pos = __any_sync(0xffffffffu, pos != 0u);
+          }
+          if (!slab_edge && !slab_diag && !slab_pos) {
             // z is monotone in s (t > 0): the slab is "all very negative" iff max s is
             float smax = v[0];
 #pragma unroll
@@ -762,10 +796,10 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
               loss_slab_fast(v, tl, bl, col0, sg, gst, p.g_scale, acc_sp, acc_g, acc_gs);
             else
               loss_slab<false>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag, false,
-                               acc_sp, acc_g, acc_gs);
+                               0u, acc_sp, acc_g, acc_gs);
           } else {
             loss_slab<true>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag, slab_diag,
-                            acc_sp, acc_g, acc_gs);
+                            pos, acc_sp, acc_g, acc_gs);
           }
         }
         kahan_add(s_sp, c_sp, acc_sp);
@@ -1359,11 +1393,12 @@ __global__ void normalize_bwd_kernel(const void* __restrict__ x, const float* __
   }
 }
 
-template <int kMode, int kStages, int kCS, bool kF8 = false>
+// kIds selects the sample-id instantiation of the loss kernel (ignored for the out kernel)
+template <int kMode, int kStages, int kCS, bool kF8 = false, bool kIds = false>
 int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensorMap* tmA1, const CUtensorMap* tmB1,
                 const CUtensorMap* tmG, const KernelParams& p, int num_sms, cudaStream_t stream) {
   using C = Cfg<kMode, kStages>;
-  auto kern = siglip_gemm_kernel<kMode, kStages, kCS, kF8>;
+  auto kern = siglip_gemm_kernel<kMode, kStages, kCS, kF8, kIds && kMode == kModeLoss>;
   static bool attr_set = false;
   cudaError_t e = cudaSuccess;
   if (!attr_set) {
@@ -1475,14 +1510,19 @@ size_t gemm_smem_bytes(int mode) {
                            : static_cast<size_t>(Cfg<kModeOut, 6>::kSmemBytes);
 }
 
-#define SIGLIP_LAUNCH(MODE, ST, CS) \
-  return launch_impl<MODE, ST, CS>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+#define SIGLIP_LAUNCH(MODE, ST, CS)                                                               \
+  return (p.row_ids != nullptr)                                                                   \
+             ? launch_impl<MODE, ST, CS, false, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream) \
+             : launch_impl<MODE, ST, CS>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
 
 #define SIGLIP_LAUNCH_STAGES(MODE, CS)   \
   do {                                   \
     if (stages == 4) SIGLIP_LAUNCH(MODE, 4, CS); \
     SIGLIP_LAUNCH(MODE, 6, CS);          \
   } while (0)
+
+// the five tensor maps and the parameter block travel as kernel parameters: keep them inside the classic 4 KiB limit
+static_assert(5 * sizeof(CUtensorMap) + sizeof(KernelParams) <= 4096, "kernel parameters exceed 4 KiB");
 
 int launch_gemm(int cta_group, int mode, int stages, int mcast, const CUtensorMap* tmA0, const CUtensorMap* tmB0,
                 const CUtensorMap* tmA1, const CUtensorMap* tmB1, const CUtensorMap* tmG, const KernelParams& p,

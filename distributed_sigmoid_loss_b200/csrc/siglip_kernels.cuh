@@ -34,7 +34,7 @@ struct Problem {
   long long ld_add;
 };
 
-constexpr int kMaxAuxJobs = 6;
+constexpr int kMaxAuxJobs = 8;   // L0 of a multi-rank step with sample ids carries 7
 enum AuxKind { kAuxNone = 0, kAuxCopy = 1, kAuxCvt = 2, kAuxFold = 3, kAuxWaitOnly = 4 };
 
 // One job of the auxiliary warps. Optional pre-wait on `wait_n` consecutive local flags (all >= wait_value, written by
@@ -76,6 +76,10 @@ struct KernelParams {
   int own_chunk;   // 1: this text chunk holds the positives of this rank's images
   int store_g;     // 0: forward only
   float g_scale;   // sigma is stored as fp16(sigma * g_scale): 2^14 keeps sigma in (3.7e-9, 1) inside fp16's normal range
+  // sample-id labels (SIGLIP_OPT_SAMPLE_IDS): pair (i, j) is positive iff row_ids[i] == col_ids[j]. row_ids: this rank's
+  // images [M]; col_ids: the text chunk being scored [N]. Null = positional labels (the own-chunk diagonal only).
+  const int64_t* row_ids;
+  const int64_t* col_ids;
   double* partials;  // [gridDim.x][4] : sum softplus, sum g, sum g*s, (unused)
   int accumulate_partials;
   // loss kernel of the LAST chunk of a forward: the CTA that finishes last (ticket counter) adds the per-CTA slots in

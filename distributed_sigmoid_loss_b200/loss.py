@@ -102,6 +102,23 @@ class SigmoidLossEngine:
     def debug_set_text_chunk(self, chunk: int, txt: torch.Tensor) -> None:
         _capi.check(self._L.siglip_debug_set_text_chunk(self._h, chunk, txt.data_ptr(), self._stream()))
 
+    def set_sample_ids(self, ids: torch.Tensor) -> None:
+        """SIGLIP_OPT_SAMPLE_IDS: this rank's sample ids ([B] int64, contiguous, on the engine's device) for the NEXT
+        step. They are copied on the current stream, so `ids` may be released or overwritten afterwards."""
+        self._check_ids(ids, self.batch)
+        with torch.cuda.device(self.device):
+            _capi.check(self._L.siglip_set_sample_ids(self._h, ids.data_ptr(), self._stream()))
+
+    def debug_set_chunk_ids(self, chunk: int, ids: torch.Tensor) -> None:
+        """Loopback: the sample ids of text chunk `chunk` as its owner would have published them."""
+        self._check_ids(ids, self.batch_per_rank[chunk])
+        _capi.check(self._L.siglip_debug_set_chunk_ids(self._h, chunk, ids.data_ptr(), self._stream()))
+
+    def _check_ids(self, ids: torch.Tensor, n: int) -> None:
+        if ids.dtype != torch.int64 or tuple(ids.shape) != (n,) or not ids.is_contiguous() or ids.device != self.device:
+            raise RuntimeError(f"sample ids must be a contiguous int64 [{n}] tensor on {self.device}, got "
+                               f"{tuple(ids.shape)} {ids.dtype} on {ids.device}")
+
     def debug_get_slot(self, chunk: int) -> torch.Tensor:
         out = torch.empty(self.batch_per_rank[chunk], self.dim, device=self.device, dtype=torch.float32)
         _capi.check(self._L.siglip_debug_get_slot(self._h, chunk, out.data_ptr(), self._stream()))
@@ -363,10 +380,12 @@ class _SigmoidLossFn(torch.autograd.Function):
       * fused  (fused=True): forward = the fused step (loss and gradient kernels alternating chunk by chunk, two sigma
         operands, every cross-rank flag handled inside the kernels) which leaves the gradients for an upstream gradient
         of 1; backward = one multiply by grad_output per tensor (siglip_scale). O(B^2) workspace.
-    normalize=True additionally fuses F.normalize of both inputs (forward) and its backward around the loss."""
+    normalize=True additionally fuses F.normalize of both inputs (forward) and its backward around the loss.
+    ids: [B] int64 sample ids (SIGLIP_OPT_SAMPLE_IDS engines), set before every step the engine runs for this call."""
 
     @staticmethod
-    def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool = False, fused: bool = False):
+    def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool = False, fused: bool = False,
+                ids: Optional[torch.Tensor] = None):
         need_grad = any(ctx.needs_input_grad[:4])
         raw = None
         # bf16 callers: bf16 operands (what autograd would multiply). Anything wider (the reference's own test feeds
@@ -400,6 +419,9 @@ class _SigmoidLossFn(torch.autograd.Function):
             b = b.to(device=img.device, dtype=torch.float32)
         b = b.reshape(1)
         ctx.fused = bool(fused and need_grad)
+        ctx.ids = ids
+        if ids is not None:
+            engine.set_sample_ids(ids)
         if ctx.fused:
             # gradients in the dtype autograd would return for these inputs (fp32 when a projection follows)
             gdt = torch.bfloat16 if (not hi and not normalize) else torch.float32
@@ -446,7 +468,9 @@ class _SigmoidLossFn(torch.autograd.Function):
             img_b, txt_b, tp, b = saved[:4]
             if eng.saved_generation != ctx.gen:
                 # another forward of the same module ran in between: rebuild the saved state (every rank takes this
-                # branch together, so the collective stays matched)
+                # branch together, so the collective stays matched); the re-run takes this call's ids again
+                if ctx.ids is not None:
+                    eng.set_sample_ids(ctx.ids)
                 eng.forward(img_b, txt_b, tp, b, True)
                 ctx.gen = eng.saved_generation
             if ctx.normalize:
@@ -463,14 +487,15 @@ class _SigmoidLossFn(torch.autograd.Function):
                 gt = dtxt.to(tdt) if ctx.needs_input_grad[1] else None
         gp = dtp.reshape(pshape).to(device=pdev, dtype=pdt) if ctx.needs_input_grad[2] else None
         gb = db.reshape(bshape).to(device=bdev, dtype=bdt) if ctx.needs_input_grad[3] else None
-        return gi, gt, gp, gb, None, None, None
+        return gi, gt, gp, gb, None, None, None, None
 
 
 class _EngineCache:
     def __init__(self, group=None, cta_group: int = 2, overlap_pull: bool = True, sync_scalar_grads: bool = False,
-                 bidir: bool = False, batch_per_rank=None):
+                 bidir: bool = False, batch_per_rank=None, multi_positive: bool = False):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
         self.sync_scalar_grads, self.bidir = sync_scalar_grads, bidir
+        self.multi_positive = multi_positive
         self.batch_per_rank = batch_per_rank
         self._engines: Dict[Tuple[int, int, int], SigmoidLossEngine] = {}
 
@@ -485,8 +510,33 @@ class _EngineCache:
                 eng.set_option(_capi.SIGLIP_OPT_SYNC_SCALAR_GRADS, 1)
             if self.bidir:
                 eng.set_option(_capi.SIGLIP_OPT_BIDIR, 1)
+            if self.multi_positive:
+                eng.set_option(_capi.SIGLIP_OPT_SAMPLE_IDS, 1)
             self._engines[key] = eng
         return eng
+
+
+_ID_DTYPES = (torch.int8, torch.uint8, torch.int16, torch.int32, torch.int64)
+
+
+def _validate_ids(sample_ids, multi_positive: bool, embeddings: torch.Tensor) -> Optional[torch.Tensor]:
+    """sample_ids of a forward: required ([B] integers on the embeddings' device) with multi_positive, refused without.
+    Returns them as contiguous int64 (what the kernels compare), or None. Raises before any GPU work."""
+    if not multi_positive:
+        if sample_ids is not None:
+            raise RuntimeError("sample_ids given, but the loss was built without multi_positive=True")
+        return None
+    if sample_ids is None:
+        raise RuntimeError("multi_positive=True: forward needs sample_ids ([batch] integer tensor, one id per sample)")
+    if not isinstance(sample_ids, torch.Tensor) or sample_ids.dtype not in _ID_DTYPES:
+        raise RuntimeError(f"sample_ids must be an integer tensor, got "
+                           f"{sample_ids.dtype if isinstance(sample_ids, torch.Tensor) else type(sample_ids)}")
+    batch = embeddings.shape[0] if embeddings.dim() >= 1 else None
+    if sample_ids.dim() != 1 or sample_ids.shape[0] != batch:
+        raise RuntimeError(f"sample_ids must have shape [{batch}] (one id per sample), got {tuple(sample_ids.shape)}")
+    if sample_ids.device != embeddings.device:
+        raise RuntimeError(f"sample_ids are on {sample_ids.device}, the embeddings on {embeddings.device}")
+    return sample_ids.to(torch.int64).contiguous()
 
 
 def _validate(image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, expect_batch: Optional[int]) -> None:
@@ -526,11 +576,15 @@ class DDPSigmoidLoss(nn.Module):
     P2P access to each other (the exchange is CUDA-IPC peer memory, not NCCL), at most 32 ranks; give a multi-node job a
     per-node ``group``. A rank waiting for a peer inside a kernel gives up after ``SIGLIP_PEER_TIMEOUT_MS`` (default
     10 minutes).
+
+    ``multi_positive=True``: every ``forward`` takes ``sample_ids`` ([B] integers, one per sample on this rank), and a pair
+    is positive iff its image and text carry the same id — on any rank (repeated captions, several captions of one
+    image, a sample drawn twice). Unique ids give exactly the default labels. Collective: set on every rank.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
                  normalize_inputs: bool = False, sync_scalar_grads: bool = False, fused_step: Optional[bool] = None,
-                 batch_per_rank=None) -> None:
+                 batch_per_rank=None, multi_positive: bool = False) -> None:
         super().__init__()
         self.t_prime = nn.Parameter(torch.tensor(math.log(10), dtype=torch.float64))
         self.bias = nn.Parameter(torch.tensor(-10.0))
@@ -545,18 +599,23 @@ class DDPSigmoidLoss(nn.Module):
         # rank, the split forward / backward otherwise (one operand either way; saves the multiply by grad_output)
         self.fused_step = fused_step
         # extension (SURVEY.md §8f-4): per-rank batch sizes may differ; every rank passes the same list
-        self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank)
+        # extension: labels from per-sample ids (positive iff same id, across ranks too)
+        self.multi_positive = multi_positive
+        self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank,
+                                   multi_positive=multi_positive)
 
     def engine_for(self, batch: int, dim: int, device: torch.device) -> SigmoidLossEngine:
         return self._cache.get(batch, (dim + 7) // 8 * 8, device)
 
-    def forward(self, image_embeddings: torch.Tensor, text_embeddings: torch.Tensor) -> torch.Tensor:
+    def forward(self, image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, *,
+                sample_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
+        ids = _validate_ids(sample_ids, self.multi_positive, image_embeddings)
         _validate(image_embeddings, text_embeddings, self.gpu_batch_size)
         image_embeddings, text_embeddings = _pad_dim(image_embeddings), _pad_dim(text_embeddings)
         eng = self._cache.get(image_embeddings.shape[0], image_embeddings.shape[1], image_embeddings.device)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
         return _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
-                                    self.normalize_inputs, fused)
+                                    self.normalize_inputs, fused, ids)
 
 
 SigmoidLoss = DDPSigmoidLoss
@@ -566,18 +625,23 @@ class SigLipLoss(nn.Module):
     """open_clip-signature adapter (rwightman_sigmoid_loss.py:12-124): scale and bias are passed in, the ring
     exchange of the original is replaced by the direct NVSwitch pulls of the fused path. ``bidir`` selects the
     visiting order of the original's bidirectional exchange (rank+1, rank-1, rank+2, ...) instead of rank+1, rank+2,
-    ...; the pairs covered and the result are the same."""
+    ...; the pairs covered and the result are the same. ``multi_positive=True``: labels from the ``sample_ids`` every
+    forward then takes, as in ``DDPSigmoidLoss``."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
-                 use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None):
+                 use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
+                 multi_positive: bool = False):
         super().__init__()
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
         self.cache_labels, self.rank, self.world_size, self.bidir = cache_labels, rank, world_size, bidir
         self.use_horovod = use_horovod
         self.fused_step = fused_step
-        self._cache = _EngineCache(group, cta_group, bidir=bidir)
+        self.multi_positive = multi_positive
+        self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive)
 
-    def forward(self, image_features, text_features, logit_scale, logit_bias, output_dict: bool = False):
+    def forward(self, image_features, text_features, logit_scale, logit_bias, output_dict: bool = False, *,
+                sample_ids: Optional[torch.Tensor] = None):
+        ids = _validate_ids(sample_ids, self.multi_positive, image_features)
         _validate(image_features, text_features, None)
         image_features, text_features = _pad_dim(image_features), _pad_dim(text_features)
         eng = self._cache.get(image_features.shape[0], image_features.shape[1], image_features.device)
@@ -588,5 +652,5 @@ class SigLipLoss(nn.Module):
         if logit_bias is None:
             logit_bias = torch.zeros((), device=image_features.device)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
-        loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused)
+        loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids)
         return {"contrastive_loss": loss} if output_dict else loss

@@ -92,6 +92,14 @@ enum {
                                  is an fp64 device scalar — the dtype of the reference's parameter
                                  (torch.tensor(np.log(10)), distributed_sigmoid_loss.py:11) — and dt_prime is written as
                                  fp64: the module hands its parameter over without a conversion kernel. Default 0 (fp32) */
+  SIGLIP_OPT_SAMPLE_IDS = 21, /* 1: labels from per-sample ids instead of positions. Image i of rank r and text j of rank c
+                                 are a positive pair iff ids_r[i] == ids_c[j] (repeated captions, several captions per
+                                 image, a sample drawn on two ranks); loss and gradients keep their formulas with these
+                                 labels. Every step takes this rank's ids from siglip_set_sample_ids; the ids travel to the
+                                 other ranks with the text. Unique ids give exactly the default labels (and bit-identical
+                                 results). Off-diagonal positives enter the gradient contractions through the fp16 sigma
+                                 operand (2^-12 relative rounding each, like the negatives). The host-buffer entries are
+                                 unavailable in this mode. Collective: set on all ranks. Default 0 */
   SIGLIP_OPT_AUX_TRACE = 18 /* 1: record globaltimer stamps of the auxiliary warps of CTA 0 for every launch (start,
                                last peer flag seen, jobs done, end of launch); read with siglip_ctx_aux_trace */
 };
@@ -202,6 +210,16 @@ int siglip_backward(siglip_ctx* ctx, const void* img, const void* txt, const flo
                     void* dimg, void* dtxt, float* dt_prime, float* dbias, void* cuda_stream);
 unsigned long long siglip_ctx_saved_generation(const siglip_ctx* ctx);
 
+/*
+ * SIGLIP_OPT_SAMPLE_IDS: the ids of this rank's B samples (image i and text i share ids_dev[i]; int64 device buffer,
+ * any values) for the NEXT siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd call. They are copied on the stream
+ * into the context, so the caller's buffer may be reused once the copy has run; nothing is read on the host (a
+ * single-rank step with ids can be captured into a CUDA graph, the copy with it). In ids mode a step without ids set
+ * since the previous step returns SIGLIP_ERR_STATE before launching anything; outside it this call returns
+ * SIGLIP_ERR_STATE. siglip_backward needs no ids (the saved sigma operand holds the labels).
+ */
+int siglip_set_sample_ids(siglip_ctx* ctx, const int64_t* ids_dev, void* cuda_stream);
+
 /* Forward only (torch.no_grad / evaluation): siglip_forward with save_for_backward = 0. */
 int siglip_fwd(siglip_ctx* ctx, const void* img, const void* txt, const float* t_prime, const float* bias,
                float* loss, void* cuda_stream);
@@ -218,6 +236,7 @@ int siglip_fwd(siglip_ctx* ctx, const void* img, const void* txt, const float* t
  * results are on the host. At most two steps may be in flight: submit blocks on the step that used the same staging
  * set. The copies of step n+1 overlap the kernels of step n; every step still pays its own copies.
  * This is the end-to-end entry the benchmark times. Host buffers must stay valid until the step's wait returns.
+ * These entries take no sample ids: under SIGLIP_OPT_SAMPLE_IDS they return SIGLIP_ERR_STATE.
  */
 int siglip_host_submit(siglip_ctx* ctx, const void* img_host, const void* txt_host, float t_prime, float bias,
                        unsigned long long* ticket, void* cuda_stream);
@@ -267,6 +286,9 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
 int siglip_debug_loopback(siglip_ctx* ctx);
 int siglip_debug_set_text_chunk(siglip_ctx* ctx, int chunk, const void* txt_dev, void* cuda_stream);
 int siglip_debug_get_slot(siglip_ctx* ctx, int chunk, float* out_dev, void* cuda_stream);
+/* The ids twin of siglip_debug_set_text_chunk (SIGLIP_OPT_SAMPLE_IDS): the sample ids of text chunk `chunk`
+ * ([batch of that rank] int64 device buffer) as the "peer" would have published them. */
+int siglip_debug_set_chunk_ids(siglip_ctx* ctx, int chunk, const int64_t* ids_dev, void* cuda_stream);
 /* Loopback only: seed the (dt_prime, dbias) mailbox standing in for peer rank `peer`, so that the mean computed under
  * SIGLIP_OPT_SYNC_SCALAR_GRADS can be checked against numbers the kernel did not produce itself. */
 int siglip_debug_set_mailbox(siglip_ctx* ctx, int peer, float dt_prime, float dbias);

@@ -38,6 +38,8 @@ def main() -> int:
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--all-variants", action="store_true", help="also time the non-overlapped variants")
     ap.add_argument("--skip-parity", action="store_true")
+    ap.add_argument("--sample-ids", action="store_true",
+                    help="also check multi-positive labels from sample ids (duplicates across ranks) against the oracle")
     ap.add_argument("--soak", type=int, default=0,
                     help="N > 0: that many back-to-back steps at the --batch/--dim shape mixing the fused step, the split "
                          "API and forward-only calls; same inputs, so every step of a kind must reproduce its first result "
@@ -190,6 +192,42 @@ def main() -> int:
                 dtxt=rel_f(dtxt_u.cpu(), dtxt_ref), dtp=abs(float(dtp_u) - dtp_ref) / abs(dtp_ref),
                 db=abs(float(db_u) - db_ref) / abs(db_ref)))
         engu.close()
+
+    # ---- multi-positive labels from sample ids: 40 classes over the global batch, so most ranks share ids with every
+    # other rank (cross-chunk positives); the ids travel with the text through the peer exchange -----------------------
+    if args.sample_ids:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the ids oracle lives with the tests
+        from sample_ids_oracle import closed_form_ids
+        for (B, D, tp, bias) in [(96, 64, math.log(10.0), -10.0), (200, 136, math.log(10.0), -8.0)]:
+            g = torch.Generator().manual_seed(77)
+            img_all = torch.nn.functional.normalize(torch.randn(world * B, D, generator=g)).to(torch.bfloat16)
+            txt_all = torch.nn.functional.normalize(torch.randn(world * B, D, generator=g)).to(torch.bfloat16)
+            ids_all = torch.randint(-(2 ** 40), -(2 ** 40) + 40, (world * B,), generator=g)
+            blk = lambda x, r: x[r * B:(r + 1) * B]  # noqa: E731
+            ref = closed_form_ids([blk(img_all, r).float().numpy() for r in range(world)],
+                                  [blk(txt_all, r).float().numpy() for r in range(world)],
+                                  [blk(ids_all, r).numpy() for r in range(world)], tp, bias)
+            mine = ref[rank]
+            dtxt_ref = torch.from_numpy(sum(ref[r]["contrib"][rank] for r in range(world)))
+            img, txt = blk(img_all, rank).to(dev).contiguous(), blk(txt_all, rank).to(dev).contiguous()
+            ids = blk(ids_all, rank).to(dev).contiguous()
+            for fused in (None, False):
+                modx = DDPSigmoidLoss(B, fused_step=fused, multi_positive=True).to(dev)
+                with torch.no_grad():
+                    modx.t_prime.fill_(tp)
+                    modx.bias.fill_(bias)
+                for rep in range(2):
+                    a, b = img.float().requires_grad_(True), txt.float().requires_grad_(True)
+                    l2 = modx(a, b, sample_ids=ids)
+                    l2.backward()
+                    torch.cuda.synchronize()
+                    report(f"sample ids fused_step={fused} B={B} D={D} rep{rep}", dict(
+                        loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
+                        dimg=rel_f(a.grad.cpu(), torch.from_numpy(mine["dimg"])),
+                        dtxt=rel_f(b.grad.cpu(), dtxt_ref),
+                        dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
+                        db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
+                del modx
 
     # ---- larger: fp32 autograd; dtxt reference summed over ranks ------------------------------------------
     B, D, tp, bias = 2048, 768, math.log(10.0), -10.0
