@@ -34,6 +34,7 @@ EXPORTED_SYMBOLS = (
     "siglip_fwd_bwd_scaled",
     "siglip_fwd",
     "siglip_set_sample_ids",
+    "siglip_request_metrics",
     "siglip_fwd_bwd_host",
     "siglip_convert_f32",
     "siglip_host_submit",
@@ -51,6 +52,7 @@ EXPORTED_SYMBOLS = (
     "siglip_debug_get_slot",
     "siglip_debug_set_chunk_ids",
     "siglip_debug_set_mailbox",
+    "siglip_debug_set_peer_metric_keys",
     "siglip_ctx_aux_trace",
     "siglip_ctx_destroy",
 )
@@ -179,6 +181,10 @@ def lib() -> ctypes.CDLL:
     L.siglip_set_sample_ids.restype = ci
     L.siglip_debug_set_chunk_ids.argtypes = [vp, ci, vp, vp]
     L.siglip_debug_set_chunk_ids.restype = ci
+    L.siglip_request_metrics.argtypes = [vp, vp, vp, vp]
+    L.siglip_request_metrics.restype = ci
+    L.siglip_debug_set_peer_metric_keys.argtypes = [vp, ci, vp, vp]
+    L.siglip_debug_set_peer_metric_keys.restype = ci
     L.siglip_ctx_launch_count.argtypes = [vp]
     L.siglip_ctx_launch_count.restype = ctypes.c_ulonglong
     L.siglip_debug_gemm.argtypes = [ci, ci, ci, ci, ci, vp, ctypes.c_longlong, ci, vp, ctypes.c_longlong, ci, vp,

@@ -130,7 +130,8 @@ constexpr int kMaxWorld = 32;
 //   0 text of forward #n is in place        1 dtxt contribution of backward #n, gradient slot j is complete
 //   2 forward #n finished pulling everyone's text     3 backward #n finished reading everyone's contributions
 //   4 (dt', dbias) of backward #n are in the owner's mailbox (SIGLIP_OPT_SYNC_SCALAR_GRADS)
-constexpr int kFlagKinds = 5;
+//   5 the retrieval-metric partials of forward #n are in place (siglip_request_metrics)
+constexpr int kFlagKinds = 6;
 // the mailbox (2 floats) lives behind the flag counters, in the same peer-mapped allocation
 constexpr int kMailboxOffset = kFlagKinds * kMaxWorld;
 constexpr size_t kFlagBytes = (kMailboxOffset + 4) * sizeof(unsigned int);
@@ -180,6 +181,13 @@ struct siglip_ctx {
   int aux_trace_on = 0;
   int sample_ids = 0;                    // SIGLIP_OPT_SAMPLE_IDS: labels from per-sample ids (collective)
   bool ids_set = false;                  // siglip_set_sample_ids was called since the previous step
+  int off[kMaxWorld + 1] = {};           // global index of every rank's first sample (prefix sums of Bs)
+  // retrieval metrics (siglip_request_metrics), armed for the next step only
+  bool metrics_armed = false;
+  float* m_top1 = nullptr;
+  int64_t* m_i2t = nullptr;
+  int64_t* m_t2i = nullptr;
+  unsigned long long* mkeys_step = nullptr;  // key block of the step being issued (null: no metrics this step)
   // diagnostics, read from the environment once at context creation (see include/siglip_b200.h)
   bool dbg_no_gstore = false, dbg_no_cvt = false, dbg_loss_waitstats = false;
   // workspaces
@@ -188,6 +196,8 @@ struct siglip_ctx {
   int64_t* ids_all = nullptr;            // [world][ids_stride] sample ids of every text chunk (world > 1)
   int64_t* ids_in = nullptr;             // [ids_stride] this rank's ids for the next step (siglip_set_sample_ids)
   int ids_stride = 0;                    // Bmax rounded up to even: every slot is a whole number of 16-byte vectors
+  unsigned long long* mkeys[2] = {};     // per step parity: [world][Bmax] column argmax partials of every text chunk
+                                         // over my images, then [Bmax] row keys. world > 1: behind ids_all (exported)
   __nv_bfloat16* G[kMaxWorld] = {};      // [Bp, Bp] sigma operands (fp16 bits x kGScale), diagonal zeroed, allocated on
                                          // first use: fused step 2 (own chunk + the chunk in flight), split API one per chunk
   __nv_bfloat16* img16 = nullptr;        // [B, D] fp16 (x kXScale) images: B operand of the dtxt contraction
@@ -202,6 +212,7 @@ struct siglip_ctx {
   unsigned int* sync_words = nullptr;    // [kSyncWords] local tickets / flags
   float* loop_mailboxes = nullptr;       // loopback only: [world][2] stand-ins for the peers' (dt', dbias) mailboxes
   float* loop_zero = nullptr;            // loopback only: [world][Bmax, D] zeros standing in for the peers' contribution slots
+  unsigned long long* loop_keys = nullptr;  // loopback only: [world][Bmax] the peers' column partials of my chunk
   float* scalars = nullptr;              // [24] device scalars: host API staging, saved dt'/dbias of the last forward
   unsigned long long* aux_trace = nullptr;  // [kTraceLaunches][16] globaltimer stamps (SIGLIP_OPT_AUX_TRACE)
   float* splitk_ws = nullptr;            // fp32 partial accumulators of the split tiles of the gradient kernel
@@ -218,6 +229,7 @@ struct siglip_ctx {
   const float** final_ptrs_dev = nullptr;    // [2] {dtxt_acc, own slot}: the local last add of the split API
   unsigned int** signal_ptrs_dev = nullptr;  // [kFlagKinds][world]
   const float** mailbox_ptrs_dev = nullptr;  // [world] every rank's (dt', dbias) mailbox
+  const unsigned long long** mkey_ptrs_dev = nullptr;  // [2][world] every rank's column partial of my chunk, per parity
   unsigned int n_fwd = 0, n_bwd = 0;         // forward / backward passes issued (flag counters)
   unsigned int prewait3 = 0;                 // highest n for which "peers finished backward n" has been waited for
   unsigned long long gen = 0;                // generation of the state saved for backward (0 = none)
@@ -249,7 +261,7 @@ int check_dbg(siglip_ctx* c, const char* where) {
   if (c->dbg_host != nullptr && c->dbg_host->code != 0) {
     char buf[320];
     const unsigned int code = c->dbg_host->code;
-    const bool peer = (code >= 5);   // 5 text pull, 6 helper wait, 7 fold, 8 last-fold flag, 9 scalar exchange, 1x aux jobs
+    const bool peer = (code >= 5);   // 5 text pull, 6 helper wait, 7 fold, 8 last-fold flag, 9 scalar exchange, 10 metric partials, 1x aux jobs
     snprintf(buf, sizeof(buf),
              "%s: device wait timed out at site %u (block %u thread %u aux %u %u %u)%s", where, code,
              c->dbg_host->block, c->dbg_host->thread, c->dbg_host->aux0, c->dbg_host->aux1, c->dbg_host->aux2,
@@ -295,6 +307,62 @@ int take_ids(siglip_ctx* c) {
 }
 inline unsigned long long peer_timeout_ns(const siglip_ctx* c) {
   return static_cast<unsigned long long>(c->peer_timeout_ms) * 1000000ull;
+}
+
+// ---- retrieval metrics (siglip_request_metrics) ----
+static_assert(siglip::kMetricsMaxWorld == kMaxWorld, "the finalisation kernel takes one batch offset per rank");
+// 64-bit keys per step parity: [world][Bmax] column partials, then [Bmax] row keys
+inline size_t mkeys_block(const siglip_ctx* c) { return static_cast<size_t>(c->world + 1) * c->Bmax; }
+// byte offset of the two key blocks in the exported text allocation: behind the gathered text and ids
+inline size_t mkeys_offset(const siglip_ctx* c) {
+  return chunk_stride(c) * c->world * sizeof(__nv_bfloat16) + static_cast<size_t>(c->world) * c->ids_stride * sizeof(int64_t);
+}
+// A metrics step starts (armed by siglip_request_metrics for this step only): the key block of the step's parity is
+// zeroed, so that no max of an earlier step survives. Double-buffered by parity: a peer may still read my partials of
+// step n in its finalisation while my step n + 1 writes; by step n + 2 that read is over (DESIGN.md, "In-batch
+// retrieval metrics").
+int take_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
+  c->mkeys_step = nullptr;
+  if (!c->metrics_armed) return 0;
+  c->metrics_armed = false;
+  c->mkeys_step = c->mkeys[s & 1u];
+  CK(cudaMemsetAsync(c->mkeys_step, 0, mkeys_block(c) * sizeof(unsigned long long), st));
+  c->launches++;
+  return 0;
+}
+// After the step's last loss kernel: combine the keys (W > 1: with every rank's partials of my chunk, flag kind 5) and
+// write the indices and the top-1 rates.
+int finalize_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
+  if (c->mkeys_step == nullptr) return 0;
+  const int W = c->world;
+  siglip::MetricsArgs a;
+  memset(&a, 0, sizeof(a));
+  a.row_keys = c->mkeys_step + static_cast<size_t>(W) * c->Bmax;
+  a.col_own = c->mkeys_step + static_cast<size_t>(c->rank) * c->Bmax;
+  a.B = c->B;
+  a.rank = c->rank;
+  a.world = W;
+  for (int p = 0; p <= W; ++p) a.off[p] = c->off[p];
+  if (c->sample_ids) {
+    a.ids_own = c->ids_in;
+    a.ids_all = c->ids_all;
+    a.ids_stride = c->ids_stride;
+  }
+  a.top1 = c->m_top1;
+  a.i2t = c->m_i2t;
+  a.t2i = c->m_t2i;
+  if (W > 1) {
+    a.col_peers = c->mkey_ptrs_dev + static_cast<size_t>(s & 1u) * W;
+    a.sig_ptrs = c->signal_ptrs_dev + 5 * W;
+    a.flags_local = c->flags + 5 * kMaxWorld;
+    a.value = s;
+    a.timeout_ns = peer_timeout_ns(c);
+  }
+  a.dbg = c->dbg_dev;
+  c->mkeys_step = nullptr;
+  CKI(siglip::launch_metrics_finalize(a, st));
+  c->launches++;
+  return 0;
 }
 
 // Sigma operand + fp16 text copy number i, allocated on first use. The fused step needs two (own chunk, chunk in
@@ -383,9 +451,9 @@ struct FinJob {   // last chunk of a forward: the loss kernel's last CTA writes 
 // The loss kernel over one text chunk (Bn rows, owner's batch): S = img @ txt_c^T on wgmma, fused
 // scale/bias/log-sigmoid/reduce. save: also write the sigma operand G[gi] (+ g_diag on the own chunk); the fp16 copies
 // the gradient kernel needs are auxiliary jobs built by the caller.
-// col_ids: sample ids of the chunk (null = positional labels).
-int run_loss_chunk(siglip_ctx* c, int gi, bool own, bool first, const void* img, const __nv_bfloat16* txt_c, int Bn,
-                   const int64_t* col_ids, const float* t_prime, const float* bias, bool save, const AuxList& aux,
+// cidx: owner rank of the chunk; col_ids: sample ids of the chunk (null = positional labels).
+int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const void* img, const __nv_bfloat16* txt_c,
+                   int Bn, const int64_t* col_ids, const float* t_prime, const float* bias, bool save, const AuxList& aux,
                    const FinJob* fin, const EndSignal& end, cudaStream_t st) {
   const int cg = c->cta_group;
   int rc;
@@ -421,6 +489,12 @@ int run_loss_chunk(siglip_ctx* c, int gi, bool own, bool first, const void* img,
   if (col_ids != nullptr) {
     p.row_ids = c->ids_in;
     p.col_ids = col_ids;
+  }
+  if (c->mkeys_step != nullptr) {   // a metrics step: the kMetrics instantiation reduces the argmax keys
+    p.row_keys = c->mkeys_step + static_cast<size_t>(c->world) * c->Bmax;
+    p.col_keys = c->mkeys_step + static_cast<size_t>(cidx) * c->Bmax;
+    p.row_off = c->off[c->rank];
+    p.col_off = c->off[cidx];
   }
   p.partials = c->partials;
   p.accumulate_partials = first ? 0 : 1;  // the first chunk of a forward overwrites every slot of the grid
@@ -680,6 +754,7 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
   const int W = c->world, r = c->rank;
   const size_t stride = chunk_stride(c);
   const unsigned int s = ++c->n_fwd;
+  if ((rc = take_metrics(c, s, st))) return rc;
   // the saved state is being overwritten (a forward without save still replaces my gathered text slot, which the
   // backward of a multi-rank job reads for the positive-pair term); valid again once a saving forward is enqueued
   if (save || c->world > 1) c->gen = 0;
@@ -719,13 +794,14 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
                              ids_bytes(c, nxt), cudaMemcpyDefault, st));
       }
     }
-    if ((rc = run_loss_chunk(c, k, k == 0, k == 0, img, txt_c, c->Bs[cidx], chunk_ids(c, cidx), t_prime, bias, save,
+    if ((rc = run_loss_chunk(c, k, cidx, k == 0, k == 0, img, txt_c, c->Bs[cidx], chunk_ids(c, cidx), t_prime, bias, save,
                              aux, (k == W - 1) ? &fin : nullptr, EndSignal(), st)))
       return rc;
   }
   if (W > 1) {
     if ((rc = signal_peers(c, 2, s, st))) return rc;
   }
+  if ((rc = finalize_metrics(c, s, st))) return rc;
   CK(cudaGetLastError());
   if (save) {
     c->saved_f16 = c->input_f16;
@@ -851,6 +927,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   const unsigned int n = ++c->n_bwd;
   const unsigned int base = (n - 1) * static_cast<unsigned int>(W);
   const bool ik = c->inkernel_sync != 0;
+  if ((rc = take_metrics(c, s, st))) return rc;
   c->gen = 0;                       // the sigma operands of a split forward (if any) are overwritten
   c->saved_f16 = c->input_f16;
   if ((rc = ensure_g(c, 0))) return rc;
@@ -906,7 +983,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       c->prewait3 = n - 1;
       add_pull_job(c, aux, step_owner(c, r, 1), s);
     }
-    if ((rc = run_loss_chunk(c, 0, true, true, img, own_txt, c->B, chunk_ids(c, r), t_prime, bias, true, aux,
+    if ((rc = run_loss_chunk(c, 0, r, true, true, img, own_txt, c->B, chunk_ids(c, r), t_prime, bias, true, aux,
                              (W == 1) ? &fin : nullptr, EndSignal(), st)))
       return rc;
   }
@@ -921,7 +998,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       if (k + 1 < W) add_pull_job(c, aux, step_owner(c, r, k + 1), s);
       const bool lastL = (k == W - 1);
       EndSignal end = (lastL && ik) ? end_signal(c, 2, s) : EndSignal();   // "I have pulled everyone's text"
-      if ((rc = run_loss_chunk(c, 1, false, false, img, txt_c, c->Bs[cidx], chunk_ids(c, cidx), t_prime, bias, true,
+      if ((rc = run_loss_chunk(c, 1, cidx, false, false, img, txt_c, c->Bs[cidx], chunk_ids(c, cidx), t_prime, bias, true,
                                aux, lastL ? &fin : nullptr, end, st)))
         return rc;
       if (lastL && !ik && (rc = signal_peers(c, 2, s, st))) return rc;
@@ -981,6 +1058,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
     if ((rc = run_grad_chunk(c, 0, true, img, own_txt, c->B, t_prime, grad_out, o, aux, end, st))) return rc;
     if (W > 1 && !ik && (rc = signal_peers(c, 3, n, st))) return rc;
   }
+  if ((rc = finalize_metrics(c, s, st))) return rc;
   if (W > 1 && c->sync_scalar_grads) {
     CKI(siglip::launch_allreduce_scalars(c->scalars + kSavedScalars, grad_out,
                                          reinterpret_cast<float*>(c->flags + kMailboxOffset), c->mailbox_ptrs_dev,
@@ -1053,6 +1131,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   c->Bmax = Bmax;
   c->D = D;
   c->Bp = round_up(Bmax, 256);
+  for (int p = 0; p < world; ++p) c->off[p + 1] = c->off[p] + Bs[p];
   c->dbg_no_gstore = getenv("SIGLIP_DEBUG_NO_GSTORE") != nullptr;
   c->dbg_no_cvt = getenv("SIGLIP_DEBUG_NO_CVT") != nullptr;
   c->dbg_loss_waitstats = getenv("SIGLIP_DEBUG_LOSS_WAITSTATS") != nullptr;
@@ -1084,10 +1163,15 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   c->ids_stride = round_up(Bmax, 2);
   const size_t ids_slot_bytes = static_cast<size_t>(c->ids_stride) * sizeof(int64_t);
   CK(alloc(reinterpret_cast<void**>(&c->ids_in), ids_slot_bytes));
+  const size_t mkeys_bytes = 2 * mkeys_block(c) * sizeof(unsigned long long);
   if (world > 1) {
-    // the gathered ids live behind the gathered text, so that one exported handle covers both
-    CK(alloc(reinterpret_cast<void**>(&c->txt_all), stride * world * sizeof(__nv_bfloat16) + world * ids_slot_bytes));
+    // the gathered ids and the two metric key blocks live behind the gathered text, so that one exported handle covers
+    // all three
+    CK(alloc(reinterpret_cast<void**>(&c->txt_all),
+             stride * world * sizeof(__nv_bfloat16) + world * ids_slot_bytes + mkeys_bytes));
     c->ids_all = reinterpret_cast<int64_t*>(c->txt_all + stride * world);   // 16-byte aligned: D % 8 == 0
+    c->mkeys[0] = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(c->txt_all) + mkeys_offset(c));
+    c->mkeys[1] = c->mkeys[0] + mkeys_block(c);
     CK(alloc(reinterpret_cast<void**>(&c->slots), stride * world * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dimg_acc), static_cast<size_t>(c->B) * D * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dtxt_acc), static_cast<size_t>(c->B) * D * sizeof(float)));
@@ -1095,6 +1179,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     CK(alloc(reinterpret_cast<void**>(&c->final_ptrs_dev), 2 * sizeof(float*)));
     CK(alloc(reinterpret_cast<void**>(&c->signal_ptrs_dev), kFlagKinds * world * sizeof(unsigned int*)));
     CK(alloc(reinterpret_cast<void**>(&c->mailbox_ptrs_dev), world * sizeof(float*)));
+    CK(alloc(reinterpret_cast<void**>(&c->mkey_ptrs_dev), 2 * world * sizeof(unsigned long long*)));
     const float* fin[2] = {c->dtxt_acc, c->slots + rank * stride};
     CK(cudaMemcpy(c->final_ptrs_dev, fin, sizeof(fin), cudaMemcpyHostToDevice));
   }
@@ -1252,6 +1337,18 @@ static int publish_peer_tables(siglip_ctx* c) {
     if (c->loopback && p != c->rank) mb[p] = c->loop_mailboxes + 2 * p;
   }
   CK(cudaMemcpy(c->mailbox_ptrs_dev, mb.data(), c->world * sizeof(float*), cudaMemcpyHostToDevice));
+  // every rank's column partial of my chunk, per step parity (loopback: the stand-ins siglip_debug_set_peer_metric_keys
+  // seeds)
+  std::vector<const unsigned long long*> mk(2 * c->world);
+  for (int q = 0; q < 2; ++q)
+    for (int p = 0; p < c->world; ++p) {
+      const unsigned long long* blk =
+          reinterpret_cast<const unsigned long long*>(reinterpret_cast<const char*>(c->peer_txt[p]) + mkeys_offset(c)) +
+          q * mkeys_block(c);
+      mk[q * c->world + p] = blk + static_cast<size_t>(c->rank) * c->Bmax;
+      if (c->loopback && p != c->rank) mk[q * c->world + p] = c->loop_keys + static_cast<size_t>(p) * c->Bmax;
+    }
+  CK(cudaMemcpy(c->mkey_ptrs_dev, mk.data(), mk.size() * sizeof(unsigned long long*), cudaMemcpyHostToDevice));
   c->peers_ready = true;
   return 0;
 }
@@ -1309,6 +1406,44 @@ int siglip_set_sample_ids(siglip_ctx* c, const int64_t* ids_dev, void* cuda_stre
   CK(cudaMemcpyAsync(c->ids_in, ids_dev, ids_bytes(c, c->rank), cudaMemcpyDeviceToDevice,
                      static_cast<cudaStream_t>(cuda_stream)));
   c->ids_set = true;
+  return 0;
+}
+
+int siglip_request_metrics(siglip_ctx* c, float* top1, int64_t* i2t_index, int64_t* t2i_index) {
+  if (c == nullptr || top1 == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument (top1 is required)");
+  if (c->mkeys[0] == nullptr) {
+    // one rank: the key blocks are allocated on the first request, so a context that never asks for metrics holds
+    // exactly the workspace it held without them. (world > 1: they are part of the exported text allocation.) The
+    // allocation is not a stream operation; the relaxed capture mode lets a first request inside a CUDA-graph capture
+    // make it, as PyTorch's caching allocator does.
+    const size_t bytes = 2 * mkeys_block(c) * sizeof(unsigned long long);
+    CK(cudaSetDevice(c->device));
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    CK(cudaThreadExchangeStreamCaptureMode(&mode));
+    unsigned long long* keys = nullptr;
+    const cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&keys), bytes);
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    CK(e);
+    c->mkeys[0] = keys;
+    c->mkeys[1] = keys + mkeys_block(c);
+    c->workspace_bytes += bytes;
+  }
+  c->m_top1 = top1;
+  c->m_i2t = i2t_index;
+  c->m_t2i = t2i_index;
+  c->metrics_armed = true;
+  return 0;
+}
+
+int siglip_debug_set_peer_metric_keys(siglip_ctx* c, int peer, const uint64_t* keys_dev, void* cuda_stream) {
+  if (c == nullptr || keys_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->loopback || peer < 0 || peer >= c->world || peer == c->rank)
+    return fail(SIGLIP_ERR_INVALID,
+                "siglip_debug_set_peer_metric_keys needs a loopback context and a peer rank != own rank");
+  CK(cudaSetDevice(c->device));
+  CK(cudaMemcpyAsync(c->loop_keys + static_cast<size_t>(peer) * c->Bmax, keys_dev,
+                     static_cast<size_t>(c->B) * sizeof(unsigned long long), cudaMemcpyDeviceToDevice,
+                     static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
 
@@ -1390,6 +1525,8 @@ int siglip_host_submit_grads(siglip_ctx* c, const void* img_host, const void* tx
     return fail(SIGLIP_ERR_INVALID, "give both gradient host buffers or neither");
   if (c->sample_ids)
     return fail(SIGLIP_ERR_STATE, "the host-buffer entries take no sample ids: unavailable under SIGLIP_OPT_SAMPLE_IDS");
+  if (c->metrics_armed)
+    return fail(SIGLIP_ERR_STATE, "the host-buffer entries return no retrieval metrics: siglip_request_metrics is armed");
   const bool with_grads = dimg_host_bf16 != nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   CK(cudaSetDevice(c->device));
@@ -1530,6 +1667,8 @@ int siglip_debug_loopback(siglip_ctx* c) {
     CK(cudaMemset(c->loop_zero, 0, stride * c->world * sizeof(float)));
     CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_mailboxes), 2 * kMaxWorld * sizeof(float)));
     CK(cudaMemset(c->loop_mailboxes, 0, 2 * kMaxWorld * sizeof(float)));
+    CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_keys), static_cast<size_t>(c->world) * c->Bmax * 8));
+    CK(cudaMemset(c->loop_keys, 0, static_cast<size_t>(c->world) * c->Bmax * 8));
   }
   for (int p = 0; p < c->world; ++p) {
     c->peer_txt[p] = c->txt_all;
@@ -1796,6 +1935,9 @@ void free_ctx(siglip_ctx* c) {
   cudaFree(c->sync_words);
   cudaFree(c->loop_mailboxes);
   cudaFree(c->loop_zero);
+  cudaFree(c->loop_keys);
+  if (c->world == 1) cudaFree(c->mkeys[0]);   // world > 1: part of txt_all
+  cudaFree(c->mkey_ptrs_dev);
   cudaFree(c->scalars);
   cudaFree(c->aux_trace);
   cudaFree(c->splitk_ws);

@@ -352,6 +352,84 @@ __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int 
   if (store_g) store_g_slab(gst, col0, packed);
 }
 
+// -------------------------------------------------------------------------------------------------
+// In-batch retrieval metrics (kMetrics): the argmax of every row and column of the logits, from the accumulator tile.
+// Key of a candidate: (order-preserving bits of s) << 32 | (0xFFFFFFFF - global index). The unsigned max of two keys is
+// the larger s, ties to the lower index; 0 is "no candidate" (every real key is larger). z = t s + b is monotone in s
+// (t > 0), so the ranking of z is the ranking of s. The accumulator is s itself, or s * 2^8 for the fp16 x 16
+// operands: a power-of-two scale changes neither the order nor the ties.
+// -------------------------------------------------------------------------------------------------
+__device__ __forceinline__ unsigned long long metric_key(float s, int gidx) {
+  const uint32_t u = __float_as_uint(__fadd_rn(s, 0.0f));     // -0 -> +0: equal values must tie on the index
+  const uint32_t ord = u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
+  return (static_cast<unsigned long long>(ord) << 32) | (0xFFFFFFFFu - static_cast<uint32_t>(gidx));
+}
+
+__device__ __forceinline__ unsigned long long max_u64(unsigned long long a, unsigned long long b) { return a > b ? a : b; }
+
+__device__ __forceinline__ void red_max_u64(unsigned long long* p, unsigned long long v) {
+  asm volatile("red.relaxed.gpu.global.max.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+
+// Row side: per fragment row, the best of the thread's 32 columns (strict > in increasing column order keeps the lowest
+// index), then the quad that holds the row (shfl_xor 1, 2), then one red.max per row and tile.
+// Column side, per 32-column slab: the better of the thread's 2 rows for each of its 8 columns, then a reduce-scatter over
+// the warp's 8 row groups (lanes xor 16, 8, 4) that leaves lane l with column q = l >> 2 of the 8 its lane % 4 group
+// holds, then one red.max per lane and slab. Rows >= M and columns >= N are never candidates.
+__device__ __forceinline__ void tile_metrics(const float (&acc)[64], int row_lo, int col_base, int c_lo, int M, int N,
+                                             int lane, const KernelParams& p) {
+  float best0 = -INFINITY, best1 = -INFINITY;
+  int bc0 = -1, bc1 = -1;
+#pragma unroll
+  for (int i = 0; i < 64; ++i) {
+    if (i & 2) continue;   // element i (row r_lo) and i + 2 (row r_lo + 8) share the column
+    const int col = col_base + 8 * (i >> 2) + c_lo + (i & 1);
+    if (col < N) {
+      if (acc[i] > best0) { best0 = acc[i]; bc0 = col; }
+      if (acc[i + 2] > best1) { best1 = acc[i + 2]; bc1 = col; }
+    }
+  }
+  unsigned long long k0 = (bc0 >= 0) ? metric_key(best0, p.col_off + bc0) : 0ull;
+  unsigned long long k1 = (bc1 >= 0) ? metric_key(best1, p.col_off + bc1) : 0ull;
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1) {
+    k0 = max_u64(k0, __shfl_xor_sync(0xffffffffu, k0, o));
+    k1 = max_u64(k1, __shfl_xor_sync(0xffffffffu, k1, o));
+  }
+  if ((lane & 3) == 0) {
+    if (row_lo < M && k0 != 0ull) red_max_u64(p.row_keys + row_lo, k0);
+    if (row_lo + 8 < M && k1 != 0ull) red_max_u64(p.row_keys + row_lo + 8, k1);
+  }
+  const bool v0 = row_lo < M, v1 = row_lo + 8 < M;
+#pragma unroll
+  for (int c = 0; c < kTileN / 32; ++c) {
+    // ck[q], q = 2 j + e: column 32 c + 8 j + c_lo + e of the tile
+    unsigned long long ck[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const int i = 16 * c + 4 * (q >> 1) + (q & 1);
+      const float a = acc[i], b = acc[i + 2];
+      const bool take_a = v0 && (!v1 || a >= b);   // tie: the lower row
+      const int col = col_base + 32 * c + 8 * (q >> 1) + c_lo + (q & 1);
+      ck[q] = (col < N && (v0 || v1)) ? metric_key(take_a ? a : b, p.row_off + (take_a ? row_lo : row_lo + 8)) : 0ull;
+    }
+    // reduce-scatter: after the step over lane bit m, ck[0 .. h) holds the columns q = k + (bit m of lane ? h : 0)
+#pragma unroll
+    for (int h = 4, m = 16; h >= 1; h >>= 1, m >>= 1) {
+      const bool hi = (lane & m) != 0;
+#pragma unroll
+      for (int k = 0; k < h; ++k) {
+        const unsigned long long send = hi ? ck[k] : ck[k + h];
+        const unsigned long long keep = hi ? ck[k + h] : ck[k];
+        ck[k] = max_u64(keep, __shfl_xor_sync(0xffffffffu, send, m));
+      }
+    }
+    const int q = lane >> 2;   // bits 4, 3, 2 of the lane = 4, 2, 1 in q
+    const int col = col_base + 32 * c + 8 * (q >> 1) + c_lo + (q & 1);
+    if (col < N && ck[0] != 0ull) red_max_u64(p.col_keys + col, ck[0]);
+  }
+}
+
 // Epilogue of the out kernel: one row of the fragment (h = 0: row_lo, 1: row_lo + 8), 16 column pairs.
 //   val = scale * (acc * acc_scale + fix * x[row, col]) (+ add_src[row, col]);  written as fp32 or bf16
 // parts / nparts: owner of a split tile — the other K-slices' fp32 partials (float4 j of this thread's fragment at
@@ -521,7 +599,9 @@ __device__ __forceinline__ void mma_loop_f8(float (&sum)[64], float (&acc)[64], 
 // mma_loop_f8 would otherwise cost the production kernels spills).
 // kIds: the loss kernel with labels from sample ids (SIGLIP_OPT_SAMPLE_IDS); its own instantiation, so that the default
 // loss kernel is exactly the code it was without the option.
-template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false>
+// kMetrics: the loss kernel that also reduces the row / column argmax keys of every tile (siglip_request_metrics); its
+// own instantiation for the same reason.
+template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
                    const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1,
@@ -529,6 +609,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
   using C = Cfg<kMode, kStagesT>;
   static_assert(kCS == 1 || kCS == 2 || kCS == 4, "clusters of 1, 2 or 4 CTAs");
   static_assert(!kIds || kMode == kModeLoss, "sample ids are a loss-kernel option");
+  static_assert(!kMetrics || kMode == kModeLoss, "retrieval metrics are a loss-kernel option");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -740,6 +821,8 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
         p.aux_trace[6] = globaltimer_ns();                                   // first tile's MMAs done (CTA 0)
 
       if constexpr (kMode == kModeLoss) {
+        // argmax keys first, on the raw accumulator: whichever path each slab then takes below
+        if constexpr (kMetrics) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
         float acc_sp = 0.f, acc_g = 0.f, acc_gs = 0.f;
         const bool edge = (row0 + kBlockM > pr.M) || (col_base + kTileN > pr.N);
         // 128-aligned row and column blocks: only a block on the diagonal holds positive pairs
@@ -1268,6 +1351,96 @@ __global__ void allreduce_scalars_kernel(const float* __restrict__ saved, const 
   }
 }
 
+// Finalisation of a metrics step, one block. W > 1 follows allreduce_scalars_kernel: publish (flag kind 5 = step) that my
+// column partials are complete, wait for every rank's, then max-combine the W partials of my chunk with relaxed
+// system-scope loads. It never triggers griddepcontrol.launch_dependents: the next step's first loss kernel (launched
+// with programmatic serialization) cannot touch global memory before this kernel has ended (DESIGN.md, "In-batch
+// retrieval metrics").
+constexpr int kMetricsThreads = 1024;
+
+__device__ __forceinline__ int metrics_owner(const MetricsArgs& a, int g) {
+  int o = 0;
+  while (o + 1 < a.world && g >= a.off[o + 1]) ++o;
+  return o;
+}
+
+// sample id of global sample g (image and text of one sample share it)
+__device__ __forceinline__ int64_t metrics_id(const MetricsArgs& a, int g) {
+  const int o = metrics_owner(a, g);
+  const int l = g - a.off[o];
+  return (o == a.rank) ? a.ids_own[l] : a.ids_all[static_cast<size_t>(o) * a.ids_stride + l];
+}
+
+__device__ __forceinline__ int key_index(unsigned long long k) {
+  return k == 0ull ? -1 : static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(k));
+}
+
+__global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const MetricsArgs a) {
+  __shared__ unsigned int hits[2];
+  const int tid = threadIdx.x;
+  if (tid < 2) hits[tid] = 0u;
+  if (a.world > 1) {
+    if (tid < a.world) {
+      __threadfence_system();   // my partials (written by the step's loss kernels) before the flag
+      asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(a.sig_ptrs[tid]), "r"(a.value) : "memory");
+      uint64_t t0 = 0;
+      uint32_t spins = 0;
+      while (true) {
+        unsigned int v;
+        asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(a.flags_local + tid) : "memory");
+        if (v >= a.value) break;
+        if ((++spins & 0xffu) == 0) {
+          const uint64_t now = globaltimer_ns();
+          if (t0 == 0) t0 = now;
+          if (now - t0 > a.timeout_ns) {
+            if (a.dbg != nullptr) {
+              a.dbg->block = tid;
+              a.dbg->aux0 = v;
+              a.dbg->aux1 = a.value;
+              a.dbg->code = 10;
+              __threadfence_system();
+            }
+            __trap();
+          }
+        }
+      }
+      __threadfence();   // order the other threads' peer reads after the observed flags
+    }
+  }
+  __syncthreads();
+  const int me0 = a.off[a.rank];
+  const bool ids = a.ids_own != nullptr;
+  unsigned int h_i2t = 0, h_t2i = 0;
+  for (int i = tid; i < a.B; i += kMetricsThreads) {
+    const int j = key_index(a.row_keys[i]);   // best text of my image i
+    if (a.i2t) a.i2t[i] = j;
+    if (j >= 0) h_i2t += ids ? (metrics_id(a, j) == a.ids_own[i]) : (j == me0 + i);
+    unsigned long long k = a.col_own[i];
+    if (a.world > 1) {
+      for (int q = 0; q < a.world; ++q) {
+        if (q == a.rank) continue;
+        unsigned long long v;
+        asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(a.col_peers[q] + i) : "memory");
+        k = max_u64(k, v);
+      }
+    }
+    const int g = key_index(k);               // best image of my text i
+    if (a.t2i) a.t2i[i] = g;
+    if (g >= 0) h_t2i += ids ? (metrics_id(a, g) == a.ids_own[i]) : (g == me0 + i);
+  }
+  // integer counts: the sum does not depend on the order
+  for (int o = 16; o > 0; o >>= 1) {
+    h_i2t += __shfl_xor_sync(0xffffffffu, h_i2t, o);
+    h_t2i += __shfl_xor_sync(0xffffffffu, h_t2i, o);
+  }
+  if ((tid & 31) == 0) {
+    atomicAdd(&hits[0], h_i2t);
+    atomicAdd(&hits[1], h_t2i);
+  }
+  __syncthreads();
+  if (tid < 2) a.top1[tid] = static_cast<float>(hits[tid]) / static_cast<float>(a.B);
+}
+
 // -------------------------------------------------------------------------------------------------
 // L2 normalisation fused around the loss (SURVEY.md §8f-1: the step the reference's callers run right before it,
 // test_distributed_sigmoid_loss.py:99-101). One warp per row; HBM-bound: coalesced 16-byte accesses, fp32 math.
@@ -1393,12 +1566,12 @@ __global__ void normalize_bwd_kernel(const void* __restrict__ x, const float* __
   }
 }
 
-// kIds selects the sample-id instantiation of the loss kernel (ignored for the out kernel)
-template <int kMode, int kStages, int kCS, bool kF8 = false, bool kIds = false>
+// kIds / kMetrics select the sample-id / retrieval-metrics instantiations of the loss kernel (ignored for the out kernel)
+template <int kMode, int kStages, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false>
 int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensorMap* tmA1, const CUtensorMap* tmB1,
                 const CUtensorMap* tmG, const KernelParams& p, int num_sms, cudaStream_t stream) {
   using C = Cfg<kMode, kStages>;
-  auto kern = siglip_gemm_kernel<kMode, kStages, kCS, kF8, kIds && kMode == kModeLoss>;
+  auto kern = siglip_gemm_kernel<kMode, kStages, kCS, kF8, kIds && kMode == kModeLoss, kMetrics && kMode == kModeLoss>;
   static bool attr_set = false;
   cudaError_t e = cudaSuccess;
   if (!attr_set) {
@@ -1510,10 +1683,15 @@ size_t gemm_smem_bytes(int mode) {
                            : static_cast<size_t>(Cfg<kModeOut, 6>::kSmemBytes);
 }
 
-#define SIGLIP_LAUNCH(MODE, ST, CS)                                                               \
-  return (p.row_ids != nullptr)                                                                   \
-             ? launch_impl<MODE, ST, CS, false, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream) \
-             : launch_impl<MODE, ST, CS>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+// the out kernel never has ids or metric keys, so only the loss kernel takes the three extra instantiations
+#define SIGLIP_LAUNCH(MODE, ST, CS)                                                                          \
+  do {                                                                                                       \
+    const bool ids__ = p.row_ids != nullptr, met__ = p.row_keys != nullptr;                                  \
+    if (ids__ && met__) return launch_impl<MODE, ST, CS, false, true, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream); \
+    if (met__) return launch_impl<MODE, ST, CS, false, false, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);        \
+    if (ids__) return launch_impl<MODE, ST, CS, false, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);               \
+    return launch_impl<MODE, ST, CS>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);                                      \
+  } while (0)
 
 #define SIGLIP_LAUNCH_STAGES(MODE, CS)   \
   do {                                   \
@@ -1596,6 +1774,11 @@ int launch_allreduce_scalars(const float* saved, const float* g, float* mailbox_
                              unsigned long long timeout_ns, DebugRecord* dbg, cudaStream_t stream) {
   allreduce_scalars_kernel<<<1, 32, 0, stream>>>(saved, g, mailbox_local, mailboxes_dev, signal_ptrs_dev, flags_local,
                                                  world, value, dt_prime, dbias, dtp_f64, timeout_ns, dbg);
+  return static_cast<int>(cudaGetLastError());
+}
+
+int launch_metrics_finalize(const MetricsArgs& a, cudaStream_t stream) {
+  metrics_finalize_kernel<<<1, kMetricsThreads, 0, stream>>>(a);
   return static_cast<int>(cudaGetLastError());
 }
 

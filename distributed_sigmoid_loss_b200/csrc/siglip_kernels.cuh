@@ -123,6 +123,14 @@ struct KernelParams {
   int pdl;                     // 1: launched with programmatic stream serialization (griddepcontrol in the kernel)
   unsigned long long peer_timeout_ns;  // bound of every wait on a peer flag (a dead peer traps instead of hanging)
   unsigned long long* aux_trace;       // optional [4] globaltimer stamps of CTA 0's aux thread: start, flags seen, jobs done
+  // In-batch retrieval metrics (siglip_request_metrics), loss kernel only. Appended last so that the parameter offsets of
+  // the default instantiation do not move. Non-null keys select the kMetrics instantiation. A key is
+  // (order-preserving bits of s) << 32 | (0xFFFFFFFF - global index), combined with an atomic unsigned max: the best
+  // candidate, ties to the lowest index, independent of the order of the atomics.
+  unsigned long long* row_keys;  // [M]: best text (global index) of each image of this rank
+  unsigned long long* col_keys;  // [N]: best image (global index) of each text of the chunk, over this rank's images
+  int row_off;                   // global index of this rank's first image
+  int col_off;                   // global index of the chunk's first text
 };
 
 enum KernelMode { kModeLoss = 0, kModeOut = 1 };
@@ -174,6 +182,30 @@ int launch_allreduce_scalars(const float* saved, const float* g, float* mailbox_
                              unsigned int value, float* dt_prime, float* dbias, int dtp_f64,
                              unsigned long long timeout_ns, DebugRecord* dbg, cudaStream_t stream);
 int launch_signal_flags(unsigned int* const* flag_ptrs_dev, int n, unsigned int value, cudaStream_t stream);
+
+// Finalisation of a metrics step (one block, after the step's last loss kernel). W > 1: publish "my column partials of
+// step `value` are complete" (flag kind 5) to every rank, wait for every rank's, and max-combine the W partials of my
+// chunk. Then decode the keys into global indices and count the hits (positional, or same sample id).
+constexpr int kMetricsMaxWorld = 32;
+struct MetricsArgs {
+  const unsigned long long* row_keys;          // [B] local
+  const unsigned long long* col_own;           // [B] my partial of my chunk
+  const unsigned long long* const* col_peers;  // [world] every rank's partial of my chunk (world > 1; own entry unused)
+  int B, rank, world;
+  int off[kMetricsMaxWorld + 1];               // prefix sums of the per-rank batches
+  const int64_t* ids_own;                      // null = positional labels; else this rank's sample ids
+  const int64_t* ids_all;                      // [world][ids_stride]: every chunk's ids, gathered in this step
+  int ids_stride;
+  float* top1;                                 // [2]: i2t, t2i
+  int64_t* i2t;                                // [B] or null
+  int64_t* t2i;                                // [B] or null
+  unsigned int* const* sig_ptrs;               // [world] flag kind 5 of every rank (world > 1)
+  const volatile unsigned int* flags_local;    // my flag kind 5 row
+  unsigned int value;
+  unsigned long long timeout_ns;
+  DebugRecord* dbg;
+};
+int launch_metrics_finalize(const MetricsArgs& a, cudaStream_t stream);
 int launch_wait_flags(const volatile unsigned int* flags, int n, unsigned int value, unsigned long long timeout_ns,
                       DebugRecord* dbg, cudaStream_t stream);
 

@@ -119,6 +119,29 @@ class SigmoidLossEngine:
             raise RuntimeError(f"sample ids must be a contiguous int64 [{n}] tensor on {self.device}, got "
                                f"{tuple(ids.shape)} {ids.dtype} on {ids.device}")
 
+    def request_metrics(self, top1: torch.Tensor, i2t_index: Optional[torch.Tensor] = None,
+                        t2i_index: Optional[torch.Tensor] = None) -> None:
+        """Arm the in-batch retrieval metrics of the NEXT step (siglip_request_metrics): top1 fp32 [2] (i2t, t2i),
+        i2t_index / t2i_index int64 [B] (global indices) or None, all contiguous on the engine's device. Nothing is read
+        on the host; the step writes them on its stream."""
+        bufs = ((top1, torch.float32, 2), (i2t_index, torch.int64, self.batch), (t2i_index, torch.int64, self.batch))
+        for k, (x, dt, n) in enumerate(bufs):
+            if x is None and k > 0:
+                continue
+            if x is None or x.dtype != dt or tuple(x.shape) != (n,) or not x.is_contiguous() or x.device != self.device:
+                raise RuntimeError(f"metric output {k} must be a contiguous {dt} [{n}] tensor on {self.device}")
+        _capi.check(self._L.siglip_request_metrics(self._h, top1.data_ptr(),
+                                                   i2t_index.data_ptr() if i2t_index is not None else None,
+                                                   t2i_index.data_ptr() if t2i_index is not None else None))
+
+    def debug_set_peer_metric_keys(self, peer: int, keys: torch.Tensor) -> None:
+        """Loopback: the column argmax keys ([B] int64 holding the 64-bit key bits) standing in for peer `peer`'s partial
+        of this rank's text chunk."""
+        if keys.dtype != torch.int64 or tuple(keys.shape) != (self.batch,) or not keys.is_contiguous() or \
+                keys.device != self.device:
+            raise RuntimeError(f"peer metric keys must be a contiguous int64 [{self.batch}] tensor on {self.device}")
+        _capi.check(self._L.siglip_debug_set_peer_metric_keys(self._h, peer, keys.data_ptr(), self._stream()))
+
     def debug_get_slot(self, chunk: int) -> torch.Tensor:
         out = torch.empty(self.batch_per_rank[chunk], self.dim, device=self.device, dtype=torch.float32)
         _capi.check(self._L.siglip_debug_get_slot(self._h, chunk, out.data_ptr(), self._stream()))
@@ -381,11 +404,13 @@ class _SigmoidLossFn(torch.autograd.Function):
         operands, every cross-rank flag handled inside the kernels) which leaves the gradients for an upstream gradient
         of 1; backward = one multiply by grad_output per tensor (siglip_scale). O(B^2) workspace.
     normalize=True additionally fuses F.normalize of both inputs (forward) and its backward around the loss.
-    ids: [B] int64 sample ids (SIGLIP_OPT_SAMPLE_IDS engines), set before every step the engine runs for this call."""
+    ids: [B] int64 sample ids (SIGLIP_OPT_SAMPLE_IDS engines), set before every step the engine runs for this call.
+    metrics: (top1, i2t_index, t2i_index) output buffers: the retrieval metrics of this call's step are armed. A re-run
+    of the forward by the backward's generation guard does not arm them again (they belong to the first run)."""
 
     @staticmethod
     def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool = False, fused: bool = False,
-                ids: Optional[torch.Tensor] = None):
+                ids: Optional[torch.Tensor] = None, metrics=None):
         need_grad = any(ctx.needs_input_grad[:4])
         raw = None
         # bf16 callers: bf16 operands (what autograd would multiply). Anything wider (the reference's own test feeds
@@ -422,6 +447,8 @@ class _SigmoidLossFn(torch.autograd.Function):
         ctx.ids = ids
         if ids is not None:
             engine.set_sample_ids(ids)
+        if metrics is not None:
+            engine.request_metrics(*metrics)
         if ctx.fused:
             # gradients in the dtype autograd would return for these inputs (fp32 when a projection follows)
             gdt = torch.bfloat16 if (not hi and not normalize) else torch.float32
@@ -487,7 +514,7 @@ class _SigmoidLossFn(torch.autograd.Function):
                 gt = dtxt.to(tdt) if ctx.needs_input_grad[1] else None
         gp = dtp.reshape(pshape).to(device=pdev, dtype=pdt) if ctx.needs_input_grad[2] else None
         gb = db.reshape(bshape).to(device=bdev, dtype=bdt) if ctx.needs_input_grad[3] else None
-        return gi, gt, gp, gb, None, None, None, None
+        return gi, gt, gp, gb, None, None, None, None, None
 
 
 class _EngineCache:
@@ -539,6 +566,24 @@ def _validate_ids(sample_ids, multi_positive: bool, embeddings: torch.Tensor) ->
     return sample_ids.to(torch.int64).contiguous()
 
 
+def _validate_return_metrics(return_metrics) -> None:
+    if not isinstance(return_metrics, bool):
+        raise RuntimeError(f"return_metrics must be a bool, got {type(return_metrics).__name__}")
+
+
+def _metric_buffers(batch: int, device: torch.device):
+    top1 = torch.empty(2, device=device, dtype=torch.float32)
+    return (top1, torch.empty(batch, device=device, dtype=torch.int64),
+            torch.empty(batch, device=device, dtype=torch.int64))
+
+
+def _metric_dict(bufs) -> Dict[str, torch.Tensor]:
+    """The in-batch retrieval metrics of a step, as device tensors (no host synchronisation): top-1 rates of this rank's
+    images / texts (0-dim fp32) and the global index of each one's best match (int64 [B])."""
+    top1, i2t, t2i = bufs
+    return {"i2t_top1": top1[0], "t2i_top1": top1[1], "i2t_index": i2t, "t2i_index": t2i}
+
+
 def _validate(image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, expect_batch: Optional[int]) -> None:
     if image_embeddings.dim() != 2 or text_embeddings.dim() != 2:
         raise RuntimeError("image_embeddings and text_embeddings must be 2-D [batch, emb_dim]")
@@ -580,6 +625,12 @@ class DDPSigmoidLoss(nn.Module):
     ``multi_positive=True``: every ``forward`` takes ``sample_ids`` ([B] integers, one per sample on this rank), and a pair
     is positive iff its image and text carry the same id — on any rank (repeated captions, several captions of one
     image, a sample drawn twice). Unique ids give exactly the default labels. Collective: set on every rank.
+
+    ``forward(..., return_metrics=True)`` returns ``(loss, metrics)``: the in-batch retrieval top-1 of this rank's images
+    and texts over the whole global batch (``i2t_top1``, ``t2i_top1``, 0-dim fp32) and the global index of each one's best
+    match (``i2t_index``, ``t2i_index``, int64 [B]), computed by the loss kernels from the logits they already hold; a
+    hit is the positional pair, or a pair with the same id under ``multi_positive``. Device tensors, no host
+    synchronisation, not differentiable; loss and gradients are unchanged. Collective: every rank asks on the same steps.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
@@ -608,14 +659,17 @@ class DDPSigmoidLoss(nn.Module):
         return self._cache.get(batch, (dim + 7) // 8 * 8, device)
 
     def forward(self, image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, *,
-                sample_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
+                sample_ids: Optional[torch.Tensor] = None, return_metrics: bool = False):
+        _validate_return_metrics(return_metrics)
         ids = _validate_ids(sample_ids, self.multi_positive, image_embeddings)
         _validate(image_embeddings, text_embeddings, self.gpu_batch_size)
         image_embeddings, text_embeddings = _pad_dim(image_embeddings), _pad_dim(text_embeddings)
         eng = self._cache.get(image_embeddings.shape[0], image_embeddings.shape[1], image_embeddings.device)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
-        return _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
-                                    self.normalize_inputs, fused, ids)
+        bufs = _metric_buffers(eng.batch, eng.device) if return_metrics else None
+        loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
+                                    self.normalize_inputs, fused, ids, bufs)
+        return (loss, _metric_dict(bufs)) if return_metrics else loss
 
 
 SigmoidLoss = DDPSigmoidLoss
@@ -626,7 +680,9 @@ class SigLipLoss(nn.Module):
     exchange of the original is replaced by the direct NVSwitch pulls of the fused path. ``bidir`` selects the
     visiting order of the original's bidirectional exchange (rank+1, rank-1, rank+2, ...) instead of rank+1, rank+2,
     ...; the pairs covered and the result are the same. ``multi_positive=True``: labels from the ``sample_ids`` every
-    forward then takes, as in ``DDPSigmoidLoss``."""
+    forward then takes, as in ``DDPSigmoidLoss``. ``return_metrics=True``: returns ``(loss_or_dict, metrics)`` with the
+    retrieval metrics of ``DDPSigmoidLoss``; they stay out of the ``output_dict``, whose values open_clip sums into the
+    total loss."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
@@ -640,7 +696,8 @@ class SigLipLoss(nn.Module):
         self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive)
 
     def forward(self, image_features, text_features, logit_scale, logit_bias, output_dict: bool = False, *,
-                sample_ids: Optional[torch.Tensor] = None):
+                sample_ids: Optional[torch.Tensor] = None, return_metrics: bool = False):
+        _validate_return_metrics(return_metrics)
         ids = _validate_ids(sample_ids, self.multi_positive, image_features)
         _validate(image_features, text_features, None)
         image_features, text_features = _pad_dim(image_features), _pad_dim(text_features)
@@ -652,5 +709,7 @@ class SigLipLoss(nn.Module):
         if logit_bias is None:
             logit_bias = torch.zeros((), device=image_features.device)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
-        loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids)
-        return {"contrastive_loss": loss} if output_dict else loss
+        bufs = _metric_buffers(eng.batch, eng.device) if return_metrics else None
+        loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs)
+        out = {"contrastive_loss": loss} if output_dict else loss
+        return (out, _metric_dict(bufs)) if return_metrics else out

@@ -220,6 +220,25 @@ unsigned long long siglip_ctx_saved_generation(const siglip_ctx* ctx);
  */
 int siglip_set_sample_ids(siglip_ctx* ctx, const int64_t* ids_dev, void* cuda_stream);
 
+/*
+ * In-batch retrieval metrics of the NEXT siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd call (that step only),
+ * computed from the logits the loss kernels already hold in registers, without a second similarity GEMM:
+ *   i2t_index[i] = argmax_j s_ij over all sum(B) texts, for each of this rank's B images (global text index)
+ *   t2i_index[j] = argmax_i s_ij over all sum(B) images, for each of this rank's B texts (global image index)
+ *   top1[0] / top1[1] = fraction of this rank's images / texts whose top-1 is a positive: the positional diagonal, or
+ *                       under SIGLIP_OPT_SAMPLE_IDS a pair with the same id, on any rank
+ * Global indices follow the concatenated batch (prefix sums of the per-rank batches). Ties go to the lowest global index;
+ * the ranking uses the kernel's fp32 <img, txt> (z = exp(t') s + b is monotone in s). Per rank, like the loss.
+ * top1: 2 fp32 device floats (required); i2t_index / t2i_index: [B] int64 device buffers or NULL. Loss and gradients are
+ * bit-identical to the same step without metrics. Cost: the step's loss kernels run an instantiation that also reduces
+ * the argmax keys, plus two launches (a memset of the keys and a one-block finalisation kernel). This call only records
+ * the pointers and reads nothing on the host, so a single-rank metrics step can be captured into a CUDA graph. On a
+ * single-rank context the first call allocates the key buffers (4 x B 64-bit words; also allowed inside a capture), so a
+ * context that never asks for metrics holds exactly the workspace it held before.
+ * Collective: every rank arms the same steps. The host-buffer entries return SIGLIP_ERR_STATE while armed.
+ */
+int siglip_request_metrics(siglip_ctx* ctx, float* top1, int64_t* i2t_index, int64_t* t2i_index);
+
 /* Forward only (torch.no_grad / evaluation): siglip_forward with save_for_backward = 0. */
 int siglip_fwd(siglip_ctx* ctx, const void* img, const void* txt, const float* t_prime, const float* bias,
                float* loss, void* cuda_stream);
@@ -292,6 +311,10 @@ int siglip_debug_set_chunk_ids(siglip_ctx* ctx, int chunk, const int64_t* ids_de
 /* Loopback only: seed the (dt_prime, dbias) mailbox standing in for peer rank `peer`, so that the mean computed under
  * SIGLIP_OPT_SYNC_SCALAR_GRADS can be checked against numbers the kernel did not produce itself. */
 int siglip_debug_set_mailbox(siglip_ctx* ctx, int peer, float dt_prime, float dbias);
+/* Loopback only: seed the column argmax partials of this rank's text chunk that stand in for peer rank `peer`'s
+ * ([B] 64-bit keys: (order-preserving fp32 bits of s) << 32 | (0xFFFFFFFF - global image index), 0 = no candidate), so
+ * that the cross-rank combine of a metrics step sees candidates the kernel did not produce itself. */
+int siglip_debug_set_peer_metric_keys(siglip_ctx* ctx, int peer, const uint64_t* keys_dev, void* cuda_stream);
 /* With SIGLIP_OPT_AUX_TRACE: device-synchronise and copy out 16 globaltimer stamps (ns) per launch since the last call:
  * [0..2] auxiliary warps of CTA 0: start, last peer flag observed (0 = no wait), jobs done; [3] launch end as seen by
  * the last CTA; [4] kernel entry (CTA 0); [5] set-up done (barriers); [6] MMAs of the first tile done (CTA 0);

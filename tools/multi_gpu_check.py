@@ -40,6 +40,9 @@ def main() -> int:
     ap.add_argument("--skip-parity", action="store_true")
     ap.add_argument("--sample-ids", action="store_true",
                     help="also check multi-positive labels from sample ids (duplicates across ranks) against the oracle")
+    ap.add_argument("--metrics", action="store_true",
+                    help="also check the in-batch retrieval metrics (return_metrics=True) against the float64 oracle, with "
+                         "and without shared sample ids, uneven batches, fused and split schedules")
     ap.add_argument("--soak", type=int, default=0,
                     help="N > 0: that many back-to-back steps at the --batch/--dim shape mixing the fused step, the split "
                          "API and forward-only calls; same inputs, so every step of a kind must reproduce its first result "
@@ -228,6 +231,58 @@ def main() -> int:
                         dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
                         db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
                 del modx
+
+    # ---- in-batch retrieval metrics: texts are perturbed images under a permutation (a fifth of them point at another
+    # rank's sample), so the top-1 of every direction crosses ranks; uneven batches; ids shared across ranks ----------
+    if args.metrics:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from retrieval_metrics_oracle import hits, retrieval_metrics
+        from distributed_sigmoid_loss_b200 import SigmoidLossEngine
+        Bs = [96 + 40 * r for r in range(world)]
+        D, tp, bias = 128, math.log(10.0), -10.0
+        g = torch.Generator().manual_seed(555)
+        n = sum(Bs)
+        img_all = torch.nn.functional.normalize(torch.randn(n, D, generator=g))
+        perm = torch.arange(n)
+        sel = torch.randperm(n, generator=g)[: n // 5]
+        perm[sel] = sel.roll(1)
+        txt_all = torch.nn.functional.normalize(img_all[perm] + 0.1 * torch.randn(n, D, generator=g))
+        img_all, txt_all = img_all.to(torch.bfloat16), txt_all.to(torch.bfloat16)
+        ids_all = torch.arange(n) % (n // 2)                 # every id twice, mostly on two different ranks
+        imgs, txts, idss = (list(torch.split(x, Bs)) for x in (img_all, txt_all, ids_all))
+        off = sum(Bs[:rank])
+        for with_ids in (False, True):
+            res = retrieval_metrics([x.float().numpy() for x in imgs], [x.float().numpy() for x in txts],
+                                    [x.numpy() for x in idss] if with_ids else None)[rank]
+            eng = SigmoidLossEngine(Bs[rank], D, dev, batch_per_rank=Bs)
+            if with_ids:
+                eng.set_option(_capi.SIGLIP_OPT_SAMPLE_IDS, 1)
+            tpt, bt = torch.tensor([tp], device=dev), torch.tensor([bias], device=dev)
+            img, txt = imgs[rank].to(dev), txts[rank].to(dev)
+            for sched in ("fused", "split", "fwd", "fused"):
+                top1 = torch.empty(2, device=dev)
+                i2t = torch.empty(Bs[rank], device=dev, dtype=torch.int64)
+                t2i = torch.empty(Bs[rank], device=dev, dtype=torch.int64)
+                if with_ids:
+                    eng.set_sample_ids(idss[rank].to(dev))
+                eng.request_metrics(top1, i2t, t2i)
+                if sched == "fused":
+                    eng.fwd_bwd(img, txt, tpt, bt)
+                elif sched == "split":
+                    eng.forward(img, txt, tpt, bt, True)
+                    eng.backward(img, txt, tpt, None)
+                else:
+                    eng.fwd(img, txt, tpt, bt)
+                torch.cuda.synchronize()
+                gi, gt = i2t.cpu().numpy(), t2i.cpu().numpy()
+                ok_i, ok_t = res["i2t_margin"] > 1e-3, res["t2i_margin"] > 1e-3
+                hi, ht = hits(gi, res["gid"], off), hits(gt, res["gid"], off)
+                report(f"retrieval metrics ids={with_ids} {sched} B={Bs}", dict(
+                    i2t_index=float((gi != res["i2t_index"])[ok_i].mean()),
+                    t2i_index=float((gt != res["t2i_index"])[ok_t].mean()),
+                    i2t_top1=abs(float(top1[0]) - hi.mean()), t2i_top1=abs(float(top1[1]) - ht.mean()),
+                    unclear_rows=float(1.0 - min(ok_i.mean(), ok_t.mean())) / 50), tol=1e-6)
+            eng.close()
 
     # ---- larger: fp32 autograd; dtxt reference summed over ranks ------------------------------------------
     B, D, tp, bias = 2048, 768, math.log(10.0), -10.0
