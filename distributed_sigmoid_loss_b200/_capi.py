@@ -22,6 +22,7 @@ EXPORTED_SYMBOLS = (
     "siglip_device_count",
     "siglip_ctx_create",
     "siglip_ctx_create_uneven",
+    "siglip_ctx_create_texts",
     "siglip_ctx_set_option",
     "siglip_ctx_workspace_bytes",
     "siglip_ctx_handle_bytes",
@@ -43,6 +44,9 @@ EXPORTED_SYMBOLS = (
     "siglip_scale",
     "siglip_normalize_fwd",
     "siglip_normalize_bwd",
+    "siglip_normalize_fwd_rows",
+    "siglip_convert_f32_rows",
+    "siglip_normalize_bwd_rows",
     "siglip_ctx_kernel_times",
     "siglip_ctx_launch_count",
     "siglip_debug_gemm",
@@ -144,6 +148,8 @@ def lib() -> ctypes.CDLL:
     L.siglip_fwd_bwd_scaled.restype = ci
     L.siglip_ctx_create_uneven.argtypes = [ctypes.POINTER(vp), ci, ci, ci, ctypes.POINTER(ci), ci]
     L.siglip_ctx_create_uneven.restype = ci
+    L.siglip_ctx_create_texts.argtypes = [ctypes.POINTER(vp), ci, ci, ci, ctypes.POINTER(ci), ctypes.POINTER(ci), ci]
+    L.siglip_ctx_create_texts.restype = ci
     L.siglip_host_submit_grads.argtypes = [vp, vp, vp, ctypes.c_float, ctypes.c_float, vp, vp,
                                            ctypes.POINTER(ctypes.c_ulonglong), vp]
     L.siglip_host_submit_grads.restype = ci
@@ -166,6 +172,12 @@ def lib() -> ctypes.CDLL:
     L.siglip_normalize_fwd.restype = ci
     L.siglip_normalize_bwd.argtypes = [vp, vp, ci, vp, vp, ci, vp, vp]
     L.siglip_normalize_bwd.restype = ci
+    L.siglip_normalize_fwd_rows.argtypes = [vp, ci, vp, ci, vp, vp, vp]
+    L.siglip_normalize_fwd_rows.restype = ci
+    L.siglip_convert_f32_rows.argtypes = [vp, ci, vp, vp, vp]
+    L.siglip_convert_f32_rows.restype = ci
+    L.siglip_normalize_bwd_rows.argtypes = [vp, ci, vp, ci, vp, vp, ci, vp, vp]
+    L.siglip_normalize_bwd_rows.restype = ci
     L.siglip_scale.argtypes = [vp, vp, vp, cs, ci, vp, vp]
     L.siglip_scale.restype = ci
     L.siglip_ctx_kernel_times.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ci),

@@ -150,6 +150,8 @@ struct IpcBlob {
   int B;
   int D;
   int Bmax;
+  int T;      // texts of the rank (B + its hard negatives)
+  int Tmax;
   char host[64];
 };
 
@@ -158,7 +160,15 @@ struct IpcBlob {
 struct siglip_ctx {
   int device = 0, rank = 0, world = 1, B = 0, D = 0, Bp = 0;
   int Bs[kMaxWorld] = {};                // per-rank batch (all equal to B unless created with siglip_ctx_create_uneven)
-  int Bmax = 0;                          // max over ranks: stride of every per-chunk buffer is Bmax * D elements
+  int Bmax = 0;                          // max over ranks
+  // text chunks (siglip_ctx_create_texts): rank p holds Ts[p] = Bs[p] + K_p texts, its B_p paired texts followed by K_p
+  // hard negatives. Without extras Ts == Bs and everything below is what it was before they existed.
+  int T = 0;                             // this rank's texts
+  int Ts[kMaxWorld] = {};
+  int Tmax = 0;                          // stride of every per-chunk text buffer is Tmax * D elements
+  int Tp = 0;                            // columns of the sigma operands: Tmax rounded up to 256
+  bool extras = false;                   // some rank has hard negatives (T_p != B_p)
+  int toff[kMaxWorld + 1] = {};          // global index of every rank's first text (prefix sums of Ts)
   int num_sms = 0;
   // options
   int cta_group = 2;
@@ -191,27 +201,27 @@ struct siglip_ctx {
   // diagnostics, read from the environment once at context creation (see include/siglip_b200.h)
   bool dbg_no_gstore = false, dbg_no_cvt = false, dbg_loss_waitstats = false;
   // workspaces
-  __nv_bfloat16* txt_all = nullptr;      // [world][Bmax, D] bf16; slot `rank` is what the peers pull (world > 1),
+  __nv_bfloat16* txt_all = nullptr;      // [world][Tmax, D] bf16; slot `rank` is what the peers pull (world > 1),
                                          // followed by ids_all in the same (IPC-exported) allocation
   int64_t* ids_all = nullptr;            // [world][ids_stride] sample ids of every text chunk (world > 1)
   int64_t* ids_in = nullptr;             // [ids_stride] this rank's ids for the next step (siglip_set_sample_ids)
   int ids_stride = 0;                    // Bmax rounded up to even: every slot is a whole number of 16-byte vectors
-  unsigned long long* mkeys[2] = {};     // per step parity: [world][Bmax] column argmax partials of every text chunk
+  unsigned long long* mkeys[2] = {};     // per step parity: [world][Tmax] column argmax partials of every text chunk
                                          // over my images, then [Bmax] row keys. world > 1: behind ids_all (exported)
-  __nv_bfloat16* G[kMaxWorld] = {};      // [Bp, Bp] sigma operands (fp16 bits x kGScale), diagonal zeroed, allocated on
+  __nv_bfloat16* G[kMaxWorld] = {};      // [Bp, Tp] sigma operands (fp16 bits x kGScale), diagonal zeroed, allocated on
                                          // first use: fused step 2 (own chunk + the chunk in flight), split API one per chunk
   __nv_bfloat16* img16 = nullptr;        // [B, D] fp16 (x kXScale) images: B operand of the dtxt contraction
-  __nv_bfloat16* txt16[kMaxWorld] = {};  // [Bmax, D] fp16 (x kXScale) text chunks: B operand of dimg (same count as G)
+  __nv_bfloat16* txt16[kMaxWorld] = {};  // [Tmax, D] fp16 (x kXScale) text chunks: B operand of dimg (same count as G)
   float* g_diag = nullptr;               // [Bp] fp32 positive-pair terms -sigma(-z_ii)
-  float* slots = nullptr;                // [world][Bmax, D] fp32 dtxt contributions, slot c is for owner c (world > 1)
+  float* slots = nullptr;                // [world][Tmax, D] fp32 dtxt contributions, slot c is for owner c (world > 1)
   float* dimg_acc = nullptr;             // [B, D] fp32 running dimg over the chunks (world > 1)
-  float* dtxt_acc = nullptr;             // [B, D] fp32 running sum of the peers' contributions (world > 1)
+  float* dtxt_acc = nullptr;             // [T, D] fp32 running sum of the peers' contributions (world > 1)
   double* partials = nullptr;            // [num_sms][4]
   unsigned int* fin_counter = nullptr;   // ticket counter of the loss kernel's last-CTA finalisation
   unsigned int* flags = nullptr;         // [kFlagKinds][kMaxWorld]
   unsigned int* sync_words = nullptr;    // [kSyncWords] local tickets / flags
   float* loop_mailboxes = nullptr;       // loopback only: [world][2] stand-ins for the peers' (dt', dbias) mailboxes
-  float* loop_zero = nullptr;            // loopback only: [world][Bmax, D] zeros standing in for the peers' contribution slots
+  float* loop_zero = nullptr;            // loopback only: [world][Tmax, D] zeros standing in for the peers' contribution slots
   unsigned long long* loop_keys = nullptr;  // loopback only: [world][Bmax] the peers' column partials of my chunk
   float* scalars = nullptr;              // [24] device scalars: host API staging, saved dt'/dbias of the last forward
   unsigned long long* aux_trace = nullptr;  // [kTraceLaunches][16] globaltimer stamps (SIGLIP_OPT_AUX_TRACE)
@@ -282,7 +292,8 @@ int timing_mark(siglip_ctx* c, std::vector<cudaEvent_t>& evs, size_t& used, cuda
   return 0;
 }
 
-inline size_t chunk_stride(const siglip_ctx* c) { return static_cast<size_t>(c->Bmax) * c->D; }
+// elements between consecutive text chunks of txt_all / slots / loop_zero (and the size of a txt16 copy)
+inline size_t chunk_stride(const siglip_ctx* c) { return static_cast<size_t>(c->Tmax) * c->D; }
 
 // Sample ids of text chunk `cidx` as the loss kernel reads them (null outside SIGLIP_OPT_SAMPLE_IDS): the caller's ids
 // for the own chunk, the gathered copy for the others.
@@ -311,8 +322,12 @@ inline unsigned long long peer_timeout_ns(const siglip_ctx* c) {
 
 // ---- retrieval metrics (siglip_request_metrics) ----
 static_assert(siglip::kMetricsMaxWorld == kMaxWorld, "the finalisation kernel takes one batch offset per rank");
-// 64-bit keys per step parity: [world][Bmax] column partials, then [Bmax] row keys
-inline size_t mkeys_block(const siglip_ctx* c) { return static_cast<size_t>(c->world + 1) * c->Bmax; }
+// 64-bit keys per step parity: [world][Tmax] column partials (the loss kernel writes one per text of the chunk; the
+// finalisation reads the paired ones), then [Bmax] row keys
+inline size_t mkeys_block(const siglip_ctx* c) {
+  return static_cast<size_t>(c->world) * c->Tmax + static_cast<size_t>(c->Bmax);
+}
+inline size_t mkeys_rows(const siglip_ctx* c) { return static_cast<size_t>(c->world) * c->Tmax; }
 // byte offset of the two key blocks in the exported text allocation: behind the gathered text and ids
 inline size_t mkeys_offset(const siglip_ctx* c) {
   return chunk_stride(c) * c->world * sizeof(__nv_bfloat16) + static_cast<size_t>(c->world) * c->ids_stride * sizeof(int64_t);
@@ -337,12 +352,15 @@ int finalize_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
   const int W = c->world;
   siglip::MetricsArgs a;
   memset(&a, 0, sizeof(a));
-  a.row_keys = c->mkeys_step + static_cast<size_t>(W) * c->Bmax;
-  a.col_own = c->mkeys_step + static_cast<size_t>(c->rank) * c->Bmax;
+  a.row_keys = c->mkeys_step + mkeys_rows(c);
+  a.col_own = c->mkeys_step + static_cast<size_t>(c->rank) * c->Tmax;
   a.B = c->B;
   a.rank = c->rank;
   a.world = W;
-  for (int p = 0; p <= W; ++p) a.off[p] = c->off[p];
+  for (int p = 0; p <= W; ++p) {
+    a.off[p] = c->off[p];
+    a.toff[p] = c->toff[p];
+  }
   if (c->sample_ids) {
     a.ids_own = c->ids_in;
     a.ids_all = c->ids_all;
@@ -369,7 +387,7 @@ int finalize_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
 // flight), the split forward / backward API one per text chunk (they all live from the forward to the backward).
 int ensure_g(siglip_ctx* c, int i) {
   if (c->G[i] != nullptr) return 0;
-  const size_t gbytes = static_cast<size_t>(c->Bp) * c->Bp * sizeof(__nv_bfloat16);
+  const size_t gbytes = static_cast<size_t>(c->Bp) * c->Tp * sizeof(__nv_bfloat16);
   const size_t tbytes = chunk_stride(c) * sizeof(__nv_bfloat16);
   cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&c->G[i]), gbytes);
   if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&c->txt16[i]), tbytes);
@@ -381,7 +399,7 @@ int ensure_g(siglip_ctx* c, int i) {
     snprintf(buf, sizeof(buf),
              "sigma operand %d needs %.2f GiB more device memory (B = %d: %d x %d 16-bit per text chunk kept for the "
              "backward; siglip_fwd_bwd needs 2 of them, the split forward/backward API one per rank): %s",
-             i, static_cast<double>(gbytes + tbytes) / (1024.0 * 1024.0 * 1024.0), c->Bmax, c->Bp, c->Bp,
+             i, static_cast<double>(gbytes + tbytes) / (1024.0 * 1024.0 * 1024.0), c->Bmax, c->Bp, c->Tp,
              cudaGetErrorString(e));
     return fail(SIGLIP_ERR_CUDA, buf);
   }
@@ -464,8 +482,8 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
   const int mc = c->mcast;
   if ((rc = encode_operand(&tmB, txt_c, Bn, c->D, c->D, 0, siglip::b_box_rows_kmajor(siglip::cluster_size(cg, mc)))))
     return rc;
-  // store map of the sigma operand: [B, Bn] inside the padded [Bp, Bp] buffer, one 16-row x 32-column slab per TMA store
-  if ((rc = encode_bf16_2d(&tmG, G, (uint64_t)Bn, (uint64_t)c->B, (uint64_t)c->Bp, 32, 16,
+  // store map of the sigma operand: [B, Bn] inside the padded [Bp, Tp] buffer, one 16-row x 32-column slab per TMA store
+  if ((rc = encode_bf16_2d(&tmG, G, (uint64_t)Bn, (uint64_t)c->B, (uint64_t)c->Tp, 32, 16,
                            CU_TENSOR_MAP_SWIZZLE_64B)))
     return rc;
   KernelParams p;
@@ -481,23 +499,26 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
   p.bias = bias;
   p.inv_b = 1.0f / static_cast<float>(c->B);
   p.G = G;
-  p.ldg = c->Bp;
+  p.ldg = c->Tp;
   p.g_diag = c->g_diag;
+  // the own chunk's positives are its first B columns (row == col < M); the hard negatives behind them never are
   p.own_chunk = own ? 1 : 0;
   p.store_g = save ? 1 : 0;
   p.g_scale = kGScale;
   if (col_ids != nullptr) {
     p.row_ids = c->ids_in;
     p.col_ids = col_ids;
+    p.col_pos_n = c->Bs[cidx];   // the chunk's ids cover its paired texts only
   }
   if (c->mkeys_step != nullptr) {   // a metrics step: the kMetrics instantiation reduces the argmax keys
-    p.row_keys = c->mkeys_step + static_cast<size_t>(c->world) * c->Bmax;
-    p.col_keys = c->mkeys_step + static_cast<size_t>(cidx) * c->Bmax;
+    p.row_keys = c->mkeys_step + mkeys_rows(c);
+    p.col_keys = c->mkeys_step + static_cast<size_t>(cidx) * c->Tmax;
     p.row_off = c->off[c->rank];
-    p.col_off = c->off[cidx];
+    p.col_off = c->toff[cidx];
   }
   p.partials = c->partials;
   p.accumulate_partials = first ? 0 : 1;  // the first chunk of a forward overwrites every slot of the grid
+  p.grid_n = c->Tmax;                     // ... and every chunk launches that same grid (see launch_gemm)
   if (fin != nullptr) {
     p.fin_counter = c->fin_counter;
     p.fin_loss = fin->loss;
@@ -572,6 +593,7 @@ struct GradOut {
 // The two gradient contractions of one chunk in one launch (g = upstream gradient, device scalar or null):
 //   prob 0: dimg (+)= g (t/B) (G @ txt_c  [+ g_diag * txt_own])      A = G K-major,  B = txt16[gi] N-major     K = Bn
 //   prob 1: dtxt_c  = g (t/B) (G^T @ img  [+ g_diag * img])          A = G M-major,  B = img16 N-major         K = B
+// Bn is the chunk's text count (its batch plus its hard negatives); the bracketed terms cover the first B rows only.
 int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_bfloat16* txt_own, int Bn,
                    const float* t_prime, const float* grad_out, const GradOut& o, const AuxList& aux,
                    const EndSignal& end, cudaStream_t st) {
@@ -580,9 +602,9 @@ int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_
   CUtensorMap tmA0, tmB0, tmA1, tmB1;
   int rc;
   if (c->G[gi] == nullptr) return fail(SIGLIP_ERR_STATE, "gradient kernel without a saved sigma operand");
-  if ((rc = encode_operand(&tmA0, c->G[gi], c->B, Bn, c->Bp, 0, 128))) return rc;
+  if ((rc = encode_operand(&tmA0, c->G[gi], c->B, Bn, c->Tp, 0, 128))) return rc;
   if ((rc = encode_operand(&tmB0, c->txt16[gi], c->D, Bn, c->D, 1, 0, bk))) return rc;
-  if ((rc = encode_operand(&tmA1, c->G[gi], Bn, c->B, c->Bp, 1, 0))) return rc;
+  if ((rc = encode_operand(&tmA1, c->G[gi], Bn, c->B, c->Tp, 1, 0))) return rc;
   if ((rc = encode_operand(&tmB1, c->img16, c->D, c->B, c->D, 1, 0, bk))) return rc;
   KernelParams p;
   memset(&p, 0, sizeof(p));
@@ -617,6 +639,9 @@ int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_
   p.prob[1].fix_mat = own ? reinterpret_cast<const __nv_bfloat16*>(img) : nullptr;
   p.p1_wait_flag = o.dtxt_add_flag;
   p.p1_wait_value = o.dtxt_add_value;
+  // g_diag and both fix matrices hold this rank's B rows; the dtxt rows of the own chunk's hard negatives (B .. Bn) have
+  // no positive-pair term
+  p.fix_rows = c->B;
   if (o.sc_dt_prime != nullptr || o.sc_dbias != nullptr) {
     p.sc_saved = c->scalars + kSavedScalars;
     p.sc_dt_prime = o.sc_dt_prime;
@@ -701,7 +726,7 @@ void add_pull_job(siglip_ctx* c, AuxList& aux, int o, unsigned int s) {
   siglip::AuxJob& j = aux.add(siglip::kAuxCopy);
   j.src = reinterpret_cast<const uint4*>(c->peer_txt[o] + o * chunk_stride(c));
   j.dst = reinterpret_cast<uint4*>(c->txt_all + o * chunk_stride(c));
-  j.n16 = static_cast<unsigned long long>(c->Bs[o]) * c->D * sizeof(__nv_bfloat16) / 16;
+  j.n16 = static_cast<unsigned long long>(c->Ts[o]) * c->D * sizeof(__nv_bfloat16) / 16;
   j.wait_flags = c->flags + 0 * kMaxWorld + o;
   j.wait_n = 1;
   j.wait_value = s;
@@ -763,7 +788,7 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
   if (W > 1) {
     // peers must have finished pulling my text slot in their previous forward before I overwrite it
     if ((rc = wait_peers(c, 2, s - 1, st))) return rc;
-    CK(cudaMemcpyAsync(c->txt_all + r * stride, txt, static_cast<size_t>(c->B) * c->D * sizeof(__nv_bfloat16),
+    CK(cudaMemcpyAsync(c->txt_all + r * stride, txt, static_cast<size_t>(c->T) * c->D * sizeof(__nv_bfloat16),
                        cudaMemcpyDeviceToDevice, st));
     if ((rc = copy_own_ids(c, st))) return rc;   // before the signal, which covers it
     if ((rc = signal_peers(c, 0, s, st))) return rc;
@@ -779,7 +804,7 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
     const __nv_bfloat16* txt_c = (k == 0) ? own_txt : c->txt_all + cidx * stride;
     if (save && (rc = ensure_g(c, k))) return rc;
     AuxList aux;
-    if (save) add_cvt_jobs(c, aux, k, k == 0, img, txt_c, c->Bs[cidx]);
+    if (save) add_cvt_jobs(c, aux, k, k == 0, img, txt_c, c->Ts[cidx]);
     if (k + 1 < W) {
       const int nxt = step_owner(c, r, k + 1);
       if (c->overlap_pull) {
@@ -788,13 +813,13 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
         // un-overlapped variant (A/B measurements): wait + copy as separate stream operations
         if ((rc = wait_one(c, 0, nxt, s, st))) return rc;
         CK(cudaMemcpyAsync(c->txt_all + nxt * stride, c->peer_txt[nxt] + nxt * stride,
-                           static_cast<size_t>(c->Bs[nxt]) * c->D * sizeof(__nv_bfloat16), cudaMemcpyDefault, st));
+                           static_cast<size_t>(c->Ts[nxt]) * c->D * sizeof(__nv_bfloat16), cudaMemcpyDefault, st));
         if (c->sample_ids)
           CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(nxt) * c->ids_stride, peer_ids(c, nxt),
                              ids_bytes(c, nxt), cudaMemcpyDefault, st));
       }
     }
-    if ((rc = run_loss_chunk(c, k, cidx, k == 0, k == 0, img, txt_c, c->Bs[cidx], chunk_ids(c, cidx), t_prime, bias, save,
+    if ((rc = run_loss_chunk(c, k, cidx, k == 0, k == 0, img, txt_c, c->Ts[cidx], chunk_ids(c, cidx), t_prime, bias, save,
                              aux, (k == W - 1) ? &fin : nullptr, EndSignal(), st)))
       return rc;
   }
@@ -857,7 +882,7 @@ int backward_impl(siglip_ctx* c, const void* img, const void* txt, const float* 
       f.src = reinterpret_cast<const uint4*>(c->peer_slots[pr] + r * stride);
       f.src2 = (j == 2) ? nullptr : reinterpret_cast<const uint4*>(c->dtxt_acc);
       f.dst = reinterpret_cast<uint4*>(c->dtxt_acc);
-      f.n16 = static_cast<unsigned long long>(c->B) * c->D * sizeof(float) / 16;
+      f.n16 = static_cast<unsigned long long>(c->T) * c->D * sizeof(float) / 16;
       f.wait_flags = c->flags + 1 * kMaxWorld + pr;
       f.wait_n = 1;
       f.wait_value = base + static_cast<unsigned int>(j - 1);
@@ -868,7 +893,7 @@ int backward_impl(siglip_ctx* c, const void* img, const void* txt, const float* 
     const bool scalars_here = last && !(W > 1 && c->sync_scalar_grads);
     o.sc_dt_prime = scalars_here ? dt_prime : nullptr;
     o.sc_dbias = scalars_here ? dbias : nullptr;
-    if ((rc = run_grad_chunk(c, k, k == 0, img, own_txt, c->Bs[cidx], t_prime, grad_out, o, aux, EndSignal(), st)))
+    if ((rc = run_grad_chunk(c, k, k == 0, img, own_txt, c->Ts[cidx], t_prime, grad_out, o, aux, EndSignal(), st)))
       return rc;
     if (W > 1 && (!last || !c->overlap_reduce)) {
       if ((rc = signal_peers(c, 1, base + static_cast<unsigned int>(j), st))) return rc;
@@ -877,11 +902,11 @@ int backward_impl(siglip_ctx* c, const void* img, const void* txt, const float* 
   if (W > 1) {
     if (c->overlap_reduce) {
       // dtxt = (sum of the W-1 remote contributions, already local) + my own contribution: a local add
-      CKI(siglip::launch_reduce_slots(dtxt, c->grad_bf16, c->final_ptrs_dev, 2, static_cast<size_t>(c->B) * c->D,
+      CKI(siglip::launch_reduce_slots(dtxt, c->grad_bf16, c->final_ptrs_dev, 2, static_cast<size_t>(c->T) * c->D,
                                       c->num_sms, st));
     } else {
       if ((rc = wait_peers(c, 1, base + static_cast<unsigned int>(W), st))) return rc;
-      CKI(siglip::launch_reduce_slots(dtxt, c->grad_bf16, c->reduce_ptrs_dev, W, static_cast<size_t>(c->B) * c->D,
+      CKI(siglip::launch_reduce_slots(dtxt, c->grad_bf16, c->reduce_ptrs_dev, W, static_cast<size_t>(c->T) * c->D,
                                       c->num_sms, st));
     }
     c->launches++;
@@ -933,7 +958,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   if ((rc = ensure_g(c, 0))) return rc;
   if (W > 1 && (rc = ensure_g(c, 1))) return rc;
   const __nv_bfloat16* own_txt = reinterpret_cast<const __nv_bfloat16*>(txt);
-  const size_t own_bytes = static_cast<size_t>(c->B) * c->D * sizeof(__nv_bfloat16);
+  const size_t own_bytes = static_cast<size_t>(c->T) * c->D * sizeof(__nv_bfloat16);
   FinJob fin;
   fin.loss = loss;
   fin.dt_prime = c->scalars + kSavedScalars;
@@ -967,7 +992,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
         if ((rc = signal_peers(c, 0, s, st))) return rc;
       }
     }
-    add_cvt_jobs(c, aux, 0, true, img, own_txt, c->B);
+    add_cvt_jobs(c, aux, 0, true, img, own_txt, c->T);
     if (W > 1) {
       if (ik) {
         // my contribution slots of the previous backward must have been read by their owners (flag 3) before G1
@@ -983,7 +1008,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       c->prewait3 = n - 1;
       add_pull_job(c, aux, step_owner(c, r, 1), s);
     }
-    if ((rc = run_loss_chunk(c, 0, r, true, true, img, own_txt, c->B, chunk_ids(c, r), t_prime, bias, true, aux,
+    if ((rc = run_loss_chunk(c, 0, r, true, true, img, own_txt, c->T, chunk_ids(c, r), t_prime, bias, true, aux,
                              (W == 1) ? &fin : nullptr, EndSignal(), st)))
       return rc;
   }
@@ -994,11 +1019,11 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
     const __nv_bfloat16* txt_c = c->txt_all + cidx * stride;
     {
       AuxList aux;
-      add_cvt_jobs(c, aux, 1, false, img, txt_c, c->Bs[cidx]);
+      add_cvt_jobs(c, aux, 1, false, img, txt_c, c->Ts[cidx]);
       if (k + 1 < W) add_pull_job(c, aux, step_owner(c, r, k + 1), s);
       const bool lastL = (k == W - 1);
       EndSignal end = (lastL && ik) ? end_signal(c, 2, s) : EndSignal();   // "I have pulled everyone's text"
-      if ((rc = run_loss_chunk(c, 1, cidx, false, false, img, txt_c, c->Bs[cidx], chunk_ids(c, cidx), t_prime, bias, true,
+      if ((rc = run_loss_chunk(c, 1, cidx, false, false, img, txt_c, c->Ts[cidx], chunk_ids(c, cidx), t_prime, bias, true,
                                aux, lastL ? &fin : nullptr, end, st)))
         return rc;
       if (lastL && !ik && (rc = signal_peers(c, 2, s, st))) return rc;
@@ -1015,14 +1040,14 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       f.src = reinterpret_cast<const uint4*>(c->peer_slots[pr] + r * stride);
       f.src2 = (j == 2) ? nullptr : reinterpret_cast<const uint4*>(c->dtxt_acc);
       f.dst = reinterpret_cast<uint4*>(c->dtxt_acc);
-      f.n16 = static_cast<unsigned long long>(c->B) * c->D * sizeof(float) / 16;
+      f.n16 = static_cast<unsigned long long>(c->T) * c->D * sizeof(float) / 16;
       f.wait_flags = c->flags + 1 * kMaxWorld + pr;
       f.wait_n = 1;
       f.wait_value = base + static_cast<unsigned int>(j - 1);
       f.site = 7;
     }
     EndSignal end = ik ? end_signal(c, 1, base + static_cast<unsigned int>(j)) : EndSignal();
-    if ((rc = run_grad_chunk(c, 1, false, img, own_txt, c->Bs[cidx], t_prime, grad_out, o, aux, end, st))) return rc;
+    if ((rc = run_grad_chunk(c, 1, false, img, own_txt, c->Ts[cidx], t_prime, grad_out, o, aux, end, st))) return rc;
     if (!ik && (rc = signal_peers(c, 1, base + static_cast<unsigned int>(j), st))) return rc;
   }
   // ---- G0: own chunk, gradient slot W. Folds the last remote contribution and adds the folded sum in its epilogue ----
@@ -1040,7 +1065,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       f.src = reinterpret_cast<const uint4*>(c->peer_slots[pr] + r * stride);
       f.src2 = (W == 2) ? nullptr : reinterpret_cast<const uint4*>(c->dtxt_acc);
       f.dst = reinterpret_cast<uint4*>(c->dtxt_acc);
-      f.n16 = static_cast<unsigned long long>(c->B) * c->D * sizeof(float) / 16;
+      f.n16 = static_cast<unsigned long long>(c->T) * c->D * sizeof(float) / 16;
       f.wait_flags = c->flags + 1 * kMaxWorld + pr;
       f.wait_n = 1;
       f.wait_value = base + static_cast<unsigned int>(W - 1);
@@ -1055,7 +1080,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
     o.sc_dt_prime = scalars_here ? dt_prime : nullptr;
     o.sc_dbias = scalars_here ? dbias : nullptr;
     EndSignal end = (W > 1 && ik) ? end_signal(c, 3, n) : EndSignal();   // "I have read everyone's contributions"
-    if ((rc = run_grad_chunk(c, 0, true, img, own_txt, c->B, t_prime, grad_out, o, aux, end, st))) return rc;
+    if ((rc = run_grad_chunk(c, 0, true, img, own_txt, c->T, t_prime, grad_out, o, aux, end, st))) return rc;
     if (W > 1 && !ik && (rc = signal_peers(c, 3, n, st))) return rc;
   }
   if ((rc = finalize_metrics(c, s, st))) return rc;
@@ -1094,15 +1119,20 @@ int siglip_device_count(void) {
   return ok;
 }
 
-static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, const int* Bs, int D) {
+// Bs[p]: rank p's images; Ts[p] >= Bs[p]: its texts (paired ones first, then its hard negatives). Every argument is
+// checked before the first CUDA call.
+static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, const int* Bs, const int* Ts, int D) {
   if (out == nullptr) return fail(SIGLIP_ERR_INVALID, "out is null");
   *out = nullptr;
   if (world < 1 || world > kMaxWorld || rank < 0 || rank >= world)
     return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
-  int Bmax = 0;
+  int Bmax = 0, Tmax = 0;
   for (int p = 0; p < world; ++p) {
     if (Bs[p] < 1) return fail(SIGLIP_ERR_INVALID, "need B >= 1 on every rank");
+    if (Ts[p] < Bs[p])
+      return fail(SIGLIP_ERR_INVALID, "need texts_per_rank[p] >= images_per_rank[p] (paired texts, then hard negatives)");
     Bmax = Bs[p] > Bmax ? Bs[p] : Bmax;
+    Tmax = Ts[p] > Tmax ? Ts[p] : Tmax;
   }
   if (D < 8 || (D % 8) != 0) return fail(SIGLIP_ERR_INVALID, "need D a positive multiple of 8");
   int ndev = 0;
@@ -1126,12 +1156,22 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   c->device = device;
   c->rank = rank;
   c->world = world;
-  for (int p = 0; p < world; ++p) c->Bs[p] = Bs[p];
+  for (int p = 0; p < world; ++p) {
+    c->Bs[p] = Bs[p];
+    c->Ts[p] = Ts[p];
+    c->extras = c->extras || Ts[p] != Bs[p];
+  }
   c->B = Bs[rank];
+  c->T = Ts[rank];
   c->Bmax = Bmax;
+  c->Tmax = Tmax;
   c->D = D;
   c->Bp = round_up(Bmax, 256);
-  for (int p = 0; p < world; ++p) c->off[p + 1] = c->off[p] + Bs[p];
+  c->Tp = round_up(Tmax, 256);
+  for (int p = 0; p < world; ++p) {
+    c->off[p + 1] = c->off[p] + Bs[p];
+    c->toff[p + 1] = c->toff[p] + Ts[p];
+  }
   c->dbg_no_gstore = getenv("SIGLIP_DEBUG_NO_GSTORE") != nullptr;
   c->dbg_no_cvt = getenv("SIGLIP_DEBUG_NO_CVT") != nullptr;
   c->dbg_loss_waitstats = getenv("SIGLIP_DEBUG_LOSS_WAITSTATS") != nullptr;
@@ -1174,7 +1214,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     c->mkeys[1] = c->mkeys[0] + mkeys_block(c);
     CK(alloc(reinterpret_cast<void**>(&c->slots), stride * world * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dimg_acc), static_cast<size_t>(c->B) * D * sizeof(float)));
-    CK(alloc(reinterpret_cast<void**>(&c->dtxt_acc), static_cast<size_t>(c->B) * D * sizeof(float)));
+    CK(alloc(reinterpret_cast<void**>(&c->dtxt_acc), static_cast<size_t>(c->T) * D * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->reduce_ptrs_dev), world * sizeof(float*)));
     CK(alloc(reinterpret_cast<void**>(&c->final_ptrs_dev), 2 * sizeof(float*)));
     CK(alloc(reinterpret_cast<void**>(&c->signal_ptrs_dev), kFlagKinds * world * sizeof(unsigned int*)));
@@ -1202,13 +1242,21 @@ int siglip_ctx_create(siglip_ctx** out, int device, int rank, int world, int B, 
   if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
   int Bs[kMaxWorld];
   for (int p = 0; p < world; ++p) Bs[p] = B;
-  return ctx_create_impl(out, device, rank, world, Bs, D);
+  return ctx_create_impl(out, device, rank, world, Bs, Bs, D);
 }
 
 int siglip_ctx_create_uneven(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank, int D) {
   if (batch_per_rank == nullptr) return fail(SIGLIP_ERR_INVALID, "batch_per_rank is null");
   if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
-  return ctx_create_impl(out, device, rank, world, batch_per_rank, D);
+  return ctx_create_impl(out, device, rank, world, batch_per_rank, batch_per_rank, D);
+}
+
+int siglip_ctx_create_texts(siglip_ctx** out, int device, int rank, int world, const int* images_per_rank,
+                            const int* texts_per_rank, int D) {
+  if (images_per_rank == nullptr || texts_per_rank == nullptr)
+    return fail(SIGLIP_ERR_INVALID, "images_per_rank / texts_per_rank is null");
+  if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
+  return ctx_create_impl(out, device, rank, world, images_per_rank, texts_per_rank, D);
 }
 
 int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
@@ -1315,6 +1363,8 @@ int siglip_ctx_export_handles(siglip_ctx* c, void* out_bytes, size_t capacity) {
   b.B = c->B;
   b.D = c->D;
   b.Bmax = c->Bmax;
+  b.T = c->T;
+  b.Tmax = c->Tmax;
   if (gethostname(b.host, sizeof(b.host) - 1) != 0) b.host[0] = 0;
   memcpy(out_bytes, &b, sizeof(b));
   return 0;
@@ -1345,7 +1395,7 @@ static int publish_peer_tables(siglip_ctx* c) {
       const unsigned long long* blk =
           reinterpret_cast<const unsigned long long*>(reinterpret_cast<const char*>(c->peer_txt[p]) + mkeys_offset(c)) +
           q * mkeys_block(c);
-      mk[q * c->world + p] = blk + static_cast<size_t>(c->rank) * c->Bmax;
+      mk[q * c->world + p] = blk + static_cast<size_t>(c->rank) * c->Tmax;
       if (c->loopback && p != c->rank) mk[q * c->world + p] = c->loop_keys + static_cast<size_t>(p) * c->Bmax;
     }
   CK(cudaMemcpy(c->mkey_ptrs_dev, mk.data(), mk.size() * sizeof(unsigned long long*), cudaMemcpyHostToDevice));
@@ -1367,6 +1417,10 @@ int siglip_ctx_import_handles(siglip_ctx* c, const void* all_ranks_bytes, size_t
       return fail(SIGLIP_ERR_INVALID,
                   "peer context has a different batch / D than this rank was told: every rank must be created with the "
                   "same D and the same per-rank batch list (equal batches unless siglip_ctx_create_uneven)");
+    if (b.T != c->Ts[p] || b.Tmax != c->Tmax)
+      return fail(SIGLIP_ERR_INVALID,
+                  "peer context has a different text count than this rank was told: every rank must be created with the "
+                  "same texts_per_rank list (siglip_ctx_create_texts; batch + hard negatives per rank)");
     if (p == c->rank) continue;
     char me[64] = {0};
     if (gethostname(me, sizeof(me) - 1) != 0) me[0] = 0;
@@ -1525,6 +1579,10 @@ int siglip_host_submit_grads(siglip_ctx* c, const void* img_host, const void* tx
     return fail(SIGLIP_ERR_INVALID, "give both gradient host buffers or neither");
   if (c->sample_ids)
     return fail(SIGLIP_ERR_STATE, "the host-buffer entries take no sample ids: unavailable under SIGLIP_OPT_SAMPLE_IDS");
+  if (c->extras)
+    return fail(SIGLIP_ERR_STATE,
+                "the host-buffer entries stage [B, D] text: unavailable for a context with hard negatives "
+                "(siglip_ctx_create_texts with texts_per_rank != images_per_rank)");
   if (c->metrics_armed)
     return fail(SIGLIP_ERR_STATE, "the host-buffer entries return no retrieval metrics: siglip_request_metrics is armed");
   const bool with_grads = dimg_host_bf16 != nullptr;
@@ -1683,7 +1741,7 @@ int siglip_debug_set_text_chunk(siglip_ctx* c, int chunk, const void* txt_dev, v
   if (c == nullptr || txt_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
   CK(cudaMemcpyAsync(c->txt_all + chunk * chunk_stride(c), txt_dev,
-                     static_cast<size_t>(c->Bs[chunk]) * c->D * sizeof(__nv_bfloat16), cudaMemcpyDeviceToDevice,
+                     static_cast<size_t>(c->Ts[chunk]) * c->D * sizeof(__nv_bfloat16), cudaMemcpyDeviceToDevice,
                      static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
@@ -1700,7 +1758,7 @@ int siglip_debug_get_slot(siglip_ctx* c, int chunk, float* out_dev, void* cuda_s
   if (c == nullptr || out_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
   CK(cudaMemcpyAsync(out_dev, c->slots + chunk * chunk_stride(c),
-                     static_cast<size_t>(c->Bs[chunk]) * c->D * sizeof(float), cudaMemcpyDeviceToDevice,
+                     static_cast<size_t>(c->Ts[chunk]) * c->D * sizeof(float), cudaMemcpyDeviceToDevice,
                      static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
@@ -1730,23 +1788,36 @@ int siglip_ctx_aux_trace(siglip_ctx* c, unsigned long long* out, int max_launche
 
 int siglip_normalize_fwd(siglip_ctx* c, const void* x, int in_bf16, void* xhat_bf16, float* inv_norm,
                          void* cuda_stream) {
+  if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  return siglip_normalize_fwd_rows(c, c->B, x, in_bf16, xhat_bf16, inv_norm, cuda_stream);
+}
+
+int siglip_normalize_fwd_rows(siglip_ctx* c, int rows, const void* x, int in_bf16, void* xhat_bf16, float* inv_norm,
+                              void* cuda_stream) {
   if (c == nullptr || x == nullptr || xhat_bf16 == nullptr || inv_norm == nullptr)
     return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (rows < 1) return fail(SIGLIP_ERR_INVALID, "rows must be >= 1");
   if ((reinterpret_cast<uintptr_t>(x) & 15u) || (reinterpret_cast<uintptr_t>(xhat_bf16) & 15u))
     return fail(SIGLIP_ERR_INVALID, "buffers must be 16-byte aligned");
   CK(cudaSetDevice(c->device));
-  CKI(siglip::launch_normalize_fwd(x, in_bf16, static_cast<__nv_bfloat16*>(xhat_bf16), inv_norm, c->B, c->D,
+  CKI(siglip::launch_normalize_fwd(x, in_bf16, static_cast<__nv_bfloat16*>(xhat_bf16), inv_norm, rows, c->D,
                                    c->input_f16 ? kXScale : 0.0f, c->num_sms, static_cast<cudaStream_t>(cuda_stream)));
   c->launches++;
   return 0;
 }
 
 int siglip_convert_f32(siglip_ctx* c, const float* x_f32, void* out_16bit, void* cuda_stream) {
+  if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  return siglip_convert_f32_rows(c, c->B, x_f32, out_16bit, cuda_stream);
+}
+
+int siglip_convert_f32_rows(siglip_ctx* c, int rows, const float* x_f32, void* out_16bit, void* cuda_stream) {
   if (c == nullptr || x_f32 == nullptr || out_16bit == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (rows < 1) return fail(SIGLIP_ERR_INVALID, "rows must be >= 1");
   if ((reinterpret_cast<uintptr_t>(x_f32) & 15u) || (reinterpret_cast<uintptr_t>(out_16bit) & 15u))
     return fail(SIGLIP_ERR_INVALID, "buffers must be 16-byte aligned");
   CK(cudaSetDevice(c->device));
-  CKI(siglip::launch_convert_f32(x_f32, out_16bit, static_cast<size_t>(c->B) * c->D, c->input_f16 ? kXScale : 0.0f,
+  CKI(siglip::launch_convert_f32(x_f32, out_16bit, static_cast<size_t>(rows) * c->D, c->input_f16 ? kXScale : 0.0f,
                                  c->num_sms, static_cast<cudaStream_t>(cuda_stream)));
   c->launches++;
   return 0;
@@ -1754,13 +1825,20 @@ int siglip_convert_f32(siglip_ctx* c, const float* x_f32, void* out_16bit, void*
 
 int siglip_normalize_bwd(siglip_ctx* c, const void* x, int in_bf16, const float* inv_norm, const void* dxhat,
                          int grad_bf16, void* dx, void* cuda_stream) {
+  if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  return siglip_normalize_bwd_rows(c, c->B, x, in_bf16, inv_norm, dxhat, grad_bf16, dx, cuda_stream);
+}
+
+int siglip_normalize_bwd_rows(siglip_ctx* c, int rows, const void* x, int in_bf16, const float* inv_norm,
+                              const void* dxhat, int grad_bf16, void* dx, void* cuda_stream) {
   if (c == nullptr || x == nullptr || inv_norm == nullptr || dxhat == nullptr || dx == nullptr)
     return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (rows < 1) return fail(SIGLIP_ERR_INVALID, "rows must be >= 1");
   if ((reinterpret_cast<uintptr_t>(x) & 15u) || (reinterpret_cast<uintptr_t>(dxhat) & 15u) ||
       (reinterpret_cast<uintptr_t>(dx) & 15u))
     return fail(SIGLIP_ERR_INVALID, "buffers must be 16-byte aligned");
   CK(cudaSetDevice(c->device));
-  CKI(siglip::launch_normalize_bwd(x, in_bf16, inv_norm, dxhat, grad_bf16, dx, c->B, c->D, c->num_sms,
+  CKI(siglip::launch_normalize_bwd(x, in_bf16, inv_norm, dxhat, grad_bf16, dx, rows, c->D, c->num_sms,
                                    static_cast<cudaStream_t>(cuda_stream)));
   c->launches++;
   return 0;

@@ -437,14 +437,17 @@ __device__ __forceinline__ void tile_metrics(const float (&acc)[64], int row_lo,
 // into the accumulator registers: a non-wgmma write to them makes ptxas serialise every wgmma of the kernel.)
 // All global loads of a group of four column pairs are issued before its stores: the stores may alias the loads as far
 // as the compiler knows, and a load -> store -> load chain exposes one L2 round trip per pair.
+// fix_rows: rows of fix_mat; a row at or past it has no positive-pair term and reads nothing there (with hard negatives
+// the dtxt problem's M = T exceeds the B rows of its fix_mat, the caller's image buffer).
 __device__ __forceinline__ void out_row(const float (&acc)[64], int h, float scale, int row, int col0, int c_lo,
-                                       const Problem& pr, float fix, const float4* parts = nullptr, int nparts = 0,
-                                       size_t part_stride = 0) {
+                                       const Problem& pr, float fix, int fix_rows, const float4* parts = nullptr,
+                                       int nparts = 0, size_t part_stride = 0) {
   if (row >= pr.M) return;
   const float as = pr.acc_scale;   // undoes the power-of-two scaling of the fp16 operands (1 for bf16)
   const float xs = (pr.fix_mat_scale != 0.f) ? pr.fix_mat_scale : 1.0f;
   const float fixs = fix * xs;
-  const __nv_bfloat16* xrow = pr.fix_mat ? pr.fix_mat + static_cast<long long>(row) * pr.ldx : nullptr;
+  const __nv_bfloat16* xrow =
+      (pr.fix_mat != nullptr && row < fix_rows) ? pr.fix_mat + static_cast<long long>(row) * pr.ldx : nullptr;
   const float* arow = pr.add_src ? pr.add_src + static_cast<long long>(row) * pr.ld_add : nullptr;
 #pragma unroll
   for (int jb = 0; jb < 4; ++jb) {
@@ -860,7 +863,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
 #pragma unroll
               for (int e1 = 0; e1 < 2; ++e1) {
                 const int col = col0 + 8 * j + c_lo + e1;
-                if (col < pr.N) {
+                if (col < p.col_pos_n) {   // paired texts only: a hard negative has no id and is never positive
                   const int64_t cid = p.col_ids[col];
                   pos |= static_cast<uint32_t>(cid == rid0) << (4 * j + e1);
                   pos |= static_cast<uint32_t>(cid == rid1) << (4 * j + 2 + e1);
@@ -890,8 +893,10 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
         kahan_add(s_gs, c_gs, acc_gs);
       } else {
         const float scale = t_exact * p.inv_b * (p.grad_out != nullptr ? *p.grad_out : 1.0f);
-        const float fix0 = (pr.fix_vec != nullptr && row_lo < pr.M) ? pr.fix_vec[row_lo] : 0.f;
-        const float fix1 = (pr.fix_vec != nullptr && row_lo + 8 < pr.M) ? pr.fix_vec[row_lo + 8] : 0.f;
+        // the positive-pair term exists for the first fix_rows rows only (the dtxt problem of an own chunk with hard
+        // negatives has M = T rows, but fix_vec / fix_mat hold this rank's B)
+        const float fix0 = (pr.fix_vec != nullptr && row_lo < p.fix_rows) ? pr.fix_vec[row_lo] : 0.f;
+        const float fix1 = (pr.fix_vec != nullptr && row_lo + 8 < p.fix_rows) ? pr.fix_vec[row_lo + 8] : 0.f;
         if (tc.prob == 1 && p.p1_wait_flag != nullptr && !p1_ready) {
           // the dtxt tiles of the LAST gradient launch add the folded sum of the peers' contributions: the fold that
           // completes it runs in this very launch (auxiliary warps of all CTAs) and must have finished everywhere
@@ -924,11 +929,11 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
           p1_ready = true;
         }
         if constexpr (kF8) {   // whole tiles only: split-K is never requested for 8-bit operands
-          out_row(acc8, 0, scale, row_lo, col_base, c_lo, pr, fix0);
-          out_row(acc8, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1);
+          out_row(acc8, 0, scale, row_lo, col_base, c_lo, pr, fix0, p.fix_rows);
+          out_row(acc8, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1, p.fix_rows);
         } else if (tc.part < 0) {
-          out_row(acc, 0, scale, row_lo, col_base, c_lo, pr, fix0);
-          out_row(acc, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1);
+          out_row(acc, 0, scale, row_lo, col_base, c_lo, pr, fix0, p.fix_rows);
+          out_row(acc, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1, p.fix_rows);
         } else {
           // split tile: this CTA's 128 x 128 fp32 partial in fragment order, thread-contiguous float4's
           const size_t kPartF4 = static_cast<size_t>(kBlockM) * kTileN / 4;
@@ -975,8 +980,8 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
               }
             }
             __syncwarp();
-            out_row(acc, 0, scale, row_lo, col_base, c_lo, pr, fix0, ws, p.sk_parts - 1, part_stride);
-            out_row(acc, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1, ws, p.sk_parts - 1, part_stride);
+            out_row(acc, 0, scale, row_lo, col_base, c_lo, pr, fix0, p.fix_rows, ws, p.sk_parts - 1, part_stride);
+            out_row(acc, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1, p.fix_rows, ws, p.sk_parts - 1, part_stride);
             // every owner warp has consumed the partials: the last one re-arms the counters for the next launch
             __syncwarp();
             if (lane == 0) {
@@ -1358,17 +1363,32 @@ __global__ void allreduce_scalars_kernel(const float* __restrict__ saved, const 
 // retrieval metrics").
 constexpr int kMetricsThreads = 1024;
 
-__device__ __forceinline__ int metrics_owner(const MetricsArgs& a, int g) {
+// owner rank of global index g under the prefix sums `off` (images: a.off, texts: a.toff)
+__device__ __forceinline__ int metrics_owner(const MetricsArgs& a, const int* off, int g) {
   int o = 0;
-  while (o + 1 < a.world && g >= a.off[o + 1]) ++o;
+  while (o + 1 < a.world && g >= off[o + 1]) ++o;
   return o;
 }
 
-// sample id of global sample g (image and text of one sample share it)
-__device__ __forceinline__ int64_t metrics_id(const MetricsArgs& a, int g) {
-  const int o = metrics_owner(a, g);
-  const int l = g - a.off[o];
+// sample id of the l-th sample of rank o (its image and its paired text share it)
+__device__ __forceinline__ int64_t metrics_id(const MetricsArgs& a, int o, int l) {
   return (o == a.rank) ? a.ids_own[l] : a.ids_all[static_cast<size_t>(o) * a.ids_stride + l];
+}
+
+// Is global text j a hit for my image i? The positional pair, or with ids a PAIRED text with the same id: a hard negative
+// (local text index >= its rank's batch) never is, so a hard negative that outranks the caption counts as a miss.
+__device__ __forceinline__ bool metrics_i2t_hit(const MetricsArgs& a, int i, int j) {
+  if (a.ids_own == nullptr) return j == a.toff[a.rank] + i;
+  const int o = metrics_owner(a, a.toff, j);
+  const int l = j - a.toff[o];
+  return l < a.off[o + 1] - a.off[o] && metrics_id(a, o, l) == a.ids_own[i];
+}
+
+// Is global image g a hit for my (paired) text i?
+__device__ __forceinline__ bool metrics_t2i_hit(const MetricsArgs& a, int i, int g) {
+  if (a.ids_own == nullptr) return g == a.off[a.rank] + i;
+  const int o = metrics_owner(a, a.off, g);
+  return metrics_id(a, o, g - a.off[o]) == a.ids_own[i];
 }
 
 __device__ __forceinline__ int key_index(unsigned long long k) {
@@ -1408,13 +1428,12 @@ __global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const
     }
   }
   __syncthreads();
-  const int me0 = a.off[a.rank];
-  const bool ids = a.ids_own != nullptr;
   unsigned int h_i2t = 0, h_t2i = 0;
+  // column partials are kept for the paired texts only (i < B); the extras' column keys are computed but never read
   for (int i = tid; i < a.B; i += kMetricsThreads) {
-    const int j = key_index(a.row_keys[i]);   // best text of my image i
+    const int j = key_index(a.row_keys[i]);   // best text of my image i, over all texts including the extras
     if (a.i2t) a.i2t[i] = j;
-    if (j >= 0) h_i2t += ids ? (metrics_id(a, j) == a.ids_own[i]) : (j == me0 + i);
+    if (j >= 0) h_i2t += metrics_i2t_hit(a, i, j);
     unsigned long long k = a.col_own[i];
     if (a.world > 1) {
       for (int q = 0; q < a.world; ++q) {
@@ -1426,7 +1445,7 @@ __global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const
     }
     const int g = key_index(k);               // best image of my text i
     if (a.t2i) a.t2i[i] = g;
-    if (g >= 0) h_t2i += ids ? (metrics_id(a, g) == a.ids_own[i]) : (g == me0 + i);
+    if (g >= 0) h_t2i += metrics_t2i_hit(a, i, g);
   }
   // integer counts: the sum does not depend on the order
   for (int o = 16; o > 0; o >>= 1) {
@@ -1637,7 +1656,12 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
       }
     }
   }
-  if (clusters > total_tiles) clusters = total_tiles;
+  // a loss launch keeps the grid of the largest chunk of its forward (KernelParams::grid_n): CTA i owns partial slot i
+  // in every chunk, and the CTAs without a tile only carry their slot forward
+  int grid_tiles = total_tiles;
+  if (kMode == kModeLoss && pl.grid_n > pl.prob[0].N)
+    grid_tiles = pl.prob[0].tiles_m * ((pl.grid_n + kTileN - 1) / kTileN);
+  if (clusters > grid_tiles) clusters = grid_tiles;
   if (clusters < 1) clusters = 1;
   cfg.gridDim = dim3(clusters * kCS);
   cfg.numAttrs = pl.pdl ? 2 : 1;

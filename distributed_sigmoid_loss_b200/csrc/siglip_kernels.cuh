@@ -131,6 +131,14 @@ struct KernelParams {
   unsigned long long* col_keys;  // [N]: best image (global index) of each text of the chunk, over this rank's images
   int row_off;                   // global index of this rank's first image
   int col_off;                   // global index of the chunk's first text
+  // Hard-negative captions (siglip_ctx_create_texts): a text chunk is [paired texts; extras]. Appended last like the
+  // metrics fields, so that the default loss kernel's parameter offsets do not move.
+  int col_pos_n;   // loss kernel, kIds: paired columns of the chunk (col_ids has this many entries; extras never match)
+  int fix_rows;    // out kernel: rows of fix_vec / fix_mat (this rank's batch); rows >= fix_rows take no fix term
+  // Host only (launch_gemm): size the grid of a loss launch as if its chunk had grid_n columns. Every loss kernel of a
+  // forward then has the same grid, so the per-CTA partial slots it accumulates and the last one sums line up when the
+  // chunks have different sizes (uneven batches, hard negatives). 0 = the chunk's own N.
+  int grid_n;
 };
 
 enum KernelMode { kModeLoss = 0, kModeOut = 1 };
@@ -192,7 +200,9 @@ struct MetricsArgs {
   const unsigned long long* col_own;           // [B] my partial of my chunk
   const unsigned long long* const* col_peers;  // [world] every rank's partial of my chunk (world > 1; own entry unused)
   int B, rank, world;
-  int off[kMetricsMaxWorld + 1];               // prefix sums of the per-rank batches
+  int off[kMetricsMaxWorld + 1];               // prefix sums of the per-rank batches (global image indices)
+  int toff[kMetricsMaxWorld + 1];              // prefix sums of the per-rank text counts (global text indices): rank
+                                               // p's texts toff[p] .. toff[p] + B_p - 1 are paired, the rest extras
   const int64_t* ids_own;                      // null = positional labels; else this rank's sample ids
   const int64_t* ids_all;                      // [world][ids_stride]: every chunk's ids, gathered in this step
   int ids_stride;

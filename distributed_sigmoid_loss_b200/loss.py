@@ -48,14 +48,28 @@ class SigmoidLossEngine:
 
     def __init__(self, batch: int, dim: int, device: torch.device, group=None, cta_group: int = 2,
                  overlap_pull: bool = True, rank_world: Optional[Tuple[int, int]] = None, loopback: bool = False,
-                 batch_per_rank=None):
+                 batch_per_rank=None, texts_per_rank=None):
         self._L = _capi.lib()
         if not torch.cuda.is_available() or self._L.siglip_device_count() == 0:
             raise RuntimeError("distributed_sigmoid_loss_b200 needs an sm_90 (H100) device; there is no CPU fallback")
         self.batch, self.dim, self.device, self.group = batch, dim, torch.device(device), group
         self.rank, self.world = rank_world if rank_world is not None else _group_rank_world(group)
         h = ctypes.c_void_p()
-        if batch_per_rank is not None:
+        if texts_per_rank is not None:
+            # hard-negative captions: rank p holds texts_per_rank[p] >= its batch texts, the paired ones first, then its
+            # extras (siglip_ctx_create_texts); every rank passes the same lists
+            bpr = [int(b) for b in batch_per_rank] if batch_per_rank is not None else [batch] * self.world
+            tpr = [int(t) for t in texts_per_rank]
+            if len(bpr) != self.world or bpr[self.rank] != batch or len(tpr) != self.world:
+                raise RuntimeError(f"batch_per_rank {bpr} / texts_per_rank {tpr} must list one entry per rank and hold "
+                                   f"batch {batch} at rank {self.rank}")
+            if any(t < b for t, b in zip(tpr, bpr)):
+                raise RuntimeError(f"texts_per_rank {tpr} must be >= batch_per_rank {bpr} on every rank")
+            _capi.check(self._L.siglip_ctx_create_texts(ctypes.byref(h), self.device.index or 0, self.rank, self.world,
+                                                        (ctypes.c_int * self.world)(*bpr),
+                                                        (ctypes.c_int * self.world)(*tpr), dim))
+            self.batch_per_rank, self.texts_per_rank = bpr, tpr
+        elif batch_per_rank is not None:
             # extension (SURVEY.md §8f-4): ranks with different batch sizes; every rank passes the same list
             bpr = [int(b) for b in batch_per_rank]
             if len(bpr) != self.world or bpr[self.rank] != batch:
@@ -68,6 +82,9 @@ class SigmoidLossEngine:
             _capi.check(self._L.siglip_ctx_create(ctypes.byref(h), self.device.index or 0, self.rank, self.world,
                                                   batch, dim))
             self.batch_per_rank = [batch] * self.world
+        if texts_per_rank is None:
+            self.texts_per_rank = list(self.batch_per_rank)
+        self.texts = self.texts_per_rank[self.rank]   # rows of txt / dtxt: the batch plus this rank's hard negatives
         self._h = h
         _capi.check(self._L.siglip_ctx_set_option(h, _capi.SIGLIP_OPT_CTA_GROUP, int(cta_group)))
         _capi.check(self._L.siglip_ctx_set_option(h, _capi.SIGLIP_OPT_OVERLAP_PULL, int(bool(overlap_pull))))
@@ -143,7 +160,7 @@ class SigmoidLossEngine:
         _capi.check(self._L.siglip_debug_set_peer_metric_keys(self._h, peer, keys.data_ptr(), self._stream()))
 
     def debug_get_slot(self, chunk: int) -> torch.Tensor:
-        out = torch.empty(self.batch_per_rank[chunk], self.dim, device=self.device, dtype=torch.float32)
+        out = torch.empty(self.texts_per_rank[chunk], self.dim, device=self.device, dtype=torch.float32)
         _capi.check(self._L.siglip_debug_get_slot(self._h, chunk, out.data_ptr(), self._stream()))
         return out
 
@@ -176,9 +193,10 @@ class SigmoidLossEngine:
                 grad_dtype: torch.dtype = torch.float32, grad_out: Optional[torch.Tensor] = None):
         """The fused step (siglip_fwd_bwd): loss and gradient kernels alternate chunk by chunk, two sigma operands
         whatever the world size. img/txt: [B, D] bf16 contiguous on self.device; t_prime/bias: fp32 [1]. Returns
-        (loss[1], dimg[B,D], dtxt[B,D], dt_prime[1], dbias[1]) for an upstream gradient of 1 (or `grad_out`, a
+        (loss[1], dimg[B,D], dtxt[T,D], dt_prime[1], dbias[1]) for an upstream gradient of 1 (or `grad_out`, a
         1-element fp32 device tensor, multiplied in by the kernel epilogues); scalars are fp32, dimg/dtxt are
-        `grad_dtype` (fp32, or bf16 written directly by the kernel epilogue)."""
+        `grad_dtype` (fp32, or bf16 written directly by the kernel epilogue). txt is [T, D]: T = B plus this rank's hard
+        negatives (texts_per_rank)."""
         self._check(img, txt)
         self._set_grad_dtype(grad_dtype)
         opts = dict(device=self.device, dtype=torch.float32)
@@ -187,7 +205,7 @@ class SigmoidLossEngine:
         if self._set_tprime_f64(t_prime):
             dtp = torch.empty(1, device=self.device, dtype=torch.float64)
         dimg = torch.empty(self.batch, self.dim, device=self.device, dtype=grad_dtype)
-        dtxt = torch.empty(self.batch, self.dim, device=self.device, dtype=grad_dtype)
+        dtxt = torch.empty(self.texts, self.dim, device=self.device, dtype=grad_dtype)
         with torch.cuda.device(self.device):
             _capi.check(self._L.siglip_fwd_bwd_scaled(
                 self._h, img.data_ptr(), txt.data_ptr(), t_prime.data_ptr(), bias.data_ptr(),
@@ -224,7 +242,7 @@ class SigmoidLossEngine:
         if self._set_tprime_f64(t_prime):
             dtp = torch.empty(1, device=self.device, dtype=torch.float64)
         dimg = torch.empty(self.batch, self.dim, device=self.device, dtype=grad_dtype)
-        dtxt = torch.empty(self.batch, self.dim, device=self.device, dtype=grad_dtype)
+        dtxt = torch.empty(self.texts, self.dim, device=self.device, dtype=grad_dtype)
         with torch.cuda.device(self.device):
             _capi.check(self._L.siglip_backward(self._h, img.data_ptr(), txt.data_ptr(), t_prime.data_ptr(),
                                                 grad_out.data_ptr() if grad_out is not None else None,
@@ -240,27 +258,36 @@ class SigmoidLossEngine:
             _capi.check(self._L.siglip_ctx_set_option(self._h, _capi.SIGLIP_OPT_GRAD_BF16, int(want_bf16)))
             self._grad_bf16 = want_bf16
 
+    def _rows_ok(self, x: torch.Tensor) -> bool:
+        """[B, D] (images, paired texts) or [T, D] (texts with this rank's hard negatives)."""
+        return x.dim() == 2 and x.shape[0] in (self.batch, self.texts) and x.shape[1] == self.dim
+
     def normalize_fwd(self, x: torch.Tensor, f16: bool = False):
-        """F.normalize(x, dim=1) fused with the rounding to the kernels' operand format: returns (xhat [B, D] bf16, or
-        float16 holding 16*xhat with f16=True; inv_norm fp32 [B]). x: fp32 or bf16 [B, D] contiguous."""
-        if tuple(x.shape) != (self.batch, self.dim) or x.dtype not in (torch.float32, torch.bfloat16) or \
+        """F.normalize(x, dim=1) fused with the rounding to the kernels' operand format: returns (xhat [N, D] bf16, or
+        float16 holding 16*xhat with f16=True; inv_norm fp32 [N]). x: fp32 or bf16 [N, D] contiguous, N = B or T."""
+        if not self._rows_ok(x) or x.dtype not in (torch.float32, torch.bfloat16) or \
                 not x.is_contiguous() or x.device != self.device:
-            raise RuntimeError(f"normalize_fwd expects a contiguous fp32/bf16 [{self.batch}, {self.dim}] tensor on {self.device}")
+            raise RuntimeError(f"normalize_fwd expects a contiguous fp32/bf16 [{self.batch} or {self.texts}, {self.dim}] "
+                               f"tensor on {self.device}")
         self._set_input_f16(f16)
-        xhat = torch.empty(self.batch, self.dim, device=self.device, dtype=torch.float16 if f16 else torch.bfloat16)
-        inv = torch.empty(self.batch, device=self.device, dtype=torch.float32)
+        n = x.shape[0]
+        xhat = torch.empty(n, self.dim, device=self.device, dtype=torch.float16 if f16 else torch.bfloat16)
+        inv = torch.empty(n, device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.device):
-            _capi.check(self._L.siglip_normalize_fwd(self._h, x.data_ptr(), int(x.dtype == torch.bfloat16),
-                                                     xhat.data_ptr(), inv.data_ptr(), self._stream()))
+            _capi.check(self._L.siglip_normalize_fwd_rows(self._h, n, x.data_ptr(), int(x.dtype == torch.bfloat16),
+                                                          xhat.data_ptr(), inv.data_ptr(), self._stream()))
         return xhat, inv
 
     def normalize_bwd(self, x: torch.Tensor, inv: torch.Tensor, dxhat: torch.Tensor) -> torch.Tensor:
         """Backward of normalize_fwd: dx = inv * (dxhat - xhat <xhat, dxhat>), in x's dtype."""
+        if not self._rows_ok(x) or tuple(dxhat.shape) != tuple(x.shape) or tuple(inv.shape) != (x.shape[0],):
+            raise RuntimeError("normalize_bwd expects x / dxhat [N, D] and inv [N] with N = B or T")
         dx = torch.empty_like(x)
         with torch.cuda.device(self.device):
-            _capi.check(self._L.siglip_normalize_bwd(self._h, x.data_ptr(), int(x.dtype == torch.bfloat16),
-                                                     inv.data_ptr(), dxhat.data_ptr(),
-                                                     int(dxhat.dtype == torch.bfloat16), dx.data_ptr(), self._stream()))
+            _capi.check(self._L.siglip_normalize_bwd_rows(self._h, x.shape[0], x.data_ptr(),
+                                                          int(x.dtype == torch.bfloat16), inv.data_ptr(),
+                                                          dxhat.data_ptr(), int(dxhat.dtype == torch.bfloat16),
+                                                          dx.data_ptr(), self._stream()))
         return dx
 
     def scale(self, src: torch.Tensor, g: torch.Tensor) -> torch.Tensor:
@@ -334,13 +361,14 @@ class SigmoidLossEngine:
                 raise RuntimeError("the host entries expect contiguous CPU bf16 tensors of shape [B, D]")
 
     def _check(self, img: torch.Tensor, txt: torch.Tensor) -> None:
-        """Operands are [B, D] contiguous device tensors, both bf16 (default format) or both float16 holding 16*x
-        (the fp32-input format, see convert_f32); the context option follows the dtype."""
-        for x in (img, txt):
+        """Operands are contiguous device tensors, img [B, D] and txt [T, D] (T = B without hard negatives), both bf16
+        (default format) or both float16 holding 16*x (the fp32-input format, see convert_f32); the context option
+        follows the dtype."""
+        for x, n in ((img, self.batch), (txt, self.texts)):
             if x.device != self.device or x.dtype not in (torch.bfloat16, torch.float16) or not x.is_contiguous() or \
-                    tuple(x.shape) != (self.batch, self.dim):
+                    tuple(x.shape) != (n, self.dim):
                 raise RuntimeError(
-                    f"expected contiguous bf16 (or fp16 x16) [{self.batch}, {self.dim}] tensors on {self.device}, got "
+                    f"expected contiguous bf16 (or fp16 x16) [{n}, {self.dim}] tensors on {self.device}, got "
                     f"{tuple(x.shape)} {x.dtype} on {x.device}")
         if img.dtype != txt.dtype:
             raise RuntimeError("image and text operands must use the same 16-bit format")
@@ -365,13 +393,14 @@ class SigmoidLossEngine:
     def convert_f32(self, x: torch.Tensor, f16: bool) -> torch.Tensor:
         """The module's cast of fp32 embeddings to the kernels' operand format: bf16 (f16=False, == x.to(bfloat16)) or
         float16 holding 16*x (f16=True: 11 significant bits, what fp32 callers get)."""
-        if tuple(x.shape) != (self.batch, self.dim) or x.dtype != torch.float32 or not x.is_contiguous() or \
-                x.device != self.device:
-            raise RuntimeError(f"convert_f32 expects a contiguous fp32 [{self.batch}, {self.dim}] tensor on {self.device}")
+        if not self._rows_ok(x) or x.dtype != torch.float32 or not x.is_contiguous() or x.device != self.device:
+            raise RuntimeError(f"convert_f32 expects a contiguous fp32 [{self.batch} or {self.texts}, {self.dim}] tensor "
+                               f"on {self.device}")
         self._set_input_f16(f16)
-        out = torch.empty(self.batch, self.dim, device=self.device, dtype=torch.float16 if f16 else torch.bfloat16)
+        out = torch.empty(x.shape[0], self.dim, device=self.device, dtype=torch.float16 if f16 else torch.bfloat16)
         with torch.cuda.device(self.device):
-            _capi.check(self._L.siglip_convert_f32(self._h, x.data_ptr(), out.data_ptr(), self._stream()))
+            _capi.check(self._L.siglip_convert_f32_rows(self._h, x.shape[0], x.data_ptr(), out.data_ptr(),
+                                                        self._stream()))
         return out
 
     def close(self) -> None:
@@ -519,11 +548,12 @@ class _SigmoidLossFn(torch.autograd.Function):
 
 class _EngineCache:
     def __init__(self, group=None, cta_group: int = 2, overlap_pull: bool = True, sync_scalar_grads: bool = False,
-                 bidir: bool = False, batch_per_rank=None, multi_positive: bool = False):
+                 bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
         self.sync_scalar_grads, self.bidir = sync_scalar_grads, bidir
         self.multi_positive = multi_positive
         self.batch_per_rank = batch_per_rank
+        self.hard_negatives = hard_negatives
         self._engines: Dict[Tuple[int, int, int], SigmoidLossEngine] = {}
 
     def get(self, batch: int, dim: int, device: torch.device) -> SigmoidLossEngine:
@@ -531,8 +561,14 @@ class _EngineCache:
         eng = self._engines.get(key)
         if eng is None:
             dev = torch.device("cuda", key[0])
+            tpr = None
+            if self.hard_negatives:
+                # every rank scores the same number K of extras: T_p = B_p + K
+                rank, world = _group_rank_world(self.group)
+                bpr = self.batch_per_rank if self.batch_per_rank is not None else [batch] * world
+                tpr = [int(b) + self.hard_negatives for b in bpr]
             eng = SigmoidLossEngine(batch, dim, dev, self.group, self.cta_group, self.overlap_pull,
-                                    batch_per_rank=self.batch_per_rank)
+                                    batch_per_rank=self.batch_per_rank, texts_per_rank=tpr)
             if self.sync_scalar_grads:
                 eng.set_option(_capi.SIGLIP_OPT_SYNC_SCALAR_GRADS, 1)
             if self.bidir:
@@ -564,6 +600,39 @@ def _validate_ids(sample_ids, multi_positive: bool, embeddings: torch.Tensor) ->
     if sample_ids.device != embeddings.device:
         raise RuntimeError(f"sample_ids are on {sample_ids.device}, the embeddings on {embeddings.device}")
     return sample_ids.to(torch.int64).contiguous()
+
+
+def _validate_hard_negatives(hard_negatives) -> int:
+    if isinstance(hard_negatives, bool) or not isinstance(hard_negatives, int) or hard_negatives < 0:
+        raise RuntimeError(f"hard_negatives must be an int >= 0, got {hard_negatives!r}")
+    return hard_negatives
+
+
+def _validate_negatives(text_embeddings: torch.Tensor, negative_text, hard_negatives: int) -> None:
+    """negative_text of a forward: required ([K, D], the dtype / device / width of the texts) when the loss was built
+    with hard_negatives = K > 0, refused otherwise. Raises before any GPU work."""
+    if hard_negatives == 0:
+        if negative_text is not None:
+            raise RuntimeError("negative_text given, but the loss was built without hard_negatives (hard_negatives=K)")
+        return
+    if negative_text is None:
+        raise RuntimeError(f"hard_negatives={hard_negatives}: forward needs negative_text ([{hard_negatives}, emb_dim])")
+    if not isinstance(negative_text, torch.Tensor):
+        raise RuntimeError(f"negative_text must be a tensor, got {type(negative_text).__name__}")
+    want = (hard_negatives, text_embeddings.shape[1] if text_embeddings.dim() == 2 else None)
+    if negative_text.dim() != 2 or tuple(negative_text.shape) != want:
+        raise RuntimeError(f"negative_text must have shape [{want[0]}, {want[1]}] (hard_negatives x the texts' width), "
+                           f"got {tuple(negative_text.shape)}")
+    if negative_text.dtype != text_embeddings.dtype:
+        raise RuntimeError(f"negative_text is {negative_text.dtype}, the texts {text_embeddings.dtype}")
+    if negative_text.device != text_embeddings.device:
+        raise RuntimeError(f"negative_text is on {negative_text.device}, the texts on {text_embeddings.device}")
+
+
+def _with_negatives(text_embeddings: torch.Tensor, negative_text) -> torch.Tensor:
+    """[txt; negative_text] as one contiguous operand; torch.cat is differentiable, so negative_text.grad comes back
+    through autograd."""
+    return text_embeddings if negative_text is None else torch.cat([text_embeddings, negative_text])
 
 
 def _validate_return_metrics(return_metrics) -> None:
@@ -631,12 +700,20 @@ class DDPSigmoidLoss(nn.Module):
     match (``i2t_index``, ``t2i_index``, int64 [B]), computed by the loss kernels from the logits they already hold; a
     hit is the positional pair, or a pair with the same id under ``multi_positive``. Device tensors, no host
     synchronisation, not differentiable; loss and gradients are unchanged. Collective: every rank asks on the same steps.
+
+    ``hard_negatives=K > 0``: every ``forward`` takes ``negative_text`` ([K, D], the dtype, device and width of the texts):
+    K perturbed captions per rank that belong to no image (NegCLIP-style fine-tuning). They are scored as negatives
+    against every image of the global batch, never as positives (whatever the ids), and ``negative_text.grad`` is the
+    gradient of the sum over ranks of their losses. The loss still divides by the rank's image batch. ``i2t_index`` then
+    ranges over all texts including the extras (global index: prefix sums of B_p + K), and a winning extra is a miss.
+    Collective: every rank uses the same K.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
                  normalize_inputs: bool = False, sync_scalar_grads: bool = False, fused_step: Optional[bool] = None,
-                 batch_per_rank=None, multi_positive: bool = False) -> None:
+                 batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0) -> None:
         super().__init__()
+        hard_negatives = _validate_hard_negatives(hard_negatives)
         self.t_prime = nn.Parameter(torch.tensor(math.log(10), dtype=torch.float64))
         self.bias = nn.Parameter(torch.tensor(-10.0))
         self.gpu_batch_size = gpu_batch_size
@@ -652,17 +729,22 @@ class DDPSigmoidLoss(nn.Module):
         # extension (SURVEY.md §8f-4): per-rank batch sizes may differ; every rank passes the same list
         # extension: labels from per-sample ids (positive iff same id, across ranks too)
         self.multi_positive = multi_positive
+        # extension: hard-negative captions, K extra texts per rank scored against every image
+        self.hard_negatives = hard_negatives
         self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank,
-                                   multi_positive=multi_positive)
+                                   multi_positive=multi_positive, hard_negatives=hard_negatives)
 
     def engine_for(self, batch: int, dim: int, device: torch.device) -> SigmoidLossEngine:
         return self._cache.get(batch, (dim + 7) // 8 * 8, device)
 
     def forward(self, image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, *,
-                sample_ids: Optional[torch.Tensor] = None, return_metrics: bool = False):
+                negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
+                return_metrics: bool = False):
         _validate_return_metrics(return_metrics)
         ids = _validate_ids(sample_ids, self.multi_positive, image_embeddings)
+        _validate_negatives(text_embeddings, negative_text, self.hard_negatives)
         _validate(image_embeddings, text_embeddings, self.gpu_batch_size)
+        text_embeddings = _with_negatives(text_embeddings, negative_text)
         image_embeddings, text_embeddings = _pad_dim(image_embeddings), _pad_dim(text_embeddings)
         eng = self._cache.get(image_embeddings.shape[0], image_embeddings.shape[1], image_embeddings.device)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
@@ -682,24 +764,30 @@ class SigLipLoss(nn.Module):
     ...; the pairs covered and the result are the same. ``multi_positive=True``: labels from the ``sample_ids`` every
     forward then takes, as in ``DDPSigmoidLoss``. ``return_metrics=True``: returns ``(loss_or_dict, metrics)`` with the
     retrieval metrics of ``DDPSigmoidLoss``; they stay out of the ``output_dict``, whose values open_clip sums into the
-    total loss."""
+    total loss. ``hard_negatives=K``: every forward takes ``negative_text`` [K, D], as in ``DDPSigmoidLoss``."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
-                 multi_positive: bool = False):
+                 multi_positive: bool = False, hard_negatives: int = 0):
         super().__init__()
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
+        hard_negatives = _validate_hard_negatives(hard_negatives)
         self.cache_labels, self.rank, self.world_size, self.bidir = cache_labels, rank, world_size, bidir
         self.use_horovod = use_horovod
         self.fused_step = fused_step
         self.multi_positive = multi_positive
-        self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive)
+        self.hard_negatives = hard_negatives
+        self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive,
+                                   hard_negatives=hard_negatives)
 
     def forward(self, image_features, text_features, logit_scale, logit_bias, output_dict: bool = False, *,
-                sample_ids: Optional[torch.Tensor] = None, return_metrics: bool = False):
+                negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
+                return_metrics: bool = False):
         _validate_return_metrics(return_metrics)
         ids = _validate_ids(sample_ids, self.multi_positive, image_features)
+        _validate_negatives(text_features, negative_text, self.hard_negatives)
         _validate(image_features, text_features, None)
+        text_features = _with_negatives(text_features, negative_text)
         image_features, text_features = _pad_dim(image_features), _pad_dim(text_features)
         eng = self._cache.get(image_features.shape[0], image_features.shape[1], image_features.device)
         if (eng.rank, eng.world) != (self.rank, self.world_size):

@@ -9,8 +9,10 @@
  * caller's stream (pass torch.cuda.current_stream().cuda_stream); nothing here synchronises the host
  * except ctx create/destroy and handle import.
  *
- * Data layout: `img`, `txt` are row-major [B, D] bf16 device buffers, 16-byte aligned, D % 8 == 0.
- * `dimg`, `dtxt` are row-major [B, D] fp32 (or bf16 with SIGLIP_OPT_GRAD_BF16). Scalars are fp32 device scalars.
+ * Data layout: `img` is a row-major [B, D] bf16 device buffer, `txt` a row-major [T, D] one (T = B unless the context
+ * was created with siglip_ctx_create_texts: then this rank's T texts are its B paired captions followed by its hard
+ * negatives), 16-byte aligned, D % 8 == 0. `dimg` [B, D] and `dtxt` [T, D] are row-major fp32 (or bf16 with
+ * SIGLIP_OPT_GRAD_BF16). Scalars are fp32 device scalars.
  */
 #ifndef SIGLIP_B200_H_
 #define SIGLIP_B200_H_
@@ -131,6 +133,24 @@ int siglip_ctx_create(siglip_ctx** out, int device, int rank, int world, int B, 
  */
 int siglip_ctx_create_uneven(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank, int D);
 
+/*
+ * Same, with HARD-NEGATIVE captions (NegCLIP-style / compositionality fine-tuning: perturbed captions that belong to
+ * no image). Rank p holds images_per_rank[p] = B_p images and texts_per_rank[p] = T_p >= B_p texts: texts 0 .. B_p - 1
+ * are the captions of its images, texts B_p .. T_p - 1 its K_p = T_p - B_p hard negatives. The global text batch is the
+ * concatenation over ranks of [paired, extras] (global text index = prefix sum of T + local index). Rank r's loss is
+ *   (1/B_r) sum_i sum_{j over all sum(T) texts} softplus(-y_ij z_ij)
+ * with y = +1 for the positional pair (or, under SIGLIP_OPT_SAMPLE_IDS, a PAIRED text with the same id) and -1 for
+ * everything else: an extra is never positive, whatever the ids. txt / dtxt of every step are [T_r, D] (dtxt includes
+ * the extras' rows: the gradient of the sum over ranks of their losses); dt' / dbias include the extras' terms. Sample
+ * ids stay [B_r] (they describe the paired texts). The host-buffer entries are unavailable (SIGLIP_ERR_STATE).
+ * Workspaces: the text-shaped ones (gathered text, dtxt slots, fp16 text copies) hold max(T) rows per chunk and the
+ * sigma operands are [Bp, Tp] (max B, max T rounded up to 256). Time grows with T / B like the FLOPs (6 B T D).
+ * Every rank passes the same two lists; texts_per_rank == images_per_rank is exactly siglip_ctx_create_uneven.
+ * Invalid arguments return SIGLIP_ERR_INVALID before any device work.
+ */
+int siglip_ctx_create_texts(siglip_ctx** out, int device, int rank, int world, const int* images_per_rank,
+                            const int* texts_per_rank, int D);
+
 int siglip_ctx_set_option(siglip_ctx* ctx, int option, int value);
 
 /* Bytes of workspace the context holds on the device. */
@@ -183,6 +203,12 @@ int siglip_normalize_fwd(siglip_ctx* ctx, const void* x, int in_bf16, void* xhat
 int siglip_convert_f32(siglip_ctx* ctx, const float* x_f32, void* out_16bit, void* cuda_stream);
 int siglip_normalize_bwd(siglip_ctx* ctx, const void* x, int in_bf16, const float* inv_norm, const void* dxhat,
                          int grad_bf16, void* dx, void* cuda_stream);
+/* The three above for `rows` rows instead of B (rows >= 1): e.g. a [T, D] text tensor with hard negatives. */
+int siglip_normalize_fwd_rows(siglip_ctx* ctx, int rows, const void* x, int in_bf16, void* xhat_bf16, float* inv_norm,
+                              void* cuda_stream);
+int siglip_convert_f32_rows(siglip_ctx* ctx, int rows, const float* x_f32, void* out_16bit, void* cuda_stream);
+int siglip_normalize_bwd_rows(siglip_ctx* ctx, int rows, const void* x, int in_bf16, const float* inv_norm,
+                              const void* dxhat, int grad_bf16, void* dx, void* cuda_stream);
 
 /*
  * dst = src * (*g) elementwise over `nbytes` (any whole number of elements) of fp32 (is_bf16 = 0) or bf16 (is_bf16 = 1) data: the whole
@@ -223,8 +249,9 @@ int siglip_set_sample_ids(siglip_ctx* ctx, const int64_t* ids_dev, void* cuda_st
 /*
  * In-batch retrieval metrics of the NEXT siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd call (that step only),
  * computed from the logits the loss kernels already hold in registers, without a second similarity GEMM:
- *   i2t_index[i] = argmax_j s_ij over all sum(B) texts, for each of this rank's B images (global text index)
- *   t2i_index[j] = argmax_i s_ij over all sum(B) images, for each of this rank's B texts (global image index)
+ *   i2t_index[i] = argmax_j s_ij over all sum(T) texts, for each of this rank's B images (global text index; with hard
+ *                  negatives a winning extra is a miss)
+ *   t2i_index[j] = argmax_i s_ij over all sum(B) images, for each of this rank's B paired texts (global image index)
  *   top1[0] / top1[1] = fraction of this rank's images / texts whose top-1 is a positive: the positional diagonal, or
  *                       under SIGLIP_OPT_SAMPLE_IDS a pair with the same id, on any rank
  * Global indices follow the concatenated batch (prefix sums of the per-rank batches). Ties go to the lowest global index;
@@ -255,7 +282,8 @@ int siglip_fwd(siglip_ctx* ctx, const void* img, const void* txt, const float* t
  * results are on the host. At most two steps may be in flight: submit blocks on the step that used the same staging
  * set. The copies of step n+1 overlap the kernels of step n; every step still pays its own copies.
  * This is the end-to-end entry the benchmark times. Host buffers must stay valid until the step's wait returns.
- * These entries take no sample ids: under SIGLIP_OPT_SAMPLE_IDS they return SIGLIP_ERR_STATE.
+ * These entries take no sample ids: under SIGLIP_OPT_SAMPLE_IDS they return SIGLIP_ERR_STATE. They stage [B, D] text:
+ * on a context with hard negatives (siglip_ctx_create_texts, some T_p != B_p) they return SIGLIP_ERR_STATE.
  */
 int siglip_host_submit(siglip_ctx* ctx, const void* img_host, const void* txt_host, float t_prime, float bias,
                        unsigned long long* ticket, void* cuda_stream);
@@ -300,13 +328,13 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
  * loopback wires every "peer" pointer to the context's own buffers (the peers' contribution slots to a zero buffer);
  * the test preloads the text chunks of the other ranks, runs the step, and reads this rank's per-owner dtxt
  * contributions back: slot c for c != rank, and the dtxt OUTPUT of the step for the own chunk (own contribution + the
- * zero "peer" contributions).
+ * zero "peer" contributions). Chunks and slots hold T_chunk rows (its batch plus its hard negatives).
  */
 int siglip_debug_loopback(siglip_ctx* ctx);
 int siglip_debug_set_text_chunk(siglip_ctx* ctx, int chunk, const void* txt_dev, void* cuda_stream);
 int siglip_debug_get_slot(siglip_ctx* ctx, int chunk, float* out_dev, void* cuda_stream);
 /* The ids twin of siglip_debug_set_text_chunk (SIGLIP_OPT_SAMPLE_IDS): the sample ids of text chunk `chunk`
- * ([batch of that rank] int64 device buffer) as the "peer" would have published them. */
+ * ([batch of that rank] int64 device buffer: its paired texts only) as the "peer" would have published them. */
 int siglip_debug_set_chunk_ids(siglip_ctx* ctx, int chunk, const int64_t* ids_dev, void* cuda_stream);
 /* Loopback only: seed the (dt_prime, dbias) mailbox standing in for peer rank `peer`, so that the mean computed under
  * SIGLIP_OPT_SYNC_SCALAR_GRADS can be checked against numbers the kernel did not produce itself. */

@@ -43,6 +43,10 @@ def main() -> int:
     ap.add_argument("--metrics", action="store_true",
                     help="also check the in-batch retrieval metrics (return_metrics=True) against the float64 oracle, with "
                          "and without shared sample ids, uneven batches, fused and split schedules")
+    ap.add_argument("--hard-negatives", action="store_true",
+                    help="also check hard-negative captions (extra texts per rank, negatives for every image) against the "
+                         "float64 oracle: the module with the same K on every rank (fused and split, uneven batches) and "
+                         "an engine with a different K per rank")
     ap.add_argument("--soak", type=int, default=0,
                     help="N > 0: that many back-to-back steps at the --batch/--dim shape mixing the fused step, the split "
                          "API and forward-only calls; same inputs, so every step of a kind must reproduce its first result "
@@ -283,6 +287,58 @@ def main() -> int:
                     i2t_top1=abs(float(top1[0]) - hi.mean()), t2i_top1=abs(float(top1[1]) - ht.mean()),
                     unclear_rows=float(1.0 - min(ok_i.mean(), ok_t.mean())) / 50), tol=1e-6)
             eng.close()
+
+    # ---- hard-negative captions: every rank's extras are pulled with its text and scored against every image; their
+    # text gradient sums every rank's contribution through the dtxt exchange -------------------------------------------
+    if args.hard_negatives:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from hard_negatives_oracle import closed_form_hard_negatives
+        from distributed_sigmoid_loss_b200 import SigmoidLossEngine
+        Bs = [160 + 24 * r for r in range(world)]
+        D, tp, bias = 136, math.log(10.0), -8.0
+        g = torch.Generator().manual_seed(4242)
+        unit = lambda n: torch.nn.functional.normalize(torch.randn(n, D, generator=g)).to(torch.bfloat16)  # noqa: E731
+        imgs, txts = [unit(b) for b in Bs], [unit(b) for b in Bs]
+        for Ks in ([37] * world, [8 + 40 * r for r in range(world)]):
+            extras = [unit(k) for k in Ks]
+            ref = closed_form_hard_negatives([x.float().numpy() for x in imgs], [x.float().numpy() for x in txts],
+                                             [x.float().numpy() for x in extras], tp, bias)
+            mine = ref[rank]
+            dtxt_ref = torch.from_numpy(sum(ref[r]["contrib"][rank] for r in range(world)))
+            img, txt, ext = imgs[rank].to(dev), txts[rank].to(dev), extras[rank].to(dev)
+            same_k = len(set(Ks)) == 1
+            for fused in ((None, False) if same_k else ("engine",)):
+                for rep in range(2):
+                    if fused == "engine":
+                        if rep == 0:
+                            eng = SigmoidLossEngine(Bs[rank], D, dev, batch_per_rank=Bs,
+                                                    texts_per_rank=[b + k for b, k in zip(Bs, Ks)])
+                        l2, gi, gt, dtp, db = eng.fwd_bwd(img, torch.cat([txt, ext]), torch.tensor([tp], device=dev),
+                                                          torch.tensor([bias], device=dev))
+                        dtp, db = float(dtp), float(db)
+                    else:
+                        if rep == 0:
+                            modx = DDPSigmoidLoss(Bs[rank], fused_step=fused, batch_per_rank=Bs,
+                                                  hard_negatives=Ks[0]).to(dev)
+                            with torch.no_grad():
+                                modx.t_prime.fill_(tp)
+                                modx.bias.fill_(bias)
+                        modx.zero_grad()
+                        a, b, e = (x.float().requires_grad_(True) for x in (img, txt, ext))
+                        l2 = modx(a, b, negative_text=e)
+                        l2.backward()
+                        gi, gt = a.grad, torch.cat([b.grad, e.grad])
+                        dtp, db = float(modx.t_prime.grad), float(modx.bias.grad)
+                    torch.cuda.synchronize()
+                    report(f"hard negatives {fused} B={Bs} K={Ks} D={D} rep{rep}", dict(
+                        loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
+                        dimg=rel_f(gi.float().cpu(), torch.from_numpy(mine["dimg"])),
+                        dtxt=rel_f(gt.float().cpu(), dtxt_ref),
+                        dneg=rel_f(gt[Bs[rank]:].float().cpu(), dtxt_ref[Bs[rank]:]),
+                        dtp=abs(dtp - mine["dt_prime"]) / abs(mine["dt_prime"]),
+                        db=abs(db - mine["dbias"]) / abs(mine["dbias"])))
+            if not same_k:
+                eng.close()
 
     # ---- larger: fp32 autograd; dtxt reference summed over ranks ------------------------------------------
     B, D, tp, bias = 2048, 768, math.log(10.0), -10.0
