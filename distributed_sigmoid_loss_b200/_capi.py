@@ -35,6 +35,7 @@ EXPORTED_SYMBOLS = (
     "siglip_fwd_bwd_scaled",
     "siglip_fwd",
     "siglip_set_sample_ids",
+    "siglip_set_extra_text_ids",
     "siglip_request_metrics",
     "siglip_fwd_bwd_host",
     "siglip_convert_f32",
@@ -88,6 +89,7 @@ SIGLIP_OPT_AUX_TRACE = 18
 SIGLIP_OPT_PDL = 19
 SIGLIP_OPT_TPRIME_F64 = 20
 SIGLIP_OPT_SAMPLE_IDS = 21
+SIGLIP_OPT_EXTRA_TEXT_IDS = 22
 
 _lib: Optional[ctypes.CDLL] = None
 
@@ -191,6 +193,8 @@ def lib() -> ctypes.CDLL:
     L.siglip_debug_get_slot.restype = ci
     L.siglip_set_sample_ids.argtypes = [vp, vp, vp]
     L.siglip_set_sample_ids.restype = ci
+    L.siglip_set_extra_text_ids.argtypes = [vp, vp, vp]
+    L.siglip_set_extra_text_ids.restype = ci
     L.siglip_debug_set_chunk_ids.argtypes = [vp, ci, vp, vp]
     L.siglip_debug_set_chunk_ids.restype = ci
     L.siglip_request_metrics.argtypes = [vp, vp, vp, vp]

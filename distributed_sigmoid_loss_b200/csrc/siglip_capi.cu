@@ -191,6 +191,8 @@ struct siglip_ctx {
   int aux_trace_on = 0;
   int sample_ids = 0;                    // SIGLIP_OPT_SAMPLE_IDS: labels from per-sample ids (collective)
   bool ids_set = false;                  // siglip_set_sample_ids was called since the previous step
+  int extra_text_ids = 0;                // SIGLIP_OPT_EXTRA_TEXT_IDS: the extras carry ids too (needs sample_ids)
+  bool extra_ids_set = false;            // siglip_set_extra_text_ids was called since the previous step
   int off[kMaxWorld + 1] = {};           // global index of every rank's first sample (prefix sums of Bs)
   // retrieval metrics (siglip_request_metrics), armed for the next step only
   bool metrics_armed = false;
@@ -203,9 +205,11 @@ struct siglip_ctx {
   // workspaces
   __nv_bfloat16* txt_all = nullptr;      // [world][Tmax, D] bf16; slot `rank` is what the peers pull (world > 1),
                                          // followed by ids_all in the same (IPC-exported) allocation
-  int64_t* ids_all = nullptr;            // [world][ids_stride] sample ids of every text chunk (world > 1)
-  int64_t* ids_in = nullptr;             // [ids_stride] this rank's ids for the next step (siglip_set_sample_ids)
-  int ids_stride = 0;                    // Bmax rounded up to even: every slot is a whole number of 16-byte vectors
+  int64_t* ids_all = nullptr;            // [world][ids_stride] ids of every text chunk (world > 1)
+  int64_t* ids_in = nullptr;             // [ids_stride] this rank's ids for the next step: B sample ids
+                                         // (siglip_set_sample_ids), then K extra-text ids (siglip_set_extra_text_ids)
+  int ids_stride = 0;                    // Tmax rounded up to even: every slot is a whole number of 16-byte vectors.
+                                         // Fixed at creation (options are set after the handle exchange)
   unsigned long long* mkeys[2] = {};     // per step parity: [world][Tmax] column argmax partials of every text chunk
                                          // over my images, then [Bmax] row keys. world > 1: behind ids_all (exported)
   __nv_bfloat16* G[kMaxWorld] = {};      // [Bp, Tp] sigma operands (fp16 bits x kGScale), diagonal zeroed, allocated on
@@ -222,7 +226,7 @@ struct siglip_ctx {
   unsigned int* sync_words = nullptr;    // [kSyncWords] local tickets / flags
   float* loop_mailboxes = nullptr;       // loopback only: [world][2] stand-ins for the peers' (dt', dbias) mailboxes
   float* loop_zero = nullptr;            // loopback only: [world][Tmax, D] zeros standing in for the peers' contribution slots
-  unsigned long long* loop_keys = nullptr;  // loopback only: [world][Bmax] the peers' column partials of my chunk
+  unsigned long long* loop_keys = nullptr;  // loopback only: [world][Tmax] the peers' column partials of my chunk
   float* scalars = nullptr;              // [24] device scalars: host API staging, saved dt'/dbias of the last forward
   unsigned long long* aux_trace = nullptr;  // [kTraceLaunches][16] globaltimer stamps (SIGLIP_OPT_AUX_TRACE)
   float* splitk_ws = nullptr;            // fp32 partial accumulators of the split tiles of the gradient kernel
@@ -301,19 +305,29 @@ inline const int64_t* chunk_ids(const siglip_ctx* c, int cidx) {
   if (!c->sample_ids) return nullptr;
   return (cidx == c->rank) ? c->ids_in : c->ids_all + static_cast<size_t>(cidx) * c->ids_stride;
 }
-// Rank o's published ids slot, seen through its exported text allocation (they sit behind its [world][Bmax, D] text)
+// Rank o's published ids slot, seen through its exported text allocation (they sit behind its [world][Tmax, D] text)
 inline const int64_t* peer_ids(const siglip_ctx* c, int o) {
   return reinterpret_cast<const int64_t*>(c->peer_txt[o] + c->world * chunk_stride(c)) +
          static_cast<size_t>(o) * c->ids_stride;
 }
+// the sample ids of a rank (siglip_set_sample_ids)
 inline size_t ids_bytes(const siglip_ctx* c, int rank) { return static_cast<size_t>(c->Bs[rank]) * sizeof(int64_t); }
+// the ids of a text chunk as the exchange moves them: its paired texts', and under SIGLIP_OPT_EXTRA_TEXT_IDS its extras'
+inline int chunk_id_count(const siglip_ctx* c, int rank) { return c->extra_text_ids ? c->Ts[rank] : c->Bs[rank]; }
+inline size_t chunk_ids_bytes(const siglip_ctx* c, int rank) {
+  return static_cast<size_t>(chunk_id_count(c, rank)) * sizeof(int64_t);
+}
 // ids of step s are given once: a step in ids mode consumes them (checked before anything is launched)
 int take_ids(siglip_ctx* c) {
   if (!c->sample_ids) return 0;
   if (!c->ids_set)
     return fail(SIGLIP_ERR_STATE,
                 "SIGLIP_OPT_SAMPLE_IDS is on but siglip_set_sample_ids was not called since the previous step");
+  if (c->extra_text_ids && !c->extra_ids_set)
+    return fail(SIGLIP_ERR_STATE,
+                "SIGLIP_OPT_EXTRA_TEXT_IDS is on but siglip_set_extra_text_ids was not called since the previous step");
   c->ids_set = false;
+  c->extra_ids_set = false;
   return 0;
 }
 inline unsigned long long peer_timeout_ns(const siglip_ctx* c) {
@@ -361,10 +375,12 @@ int finalize_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
     a.off[p] = c->off[p];
     a.toff[p] = c->toff[p];
   }
+  a.T = c->T;
   if (c->sample_ids) {
     a.ids_own = c->ids_in;
     a.ids_all = c->ids_all;
     a.ids_stride = c->ids_stride;
+    a.extra_ids = c->extra_text_ids;
   }
   a.top1 = c->m_top1;
   a.i2t = c->m_i2t;
@@ -508,7 +524,8 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
   if (col_ids != nullptr) {
     p.row_ids = c->ids_in;
     p.col_ids = col_ids;
-    p.col_pos_n = c->Bs[cidx];   // the chunk's ids cover its paired texts only
+    // the chunk's ids cover its paired texts, and under SIGLIP_OPT_EXTRA_TEXT_IDS its extras too
+    p.col_pos_n = chunk_id_count(c, cidx);
   }
   if (c->mkeys_step != nullptr) {   // a metrics step: the kMetrics instantiation reduces the argmax keys
     p.row_keys = c->mkeys_step + mkeys_rows(c);
@@ -737,7 +754,7 @@ void add_pull_job(siglip_ctx* c, AuxList& aux, int o, unsigned int s) {
     siglip::AuxJob& ji = aux.add(siglip::kAuxCopy);
     ji.src = reinterpret_cast<const uint4*>(peer_ids(c, o));
     ji.dst = reinterpret_cast<uint4*>(c->ids_all + static_cast<size_t>(o) * c->ids_stride);
-    ji.n16 = (ids_bytes(c, o) + 15) / 16;   // within the slot: ids_stride is even
+    ji.n16 = (chunk_ids_bytes(c, o) + 15) / 16;   // within the slot: ids_stride is even
   }
 }
 
@@ -747,7 +764,7 @@ void add_ids_publish_job(siglip_ctx* c, AuxList& aux, unsigned int s) {
   siglip::AuxJob& j = aux.add(siglip::kAuxCopy);
   j.src = reinterpret_cast<const uint4*>(c->ids_in);
   j.dst = reinterpret_cast<uint4*>(c->ids_all + static_cast<size_t>(c->rank) * c->ids_stride);
-  j.n16 = (ids_bytes(c, c->rank) + 15) / 16;
+  j.n16 = (chunk_ids_bytes(c, c->rank) + 15) / 16;
   j.wait_flags = c->flags + 2 * kMaxWorld;
   j.wait_n = c->world;
   j.wait_value = s - 1;
@@ -757,7 +774,7 @@ void add_ids_publish_job(siglip_ctx* c, AuxList& aux, unsigned int s) {
 // the same publish as a stream copy (split forward, helper-kernel variant of the fused step)
 int copy_own_ids(siglip_ctx* c, cudaStream_t st) {
   if (!c->sample_ids) return 0;
-  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(c->rank) * c->ids_stride, c->ids_in, ids_bytes(c, c->rank),
+  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(c->rank) * c->ids_stride, c->ids_in, chunk_ids_bytes(c, c->rank),
                      cudaMemcpyDeviceToDevice, st));
   return 0;
 }
@@ -816,7 +833,7 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
                            static_cast<size_t>(c->Ts[nxt]) * c->D * sizeof(__nv_bfloat16), cudaMemcpyDefault, st));
         if (c->sample_ids)
           CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(nxt) * c->ids_stride, peer_ids(c, nxt),
-                             ids_bytes(c, nxt), cudaMemcpyDefault, st));
+                             chunk_ids_bytes(c, nxt), cudaMemcpyDefault, st));
       }
     }
     if ((rc = run_loss_chunk(c, k, cidx, k == 0, k == 0, img, txt_c, c->Ts[cidx], chunk_ids(c, cidx), t_prime, bias, save,
@@ -1200,7 +1217,9 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   CK(alloc(reinterpret_cast<void**>(&c->flags), kFlagBytes));
   CK(alloc(reinterpret_cast<void**>(&c->sync_words), kSyncWords * sizeof(unsigned int)));
   CK(alloc(reinterpret_cast<void**>(&c->scalars), 24 * sizeof(float)));
-  c->ids_stride = round_up(Bmax, 2);
+  // one slot per chunk holds its T ids (SIGLIP_OPT_EXTRA_TEXT_IDS may be set after the handle exchange, so the layout
+  // cannot depend on it); without extras this is Bmax rounded up, as it was before they existed
+  c->ids_stride = round_up(Tmax, 2);
   const size_t ids_slot_bytes = static_cast<size_t>(c->ids_stride) * sizeof(int64_t);
   CK(alloc(reinterpret_cast<void**>(&c->ids_in), ids_slot_bytes));
   const size_t mkeys_bytes = 2 * mkeys_block(c) * sizeof(unsigned long long);
@@ -1298,6 +1317,14 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
     case SIGLIP_OPT_SAMPLE_IDS:
       c->sample_ids = value ? 1 : 0;
       c->ids_set = false;
+      if (!c->sample_ids) c->extra_text_ids = 0;   // the extras' ids extend the sample ids
+      c->extra_ids_set = false;
+      return 0;
+    case SIGLIP_OPT_EXTRA_TEXT_IDS:
+      if (value && !c->sample_ids)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_EXTRA_TEXT_IDS needs SIGLIP_OPT_SAMPLE_IDS on first");
+      c->extra_text_ids = value ? 1 : 0;
+      c->extra_ids_set = false;
       return 0;
     case SIGLIP_OPT_STAGES_LOSS:
     case SIGLIP_OPT_STAGES_GRAD:
@@ -1396,7 +1423,7 @@ static int publish_peer_tables(siglip_ctx* c) {
           reinterpret_cast<const unsigned long long*>(reinterpret_cast<const char*>(c->peer_txt[p]) + mkeys_offset(c)) +
           q * mkeys_block(c);
       mk[q * c->world + p] = blk + static_cast<size_t>(c->rank) * c->Tmax;
-      if (c->loopback && p != c->rank) mk[q * c->world + p] = c->loop_keys + static_cast<size_t>(p) * c->Bmax;
+      if (c->loopback && p != c->rank) mk[q * c->world + p] = c->loop_keys + static_cast<size_t>(p) * c->Tmax;
     }
   CK(cudaMemcpy(c->mkey_ptrs_dev, mk.data(), mk.size() * sizeof(unsigned long long*), cudaMemcpyHostToDevice));
   c->peers_ready = true;
@@ -1463,6 +1490,21 @@ int siglip_set_sample_ids(siglip_ctx* c, const int64_t* ids_dev, void* cuda_stre
   return 0;
 }
 
+int siglip_set_extra_text_ids(siglip_ctx* c, const int64_t* ids_dev, void* cuda_stream) {
+  if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  // behind this rank's B sample ids: ids_in is then the [T] id list of my text chunk
+  const size_t k = static_cast<size_t>(c->T - c->B);
+  if (ids_dev == nullptr && k > 0) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->extra_text_ids)
+    return fail(SIGLIP_ERR_STATE, "siglip_set_extra_text_ids needs SIGLIP_OPT_EXTRA_TEXT_IDS on");
+  CK(cudaSetDevice(c->device));
+  if (k > 0)
+    CK(cudaMemcpyAsync(c->ids_in + c->B, ids_dev, k * sizeof(int64_t), cudaMemcpyDeviceToDevice,
+                       static_cast<cudaStream_t>(cuda_stream)));
+  c->extra_ids_set = true;
+  return 0;
+}
+
 int siglip_request_metrics(siglip_ctx* c, float* top1, int64_t* i2t_index, int64_t* t2i_index) {
   if (c == nullptr || top1 == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument (top1 is required)");
   if (c->mkeys[0] == nullptr) {
@@ -1495,9 +1537,9 @@ int siglip_debug_set_peer_metric_keys(siglip_ctx* c, int peer, const uint64_t* k
     return fail(SIGLIP_ERR_INVALID,
                 "siglip_debug_set_peer_metric_keys needs a loopback context and a peer rank != own rank");
   CK(cudaSetDevice(c->device));
-  CK(cudaMemcpyAsync(c->loop_keys + static_cast<size_t>(peer) * c->Bmax, keys_dev,
-                     static_cast<size_t>(c->B) * sizeof(unsigned long long), cudaMemcpyDeviceToDevice,
-                     static_cast<cudaStream_t>(cuda_stream)));
+  CK(cudaMemcpyAsync(c->loop_keys + static_cast<size_t>(peer) * c->Tmax, keys_dev,
+                     static_cast<size_t>(chunk_id_count(c, c->rank)) * sizeof(unsigned long long),
+                     cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
 
@@ -1725,8 +1767,8 @@ int siglip_debug_loopback(siglip_ctx* c) {
     CK(cudaMemset(c->loop_zero, 0, stride * c->world * sizeof(float)));
     CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_mailboxes), 2 * kMaxWorld * sizeof(float)));
     CK(cudaMemset(c->loop_mailboxes, 0, 2 * kMaxWorld * sizeof(float)));
-    CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_keys), static_cast<size_t>(c->world) * c->Bmax * 8));
-    CK(cudaMemset(c->loop_keys, 0, static_cast<size_t>(c->world) * c->Bmax * 8));
+    CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_keys), static_cast<size_t>(c->world) * c->Tmax * 8));
+    CK(cudaMemset(c->loop_keys, 0, static_cast<size_t>(c->world) * c->Tmax * 8));
   }
   for (int p = 0; p < c->world; ++p) {
     c->peer_txt[p] = c->txt_all;
@@ -1749,7 +1791,7 @@ int siglip_debug_set_text_chunk(siglip_ctx* c, int chunk, const void* txt_dev, v
 int siglip_debug_set_chunk_ids(siglip_ctx* c, int chunk, const int64_t* ids_dev, void* cuda_stream) {
   if (c == nullptr || ids_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
-  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * c->ids_stride, ids_dev, ids_bytes(c, chunk),
+  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * c->ids_stride, ids_dev, chunk_ids_bytes(c, chunk),
                      cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }

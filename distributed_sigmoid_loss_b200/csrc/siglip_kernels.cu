@@ -863,7 +863,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
 #pragma unroll
               for (int e1 = 0; e1 < 2; ++e1) {
                 const int col = col0 + 8 * j + c_lo + e1;
-                if (col < p.col_pos_n) {   // paired texts only: a hard negative has no id and is never positive
+                if (col < p.col_pos_n) {   // texts with ids only: a hard negative has none and is never positive
                   const int64_t cid = p.col_ids[col];
                   pos |= static_cast<uint32_t>(cid == rid0) << (4 * j + e1);
                   pos |= static_cast<uint32_t>(cid == rid1) << (4 * j + 2 + e1);
@@ -1370,21 +1370,24 @@ __device__ __forceinline__ int metrics_owner(const MetricsArgs& a, const int* of
   return o;
 }
 
-// sample id of the l-th sample of rank o (its image and its paired text share it)
+// sample id of the l-th sample of rank o (its image and its paired text share it); under extra_ids, l >= B_o is the id
+// of its text l
 __device__ __forceinline__ int64_t metrics_id(const MetricsArgs& a, int o, int l) {
   return (o == a.rank) ? a.ids_own[l] : a.ids_all[static_cast<size_t>(o) * a.ids_stride + l];
 }
 
-// Is global text j a hit for my image i? The positional pair, or with ids a PAIRED text with the same id: a hard negative
-// (local text index >= its rank's batch) never is, so a hard negative that outranks the caption counts as a miss.
+// Is global text j a hit for my image i? The positional pair, or with ids a text with the same id. Only the paired texts
+// carry ids unless extra_ids: a hard negative (local text index >= its rank's batch) then never is a hit, so one that
+// outranks the caption counts as a miss. Under extra_ids every text of rank o (l < T_o) carries one.
 __device__ __forceinline__ bool metrics_i2t_hit(const MetricsArgs& a, int i, int j) {
   if (a.ids_own == nullptr) return j == a.toff[a.rank] + i;
   const int o = metrics_owner(a, a.toff, j);
   const int l = j - a.toff[o];
-  return l < a.off[o + 1] - a.off[o] && metrics_id(a, o, l) == a.ids_own[i];
+  const int with_ids = a.extra_ids ? a.toff[o + 1] - a.toff[o] : a.off[o + 1] - a.off[o];
+  return l < with_ids && metrics_id(a, o, l) == a.ids_own[i];
 }
 
-// Is global image g a hit for my (paired) text i?
+// Is global image g a hit for my text i (a paired one, or any under extra_ids)?
 __device__ __forceinline__ bool metrics_t2i_hit(const MetricsArgs& a, int i, int g) {
   if (a.ids_own == nullptr) return g == a.off[a.rank] + i;
   const int o = metrics_owner(a, a.off, g);
@@ -1429,11 +1432,17 @@ __global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const
   }
   __syncthreads();
   unsigned int h_i2t = 0, h_t2i = 0;
-  // column partials are kept for the paired texts only (i < B); the extras' column keys are computed but never read
-  for (int i = tid; i < a.B; i += kMetricsThreads) {
-    const int j = key_index(a.row_keys[i]);   // best text of my image i, over all texts including the extras
-    if (a.i2t) a.i2t[i] = j;
-    if (j >= 0) h_i2t += metrics_i2t_hit(a, i, j);
+  // column partials are read for the paired texts (i < B), and under extra_ids for every text of this rank (i < T);
+  // otherwise the extras' column keys are computed but never read
+  const int nt = a.extra_ids ? a.T : a.B;
+  const int n = a.B > nt ? a.B : nt;
+  for (int i = tid; i < n; i += kMetricsThreads) {
+    if (i < a.B) {
+      const int j = key_index(a.row_keys[i]);   // best text of my image i, over all texts including the extras
+      if (a.i2t) a.i2t[i] = j;
+      if (j >= 0) h_i2t += metrics_i2t_hit(a, i, j);
+    }
+    if (i >= nt) continue;
     unsigned long long k = a.col_own[i];
     if (a.world > 1) {
       for (int q = 0; q < a.world; ++q) {
@@ -1457,7 +1466,7 @@ __global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const
     atomicAdd(&hits[1], h_t2i);
   }
   __syncthreads();
-  if (tid < 2) a.top1[tid] = static_cast<float>(hits[tid]) / static_cast<float>(a.B);
+  if (tid < 2) a.top1[tid] = static_cast<float>(hits[tid]) / static_cast<float>(tid == 0 ? a.B : nt);
 }
 
 // -------------------------------------------------------------------------------------------------

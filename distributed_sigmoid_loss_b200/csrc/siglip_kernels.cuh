@@ -133,7 +133,8 @@ struct KernelParams {
   int col_off;                   // global index of the chunk's first text
   // Hard-negative captions (siglip_ctx_create_texts): a text chunk is [paired texts; extras]. Appended last like the
   // metrics fields, so that the default loss kernel's parameter offsets do not move.
-  int col_pos_n;   // loss kernel, kIds: paired columns of the chunk (col_ids has this many entries; extras never match)
+  int col_pos_n;   // loss kernel, kIds: columns of the chunk that carry ids (col_ids has this many entries): its paired
+                   // texts, or all of them under SIGLIP_OPT_EXTRA_TEXT_IDS. Columns past it never match
   int fix_rows;    // out kernel: rows of fix_vec / fix_mat (this rank's batch); rows >= fix_rows take no fix term
   // Host only (launch_gemm): size the grid of a loss launch as if its chunk had grid_n columns. Every loss kernel of a
   // forward then has the same grid, so the per-CTA partial slots it accumulates and the last one sums line up when the
@@ -197,7 +198,7 @@ int launch_signal_flags(unsigned int* const* flag_ptrs_dev, int n, unsigned int 
 constexpr int kMetricsMaxWorld = 32;
 struct MetricsArgs {
   const unsigned long long* row_keys;          // [B] local
-  const unsigned long long* col_own;           // [B] my partial of my chunk
+  const unsigned long long* col_own;           // [T] my partial of my chunk
   const unsigned long long* const* col_peers;  // [world] every rank's partial of my chunk (world > 1; own entry unused)
   int B, rank, world;
   int off[kMetricsMaxWorld + 1];               // prefix sums of the per-rank batches (global image indices)
@@ -206,9 +207,12 @@ struct MetricsArgs {
   const int64_t* ids_own;                      // null = positional labels; else this rank's sample ids
   const int64_t* ids_all;                      // [world][ids_stride]: every chunk's ids, gathered in this step
   int ids_stride;
+  int extra_ids;                               // SIGLIP_OPT_EXTRA_TEXT_IDS: every text has an id (ids_own: [T]),
+                                               // extras can be hits, and t2i covers all T texts of this rank
+  int T;                                       // this rank's texts
   float* top1;                                 // [2]: i2t, t2i
   int64_t* i2t;                                // [B] or null
-  int64_t* t2i;                                // [B] or null
+  int64_t* t2i;                                // [B] ([T] under extra_ids) or null
   unsigned int* const* sig_ptrs;               // [world] flag kind 5 of every rank (world > 1)
   const volatile unsigned int* flags_local;    // my flag kind 5 row
   unsigned int value;

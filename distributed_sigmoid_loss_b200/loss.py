@@ -85,6 +85,7 @@ class SigmoidLossEngine:
         if texts_per_rank is None:
             self.texts_per_rank = list(self.batch_per_rank)
         self.texts = self.texts_per_rank[self.rank]   # rows of txt / dtxt: the batch plus this rank's hard negatives
+        self.extra_text_ids = False   # SIGLIP_OPT_EXTRA_TEXT_IDS: every text of a chunk carries an id (see set_option)
         self._h = h
         _capi.check(self._L.siglip_ctx_set_option(h, _capi.SIGLIP_OPT_CTA_GROUP, int(cta_group)))
         _capi.check(self._L.siglip_ctx_set_option(h, _capi.SIGLIP_OPT_OVERLAP_PULL, int(bool(overlap_pull))))
@@ -107,6 +108,8 @@ class SigmoidLossEngine:
 
     def set_option(self, option: int, value: int) -> None:
         _capi.check(self._L.siglip_ctx_set_option(self._h, option, value))
+        if option == _capi.SIGLIP_OPT_EXTRA_TEXT_IDS or (option == _capi.SIGLIP_OPT_SAMPLE_IDS and not value):
+            self.extra_text_ids = bool(value)   # the library clears the extras' ids with the sample ids
 
     def kernel_times(self):
         """(loss_ms, loss_launches, grad_ms, grad_launches) since the last call; needs SIGLIP_OPT_KERNEL_TIMING."""
@@ -126,9 +129,17 @@ class SigmoidLossEngine:
         with torch.cuda.device(self.device):
             _capi.check(self._L.siglip_set_sample_ids(self._h, ids.data_ptr(), self._stream()))
 
+    def set_extra_text_ids(self, ids: torch.Tensor) -> None:
+        """SIGLIP_OPT_EXTRA_TEXT_IDS: the ids of this rank's T - B extra texts ([T - B] int64, contiguous, on the engine's
+        device) for the NEXT step, copied on the current stream like set_sample_ids."""
+        self._check_ids(ids, self.texts - self.batch)
+        with torch.cuda.device(self.device):
+            _capi.check(self._L.siglip_set_extra_text_ids(self._h, ids.data_ptr(), self._stream()))
+
     def debug_set_chunk_ids(self, chunk: int, ids: torch.Tensor) -> None:
-        """Loopback: the sample ids of text chunk `chunk` as its owner would have published them."""
-        self._check_ids(ids, self.batch_per_rank[chunk])
+        """Loopback: the ids of text chunk `chunk` as its owner would have published them: its sample ids ([B_c]), or
+        under SIGLIP_OPT_EXTRA_TEXT_IDS the ids of all its texts ([T_c])."""
+        self._check_ids(ids, (self.texts_per_rank if self.extra_text_ids else self.batch_per_rank)[chunk])
         _capi.check(self._L.siglip_debug_set_chunk_ids(self._h, chunk, ids.data_ptr(), self._stream()))
 
     def _check_ids(self, ids: torch.Tensor, n: int) -> None:
@@ -139,9 +150,10 @@ class SigmoidLossEngine:
     def request_metrics(self, top1: torch.Tensor, i2t_index: Optional[torch.Tensor] = None,
                         t2i_index: Optional[torch.Tensor] = None) -> None:
         """Arm the in-batch retrieval metrics of the NEXT step (siglip_request_metrics): top1 fp32 [2] (i2t, t2i),
-        i2t_index / t2i_index int64 [B] (global indices) or None, all contiguous on the engine's device. Nothing is read
-        on the host; the step writes them on its stream."""
-        bufs = ((top1, torch.float32, 2), (i2t_index, torch.int64, self.batch), (t2i_index, torch.int64, self.batch))
+        i2t_index int64 [B] and t2i_index int64 [B] ([T] under SIGLIP_OPT_EXTRA_TEXT_IDS) (global indices) or None, all
+        contiguous on the engine's device. Nothing is read on the host; the step writes them on its stream."""
+        bufs = ((top1, torch.float32, 2), (i2t_index, torch.int64, self.batch),
+                (t2i_index, torch.int64, self.metric_texts))
         for k, (x, dt, n) in enumerate(bufs):
             if x is None and k > 0:
                 continue
@@ -152,12 +164,18 @@ class SigmoidLossEngine:
                                                    t2i_index.data_ptr() if t2i_index is not None else None))
 
     def debug_set_peer_metric_keys(self, peer: int, keys: torch.Tensor) -> None:
-        """Loopback: the column argmax keys ([B] int64 holding the 64-bit key bits) standing in for peer `peer`'s partial
-        of this rank's text chunk."""
-        if keys.dtype != torch.int64 or tuple(keys.shape) != (self.batch,) or not keys.is_contiguous() or \
+        """Loopback: the column argmax keys ([B] int64 holding the 64-bit key bits, [T] under SIGLIP_OPT_EXTRA_TEXT_IDS)
+        standing in for peer `peer`'s partial of this rank's text chunk."""
+        n = self.metric_texts
+        if keys.dtype != torch.int64 or tuple(keys.shape) != (n,) or not keys.is_contiguous() or \
                 keys.device != self.device:
-            raise RuntimeError(f"peer metric keys must be a contiguous int64 [{self.batch}] tensor on {self.device}")
+            raise RuntimeError(f"peer metric keys must be a contiguous int64 [{n}] tensor on {self.device}")
         _capi.check(self._L.siglip_debug_set_peer_metric_keys(self._h, peer, keys.data_ptr(), self._stream()))
+
+    @property
+    def metric_texts(self) -> int:
+        """Texts of this rank that t2i ranks: the paired ones, or all T under SIGLIP_OPT_EXTRA_TEXT_IDS."""
+        return self.texts if self.extra_text_ids else self.batch
 
     def debug_get_slot(self, chunk: int) -> torch.Tensor:
         out = torch.empty(self.texts_per_rank[chunk], self.dim, device=self.device, dtype=torch.float32)
@@ -434,12 +452,13 @@ class _SigmoidLossFn(torch.autograd.Function):
         of 1; backward = one multiply by grad_output per tensor (siglip_scale). O(B^2) workspace.
     normalize=True additionally fuses F.normalize of both inputs (forward) and its backward around the loss.
     ids: [B] int64 sample ids (SIGLIP_OPT_SAMPLE_IDS engines), set before every step the engine runs for this call.
+    extra_ids: [T - B] int64 ids of the extra texts (SIGLIP_OPT_EXTRA_TEXT_IDS engines), set along with ids.
     metrics: (top1, i2t_index, t2i_index) output buffers: the retrieval metrics of this call's step are armed. A re-run
     of the forward by the backward's generation guard does not arm them again (they belong to the first run)."""
 
     @staticmethod
     def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool = False, fused: bool = False,
-                ids: Optional[torch.Tensor] = None, metrics=None):
+                ids: Optional[torch.Tensor] = None, metrics=None, extra_ids: Optional[torch.Tensor] = None):
         need_grad = any(ctx.needs_input_grad[:4])
         raw = None
         # bf16 callers: bf16 operands (what autograd would multiply). Anything wider (the reference's own test feeds
@@ -473,9 +492,11 @@ class _SigmoidLossFn(torch.autograd.Function):
             b = b.to(device=img.device, dtype=torch.float32)
         b = b.reshape(1)
         ctx.fused = bool(fused and need_grad)
-        ctx.ids = ids
+        ctx.ids, ctx.extra_ids = ids, extra_ids
         if ids is not None:
             engine.set_sample_ids(ids)
+        if extra_ids is not None:
+            engine.set_extra_text_ids(extra_ids)
         if metrics is not None:
             engine.request_metrics(*metrics)
         if ctx.fused:
@@ -527,6 +548,8 @@ class _SigmoidLossFn(torch.autograd.Function):
                 # branch together, so the collective stays matched); the re-run takes this call's ids again
                 if ctx.ids is not None:
                     eng.set_sample_ids(ctx.ids)
+                if ctx.extra_ids is not None:
+                    eng.set_extra_text_ids(ctx.extra_ids)
                 eng.forward(img_b, txt_b, tp, b, True)
                 ctx.gen = eng.saved_generation
             if ctx.normalize:
@@ -543,17 +566,19 @@ class _SigmoidLossFn(torch.autograd.Function):
                 gt = dtxt.to(tdt) if ctx.needs_input_grad[1] else None
         gp = dtp.reshape(pshape).to(device=pdev, dtype=pdt) if ctx.needs_input_grad[2] else None
         gb = db.reshape(bshape).to(device=bdev, dtype=bdt) if ctx.needs_input_grad[3] else None
-        return gi, gt, gp, gb, None, None, None, None, None
+        return gi, gt, gp, gb, None, None, None, None, None, None
 
 
 class _EngineCache:
     def __init__(self, group=None, cta_group: int = 2, overlap_pull: bool = True, sync_scalar_grads: bool = False,
-                 bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0):
+                 bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
+                 extra_texts: int = 0):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
         self.sync_scalar_grads, self.bidir = sync_scalar_grads, bidir
         self.multi_positive = multi_positive
         self.batch_per_rank = batch_per_rank
         self.hard_negatives = hard_negatives
+        self.extra_texts = extra_texts
         self._engines: Dict[Tuple[int, int, int], SigmoidLossEngine] = {}
 
     def get(self, batch: int, dim: int, device: torch.device) -> SigmoidLossEngine:
@@ -562,11 +587,12 @@ class _EngineCache:
         if eng is None:
             dev = torch.device("cuda", key[0])
             tpr = None
-            if self.hard_negatives:
+            extras = self.hard_negatives + self.extra_texts   # at most one of the two is non-zero
+            if extras:
                 # every rank scores the same number K of extras: T_p = B_p + K
                 rank, world = _group_rank_world(self.group)
                 bpr = self.batch_per_rank if self.batch_per_rank is not None else [batch] * world
-                tpr = [int(b) + self.hard_negatives for b in bpr]
+                tpr = [int(b) + extras for b in bpr]
             eng = SigmoidLossEngine(batch, dim, dev, self.group, self.cta_group, self.overlap_pull,
                                     batch_per_rank=self.batch_per_rank, texts_per_rank=tpr)
             if self.sync_scalar_grads:
@@ -575,6 +601,8 @@ class _EngineCache:
                 eng.set_option(_capi.SIGLIP_OPT_BIDIR, 1)
             if self.multi_positive:
                 eng.set_option(_capi.SIGLIP_OPT_SAMPLE_IDS, 1)
+            if self.extra_texts:
+                eng.set_option(_capi.SIGLIP_OPT_EXTRA_TEXT_IDS, 1)   # needs the sample ids on first
             self._engines[key] = eng
         return eng
 
@@ -602,31 +630,65 @@ def _validate_ids(sample_ids, multi_positive: bool, embeddings: torch.Tensor) ->
     return sample_ids.to(torch.int64).contiguous()
 
 
-def _validate_hard_negatives(hard_negatives) -> int:
+def _validate_hard_negatives(hard_negatives, name: str = "hard_negatives") -> int:
     if isinstance(hard_negatives, bool) or not isinstance(hard_negatives, int) or hard_negatives < 0:
-        raise RuntimeError(f"hard_negatives must be an int >= 0, got {hard_negatives!r}")
+        raise RuntimeError(f"{name} must be an int >= 0, got {hard_negatives!r}")
     return hard_negatives
 
 
-def _validate_negatives(text_embeddings: torch.Tensor, negative_text, hard_negatives: int) -> None:
+def _validate_extra_texts(extra_texts, multi_positive: bool, hard_negatives: int) -> int:
+    """extra_texts=K of a module: K extra captions per rank with ids of their own, so it needs the sample ids of
+    multi_positive, and it is a different meaning of the extras than hard_negatives (never positive)."""
+    extra_texts = _validate_hard_negatives(extra_texts, "extra_texts")
+    if extra_texts and not multi_positive:
+        raise RuntimeError("extra_texts=K needs multi_positive=True (the extras' ids are compared with the sample ids)")
+    if extra_texts and hard_negatives:
+        raise RuntimeError("extra_texts and hard_negatives cannot be combined: give the hard negatives as extra texts "
+                           "whose ids match no image")
+    return extra_texts
+
+
+def _validate_negatives(text_embeddings: torch.Tensor, negative_text, hard_negatives: int,
+                        name: str = "negative_text", option: str = "hard_negatives") -> None:
     """negative_text of a forward: required ([K, D], the dtype / device / width of the texts) when the loss was built
-    with hard_negatives = K > 0, refused otherwise. Raises before any GPU work."""
+    with hard_negatives = K > 0, refused otherwise. Raises before any GPU work. (name / option: the same check for
+    extra_text and extra_texts.)"""
     if hard_negatives == 0:
         if negative_text is not None:
-            raise RuntimeError("negative_text given, but the loss was built without hard_negatives (hard_negatives=K)")
+            raise RuntimeError(f"{name} given, but the loss was built without {option} ({option}=K)")
         return
     if negative_text is None:
-        raise RuntimeError(f"hard_negatives={hard_negatives}: forward needs negative_text ([{hard_negatives}, emb_dim])")
+        raise RuntimeError(f"{option}={hard_negatives}: forward needs {name} ([{hard_negatives}, emb_dim])")
     if not isinstance(negative_text, torch.Tensor):
-        raise RuntimeError(f"negative_text must be a tensor, got {type(negative_text).__name__}")
+        raise RuntimeError(f"{name} must be a tensor, got {type(negative_text).__name__}")
     want = (hard_negatives, text_embeddings.shape[1] if text_embeddings.dim() == 2 else None)
     if negative_text.dim() != 2 or tuple(negative_text.shape) != want:
-        raise RuntimeError(f"negative_text must have shape [{want[0]}, {want[1]}] (hard_negatives x the texts' width), "
+        raise RuntimeError(f"{name} must have shape [{want[0]}, {want[1]}] ({option} x the texts' width), "
                            f"got {tuple(negative_text.shape)}")
     if negative_text.dtype != text_embeddings.dtype:
-        raise RuntimeError(f"negative_text is {negative_text.dtype}, the texts {text_embeddings.dtype}")
+        raise RuntimeError(f"{name} is {negative_text.dtype}, the texts {text_embeddings.dtype}")
     if negative_text.device != text_embeddings.device:
-        raise RuntimeError(f"negative_text is on {negative_text.device}, the texts on {text_embeddings.device}")
+        raise RuntimeError(f"{name} is on {negative_text.device}, the texts on {text_embeddings.device}")
+
+
+def _validate_extra_text_ids(extra_text_ids, extra_texts: int, text_embeddings: torch.Tensor) -> Optional[torch.Tensor]:
+    """extra_text_ids of a forward: required ([K] integers on the texts' device) when the loss was built with
+    extra_texts = K > 0, refused otherwise. Returns them as contiguous int64, or None. Raises before any GPU work."""
+    if extra_texts == 0:
+        if extra_text_ids is not None:
+            raise RuntimeError("extra_text_ids given, but the loss was built without extra_texts (extra_texts=K)")
+        return None
+    if extra_text_ids is None:
+        raise RuntimeError(f"extra_texts={extra_texts}: forward needs extra_text_ids ([{extra_texts}] integer tensor)")
+    if not isinstance(extra_text_ids, torch.Tensor) or extra_text_ids.dtype not in _ID_DTYPES:
+        raise RuntimeError(f"extra_text_ids must be an integer tensor, got "
+                           f"{extra_text_ids.dtype if isinstance(extra_text_ids, torch.Tensor) else type(extra_text_ids)}")
+    if extra_text_ids.dim() != 1 or extra_text_ids.shape[0] != extra_texts:
+        raise RuntimeError(f"extra_text_ids must have shape [{extra_texts}] (one id per extra text), got "
+                           f"{tuple(extra_text_ids.shape)}")
+    if extra_text_ids.device != text_embeddings.device:
+        raise RuntimeError(f"extra_text_ids are on {extra_text_ids.device}, the texts on {text_embeddings.device}")
+    return extra_text_ids.to(torch.int64).contiguous()
 
 
 def _with_negatives(text_embeddings: torch.Tensor, negative_text) -> torch.Tensor:
@@ -640,10 +702,11 @@ def _validate_return_metrics(return_metrics) -> None:
         raise RuntimeError(f"return_metrics must be a bool, got {type(return_metrics).__name__}")
 
 
-def _metric_buffers(batch: int, device: torch.device):
+def _metric_buffers(batch: int, device: torch.device, texts: Optional[int] = None):
+    """texts: rows of t2i_index (all T texts under extra_texts; the batch otherwise)."""
     top1 = torch.empty(2, device=device, dtype=torch.float32)
     return (top1, torch.empty(batch, device=device, dtype=torch.int64),
-            torch.empty(batch, device=device, dtype=torch.int64))
+            torch.empty(batch if texts is None else texts, device=device, dtype=torch.int64))
 
 
 def _metric_dict(bufs) -> Dict[str, torch.Tensor]:
@@ -707,13 +770,25 @@ class DDPSigmoidLoss(nn.Module):
     gradient of the sum over ranks of their losses. The loss still divides by the rank's image batch. ``i2t_index`` then
     ranges over all texts including the extras (global index: prefix sums of B_p + K), and a winning extra is a miss.
     Collective: every rank uses the same K.
+
+    ``multi_positive=True, extra_texts=K > 0``: several captions per image without repeating the image. Every
+    ``forward`` also takes ``extra_text`` ([K, D], like ``negative_text``) and ``extra_text_ids`` ([K] integers). Extra
+    j is positive for every image of the global batch whose sample id equals ``extra_text_ids[j]``: a further caption of
+    that image. An extra whose id matches no image is a hard negative. This scores ``B x (B + K)`` pairs per rank where
+    repeating each image once per caption would score ``M·B x M·B``. The loss still divides by the image batch, and
+    ``extra_text.grad`` comes back through autograd. With ``return_metrics``, a winning extra caption is an i2t hit,
+    and ``t2i_index`` is ``[B + K]``: ``t2i_top1`` counts over every text of the rank, so a pure-negative extra is always
+    a t2i miss. A caller who mixes N of them in gets the caption-only rate as ``t2i_top1 · T / (T − N)``, T = B + K.
+    Cannot be combined with ``hard_negatives``. Collective: every rank uses the same K.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
                  normalize_inputs: bool = False, sync_scalar_grads: bool = False, fused_step: Optional[bool] = None,
-                 batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0) -> None:
+                 batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
+                 extra_texts: int = 0) -> None:
         super().__init__()
         hard_negatives = _validate_hard_negatives(hard_negatives)
+        extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
         self.t_prime = nn.Parameter(torch.tensor(math.log(10), dtype=torch.float64))
         self.bias = nn.Parameter(torch.tensor(-10.0))
         self.gpu_batch_size = gpu_batch_size
@@ -731,26 +806,32 @@ class DDPSigmoidLoss(nn.Module):
         self.multi_positive = multi_positive
         # extension: hard-negative captions, K extra texts per rank scored against every image
         self.hard_negatives = hard_negatives
+        # extension: extra captions with ids of their own (several captions per image)
+        self.extra_texts = extra_texts
         self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank,
-                                   multi_positive=multi_positive, hard_negatives=hard_negatives)
+                                   multi_positive=multi_positive, hard_negatives=hard_negatives,
+                                   extra_texts=extra_texts)
 
     def engine_for(self, batch: int, dim: int, device: torch.device) -> SigmoidLossEngine:
         return self._cache.get(batch, (dim + 7) // 8 * 8, device)
 
     def forward(self, image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, *,
                 negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
-                return_metrics: bool = False):
+                return_metrics: bool = False, extra_text: Optional[torch.Tensor] = None,
+                extra_text_ids: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
         ids = _validate_ids(sample_ids, self.multi_positive, image_embeddings)
         _validate_negatives(text_embeddings, negative_text, self.hard_negatives)
+        _validate_negatives(text_embeddings, extra_text, self.extra_texts, "extra_text", "extra_texts")
+        extra_ids = _validate_extra_text_ids(extra_text_ids, self.extra_texts, text_embeddings)
         _validate(image_embeddings, text_embeddings, self.gpu_batch_size)
-        text_embeddings = _with_negatives(text_embeddings, negative_text)
+        text_embeddings = _with_negatives(_with_negatives(text_embeddings, negative_text), extra_text)
         image_embeddings, text_embeddings = _pad_dim(image_embeddings), _pad_dim(text_embeddings)
         eng = self._cache.get(image_embeddings.shape[0], image_embeddings.shape[1], image_embeddings.device)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
-        bufs = _metric_buffers(eng.batch, eng.device) if return_metrics else None
+        bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts) if return_metrics else None
         loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
-                                    self.normalize_inputs, fused, ids, bufs)
+                                    self.normalize_inputs, fused, ids, bufs, extra_ids)
         return (loss, _metric_dict(bufs)) if return_metrics else loss
 
 
@@ -764,30 +845,38 @@ class SigLipLoss(nn.Module):
     ...; the pairs covered and the result are the same. ``multi_positive=True``: labels from the ``sample_ids`` every
     forward then takes, as in ``DDPSigmoidLoss``. ``return_metrics=True``: returns ``(loss_or_dict, metrics)`` with the
     retrieval metrics of ``DDPSigmoidLoss``; they stay out of the ``output_dict``, whose values open_clip sums into the
-    total loss. ``hard_negatives=K``: every forward takes ``negative_text`` [K, D], as in ``DDPSigmoidLoss``."""
+    total loss. ``hard_negatives=K``: every forward takes ``negative_text`` [K, D], as in ``DDPSigmoidLoss``.
+    ``multi_positive=True, extra_texts=K``: every forward takes ``extra_text`` [K, D] and ``extra_text_ids`` [K], extra
+    captions positive for the images with the same id, as in ``DDPSigmoidLoss`` (a pure-negative extra is always a t2i
+    miss: the caption-only rate is ``t2i_top1 · T / (T − N)`` for N of them among T = B + K texts)."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
-                 multi_positive: bool = False, hard_negatives: int = 0):
+                 multi_positive: bool = False, hard_negatives: int = 0, extra_texts: int = 0):
         super().__init__()
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
         hard_negatives = _validate_hard_negatives(hard_negatives)
+        extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
         self.cache_labels, self.rank, self.world_size, self.bidir = cache_labels, rank, world_size, bidir
         self.use_horovod = use_horovod
         self.fused_step = fused_step
         self.multi_positive = multi_positive
         self.hard_negatives = hard_negatives
+        self.extra_texts = extra_texts
         self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive,
-                                   hard_negatives=hard_negatives)
+                                   hard_negatives=hard_negatives, extra_texts=extra_texts)
 
     def forward(self, image_features, text_features, logit_scale, logit_bias, output_dict: bool = False, *,
                 negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
-                return_metrics: bool = False):
+                return_metrics: bool = False, extra_text: Optional[torch.Tensor] = None,
+                extra_text_ids: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
         ids = _validate_ids(sample_ids, self.multi_positive, image_features)
         _validate_negatives(text_features, negative_text, self.hard_negatives)
+        _validate_negatives(text_features, extra_text, self.extra_texts, "extra_text", "extra_texts")
+        extra_ids = _validate_extra_text_ids(extra_text_ids, self.extra_texts, text_features)
         _validate(image_features, text_features, None)
-        text_features = _with_negatives(text_features, negative_text)
+        text_features = _with_negatives(_with_negatives(text_features, negative_text), extra_text)
         image_features, text_features = _pad_dim(image_features), _pad_dim(text_features)
         eng = self._cache.get(image_features.shape[0], image_features.shape[1], image_features.device)
         if (eng.rank, eng.world) != (self.rank, self.world_size):
@@ -797,7 +886,8 @@ class SigLipLoss(nn.Module):
         if logit_bias is None:
             logit_bias = torch.zeros((), device=image_features.device)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
-        bufs = _metric_buffers(eng.batch, eng.device) if return_metrics else None
-        loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs)
+        bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts) if return_metrics else None
+        loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs,
+                                    extra_ids)
         out = {"contrastive_loss": loss} if output_dict else loss
         return (out, _metric_dict(bufs)) if return_metrics else out

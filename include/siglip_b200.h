@@ -102,6 +102,15 @@ enum {
                                  results). Off-diagonal positives enter the gradient contractions through the fp16 sigma
                                  operand (2^-12 relative rounding each, like the negatives). The host-buffer entries are
                                  unavailable in this mode. Collective: set on all ranks. Default 0 */
+  SIGLIP_OPT_EXTRA_TEXT_IDS = 22, /* 1: the extra texts of a siglip_ctx_create_texts context carry ids too (several
+                                     captions per image). Text j of chunk c has id text_ids_c[j]: sample_ids_c[j] for
+                                     j < B_c, and the extra's own id (siglip_set_extra_text_ids) for j >= B_c. Pair (i, j)
+                                     is positive iff sample_ids_r[i] == text_ids_c[j], on any rank: an extra that carries
+                                     an image's id is another caption of that image, an extra whose id matches no image
+                                     is a hard negative. The loss still divides by the image batch B_r. Needs
+                                     SIGLIP_OPT_SAMPLE_IDS on (else SIGLIP_ERR_STATE); turning that option off clears this
+                                     one. Accepted on any context; with T == B it changes nothing. Collective: set on all
+                                     ranks. Default 0 */
   SIGLIP_OPT_AUX_TRACE = 18 /* 1: record globaltimer stamps of the auxiliary warps of CTA 0 for every launch (start,
                                last peer flag seen, jobs done, end of launch); read with siglip_ctx_aux_trace */
 };
@@ -142,7 +151,8 @@ int siglip_ctx_create_uneven(siglip_ctx** out, int device, int rank, int world, 
  * with y = +1 for the positional pair (or, under SIGLIP_OPT_SAMPLE_IDS, a PAIRED text with the same id) and -1 for
  * everything else: an extra is never positive, whatever the ids. txt / dtxt of every step are [T_r, D] (dtxt includes
  * the extras' rows: the gradient of the sum over ranks of their losses); dt' / dbias include the extras' terms. Sample
- * ids stay [B_r] (they describe the paired texts). The host-buffer entries are unavailable (SIGLIP_ERR_STATE).
+ * ids stay [B_r] (they describe the paired texts); SIGLIP_OPT_EXTRA_TEXT_IDS gives the extras ids of their own, so that
+ * they can be further captions of an image. The host-buffer entries are unavailable (SIGLIP_ERR_STATE).
  * Workspaces: the text-shaped ones (gathered text, dtxt slots, fp16 text copies) hold max(T) rows per chunk and the
  * sigma operands are [Bp, Tp] (max B, max T rounded up to 256). Time grows with T / B like the FLOPs (6 B T D).
  * Every rank passes the same two lists; texts_per_rank == images_per_rank is exactly siglip_ctx_create_uneven.
@@ -247,13 +257,25 @@ unsigned long long siglip_ctx_saved_generation(const siglip_ctx* ctx);
 int siglip_set_sample_ids(siglip_ctx* ctx, const int64_t* ids_dev, void* cuda_stream);
 
 /*
+ * SIGLIP_OPT_EXTRA_TEXT_IDS: the ids of this rank's K_r = T_r - B_r extra texts (int64 device buffer of K_r values; may
+ * be NULL when K_r = 0) for
+ * the NEXT step, copied on the stream like the sample ids (a single-rank step with both copies can be captured into a
+ * CUDA graph). In this mode a step needs both this call and siglip_set_sample_ids since the previous step, else it
+ * returns SIGLIP_ERR_STATE before launching anything; outside the mode this call returns SIGLIP_ERR_STATE.
+ */
+int siglip_set_extra_text_ids(siglip_ctx* ctx, const int64_t* ids_dev, void* cuda_stream);
+
+/*
  * In-batch retrieval metrics of the NEXT siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd call (that step only),
  * computed from the logits the loss kernels already hold in registers, without a second similarity GEMM:
  *   i2t_index[i] = argmax_j s_ij over all sum(T) texts, for each of this rank's B images (global text index; with hard
  *                  negatives a winning extra is a miss)
- *   t2i_index[j] = argmax_i s_ij over all sum(B) images, for each of this rank's B paired texts (global image index)
+ *   t2i_index[j] = argmax_i s_ij over all sum(B) images, for each of this rank's B paired texts (global image index;
+ *                  under SIGLIP_OPT_EXTRA_TEXT_IDS for each of its T texts, so t2i_index is then [T])
  *   top1[0] / top1[1] = fraction of this rank's images / texts whose top-1 is a positive: the positional diagonal, or
- *                       under SIGLIP_OPT_SAMPLE_IDS a pair with the same id, on any rank
+ *                       under SIGLIP_OPT_SAMPLE_IDS a pair with the same id, on any rank. Under
+ *                       SIGLIP_OPT_EXTRA_TEXT_IDS an extra with the image's id is a hit for i2t, and top1[1] counts
+ *                       over all T texts: an extra whose id matches no image is always a t2i miss
  * Global indices follow the concatenated batch (prefix sums of the per-rank batches). Ties go to the lowest global index;
  * the ranking uses the kernel's fp32 <img, txt> (z = exp(t') s + b is monotone in s). Per rank, like the loss.
  * top1: 2 fp32 device floats (required); i2t_index / t2i_index: [B] int64 device buffers or NULL. Loss and gradients are
@@ -334,13 +356,15 @@ int siglip_debug_loopback(siglip_ctx* ctx);
 int siglip_debug_set_text_chunk(siglip_ctx* ctx, int chunk, const void* txt_dev, void* cuda_stream);
 int siglip_debug_get_slot(siglip_ctx* ctx, int chunk, float* out_dev, void* cuda_stream);
 /* The ids twin of siglip_debug_set_text_chunk (SIGLIP_OPT_SAMPLE_IDS): the sample ids of text chunk `chunk`
- * ([batch of that rank] int64 device buffer: its paired texts only) as the "peer" would have published them. */
+ * ([batch of that rank] int64 device buffer: its paired texts only; [T of that rank] under SIGLIP_OPT_EXTRA_TEXT_IDS:
+ * its paired texts, then its extras) as the "peer" would have published them. */
 int siglip_debug_set_chunk_ids(siglip_ctx* ctx, int chunk, const int64_t* ids_dev, void* cuda_stream);
 /* Loopback only: seed the (dt_prime, dbias) mailbox standing in for peer rank `peer`, so that the mean computed under
  * SIGLIP_OPT_SYNC_SCALAR_GRADS can be checked against numbers the kernel did not produce itself. */
 int siglip_debug_set_mailbox(siglip_ctx* ctx, int peer, float dt_prime, float dbias);
 /* Loopback only: seed the column argmax partials of this rank's text chunk that stand in for peer rank `peer`'s
- * ([B] 64-bit keys: (order-preserving fp32 bits of s) << 32 | (0xFFFFFFFF - global image index), 0 = no candidate), so
+ * ([B] 64-bit keys, [T] under SIGLIP_OPT_EXTRA_TEXT_IDS: (order-preserving fp32 bits of s) << 32 |
+ * (0xFFFFFFFF - global image index), 0 = no candidate), so
  * that the cross-rank combine of a metrics step sees candidates the kernel did not produce itself. */
 int siglip_debug_set_peer_metric_keys(siglip_ctx* ctx, int peer, const uint64_t* keys_dev, void* cuda_stream);
 /* With SIGLIP_OPT_AUX_TRACE: device-synchronise and copy out 16 globaltimer stamps (ns) per launch since the last call:

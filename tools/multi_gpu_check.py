@@ -47,6 +47,9 @@ def main() -> int:
                     help="also check hard-negative captions (extra texts per rank, negatives for every image) against the "
                          "float64 oracle: the module with the same K on every rank (fused and split, uneven batches) and "
                          "an engine with a different K per rank")
+    ap.add_argument("--extra-texts", action="store_true",
+                    help="also check extra captions with ids (several captions per image) against the float64 oracle: "
+                         "extras that caption images of other ranks, extras that match nothing, fused and split")
     ap.add_argument("--soak", type=int, default=0,
                     help="N > 0: that many back-to-back steps at the --batch/--dim shape mixing the fused step, the split "
                          "API and forward-only calls; same inputs, so every step of a kind must reproduce its first result "
@@ -339,6 +342,51 @@ def main() -> int:
                         db=abs(db - mine["dbias"]) / abs(mine["dbias"])))
             if not same_k:
                 eng.close()
+
+    # ---- extra captions with ids: an extra of one rank is a positive for the images with its id on every rank; the
+    # ids travel with the text through the peer pulls --------------------------------------------------------------
+    if args.extra_texts:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from extra_text_ids_oracle import closed_form_extra_text_ids
+        Bs = [160 + 24 * r for r in range(world)]
+        K, D, tp, bias = 300, 136, math.log(10.0), -8.0
+        g = torch.Generator().manual_seed(4343)
+        unit = lambda n: torch.nn.functional.normalize(torch.randn(n, D, generator=g)).to(torch.bfloat16)  # noqa: E731
+        imgs, txts, extras = [unit(b) for b in Bs], [unit(b) for b in Bs], [unit(K) for _ in Bs]
+        ids = list(torch.split(torch.arange(sum(Bs), dtype=torch.int64) * 2, Bs))
+        # extra j of rank r: a caption of image j of rank (r + 1) % world (its id), every fourth one an id no image has
+        eids = []
+        for r in range(world):
+            own = ids[(r + 1) % world]
+            e = own[torch.arange(K) % len(own)].clone()
+            e[::4] = -1 - torch.arange(len(e[::4]))
+            eids.append(e)
+        ref = closed_form_extra_text_ids([x.float().numpy() for x in imgs], [x.float().numpy() for x in txts],
+                                         [x.float().numpy() for x in extras], [x.numpy() for x in ids],
+                                         [x.numpy() for x in eids], tp, bias)
+        mine = ref[rank]
+        dtxt_ref = torch.from_numpy(sum(ref[r]["contrib"][rank] for r in range(world)))
+        img, txt, ext = imgs[rank].to(dev), txts[rank].to(dev), extras[rank].to(dev)
+        for fused in (None, False):
+            modx = DDPSigmoidLoss(Bs[rank], fused_step=fused, batch_per_rank=Bs, multi_positive=True,
+                                  extra_texts=K).to(dev)
+            with torch.no_grad():
+                modx.t_prime.fill_(tp)
+                modx.bias.fill_(bias)
+            for rep in range(2):
+                modx.zero_grad()
+                a, b, e = (x.float().requires_grad_(True) for x in (img, txt, ext))
+                l2 = modx(a, b, sample_ids=ids[rank].to(dev), extra_text=e, extra_text_ids=eids[rank].to(dev))
+                l2.backward()
+                torch.cuda.synchronize()
+                gt = torch.cat([b.grad, e.grad])
+                report(f"extra texts {fused} B={Bs} K={K} D={D} rep{rep}", dict(
+                    loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
+                    dimg=rel_f(a.grad.float().cpu(), torch.from_numpy(mine["dimg"])),
+                    dtxt=rel_f(gt.float().cpu(), dtxt_ref),
+                    dextra=rel_f(e.grad.float().cpu(), dtxt_ref[Bs[rank]:]),
+                    dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
+                    db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
 
     # ---- larger: fp32 autograd; dtxt reference summed over ranks ------------------------------------------
     B, D, tp, bias = 2048, 768, math.log(10.0), -10.0
