@@ -36,6 +36,7 @@ EXPORTED_SYMBOLS = (
     "siglip_fwd",
     "siglip_set_sample_ids",
     "siglip_set_extra_text_ids",
+    "siglip_set_sample_weights",
     "siglip_request_metrics",
     "siglip_fwd_bwd_host",
     "siglip_convert_f32",
@@ -56,6 +57,7 @@ EXPORTED_SYMBOLS = (
     "siglip_debug_set_text_chunk",
     "siglip_debug_get_slot",
     "siglip_debug_set_chunk_ids",
+    "siglip_debug_set_chunk_weights",
     "siglip_debug_set_mailbox",
     "siglip_debug_set_peer_metric_keys",
     "siglip_ctx_aux_trace",
@@ -90,6 +92,7 @@ SIGLIP_OPT_PDL = 19
 SIGLIP_OPT_TPRIME_F64 = 20
 SIGLIP_OPT_SAMPLE_IDS = 21
 SIGLIP_OPT_EXTRA_TEXT_IDS = 22
+SIGLIP_OPT_SAMPLE_WEIGHTS = 23
 
 _lib: Optional[ctypes.CDLL] = None
 
@@ -197,6 +200,10 @@ def lib() -> ctypes.CDLL:
     L.siglip_set_extra_text_ids.restype = ci
     L.siglip_debug_set_chunk_ids.argtypes = [vp, ci, vp, vp]
     L.siglip_debug_set_chunk_ids.restype = ci
+    L.siglip_set_sample_weights.argtypes = [vp, vp, vp, vp]
+    L.siglip_set_sample_weights.restype = ci
+    L.siglip_debug_set_chunk_weights.argtypes = [vp, ci, vp, vp]
+    L.siglip_debug_set_chunk_weights.restype = ci
     L.siglip_request_metrics.argtypes = [vp, vp, vp, vp]
     L.siglip_request_metrics.restype = ci
     L.siglip_debug_set_peer_metric_keys.argtypes = [vp, ci, vp, vp]

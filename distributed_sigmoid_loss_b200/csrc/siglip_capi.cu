@@ -193,6 +193,8 @@ struct siglip_ctx {
   bool ids_set = false;                  // siglip_set_sample_ids was called since the previous step
   int extra_text_ids = 0;                // SIGLIP_OPT_EXTRA_TEXT_IDS: the extras carry ids too (needs sample_ids)
   bool extra_ids_set = false;            // siglip_set_extra_text_ids was called since the previous step
+  int sample_weights = 0;                // SIGLIP_OPT_SAMPLE_WEIGHTS: per-sample loss weights (collective)
+  bool weights_set = false;              // siglip_set_sample_weights was called since the previous step
   int off[kMaxWorld + 1] = {};           // global index of every rank's first sample (prefix sums of Bs)
   // retrieval metrics (siglip_request_metrics), armed for the next step only
   bool metrics_armed = false;
@@ -212,6 +214,11 @@ struct siglip_ctx {
                                          // Fixed at creation (options are set after the handle exchange)
   unsigned long long* mkeys[2] = {};     // per step parity: [world][Tmax] column argmax partials of every text chunk
                                          // over my images, then [Bmax] row keys. world > 1: behind ids_all (exported)
+  float* w_all = nullptr;                // [world][w_stride] text weights of every chunk (world > 1): behind the metric
+                                         // keys in the exported allocation, sized at creation whatever the options
+  float* w_in = nullptr;                 // [w_stride] my text weights, then [B] my image weights, clamped into [0, 1];
+                                         // allocated by the first siglip_set_sample_weights
+  int w_stride = 0;                      // Tmax rounded up to 4: every slot is a whole number of 16-byte vectors
   __nv_bfloat16* G[kMaxWorld] = {};      // [Bp, Tp] sigma operands (fp16 bits x kGScale), diagonal zeroed, allocated on
                                          // first use: fused step 2 (own chunk + the chunk in flight), split API one per chunk
   __nv_bfloat16* img16 = nullptr;        // [B, D] fp16 (x kXScale) images: B operand of the dtxt contraction
@@ -317,18 +324,34 @@ inline int chunk_id_count(const siglip_ctx* c, int rank) { return c->extra_text_
 inline size_t chunk_ids_bytes(const siglip_ctx* c, int rank) {
   return static_cast<size_t>(chunk_id_count(c, rank)) * sizeof(int64_t);
 }
-// ids of step s are given once: a step in ids mode consumes them (checked before anything is launched)
+// ids and weights of step s are given once: a step in ids / weights mode consumes them (all checked before anything is
+// launched or consumed)
 int take_ids(siglip_ctx* c) {
-  if (!c->sample_ids) return 0;
-  if (!c->ids_set)
+  if (c->sample_ids && !c->ids_set)
     return fail(SIGLIP_ERR_STATE,
                 "SIGLIP_OPT_SAMPLE_IDS is on but siglip_set_sample_ids was not called since the previous step");
-  if (c->extra_text_ids && !c->extra_ids_set)
+  if (c->sample_ids && c->extra_text_ids && !c->extra_ids_set)
     return fail(SIGLIP_ERR_STATE,
                 "SIGLIP_OPT_EXTRA_TEXT_IDS is on but siglip_set_extra_text_ids was not called since the previous step");
+  if (c->sample_weights && !c->weights_set)
+    return fail(SIGLIP_ERR_STATE,
+                "SIGLIP_OPT_SAMPLE_WEIGHTS is on but siglip_set_sample_weights was not called since the previous step");
   c->ids_set = false;
   c->extra_ids_set = false;
+  c->weights_set = false;
   return 0;
+}
+
+// ---- per-sample weights (SIGLIP_OPT_SAMPLE_WEIGHTS) ----
+// Text weights of chunk `cidx` as the loss kernel reads them (null outside the mode): mine for the own chunk, the
+// gathered copy for the others; the image weights are always mine (rows are local)
+inline const float* chunk_weights(const siglip_ctx* c, int cidx) {
+  if (!c->sample_weights) return nullptr;
+  return (cidx == c->rank) ? c->w_in : c->w_all + static_cast<size_t>(cidx) * c->w_stride;
+}
+inline const float* image_weights(const siglip_ctx* c) { return c->sample_weights ? c->w_in + c->w_stride : nullptr; }
+inline size_t chunk_weights_bytes(const siglip_ctx* c, int rank) {
+  return static_cast<size_t>(c->Ts[rank]) * sizeof(float);
 }
 inline unsigned long long peer_timeout_ns(const siglip_ctx* c) {
   return static_cast<unsigned long long>(c->peer_timeout_ms) * 1000000ull;
@@ -345,6 +368,15 @@ inline size_t mkeys_rows(const siglip_ctx* c) { return static_cast<size_t>(c->wo
 // byte offset of the two key blocks in the exported text allocation: behind the gathered text and ids
 inline size_t mkeys_offset(const siglip_ctx* c) {
   return chunk_stride(c) * c->world * sizeof(__nv_bfloat16) + static_cast<size_t>(c->world) * c->ids_stride * sizeof(int64_t);
+}
+// byte offset of the text-weight slots in the exported text allocation: behind the two key blocks
+inline size_t weights_offset(const siglip_ctx* c) {
+  return mkeys_offset(c) + 2 * mkeys_block(c) * sizeof(unsigned long long);
+}
+// Rank o's published text-weight slot, seen through its exported text allocation
+inline const float* peer_weights(const siglip_ctx* c, int o) {
+  return reinterpret_cast<const float*>(reinterpret_cast<const char*>(c->peer_txt[o]) + weights_offset(c)) +
+         static_cast<size_t>(o) * c->w_stride;
 }
 // A metrics step starts (armed by siglip_request_metrics for this step only): the key block of the step's parity is
 // zeroed, so that no max of an earlier step survives. Double-buffered by parity: a peer may still read my partials of
@@ -527,6 +559,10 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
     // the chunk's ids cover its paired texts, and under SIGLIP_OPT_EXTRA_TEXT_IDS its extras too
     p.col_pos_n = chunk_id_count(c, cidx);
   }
+  if (c->sample_weights) {   // the kWeights instantiation: w_ij = image weight i x text weight j of the chunk
+    p.row_w = image_weights(c);
+    p.col_w = chunk_weights(c, cidx);
+  }
   if (c->mkeys_step != nullptr) {   // a metrics step: the kMetrics instantiation reduces the argmax keys
     p.row_keys = c->mkeys_step + mkeys_rows(c);
     p.col_keys = c->mkeys_step + static_cast<size_t>(cidx) * c->Tmax;
@@ -576,6 +612,16 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
   return 0;
 }
 
+// the fp16 image copy (B operand of the dtxt contraction)
+void add_img_cvt_job(siglip_ctx* c, AuxList& aux, const void* img) {
+  if (c->dbg_no_cvt) return;
+  siglip::AuxJob& ji = aux.add(siglip::kAuxCvt);
+  ji.src = reinterpret_cast<const uint4*>(img);
+  ji.dst = reinterpret_cast<uint4*>(c->img16);
+  ji.n16 = static_cast<unsigned long long>(c->B) * c->D * sizeof(__nv_bfloat16) / 16;
+  ji.cvt_copy = c->input_f16;
+}
+
 // auxiliary jobs of a saving loss kernel: bf16 -> fp16 x 16 copies of the chunk's text (and, on the own chunk, of the
 // images) for the gradient kernel
 void add_cvt_jobs(siglip_ctx* c, AuxList& aux, int gi, bool own, const void* img, const __nv_bfloat16* txt_c, int Bn) {
@@ -585,13 +631,7 @@ void add_cvt_jobs(siglip_ctx* c, AuxList& aux, int gi, bool own, const void* img
   jt.dst = reinterpret_cast<uint4*>(c->txt16[gi]);
   jt.n16 = static_cast<unsigned long long>(Bn) * c->D * sizeof(__nv_bfloat16) / 16;
   jt.cvt_copy = c->input_f16;
-  if (own) {
-    siglip::AuxJob& ji = aux.add(siglip::kAuxCvt);
-    ji.src = reinterpret_cast<const uint4*>(img);
-    ji.dst = reinterpret_cast<uint4*>(c->img16);
-    ji.n16 = static_cast<unsigned long long>(c->B) * c->D * sizeof(__nv_bfloat16) / 16;
-    ji.cvt_copy = c->input_f16;
-  }
+  if (own) add_img_cvt_job(c, aux, img);
 }
 
 struct GradOut {
@@ -756,6 +796,25 @@ void add_pull_job(siglip_ctx* c, AuxList& aux, int o, unsigned int s) {
     ji.dst = reinterpret_cast<uint4*>(c->ids_all + static_cast<size_t>(o) * c->ids_stride);
     ji.n16 = (chunk_ids_bytes(c, o) + 15) / 16;   // within the slot: ids_stride is even
   }
+  if (c->sample_weights) {
+    // the chunk's text weights ride the same flag, like its ids
+    siglip::AuxJob& jw = aux.add(siglip::kAuxCopy);
+    jw.src = reinterpret_cast<const uint4*>(peer_weights(c, o));
+    jw.dst = reinterpret_cast<uint4*>(c->w_all + static_cast<size_t>(o) * c->w_stride);
+    jw.n16 = (chunk_weights_bytes(c, o) + 15) / 16;   // within the slot: w_stride is a multiple of 4
+  }
+}
+
+// publish job of my text weights (L0 of the fused step), the twin of the ids publish job below
+void add_weights_publish_job(siglip_ctx* c, AuxList& aux, unsigned int s) {
+  siglip::AuxJob& j = aux.add(siglip::kAuxCopy);
+  j.src = reinterpret_cast<const uint4*>(c->w_in);
+  j.dst = reinterpret_cast<uint4*>(c->w_all + static_cast<size_t>(c->rank) * c->w_stride);
+  j.n16 = (chunk_weights_bytes(c, c->rank) + 15) / 16;
+  j.wait_flags = c->flags + 2 * kMaxWorld;
+  j.wait_n = c->world;
+  j.wait_value = s - 1;
+  j.site = 11;
 }
 
 // publish job of my ids (L0 of the fused step): same flag-2 wait as the text publish job that must follow it in the
@@ -771,11 +830,14 @@ void add_ids_publish_job(siglip_ctx* c, AuxList& aux, unsigned int s) {
   j.site = 11;
 }
 
-// the same publish as a stream copy (split forward, helper-kernel variant of the fused step)
-int copy_own_ids(siglip_ctx* c, cudaStream_t st) {
-  if (!c->sample_ids) return 0;
-  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(c->rank) * c->ids_stride, c->ids_in, chunk_ids_bytes(c, c->rank),
-                     cudaMemcpyDeviceToDevice, st));
+// the same publishes (ids, text weights) as stream copies (split forward, helper-kernel variant of the fused step)
+int copy_own_chunk_data(siglip_ctx* c, cudaStream_t st) {
+  if (c->sample_ids)
+    CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(c->rank) * c->ids_stride, c->ids_in,
+                       chunk_ids_bytes(c, c->rank), cudaMemcpyDeviceToDevice, st));
+  if (c->sample_weights)
+    CK(cudaMemcpyAsync(c->w_all + static_cast<size_t>(c->rank) * c->w_stride, c->w_in, chunk_weights_bytes(c, c->rank),
+                       cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
@@ -807,7 +869,7 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
     if ((rc = wait_peers(c, 2, s - 1, st))) return rc;
     CK(cudaMemcpyAsync(c->txt_all + r * stride, txt, static_cast<size_t>(c->T) * c->D * sizeof(__nv_bfloat16),
                        cudaMemcpyDeviceToDevice, st));
-    if ((rc = copy_own_ids(c, st))) return rc;   // before the signal, which covers it
+    if ((rc = copy_own_chunk_data(c, st))) return rc;   // before the signal, which covers it
     if ((rc = signal_peers(c, 0, s, st))) return rc;
     own_txt = c->txt_all + r * stride;
   }
@@ -834,6 +896,9 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
         if (c->sample_ids)
           CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(nxt) * c->ids_stride, peer_ids(c, nxt),
                              chunk_ids_bytes(c, nxt), cudaMemcpyDefault, st));
+        if (c->sample_weights)
+          CK(cudaMemcpyAsync(c->w_all + static_cast<size_t>(nxt) * c->w_stride, peer_weights(c, nxt),
+                             chunk_weights_bytes(c, nxt), cudaMemcpyDefault, st));
       }
     }
     if ((rc = run_loss_chunk(c, k, cidx, k == 0, k == 0, img, txt_c, c->Ts[cidx], chunk_ids(c, cidx), t_prime, bias, save,
@@ -980,6 +1045,9 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   fin.loss = loss;
   fin.dt_prime = c->scalars + kSavedScalars;
   fin.dbias = c->scalars + kSavedScalars + 1;
+  // With ids and weights, L0 would carry 9 jobs (3 publishes, 2 conversions, the flag-3 wait, 3 pulls) of
+  // kMaxAuxJobs = 8: the image conversion then runs in L1 instead (its first reader is G1, behind L1).
+  const bool img_cvt_in_l1 = W > 1 && ik && c->sample_ids && c->sample_weights;
 
   // ---- L0: own chunk. Its auxiliary warps also publish my text to the peers and start the first pull ----
   {
@@ -988,9 +1056,10 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       if (ik) {
         // my gathered slot is what the peers pull: they must be done with the previous forward's copy (flag 2),
         // then "text of forward s in place" (flag 0) goes to every rank once all CTAs have copied their share. My
-        // ids (sample-id mode) are copied by a job before it: each CTA finishes both before the text job's ticket, so
-        // the same signal covers them.
+        // ids (sample-id mode) and text weights (weights mode) are copied by jobs before it: each CTA finishes them
+        // before the text job's ticket, so the same signal covers them.
         if (c->sample_ids) add_ids_publish_job(c, aux, s);
+        if (c->sample_weights) add_weights_publish_job(c, aux, s);
         siglip::AuxJob& cp = aux.add(siglip::kAuxCopy);
         cp.src = reinterpret_cast<const uint4*>(txt);
         cp.dst = reinterpret_cast<uint4*>(c->txt_all + r * stride);
@@ -1005,11 +1074,11 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       } else {
         if ((rc = wait_peers(c, 2, s - 1, st))) return rc;
         CK(cudaMemcpyAsync(c->txt_all + r * stride, txt, own_bytes, cudaMemcpyDeviceToDevice, st));
-        if ((rc = copy_own_ids(c, st))) return rc;
+        if ((rc = copy_own_chunk_data(c, st))) return rc;
         if ((rc = signal_peers(c, 0, s, st))) return rc;
       }
     }
-    add_cvt_jobs(c, aux, 0, true, img, own_txt, c->T);
+    add_cvt_jobs(c, aux, 0, !img_cvt_in_l1, img, own_txt, c->T);
     if (W > 1) {
       if (ik) {
         // my contribution slots of the previous backward must have been read by their owners (flag 3) before G1
@@ -1036,7 +1105,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
     const __nv_bfloat16* txt_c = c->txt_all + cidx * stride;
     {
       AuxList aux;
-      add_cvt_jobs(c, aux, 1, false, img, txt_c, c->Ts[cidx]);
+      add_cvt_jobs(c, aux, 1, k == 1 && img_cvt_in_l1, img, txt_c, c->Ts[cidx]);
       if (k + 1 < W) add_pull_job(c, aux, step_owner(c, r, k + 1), s);
       const bool lastL = (k == W - 1);
       EndSignal end = (lastL && ik) ? end_signal(c, 2, s) : EndSignal();   // "I have pulled everyone's text"
@@ -1223,14 +1292,18 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   const size_t ids_slot_bytes = static_cast<size_t>(c->ids_stride) * sizeof(int64_t);
   CK(alloc(reinterpret_cast<void**>(&c->ids_in), ids_slot_bytes));
   const size_t mkeys_bytes = 2 * mkeys_block(c) * sizeof(unsigned long long);
+  c->w_stride = round_up(Tmax, 4);
   if (world > 1) {
-    // the gathered ids and the two metric key blocks live behind the gathered text, so that one exported handle covers
-    // all three
+    // the gathered ids, the two metric key blocks and the gathered text weights live behind the gathered text, so that
+    // one exported handle covers all four (SIGLIP_OPT_SAMPLE_WEIGHTS may be set after the handle exchange, so the
+    // weight slots exist whatever the options)
+    const size_t w_bytes = static_cast<size_t>(world) * c->w_stride * sizeof(float);
     CK(alloc(reinterpret_cast<void**>(&c->txt_all),
-             stride * world * sizeof(__nv_bfloat16) + world * ids_slot_bytes + mkeys_bytes));
+             stride * world * sizeof(__nv_bfloat16) + world * ids_slot_bytes + mkeys_bytes + w_bytes));
     c->ids_all = reinterpret_cast<int64_t*>(c->txt_all + stride * world);   // 16-byte aligned: D % 8 == 0
     c->mkeys[0] = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(c->txt_all) + mkeys_offset(c));
     c->mkeys[1] = c->mkeys[0] + mkeys_block(c);
+    c->w_all = reinterpret_cast<float*>(reinterpret_cast<char*>(c->txt_all) + weights_offset(c));
     CK(alloc(reinterpret_cast<void**>(&c->slots), stride * world * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dimg_acc), static_cast<size_t>(c->B) * D * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dtxt_acc), static_cast<size_t>(c->T) * D * sizeof(float)));
@@ -1325,6 +1398,10 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_EXTRA_TEXT_IDS needs SIGLIP_OPT_SAMPLE_IDS on first");
       c->extra_text_ids = value ? 1 : 0;
       c->extra_ids_set = false;
+      return 0;
+    case SIGLIP_OPT_SAMPLE_WEIGHTS:
+      c->sample_weights = value ? 1 : 0;
+      c->weights_set = false;
       return 0;
     case SIGLIP_OPT_STAGES_LOSS:
     case SIGLIP_OPT_STAGES_GRAD:
@@ -1505,6 +1582,36 @@ int siglip_set_extra_text_ids(siglip_ctx* c, const int64_t* ids_dev, void* cuda_
   return 0;
 }
 
+// the weight buffer of my chunk and images, allocated on the first call like the metric keys (so a context that never
+// uses weights holds the workspace it held without them; allowed inside a CUDA-graph capture)
+static int ensure_weights(siglip_ctx* c) {
+  if (c->w_in != nullptr) return 0;
+  const size_t bytes = (static_cast<size_t>(c->w_stride) + c->B) * sizeof(float);
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  CK(cudaThreadExchangeStreamCaptureMode(&mode));
+  float* w = nullptr;
+  const cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&w), bytes);
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  CK(e);
+  c->w_in = w;
+  c->workspace_bytes += bytes;
+  return 0;
+}
+
+int siglip_set_sample_weights(siglip_ctx* c, const float* image_w, const float* text_w, void* cuda_stream) {
+  if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "ctx is null");
+  if (!c->sample_weights)
+    return fail(SIGLIP_ERR_STATE, "siglip_set_sample_weights needs SIGLIP_OPT_SAMPLE_WEIGHTS = 1");
+  CK(cudaSetDevice(c->device));
+  int rc;
+  if ((rc = ensure_weights(c))) return rc;
+  CKI(siglip::launch_clamp_weights(text_w, c->w_in, c->T, image_w, c->w_in + c->w_stride, c->B,
+                                   static_cast<cudaStream_t>(cuda_stream)));
+  c->launches++;
+  c->weights_set = true;
+  return 0;
+}
+
 int siglip_request_metrics(siglip_ctx* c, float* top1, int64_t* i2t_index, int64_t* t2i_index) {
   if (c == nullptr || top1 == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument (top1 is required)");
   if (c->mkeys[0] == nullptr) {
@@ -1627,6 +1734,9 @@ int siglip_host_submit_grads(siglip_ctx* c, const void* img_host, const void* tx
                 "(siglip_ctx_create_texts with texts_per_rank != images_per_rank)");
   if (c->metrics_armed)
     return fail(SIGLIP_ERR_STATE, "the host-buffer entries return no retrieval metrics: siglip_request_metrics is armed");
+  if (c->sample_weights)
+    return fail(SIGLIP_ERR_STATE,
+                "the host-buffer entries take no sample weights: unavailable under SIGLIP_OPT_SAMPLE_WEIGHTS");
   const bool with_grads = dimg_host_bf16 != nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   CK(cudaSetDevice(c->device));
@@ -1793,6 +1903,16 @@ int siglip_debug_set_chunk_ids(siglip_ctx* c, int chunk, const int64_t* ids_dev,
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
   CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * c->ids_stride, ids_dev, chunk_ids_bytes(c, chunk),
                      cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
+  return 0;
+}
+
+int siglip_debug_set_chunk_weights(siglip_ctx* c, int chunk, const float* text_w_dev, void* cuda_stream) {
+  if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "ctx is null");
+  if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
+  // clamped like the owner's siglip_set_sample_weights (NULL = ones)
+  CKI(siglip::launch_clamp_weights(text_w_dev, c->w_all + static_cast<size_t>(chunk) * c->w_stride, c->Ts[chunk],
+                                   nullptr, nullptr, 0, static_cast<cudaStream_t>(cuda_stream)));
+  c->launches++;
   return 0;
 }
 
@@ -2044,6 +2164,7 @@ void free_ctx(siglip_ctx* c) {
   }
   cudaFree(c->g_diag);
   cudaFree(c->ids_in);
+  cudaFree(c->w_in);   // w_all: part of txt_all
   cudaFree(c->img16);
   cudaFree(c->slots);
   cudaFree(c->dimg_acc);

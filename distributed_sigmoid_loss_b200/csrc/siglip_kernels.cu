@@ -266,13 +266,23 @@ __device__ __forceinline__ void store_g_slab(const GStore& gs, int col0, const u
   }
 }
 
+// Weight of fragment element i = 4 j + 2 h + e1 (row half h, column 8 j + e1) of a slab (SIGLIP_OPT_SAMPLE_WEIGHTS):
+// the thread's row weight times the column weight cw[2 j + e1]
+__device__ __forceinline__ float slab_w(int i, const float* cw, float rw0, float rw1) {
+  return (((i >> 1) & 1) ? rw1 : rw0) * cw[2 * (i >> 2) + (i & 1)];
+}
+
 // Fast path: every z of the slab is < kFastZ, so e = exp(z) < 2^-6 and both sigma(z) = e / (1 + e) and log1p(e) are
 // evaluated by their alternating series on the FMA pipe (truncation < 3.4e-6 relative at the edge of the path, < 1e-8
 // for the z ~ -10 of a SigLIP batch; the tolerance is 1e-3). One MUFU (ex2) per element instead of two: the epilogue
 // is bound by the MUFU and FMA pipes.
+// kW (SIGLIP_OPT_SAMPLE_WEIGHTS): element i has weight slab_w(i, cw, rw0, rw1); it scales e where e multiplies into both
+// terms, so a weight of exactly 1 leaves every value bit-identical to the unweighted path.
+template <bool kW = false>
 __device__ __forceinline__ void loss_slab_fast(const float* v, float tl, float bl, int col0, bool store_g,
                                                const GStore& gst, float gscale, float& acc_sp, float& acc_g,
-                                               float& acc_gs) {
+                                               float& acc_gs, const float* cw = nullptr, float rw0 = 1.f,
+                                               float rw1 = 1.f) {
   uint32_t packed[8];
   float a_sp = 0.f, a_g = 0.f, a_gs = 0.f;
   float g_prev = 0.f;
@@ -280,14 +290,16 @@ __device__ __forceinline__ void loss_slab_fast(const float* v, float tl, float b
   for (int i = 0; i < 16; ++i) {
     const float s = v[i];
     const float e = ex2_approx(fmaf(s, tl, bl));        // exp(z), z < kFastZ
+    float ew = e;
+    if constexpr (kW) ew = e * slab_w(i, cw, rw0, rw1);
     // sigma is produced already multiplied by the power-of-two scale of the 16-bit operand (exact), and the two sums
     // that use it are un-scaled once per slab
     float q = fmaf(e, gscale, -gscale);                  // S sigma(z) / e = S (1 - e + e^2)  [- e^3 < 3.8e-6 dropped]
     q = fmaf(e, q, gscale);
-    const float g = e * q;                               // S sigma(z)
+    const float g = ew * q;                              // S sigma(z) (x w)
     float l = fmaf(e, 0.33333334f, -0.5f);               // log1p(e) / e = 1 - e/2 + e^2/3    [- e^3/4 < 1e-6 dropped]
     l = fmaf(e, l, 1.0f);
-    a_sp = fmaf(e, l, a_sp);
+    a_sp = fmaf(ew, l, a_sp);
     a_g += g;
     a_gs = fmaf(g, s, a_gs);
     // element i = 4 j + e': row half e' >> 1, column e' & 1 -> packed[2 j + (e' >> 1)]
@@ -305,10 +317,12 @@ __device__ __forceinline__ void loss_slab_fast(const float* v, float tl, float b
 
 // General path. row_lo: global row of this thread's first fragment row; col0: global column of the slab; c_lo as above.
 // pos (kMask only): bit i set = element i is a positive pair by sample id (SIGLIP_OPT_SAMPLE_IDS); 0 without ids.
-template <bool kMask>
+// kW: element i's weight multiplies its three terms once its label is applied (x * 1 == x: unit weights change no bit).
+template <bool kMask, bool kW = false>
 __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int row_lo, int col0, int c_lo, int nrows,
                                           int ncols, bool store_g, const GStore& gst, float gscale, float* g_diag,
-                                          bool on_diag, uint32_t pos, float& acc_sp, float& acc_g, float& acc_gs) {
+                                          bool on_diag, uint32_t pos, float& acc_sp, float& acc_g, float& acc_gs,
+                                          const float* cw = nullptr, float rw0 = 1.f, float rw1 = 1.f) {
   uint32_t packed[8];
   float g_prev = 0.f;
 #pragma unroll
@@ -331,7 +345,12 @@ __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int 
         sp = fmaxf(-z, 0.f) + l;
         g = -((z >= 0.f) ? e * r : r);                 // sigma(-z) without the 1 - sigma(z) cancellation
         g_store = 0.f;                                 // the own diagonal stays out of the 16-bit operand
-        if (store_g && valid) g_diag[row] = g;
+        if (store_g && valid) {
+          if constexpr (kW)
+            g_diag[row] = g * slab_w(i, cw, rw0, rw1);
+          else
+            g_diag[row] = g;
+        }
       } else if ((pos >> i) & 1u) {                    // any other positive (same sample id): same terms, and its
         sp = fmaxf(-z, 0.f) + l;                       // g * 2^14 in [-16384, 0) goes into the fp16 operand
         g = -((z >= 0.f) ? e * r : r);
@@ -340,6 +359,12 @@ __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int 
       sp = valid ? sp : 0.f;
       g = valid ? g : 0.f;
       g_store = valid ? g_store : 0.f;
+    }
+    if constexpr (kW) {
+      const float w = slab_w(i, cw, rw0, rw1);
+      sp *= w;
+      g *= w;
+      g_store *= w;
     }
     acc_sp += sp;
     acc_g += g;
@@ -604,7 +629,10 @@ __device__ __forceinline__ void mma_loop_f8(float (&sum)[64], float (&acc)[64], 
 // loss kernel is exactly the code it was without the option.
 // kMetrics: the loss kernel that also reduces the row / column argmax keys of every tile (siglip_request_metrics); its
 // own instantiation for the same reason.
-template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false>
+// kWeights: the loss kernel with per-sample weights (SIGLIP_OPT_SAMPLE_WEIGHTS); its own instantiation for the same
+// reason, composing with kIds and kMetrics.
+template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false,
+          bool kWeights = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
                    const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1,
@@ -613,6 +641,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
   static_assert(kCS == 1 || kCS == 2 || kCS == 4, "clusters of 1, 2 or 4 CTAs");
   static_assert(!kIds || kMode == kModeLoss, "sample ids are a loss-kernel option");
   static_assert(!kMetrics || kMode == kModeLoss, "retrieval metrics are a loss-kernel option");
+  static_assert(!kWeights || kMode == kModeLoss, "sample weights are a loss-kernel option");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -844,10 +873,23 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
           rid0 = p.row_ids[min(row_lo, pr.M - 1)];
           rid1 = p.row_ids[min(row_lo + 8, pr.M - 1)];
         }
+        // Sample weights (kWeights): the weights of the two fragment rows, once per tile (clamped like the ids)
+        float rw0 = 1.f, rw1 = 1.f;
+        if constexpr (kWeights) {
+          rw0 = p.row_w[min(row_lo, pr.M - 1)];
+          rw1 = p.row_w[min(row_lo + 8, pr.M - 1)];
+        }
 #pragma unroll
         for (int c = 0; c < kTileN / 32; ++c) {
           const float* v = acc + 16 * c;
           const int col0 = col_base + 32 * c;
+          // kWeights: the slab's 8 column weights of this thread, cw[2 j + e1] for column 8 j + c_lo + e1 (a column
+          // beyond N reads column N - 1: it only lies in edge slabs, which mask it)
+          float cw[kWeights ? 8 : 1];
+          if constexpr (kWeights) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) cw[j] = p.col_w[min(col0 + 8 * (j >> 1) + c_lo + (j & 1), pr.N - 1)];
+          }
           // Only the 16x32 slabs that touch the diagonal of a diagonal block hold positive pairs, and only the slabs
           // that cross the matrix border of an edge block need masking; every other slab takes the fast path like
           // the rest of the matrix.
@@ -879,13 +921,13 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
             for (int j = 1; j < 16; ++j) smax = fmaxf(smax, v[j]);
             const bool fast = __all_sync(0xffffffffu, fmaf(smax, t_eff, bias) < kFastZ);
             if (fast)
-              loss_slab_fast(v, tl, bl, col0, sg, gst, p.g_scale, acc_sp, acc_g, acc_gs);
+              loss_slab_fast<kWeights>(v, tl, bl, col0, sg, gst, p.g_scale, acc_sp, acc_g, acc_gs, cw, rw0, rw1);
             else
-              loss_slab<false>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag, false,
-                               0u, acc_sp, acc_g, acc_gs);
+              loss_slab<false, kWeights>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag,
+                                         false, 0u, acc_sp, acc_g, acc_gs, cw, rw0, rw1);
           } else {
-            loss_slab<true>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag, slab_diag,
-                            pos, acc_sp, acc_g, acc_gs);
+            loss_slab<true, kWeights>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag,
+                                      slab_diag, pos, acc_sp, acc_g, acc_gs, cw, rw0, rw1);
           }
         }
         kahan_add(s_sp, c_sp, acc_sp);
@@ -1594,12 +1636,15 @@ __global__ void normalize_bwd_kernel(const void* __restrict__ x, const float* __
   }
 }
 
-// kIds / kMetrics select the sample-id / retrieval-metrics instantiations of the loss kernel (ignored for the out kernel)
-template <int kMode, int kStages, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false>
+// kIds / kMetrics / kWeights select the sample-id / retrieval-metrics / sample-weight instantiations of the loss kernel
+// (ignored for the out kernel)
+template <int kMode, int kStages, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false,
+          bool kWeights = false>
 int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensorMap* tmA1, const CUtensorMap* tmB1,
                 const CUtensorMap* tmG, const KernelParams& p, int num_sms, cudaStream_t stream) {
   using C = Cfg<kMode, kStages>;
-  auto kern = siglip_gemm_kernel<kMode, kStages, kCS, kF8, kIds && kMode == kModeLoss, kMetrics && kMode == kModeLoss>;
+  auto kern = siglip_gemm_kernel<kMode, kStages, kCS, kF8, kIds && kMode == kModeLoss, kMetrics && kMode == kModeLoss,
+                                 kWeights && kMode == kModeLoss>;
   static bool attr_set = false;
   cudaError_t e = cudaSuccess;
   if (!attr_set) {
@@ -1716,10 +1761,16 @@ size_t gemm_smem_bytes(int mode) {
                            : static_cast<size_t>(Cfg<kModeOut, 6>::kSmemBytes);
 }
 
-// the out kernel never has ids or metric keys, so only the loss kernel takes the three extra instantiations
+// the out kernel never has ids, metric keys or weights, so only the loss kernel takes the seven extra instantiations
 #define SIGLIP_LAUNCH(MODE, ST, CS)                                                                          \
   do {                                                                                                       \
     const bool ids__ = p.row_ids != nullptr, met__ = p.row_keys != nullptr;                                  \
+    if (MODE == kModeLoss && p.row_w != nullptr) {                                                           \
+      if (ids__ && met__) return launch_impl<MODE, ST, CS, false, true, true, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream); \
+      if (met__) return launch_impl<MODE, ST, CS, false, false, true, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);        \
+      if (ids__) return launch_impl<MODE, ST, CS, false, true, false, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);        \
+      return launch_impl<MODE, ST, CS, false, false, false, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);                  \
+    }                                                                                                        \
     if (ids__ && met__) return launch_impl<MODE, ST, CS, false, true, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream); \
     if (met__) return launch_impl<MODE, ST, CS, false, false, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);        \
     if (ids__) return launch_impl<MODE, ST, CS, false, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);               \
@@ -1807,6 +1858,24 @@ int launch_allreduce_scalars(const float* saved, const float* g, float* mailbox_
                              unsigned long long timeout_ns, DebugRecord* dbg, cudaStream_t stream) {
   allreduce_scalars_kernel<<<1, 32, 0, stream>>>(saved, g, mailbox_local, mailboxes_dev, signal_ptrs_dev, flags_local,
                                                  world, value, dt_prime, dbias, dtp_f64, timeout_ns, dbg);
+  return static_cast<int>(cudaGetLastError());
+}
+
+// fmaxf returns the non-NaN operand, so NaN -> 0 and the result is in [0, 1]
+__global__ void clamp_weights_kernel(const float* src_a, float* dst_a, int na, const float* src_b, float* dst_b,
+                                     int nb) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < na + nb; i += gridDim.x * blockDim.x) {
+    const float* src = (i < na) ? src_a : src_b;
+    const int k = (i < na) ? i : i - na;
+    (i < na ? dst_a : dst_b)[k] = (src != nullptr) ? fminf(fmaxf(src[k], 0.f), 1.f) : 1.f;
+  }
+}
+
+int launch_clamp_weights(const float* src_a, float* dst_a, int na, const float* src_b, float* dst_b, int nb,
+                         cudaStream_t stream) {
+  const int n = na + nb;
+  const int blocks = (n + 255) / 256 < 1024 ? (n + 255) / 256 : 1024;
+  clamp_weights_kernel<<<blocks > 0 ? blocks : 1, 256, 0, stream>>>(src_a, dst_a, na, src_b, dst_b, nb);
   return static_cast<int>(cudaGetLastError());
 }
 

@@ -34,7 +34,8 @@ struct Problem {
   long long ld_add;
 };
 
-constexpr int kMaxAuxJobs = 8;   // L0 of a multi-rank step with sample ids carries 7
+constexpr int kMaxAuxJobs = 8;   // L0 of a multi-rank step with sample ids carries 7, with ids and weights 8
+                                 // (DESIGN.md, "Per-sample loss weights")
 enum AuxKind { kAuxNone = 0, kAuxCopy = 1, kAuxCvt = 2, kAuxFold = 3, kAuxWaitOnly = 4 };
 
 // One job of the auxiliary warps. Optional pre-wait on `wait_n` consecutive local flags (all >= wait_value, written by
@@ -140,6 +141,11 @@ struct KernelParams {
   // forward then has the same grid, so the per-CTA partial slots it accumulates and the last one sums line up when the
   // chunks have different sizes (uneven batches, hard negatives). 0 = the chunk's own N.
   int grid_n;
+  // Per-sample loss weights (SIGLIP_OPT_SAMPLE_WEIGHTS), loss kernel only. Appended last like the fields above. Non-null
+  // row_w selects the kWeights instantiation: pair (i, j) contributes w_ij = row_w[i] * col_w[j] times its softplus and
+  // sigma terms, to the three sums, to g_diag and to the stored sigma operand. Both in [0, 1] (clamped on the way in).
+  const float* row_w;   // [M]: this rank's image weights
+  const float* col_w;   // [N]: weights of the texts of the chunk being scored
 };
 
 enum KernelMode { kModeLoss = 0, kModeOut = 1 };
@@ -222,5 +228,10 @@ struct MetricsArgs {
 int launch_metrics_finalize(const MetricsArgs& a, cudaStream_t stream);
 int launch_wait_flags(const volatile unsigned int* flags, int n, unsigned int value, unsigned long long timeout_ns,
                       DebugRecord* dbg, cudaStream_t stream);
+
+// SIGLIP_OPT_SAMPLE_WEIGHTS: dst_a[0, na) = clamp(src_a) and dst_b[0, nb) = clamp(src_b) in one launch, where
+// clamp(x) = min(max(x, 0), 1) and NaN -> 0; a null source gives ones.
+int launch_clamp_weights(const float* src_a, float* dst_a, int na, const float* src_b, float* dst_b, int nb,
+                         cudaStream_t stream);
 
 }  // namespace siglip

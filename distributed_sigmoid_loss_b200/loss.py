@@ -136,6 +136,30 @@ class SigmoidLossEngine:
         with torch.cuda.device(self.device):
             _capi.check(self._L.siglip_set_extra_text_ids(self._h, ids.data_ptr(), self._stream()))
 
+    def set_sample_weights(self, image_weights: Optional[torch.Tensor], text_weights: Optional[torch.Tensor]) -> None:
+        """SIGLIP_OPT_SAMPLE_WEIGHTS: this rank's image weights ([B] fp32) and text weights ([T] fp32: the paired texts,
+        then the extras), contiguous on the engine's device, or None for ones, for the NEXT step. Copied on the current
+        stream with every value clamped into [0, 1] (NaN -> 0), so the tensors may be released or overwritten afterwards."""
+        self._check_weights(image_weights, self.batch)
+        self._check_weights(text_weights, self.texts)
+        with torch.cuda.device(self.device):
+            _capi.check(self._L.siglip_set_sample_weights(
+                self._h, image_weights.data_ptr() if image_weights is not None else None,
+                text_weights.data_ptr() if text_weights is not None else None, self._stream()))
+
+    def debug_set_chunk_weights(self, chunk: int, text_weights: Optional[torch.Tensor]) -> None:
+        """Loopback: the text weights of chunk `chunk` ([T_c] fp32, or None for ones) as its owner would have published
+        them (clamped the same way)."""
+        self._check_weights(text_weights, self.texts_per_rank[chunk])
+        _capi.check(self._L.siglip_debug_set_chunk_weights(
+            self._h, chunk, text_weights.data_ptr() if text_weights is not None else None, self._stream()))
+
+    def _check_weights(self, w: Optional[torch.Tensor], n: int) -> None:
+        if w is not None and (w.dtype != torch.float32 or tuple(w.shape) != (n,) or not w.is_contiguous() or
+                              w.device != self.device):
+            raise RuntimeError(f"sample weights must be a contiguous fp32 [{n}] tensor on {self.device} (or None), got "
+                               f"{tuple(w.shape)} {w.dtype} on {w.device}")
+
     def debug_set_chunk_ids(self, chunk: int, ids: torch.Tensor) -> None:
         """Loopback: the ids of text chunk `chunk` as its owner would have published them: its sample ids ([B_c]), or
         under SIGLIP_OPT_EXTRA_TEXT_IDS the ids of all its texts ([T_c])."""
@@ -454,11 +478,13 @@ class _SigmoidLossFn(torch.autograd.Function):
     ids: [B] int64 sample ids (SIGLIP_OPT_SAMPLE_IDS engines), set before every step the engine runs for this call.
     extra_ids: [T - B] int64 ids of the extra texts (SIGLIP_OPT_EXTRA_TEXT_IDS engines), set along with ids.
     metrics: (top1, i2t_index, t2i_index) output buffers: the retrieval metrics of this call's step are armed. A re-run
-    of the forward by the backward's generation guard does not arm them again (they belong to the first run)."""
+    of the forward by the backward's generation guard does not arm them again (they belong to the first run).
+    weights: (image_weights [B] or None, text_weights [T] or None) fp32 (SIGLIP_OPT_SAMPLE_WEIGHTS engines), set before
+    every step the engine runs for this call, like the ids."""
 
     @staticmethod
     def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool = False, fused: bool = False,
-                ids: Optional[torch.Tensor] = None, metrics=None, extra_ids: Optional[torch.Tensor] = None):
+                ids: Optional[torch.Tensor] = None, metrics=None, extra_ids: Optional[torch.Tensor] = None, weights=None):
         need_grad = any(ctx.needs_input_grad[:4])
         raw = None
         # bf16 callers: bf16 operands (what autograd would multiply). Anything wider (the reference's own test feeds
@@ -492,11 +518,13 @@ class _SigmoidLossFn(torch.autograd.Function):
             b = b.to(device=img.device, dtype=torch.float32)
         b = b.reshape(1)
         ctx.fused = bool(fused and need_grad)
-        ctx.ids, ctx.extra_ids = ids, extra_ids
+        ctx.ids, ctx.extra_ids, ctx.weights = ids, extra_ids, weights
         if ids is not None:
             engine.set_sample_ids(ids)
         if extra_ids is not None:
             engine.set_extra_text_ids(extra_ids)
+        if weights is not None:
+            engine.set_sample_weights(*weights)
         if metrics is not None:
             engine.request_metrics(*metrics)
         if ctx.fused:
@@ -545,11 +573,13 @@ class _SigmoidLossFn(torch.autograd.Function):
             img_b, txt_b, tp, b = saved[:4]
             if eng.saved_generation != ctx.gen:
                 # another forward of the same module ran in between: rebuild the saved state (every rank takes this
-                # branch together, so the collective stays matched); the re-run takes this call's ids again
+                # branch together, so the collective stays matched); the re-run takes this call's ids and weights again
                 if ctx.ids is not None:
                     eng.set_sample_ids(ctx.ids)
                 if ctx.extra_ids is not None:
                     eng.set_extra_text_ids(ctx.extra_ids)
+                if ctx.weights is not None:
+                    eng.set_sample_weights(*ctx.weights)
                 eng.forward(img_b, txt_b, tp, b, True)
                 ctx.gen = eng.saved_generation
             if ctx.normalize:
@@ -566,14 +596,15 @@ class _SigmoidLossFn(torch.autograd.Function):
                 gt = dtxt.to(tdt) if ctx.needs_input_grad[1] else None
         gp = dtp.reshape(pshape).to(device=pdev, dtype=pdt) if ctx.needs_input_grad[2] else None
         gb = db.reshape(bshape).to(device=bdev, dtype=bdt) if ctx.needs_input_grad[3] else None
-        return gi, gt, gp, gb, None, None, None, None, None, None
+        return gi, gt, gp, gb, None, None, None, None, None, None, None
 
 
 class _EngineCache:
     def __init__(self, group=None, cta_group: int = 2, overlap_pull: bool = True, sync_scalar_grads: bool = False,
                  bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
-                 extra_texts: int = 0):
+                 extra_texts: int = 0, sample_weights: bool = False):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
+        self.sample_weights = sample_weights
         self.sync_scalar_grads, self.bidir = sync_scalar_grads, bidir
         self.multi_positive = multi_positive
         self.batch_per_rank = batch_per_rank
@@ -603,6 +634,8 @@ class _EngineCache:
                 eng.set_option(_capi.SIGLIP_OPT_SAMPLE_IDS, 1)
             if self.extra_texts:
                 eng.set_option(_capi.SIGLIP_OPT_EXTRA_TEXT_IDS, 1)   # needs the sample ids on first
+            if self.sample_weights:
+                eng.set_option(_capi.SIGLIP_OPT_SAMPLE_WEIGHTS, 1)
             self._engines[key] = eng
         return eng
 
@@ -689,6 +722,50 @@ def _validate_extra_text_ids(extra_text_ids, extra_texts: int, text_embeddings: 
     if extra_text_ids.device != text_embeddings.device:
         raise RuntimeError(f"extra_text_ids are on {extra_text_ids.device}, the texts on {text_embeddings.device}")
     return extra_text_ids.to(torch.int64).contiguous()
+
+
+def _validate_sample_weights(sample_weights) -> bool:
+    if not isinstance(sample_weights, bool):
+        raise RuntimeError(f"sample_weights must be a bool, got {type(sample_weights).__name__}")
+    return sample_weights
+
+
+def _validate_weights(weights, sample_weights: bool, n: Optional[int], name: str,
+                      device: torch.device) -> Optional[torch.Tensor]:
+    """image_weights / text_weights of a forward: accepted only when the loss was built with sample_weights=True. None
+    means ones; otherwise a floating [n] tensor on the embeddings' device that does not require grad (the weights are
+    inputs: no gradient with respect to them is computed). Returns it as contiguous fp32, or None. Raises before any GPU
+    work. Values outside [0, 1] are clamped into it by the copy (NaN -> 0)."""
+    if not sample_weights:
+        if weights is not None:
+            raise RuntimeError(f"{name} given, but the loss was built without sample_weights=True")
+        return None
+    if weights is None:
+        return None
+    if not isinstance(weights, torch.Tensor) or not weights.is_floating_point():
+        raise RuntimeError(f"{name} must be a floating-point tensor, got "
+                           f"{weights.dtype if isinstance(weights, torch.Tensor) else type(weights).__name__}")
+    if weights.dim() != 1 or weights.shape[0] != n:
+        raise RuntimeError(f"{name} must have shape [{n}], got {tuple(weights.shape)}")
+    if weights.device != device:
+        raise RuntimeError(f"{name} is on {weights.device}, the embeddings on {device}")
+    if weights.requires_grad:
+        raise RuntimeError(f"{name} requires grad, but no gradient with respect to the sample weights is computed: "
+                           f"pass {name}.detach()")
+    return weights.to(torch.float32).contiguous()
+
+
+def _weights_of(sample_weights: bool, image_weights, text_weights, image_embeddings: torch.Tensor,
+                text_embeddings: torch.Tensor, extras: int):
+    """Both weight arguments checked; (image_weights, text_weights) for the step, or None without sample_weights. The
+    texts are the paired ones followed by the K extras, so text_weights has B + K entries."""
+    rows = lambda x: x.shape[0] if x.dim() >= 1 else None  # noqa: E731
+    iw = _validate_weights(image_weights, sample_weights, rows(image_embeddings), "image_weights",
+                           image_embeddings.device)
+    nt = rows(text_embeddings)
+    tw = _validate_weights(text_weights, sample_weights, nt + extras if nt is not None else None, "text_weights",
+                           text_embeddings.device)
+    return (iw, tw) if sample_weights else None
 
 
 def _with_negatives(text_embeddings: torch.Tensor, negative_text) -> torch.Tensor:
@@ -780,15 +857,25 @@ class DDPSigmoidLoss(nn.Module):
     and ``t2i_index`` is ``[B + K]``: ``t2i_top1`` counts over every text of the rank, so a pure-negative extra is always
     a t2i miss. A caller who mixes N of them in gets the caption-only rate as ``t2i_top1 · T / (T − N)``, T = B + K.
     Cannot be combined with ``hard_negatives``. Collective: every rank uses the same K.
+
+    ``sample_weights=True``: every ``forward`` also takes ``image_weights`` ([B]) and ``text_weights`` ([T], T = B + K
+    with extras, in the order the texts are concatenated: captions, then ``negative_text`` / ``extra_text``), floating
+    tensors in [0, 1] on the embeddings' device, either of them ``None`` for ones. Pair (i, j) contributes
+    ``image_weights[i] · text_weights_c[j] · softplus(−y z)`` (c: the rank that owns text j), the gradients follow, and the
+    loss still divides by B. A sample with both weights 0 leaves loss and gradients exactly, at the same shapes: multiply
+    the loss by ``B / (B − m)`` for the mean over the m samples kept. Values outside [0, 1] are clamped into it (NaN → 0);
+    larger importance weights: divide by their maximum and scale the loss by it. No gradient with respect to the weights.
+    Retrieval metrics ignore the weights. Collective: set on every rank.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
                  normalize_inputs: bool = False, sync_scalar_grads: bool = False, fused_step: Optional[bool] = None,
                  batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
-                 extra_texts: int = 0) -> None:
+                 extra_texts: int = 0, sample_weights: bool = False) -> None:
         super().__init__()
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
+        sample_weights = _validate_sample_weights(sample_weights)
         self.t_prime = nn.Parameter(torch.tensor(math.log(10), dtype=torch.float64))
         self.bias = nn.Parameter(torch.tensor(-10.0))
         self.gpu_batch_size = gpu_batch_size
@@ -808,9 +895,11 @@ class DDPSigmoidLoss(nn.Module):
         self.hard_negatives = hard_negatives
         # extension: extra captions with ids of their own (several captions per image)
         self.extra_texts = extra_texts
+        # extension: per-sample loss weights (weight 0 drops a sample at a fixed batch shape)
+        self.sample_weights = sample_weights
         self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank,
                                    multi_positive=multi_positive, hard_negatives=hard_negatives,
-                                   extra_texts=extra_texts)
+                                   extra_texts=extra_texts, sample_weights=sample_weights)
 
     def engine_for(self, batch: int, dim: int, device: torch.device) -> SigmoidLossEngine:
         return self._cache.get(batch, (dim + 7) // 8 * 8, device)
@@ -818,12 +907,15 @@ class DDPSigmoidLoss(nn.Module):
     def forward(self, image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, *,
                 negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
                 return_metrics: bool = False, extra_text: Optional[torch.Tensor] = None,
-                extra_text_ids: Optional[torch.Tensor] = None):
+                extra_text_ids: Optional[torch.Tensor] = None, image_weights: Optional[torch.Tensor] = None,
+                text_weights: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
         ids = _validate_ids(sample_ids, self.multi_positive, image_embeddings)
         _validate_negatives(text_embeddings, negative_text, self.hard_negatives)
         _validate_negatives(text_embeddings, extra_text, self.extra_texts, "extra_text", "extra_texts")
         extra_ids = _validate_extra_text_ids(extra_text_ids, self.extra_texts, text_embeddings)
+        weights = _weights_of(self.sample_weights, image_weights, text_weights, image_embeddings, text_embeddings,
+                              self.hard_negatives + self.extra_texts)
         _validate(image_embeddings, text_embeddings, self.gpu_batch_size)
         text_embeddings = _with_negatives(_with_negatives(text_embeddings, negative_text), extra_text)
         image_embeddings, text_embeddings = _pad_dim(image_embeddings), _pad_dim(text_embeddings)
@@ -831,7 +923,7 @@ class DDPSigmoidLoss(nn.Module):
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts) if return_metrics else None
         loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
-                                    self.normalize_inputs, fused, ids, bufs, extra_ids)
+                                    self.normalize_inputs, fused, ids, bufs, extra_ids, weights)
         return (loss, _metric_dict(bufs)) if return_metrics else loss
 
 
@@ -848,33 +940,41 @@ class SigLipLoss(nn.Module):
     total loss. ``hard_negatives=K``: every forward takes ``negative_text`` [K, D], as in ``DDPSigmoidLoss``.
     ``multi_positive=True, extra_texts=K``: every forward takes ``extra_text`` [K, D] and ``extra_text_ids`` [K], extra
     captions positive for the images with the same id, as in ``DDPSigmoidLoss`` (a pure-negative extra is always a t2i
-    miss: the caption-only rate is ``t2i_top1 · T / (T − N)`` for N of them among T = B + K texts)."""
+    miss: the caption-only rate is ``t2i_top1 · T / (T − N)`` for N of them among T = B + K texts).
+    ``sample_weights=True``: every forward takes ``image_weights`` [B] and ``text_weights`` [B + K] (or None for ones),
+    per-sample loss weights in [0, 1] as in ``DDPSigmoidLoss``."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
-                 multi_positive: bool = False, hard_negatives: int = 0, extra_texts: int = 0):
+                 multi_positive: bool = False, hard_negatives: int = 0, extra_texts: int = 0,
+                 sample_weights: bool = False):
         super().__init__()
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
+        sample_weights = _validate_sample_weights(sample_weights)
         self.cache_labels, self.rank, self.world_size, self.bidir = cache_labels, rank, world_size, bidir
         self.use_horovod = use_horovod
         self.fused_step = fused_step
         self.multi_positive = multi_positive
         self.hard_negatives = hard_negatives
         self.extra_texts = extra_texts
+        self.sample_weights = sample_weights
         self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive,
-                                   hard_negatives=hard_negatives, extra_texts=extra_texts)
+                                   hard_negatives=hard_negatives, extra_texts=extra_texts, sample_weights=sample_weights)
 
     def forward(self, image_features, text_features, logit_scale, logit_bias, output_dict: bool = False, *,
                 negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
                 return_metrics: bool = False, extra_text: Optional[torch.Tensor] = None,
-                extra_text_ids: Optional[torch.Tensor] = None):
+                extra_text_ids: Optional[torch.Tensor] = None, image_weights: Optional[torch.Tensor] = None,
+                text_weights: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
         ids = _validate_ids(sample_ids, self.multi_positive, image_features)
         _validate_negatives(text_features, negative_text, self.hard_negatives)
         _validate_negatives(text_features, extra_text, self.extra_texts, "extra_text", "extra_texts")
         extra_ids = _validate_extra_text_ids(extra_text_ids, self.extra_texts, text_features)
+        weights = _weights_of(self.sample_weights, image_weights, text_weights, image_features, text_features,
+                              self.hard_negatives + self.extra_texts)
         _validate(image_features, text_features, None)
         text_features = _with_negatives(_with_negatives(text_features, negative_text), extra_text)
         image_features, text_features = _pad_dim(image_features), _pad_dim(text_features)
@@ -888,6 +988,6 @@ class SigLipLoss(nn.Module):
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts) if return_metrics else None
         loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs,
-                                    extra_ids)
+                                    extra_ids, weights)
         out = {"contrastive_loss": loss} if output_dict else loss
         return (out, _metric_dict(bufs)) if return_metrics else out

@@ -111,6 +111,16 @@ enum {
                                      SIGLIP_OPT_SAMPLE_IDS on (else SIGLIP_ERR_STATE); turning that option off clears this
                                      one. Accepted on any context; with T == B it changes nothing. Collective: set on all
                                      ranks. Default 0 */
+  SIGLIP_OPT_SAMPLE_WEIGHTS = 23, /* 1: per-sample loss weights. Rank r's images carry weights a_r[i], the texts of
+                                     chunk c (paired, then extras) weights c_c[j], all in [0, 1]; pair (i, j) has weight
+                                     w_ij = a_r[i] c_c[j] and rank r's loss is (1/B_r) sum_ij w_ij softplus(-y_ij z_ij)
+                                     (labels as without weights), with every gradient following (G_ij = w_ij x the
+                                     unweighted term). Still divided by B_r. A sample whose image and text weights are
+                                     both 0 leaves loss and gradients exactly, at the same shapes; unit weights give
+                                     bit-identical results. Every step takes this rank's weights from
+                                     siglip_set_sample_weights; the text weights travel to the other ranks with the text.
+                                     Retrieval metrics ignore the weights. The host-buffer entries are unavailable in
+                                     this mode. Collective: set on all ranks. Default 0 */
   SIGLIP_OPT_AUX_TRACE = 18 /* 1: record globaltimer stamps of the auxiliary warps of CTA 0 for every launch (start,
                                last peer flag seen, jobs done, end of launch); read with siglip_ctx_aux_trace */
 };
@@ -266,6 +276,19 @@ int siglip_set_sample_ids(siglip_ctx* ctx, const int64_t* ids_dev, void* cuda_st
 int siglip_set_extra_text_ids(siglip_ctx* ctx, const int64_t* ids_dev, void* cuda_stream);
 
 /*
+ * SIGLIP_OPT_SAMPLE_WEIGHTS: this rank's image weights (image_w, [B_r] fp32 device buffer, or NULL = ones) and text
+ * weights (text_w, [T_r] fp32: its paired texts, then its extras; NULL = ones) for the NEXT siglip_fwd_bwd(_scaled) /
+ * siglip_forward / siglip_fwd call. A stream-ordered copy into the context that clamps every value into [0, 1] and maps
+ * NaN to 0 (one small kernel launch); nothing is read on the host, so the caller's buffers may be reused once the copy has
+ * run and a single-rank step with weights can be captured into a CUDA graph. The first call allocates the context's
+ * weight buffer ((round_up(T_r, 4) + B_r) floats; also allowed inside a capture). In the mode a step without this call
+ * since the previous step returns SIGLIP_ERR_STATE before launching anything; outside it this call returns
+ * SIGLIP_ERR_STATE. siglip_backward needs no weights (the saved sigma operand and positive-pair terms carry them).
+ * Weights above 1 do not fit the fp16 sigma operand's range: divide by their maximum and scale the loss by it.
+ */
+int siglip_set_sample_weights(siglip_ctx* ctx, const float* image_w, const float* text_w, void* cuda_stream);
+
+/*
  * In-batch retrieval metrics of the NEXT siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd call (that step only),
  * computed from the logits the loss kernels already hold in registers, without a second similarity GEMM:
  *   i2t_index[i] = argmax_j s_ij over all sum(T) texts, for each of this rank's B images (global text index; with hard
@@ -304,7 +327,8 @@ int siglip_fwd(siglip_ctx* ctx, const void* img, const void* txt, const float* t
  * results are on the host. At most two steps may be in flight: submit blocks on the step that used the same staging
  * set. The copies of step n+1 overlap the kernels of step n; every step still pays its own copies.
  * This is the end-to-end entry the benchmark times. Host buffers must stay valid until the step's wait returns.
- * These entries take no sample ids: under SIGLIP_OPT_SAMPLE_IDS they return SIGLIP_ERR_STATE. They stage [B, D] text:
+ * These entries take no sample ids or weights: under SIGLIP_OPT_SAMPLE_IDS or SIGLIP_OPT_SAMPLE_WEIGHTS they return
+ * SIGLIP_ERR_STATE. They stage [B, D] text:
  * on a context with hard negatives (siglip_ctx_create_texts, some T_p != B_p) they return SIGLIP_ERR_STATE.
  */
 int siglip_host_submit(siglip_ctx* ctx, const void* img_host, const void* txt_host, float t_prime, float bias,
@@ -359,6 +383,9 @@ int siglip_debug_get_slot(siglip_ctx* ctx, int chunk, float* out_dev, void* cuda
  * ([batch of that rank] int64 device buffer: its paired texts only; [T of that rank] under SIGLIP_OPT_EXTRA_TEXT_IDS:
  * its paired texts, then its extras) as the "peer" would have published them. */
 int siglip_debug_set_chunk_ids(siglip_ctx* ctx, int chunk, const int64_t* ids_dev, void* cuda_stream);
+/* The weights twin (SIGLIP_OPT_SAMPLE_WEIGHTS): the text weights of chunk `chunk` ([T of that rank] fp32 device buffer,
+ * or NULL = ones), clamped like siglip_set_sample_weights, as the "peer" would have published them. */
+int siglip_debug_set_chunk_weights(siglip_ctx* ctx, int chunk, const float* text_w_dev, void* cuda_stream);
 /* Loopback only: seed the (dt_prime, dbias) mailbox standing in for peer rank `peer`, so that the mean computed under
  * SIGLIP_OPT_SYNC_SCALAR_GRADS can be checked against numbers the kernel did not produce itself. */
 int siglip_debug_set_mailbox(siglip_ctx* ctx, int peer, float dt_prime, float dbias);

@@ -50,6 +50,10 @@ def main() -> int:
     ap.add_argument("--extra-texts", action="store_true",
                     help="also check extra captions with ids (several captions per image) against the float64 oracle: "
                          "extras that caption images of other ranks, extras that match nothing, fused and split")
+    ap.add_argument("--weights", action="store_true",
+                    help="also check per-sample loss weights against the float64 oracle: random weights with zeros on "
+                         "every rank, the text weights travelling with the text, uneven batches, with and without sample "
+                         "ids and hard negatives, fused and split")
     ap.add_argument("--soak", type=int, default=0,
                     help="N > 0: that many back-to-back steps at the --batch/--dim shape mixing the fused step, the split "
                          "API and forward-only calls; same inputs, so every step of a kind must reproduce its first result "
@@ -387,6 +391,55 @@ def main() -> int:
                     dextra=rel_f(e.grad.float().cpu(), dtxt_ref[Bs[rank]:]),
                     dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
                     db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
+
+    # ---- per-sample weights: image weights stay local, text weights travel with the text through the peer pulls ----
+    if args.weights:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from sample_weights_oracle import closed_form_weighted, label_blocks
+        Bs = [160 + 24 * r for r in range(world)]
+        D, tp, bias = 136, math.log(10.0), -8.0
+        g = torch.Generator().manual_seed(4444)
+        unit = lambda n: torch.nn.functional.normalize(torch.randn(n, D, generator=g)).to(torch.bfloat16)  # noqa: E731
+        for K, with_ids in ((0, False), (0, True), (37, True)):
+            Ts = [b + K for b in Bs]
+            imgs, texts = [unit(b) for b in Bs], [unit(t) for t in Ts]
+            ids = list(torch.split(torch.randint(0, 200, (sum(Bs),), generator=g), Bs)) if with_ids else None
+
+            def weights(n):
+                w = torch.rand(n, generator=g)
+                w[torch.rand(n, generator=g) < 0.1] = 0.0
+                return w
+            iws, tws = [weights(b) for b in Bs], [weights(t) for t in Ts]
+            f = lambda xs: [x.double().numpy() for x in xs]  # noqa: E731
+            ref = closed_form_weighted(f(imgs), f(texts), tp, bias, f(iws), f(tws),
+                                       label_blocks(Bs, Ts, f(ids) if ids else None))
+            mine = ref[rank]
+            dtxt_ref = torch.from_numpy(sum(ref[r]["contrib"][rank] for r in range(world)))
+            img, txt = imgs[rank].to(dev), texts[rank].to(dev)
+            for fused in (None, False):
+                modx = DDPSigmoidLoss(Bs[rank], fused_step=fused, batch_per_rank=Bs, multi_positive=with_ids,
+                                      hard_negatives=K, sample_weights=True).to(dev)
+                with torch.no_grad():
+                    modx.t_prime.fill_(tp)
+                    modx.bias.fill_(bias)
+                for rep in range(2):
+                    modx.zero_grad()
+                    a, b = (x.float().requires_grad_(True) for x in (img, txt))
+                    kw = dict(image_weights=iws[rank].to(dev), text_weights=tws[rank].to(dev))
+                    if with_ids:
+                        kw["sample_ids"] = ids[rank].to(dev)
+                    if K:
+                        l2 = modx(a, b[:Bs[rank]], negative_text=b[Bs[rank]:], **kw)
+                    else:
+                        l2 = modx(a, b, **kw)
+                    l2.backward()
+                    torch.cuda.synchronize()
+                    report(f"weights {fused} B={Bs} K={K} ids={with_ids} D={D} rep{rep}", dict(
+                        loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
+                        dimg=rel_f(a.grad.float().cpu(), torch.from_numpy(mine["dimg"])),
+                        dtxt=rel_f(b.grad.float().cpu(), dtxt_ref),
+                        dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
+                        db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
 
     # ---- larger: fp32 autograd; dtxt reference summed over ranks ------------------------------------------
     B, D, tp, bias = 2048, 768, math.log(10.0), -10.0
