@@ -267,8 +267,39 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, ui
         : "l"(adesc), "l"(bdesc), "r"(accumulate));
   }
 }
+
+// D[64 x 256] (+)= A * B: the gradient kernel's 256-column tiles, 16-bit operands only (the same transpose bits).
+#define SIGLIP_WGMMA_ACC128                                                                                         \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
+  "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "    \
+  "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, "    \
+  "%68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, "    \
+  "%90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, "    \
+  "%110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
+template <int kType, int kTA, int kTB>
+__device__ __forceinline__ void wgmma_m64n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  static_assert(kType == 0 || kType == 1, "m64n256: bf16 or fp16 operands");
+  float* h = d + 64;   // second half of the fragment: columns 128 .. 255
+  if constexpr (kType == 0) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 " SIGLIP_WGMMA_ACC128
+        ", %128, %129, p, 1, 1, %131, %132;\n\t}"
+        : SIGLIP_WGMMA_OUT64(d), SIGLIP_WGMMA_OUT64(h)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTA), "n"(kTB));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 " SIGLIP_WGMMA_ACC128
+        ", %128, %129, p, 1, 1, %131, %132;\n\t}"
+        : SIGLIP_WGMMA_OUT64(d), SIGLIP_WGMMA_OUT64(h)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTA), "n"(kTB));
+  }
+}
+#undef SIGLIP_WGMMA_ACC128
 #undef SIGLIP_WGMMA_ACC64
 #undef SIGLIP_WGMMA_OUT64
+
 
 // ---------------------------------------------------------------------------------------------
 // Shared-memory matrix descriptor of wgmma (PTX ISA "Matrix Descriptor Format", sm_90), 128-byte swizzle:

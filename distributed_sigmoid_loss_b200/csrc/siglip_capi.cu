@@ -176,6 +176,7 @@ struct siglip_ctx {
   int overlap_reduce = 1;                // fold the peers' dtxt contributions inside the gradient kernels
   int kernel_timing = 0;
   int stages_loss = 0, stages_grad = 0;  // 0 = kernel default
+  int grad_tile_n = 0;                   // gradient kernel's column tiles: 0 = from the shape (grad_tile_cols), 128, 256
   int mcast = 1;                         // 2: vertically adjacent tiles share the B tile by TMA multicast
   int grad_bf16 = 0;                     // dimg / dtxt outputs are bf16 instead of fp32
   int sync_scalar_grads = 0;             // backward returns the mean over ranks of dt' / dbias
@@ -588,8 +589,8 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
     p.wait_stats = wstats;
   }
   if ((rc = timing_mark(c, c->ev_loss, c->ev_loss_used, st))) return rc;
-  CKI(siglip::launch_gemm(cg, siglip::kModeLoss, c->stages_loss, mc, &tmA, &tmB, &tmA, &tmB, &tmG, p, c->num_sms,
-                          st));
+  CKI(siglip::launch_gemm(cg, siglip::kModeLoss, c->stages_loss, mc, siglip::kTileCols, &tmA, &tmB, &tmA, &tmB, &tmG,
+                          p, c->num_sms, st));
   if ((rc = timing_mark(c, c->ev_loss, c->ev_loss_used, st))) return rc;
   if (wstats != nullptr) {
     CK(cudaStreamSynchronize(st));
@@ -651,11 +652,33 @@ struct GradOut {
 //   prob 0: dimg (+)= g (t/B) (G @ txt_c  [+ g_diag * txt_own])      A = G K-major,  B = txt16[gi] N-major     K = Bn
 //   prob 1: dtxt_c  = g (t/B) (G^T @ img  [+ g_diag * img])          A = G M-major,  B = img16 N-major         K = B
 // Bn is the chunk's text count (its batch plus its hard negatives); the bracketed terms cover the first B rows only.
+//
+// Column-tile width of a gradient launch whose two problems have M0 and M1 rows (N = D both). A 256-column tile does
+// the work of two 128-column ones in less time (one wgmma m64n256 instead of two m64n128 reading the A tile twice), but
+// there are half as many tiles to spread over the clusters of the persistent grid. A launch lasts about (waves: tiles
+// per cluster, rounded up) x (time of one tile), and a 256-column tile took 0.84 - 0.9 x the time of two 128-column
+// ones on an H100 SXM (400 W, tools/tile_width_ab.py). So 256 when 2 x 0.9 x its waves <= the waves of 128-column
+// tiles: B = 16384 with D = 768, 1024 or 1152, but not D <= 128, B = 16384 with D = 384 (4 waves against 6) nor
+// B = 4096 with D = 768 (2 against 3). Split-K (SIGLIP_OPT_SPLIT_K) keeps its workspace of 128-column partials.
+int grad_tile_cols(const siglip_ctx* c, int M0, int M1) {
+  if (c->split_k != 0 && c->mcast == 1) return siglip::kTileCols;
+  if (c->grad_tile_n != 0) return c->grad_tile_n;
+  const int cs = siglip::cluster_size(c->cta_group, c->mcast);
+  const long long units = c->num_sms / cs > 0 ? c->num_sms / cs : 1;
+  auto waves = [&](int w) {
+    const long long tiles =
+        static_cast<long long>(ceil_div(M0, 128 * cs) + ceil_div(M1, 128 * cs)) * ceil_div(c->D, w);
+    return (tiles + units - 1) / units;
+  };
+  return 18 * waves(siglip::kWideTileCols) <= 10 * waves(siglip::kTileCols) ? siglip::kWideTileCols : siglip::kTileCols;
+}
+
 int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_bfloat16* txt_own, int Bn,
                    const float* t_prime, const float* grad_out, const GradOut& o, const AuxList& aux,
                    const EndSignal& end, cudaStream_t st) {
   const int cg = c->cta_group;
-  const int bk = siglip::b_box_k_mnmajor(siglip::cluster_size(cg, c->mcast));
+  const int tile_n = grad_tile_cols(c, c->B, Bn);
+  const int bk = siglip::b_box_k_mnmajor(siglip::cluster_size(cg, c->mcast), tile_n);
   CUtensorMap tmA0, tmB0, tmA1, tmB1;
   int rc;
   if (c->G[gi] == nullptr) return fail(SIGLIP_ERR_STATE, "gradient kernel without a saved sigma operand");
@@ -718,7 +741,7 @@ int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_
   }
   apply_aux(c, p, aux, end);
   if ((rc = timing_mark(c, c->ev_grad, c->ev_grad_used, st))) return rc;
-  CKI(siglip::launch_gemm(cg, siglip::kModeOut, c->stages_grad, c->mcast, &tmA0, &tmB0, &tmA1, &tmB1,
+  CKI(siglip::launch_gemm(cg, siglip::kModeOut, c->stages_grad, c->mcast, tile_n, &tmA0, &tmB0, &tmA1, &tmB1,
                           &tmA0, p, c->num_sms, st));
   if ((rc = timing_mark(c, c->ev_grad, c->ev_grad_used, st))) return rc;
   c->launches++;
@@ -1374,8 +1397,9 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
     case SIGLIP_OPT_EPI_SLEEP_GRAD_NS:   // accepted for existing callers; no effect on sm_90a (see the header)
     case SIGLIP_OPT_EPI_SLEEP_LOSS_NS:
       return 0;
-    case SIGLIP_OPT_GRAD_TILE_N:         // accepted for existing callers; every column tile is 128 wide on sm_90a
+    case SIGLIP_OPT_GRAD_TILE_N:
       if (value != 0 && value != 128 && value != 256) return fail(SIGLIP_ERR_INVALID, "grad_tile_n must be 0, 128 or 256");
+      c->grad_tile_n = value;
       return 0;
     case SIGLIP_OPT_INPUT_F16:
       c->input_f16 = value ? 1 : 0;
@@ -2042,6 +2066,11 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
   const char* env_mc = getenv("SIGLIP_DEBUG_MCAST");
   const int mcast = env_mc ? atoi(env_mc) : 1;
   if (mcast != 1 && mcast != 2) return fail(SIGLIP_ERR_INVALID, "SIGLIP_DEBUG_MCAST must be 1 or 2");
+  const char* env_tn = getenv("SIGLIP_DEBUG_TILE_N");
+  const int tile_n = env_tn ? atoi(env_tn) : siglip::kTileCols;
+  if (tile_n != siglip::kTileCols && tile_n != siglip::kWideTileCols)
+    return fail(SIGLIP_ERR_INVALID, "SIGLIP_DEBUG_TILE_N must be 128 or 256");
+  if (fp8 && tile_n != siglip::kTileCols) return fail(SIGLIP_ERR_INVALID, "the fp8 measurement path has 128-column tiles");
   if (fp8) {
     if (a_mn || b_mn || mcast != 1) return fail(SIGLIP_ERR_INVALID, "the fp8 measurement path is K-major, no multicast");
     if ((rc = encode_u8_kmajor(&tmA, A, M, K, lda, 128))) return rc;
@@ -2049,7 +2078,8 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
   } else {
     const int cs = siglip::cluster_size(cta_group, mcast);
     if ((rc = encode_operand(&tmA, A, M, K, lda, a_mn, 128))) return rc;
-    if ((rc = encode_operand(&tmB, Bm, N, K, ldb, b_mn, siglip::b_box_rows_kmajor(cs), siglip::b_box_k_mnmajor(cs))))
+    if ((rc = encode_operand(&tmB, Bm, N, K, ldb, b_mn, siglip::b_box_rows_kmajor(cs, tile_n),
+                             siglip::b_box_k_mnmajor(cs, tile_n))))
       return rc;
   }
   float* zero = nullptr;  // t' = 0 -> scale exp(0) * 1 = 1
@@ -2091,10 +2121,12 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
   const int stages = env_st ? atoi(env_st) : 0;
   if (stages != 0 && stages != 4 && stages != 6) return fail(SIGLIP_ERR_INVALID, "SIGLIP_DEBUG_STAGES must be 4 or 6");
   if (iters > 1)  // warm-up
-    lrc = siglip::launch_gemm(cta_group, siglip::kModeOut, stages, mcast, &tmA, &tmB, &tmA, &tmB, &tmA, p, num_sms, st);
+    lrc = siglip::launch_gemm(cta_group, siglip::kModeOut, stages, mcast, tile_n, &tmA, &tmB, &tmA, &tmB, &tmA, p,
+                              num_sms, st);
   cudaEventRecord(e0, st);
   for (int it = 0; it < iters && lrc == 0; ++it)
-    lrc = siglip::launch_gemm(cta_group, siglip::kModeOut, stages, mcast, &tmA, &tmB, &tmA, &tmB, &tmA, p, num_sms, st);
+    lrc = siglip::launch_gemm(cta_group, siglip::kModeOut, stages, mcast, tile_n, &tmA, &tmB, &tmA, &tmB, &tmA, p,
+                              num_sms, st);
   cudaEventRecord(e1, st);
   cudaError_t se = cudaStreamSynchronize(st);
   if (ms_per_iter != nullptr && se == cudaSuccess && lrc == 0) {

@@ -38,10 +38,15 @@ constexpr int kNumThreads = (kNumEpiWarps + 4) * 32;
 
 constexpr int kStagingBytesPerWarp = 1024;  // one 16x32 16-bit slab, 64-byte rows, 64B-swizzled (TMA store source)
 
-template <int kMode, int kStagesT>
+// Gradient kernel with 256-column tiles (wgmma m64n256, 128 accumulator registers per consumer thread): 48 KiB per
+// stage, so 4 stages. The consumers fit the even split of __launch_bounds__(384, 1), 168 registers per thread.
+constexpr int kWideTileN = kWideTileCols;
+constexpr int kWideStages = 4;
+
+template <int kMode, int kStagesT, int kTileNT = kTileN>
 struct Cfg {
   static constexpr int kABytes = kBlockM * kBlockK * 2;            // 16 KiB
-  static constexpr int kBBytes = kTileN * kBlockK * 2;             // 16 KiB
+  static constexpr int kBBytes = kTileNT * kBlockK * 2;            // 16 KiB (32 KiB for 256-column tiles)
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = kStagesT;
   static constexpr int kStagingBytes = (kMode == kModeLoss) ? kNumEpiWarps * kStagingBytesPerWarp : 0;
@@ -455,7 +460,8 @@ __device__ __forceinline__ void tile_metrics(const float (&acc)[64], int row_lo,
   }
 }
 
-// Epilogue of the out kernel: one row of the fragment (h = 0: row_lo, 1: row_lo + 8), 16 column pairs.
+// Epilogue of the out kernel: one row of the fragment (h = 0: row_lo, 1: row_lo + 8), kN / 8 column pairs (16 for
+// 128-column tiles, 32 for 256-column ones).
 //   val = scale * (acc * acc_scale + fix * x[row, col]) (+ add_src[row, col]);  written as fp32 or bf16
 // parts / nparts: owner of a split tile — the other K-slices' fp32 partials (float4 j of this thread's fragment at
 // parts[j * 256], slices part_stride apart) are added to acc first, in slice order. (Read here instead of being added
@@ -464,7 +470,8 @@ __device__ __forceinline__ void tile_metrics(const float (&acc)[64], int row_lo,
 // as the compiler knows, and a load -> store -> load chain exposes one L2 round trip per pair.
 // fix_rows: rows of fix_mat; a row at or past it has no positive-pair term and reads nothing there (with hard negatives
 // the dtxt problem's M = T exceeds the B rows of its fix_mat, the caller's image buffer).
-__device__ __forceinline__ void out_row(const float (&acc)[64], int h, float scale, int row, int col0, int c_lo,
+template <int kN>
+__device__ __forceinline__ void out_row(const float (&acc)[kN / 2], int h, float scale, int row, int col0, int c_lo,
                                        const Problem& pr, float fix, int fix_rows, const float4* parts = nullptr,
                                        int nparts = 0, size_t part_stride = 0) {
   if (row >= pr.M) return;
@@ -475,7 +482,7 @@ __device__ __forceinline__ void out_row(const float (&acc)[64], int h, float sca
       (pr.fix_mat != nullptr && row < fix_rows) ? pr.fix_mat + static_cast<long long>(row) * pr.ldx : nullptr;
   const float* arow = pr.add_src ? pr.add_src + static_cast<long long>(row) * pr.ld_add : nullptr;
 #pragma unroll
-  for (int jb = 0; jb < 4; ++jb) {
+  for (int jb = 0; jb < kN / 32; ++jb) {
     uint32_t xw[4];
     float2 ad[4];
 #pragma unroll
@@ -526,12 +533,12 @@ __device__ __forceinline__ void out_row(const float (&acc)[64], int h, float sca
 }
 
 // -------------------------------------------------------------------------------------------------
-// Mainloop of one consumer warpgroup: acc (+)= A[its 64 rows] * B[128 columns]^T over k-blocks [kb0, kb1), operands
+// Mainloop of one consumer warpgroup: acc (+)= A[its 64 rows] * B[kN columns]^T over k-blocks [kb0, kb1), operands
 // from the shared-memory ring. One k block = 4 wgmma's; the stage of the previous k block is handed back (to every CTA
 // of the cluster that multicasts into it) once wgmma.wait_group says its MMAs have finished reading it.
 // -------------------------------------------------------------------------------------------------
-template <int kType, int kTA, int kTB, int kCS, int kStageBytes>
-__device__ __forceinline__ void mma_loop(float (&acc)[64], int kb0, int kb1, int& stage, uint32_t& phase, int nstages,
+template <int kType, int kTA, int kTB, int kCS, int kStageBytes, int kN = kTileN>
+__device__ __forceinline__ void mma_loop(float (&acc)[kN / 2], int kb0, int kb1, int& stage, uint32_t& phase, int nstages,
                                          uint64_t adesc0, uint64_t bdesc0, uint32_t a_adv, uint32_t b_adv,
                                          uint32_t full0, uint32_t empty0, int lane, DebugRecord* dbg, int t,
                                          long long* waited) {
@@ -547,7 +554,7 @@ __device__ __forceinline__ void mma_loop(float (&acc)[64], int kb0, int kb1, int
     }
   };
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc_fence(acc[i]);
+  for (int i = 0; i < kN / 2; ++i) acc_fence(acc[i]);
   int prev = -1;
   for (int kb = kb0; kb < kb1; ++kb) {
     mbar_wait(full0 + 8u * static_cast<uint32_t>(stage), phase, dbg, 3, t, kb, 0, waited);
@@ -555,8 +562,12 @@ __device__ __forceinline__ void mma_loop(float (&acc)[64], int kb0, int kb1, int
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < kBlockK / kMmaK; ++k) {
-      wgmma_m64n128<kType, kTA, kTB>(acc, adesc0 + so + static_cast<uint64_t>(k * a_adv),
-                                     bdesc0 + so + static_cast<uint64_t>(k * b_adv), (kb != kb0 || k != 0) ? 1u : 0u);
+      if constexpr (kN == kWideTileN)
+        wgmma_m64n256<kType, kTA, kTB>(acc, adesc0 + so + static_cast<uint64_t>(k * a_adv),
+                                       bdesc0 + so + static_cast<uint64_t>(k * b_adv), (kb != kb0 || k != 0) ? 1u : 0u);
+      else
+        wgmma_m64n128<kType, kTA, kTB>(acc, adesc0 + so + static_cast<uint64_t>(k * a_adv),
+                                       bdesc0 + so + static_cast<uint64_t>(k * b_adv), (kb != kb0 || k != 0) ? 1u : 0u);
     }
     wgmma_commit();
     wgmma_wait<1>();   // the MMAs of the previous k block are done: its stage may be refilled
@@ -569,7 +580,7 @@ __device__ __forceinline__ void mma_loop(float (&acc)[64], int kb0, int kb1, int
   }
   wgmma_wait<0>();
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc_fence(acc[i]);
+  for (int i = 0; i < kN / 2; ++i) acc_fence(acc[i]);
   if (prev >= 0) release(prev);
 }
 
@@ -631,17 +642,20 @@ __device__ __forceinline__ void mma_loop_f8(float (&sum)[64], float (&acc)[64], 
 // own instantiation for the same reason.
 // kWeights: the loss kernel with per-sample weights (SIGLIP_OPT_SAMPLE_WEIGHTS); its own instantiation for the same
 // reason, composing with kIds and kMetrics.
+// kTileNT: columns of a tile. 256 (kWideTileN) exists for the out kernel with 16-bit operands only (no split-K).
 template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false,
-          bool kWeights = false>
+          bool kWeights = false, int kTileNT = kTileN>
 __global__ void __launch_bounds__(kNumThreads, 1)
 siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmB0,
                    const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmB1,
                    const __grid_constant__ CUtensorMap tmG, const __grid_constant__ KernelParams p) {
-  using C = Cfg<kMode, kStagesT>;
+  using C = Cfg<kMode, kStagesT, kTileNT>;
   static_assert(kCS == 1 || kCS == 2 || kCS == 4, "clusters of 1, 2 or 4 CTAs");
   static_assert(!kIds || kMode == kModeLoss, "sample ids are a loss-kernel option");
   static_assert(!kMetrics || kMode == kModeLoss, "retrieval metrics are a loss-kernel option");
   static_assert(!kWeights || kMode == kModeLoss, "sample weights are a loss-kernel option");
+  static_assert(kTileNT == kTileN || (kTileNT == kWideTileN && kMode == kModeOut && !kF8),
+                "256-column tiles: out kernel, 16-bit operands");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -717,7 +731,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       const CUtensorMap* tmA = tc.prob ? &tmA1 : &tmA0;
       const CUtensorMap* tmB = tc.prob ? &tmB1 : &tmB0;
       const int m_idx = tc.m_blk * kBlockM;
-      const int n_idx = tc.n_blk * kTileN;
+      const int n_idx = tc.n_blk * kTileNT;
       // elements per 128-byte swizzle row: 64 16-bit values, or 128 8-bit ones (fp8 measurement path, K-major only)
       const int kblk = (pr.ab_f16 == 2) ? 2 * kBlockK : kBlockK;
       const int num_kb = (pr.K + kblk - 1) / kblk;
@@ -749,16 +763,17 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
             }
           };
           if (!b_mn) {
-            constexpr int kRows = kTileN / kCS;                     // box {64 k, kRows rows}
+            constexpr int kRows = kTileNT / kCS;                    // box {64 k, kRows rows}
             load_b(sB + crank * (kRows * 128), k_idx, n_idx + static_cast<int>(crank) * kRows);
-          } else if constexpr (kCS == 4) {
+          } else if constexpr (kCS == 4 && kTileNT == kTileN) {
             // boxes {64 columns, 32 k}: CTA r fetches k half (r & 1) of the 64-column block (r >> 1)
             const int h = static_cast<int>(crank >> 1), kh = static_cast<int>(crank & 1u);
             load_b(sB + h * 8192 + kh * 4096, n_idx + 64 * h, k_idx + 32 * kh);
           } else {
+            constexpr int kBoxes = kTileNT / 64;                    // boxes {64 columns, 64 k}, kBoxes / kCS per CTA
 #pragma unroll
-            for (int h = static_cast<int>(crank) * (2 / kCS); h < (static_cast<int>(crank) + 1) * (2 / kCS); ++h)
-              load_b(sB + h * 8192, n_idx + 64 * h, k_idx);         // boxes {64 columns, 64 k}
+            for (int h = static_cast<int>(crank) * (kBoxes / kCS); h < (static_cast<int>(crank) + 1) * (kBoxes / kCS); ++h)
+              load_b(sB + h * 8192, n_idx + 64 * h, k_idx);
           }
         }
         __syncwarp();
@@ -802,13 +817,13 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
     int stage = 0;
     uint32_t phase = 0;
     bool p1_ready = false;
-    float acc[64];
+    float acc[kTileNT / 2];
     float acc8[kF8 ? 64 : 1];   // result of the 8-bit mainloop (see mma_loop_f8)
     for (int t = cluster_id; t < total_tiles; t += num_clusters) {
       const TileCoord tc = decode_tile<kCS>(p, t, static_cast<int>(crank));
       const Problem& pr = p.prob[tc.prob];
       const int row0 = tc.m_blk * kBlockM;            // first row of this CTA's block
-      const int col_base = tc.n_blk * kTileN;
+      const int col_base = tc.n_blk * kTileNT;
       const int row_lo = row0 + r_lo;                 // global rows of this thread: row_lo, row_lo + 8
       const bool fp8 = (pr.ab_f16 == 2);
       const int num_kb = (pr.K + (fp8 ? 2 * kBlockK : kBlockK) - 1) / (fp8 ? 2 * kBlockK : kBlockK);
@@ -817,15 +832,16 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       {
         // K-major: 8-row groups 1024 B apart (SBO), K advance 32 B inside the swizzle row (16 16-bit or 32 8-bit values).
         // MN-major: 64-element MN blocks 8192 B apart (LBO), 8-k groups 1024 B apart (SBO), K advance 16 rows.
-        // This warpgroup's 64 A rows start 8192 B into the A tile in both layouts.
+        // This warpgroup's 64 A rows start 8192 B into the A tile in both layouts. A 256-column MN-major B tile is 4
+        // such 64-column blocks (the same LBO), a K-major one 256 rows of 8-row groups (the same SBO).
         const uint32_t a_lbo = pr.a_mn ? 8192u : 16u, b_lbo = pr.b_mn ? 8192u : 16u;
         const uint32_t a_adv = pr.a_mn ? (kMmaK * 128u) >> 4 : 32u >> 4;
         const uint32_t b_adv = pr.b_mn ? (kMmaK * 128u) >> 4 : 32u >> 4;
         const uint64_t adesc0 = make_smem_desc_sw128(smem_base + static_cast<uint32_t>(wg) * 8192u, a_lbo, 1024u);
         const uint64_t bdesc0 = make_smem_desc_sw128(smem_base + C::kABytes, b_lbo, 1024u);
 #define SIGLIP_MMA_LOOP(T, TA, TB)                                                                                  \
-  mma_loop<T, TA, TB, kCS, C::kStageBytes>(acc, kb0, kb1, stage, phase, C::kStages, adesc0, bdesc0, a_adv, b_adv, \
-                                           full0, empty0, lane, p.dbg, t, w_full_p)
+  mma_loop<T, TA, TB, kCS, C::kStageBytes, kTileNT>(acc, kb0, kb1, stage, phase, C::kStages, adesc0, bdesc0, a_adv, \
+                                                    b_adv, full0, empty0, lane, p.dbg, t, w_full_p)
         const int sel = pr.a_mn * 2 + pr.b_mn;
         if (fp8) {
           // kF8 instantiation only (launch_gemm routes 8-bit operands there): the result lands in acc8
@@ -971,12 +987,12 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
           p1_ready = true;
         }
         if constexpr (kF8) {   // whole tiles only: split-K is never requested for 8-bit operands
-          out_row(acc8, 0, scale, row_lo, col_base, c_lo, pr, fix0, p.fix_rows);
-          out_row(acc8, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1, p.fix_rows);
+          out_row<kTileN>(acc8, 0, scale, row_lo, col_base, c_lo, pr, fix0, p.fix_rows);
+          out_row<kTileN>(acc8, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1, p.fix_rows);
         } else if (tc.part < 0) {
-          out_row(acc, 0, scale, row_lo, col_base, c_lo, pr, fix0, p.fix_rows);
-          out_row(acc, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1, p.fix_rows);
-        } else {
+          out_row<kTileNT>(acc, 0, scale, row_lo, col_base, c_lo, pr, fix0, p.fix_rows);
+          out_row<kTileNT>(acc, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1, p.fix_rows);
+        } else if constexpr (kTileNT == kTileN) {   // launch_impl splits 128-column tiles only
           // split tile: this CTA's 128 x 128 fp32 partial in fragment order, thread-contiguous float4's
           const size_t kPartF4 = static_cast<size_t>(kBlockM) * kTileN / 4;
           float4* ws = reinterpret_cast<float4*>(p.sk_ws) +
@@ -1022,8 +1038,10 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
               }
             }
             __syncwarp();
-            out_row(acc, 0, scale, row_lo, col_base, c_lo, pr, fix0, p.fix_rows, ws, p.sk_parts - 1, part_stride);
-            out_row(acc, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1, p.fix_rows, ws, p.sk_parts - 1, part_stride);
+            out_row<kTileN>(acc, 0, scale, row_lo, col_base, c_lo, pr, fix0, p.fix_rows, ws, p.sk_parts - 1,
+                            part_stride);
+            out_row<kTileN>(acc, 1, scale, row_lo + 8, col_base, c_lo, pr, fix1, p.fix_rows, ws, p.sk_parts - 1,
+                            part_stride);
             // every owner warp has consumed the partials: the last one re-arms the counters for the next launch
             __syncwarp();
             if (lane == 0) {
@@ -1637,14 +1655,14 @@ __global__ void normalize_bwd_kernel(const void* __restrict__ x, const float* __
 }
 
 // kIds / kMetrics / kWeights select the sample-id / retrieval-metrics / sample-weight instantiations of the loss kernel
-// (ignored for the out kernel)
+// (ignored for the out kernel); kTileNT the column-tile width
 template <int kMode, int kStages, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false,
-          bool kWeights = false>
+          bool kWeights = false, int kTileNT = kTileN>
 int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensorMap* tmA1, const CUtensorMap* tmB1,
                 const CUtensorMap* tmG, const KernelParams& p, int num_sms, cudaStream_t stream) {
-  using C = Cfg<kMode, kStages>;
+  using C = Cfg<kMode, kStages, kTileNT>;
   auto kern = siglip_gemm_kernel<kMode, kStages, kCS, kF8, kIds && kMode == kModeLoss, kMetrics && kMode == kModeLoss,
-                                 kWeights && kMode == kModeLoss>;
+                                 kWeights && kMode == kModeLoss, kTileNT>;
   static bool attr_set = false;
   cudaError_t e = cudaSuccess;
   if (!attr_set) {
@@ -1657,7 +1675,7 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
   for (int i = 0; i < pl.nprob; ++i) {
     Problem& pr = pl.prob[i];
     pr.tiles_m = (pr.M + kBlockM * kCS - 1) / (kBlockM * kCS);
-    pr.tiles_n = (pr.N + kTileN - 1) / kTileN;
+    pr.tiles_n = (pr.N + kTileNT - 1) / kTileNT;
     total_tiles += pr.tiles_m * pr.tiles_n;
   }
   cudaLaunchConfig_t cfg{};
@@ -1688,7 +1706,7 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
   }
   int clusters = max_clusters < num_sms / kCS ? max_clusters : num_sms / kCS;
   pl.sk_parts = 0;
-  if (kMode == kModeOut && p.sk_request != 0 && p.sk_ws != nullptr && clusters > 1) {
+  if (kMode == kModeOut && kTileNT == kTileN && p.sk_request != 0 && p.sk_ws != nullptr && clusters > 1) {
     // Split-K of the ragged last wave: `rem` tiles left after the full waves would occupy rem of `clusters` units for
     // a whole tile time. Cut each of them into S = floor(clusters / rem) K-slices (S * rem <= clusters work items, one
     // per unit): the last wave then lasts ~1/S of a tile. Not worth it when the last wave is more than half full
@@ -1786,15 +1804,31 @@ size_t gemm_smem_bytes(int mode) {
 // the five tensor maps and the parameter block travel as kernel parameters: keep them inside the classic 4 KiB limit
 static_assert(5 * sizeof(CUtensorMap) + sizeof(KernelParams) <= 4096, "kernel parameters exceed 4 KiB");
 
-int launch_gemm(int cta_group, int mode, int stages, int mcast, const CUtensorMap* tmA0, const CUtensorMap* tmB0,
-                const CUtensorMap* tmA1, const CUtensorMap* tmB1, const CUtensorMap* tmG, const KernelParams& p,
-                int num_sms, cudaStream_t stream) {
+int launch_gemm(int cta_group, int mode, int stages, int mcast, int tile_n, const CUtensorMap* tmA0,
+                const CUtensorMap* tmB0, const CUtensorMap* tmA1, const CUtensorMap* tmB1, const CUtensorMap* tmG,
+                const KernelParams& p, int num_sms, cudaStream_t stream) {
   if (stages <= 0) stages = default_stages(mode);
   if (mode == kModeOut && p.prob[0].ab_f16 == 2) {   // 8-bit measurement path: K-major, no multicast, no split-K
+    if (tile_n != kTileN) return static_cast<int>(cudaErrorInvalidValue);
     if (cluster_size(cta_group, mcast) == 2)
       return launch_impl<kModeOut, 6, 2, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
     return launch_impl<kModeOut, 6, 1, true>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
   }
+  if (tile_n == kWideTileN) {   // every stage request maps to the 4 stages that fit
+    if (mode != kModeOut) return static_cast<int>(cudaErrorInvalidValue);
+    switch (cluster_size(cta_group, mcast)) {
+      case 4:
+        return launch_impl<kModeOut, kWideStages, 4, false, false, false, false, kWideTileN>(tmA0, tmB0, tmA1, tmB1,
+                                                                                            tmG, p, num_sms, stream);
+      case 2:
+        return launch_impl<kModeOut, kWideStages, 2, false, false, false, false, kWideTileN>(tmA0, tmB0, tmA1, tmB1,
+                                                                                            tmG, p, num_sms, stream);
+      default:
+        return launch_impl<kModeOut, kWideStages, 1, false, false, false, false, kWideTileN>(tmA0, tmB0, tmA1, tmB1,
+                                                                                            tmG, p, num_sms, stream);
+    }
+  }
+  if (tile_n != kTileN) return static_cast<int>(cudaErrorInvalidValue);
   switch (cluster_size(cta_group, mcast)) {
     case 4:
       if (mode == kModeLoss) SIGLIP_LAUNCH_STAGES(kModeLoss, 4);

@@ -15,7 +15,7 @@ namespace siglip {
 //   1: MN-major — global tensor is [K][rows], rows contiguous   (TMA boxes {64 rows, 64 k}; B of a 4-CTA cluster {64, 32})
 struct Problem {
   int M, N, K;
-  int tiles_m, tiles_n;   // filled in by launch_gemm: row panels of one cluster, 128-column tiles
+  int tiles_m, tiles_n;   // filled in by launch_gemm: row panels of one cluster, column tiles (128 or 256 wide)
   int a_mn, b_mn;
   int ab_f16;       // 0: bf16 operands; 1: both IEEE fp16 (gradient contractions: scaled sigma x scaled embeddings);
                     // 2: both fp8 e4m3, K-major only (the SURVEY.md §8f-4 measurement, siglip_debug_gemm)
@@ -151,14 +151,16 @@ struct KernelParams {
 enum KernelMode { kModeLoss = 0, kModeOut = 1 };
 
 constexpr int kTileCols = 128;   // columns of a tile (wgmma N); a CTA computes 128 rows of it
+constexpr int kWideTileCols = 256;   // the gradient kernel's wide tiles (out mode, 16-bit operands, no split-K)
 
 // CTAs per cluster: cta_group (1 or 2) CTAs compute one 128- or 256-row tile, mcast (1 or 2) such tiles share their B
 // tile as well; either way a cluster is a column of vertically adjacent 128-row blocks sharing B through TMA multicast.
 inline int cluster_size(int cta_group, int mcast) { return cta_group * mcast; }
-// Box of the B operand's tensor map for a cluster of `cs` CTAs (each CTA fetches 1 / cs of the B tile):
-// K-major rows, MN-major k extent.
-inline int b_box_rows_kmajor(int cs) { return kTileCols / cs; }
-inline int b_box_k_mnmajor(int cs) { return cs == 4 ? 32 : 64; }
+// Box of the B operand's tensor map for a cluster of `cs` CTAs and tiles `tile_n` columns wide (each CTA fetches
+// 1 / cs of the B tile): K-major rows, MN-major k extent. MN-major boxes are 64 columns wide: a 128-column tile of a
+// 4-CTA cluster is fetched in k halves, every other tile in whole {64, 64} boxes.
+inline int b_box_rows_kmajor(int cs, int tile_n = kTileCols) { return tile_n / cs; }
+inline int b_box_k_mnmajor(int cs, int tile_n = kTileCols) { return (cs == 4 && tile_n == kTileCols) ? 32 : 64; }
 
 // Dynamic shared memory needed by the default configuration of `mode`.
 size_t gemm_smem_bytes(int mode);
@@ -169,10 +171,12 @@ int query_max_active_clusters(int cluster);  // co-resident clusters of the out 
 // tmG: store map of the sigma operand (loss mode; 16-bit [B, B], box {32, 16}, 64B swizzle) — any valid map in out mode.
 // Returns cudaError_t as int.
 // cta_group x mcast = CTAs per cluster (1, 2 or 4); the B maps must have the boxes b_box_rows_kmajor /
-// b_box_k_mnmajor give for that cluster size.
-int launch_gemm(int cta_group, int mode, int stages, int mcast, const CUtensorMap* tmA0, const CUtensorMap* tmB0,
-                const CUtensorMap* tmA1, const CUtensorMap* tmB1, const CUtensorMap* tmG, const KernelParams& p,
-                int num_sms, cudaStream_t stream);
+// b_box_k_mnmajor give for that cluster size and tile width.
+// tile_n: kTileCols, or kWideTileCols for the out kernel with 16-bit operands (4 stages whatever `stages` asks; never
+// split along K). Anything else is cudaErrorInvalidValue.
+int launch_gemm(int cta_group, int mode, int stages, int mcast, int tile_n, const CUtensorMap* tmA0,
+                const CUtensorMap* tmB0, const CUtensorMap* tmA1, const CUtensorMap* tmB1, const CUtensorMap* tmG,
+                const KernelParams& p, int num_sms, cudaStream_t stream);
 
 // loss = inv_b * S0 ; dbias = inv_b * S1 ; dt_prime = exp(t') * inv_b * S2  (S* = fixed-order sums of partials)
 // dtxt[j, d] = sum_r slots[r][j, d]   (slots may be peer-mapped pointers; fp32; n = elements)

@@ -40,17 +40,20 @@ enum {
  *   SIGLIP_DEBUG_NO_GSTORE, SIGLIP_DEBUG_NO_CVT   timing experiments: skip the sigma store / the fp16 operand copies
  *                                (the gradients are then WRONG)
  *   SIGLIP_DEBUG_PRINT_TIMES     print the per-launch CUDA-event times collected under SIGLIP_OPT_KERNEL_TIMING
- *   SIGLIP_DEBUG_MCAST, _AB_F16, _AB_FP8, _WAITSTATS, _STAGES   variants of siglip_debug_gemm(_timed) only
+ *   SIGLIP_DEBUG_MCAST, _AB_F16, _AB_FP8, _WAITSTATS, _STAGES, _TILE_N (128 or 256)   variants of
+ *                                siglip_debug_gemm(_timed) only
  */
 
 /* tuning knobs (siglip_ctx_set_option) */
 enum {
   SIGLIP_OPT_CTA_GROUP = 1, /* 1: every CTA computes its own 128-row tile; 2 (default): clusters of two CTAs on adjacent
-                               128-row blocks share the B tile by TMA multicast. Tiles are 128 columns wide */
+                               128-row blocks share the B tile by TMA multicast. Loss-kernel tiles are 128 columns
+                               wide, gradient-kernel tiles 128 or 256 (SIGLIP_OPT_GRAD_TILE_N) */
   SIGLIP_OPT_OVERLAP_PULL = 2, /* 1 (default): pull the next text chunk inside the loss kernel; 0: separate copy */
   SIGLIP_OPT_KERNEL_TIMING = 3, /* 1: bracket every loss / gradient kernel launch with CUDA events on the caller's stream */
   SIGLIP_OPT_STAGES_LOSS = 4,  /* TMA->MMA pipeline depth of the loss kernel: 0 (default, = 6), 4 or 6 */
-  SIGLIP_OPT_STAGES_GRAD = 5,  /* ... of the gradient kernel */
+  SIGLIP_OPT_STAGES_GRAD = 5,  /* ... of the gradient kernel with 128-column tiles; 256-column tiles (48 KiB per stage)
+                                  always run 4 stages, whatever is asked */
   SIGLIP_OPT_MCAST = 6,        /* 2: twice as many vertically adjacent CTAs share the B tile by TMA multicast (cta_group 2:
                                   clusters of 4); default 1 */
   SIGLIP_OPT_GRAD_BF16 = 7,     /* 1: siglip_fwd_bwd writes dimg / dtxt as bf16 [B, D] (the dtype autograd returns for bf16 inputs); default 0 = fp32 */
@@ -70,8 +73,12 @@ enum {
                                 bf16: 11 significant bits for callers with fp32 embeddings (the reference's own test feeds fp32,
                                 test_distributed_sigmoid_loss.py:57-68; bf16 rounding of such inputs costs 1.7e-3 in the
                                 gradients, this format 2e-4). Same on all ranks. Default 0 */
-  SIGLIP_OPT_GRAD_TILE_N = 14, /* 0, 128 or 256; accepted, no effect on sm_90a: every column tile is 128 wide (the wgmma
-                                  accumulator lives in registers) */
+  SIGLIP_OPT_GRAD_TILE_N = 14, /* column tiles of the gradient kernel: 128 (wgmma m64n128), 256 (m64n256: one
+                                  instruction per k step instead of two, a third less operand traffic per FLOP) or 0
+                                  (default): 256 when 1.8 x its waves over the persistent grid are at most the waves
+                                  of 128-column tiles (B = 16384 with D = 768, 1024 or 1152), else 128 (D <= 128,
+                                  B = 16384 with D = 384, B = 4096 with D = 768). Same results bit for bit. Split-K
+                                  (SIGLIP_OPT_SPLIT_K with SIGLIP_OPT_MCAST 1) always takes 128 */
   SIGLIP_OPT_PEER_TIMEOUT_MS = 15, /* bound of every in-kernel wait on a PEER rank (text-ready / contribution-ready /
                                       buffer-free flags, scalar exchange). Default 600000 (10 min, the order of a process
                                       group's collective timeout: a peer may be late by a checkpoint save or an evaluation
