@@ -23,6 +23,7 @@ EXPORTED_SYMBOLS = (
     "siglip_ctx_create",
     "siglip_ctx_create_uneven",
     "siglip_ctx_create_texts",
+    "siglip_ctx_create_extras",
     "siglip_ctx_set_option",
     "siglip_ctx_workspace_bytes",
     "siglip_ctx_handle_bytes",
@@ -36,6 +37,7 @@ EXPORTED_SYMBOLS = (
     "siglip_fwd",
     "siglip_set_sample_ids",
     "siglip_set_extra_text_ids",
+    "siglip_set_extra_image_ids",
     "siglip_set_sample_weights",
     "siglip_request_metrics",
     "siglip_fwd_bwd_host",
@@ -60,6 +62,7 @@ EXPORTED_SYMBOLS = (
     "siglip_debug_set_chunk_weights",
     "siglip_debug_set_mailbox",
     "siglip_debug_set_peer_metric_keys",
+    "siglip_debug_set_peer_extra_image_ids",
     "siglip_ctx_aux_trace",
     "siglip_ctx_destroy",
 )
@@ -93,6 +96,7 @@ SIGLIP_OPT_TPRIME_F64 = 20
 SIGLIP_OPT_SAMPLE_IDS = 21
 SIGLIP_OPT_EXTRA_TEXT_IDS = 22
 SIGLIP_OPT_SAMPLE_WEIGHTS = 23
+SIGLIP_OPT_EXTRA_IMAGE_IDS = 24
 
 _lib: Optional[ctypes.CDLL] = None
 
@@ -155,6 +159,13 @@ def lib() -> ctypes.CDLL:
     L.siglip_ctx_create_uneven.restype = ci
     L.siglip_ctx_create_texts.argtypes = [ctypes.POINTER(vp), ci, ci, ci, ctypes.POINTER(ci), ctypes.POINTER(ci), ci]
     L.siglip_ctx_create_texts.restype = ci
+    L.siglip_ctx_create_extras.argtypes = [ctypes.POINTER(vp), ci, ci, ci, ctypes.POINTER(ci), ctypes.POINTER(ci),
+                                           ctypes.POINTER(ci), ci]
+    L.siglip_ctx_create_extras.restype = ci
+    L.siglip_set_extra_image_ids.argtypes = [vp, vp, vp]
+    L.siglip_set_extra_image_ids.restype = ci
+    L.siglip_debug_set_peer_extra_image_ids.argtypes = [vp, ci, vp, vp]
+    L.siglip_debug_set_peer_extra_image_ids.restype = ci
     L.siglip_host_submit_grads.argtypes = [vp, vp, vp, ctypes.c_float, ctypes.c_float, vp, vp,
                                            ctypes.POINTER(ctypes.c_ulonglong), vp]
     L.siglip_host_submit_grads.restype = ci

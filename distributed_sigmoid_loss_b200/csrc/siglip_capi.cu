@@ -152,6 +152,8 @@ struct IpcBlob {
   int Bmax;
   int T;      // texts of the rank (B + its hard negatives)
   int Tmax;
+  int R;      // images of the rank (B + its extra images)
+  int Rmax;
   char host[64];
 };
 
@@ -169,6 +171,24 @@ struct siglip_ctx {
   int Tp = 0;                            // columns of the sigma operands: Tmax rounded up to 256
   bool extras = false;                   // some rank has hard negatives (T_p != B_p)
   int toff[kMaxWorld + 1] = {};          // global index of every rank's first text (prefix sums of Ts)
+  // extra images (siglip_ctx_create_extras): rank p holds Rs[p] = Bs[p] + E_p images, its B_p paired images followed by
+  // E_p extras. Images never leave their rank. Without extra images Rs == Bs and everything below is what it was before
+  // they existed.
+  int R = 0;                             // this rank's images: rows of img / dimg
+  int Rs[kMaxWorld] = {};
+  int Rmax = 0;
+  int Rp = 0;                            // rows of the sigma operands: Rmax rounded up to 256
+  int Emax = 0;                          // max over ranks of the extra images (published ids per metrics step)
+  bool ximg = false;                     // some rank has extra images (R_p != B_p)
+  // this rank has extra images AND extra texts: the own chunk's positional diagonal row == col would also meet extra
+  // rows and extra columns, so its loss kernel runs with own_chunk = 0 and takes every positive from ids instead (the
+  // kIds instantiation, with row and column bounds; positional labels use iota ids)
+  bool own_pos_ids = false;
+  int extra_image_ids = 0;               // SIGLIP_OPT_EXTRA_IMAGE_IDS: the extra images carry ids (needs sample_ids)
+  bool ximg_ids_set = false;             // siglip_set_extra_image_ids was called since the previous step
+  int64_t* rids = nullptr;               // [R] ids of my images: B sample ids, then E extra-image ids (R > B only;
+                                         // R == B: ids_in). Never exported
+  int64_t* iota = nullptr;               // [max(R, T)] 0, 1, 2, ...: the positional labels of own_pos_ids
   int num_sms = 0;
   // options
   int cta_group = 2;
@@ -196,7 +216,7 @@ struct siglip_ctx {
   bool extra_ids_set = false;            // siglip_set_extra_text_ids was called since the previous step
   int sample_weights = 0;                // SIGLIP_OPT_SAMPLE_WEIGHTS: per-sample loss weights (collective)
   bool weights_set = false;              // siglip_set_sample_weights was called since the previous step
-  int off[kMaxWorld + 1] = {};           // global index of every rank's first sample (prefix sums of Bs)
+  int off[kMaxWorld + 1] = {};           // global index of every rank's first image (prefix sums of Rs)
   // retrieval metrics (siglip_request_metrics), armed for the next step only
   bool metrics_armed = false;
   float* m_top1 = nullptr;
@@ -214,19 +234,20 @@ struct siglip_ctx {
   int ids_stride = 0;                    // Tmax rounded up to even: every slot is a whole number of 16-byte vectors.
                                          // Fixed at creation (options are set after the handle exchange)
   unsigned long long* mkeys[2] = {};     // per step parity: [world][Tmax] column argmax partials of every text chunk
-                                         // over my images, then [Bmax] row keys. world > 1: behind ids_all (exported)
+                                         // over my images, then [Rmax] row keys, then [Emax] my extra-image ids (world > 1
+                                         // under SIGLIP_OPT_EXTRA_IMAGE_IDS). world > 1: behind ids_all (exported)
   float* w_all = nullptr;                // [world][w_stride] text weights of every chunk (world > 1): behind the metric
                                          // keys in the exported allocation, sized at creation whatever the options
-  float* w_in = nullptr;                 // [w_stride] my text weights, then [B] my image weights, clamped into [0, 1];
+  float* w_in = nullptr;                 // [w_stride] my text weights, then [R] my image weights, clamped into [0, 1];
                                          // allocated by the first siglip_set_sample_weights
   int w_stride = 0;                      // Tmax rounded up to 4: every slot is a whole number of 16-byte vectors
-  __nv_bfloat16* G[kMaxWorld] = {};      // [Bp, Tp] sigma operands (fp16 bits x kGScale), diagonal zeroed, allocated on
+  __nv_bfloat16* G[kMaxWorld] = {};      // [Rp, Tp] sigma operands (fp16 bits x kGScale), diagonal zeroed, allocated on
                                          // first use: fused step 2 (own chunk + the chunk in flight), split API one per chunk
-  __nv_bfloat16* img16 = nullptr;        // [B, D] fp16 (x kXScale) images: B operand of the dtxt contraction
+  __nv_bfloat16* img16 = nullptr;        // [R, D] fp16 (x kXScale) images: B operand of the dtxt contraction
   __nv_bfloat16* txt16[kMaxWorld] = {};  // [Tmax, D] fp16 (x kXScale) text chunks: B operand of dimg (same count as G)
   float* g_diag = nullptr;               // [Bp] fp32 positive-pair terms -sigma(-z_ii)
   float* slots = nullptr;                // [world][Tmax, D] fp32 dtxt contributions, slot c is for owner c (world > 1)
-  float* dimg_acc = nullptr;             // [B, D] fp32 running dimg over the chunks (world > 1)
+  float* dimg_acc = nullptr;             // [R, D] fp32 running dimg over the chunks (world > 1)
   float* dtxt_acc = nullptr;             // [T, D] fp32 running sum of the peers' contributions (world > 1)
   double* partials = nullptr;            // [num_sms][4]
   unsigned int* fin_counter = nullptr;   // ticket counter of the loss kernel's last-CTA finalisation
@@ -235,6 +256,7 @@ struct siglip_ctx {
   float* loop_mailboxes = nullptr;       // loopback only: [world][2] stand-ins for the peers' (dt', dbias) mailboxes
   float* loop_zero = nullptr;            // loopback only: [world][Tmax, D] zeros standing in for the peers' contribution slots
   unsigned long long* loop_keys = nullptr;  // loopback only: [world][Tmax] the peers' column partials of my chunk
+  int64_t* loop_xids = nullptr;          // loopback only: [world][Emax] the peers' published extra-image ids
   float* scalars = nullptr;              // [24] device scalars: host API staging, saved dt'/dbias of the last forward
   unsigned long long* aux_trace = nullptr;  // [kTraceLaunches][16] globaltimer stamps (SIGLIP_OPT_AUX_TRACE)
   float* splitk_ws = nullptr;            // fp32 partial accumulators of the split tiles of the gradient kernel
@@ -252,6 +274,7 @@ struct siglip_ctx {
   unsigned int** signal_ptrs_dev = nullptr;  // [kFlagKinds][world]
   const float** mailbox_ptrs_dev = nullptr;  // [world] every rank's (dt', dbias) mailbox
   const unsigned long long** mkey_ptrs_dev = nullptr;  // [2][world] every rank's column partial of my chunk, per parity
+  const int64_t** xid_ptrs_dev = nullptr;    // [2][world] every rank's published extra-image ids, per parity
   unsigned int n_fwd = 0, n_bwd = 0;         // forward / backward passes issued (flag counters)
   unsigned int prewait3 = 0;                 // highest n for which "peers finished backward n" has been waited for
   unsigned long long gen = 0;                // generation of the state saved for backward (0 = none)
@@ -334,14 +357,23 @@ int take_ids(siglip_ctx* c) {
   if (c->sample_ids && c->extra_text_ids && !c->extra_ids_set)
     return fail(SIGLIP_ERR_STATE,
                 "SIGLIP_OPT_EXTRA_TEXT_IDS is on but siglip_set_extra_text_ids was not called since the previous step");
+  if (c->sample_ids && c->extra_image_ids && !c->ximg_ids_set)
+    return fail(SIGLIP_ERR_STATE,
+                "SIGLIP_OPT_EXTRA_IMAGE_IDS is on but siglip_set_extra_image_ids was not called since the previous step");
   if (c->sample_weights && !c->weights_set)
     return fail(SIGLIP_ERR_STATE,
                 "SIGLIP_OPT_SAMPLE_WEIGHTS is on but siglip_set_sample_weights was not called since the previous step");
   c->ids_set = false;
   c->extra_ids_set = false;
+  c->ximg_ids_set = false;
   c->weights_set = false;
   return 0;
 }
+
+// ids of my images as the loss kernel reads them (ids mode): the sample ids, then the extra images' ids
+inline const int64_t* row_ids(const siglip_ctx* c) { return c->rids != nullptr ? c->rids : c->ids_in; }
+// rows that carry ids: the paired images, and under SIGLIP_OPT_EXTRA_IMAGE_IDS the extras too
+inline int row_id_count(const siglip_ctx* c) { return c->extra_image_ids ? c->R : c->B; }
 
 // ---- per-sample weights (SIGLIP_OPT_SAMPLE_WEIGHTS) ----
 // Text weights of chunk `cidx` as the loss kernel reads them (null outside the mode): mine for the own chunk, the
@@ -360,11 +392,14 @@ inline unsigned long long peer_timeout_ns(const siglip_ctx* c) {
 
 // ---- retrieval metrics (siglip_request_metrics) ----
 static_assert(siglip::kMetricsMaxWorld == kMaxWorld, "the finalisation kernel takes one batch offset per rank");
-// 64-bit keys per step parity: [world][Tmax] column partials (the loss kernel writes one per text of the chunk; the
-// finalisation reads the paired ones), then [Bmax] row keys
+// 64-bit words per step parity: [world][Tmax] column partials (the loss kernel writes one per text of the chunk; the
+// finalisation reads the paired ones), then [Rmax] row keys, then [Emax] extra-image ids of this rank (published for the
+// peers' t2i hit test under SIGLIP_OPT_EXTRA_IMAGE_IDS). Without extra images: [Bmax] row keys and nothing behind.
 inline size_t mkeys_block(const siglip_ctx* c) {
-  return static_cast<size_t>(c->world) * c->Tmax + static_cast<size_t>(c->Bmax);
+  return static_cast<size_t>(c->world) * c->Tmax + static_cast<size_t>(c->Rmax) + static_cast<size_t>(c->Emax);
 }
+// offset of the published extra-image ids in a key block
+inline size_t mkeys_xids(const siglip_ctx* c) { return static_cast<size_t>(c->world) * c->Tmax + c->Rmax; }
 inline size_t mkeys_rows(const siglip_ctx* c) { return static_cast<size_t>(c->world) * c->Tmax; }
 // byte offset of the two key blocks in the exported text allocation: behind the gathered text and ids
 inline size_t mkeys_offset(const siglip_ctx* c) {
@@ -390,6 +425,12 @@ int take_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
   c->mkeys_step = c->mkeys[s & 1u];
   CK(cudaMemsetAsync(c->mkeys_step, 0, mkeys_block(c) * sizeof(unsigned long long), st));
   c->launches++;
+  if (c->world > 1 && c->sample_ids && c->extra_image_ids && c->R > c->B) {
+    // my extra images' ids, for the peers whose texts an extra image of mine wins: read by their finalisation after
+    // flag kind 5 of this step, reused two steps later like the keys
+    CK(cudaMemcpyAsync(c->mkeys_step + mkeys_xids(c), c->rids + c->B,
+                       static_cast<size_t>(c->R - c->B) * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
+  }
   return 0;
 }
 // After the step's last loss kernel: combine the keys (W > 1: with every rank's partials of my chunk, flag kind 5) and
@@ -402,18 +443,23 @@ int finalize_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
   a.row_keys = c->mkeys_step + mkeys_rows(c);
   a.col_own = c->mkeys_step + static_cast<size_t>(c->rank) * c->Tmax;
   a.B = c->B;
+  a.R = c->R;
   a.rank = c->rank;
   a.world = W;
   for (int p = 0; p <= W; ++p) {
     a.off[p] = c->off[p];
     a.toff[p] = c->toff[p];
   }
+  for (int p = 0; p < W; ++p) a.bs[p] = c->Bs[p];
   a.T = c->T;
   if (c->sample_ids) {
     a.ids_own = c->ids_in;
+    a.row_ids = row_ids(c);
     a.ids_all = c->ids_all;
     a.ids_stride = c->ids_stride;
     a.extra_ids = c->extra_text_ids;
+    a.extra_image_ids = c->extra_image_ids;
+    if (W > 1 && c->xid_ptrs_dev != nullptr) a.xids_peers = c->xid_ptrs_dev + static_cast<size_t>(s & 1u) * W;
   }
   a.top1 = c->m_top1;
   a.i2t = c->m_i2t;
@@ -436,7 +482,7 @@ int finalize_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
 // flight), the split forward / backward API one per text chunk (they all live from the forward to the backward).
 int ensure_g(siglip_ctx* c, int i) {
   if (c->G[i] != nullptr) return 0;
-  const size_t gbytes = static_cast<size_t>(c->Bp) * c->Tp * sizeof(__nv_bfloat16);
+  const size_t gbytes = static_cast<size_t>(c->Rp) * c->Tp * sizeof(__nv_bfloat16);
   const size_t tbytes = chunk_stride(c) * sizeof(__nv_bfloat16);
   cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&c->G[i]), gbytes);
   if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&c->txt16[i]), tbytes);
@@ -448,7 +494,7 @@ int ensure_g(siglip_ctx* c, int i) {
     snprintf(buf, sizeof(buf),
              "sigma operand %d needs %.2f GiB more device memory (B = %d: %d x %d 16-bit per text chunk kept for the "
              "backward; siglip_fwd_bwd needs 2 of them, the split forward/backward API one per rank): %s",
-             i, static_cast<double>(gbytes + tbytes) / (1024.0 * 1024.0 * 1024.0), c->Bmax, c->Bp, c->Tp,
+             i, static_cast<double>(gbytes + tbytes) / (1024.0 * 1024.0 * 1024.0), c->Bmax, c->Rp, c->Tp,
              cudaGetErrorString(e));
     return fail(SIGLIP_ERR_CUDA, buf);
   }
@@ -527,12 +573,12 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
   if ((rc = ensure_g(c, save ? gi : 0))) return rc;
   __nv_bfloat16* G = c->G[save ? gi : 0];
   CUtensorMap tmA, tmB, tmG;
-  if ((rc = encode_operand(&tmA, img, c->B, c->D, c->D, 0, 128))) return rc;
+  if ((rc = encode_operand(&tmA, img, c->R, c->D, c->D, 0, 128))) return rc;
   const int mc = c->mcast;
   if ((rc = encode_operand(&tmB, txt_c, Bn, c->D, c->D, 0, siglip::b_box_rows_kmajor(siglip::cluster_size(cg, mc)))))
     return rc;
-  // store map of the sigma operand: [B, Bn] inside the padded [Bp, Tp] buffer, one 16-row x 32-column slab per TMA store
-  if ((rc = encode_bf16_2d(&tmG, G, (uint64_t)Bn, (uint64_t)c->B, (uint64_t)c->Tp, 32, 16,
+  // store map of the sigma operand: [R, Bn] inside the padded [Rp, Tp] buffer, one 16-row x 32-column slab per TMA store
+  if ((rc = encode_bf16_2d(&tmG, G, (uint64_t)Bn, (uint64_t)c->R, (uint64_t)c->Tp, 32, 16,
                            CU_TENSOR_MAP_SWIZZLE_64B)))
     return rc;
   KernelParams p;
@@ -541,7 +587,8 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
   // fp32-input path: both operands are fp16(x * kXScale), the accumulator is kXScale^2 <img, txt>
   p.prob[0].ab_f16 = c->input_f16;
   p.s_scale = c->input_f16 ? 1.0f / (kXScale * kXScale) : 1.0f;
-  p.prob[0].M = c->B;
+  // rows: my images, the paired ones and then the extras; the loss still divides by the paired batch
+  p.prob[0].M = c->R;
   p.prob[0].N = Bn;
   p.prob[0].K = c->D;
   p.t_prime = t_prime;
@@ -550,15 +597,24 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
   p.G = G;
   p.ldg = c->Tp;
   p.g_diag = c->g_diag;
-  // the own chunk's positives are its first B columns (row == col < M); the hard negatives behind them never are
-  p.own_chunk = own ? 1 : 0;
+  // the own chunk's positives are its first B columns (row == col < M); the hard negatives behind them never are. With
+  // extra images and extra texts on this rank, row == col would also meet them: the own chunk then takes its positives
+  // from ids, bounded to the first B rows and columns (iota ids for positional labels), and leaves g_diag alone
+  p.own_chunk = (own && !c->own_pos_ids) ? 1 : 0;
   p.store_g = save ? 1 : 0;
   p.g_scale = kGScale;
   if (col_ids != nullptr) {
-    p.row_ids = c->ids_in;
+    p.row_ids = row_ids(c);
     p.col_ids = col_ids;
     // the chunk's ids cover its paired texts, and under SIGLIP_OPT_EXTRA_TEXT_IDS its extras too
     p.col_pos_n = chunk_id_count(c, cidx);
+    // the rows' ids cover the paired images, and under SIGLIP_OPT_EXTRA_IMAGE_IDS the extras too
+    p.row_pos_n = row_id_count(c);
+  } else if (own && c->own_pos_ids) {
+    p.row_ids = c->iota;
+    p.col_ids = c->iota;
+    p.col_pos_n = c->B;
+    p.row_pos_n = c->B;
   }
   if (c->sample_weights) {   // the kWeights instantiation: w_ij = image weight i x text weight j of the chunk
     p.row_w = image_weights(c);
@@ -619,7 +675,7 @@ void add_img_cvt_job(siglip_ctx* c, AuxList& aux, const void* img) {
   siglip::AuxJob& ji = aux.add(siglip::kAuxCvt);
   ji.src = reinterpret_cast<const uint4*>(img);
   ji.dst = reinterpret_cast<uint4*>(c->img16);
-  ji.n16 = static_cast<unsigned long long>(c->B) * c->D * sizeof(__nv_bfloat16) / 16;
+  ji.n16 = static_cast<unsigned long long>(c->R) * c->D * sizeof(__nv_bfloat16) / 16;
   ji.cvt_copy = c->input_f16;
 }
 
@@ -677,15 +733,17 @@ int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_
                    const float* t_prime, const float* grad_out, const GradOut& o, const AuxList& aux,
                    const EndSignal& end, cudaStream_t st) {
   const int cg = c->cta_group;
-  const int tile_n = grad_tile_cols(c, c->B, Bn);
+  const int tile_n = grad_tile_cols(c, c->R, Bn);
   const int bk = siglip::b_box_k_mnmajor(siglip::cluster_size(cg, c->mcast), tile_n);
   CUtensorMap tmA0, tmB0, tmA1, tmB1;
   int rc;
   if (c->G[gi] == nullptr) return fail(SIGLIP_ERR_STATE, "gradient kernel without a saved sigma operand");
-  if ((rc = encode_operand(&tmA0, c->G[gi], c->B, Bn, c->Tp, 0, 128))) return rc;
+  // G is [R, Bn]: the MN-major map of the dtxt problem reads R k-rows of it and the image copy R rows; TMA fills the
+  // boxes past R with zeros, so a partial last k block adds nothing
+  if ((rc = encode_operand(&tmA0, c->G[gi], c->R, Bn, c->Tp, 0, 128))) return rc;
   if ((rc = encode_operand(&tmB0, c->txt16[gi], c->D, Bn, c->D, 1, 0, bk))) return rc;
-  if ((rc = encode_operand(&tmA1, c->G[gi], Bn, c->B, c->Tp, 1, 0))) return rc;
-  if ((rc = encode_operand(&tmB1, c->img16, c->D, c->B, c->D, 1, 0, bk))) return rc;
+  if ((rc = encode_operand(&tmA1, c->G[gi], Bn, c->R, c->Tp, 1, 0))) return rc;
+  if ((rc = encode_operand(&tmB1, c->img16, c->D, c->R, c->D, 1, 0, bk))) return rc;
   KernelParams p;
   memset(&p, 0, sizeof(p));
   p.nprob = 2;
@@ -697,30 +755,30 @@ int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_
     pr.acc_scale = 1.0f / (kGScale * kXScale);
     pr.ldo = c->D;
     pr.ldx = c->D;
-    pr.fix_vec = own ? c->g_diag : nullptr;
+    pr.fix_vec = (own && !c->own_pos_ids) ? c->g_diag : nullptr;   // own_pos_ids: the positives are in G
     pr.fix_f16 = c->saved_f16;
     pr.fix_mat_scale = c->saved_f16 ? 1.0f / kXScale : 1.0f;
   }
-  p.prob[0].M = c->B;
+  p.prob[0].M = c->R;
   p.prob[0].K = Bn;
   p.prob[0].a_mn = 0;
   p.prob[0].out = o.dimg_out;
   p.prob[0].out_bf16 = o.dimg_bf16 ? 1 : 0;
   p.prob[0].add_src = o.dimg_add;
   p.prob[0].ld_add = c->D;
-  p.prob[0].fix_mat = own ? txt_own : nullptr;
+  p.prob[0].fix_mat = (own && !c->own_pos_ids) ? txt_own : nullptr;
   p.prob[1].M = Bn;
-  p.prob[1].K = c->B;
+  p.prob[1].K = c->R;
   p.prob[1].a_mn = 1;
   p.prob[1].out = o.dtxt_out;
   p.prob[1].out_bf16 = o.dtxt_bf16 ? 1 : 0;
   p.prob[1].add_src = o.dtxt_add;
   p.prob[1].ld_add = c->D;
-  p.prob[1].fix_mat = own ? reinterpret_cast<const __nv_bfloat16*>(img) : nullptr;
+  p.prob[1].fix_mat = (own && !c->own_pos_ids) ? reinterpret_cast<const __nv_bfloat16*>(img) : nullptr;
   p.p1_wait_flag = o.dtxt_add_flag;
   p.p1_wait_value = o.dtxt_add_value;
-  // g_diag and both fix matrices hold this rank's B rows; the dtxt rows of the own chunk's hard negatives (B .. Bn) have
-  // no positive-pair term
+  // g_diag and both fix matrices hold this rank's B rows; the dtxt rows of the own chunk's hard negatives (B .. Bn) and
+  // the dimg rows of its extra images (B .. R) have no positive-pair term
   p.fix_rows = c->B;
   if (o.sc_dt_prime != nullptr || o.sc_dbias != nullptr) {
     p.sc_saved = c->scalars + kSavedScalars;
@@ -1228,20 +1286,25 @@ int siglip_device_count(void) {
   return ok;
 }
 
-// Bs[p]: rank p's images; Ts[p] >= Bs[p]: its texts (paired ones first, then its hard negatives). Every argument is
-// checked before the first CUDA call.
-static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, const int* Bs, const int* Ts, int D) {
+// Bs[p]: rank p's batch; Rs[p] >= Bs[p]: its images (paired ones first, then its extra images); Ts[p] >= Bs[p]: its
+// texts (paired ones first, then its hard negatives). Every argument is checked before the first CUDA call.
+static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, const int* Bs, const int* Rs,
+                           const int* Ts, int D) {
   if (out == nullptr) return fail(SIGLIP_ERR_INVALID, "out is null");
   *out = nullptr;
   if (world < 1 || world > kMaxWorld || rank < 0 || rank >= world)
     return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
-  int Bmax = 0, Tmax = 0;
+  int Bmax = 0, Tmax = 0, Rmax = 0, Emax = 0;
   for (int p = 0; p < world; ++p) {
     if (Bs[p] < 1) return fail(SIGLIP_ERR_INVALID, "need B >= 1 on every rank");
     if (Ts[p] < Bs[p])
-      return fail(SIGLIP_ERR_INVALID, "need texts_per_rank[p] >= images_per_rank[p] (paired texts, then hard negatives)");
+      return fail(SIGLIP_ERR_INVALID, "need texts_per_rank[p] >= batch_per_rank[p] (paired texts, then hard negatives)");
+    if (Rs[p] < Bs[p])
+      return fail(SIGLIP_ERR_INVALID, "need images_per_rank[p] >= batch_per_rank[p] (paired images, then extra images)");
     Bmax = Bs[p] > Bmax ? Bs[p] : Bmax;
     Tmax = Ts[p] > Tmax ? Ts[p] : Tmax;
+    Rmax = Rs[p] > Rmax ? Rs[p] : Rmax;
+    Emax = Rs[p] - Bs[p] > Emax ? Rs[p] - Bs[p] : Emax;
   }
   if (D < 8 || (D % 8) != 0) return fail(SIGLIP_ERR_INVALID, "need D a positive multiple of 8");
   int ndev = 0;
@@ -1268,17 +1331,24 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   for (int p = 0; p < world; ++p) {
     c->Bs[p] = Bs[p];
     c->Ts[p] = Ts[p];
+    c->Rs[p] = Rs[p];
     c->extras = c->extras || Ts[p] != Bs[p];
+    c->ximg = c->ximg || Rs[p] != Bs[p];
   }
   c->B = Bs[rank];
   c->T = Ts[rank];
+  c->R = Rs[rank];
   c->Bmax = Bmax;
   c->Tmax = Tmax;
+  c->Rmax = Rmax;
+  c->Emax = Emax;
+  c->own_pos_ids = c->R > c->B && c->T > c->B;
   c->D = D;
   c->Bp = round_up(Bmax, 256);
   c->Tp = round_up(Tmax, 256);
+  c->Rp = round_up(Rmax, 256);
   for (int p = 0; p < world; ++p) {
-    c->off[p + 1] = c->off[p] + Bs[p];
+    c->off[p + 1] = c->off[p] + Rs[p];
     c->toff[p + 1] = c->toff[p] + Ts[p];
   }
   c->dbg_no_gstore = getenv("SIGLIP_DEBUG_NO_GSTORE") != nullptr;
@@ -1303,7 +1373,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     return e;
   };
   CK(alloc(reinterpret_cast<void**>(&c->g_diag), static_cast<size_t>(c->Bp) * sizeof(float)));
-  CK(alloc(reinterpret_cast<void**>(&c->img16), static_cast<size_t>(c->B) * D * sizeof(__nv_bfloat16)));
+  CK(alloc(reinterpret_cast<void**>(&c->img16), static_cast<size_t>(c->R) * D * sizeof(__nv_bfloat16)));
   CK(alloc(reinterpret_cast<void**>(&c->partials), static_cast<size_t>(c->num_sms) * 4 * sizeof(double)));
   CK(alloc(reinterpret_cast<void**>(&c->fin_counter), sizeof(unsigned int)));
   CK(alloc(reinterpret_cast<void**>(&c->flags), kFlagBytes));
@@ -1314,6 +1384,14 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   c->ids_stride = round_up(Tmax, 2);
   const size_t ids_slot_bytes = static_cast<size_t>(c->ids_stride) * sizeof(int64_t);
   CK(alloc(reinterpret_cast<void**>(&c->ids_in), ids_slot_bytes));
+  if (c->R > c->B) CK(alloc(reinterpret_cast<void**>(&c->rids), static_cast<size_t>(c->R) * sizeof(int64_t)));
+  if (c->own_pos_ids) {
+    const int n = c->R > c->T ? c->R : c->T;
+    std::vector<int64_t> iota(n);
+    for (int i = 0; i < n; ++i) iota[i] = i;
+    CK(alloc(reinterpret_cast<void**>(&c->iota), n * sizeof(int64_t)));
+    CK(cudaMemcpy(c->iota, iota.data(), n * sizeof(int64_t), cudaMemcpyHostToDevice));
+  }
   const size_t mkeys_bytes = 2 * mkeys_block(c) * sizeof(unsigned long long);
   c->w_stride = round_up(Tmax, 4);
   if (world > 1) {
@@ -1328,13 +1406,14 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     c->mkeys[1] = c->mkeys[0] + mkeys_block(c);
     c->w_all = reinterpret_cast<float*>(reinterpret_cast<char*>(c->txt_all) + weights_offset(c));
     CK(alloc(reinterpret_cast<void**>(&c->slots), stride * world * sizeof(float)));
-    CK(alloc(reinterpret_cast<void**>(&c->dimg_acc), static_cast<size_t>(c->B) * D * sizeof(float)));
+    CK(alloc(reinterpret_cast<void**>(&c->dimg_acc), static_cast<size_t>(c->R) * D * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dtxt_acc), static_cast<size_t>(c->T) * D * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->reduce_ptrs_dev), world * sizeof(float*)));
     CK(alloc(reinterpret_cast<void**>(&c->final_ptrs_dev), 2 * sizeof(float*)));
     CK(alloc(reinterpret_cast<void**>(&c->signal_ptrs_dev), kFlagKinds * world * sizeof(unsigned int*)));
     CK(alloc(reinterpret_cast<void**>(&c->mailbox_ptrs_dev), world * sizeof(float*)));
     CK(alloc(reinterpret_cast<void**>(&c->mkey_ptrs_dev), 2 * world * sizeof(unsigned long long*)));
+    if (c->ximg) CK(alloc(reinterpret_cast<void**>(&c->xid_ptrs_dev), 2 * world * sizeof(int64_t*)));
     const float* fin[2] = {c->dtxt_acc, c->slots + rank * stride};
     CK(cudaMemcpy(c->final_ptrs_dev, fin, sizeof(fin), cudaMemcpyHostToDevice));
   }
@@ -1357,13 +1436,13 @@ int siglip_ctx_create(siglip_ctx** out, int device, int rank, int world, int B, 
   if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
   int Bs[kMaxWorld];
   for (int p = 0; p < world; ++p) Bs[p] = B;
-  return ctx_create_impl(out, device, rank, world, Bs, Bs, D);
+  return ctx_create_impl(out, device, rank, world, Bs, Bs, Bs, D);
 }
 
 int siglip_ctx_create_uneven(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank, int D) {
   if (batch_per_rank == nullptr) return fail(SIGLIP_ERR_INVALID, "batch_per_rank is null");
   if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
-  return ctx_create_impl(out, device, rank, world, batch_per_rank, batch_per_rank, D);
+  return ctx_create_impl(out, device, rank, world, batch_per_rank, batch_per_rank, batch_per_rank, D);
 }
 
 int siglip_ctx_create_texts(siglip_ctx** out, int device, int rank, int world, const int* images_per_rank,
@@ -1371,7 +1450,15 @@ int siglip_ctx_create_texts(siglip_ctx** out, int device, int rank, int world, c
   if (images_per_rank == nullptr || texts_per_rank == nullptr)
     return fail(SIGLIP_ERR_INVALID, "images_per_rank / texts_per_rank is null");
   if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
-  return ctx_create_impl(out, device, rank, world, images_per_rank, texts_per_rank, D);
+  return ctx_create_impl(out, device, rank, world, images_per_rank, images_per_rank, texts_per_rank, D);
+}
+
+int siglip_ctx_create_extras(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank,
+                             const int* images_per_rank, const int* texts_per_rank, int D) {
+  if (batch_per_rank == nullptr || images_per_rank == nullptr || texts_per_rank == nullptr)
+    return fail(SIGLIP_ERR_INVALID, "batch_per_rank / images_per_rank / texts_per_rank is null");
+  if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
+  return ctx_create_impl(out, device, rank, world, batch_per_rank, images_per_rank, texts_per_rank, D);
 }
 
 int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
@@ -1414,8 +1501,15 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
     case SIGLIP_OPT_SAMPLE_IDS:
       c->sample_ids = value ? 1 : 0;
       c->ids_set = false;
-      if (!c->sample_ids) c->extra_text_ids = 0;   // the extras' ids extend the sample ids
+      if (!c->sample_ids) c->extra_text_ids = c->extra_image_ids = 0;   // the extras' ids extend the sample ids
       c->extra_ids_set = false;
+      c->ximg_ids_set = false;
+      return 0;
+    case SIGLIP_OPT_EXTRA_IMAGE_IDS:
+      if (value && !c->sample_ids)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_EXTRA_IMAGE_IDS needs SIGLIP_OPT_SAMPLE_IDS on first");
+      c->extra_image_ids = value ? 1 : 0;
+      c->ximg_ids_set = false;
       return 0;
     case SIGLIP_OPT_EXTRA_TEXT_IDS:
       if (value && !c->sample_ids)
@@ -1493,6 +1587,8 @@ int siglip_ctx_export_handles(siglip_ctx* c, void* out_bytes, size_t capacity) {
   b.Bmax = c->Bmax;
   b.T = c->T;
   b.Tmax = c->Tmax;
+  b.R = c->R;
+  b.Rmax = c->Rmax;
   if (gethostname(b.host, sizeof(b.host) - 1) != 0) b.host[0] = 0;
   memcpy(out_bytes, &b, sizeof(b));
   return 0;
@@ -1527,6 +1623,19 @@ static int publish_peer_tables(siglip_ctx* c) {
       if (c->loopback && p != c->rank) mk[q * c->world + p] = c->loop_keys + static_cast<size_t>(p) * c->Tmax;
     }
   CK(cudaMemcpy(c->mkey_ptrs_dev, mk.data(), mk.size() * sizeof(unsigned long long*), cudaMemcpyHostToDevice));
+  if (c->xid_ptrs_dev != nullptr) {
+    // every rank's published extra-image ids, per step parity (loopback: the stand-ins
+    // siglip_debug_set_peer_extra_image_ids seeds)
+    std::vector<const int64_t*> xi(2 * c->world);
+    for (int q = 0; q < 2; ++q)
+      for (int p = 0; p < c->world; ++p) {
+        xi[q * c->world + p] = reinterpret_cast<const int64_t*>(
+            reinterpret_cast<const unsigned long long*>(reinterpret_cast<const char*>(c->peer_txt[p]) + mkeys_offset(c)) +
+            q * mkeys_block(c) + mkeys_xids(c));
+        if (c->loopback && p != c->rank) xi[q * c->world + p] = c->loop_xids + static_cast<size_t>(p) * c->Emax;
+      }
+    CK(cudaMemcpy(c->xid_ptrs_dev, xi.data(), xi.size() * sizeof(int64_t*), cudaMemcpyHostToDevice));
+  }
   c->peers_ready = true;
   return 0;
 }
@@ -1549,6 +1658,10 @@ int siglip_ctx_import_handles(siglip_ctx* c, const void* all_ranks_bytes, size_t
       return fail(SIGLIP_ERR_INVALID,
                   "peer context has a different text count than this rank was told: every rank must be created with the "
                   "same texts_per_rank list (siglip_ctx_create_texts; batch + hard negatives per rank)");
+    if (b.R != c->Rs[p] || b.Rmax != c->Rmax)
+      return fail(SIGLIP_ERR_INVALID,
+                  "peer context has a different image count than this rank was told: every rank must be created with "
+                  "the same images_per_rank list (siglip_ctx_create_extras; batch + extra images per rank)");
     if (p == c->rank) continue;
     char me[64] = {0};
     if (gethostname(me, sizeof(me) - 1) != 0) me[0] = 0;
@@ -1587,7 +1700,25 @@ int siglip_set_sample_ids(siglip_ctx* c, const int64_t* ids_dev, void* cuda_stre
   CK(cudaSetDevice(c->device));
   CK(cudaMemcpyAsync(c->ids_in, ids_dev, ids_bytes(c, c->rank), cudaMemcpyDeviceToDevice,
                      static_cast<cudaStream_t>(cuda_stream)));
+  if (c->rids != nullptr)   // the paired images' ids head my row ids too
+    CK(cudaMemcpyAsync(c->rids, ids_dev, ids_bytes(c, c->rank), cudaMemcpyDeviceToDevice,
+                       static_cast<cudaStream_t>(cuda_stream)));
   c->ids_set = true;
+  return 0;
+}
+
+int siglip_set_extra_image_ids(siglip_ctx* c, const int64_t* ids_dev, void* cuda_stream) {
+  if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  // behind this rank's B sample ids in its private row ids: the [R] ids of my images
+  const size_t e = static_cast<size_t>(c->R - c->B);
+  if (ids_dev == nullptr && e > 0) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->extra_image_ids)
+    return fail(SIGLIP_ERR_STATE, "siglip_set_extra_image_ids needs SIGLIP_OPT_EXTRA_IMAGE_IDS on");
+  CK(cudaSetDevice(c->device));
+  if (e > 0)
+    CK(cudaMemcpyAsync(c->rids + c->B, ids_dev, e * sizeof(int64_t), cudaMemcpyDeviceToDevice,
+                       static_cast<cudaStream_t>(cuda_stream)));
+  c->ximg_ids_set = true;
   return 0;
 }
 
@@ -1610,7 +1741,7 @@ int siglip_set_extra_text_ids(siglip_ctx* c, const int64_t* ids_dev, void* cuda_
 // uses weights holds the workspace it held without them; allowed inside a CUDA-graph capture)
 static int ensure_weights(siglip_ctx* c) {
   if (c->w_in != nullptr) return 0;
-  const size_t bytes = (static_cast<size_t>(c->w_stride) + c->B) * sizeof(float);
+  const size_t bytes = (static_cast<size_t>(c->w_stride) + c->R) * sizeof(float);
   cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
   CK(cudaThreadExchangeStreamCaptureMode(&mode));
   float* w = nullptr;
@@ -1629,7 +1760,7 @@ int siglip_set_sample_weights(siglip_ctx* c, const float* image_w, const float* 
   CK(cudaSetDevice(c->device));
   int rc;
   if ((rc = ensure_weights(c))) return rc;
-  CKI(siglip::launch_clamp_weights(text_w, c->w_in, c->T, image_w, c->w_in + c->w_stride, c->B,
+  CKI(siglip::launch_clamp_weights(text_w, c->w_in, c->T, image_w, c->w_in + c->w_stride, c->R,
                                    static_cast<cudaStream_t>(cuda_stream)));
   c->launches++;
   c->weights_set = true;
@@ -1670,6 +1801,20 @@ int siglip_debug_set_peer_metric_keys(siglip_ctx* c, int peer, const uint64_t* k
   CK(cudaSetDevice(c->device));
   CK(cudaMemcpyAsync(c->loop_keys + static_cast<size_t>(peer) * c->Tmax, keys_dev,
                      static_cast<size_t>(chunk_id_count(c, c->rank)) * sizeof(unsigned long long),
+                     cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
+  return 0;
+}
+
+int siglip_debug_set_peer_extra_image_ids(siglip_ctx* c, int peer, const int64_t* ids_dev, void* cuda_stream) {
+  if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->loopback || peer < 0 || peer >= c->world || peer == c->rank)
+    return fail(SIGLIP_ERR_INVALID,
+                "siglip_debug_set_peer_extra_image_ids needs a loopback context and a peer rank != own rank");
+  const size_t e = static_cast<size_t>(c->Rs[peer] - c->Bs[peer]);
+  if (e == 0) return 0;
+  if (ids_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(c->device));
+  CK(cudaMemcpyAsync(c->loop_xids + static_cast<size_t>(peer) * c->Emax, ids_dev, e * sizeof(int64_t),
                      cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
@@ -1756,6 +1901,10 @@ int siglip_host_submit_grads(siglip_ctx* c, const void* img_host, const void* tx
     return fail(SIGLIP_ERR_STATE,
                 "the host-buffer entries stage [B, D] text: unavailable for a context with hard negatives "
                 "(siglip_ctx_create_texts with texts_per_rank != images_per_rank)");
+  if (c->ximg)
+    return fail(SIGLIP_ERR_STATE,
+                "the host-buffer entries stage [B, D] images: unavailable for a context with extra images "
+                "(siglip_ctx_create_extras with images_per_rank != batch_per_rank)");
   if (c->metrics_armed)
     return fail(SIGLIP_ERR_STATE, "the host-buffer entries return no retrieval metrics: siglip_request_metrics is armed");
   if (c->sample_weights)
@@ -1903,6 +2052,10 @@ int siglip_debug_loopback(siglip_ctx* c) {
     CK(cudaMemset(c->loop_mailboxes, 0, 2 * kMaxWorld * sizeof(float)));
     CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_keys), static_cast<size_t>(c->world) * c->Tmax * 8));
     CK(cudaMemset(c->loop_keys, 0, static_cast<size_t>(c->world) * c->Tmax * 8));
+    if (c->Emax > 0) {
+      CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_xids), static_cast<size_t>(c->world) * c->Emax * 8));
+      CK(cudaMemset(c->loop_xids, 0, static_cast<size_t>(c->world) * c->Emax * 8));
+    }
   }
   for (int p = 0; p < c->world; ++p) {
     c->peer_txt[p] = c->txt_all;
@@ -2196,6 +2349,10 @@ void free_ctx(siglip_ctx* c) {
   }
   cudaFree(c->g_diag);
   cudaFree(c->ids_in);
+  cudaFree(c->rids);
+  cudaFree(c->iota);
+  cudaFree(c->loop_xids);
+  cudaFree(c->xid_ptrs_dev);
   cudaFree(c->w_in);   // w_all: part of txt_all
   cudaFree(c->img16);
   cudaFree(c->slots);

@@ -885,9 +885,11 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
         // Sample-id labels (kIds): the ids of this thread's two fragment rows, loaded once per tile (a row beyond M takes
         // row M - 1's id: it only lies in edge slabs, which mask it).
         int64_t rid0 = 0, rid1 = 0;
+        uint32_t rpos = 0u;   // pos bits of the rows that carry ids: an extra image past row_pos_n never matches
         if constexpr (kIds) {
           rid0 = p.row_ids[min(row_lo, pr.M - 1)];
           rid1 = p.row_ids[min(row_lo + 8, pr.M - 1)];
+          rpos = (row_lo < p.row_pos_n ? 0x3333u : 0u) | (row_lo + 8 < p.row_pos_n ? 0xCCCCu : 0u);
         }
         // Sample weights (kWeights): the weights of the two fragment rows, once per tile (clamped like the ids)
         float rw0 = 1.f, rw1 = 1.f;
@@ -928,6 +930,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
                 }
               }
             }
+            pos &= rpos;
             slab_pos = __any_sync(0xffffffffu, pos != 0u);
           }
           if (!slab_edge && !slab_diag && !slab_pos) {
@@ -1443,15 +1446,25 @@ __device__ __forceinline__ bool metrics_i2t_hit(const MetricsArgs& a, int i, int
   if (a.ids_own == nullptr) return j == a.toff[a.rank] + i;
   const int o = metrics_owner(a, a.toff, j);
   const int l = j - a.toff[o];
-  const int with_ids = a.extra_ids ? a.toff[o + 1] - a.toff[o] : a.off[o + 1] - a.off[o];
-  return l < with_ids && metrics_id(a, o, l) == a.ids_own[i];
+  const int with_ids = a.extra_ids ? a.toff[o + 1] - a.toff[o] : a.bs[o];
+  return l < with_ids && metrics_id(a, o, l) == a.row_ids[i];
 }
 
-// Is global image g a hit for my text i (a paired one, or any under extra_ids)?
+// Is global image g a hit for my text i (a paired one, or any under extra_ids)? An extra image (local index >= its
+// rank's batch) carries an id only under extra_image_ids: its owner's row ids, or the copy that owner published.
 __device__ __forceinline__ bool metrics_t2i_hit(const MetricsArgs& a, int i, int g) {
   if (a.ids_own == nullptr) return g == a.off[a.rank] + i;
   const int o = metrics_owner(a, a.off, g);
-  return metrics_id(a, o, g - a.off[o]) == a.ids_own[i];
+  const int l = g - a.off[o];
+  if (l < a.bs[o]) return metrics_id(a, o, l) == a.ids_own[i];
+  if (!a.extra_image_ids) return false;
+  int64_t id;
+  if (o == a.rank) {
+    id = a.row_ids[l];
+  } else {
+    asm volatile("ld.relaxed.sys.global.s64 %0, [%1];" : "=l"(id) : "l"(a.xids_peers[o] + (l - a.bs[o])) : "memory");
+  }
+  return id == a.ids_own[i];
 }
 
 __device__ __forceinline__ int key_index(unsigned long long k) {
@@ -1495,9 +1508,12 @@ __global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const
   // column partials are read for the paired texts (i < B), and under extra_ids for every text of this rank (i < T);
   // otherwise the extras' column keys are computed but never read
   const int nt = a.extra_ids ? a.T : a.B;
-  const int n = a.B > nt ? a.B : nt;
+  // images ranked by i2t: the paired ones, and under extra_image_ids every image of this rank (row keys of the extras
+  // are computed but never read otherwise)
+  const int ni = a.extra_image_ids ? a.R : a.B;
+  const int n = ni > nt ? ni : nt;
   for (int i = tid; i < n; i += kMetricsThreads) {
-    if (i < a.B) {
+    if (i < ni) {
       const int j = key_index(a.row_keys[i]);   // best text of my image i, over all texts including the extras
       if (a.i2t) a.i2t[i] = j;
       if (j >= 0) h_i2t += metrics_i2t_hit(a, i, j);
@@ -1526,7 +1542,7 @@ __global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const
     atomicAdd(&hits[1], h_t2i);
   }
   __syncthreads();
-  if (tid < 2) a.top1[tid] = static_cast<float>(hits[tid]) / static_cast<float>(tid == 0 ? a.B : nt);
+  if (tid < 2) a.top1[tid] = static_cast<float>(hits[tid]) / static_cast<float>(tid == 0 ? ni : nt);
 }
 
 // -------------------------------------------------------------------------------------------------

@@ -146,6 +146,10 @@ struct KernelParams {
   // sigma terms, to the three sums, to g_diag and to the stored sigma operand. Both in [0, 1] (clamped on the way in).
   const float* row_w;   // [M]: this rank's image weights
   const float* col_w;   // [N]: weights of the texts of the chunk being scored
+  // Extra images (siglip_ctx_create_extras): the rows are [paired images; extras]. Appended last like the fields above,
+  // and read only by the kIds instantiations: the row twin of col_pos_n.
+  int row_pos_n;   // loss kernel, kIds: rows that carry ids (row_ids has this many entries): the paired images, or all
+                   // of them under SIGLIP_OPT_EXTRA_IMAGE_IDS. Rows past it never match
 };
 
 enum KernelMode { kModeLoss = 0, kModeOut = 1 };
@@ -211,9 +215,18 @@ struct MetricsArgs {
   const unsigned long long* col_own;           // [T] my partial of my chunk
   const unsigned long long* const* col_peers;  // [world] every rank's partial of my chunk (world > 1; own entry unused)
   int B, rank, world;
-  int off[kMetricsMaxWorld + 1];               // prefix sums of the per-rank batches (global image indices)
+  int off[kMetricsMaxWorld + 1];               // prefix sums of the per-rank image counts (global image indices): rank
+                                               // p's images off[p] .. off[p] + B_p - 1 are paired, the rest extras
   int toff[kMetricsMaxWorld + 1];              // prefix sums of the per-rank text counts (global text indices): rank
                                                // p's texts toff[p] .. toff[p] + B_p - 1 are paired, the rest extras
+  int bs[kMetricsMaxWorld];                    // per-rank batches B_p (paired images / texts)
+  int R;                                       // this rank's images (B + its extra images)
+  int extra_image_ids;                         // SIGLIP_OPT_EXTRA_IMAGE_IDS: i2t covers all R images (i2t: [R]) and a
+                                               // winning extra image is a t2i hit when its id is the text's
+  const int64_t* row_ids;                      // [R] ids of this rank's images (ids mode): the sample ids, then the
+                                               // extra images' ids
+  const int64_t* const* xids_peers;            // [world] every rank's published extra-image ids of this step (world > 1
+                                               // under extra_image_ids; own entry unused)
   const int64_t* ids_own;                      // null = positional labels; else this rank's sample ids
   const int64_t* ids_all;                      // [world][ids_stride]: every chunk's ids, gathered in this step
   int ids_stride;
@@ -221,7 +234,7 @@ struct MetricsArgs {
                                                // extras can be hits, and t2i covers all T texts of this rank
   int T;                                       // this rank's texts
   float* top1;                                 // [2]: i2t, t2i
-  int64_t* i2t;                                // [B] or null
+  int64_t* i2t;                                // [B] ([R] under extra_image_ids) or null
   int64_t* t2i;                                // [B] ([T] under extra_ids) or null
   unsigned int* const* sig_ptrs;               // [world] flag kind 5 of every rank (world > 1)
   const volatile unsigned int* flags_local;    // my flag kind 5 row

@@ -48,14 +48,31 @@ class SigmoidLossEngine:
 
     def __init__(self, batch: int, dim: int, device: torch.device, group=None, cta_group: int = 2,
                  overlap_pull: bool = True, rank_world: Optional[Tuple[int, int]] = None, loopback: bool = False,
-                 batch_per_rank=None, texts_per_rank=None):
+                 batch_per_rank=None, texts_per_rank=None, images_per_rank=None):
         self._L = _capi.lib()
         if not torch.cuda.is_available() or self._L.siglip_device_count() == 0:
             raise RuntimeError("distributed_sigmoid_loss_b200 needs an sm_90 (H100) device; there is no CPU fallback")
         self.batch, self.dim, self.device, self.group = batch, dim, torch.device(device), group
         self.rank, self.world = rank_world if rank_world is not None else _group_rank_world(group)
         h = ctypes.c_void_p()
-        if texts_per_rank is not None:
+        if images_per_rank is not None:
+            # extra images: rank p holds images_per_rank[p] >= its batch images, the paired ones first, then its extras
+            # (siglip_ctx_create_extras); every rank passes the same three lists
+            bpr = [int(b) for b in batch_per_rank] if batch_per_rank is not None else [batch] * self.world
+            ipr = [int(r) for r in images_per_rank]
+            tpr = [int(t) for t in texts_per_rank] if texts_per_rank is not None else list(bpr)
+            if len(bpr) != self.world or bpr[self.rank] != batch or len(ipr) != self.world or len(tpr) != self.world:
+                raise RuntimeError(f"batch_per_rank {bpr} / images_per_rank {ipr} / texts_per_rank {tpr} must list one "
+                                   f"entry per rank and hold batch {batch} at rank {self.rank}")
+            if any(r < b for r, b in zip(ipr, bpr)) or any(t < b for t, b in zip(tpr, bpr)):
+                raise RuntimeError(f"images_per_rank {ipr} and texts_per_rank {tpr} must be >= batch_per_rank {bpr} on "
+                                   f"every rank")
+            _capi.check(self._L.siglip_ctx_create_extras(ctypes.byref(h), self.device.index or 0, self.rank, self.world,
+                                                         (ctypes.c_int * self.world)(*bpr),
+                                                         (ctypes.c_int * self.world)(*ipr),
+                                                         (ctypes.c_int * self.world)(*tpr), dim))
+            self.batch_per_rank, self.images_per_rank, self.texts_per_rank = bpr, ipr, tpr
+        elif texts_per_rank is not None:
             # hard-negative captions: rank p holds texts_per_rank[p] >= its batch texts, the paired ones first, then its
             # extras (siglip_ctx_create_texts); every rank passes the same lists
             bpr = [int(b) for b in batch_per_rank] if batch_per_rank is not None else [batch] * self.world
@@ -84,8 +101,12 @@ class SigmoidLossEngine:
             self.batch_per_rank = [batch] * self.world
         if texts_per_rank is None:
             self.texts_per_rank = list(self.batch_per_rank)
+        if images_per_rank is None:
+            self.images_per_rank = list(self.batch_per_rank)
         self.texts = self.texts_per_rank[self.rank]   # rows of txt / dtxt: the batch plus this rank's hard negatives
+        self.images = self.images_per_rank[self.rank]   # rows of img / dimg: the batch plus this rank's extra images
         self.extra_text_ids = False   # SIGLIP_OPT_EXTRA_TEXT_IDS: every text of a chunk carries an id (see set_option)
+        self.extra_image_ids = False  # SIGLIP_OPT_EXTRA_IMAGE_IDS: every image of this rank carries an id
         self._h = h
         _capi.check(self._L.siglip_ctx_set_option(h, _capi.SIGLIP_OPT_CTA_GROUP, int(cta_group)))
         _capi.check(self._L.siglip_ctx_set_option(h, _capi.SIGLIP_OPT_OVERLAP_PULL, int(bool(overlap_pull))))
@@ -110,6 +131,8 @@ class SigmoidLossEngine:
         _capi.check(self._L.siglip_ctx_set_option(self._h, option, value))
         if option == _capi.SIGLIP_OPT_EXTRA_TEXT_IDS or (option == _capi.SIGLIP_OPT_SAMPLE_IDS and not value):
             self.extra_text_ids = bool(value)   # the library clears the extras' ids with the sample ids
+        if option == _capi.SIGLIP_OPT_EXTRA_IMAGE_IDS or (option == _capi.SIGLIP_OPT_SAMPLE_IDS and not value):
+            self.extra_image_ids = bool(value)
 
     def kernel_times(self):
         """(loss_ms, loss_launches, grad_ms, grad_launches) since the last call; needs SIGLIP_OPT_KERNEL_TIMING."""
@@ -136,11 +159,25 @@ class SigmoidLossEngine:
         with torch.cuda.device(self.device):
             _capi.check(self._L.siglip_set_extra_text_ids(self._h, ids.data_ptr(), self._stream()))
 
+    def set_extra_image_ids(self, ids: torch.Tensor) -> None:
+        """SIGLIP_OPT_EXTRA_IMAGE_IDS: the ids of this rank's R - B extra images ([R - B] int64, contiguous, on the engine's
+        device) for the NEXT step, copied on the current stream like set_sample_ids."""
+        self._check_ids(ids, self.images - self.batch)
+        with torch.cuda.device(self.device):
+            _capi.check(self._L.siglip_set_extra_image_ids(self._h, ids.data_ptr(), self._stream()))
+
+    def debug_set_peer_extra_image_ids(self, peer: int, ids: torch.Tensor) -> None:
+        """Loopback: the extra-image ids ([R_peer - B_peer] int64) standing in for what peer `peer` publishes in a
+        metrics step."""
+        self._check_ids(ids, self.images_per_rank[peer] - self.batch_per_rank[peer])
+        _capi.check(self._L.siglip_debug_set_peer_extra_image_ids(self._h, peer, ids.data_ptr(), self._stream()))
+
     def set_sample_weights(self, image_weights: Optional[torch.Tensor], text_weights: Optional[torch.Tensor]) -> None:
-        """SIGLIP_OPT_SAMPLE_WEIGHTS: this rank's image weights ([B] fp32) and text weights ([T] fp32: the paired texts,
-        then the extras), contiguous on the engine's device, or None for ones, for the NEXT step. Copied on the current
-        stream with every value clamped into [0, 1] (NaN -> 0), so the tensors may be released or overwritten afterwards."""
-        self._check_weights(image_weights, self.batch)
+        """SIGLIP_OPT_SAMPLE_WEIGHTS: this rank's image weights ([R] fp32: the paired images, then the extra images) and
+        text weights ([T] fp32: the paired texts, then the extras), contiguous on the engine's device, or None for ones,
+        for the NEXT step. Copied on the current stream with every value clamped into [0, 1] (NaN -> 0), so the tensors may
+        be released or overwritten afterwards."""
+        self._check_weights(image_weights, self.images)
         self._check_weights(text_weights, self.texts)
         with torch.cuda.device(self.device):
             _capi.check(self._L.siglip_set_sample_weights(
@@ -174,9 +211,10 @@ class SigmoidLossEngine:
     def request_metrics(self, top1: torch.Tensor, i2t_index: Optional[torch.Tensor] = None,
                         t2i_index: Optional[torch.Tensor] = None) -> None:
         """Arm the in-batch retrieval metrics of the NEXT step (siglip_request_metrics): top1 fp32 [2] (i2t, t2i),
-        i2t_index int64 [B] and t2i_index int64 [B] ([T] under SIGLIP_OPT_EXTRA_TEXT_IDS) (global indices) or None, all
-        contiguous on the engine's device. Nothing is read on the host; the step writes them on its stream."""
-        bufs = ((top1, torch.float32, 2), (i2t_index, torch.int64, self.batch),
+        i2t_index int64 [B] ([R] under SIGLIP_OPT_EXTRA_IMAGE_IDS) and t2i_index int64 [B] ([T] under
+        SIGLIP_OPT_EXTRA_TEXT_IDS) (global indices) or None, all contiguous on the engine's device. Nothing is read on the
+        host; the step writes them on its stream."""
+        bufs = ((top1, torch.float32, 2), (i2t_index, torch.int64, self.metric_images),
                 (t2i_index, torch.int64, self.metric_texts))
         for k, (x, dt, n) in enumerate(bufs):
             if x is None and k > 0:
@@ -195,6 +233,11 @@ class SigmoidLossEngine:
                 keys.device != self.device:
             raise RuntimeError(f"peer metric keys must be a contiguous int64 [{n}] tensor on {self.device}")
         _capi.check(self._L.siglip_debug_set_peer_metric_keys(self._h, peer, keys.data_ptr(), self._stream()))
+
+    @property
+    def metric_images(self) -> int:
+        """Images of this rank that i2t ranks: the paired ones, or all R under SIGLIP_OPT_EXTRA_IMAGE_IDS."""
+        return self.images if self.extra_image_ids else self.batch
 
     @property
     def metric_texts(self) -> int:
@@ -246,7 +289,7 @@ class SigmoidLossEngine:
         loss, dtp, db = scal[0:1], scal[1:2], scal[2:3]
         if self._set_tprime_f64(t_prime):
             dtp = torch.empty(1, device=self.device, dtype=torch.float64)
-        dimg = torch.empty(self.batch, self.dim, device=self.device, dtype=grad_dtype)
+        dimg = torch.empty(self.images, self.dim, device=self.device, dtype=grad_dtype)
         dtxt = torch.empty(self.texts, self.dim, device=self.device, dtype=grad_dtype)
         with torch.cuda.device(self.device):
             _capi.check(self._L.siglip_fwd_bwd_scaled(
@@ -283,7 +326,7 @@ class SigmoidLossEngine:
         dtp, db = scal[0:1], scal[1:2]
         if self._set_tprime_f64(t_prime):
             dtp = torch.empty(1, device=self.device, dtype=torch.float64)
-        dimg = torch.empty(self.batch, self.dim, device=self.device, dtype=grad_dtype)
+        dimg = torch.empty(self.images, self.dim, device=self.device, dtype=grad_dtype)
         dtxt = torch.empty(self.texts, self.dim, device=self.device, dtype=grad_dtype)
         with torch.cuda.device(self.device):
             _capi.check(self._L.siglip_backward(self._h, img.data_ptr(), txt.data_ptr(), t_prime.data_ptr(),
@@ -301,15 +344,17 @@ class SigmoidLossEngine:
             self._grad_bf16 = want_bf16
 
     def _rows_ok(self, x: torch.Tensor) -> bool:
-        """[B, D] (images, paired texts) or [T, D] (texts with this rank's hard negatives)."""
-        return x.dim() == 2 and x.shape[0] in (self.batch, self.texts) and x.shape[1] == self.dim
+        """[B, D] (images, paired texts), [T, D] (texts with this rank's hard negatives) or [R, D] (images with its extra
+        images)."""
+        return x.dim() == 2 and x.shape[0] in (self.batch, self.texts, self.images) and x.shape[1] == self.dim
 
     def normalize_fwd(self, x: torch.Tensor, f16: bool = False):
         """F.normalize(x, dim=1) fused with the rounding to the kernels' operand format: returns (xhat [N, D] bf16, or
         float16 holding 16*xhat with f16=True; inv_norm fp32 [N]). x: fp32 or bf16 [N, D] contiguous, N = B or T."""
         if not self._rows_ok(x) or x.dtype not in (torch.float32, torch.bfloat16) or \
                 not x.is_contiguous() or x.device != self.device:
-            raise RuntimeError(f"normalize_fwd expects a contiguous fp32/bf16 [{self.batch} or {self.texts}, {self.dim}] "
+            raise RuntimeError(f"normalize_fwd expects a contiguous fp32/bf16 [{self.batch}, {self.texts} or "
+                               f"{self.images}, {self.dim}] "
                                f"tensor on {self.device}")
         self._set_input_f16(f16)
         n = x.shape[0]
@@ -323,7 +368,7 @@ class SigmoidLossEngine:
     def normalize_bwd(self, x: torch.Tensor, inv: torch.Tensor, dxhat: torch.Tensor) -> torch.Tensor:
         """Backward of normalize_fwd: dx = inv * (dxhat - xhat <xhat, dxhat>), in x's dtype."""
         if not self._rows_ok(x) or tuple(dxhat.shape) != tuple(x.shape) or tuple(inv.shape) != (x.shape[0],):
-            raise RuntimeError("normalize_bwd expects x / dxhat [N, D] and inv [N] with N = B or T")
+            raise RuntimeError("normalize_bwd expects x / dxhat [N, D] and inv [N] with N = B, T or R")
         dx = torch.empty_like(x)
         with torch.cuda.device(self.device):
             _capi.check(self._L.siglip_normalize_bwd_rows(self._h, x.shape[0], x.data_ptr(),
@@ -403,10 +448,10 @@ class SigmoidLossEngine:
                 raise RuntimeError("the host entries expect contiguous CPU bf16 tensors of shape [B, D]")
 
     def _check(self, img: torch.Tensor, txt: torch.Tensor) -> None:
-        """Operands are contiguous device tensors, img [B, D] and txt [T, D] (T = B without hard negatives), both bf16
+        """Operands are contiguous device tensors, img [R, D] and txt [T, D] (R = T = B without extras), both bf16
         (default format) or both float16 holding 16*x (the fp32-input format, see convert_f32); the context option
         follows the dtype."""
-        for x, n in ((img, self.batch), (txt, self.texts)):
+        for x, n in ((img, self.images), (txt, self.texts)):
             if x.device != self.device or x.dtype not in (torch.bfloat16, torch.float16) or not x.is_contiguous() or \
                     tuple(x.shape) != (n, self.dim):
                 raise RuntimeError(
@@ -436,7 +481,8 @@ class SigmoidLossEngine:
         """The module's cast of fp32 embeddings to the kernels' operand format: bf16 (f16=False, == x.to(bfloat16)) or
         float16 holding 16*x (f16=True: 11 significant bits, what fp32 callers get)."""
         if not self._rows_ok(x) or x.dtype != torch.float32 or not x.is_contiguous() or x.device != self.device:
-            raise RuntimeError(f"convert_f32 expects a contiguous fp32 [{self.batch} or {self.texts}, {self.dim}] tensor "
+            raise RuntimeError(f"convert_f32 expects a contiguous fp32 [{self.batch}, {self.texts} or {self.images}, "
+                               f"{self.dim}] tensor "
                                f"on {self.device}")
         self._set_input_f16(f16)
         out = torch.empty(x.shape[0], self.dim, device=self.device, dtype=torch.float16 if f16 else torch.bfloat16)
@@ -479,12 +525,14 @@ class _SigmoidLossFn(torch.autograd.Function):
     extra_ids: [T - B] int64 ids of the extra texts (SIGLIP_OPT_EXTRA_TEXT_IDS engines), set along with ids.
     metrics: (top1, i2t_index, t2i_index) output buffers: the retrieval metrics of this call's step are armed. A re-run
     of the forward by the backward's generation guard does not arm them again (they belong to the first run).
-    weights: (image_weights [B] or None, text_weights [T] or None) fp32 (SIGLIP_OPT_SAMPLE_WEIGHTS engines), set before
-    every step the engine runs for this call, like the ids."""
+    weights: (image_weights [R] or None, text_weights [T] or None) fp32 (SIGLIP_OPT_SAMPLE_WEIGHTS engines), set before
+    every step the engine runs for this call, like the ids.
+    extra_img_ids: [R - B] int64 ids of the extra images (SIGLIP_OPT_EXTRA_IMAGE_IDS engines), set along with ids."""
 
     @staticmethod
     def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool = False, fused: bool = False,
-                ids: Optional[torch.Tensor] = None, metrics=None, extra_ids: Optional[torch.Tensor] = None, weights=None):
+                ids: Optional[torch.Tensor] = None, metrics=None, extra_ids: Optional[torch.Tensor] = None, weights=None,
+                extra_img_ids: Optional[torch.Tensor] = None):
         need_grad = any(ctx.needs_input_grad[:4])
         raw = None
         # bf16 callers: bf16 operands (what autograd would multiply). Anything wider (the reference's own test feeds
@@ -518,11 +566,13 @@ class _SigmoidLossFn(torch.autograd.Function):
             b = b.to(device=img.device, dtype=torch.float32)
         b = b.reshape(1)
         ctx.fused = bool(fused and need_grad)
-        ctx.ids, ctx.extra_ids, ctx.weights = ids, extra_ids, weights
+        ctx.ids, ctx.extra_ids, ctx.weights, ctx.extra_img_ids = ids, extra_ids, weights, extra_img_ids
         if ids is not None:
             engine.set_sample_ids(ids)
         if extra_ids is not None:
             engine.set_extra_text_ids(extra_ids)
+        if extra_img_ids is not None:
+            engine.set_extra_image_ids(extra_img_ids)
         if weights is not None:
             engine.set_sample_weights(*weights)
         if metrics is not None:
@@ -578,6 +628,8 @@ class _SigmoidLossFn(torch.autograd.Function):
                     eng.set_sample_ids(ctx.ids)
                 if ctx.extra_ids is not None:
                     eng.set_extra_text_ids(ctx.extra_ids)
+                if ctx.extra_img_ids is not None:
+                    eng.set_extra_image_ids(ctx.extra_img_ids)
                 if ctx.weights is not None:
                     eng.set_sample_weights(*ctx.weights)
                 eng.forward(img_b, txt_b, tp, b, True)
@@ -596,14 +648,15 @@ class _SigmoidLossFn(torch.autograd.Function):
                 gt = dtxt.to(tdt) if ctx.needs_input_grad[1] else None
         gp = dtp.reshape(pshape).to(device=pdev, dtype=pdt) if ctx.needs_input_grad[2] else None
         gb = db.reshape(bshape).to(device=bdev, dtype=bdt) if ctx.needs_input_grad[3] else None
-        return gi, gt, gp, gb, None, None, None, None, None, None, None
+        return gi, gt, gp, gb, None, None, None, None, None, None, None, None
 
 
 class _EngineCache:
     def __init__(self, group=None, cta_group: int = 2, overlap_pull: bool = True, sync_scalar_grads: bool = False,
                  bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
-                 extra_texts: int = 0, sample_weights: bool = False):
+                 extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
+        self.extra_images = extra_images
         self.sample_weights = sample_weights
         self.sync_scalar_grads, self.bidir = sync_scalar_grads, bidir
         self.multi_positive = multi_positive
@@ -617,15 +670,18 @@ class _EngineCache:
         eng = self._engines.get(key)
         if eng is None:
             dev = torch.device("cuda", key[0])
-            tpr = None
+            tpr = ipr = None
             extras = self.hard_negatives + self.extra_texts   # at most one of the two is non-zero
+            rank, world = _group_rank_world(self.group)
+            bpr = self.batch_per_rank if self.batch_per_rank is not None else [batch] * world
             if extras:
                 # every rank scores the same number K of extras: T_p = B_p + K
-                rank, world = _group_rank_world(self.group)
-                bpr = self.batch_per_rank if self.batch_per_rank is not None else [batch] * world
                 tpr = [int(b) + extras for b in bpr]
+            if self.extra_images:
+                # every rank holds the same number K of extra images: R_p = B_p + K
+                ipr = [int(b) + self.extra_images for b in bpr]
             eng = SigmoidLossEngine(batch, dim, dev, self.group, self.cta_group, self.overlap_pull,
-                                    batch_per_rank=self.batch_per_rank, texts_per_rank=tpr)
+                                    batch_per_rank=self.batch_per_rank, texts_per_rank=tpr, images_per_rank=ipr)
             if self.sync_scalar_grads:
                 eng.set_option(_capi.SIGLIP_OPT_SYNC_SCALAR_GRADS, 1)
             if self.bidir:
@@ -634,6 +690,8 @@ class _EngineCache:
                 eng.set_option(_capi.SIGLIP_OPT_SAMPLE_IDS, 1)
             if self.extra_texts:
                 eng.set_option(_capi.SIGLIP_OPT_EXTRA_TEXT_IDS, 1)   # needs the sample ids on first
+            if self.extra_images and self.multi_positive:
+                eng.set_option(_capi.SIGLIP_OPT_EXTRA_IMAGE_IDS, 1)
             if self.sample_weights:
                 eng.set_option(_capi.SIGLIP_OPT_SAMPLE_WEIGHTS, 1)
             self._engines[key] = eng
@@ -682,10 +740,10 @@ def _validate_extra_texts(extra_texts, multi_positive: bool, hard_negatives: int
 
 
 def _validate_negatives(text_embeddings: torch.Tensor, negative_text, hard_negatives: int,
-                        name: str = "negative_text", option: str = "hard_negatives") -> None:
+                        name: str = "negative_text", option: str = "hard_negatives", what: str = "texts") -> None:
     """negative_text of a forward: required ([K, D], the dtype / device / width of the texts) when the loss was built
-    with hard_negatives = K > 0, refused otherwise. Raises before any GPU work. (name / option: the same check for
-    extra_text and extra_texts.)"""
+    with hard_negatives = K > 0, refused otherwise. Raises before any GPU work. (name / option / what: the same check for
+    extra_text and extra_texts, and for extra_image and extra_images against the images.)"""
     if hard_negatives == 0:
         if negative_text is not None:
             raise RuntimeError(f"{name} given, but the loss was built without {option} ({option}=K)")
@@ -696,12 +754,12 @@ def _validate_negatives(text_embeddings: torch.Tensor, negative_text, hard_negat
         raise RuntimeError(f"{name} must be a tensor, got {type(negative_text).__name__}")
     want = (hard_negatives, text_embeddings.shape[1] if text_embeddings.dim() == 2 else None)
     if negative_text.dim() != 2 or tuple(negative_text.shape) != want:
-        raise RuntimeError(f"{name} must have shape [{want[0]}, {want[1]}] ({option} x the texts' width), "
+        raise RuntimeError(f"{name} must have shape [{want[0]}, {want[1]}] ({option} x the {what}' width), "
                            f"got {tuple(negative_text.shape)}")
     if negative_text.dtype != text_embeddings.dtype:
-        raise RuntimeError(f"{name} is {negative_text.dtype}, the texts {text_embeddings.dtype}")
+        raise RuntimeError(f"{name} is {negative_text.dtype}, the {what} {text_embeddings.dtype}")
     if negative_text.device != text_embeddings.device:
-        raise RuntimeError(f"{name} is on {negative_text.device}, the texts on {text_embeddings.device}")
+        raise RuntimeError(f"{name} is on {negative_text.device}, the {what} on {text_embeddings.device}")
 
 
 def _validate_extra_text_ids(extra_text_ids, extra_texts: int, text_embeddings: torch.Tensor) -> Optional[torch.Tensor]:
@@ -722,6 +780,30 @@ def _validate_extra_text_ids(extra_text_ids, extra_texts: int, text_embeddings: 
     if extra_text_ids.device != text_embeddings.device:
         raise RuntimeError(f"extra_text_ids are on {extra_text_ids.device}, the texts on {text_embeddings.device}")
     return extra_text_ids.to(torch.int64).contiguous()
+
+
+def _validate_extra_image_ids(extra_image_ids, extra_images: int, multi_positive: bool,
+                              image_embeddings: torch.Tensor) -> Optional[torch.Tensor]:
+    """extra_image_ids of a forward: required ([K] integers on the images' device) when the loss was built with
+    extra_images = K > 0 and multi_positive=True (several images per caption), refused otherwise (without ids the extra
+    images are hard negatives). Returns them as contiguous int64, or None. Raises before any GPU work."""
+    if extra_images == 0 or not multi_positive:
+        if extra_image_ids is not None:
+            raise RuntimeError("extra_image_ids given, but the loss was built without extra_images=K and "
+                               "multi_positive=True (without ids the extra images are hard negatives)")
+        return None
+    if extra_image_ids is None:
+        raise RuntimeError(f"extra_images={extra_images} with multi_positive=True: forward needs extra_image_ids "
+                           f"([{extra_images}] integer tensor)")
+    if not isinstance(extra_image_ids, torch.Tensor) or extra_image_ids.dtype not in _ID_DTYPES:
+        raise RuntimeError(f"extra_image_ids must be an integer tensor, got "
+                           f"{extra_image_ids.dtype if isinstance(extra_image_ids, torch.Tensor) else type(extra_image_ids)}")
+    if extra_image_ids.dim() != 1 or extra_image_ids.shape[0] != extra_images:
+        raise RuntimeError(f"extra_image_ids must have shape [{extra_images}] (one id per extra image), got "
+                           f"{tuple(extra_image_ids.shape)}")
+    if extra_image_ids.device != image_embeddings.device:
+        raise RuntimeError(f"extra_image_ids are on {extra_image_ids.device}, the images on {image_embeddings.device}")
+    return extra_image_ids.to(torch.int64).contiguous()
 
 
 def _validate_sample_weights(sample_weights) -> bool:
@@ -756,12 +838,14 @@ def _validate_weights(weights, sample_weights: bool, n: Optional[int], name: str
 
 
 def _weights_of(sample_weights: bool, image_weights, text_weights, image_embeddings: torch.Tensor,
-                text_embeddings: torch.Tensor, extras: int):
+                text_embeddings: torch.Tensor, extras: int, extra_images: int = 0):
     """Both weight arguments checked; (image_weights, text_weights) for the step, or None without sample_weights. The
-    texts are the paired ones followed by the K extras, so text_weights has B + K entries."""
+    texts are the paired ones followed by the K extras, so text_weights has B + K entries; the images likewise, so
+    image_weights has B + K_img entries."""
     rows = lambda x: x.shape[0] if x.dim() >= 1 else None  # noqa: E731
-    iw = _validate_weights(image_weights, sample_weights, rows(image_embeddings), "image_weights",
-                           image_embeddings.device)
+    ni = rows(image_embeddings)
+    iw = _validate_weights(image_weights, sample_weights, ni + extra_images if ni is not None else None,
+                           "image_weights", image_embeddings.device)
     nt = rows(text_embeddings)
     tw = _validate_weights(text_weights, sample_weights, nt + extras if nt is not None else None, "text_weights",
                            text_embeddings.device)
@@ -779,10 +863,11 @@ def _validate_return_metrics(return_metrics) -> None:
         raise RuntimeError(f"return_metrics must be a bool, got {type(return_metrics).__name__}")
 
 
-def _metric_buffers(batch: int, device: torch.device, texts: Optional[int] = None):
-    """texts: rows of t2i_index (all T texts under extra_texts; the batch otherwise)."""
+def _metric_buffers(batch: int, device: torch.device, texts: Optional[int] = None, images: Optional[int] = None):
+    """texts: rows of t2i_index (all T texts under extra_texts; the batch otherwise). images: rows of i2t_index (all R
+    images under extra_images with ids; the batch otherwise)."""
     top1 = torch.empty(2, device=device, dtype=torch.float32)
-    return (top1, torch.empty(batch, device=device, dtype=torch.int64),
+    return (top1, torch.empty(batch if images is None else images, device=device, dtype=torch.int64),
             torch.empty(batch if texts is None else texts, device=device, dtype=torch.int64))
 
 
@@ -866,14 +951,28 @@ class DDPSigmoidLoss(nn.Module):
     the loss by ``B / (B − m)`` for the mean over the m samples kept. Values outside [0, 1] are clamped into it (NaN → 0);
     larger importance weights: divide by their maximum and scale the loss by it. No gradient with respect to the weights.
     Retrieval metrics ignore the weights. Collective: set on every rank.
+
+    ``extra_images=K > 0``: every ``forward`` also takes ``extra_image`` ([K, D], the dtype, device and width of the
+    images): K more images per rank that pair with no caption position. They are scored against every text of the
+    global batch and ``extra_image.grad`` comes back through autograd; the loss still divides by the paired batch B.
+    Without ``multi_positive`` they are hard-negative images: every text is a negative for them. With
+    ``multi_positive=True`` every forward also takes ``extra_image_ids`` ([K] integers), and extra image i is positive
+    for every text of the global batch with the same id: another image of that caption (several photos of one product,
+    frames of one clip, augmented crops); an id that matches no text makes it a hard-negative image. This scores
+    ``(B + K) x T`` pairs per rank where repeating each caption once per image would score ``M·B x M·B``, and the images
+    never leave their rank. ``image_weights`` then has B + K entries. With ``return_metrics`` a text whose best image is
+    an extra is a t2i miss unless that image carries the text's id; with ids ``i2t_index`` is ``[B + K]`` and covers the
+    extras (an extra whose id matches no text is always an i2t miss). Composes with ``hard_negatives`` /
+    ``extra_texts``. Collective: every rank uses the same K.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
                  normalize_inputs: bool = False, sync_scalar_grads: bool = False, fused_step: Optional[bool] = None,
                  batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
-                 extra_texts: int = 0, sample_weights: bool = False) -> None:
+                 extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0) -> None:
         super().__init__()
         hard_negatives = _validate_hard_negatives(hard_negatives)
+        extra_images = _validate_hard_negatives(extra_images, "extra_images")
         extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
         sample_weights = _validate_sample_weights(sample_weights)
         self.t_prime = nn.Parameter(torch.tensor(math.log(10), dtype=torch.float64))
@@ -897,9 +996,11 @@ class DDPSigmoidLoss(nn.Module):
         self.extra_texts = extra_texts
         # extension: per-sample loss weights (weight 0 drops a sample at a fixed batch shape)
         self.sample_weights = sample_weights
+        # extension: extra images per rank (hard-negative images, or with ids several images per caption)
+        self.extra_images = extra_images
         self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank,
                                    multi_positive=multi_positive, hard_negatives=hard_negatives,
-                                   extra_texts=extra_texts, sample_weights=sample_weights)
+                                   extra_texts=extra_texts, sample_weights=sample_weights, extra_images=extra_images)
 
     def engine_for(self, batch: int, dim: int, device: torch.device) -> SigmoidLossEngine:
         return self._cache.get(batch, (dim + 7) // 8 * 8, device)
@@ -908,22 +1009,26 @@ class DDPSigmoidLoss(nn.Module):
                 negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
                 return_metrics: bool = False, extra_text: Optional[torch.Tensor] = None,
                 extra_text_ids: Optional[torch.Tensor] = None, image_weights: Optional[torch.Tensor] = None,
-                text_weights: Optional[torch.Tensor] = None):
+                text_weights: Optional[torch.Tensor] = None, extra_image: Optional[torch.Tensor] = None,
+                extra_image_ids: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
         ids = _validate_ids(sample_ids, self.multi_positive, image_embeddings)
         _validate_negatives(text_embeddings, negative_text, self.hard_negatives)
         _validate_negatives(text_embeddings, extra_text, self.extra_texts, "extra_text", "extra_texts")
         extra_ids = _validate_extra_text_ids(extra_text_ids, self.extra_texts, text_embeddings)
+        _validate_negatives(image_embeddings, extra_image, self.extra_images, "extra_image", "extra_images", "images")
+        ximg_ids = _validate_extra_image_ids(extra_image_ids, self.extra_images, self.multi_positive, image_embeddings)
         weights = _weights_of(self.sample_weights, image_weights, text_weights, image_embeddings, text_embeddings,
-                              self.hard_negatives + self.extra_texts)
+                              self.hard_negatives + self.extra_texts, self.extra_images)
         _validate(image_embeddings, text_embeddings, self.gpu_batch_size)
         text_embeddings = _with_negatives(_with_negatives(text_embeddings, negative_text), extra_text)
+        image_embeddings = _with_negatives(image_embeddings, extra_image)
         image_embeddings, text_embeddings = _pad_dim(image_embeddings), _pad_dim(text_embeddings)
-        eng = self._cache.get(image_embeddings.shape[0], image_embeddings.shape[1], image_embeddings.device)
+        eng = self._cache.get(self.gpu_batch_size, image_embeddings.shape[1], image_embeddings.device)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
-        bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts) if return_metrics else None
+        bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
         loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
-                                    self.normalize_inputs, fused, ids, bufs, extra_ids, weights)
+                                    self.normalize_inputs, fused, ids, bufs, extra_ids, weights, ximg_ids)
         return (loss, _metric_dict(bufs)) if return_metrics else loss
 
 
@@ -942,15 +1047,18 @@ class SigLipLoss(nn.Module):
     captions positive for the images with the same id, as in ``DDPSigmoidLoss`` (a pure-negative extra is always a t2i
     miss: the caption-only rate is ``t2i_top1 · T / (T − N)`` for N of them among T = B + K texts).
     ``sample_weights=True``: every forward takes ``image_weights`` [B] and ``text_weights`` [B + K] (or None for ones),
-    per-sample loss weights in [0, 1] as in ``DDPSigmoidLoss``."""
+    per-sample loss weights in [0, 1] as in ``DDPSigmoidLoss``. ``extra_images=K``: every forward takes ``extra_image``
+    [K, D] (and with ``multi_positive`` ``extra_image_ids`` [K]), hard-negative images or further images of a caption as
+    in ``DDPSigmoidLoss``; ``image_weights`` then has B + K entries."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
                  multi_positive: bool = False, hard_negatives: int = 0, extra_texts: int = 0,
-                 sample_weights: bool = False):
+                 sample_weights: bool = False, extra_images: int = 0):
         super().__init__()
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
         hard_negatives = _validate_hard_negatives(hard_negatives)
+        extra_images = _validate_hard_negatives(extra_images, "extra_images")
         extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
         sample_weights = _validate_sample_weights(sample_weights)
         self.cache_labels, self.rank, self.world_size, self.bidir = cache_labels, rank, world_size, bidir
@@ -960,25 +1068,32 @@ class SigLipLoss(nn.Module):
         self.hard_negatives = hard_negatives
         self.extra_texts = extra_texts
         self.sample_weights = sample_weights
+        self.extra_images = extra_images
         self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive,
-                                   hard_negatives=hard_negatives, extra_texts=extra_texts, sample_weights=sample_weights)
+                                   hard_negatives=hard_negatives, extra_texts=extra_texts, sample_weights=sample_weights,
+                                   extra_images=extra_images)
 
     def forward(self, image_features, text_features, logit_scale, logit_bias, output_dict: bool = False, *,
                 negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
                 return_metrics: bool = False, extra_text: Optional[torch.Tensor] = None,
                 extra_text_ids: Optional[torch.Tensor] = None, image_weights: Optional[torch.Tensor] = None,
-                text_weights: Optional[torch.Tensor] = None):
+                text_weights: Optional[torch.Tensor] = None, extra_image: Optional[torch.Tensor] = None,
+                extra_image_ids: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
         ids = _validate_ids(sample_ids, self.multi_positive, image_features)
         _validate_negatives(text_features, negative_text, self.hard_negatives)
         _validate_negatives(text_features, extra_text, self.extra_texts, "extra_text", "extra_texts")
         extra_ids = _validate_extra_text_ids(extra_text_ids, self.extra_texts, text_features)
+        _validate_negatives(image_features, extra_image, self.extra_images, "extra_image", "extra_images", "images")
+        ximg_ids = _validate_extra_image_ids(extra_image_ids, self.extra_images, self.multi_positive, image_features)
         weights = _weights_of(self.sample_weights, image_weights, text_weights, image_features, text_features,
-                              self.hard_negatives + self.extra_texts)
+                              self.hard_negatives + self.extra_texts, self.extra_images)
         _validate(image_features, text_features, None)
+        batch = image_features.shape[0]
         text_features = _with_negatives(_with_negatives(text_features, negative_text), extra_text)
+        image_features = _with_negatives(image_features, extra_image)
         image_features, text_features = _pad_dim(image_features), _pad_dim(text_features)
-        eng = self._cache.get(image_features.shape[0], image_features.shape[1], image_features.device)
+        eng = self._cache.get(batch, image_features.shape[1], image_features.device)
         if (eng.rank, eng.world) != (self.rank, self.world_size):
             raise RuntimeError(
                 f"SigLipLoss(rank={self.rank}, world_size={self.world_size}) does not match the process group "
@@ -986,8 +1101,8 @@ class SigLipLoss(nn.Module):
         if logit_bias is None:
             logit_bias = torch.zeros((), device=image_features.device)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
-        bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts) if return_metrics else None
+        bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
         loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs,
-                                    extra_ids, weights)
+                                    extra_ids, weights, ximg_ids)
         out = {"contrastive_loss": loss} if output_dict else loss
         return (out, _metric_dict(bufs)) if return_metrics else out

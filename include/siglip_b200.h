@@ -9,10 +9,11 @@
  * caller's stream (pass torch.cuda.current_stream().cuda_stream); nothing here synchronises the host
  * except ctx create/destroy and handle import.
  *
- * Data layout: `img` is a row-major [B, D] bf16 device buffer, `txt` a row-major [T, D] one (T = B unless the context
- * was created with siglip_ctx_create_texts: then this rank's T texts are its B paired captions followed by its hard
- * negatives), 16-byte aligned, D % 8 == 0. `dimg` [B, D] and `dtxt` [T, D] are row-major fp32 (or bf16 with
- * SIGLIP_OPT_GRAD_BF16). Scalars are fp32 device scalars.
+ * Data layout: `img` is a row-major [R, D] bf16 device buffer (R = B unless the context was created with
+ * siglip_ctx_create_extras: then this rank's R images are its B paired images followed by its extra images), `txt` a
+ * row-major [T, D] one (T = B unless the context was created with siglip_ctx_create_texts / _extras: then this rank's T
+ * texts are its B paired captions followed by its hard negatives), 16-byte aligned, D % 8 == 0. `dimg` [R, D] and
+ * `dtxt` [T, D] are row-major fp32 (or bf16 with SIGLIP_OPT_GRAD_BF16). Scalars are fp32 device scalars.
  */
 #ifndef SIGLIP_B200_H_
 #define SIGLIP_B200_H_
@@ -128,6 +129,14 @@ enum {
                                      siglip_set_sample_weights; the text weights travel to the other ranks with the text.
                                      Retrieval metrics ignore the weights. The host-buffer entries are unavailable in
                                      this mode. Collective: set on all ranks. Default 0 */
+  SIGLIP_OPT_EXTRA_IMAGE_IDS = 24, /* 1: the extra images of a siglip_ctx_create_extras context carry ids too (several
+                                      images per caption). Image i of rank r has id row_ids_r[i]: sample_ids_r[i] for
+                                      i < B_r, the extra's own id (siglip_set_extra_image_ids) for i >= B_r. Pair (i, j)
+                                      is positive iff row_ids_r[i] == text_ids_c[j], on any rank: an extra image with a
+                                      caption's id is another image of that caption, one whose id matches no text is a
+                                      hard-negative image. Without this option an extra image matches no id. The loss
+                                      still divides by B_r. Needs SIGLIP_OPT_SAMPLE_IDS on (else SIGLIP_ERR_STATE);
+                                      turning that option off clears this one. Collective: set on all ranks. Default 0 */
   SIGLIP_OPT_AUX_TRACE = 18 /* 1: record globaltimer stamps of the auxiliary warps of CTA 0 for every launch (start,
                                last peer flag seen, jobs done, end of launch); read with siglip_ctx_aux_trace */
 };
@@ -178,6 +187,25 @@ int siglip_ctx_create_uneven(siglip_ctx** out, int device, int rank, int world, 
 int siglip_ctx_create_texts(siglip_ctx** out, int device, int rank, int world, const int* images_per_rank,
                             const int* texts_per_rank, int D);
 
+/*
+ * Same, with EXTRA IMAGES as well (several images per caption: product photos, video frames, augmented crops; or
+ * hard-negative images). Rank p has batch_per_rank[p] = B_p paired samples, images_per_rank[p] = R_p >= B_p images and
+ * texts_per_rank[p] = T_p >= B_p texts: images 0 .. B_p - 1 are paired with texts 0 .. B_p - 1, images B_p .. R_p - 1
+ * are its E_p = R_p - B_p extra images. Rank r's loss is
+ *   (1/B_r) sum_{i < R_r} sum_{j over all sum(T) texts} softplus(-y_ij z_ij)
+ * (the divisor stays the paired batch). The positional positive is row == col < B_r of the own chunk: an extra image is
+ * never a positional positive, and under SIGLIP_OPT_SAMPLE_IDS it matches no id unless SIGLIP_OPT_EXTRA_IMAGE_IDS gives
+ * it one. img / dimg of every step are [R_r, D]; dtxt contracts over all R_r rows of every rank; dt' / dbias include
+ * the extras' terms. Images never leave their rank: the text exchange is unchanged, and the only new cross-rank data are
+ * the extra images' ids of a metrics step. Workspaces: the sigma operands are [Rp, Tp] (max R rounded up to 256), the
+ * fp16 image copy and the running dimg hold R rows. Time grows with R / B like the FLOPs (6 R T D). With
+ * images_per_rank == batch_per_rank this is exactly siglip_ctx_create_texts. Every rank passes the same three lists.
+ * The host-buffer entries are unavailable (SIGLIP_ERR_STATE). Invalid arguments return SIGLIP_ERR_INVALID before any
+ * device work.
+ */
+int siglip_ctx_create_extras(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank,
+                             const int* images_per_rank, const int* texts_per_rank, int D);
+
 int siglip_ctx_set_option(siglip_ctx* ctx, int option, int value);
 
 /* Bytes of workspace the context holds on the device. */
@@ -198,7 +226,7 @@ int siglip_ctx_import_handles(siglip_ctx* ctx, const void* all_ranks_bytes, size
  * One training step of the loss, fused: replaces DDPSigmoidLoss.forward (distributed_sigmoid_loss.py:17-48) AND
  * the autograd backward of it (SURVEY.md §3.2), i.e. loss plus the four gradients for upstream grad 1:
  *   loss      [1]    = (1/B) sum_ij softplus(-y_ij z_ij)
- *   dimg      [B,D]  = dloss/dimg           (this rank's loss only)
+ *   dimg      [B,D]  = dloss/dimg           (this rank's loss only; [R, D] with extra images)
  *   dtxt      [B,D]  = d(sum over ranks of their losses)/dtxt   (what all_gather's backward delivers)
  *   dt_prime  [1], dbias [1]                (this rank's loss only; DDP averages them later)
  * Collective: every rank of the context's world must call it the same number of times.
@@ -283,12 +311,22 @@ int siglip_set_sample_ids(siglip_ctx* ctx, const int64_t* ids_dev, void* cuda_st
 int siglip_set_extra_text_ids(siglip_ctx* ctx, const int64_t* ids_dev, void* cuda_stream);
 
 /*
- * SIGLIP_OPT_SAMPLE_WEIGHTS: this rank's image weights (image_w, [B_r] fp32 device buffer, or NULL = ones) and text
+ * SIGLIP_OPT_EXTRA_IMAGE_IDS: the ids of this rank's E_r = R_r - B_r extra images (int64 device buffer of E_r values;
+ * may be NULL when E_r = 0) for the NEXT step, copied on the stream into a private [R] row-id buffer behind the sample ids
+ * (never exported; a single-rank step with these ids can be captured into a CUDA graph). In this mode a step needs this
+ * call and siglip_set_sample_ids since the previous step, else it returns SIGLIP_ERR_STATE before launching anything;
+ * outside the mode this call returns SIGLIP_ERR_STATE.
+ */
+int siglip_set_extra_image_ids(siglip_ctx* ctx, const int64_t* ids_dev, void* cuda_stream);
+
+/*
+ * SIGLIP_OPT_SAMPLE_WEIGHTS: this rank's image weights (image_w, [R_r] fp32 device buffer: its paired images, then its
+ * extra images; or NULL = ones) and text
  * weights (text_w, [T_r] fp32: its paired texts, then its extras; NULL = ones) for the NEXT siglip_fwd_bwd(_scaled) /
  * siglip_forward / siglip_fwd call. A stream-ordered copy into the context that clamps every value into [0, 1] and maps
  * NaN to 0 (one small kernel launch); nothing is read on the host, so the caller's buffers may be reused once the copy has
  * run and a single-rank step with weights can be captured into a CUDA graph. The first call allocates the context's
- * weight buffer ((round_up(T_r, 4) + B_r) floats; also allowed inside a capture). In the mode a step without this call
+ * weight buffer ((round_up(T_r, 4) + R_r) floats; also allowed inside a capture). In the mode a step without this call
  * since the previous step returns SIGLIP_ERR_STATE before launching anything; outside it this call returns
  * SIGLIP_ERR_STATE. siglip_backward needs no weights (the saved sigma operand and positive-pair terms carry them).
  * Weights above 1 do not fit the fp16 sigma operand's range: divide by their maximum and scale the loss by it.
@@ -300,13 +338,16 @@ int siglip_set_sample_weights(siglip_ctx* ctx, const float* image_w, const float
  * computed from the logits the loss kernels already hold in registers, without a second similarity GEMM:
  *   i2t_index[i] = argmax_j s_ij over all sum(T) texts, for each of this rank's B images (global text index; with hard
  *                  negatives a winning extra is a miss)
- *   t2i_index[j] = argmax_i s_ij over all sum(B) images, for each of this rank's B paired texts (global image index;
- *                  under SIGLIP_OPT_EXTRA_TEXT_IDS for each of its T texts, so t2i_index is then [T])
+ *   t2i_index[j] = argmax_i s_ij over all sum(R) images, for each of this rank's B paired texts (global image index;
+ *                  under SIGLIP_OPT_EXTRA_TEXT_IDS for each of its T texts, so t2i_index is then [T]). A winning extra
+ *                  image is a miss unless SIGLIP_OPT_EXTRA_IMAGE_IDS is on and its id is the text's
+ *   With extra images, i2t ranks the B paired images ([B]), or under SIGLIP_OPT_EXTRA_IMAGE_IDS all R images ([R]:
+ *                  an extra image whose id matches no text is always an i2t miss)
  *   top1[0] / top1[1] = fraction of this rank's images / texts whose top-1 is a positive: the positional diagonal, or
  *                       under SIGLIP_OPT_SAMPLE_IDS a pair with the same id, on any rank. Under
  *                       SIGLIP_OPT_EXTRA_TEXT_IDS an extra with the image's id is a hit for i2t, and top1[1] counts
  *                       over all T texts: an extra whose id matches no image is always a t2i miss
- * Global indices follow the concatenated batch (prefix sums of the per-rank batches). Ties go to the lowest global index;
+ * Global indices follow the concatenated batch (prefix sums of the per-rank image / text counts). Ties go to the lowest global index;
  * the ranking uses the kernel's fp32 <img, txt> (z = exp(t') s + b is monotone in s). Per rank, like the loss.
  * top1: 2 fp32 device floats (required); i2t_index / t2i_index: [B] int64 device buffers or NULL. Loss and gradients are
  * bit-identical to the same step without metrics. Cost: the step's loss kernels run an instantiation that also reduces
@@ -335,8 +376,9 @@ int siglip_fwd(siglip_ctx* ctx, const void* img, const void* txt, const float* t
  * set. The copies of step n+1 overlap the kernels of step n; every step still pays its own copies.
  * This is the end-to-end entry the benchmark times. Host buffers must stay valid until the step's wait returns.
  * These entries take no sample ids or weights: under SIGLIP_OPT_SAMPLE_IDS or SIGLIP_OPT_SAMPLE_WEIGHTS they return
- * SIGLIP_ERR_STATE. They stage [B, D] text:
- * on a context with hard negatives (siglip_ctx_create_texts, some T_p != B_p) they return SIGLIP_ERR_STATE.
+ * SIGLIP_ERR_STATE. They stage [B, D] text and images:
+ * on a context with hard negatives (siglip_ctx_create_texts, some T_p != B_p) or extra images (siglip_ctx_create_extras,
+ * some R_p != B_p) they return SIGLIP_ERR_STATE.
  */
 int siglip_host_submit(siglip_ctx* ctx, const void* img_host, const void* txt_host, float t_prime, float bias,
                        unsigned long long* ticket, void* cuda_stream);
@@ -401,6 +443,10 @@ int siglip_debug_set_mailbox(siglip_ctx* ctx, int peer, float dt_prime, float db
  * (0xFFFFFFFF - global image index), 0 = no candidate), so
  * that the cross-rank combine of a metrics step sees candidates the kernel did not produce itself. */
 int siglip_debug_set_peer_metric_keys(siglip_ctx* ctx, int peer, const uint64_t* keys_dev, void* cuda_stream);
+/* Loopback only (SIGLIP_OPT_EXTRA_IMAGE_IDS): seed the extra-image ids that stand in for what peer rank `peer` publishes
+ * in a metrics step ([R_peer - B_peer] int64 device buffer), so that a t2i winner among its extra images is judged by
+ * ids the test chose. */
+int siglip_debug_set_peer_extra_image_ids(siglip_ctx* ctx, int peer, const int64_t* ids_dev, void* cuda_stream);
 /* With SIGLIP_OPT_AUX_TRACE: device-synchronise and copy out 16 globaltimer stamps (ns) per launch since the last call:
  * [0..2] auxiliary warps of CTA 0: start, last peer flag observed (0 = no wait), jobs done; [3] launch end as seen by
  * the last CTA; [4] kernel entry (CTA 0); [5] set-up done (barriers); [6] MMAs of the first tile done (CTA 0);

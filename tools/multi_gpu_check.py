@@ -50,6 +50,10 @@ def main() -> int:
     ap.add_argument("--extra-texts", action="store_true",
                     help="also check extra captions with ids (several captions per image) against the float64 oracle: "
                          "extras that caption images of other ranks, extras that match nothing, fused and split")
+    ap.add_argument("--extra-images", action="store_true",
+                    help="also check extra images per rank against the float64 oracle: hard-negative images, and with ids "
+                         "extra images whose ids caption texts of other ranks, with extra texts too, fused and split, "
+                         "and the retrieval metrics over the published extra-image ids")
     ap.add_argument("--weights", action="store_true",
                     help="also check per-sample loss weights against the float64 oracle: random weights with zeros on "
                          "every rank, the text weights travelling with the text, uneven batches, with and without sample "
@@ -391,6 +395,63 @@ def main() -> int:
                     dextra=rel_f(e.grad.float().cpu(), dtxt_ref[Bs[rank]:]),
                     dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
                     db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
+
+    # ---- extra images: they never leave their rank; their ids meet the texts of every rank, and a metrics step
+    # publishes them for the other ranks' t2i hit test ----------------------------------------------------------------
+    if args.extra_images:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from extra_images_oracle import closed_form_extras, label_blocks, retrieval_metrics_extras
+        Bs = [160 + 24 * r for r in range(world)]
+        K, Kt, D, tp, bias = 200, 40, 136, math.log(10.0), -8.0
+        Rs, Ts = [b + K for b in Bs], [b + Kt for b in Bs]
+        g = torch.Generator().manual_seed(4545)
+        unit = lambda n: torch.nn.functional.normalize(torch.randn(n, D, generator=g)).to(torch.bfloat16)  # noqa: E731
+        imgs, txts = [unit(r) for r in Rs], [unit(t) for t in Ts]
+        ids = [np.arange(sum(Bs[:r]), sum(Bs[:r + 1]), dtype=np.int64) * 2 for r in range(world)]
+        xt = [ids[r][np.arange(Kt) % Bs[r]].copy() for r in range(world)]
+        xi = []
+        for r in range(world):   # extra image j of rank r: an image of a caption of rank (r + 1) % world, or of nothing
+            e = ids[(r + 1) % world][np.arange(K) % Bs[(r + 1) % world]].copy()
+            e[::4] = -1 - np.arange(len(e[::4]))
+            xi.append(e)
+        for multi in (False, True):
+            labels = label_blocks(Bs, Rs, Ts, ids if multi else None, xt if multi else None, xi if multi else None)
+            ref = closed_form_extras([x.float().numpy() for x in imgs], [x.float().numpy() for x in txts], Bs, tp, bias,
+                                     labels)
+            mine = ref[rank]
+            dtxt_ref = torch.from_numpy(sum(ref[r]["contrib"][rank] for r in range(world)))
+            met = retrieval_metrics_extras([x.float().numpy() for x in imgs], [x.float().numpy() for x in txts], Bs,
+                                           ids if multi else None, xt if multi else None, xi if multi else None)[rank]
+            img, txt = imgs[rank].to(dev), txts[rank].to(dev)
+            for fused in (None, False):
+                kw = dict(multi_positive=True, extra_texts=Kt) if multi else dict(hard_negatives=Kt)
+                modx = DDPSigmoidLoss(Bs[rank], fused_step=fused, batch_per_rank=Bs, extra_images=K, **kw).to(dev)
+                with torch.no_grad():
+                    modx.t_prime.fill_(tp)
+                    modx.bias.fill_(bias)
+                for rep in range(2):
+                    modx.zero_grad()
+                    a, e = img[:Bs[rank]].float().requires_grad_(True), img[Bs[rank]:].float().requires_grad_(True)
+                    b, x = txt[:Bs[rank]].float().requires_grad_(True), txt[Bs[rank]:].float().requires_grad_(True)
+                    fw = dict(extra_image=e, return_metrics=True)
+                    if multi:
+                        fw.update(sample_ids=torch.from_numpy(ids[rank]).to(dev), extra_text=x,
+                                  extra_text_ids=torch.from_numpy(xt[rank]).to(dev),
+                                  extra_image_ids=torch.from_numpy(xi[rank]).to(dev))
+                    else:
+                        fw.update(negative_text=x)
+                    l2, m = modx(a, b, **fw)
+                    l2.backward()
+                    torch.cuda.synchronize()
+                    clear = met["t2i_margin"] > 1e-4
+                    t2i_bad = int(((m["t2i_index"].cpu().numpy() != met["t2i_index"]) & clear).sum())
+                    report(f"extra images ids={multi} {fused} B={Bs} K={K} D={D} rep{rep}", dict(
+                        loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
+                        dimg=rel_f(torch.cat([a.grad, e.grad]).float().cpu(), torch.from_numpy(mine["dimg"])),
+                        dtxt=rel_f(torch.cat([b.grad, x.grad]).float().cpu(), dtxt_ref),
+                        dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
+                        db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"]),
+                        t2i_rows_off=float(t2i_bad)))
 
     # ---- per-sample weights: image weights stay local, text weights travel with the text through the peer pulls ----
     if args.weights:
