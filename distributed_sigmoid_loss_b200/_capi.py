@@ -24,6 +24,11 @@ EXPORTED_SYMBOLS = (
     "siglip_ctx_create_uneven",
     "siglip_ctx_create_texts",
     "siglip_ctx_create_extras",
+    "siglip_ctx_create_distill",
+    "siglip_set_teacher",
+    "siglip_debug_set_teacher_text_chunk",
+    "siglip_teacher_convert_f32",
+    "siglip_teacher_normalize_fwd",
     "siglip_ctx_set_option",
     "siglip_ctx_workspace_bytes",
     "siglip_ctx_handle_bytes",
@@ -97,6 +102,7 @@ SIGLIP_OPT_SAMPLE_IDS = 21
 SIGLIP_OPT_EXTRA_TEXT_IDS = 22
 SIGLIP_OPT_SAMPLE_WEIGHTS = 23
 SIGLIP_OPT_EXTRA_IMAGE_IDS = 24
+SIGLIP_OPT_DISTILL = 25
 
 _lib: Optional[ctypes.CDLL] = None
 
@@ -162,6 +168,16 @@ def lib() -> ctypes.CDLL:
     L.siglip_ctx_create_extras.argtypes = [ctypes.POINTER(vp), ci, ci, ci, ctypes.POINTER(ci), ctypes.POINTER(ci),
                                            ctypes.POINTER(ci), ci]
     L.siglip_ctx_create_extras.restype = ci
+    L.siglip_ctx_create_distill.argtypes = [ctypes.POINTER(vp), ci, ci, ci, ctypes.POINTER(ci), ci, ci]
+    L.siglip_ctx_create_distill.restype = ci
+    L.siglip_set_teacher.argtypes = [vp, vp, vp, ci, vp, vp, ctypes.c_float]
+    L.siglip_set_teacher.restype = ci
+    L.siglip_debug_set_teacher_text_chunk.argtypes = [vp, ci, vp, vp]
+    L.siglip_debug_set_teacher_text_chunk.restype = ci
+    L.siglip_teacher_convert_f32.argtypes = [vp, ci, vp, vp, ci, vp]
+    L.siglip_teacher_convert_f32.restype = ci
+    L.siglip_teacher_normalize_fwd.argtypes = [vp, ci, vp, ci, vp, vp, ci, vp]
+    L.siglip_teacher_normalize_fwd.restype = ci
     L.siglip_set_extra_image_ids.argtypes = [vp, vp, vp]
     L.siglip_set_extra_image_ids.restype = ci
     L.siglip_debug_set_peer_extra_image_ids.argtypes = [vp, ci, vp, vp]

@@ -154,7 +154,8 @@ struct IpcBlob {
   int Tmax;
   int R;      // images of the rank (B + its extra images)
   int Rmax;
-  char host[64];
+  char host[60];
+  int D_teacher;   // width of the gathered teacher text (0: none); inside the 64 bytes the host name had before
 };
 
 }  // namespace
@@ -216,6 +217,18 @@ struct siglip_ctx {
   bool extra_ids_set = false;            // siglip_set_extra_text_ids was called since the previous step
   int sample_weights = 0;                // SIGLIP_OPT_SAMPLE_WEIGHTS: per-sample loss weights (collective)
   bool weights_set = false;              // siglip_set_sample_weights was called since the previous step
+  // distillation (siglip_ctx_create_distill, SIGLIP_OPT_DISTILL)
+  int DT = 0;                            // teacher width D_teacher (0: a context without a teacher)
+  int distill = 0;                       // SIGLIP_OPT_DISTILL (collective)
+  bool teacher_set = false;              // siglip_set_teacher was called since the previous step
+  const void* t_img = nullptr;           // [B, DT] teacher images of the step (caller's buffer)
+  const void* t_txt = nullptr;           // [B, DT] teacher texts of the step (caller's buffer)
+  int t_f16 = 0;                         // teacher operands are fp16(x * 16)
+  const float* t_tprime = nullptr;       // fp32 device scalars of the teacher
+  const float* t_bias = nullptr;
+  float t_lambda = 1.0f;
+  __nv_bfloat16* ttxt_all = nullptr;     // [world][Bmax, DT] gathered teacher text (world > 1): behind the text weights in
+                                         // the exported text allocation
   int off[kMaxWorld + 1] = {};           // global index of every rank's first image (prefix sums of Rs)
   // retrieval metrics (siglip_request_metrics), armed for the next step only
   bool metrics_armed = false;
@@ -363,6 +376,9 @@ int take_ids(siglip_ctx* c) {
   if (c->sample_weights && !c->weights_set)
     return fail(SIGLIP_ERR_STATE,
                 "SIGLIP_OPT_SAMPLE_WEIGHTS is on but siglip_set_sample_weights was not called since the previous step");
+  if (c->distill && !c->teacher_set)
+    return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is on but siglip_set_teacher was not called since the previous step");
+  c->teacher_set = false;
   c->ids_set = false;
   c->extra_ids_set = false;
   c->ximg_ids_set = false;
@@ -414,6 +430,26 @@ inline const float* peer_weights(const siglip_ctx* c, int o) {
   return reinterpret_cast<const float*>(reinterpret_cast<const char*>(c->peer_txt[o]) + weights_offset(c)) +
          static_cast<size_t>(o) * c->w_stride;
 }
+// ---- distillation (SIGLIP_OPT_DISTILL) ----
+// elements between consecutive teacher text chunks of ttxt_all
+inline size_t teacher_stride(const siglip_ctx* c) { return static_cast<size_t>(c->Bmax) * c->DT; }
+inline size_t teacher_chunk_bytes(const siglip_ctx* c, int rank) {
+  return static_cast<size_t>(c->Bs[rank]) * c->DT * sizeof(__nv_bfloat16);
+}
+// byte offset of the gathered teacher text in the exported text allocation: behind the text weights
+inline size_t teacher_offset(const siglip_ctx* c) {
+  return weights_offset(c) + static_cast<size_t>(c->world) * c->w_stride * sizeof(float);
+}
+// Rank o's published teacher text slot, seen through its exported text allocation
+inline const __nv_bfloat16* peer_teacher(const siglip_ctx* c, int o) {
+  return reinterpret_cast<const __nv_bfloat16*>(reinterpret_cast<const char*>(c->peer_txt[o]) + teacher_offset(c)) +
+         static_cast<size_t>(o) * teacher_stride(c);
+}
+// teacher text of chunk `cidx` as the loss kernel reads it: the caller's for the own chunk, the gathered copy otherwise
+inline const void* teacher_chunk(const siglip_ctx* c, int cidx) {
+  return (cidx == c->rank) ? c->t_txt : static_cast<const void*>(c->ttxt_all + cidx * teacher_stride(c));
+}
+
 // A metrics step starts (armed by siglip_request_metrics for this step only): the key block of the step's parity is
 // zeroed, so that no max of an earlier step survives. Double-buffered by parity: a peer may still read my partials of
 // step n in its finalisation while my step n + 1 writes; by step n + 2 that read is over (DESIGN.md, "In-batch
@@ -583,6 +619,19 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
     return rc;
   KernelParams p;
   memset(&p, 0, sizeof(p));
+  // distillation: the teacher's images and text chunk are the second operand pair (K = DT), same boxes as the student's
+  CUtensorMap tmTA = tmA, tmTB = tmB;
+  if (c->distill) {
+    if ((rc = encode_operand(&tmTA, c->t_img, c->R, c->DT, c->DT, 0, 128))) return rc;
+    if ((rc = encode_operand(&tmTB, teacher_chunk(c, cidx), Bn, c->DT, c->DT, 0,
+                             siglip::b_box_rows_kmajor(siglip::cluster_size(cg, mc)))))
+      return rc;
+    p.k_teacher = c->DT;
+    p.teacher_f16 = c->t_f16;
+    p.t_prime_T = c->t_tprime;
+    p.bias_T = c->t_bias;
+    p.distill_lambda = c->t_lambda;
+  }
   p.nprob = 1;
   // fp32-input path: both operands are fp16(x * kXScale), the accumulator is kXScale^2 <img, txt>
   p.prob[0].ab_f16 = c->input_f16;
@@ -645,8 +694,8 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
     p.wait_stats = wstats;
   }
   if ((rc = timing_mark(c, c->ev_loss, c->ev_loss_used, st))) return rc;
-  CKI(siglip::launch_gemm(cg, siglip::kModeLoss, c->stages_loss, mc, siglip::kTileCols, &tmA, &tmB, &tmA, &tmB, &tmG,
-                          p, c->num_sms, st));
+  CKI(siglip::launch_gemm(cg, siglip::kModeLoss, c->stages_loss, mc, siglip::kTileCols, &tmA, &tmB, &tmTA, &tmTB,
+                          &tmG, p, c->num_sms, st));
   if ((rc = timing_mark(c, c->ev_loss, c->ev_loss_used, st))) return rc;
   if (wstats != nullptr) {
     CK(cudaStreamSynchronize(st));
@@ -884,6 +933,25 @@ void add_pull_job(siglip_ctx* c, AuxList& aux, int o, unsigned int s) {
     jw.dst = reinterpret_cast<uint4*>(c->w_all + static_cast<size_t>(o) * c->w_stride);
     jw.n16 = (chunk_weights_bytes(c, o) + 15) / 16;   // within the slot: w_stride is a multiple of 4
   }
+  if (c->distill) {
+    // the chunk's teacher text rides the same flag, like its ids
+    siglip::AuxJob& jt = aux.add(siglip::kAuxCopy);
+    jt.src = reinterpret_cast<const uint4*>(peer_teacher(c, o));
+    jt.dst = reinterpret_cast<uint4*>(c->ttxt_all + o * teacher_stride(c));
+    jt.n16 = teacher_chunk_bytes(c, o) / 16;   // DT % 8 == 0
+  }
+}
+
+// publish job of my teacher text (L0 of the fused step), the twin of the ids publish job below
+void add_teacher_publish_job(siglip_ctx* c, AuxList& aux, unsigned int s) {
+  siglip::AuxJob& j = aux.add(siglip::kAuxCopy);
+  j.src = reinterpret_cast<const uint4*>(c->t_txt);
+  j.dst = reinterpret_cast<uint4*>(c->ttxt_all + c->rank * teacher_stride(c));
+  j.n16 = teacher_chunk_bytes(c, c->rank) / 16;
+  j.wait_flags = c->flags + 2 * kMaxWorld;
+  j.wait_n = c->world;
+  j.wait_value = s - 1;
+  j.site = 11;
 }
 
 // publish job of my text weights (L0 of the fused step), the twin of the ids publish job below
@@ -918,6 +986,9 @@ int copy_own_chunk_data(siglip_ctx* c, cudaStream_t st) {
                        chunk_ids_bytes(c, c->rank), cudaMemcpyDeviceToDevice, st));
   if (c->sample_weights)
     CK(cudaMemcpyAsync(c->w_all + static_cast<size_t>(c->rank) * c->w_stride, c->w_in, chunk_weights_bytes(c, c->rank),
+                       cudaMemcpyDeviceToDevice, st));
+  if (c->distill)
+    CK(cudaMemcpyAsync(c->ttxt_all + c->rank * teacher_stride(c), c->t_txt, teacher_chunk_bytes(c, c->rank),
                        cudaMemcpyDeviceToDevice, st));
   return 0;
 }
@@ -980,6 +1051,9 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
         if (c->sample_weights)
           CK(cudaMemcpyAsync(c->w_all + static_cast<size_t>(nxt) * c->w_stride, peer_weights(c, nxt),
                              chunk_weights_bytes(c, nxt), cudaMemcpyDefault, st));
+        if (c->distill)
+          CK(cudaMemcpyAsync(c->ttxt_all + nxt * teacher_stride(c), peer_teacher(c, nxt), teacher_chunk_bytes(c, nxt),
+                             cudaMemcpyDefault, st));
       }
     }
     if ((rc = run_loss_chunk(c, k, cidx, k == 0, k == 0, img, txt_c, c->Ts[cidx], chunk_ids(c, cidx), t_prime, bias, save,
@@ -1128,7 +1202,10 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   fin.dbias = c->scalars + kSavedScalars + 1;
   // With ids and weights, L0 would carry 9 jobs (3 publishes, 2 conversions, the flag-3 wait, 3 pulls) of
   // kMaxAuxJobs = 8: the image conversion then runs in L1 instead (its first reader is G1, behind L1).
-  const bool img_cvt_in_l1 = W > 1 && ik && c->sample_ids && c->sample_weights;
+  const bool img_cvt_in_l1 = W > 1 && ik && ((c->sample_ids && c->sample_weights) || c->distill);
+  // Distillation adds a teacher publish and a teacher pull to L0 (up to 8 jobs with ids and weights): the own text's
+  // conversion and the flag-3 wait move to L1 as well. G0, their first consumer, and G1 run behind L1.
+  const bool l0_work_in_l1 = W > 1 && ik && c->distill;
 
   // ---- L0: own chunk. Its auxiliary warps also publish my text to the peers and start the first pull ----
   {
@@ -1141,6 +1218,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
         // before the text job's ticket, so the same signal covers them.
         if (c->sample_ids) add_ids_publish_job(c, aux, s);
         if (c->sample_weights) add_weights_publish_job(c, aux, s);
+        if (c->distill) add_teacher_publish_job(c, aux, s);
         siglip::AuxJob& cp = aux.add(siglip::kAuxCopy);
         cp.src = reinterpret_cast<const uint4*>(txt);
         cp.dst = reinterpret_cast<uint4*>(c->txt_all + r * stride);
@@ -1159,9 +1237,11 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
         if ((rc = signal_peers(c, 0, s, st))) return rc;
       }
     }
-    add_cvt_jobs(c, aux, 0, !img_cvt_in_l1, img, own_txt, c->T);
+    if (!l0_work_in_l1) add_cvt_jobs(c, aux, 0, !img_cvt_in_l1, img, own_txt, c->T);
     if (W > 1) {
-      if (ik) {
+      if (ik && l0_work_in_l1) {
+        // the flag-3 wait runs in L1 (before G1 all the same)
+      } else if (ik) {
         // my contribution slots of the previous backward must have been read by their owners (flag 3) before G1
         // overwrites the first of them
         siglip::AuxJob& w3 = aux.add(siglip::kAuxWaitOnly);
@@ -1187,6 +1267,14 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
     {
       AuxList aux;
       add_cvt_jobs(c, aux, 1, k == 1 && img_cvt_in_l1, img, txt_c, c->Ts[cidx]);
+      if (k == 1 && l0_work_in_l1) {
+        add_cvt_jobs(c, aux, 0, false, img, reinterpret_cast<const __nv_bfloat16*>(txt), c->T);
+        siglip::AuxJob& w3 = aux.add(siglip::kAuxWaitOnly);
+        w3.wait_flags = c->flags + 3 * kMaxWorld;
+        w3.wait_n = W;
+        w3.wait_value = n - 1;
+        w3.site = 13;
+      }
       if (k + 1 < W) add_pull_job(c, aux, step_owner(c, r, k + 1), s);
       const bool lastL = (k == W - 1);
       EndSignal end = (lastL && ik) ? end_signal(c, 2, s) : EndSignal();   // "I have pulled everyone's text"
@@ -1289,7 +1377,7 @@ int siglip_device_count(void) {
 // Bs[p]: rank p's batch; Rs[p] >= Bs[p]: its images (paired ones first, then its extra images); Ts[p] >= Bs[p]: its
 // texts (paired ones first, then its hard negatives). Every argument is checked before the first CUDA call.
 static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, const int* Bs, const int* Rs,
-                           const int* Ts, int D) {
+                           const int* Ts, int D, int DT = 0) {
   if (out == nullptr) return fail(SIGLIP_ERR_INVALID, "out is null");
   *out = nullptr;
   if (world < 1 || world > kMaxWorld || rank < 0 || rank >= world)
@@ -1307,6 +1395,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     Emax = Rs[p] - Bs[p] > Emax ? Rs[p] - Bs[p] : Emax;
   }
   if (D < 8 || (D % 8) != 0) return fail(SIGLIP_ERR_INVALID, "need D a positive multiple of 8");
+  if (DT < 0 || (DT % 8) != 0) return fail(SIGLIP_ERR_INVALID, "need D_teacher a positive multiple of 8 (0: no teacher)");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     cudaGetLastError();
@@ -1344,6 +1433,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   c->Emax = Emax;
   c->own_pos_ids = c->R > c->B && c->T > c->B;
   c->D = D;
+  c->DT = DT;
   c->Bp = round_up(Bmax, 256);
   c->Tp = round_up(Tmax, 256);
   c->Rp = round_up(Rmax, 256);
@@ -1399,12 +1489,16 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     // one exported handle covers all four (SIGLIP_OPT_SAMPLE_WEIGHTS may be set after the handle exchange, so the
     // weight slots exist whatever the options)
     const size_t w_bytes = static_cast<size_t>(world) * c->w_stride * sizeof(float);
+    // a distillation context also gathers the teacher text there (nothing without a teacher)
+    const size_t t_bytes = teacher_stride(c) * world * sizeof(__nv_bfloat16);
     CK(alloc(reinterpret_cast<void**>(&c->txt_all),
-             stride * world * sizeof(__nv_bfloat16) + world * ids_slot_bytes + mkeys_bytes + w_bytes));
+             stride * world * sizeof(__nv_bfloat16) + world * ids_slot_bytes + mkeys_bytes + w_bytes + t_bytes));
     c->ids_all = reinterpret_cast<int64_t*>(c->txt_all + stride * world);   // 16-byte aligned: D % 8 == 0
     c->mkeys[0] = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(c->txt_all) + mkeys_offset(c));
     c->mkeys[1] = c->mkeys[0] + mkeys_block(c);
     c->w_all = reinterpret_cast<float*>(reinterpret_cast<char*>(c->txt_all) + weights_offset(c));
+    if (DT > 0)
+      c->ttxt_all = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<char*>(c->txt_all) + teacher_offset(c));
     CK(alloc(reinterpret_cast<void**>(&c->slots), stride * world * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dimg_acc), static_cast<size_t>(c->R) * D * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dtxt_acc), static_cast<size_t>(c->T) * D * sizeof(float)));
@@ -1461,9 +1555,41 @@ int siglip_ctx_create_extras(siglip_ctx** out, int device, int rank, int world, 
   return ctx_create_impl(out, device, rank, world, batch_per_rank, images_per_rank, texts_per_rank, D);
 }
 
+int siglip_ctx_create_distill(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank, int D,
+                              int D_teacher) {
+  if (batch_per_rank == nullptr) return fail(SIGLIP_ERR_INVALID, "batch_per_rank is null");
+  if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
+  return ctx_create_impl(out, device, rank, world, batch_per_rank, batch_per_rank, batch_per_rank, D, D_teacher);
+}
+
+int siglip_set_teacher(siglip_ctx* c, const void* timg, const void* ttxt, int teacher_f16, const float* t_prime_T,
+                       const float* bias_T, float lambda) {
+  if (c == nullptr || timg == nullptr || ttxt == nullptr || t_prime_T == nullptr || bias_T == nullptr)
+    return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->distill) return fail(SIGLIP_ERR_STATE, "siglip_set_teacher needs SIGLIP_OPT_DISTILL = 1");
+  if (!(lambda > 0.0f && lambda <= 1.0f)) return fail(SIGLIP_ERR_INVALID, "distillation lambda must be in (0, 1]");
+  if (teacher_f16 != 0 && teacher_f16 != 1) return fail(SIGLIP_ERR_INVALID, "teacher_f16 must be 0 or 1");
+  if ((reinterpret_cast<uintptr_t>(timg) | reinterpret_cast<uintptr_t>(ttxt)) & 15u)
+    return fail(SIGLIP_ERR_INVALID, "teacher embeddings must be 16-byte aligned");
+  c->t_img = timg;
+  c->t_txt = ttxt;
+  c->t_f16 = teacher_f16;
+  c->t_tprime = t_prime_T;
+  c->t_bias = bias_T;
+  c->t_lambda = lambda;
+  c->teacher_set = true;
+  return 0;
+}
+
 int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
   if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "ctx is null");
   switch (option) {
+    case SIGLIP_OPT_DISTILL:
+      if (value && c->DT == 0)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL needs a context created with siglip_ctx_create_distill");
+      c->distill = value ? 1 : 0;
+      c->teacher_set = false;
+      return 0;
     case SIGLIP_OPT_CTA_GROUP:
       if (value != 1 && value != 2) return fail(SIGLIP_ERR_INVALID, "cta_group must be 1 or 2");
       c->cta_group = value;
@@ -1589,6 +1715,7 @@ int siglip_ctx_export_handles(siglip_ctx* c, void* out_bytes, size_t capacity) {
   b.Tmax = c->Tmax;
   b.R = c->R;
   b.Rmax = c->Rmax;
+  b.D_teacher = c->DT;
   if (gethostname(b.host, sizeof(b.host) - 1) != 0) b.host[0] = 0;
   memcpy(out_bytes, &b, sizeof(b));
   return 0;
@@ -1662,8 +1789,12 @@ int siglip_ctx_import_handles(siglip_ctx* c, const void* all_ranks_bytes, size_t
       return fail(SIGLIP_ERR_INVALID,
                   "peer context has a different image count than this rank was told: every rank must be created with "
                   "the same images_per_rank list (siglip_ctx_create_extras; batch + extra images per rank)");
+    if (b.D_teacher != c->DT)
+      return fail(SIGLIP_ERR_INVALID,
+                  "peer context has a different D_teacher than this rank: every rank must be created with the same "
+                  "siglip_ctx_create_distill arguments");
     if (p == c->rank) continue;
-    char me[64] = {0};
+    char me[sizeof(b.host)] = {0};
     if (gethostname(me, sizeof(me) - 1) != 0) me[0] = 0;
     if (strncmp(me, b.host, sizeof(me)) != 0) {
       char buf[384];
@@ -1910,6 +2041,8 @@ int siglip_host_submit_grads(siglip_ctx* c, const void* img_host, const void* tx
   if (c->sample_weights)
     return fail(SIGLIP_ERR_STATE,
                 "the host-buffer entries take no sample weights: unavailable under SIGLIP_OPT_SAMPLE_WEIGHTS");
+  if (c->distill)
+    return fail(SIGLIP_ERR_STATE, "the host-buffer entries take no teacher: unavailable under SIGLIP_OPT_DISTILL");
   const bool with_grads = dimg_host_bf16 != nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   CK(cudaSetDevice(c->device));
@@ -2072,6 +2205,44 @@ int siglip_debug_set_text_chunk(siglip_ctx* c, int chunk, const void* txt_dev, v
   CK(cudaMemcpyAsync(c->txt_all + chunk * chunk_stride(c), txt_dev,
                      static_cast<size_t>(c->Ts[chunk]) * c->D * sizeof(__nv_bfloat16), cudaMemcpyDeviceToDevice,
                      static_cast<cudaStream_t>(cuda_stream)));
+  return 0;
+}
+
+int siglip_debug_set_teacher_text_chunk(siglip_ctx* c, int chunk, const void* ttxt_dev, void* cuda_stream) {
+  if (c == nullptr || ttxt_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (c->DT == 0) return fail(SIGLIP_ERR_STATE, "not a distillation context (siglip_ctx_create_distill)");
+  if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
+  CK(cudaMemcpyAsync(c->ttxt_all + chunk * teacher_stride(c), ttxt_dev, teacher_chunk_bytes(c, chunk),
+                     cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
+  return 0;
+}
+
+int siglip_teacher_convert_f32(siglip_ctx* c, int rows, const float* x_f32, void* out_16bit, int f16,
+                               void* cuda_stream) {
+  if (c == nullptr || x_f32 == nullptr || out_16bit == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (c->DT == 0) return fail(SIGLIP_ERR_STATE, "not a distillation context (siglip_ctx_create_distill)");
+  if (rows < 1) return fail(SIGLIP_ERR_INVALID, "rows must be >= 1");
+  if ((reinterpret_cast<uintptr_t>(x_f32) & 15u) || (reinterpret_cast<uintptr_t>(out_16bit) & 15u))
+    return fail(SIGLIP_ERR_INVALID, "buffers must be 16-byte aligned");
+  CK(cudaSetDevice(c->device));
+  CKI(siglip::launch_convert_f32(x_f32, out_16bit, static_cast<size_t>(rows) * c->DT, f16 ? kXScale : 0.0f, c->num_sms,
+                                 static_cast<cudaStream_t>(cuda_stream)));
+  c->launches++;
+  return 0;
+}
+
+int siglip_teacher_normalize_fwd(siglip_ctx* c, int rows, const void* x, int in_bf16, void* xhat, float* inv_norm,
+                                 int f16, void* cuda_stream) {
+  if (c == nullptr || x == nullptr || xhat == nullptr || inv_norm == nullptr)
+    return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (c->DT == 0) return fail(SIGLIP_ERR_STATE, "not a distillation context (siglip_ctx_create_distill)");
+  if (rows < 1) return fail(SIGLIP_ERR_INVALID, "rows must be >= 1");
+  if ((reinterpret_cast<uintptr_t>(x) & 15u) || (reinterpret_cast<uintptr_t>(xhat) & 15u))
+    return fail(SIGLIP_ERR_INVALID, "buffers must be 16-byte aligned");
+  CK(cudaSetDevice(c->device));
+  CKI(siglip::launch_normalize_fwd(x, in_bf16, static_cast<__nv_bfloat16*>(xhat), inv_norm, rows, c->DT,
+                                   f16 ? kXScale : 0.0f, c->num_sms, static_cast<cudaStream_t>(cuda_stream)));
+  c->launches++;
   return 0;
 }
 

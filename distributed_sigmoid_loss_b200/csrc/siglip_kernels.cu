@@ -49,9 +49,11 @@ struct Cfg {
   static constexpr int kBBytes = kTileNT * kBlockK * 2;            // 16 KiB (32 KiB for 256-column tiles)
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = kStagesT;
-  static constexpr int kStagingBytes = (kMode == kModeLoss) ? kNumEpiWarps * kStagingBytesPerWarp : 0;
+  static constexpr int kStagingBytes = (kMode != kModeOut) ? kNumEpiWarps * kStagingBytesPerWarp : 0;
+  // kModeDistill: the teacher's probabilities (fp32, one 128 x 128 tile) follow the barrier block
+  static constexpr int kPBytes = (kMode == kModeDistill) ? kBlockM * kTileNT * 4 : 0;
   static constexpr int kSmemBytes =
-      kStages * kStageBytes + kStagingBytes + 1024 /*barriers, reduction*/ + 1024 /*alignment slack*/;
+      kStages * kStageBytes + kStagingBytes + 1024 /*barriers, reduction*/ + kPBytes + 1024 /*alignment slack*/;
   static_assert(kSmemBytes <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
 };
 
@@ -383,6 +385,107 @@ __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int 
 }
 
 // -------------------------------------------------------------------------------------------------
+// Distillation (kModeDistill). Per element, with p the teacher's probability of the pair and y its hard label:
+//   q = (1 - lambda) y + lambda p,   term = softplus(z) - q z,   g = sigma(z) - q      (times the pair's weight)
+// sigma and softplus take the series of loss_slab_fast in a 16x32 slab whose z are all < kFastZ (warp vote, as in the
+// plain loss kernel) and the exact form in every other slab. The teacher's accumulator goes through the same functions
+// (distill_slab_series, distill_sigma) on the same slab geometry, so a teacher equal to the student gives
+// p == sigma(z) bit for bit, and g == 0 at lambda = 1.
+// -------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool distill_slab_series(const float* v, float t, float b) {
+  float smax = v[0];
+#pragma unroll
+  for (int j = 1; j < 16; ++j) smax = fmaxf(smax, v[j]);
+  return __all_sync(0xffffffffu, fmaf(smax, t, b) < kFastZ);   // z is monotone in s (t > 0)
+}
+
+__device__ __forceinline__ void distill_terms(float s, float t, float b, float tl, float bl, bool series, float& z,
+                                              float& sig, float& l) {
+  z = fmaf(s, t, b);
+  if (series) {
+    const float e = ex2_approx(fmaf(s, tl, bl));        // exp(z) < 2^-6
+    sig = e * fmaf(e, e - 1.0f, 1.0f);                  // e (1 - e + e^2)
+    l = e * fmaf(e, fmaf(e, 0.33333334f, -0.5f), 1.0f); // log1p(e) = e (1 - e/2 + e^2/3)
+  } else {
+    const float e = ex2_approx(-fabsf(z) * kLog2e);    // exp(-|z|)
+    const float r = rcp_approx(1.0f + e);
+    sig = (z >= 0.f) ? r : e * r;
+    l = e * log1p_over_e(e);                           // softplus(z) - max(z, 0)
+  }
+}
+
+__device__ __forceinline__ float distill_sigma(float s, float t, float b, float tl, float bl, bool series) {
+  float z, sig, l;
+  distill_terms(s, t, b, tl, bl, series, z, sig, l);
+  return sig;
+}
+
+// Thread-private fp32 slot of fragment element i in the teacher-probability buffer: element-major, so that the 256
+// consumer threads touch 256 consecutive words (no bank conflicts) and each reads back only what it wrote.
+__device__ __forceinline__ uint32_t distill_p_addr(uint32_t pbuf, int i) {
+  return pbuf + 4u * (static_cast<uint32_t>(i) * (kNumEpiWarps * 32u) + threadIdx.x);
+}
+
+// One 16x32 slab of the distillation epilogue. kMask: rows / columns past the matrix are dropped and labels are applied
+// (the own-chunk diagonal, whose g goes to g_diag in fp32, and the pos bits of sample ids); without it y = 0.
+// w: per-sample weights (cw / rw0 / rw1 as in slab_w) when non-zero.
+template <bool kMask>
+__device__ __forceinline__ void distill_slab(const float* v, uint32_t pbuf, int c, float t, float b, float tl, float bl,
+                                             float lambda, int row_lo, int col0, int c_lo, int nrows, int ncols,
+                                             bool store_g, const GStore& gst, float gscale, float* g_diag, bool on_diag,
+                                             uint32_t pos, bool w, const float* cw, float rw0, float rw1,
+                                             float& acc_sp, float& acc_g, float& acc_gs) {
+  uint32_t packed[8];
+  float g_prev = 0.f;
+  const float one_minus = 1.0f - lambda;
+  const bool series = distill_slab_series(v, t, b);
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const float s = v[i];
+    float pt;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(pt) : "r"(distill_p_addr(pbuf, 16 * c + i)));
+    float z, sig, l;
+    distill_terms(s, t, b, tl, bl, series, z, sig, l);
+    float y = 0.f;
+    bool valid = true, own_diag = false;
+    int row = 0;
+    if constexpr (kMask) {
+      row = row_lo + 8 * ((i >> 1) & 1);
+      const int col = col0 + 8 * (i >> 2) + c_lo + (i & 1);
+      valid = (row < nrows) && (col < ncols);
+      own_diag = on_diag && row == col;
+      y = (own_diag || ((pos >> i) & 1u)) ? 1.0f : 0.f;
+    }
+    const float q = fmaf(lambda, pt, one_minus * y);
+    float sp = ((z >= 0.f) ? (1.0f - q) * z : -q * z) + l;   // softplus(z) - q z without cancelling at q = 1
+    float g = sig - q;
+    if (w) {
+      const float wi = slab_w(i, cw, rw0, rw1);
+      sp *= wi;
+      g *= wi;
+    }
+    float g_store = g;
+    if constexpr (kMask) {
+      if (own_diag) {                                  // the own diagonal stays out of the 16-bit operand
+        if (store_g && valid) g_diag[row] = g;
+        g_store = 0.f;
+      }
+      sp = valid ? sp : 0.f;
+      g = valid ? g : 0.f;
+      g_store = valid ? g_store : 0.f;
+    }
+    acc_sp += sp;
+    acc_g += g;
+    acc_gs = fmaf(g, s, acc_gs);
+    if (i & 1)
+      packed[2 * (i >> 2) + ((i >> 1) & 1)] = pack_16x2<true>(g_prev, g_store * gscale);
+    else
+      g_prev = g_store * gscale;
+  }
+  if (store_g) store_g_slab(gst, col0, packed);
+}
+
+// -------------------------------------------------------------------------------------------------
 // In-batch retrieval metrics (kMetrics): the argmax of every row and column of the logits, from the accumulator tile.
 // Key of a candidate: (order-preserving bits of s) << 32 | (0xFFFFFFFF - global index). The unsigned max of two keys is
 // the larger s, ties to the lower index; 0 is "no candidate" (every real key is larger). z = t s + b is monotone in s
@@ -631,6 +734,81 @@ __device__ __forceinline__ void mma_loop_f8(float (&sum)[64], float (&acc)[64], 
   }
 }
 
+// Epilogue of the distillation loss kernel over one 128 x 128 tile: the loss kernel's slab walk (metric keys, masking,
+// the own diagonal, sample ids and weights, now read at run time) with distill_slab in place of the hard-label slabs.
+// The three sums go into the thread's compensated running sums.
+__device__ __forceinline__ void distill_epilogue(const KernelParams& p, const float (&acc)[kTileN / 2], uint32_t pbuf,
+                                                 const CUtensorMap* tmG, uint32_t staging_base, int warp, int wg,
+                                                 int lane, int row0, int col_base, int row_lo, int c_lo,
+                                                 const Problem& pr, float t_eff, float bias, float tl, float bl,
+                                                 uint64_t policy, float& s_sp, float& c_sp, float& s_g, float& c_g,
+                                                 float& s_gs, float& c_gs) {
+  if (p.row_keys != nullptr) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
+  float acc_sp = 0.f, acc_g = 0.f, acc_gs = 0.f;
+  const bool edge = (row0 + kBlockM > pr.M) || (col_base + kTileN > pr.N);
+  const bool diag = p.own_chunk && (row0 == col_base);
+  const bool sg = p.store_g != 0;
+  GStore gst;
+  gst.tmap = tmG;
+  gst.stage = staging_base + static_cast<uint32_t>(warp) * kStagingBytesPerWarp;
+  gst.row0 = row0 + wg * 64 + (warp & 3) * 16;
+  gst.lane = lane;
+  gst.policy = policy;
+  const bool ids = p.row_ids != nullptr, w = p.row_w != nullptr;
+  int64_t rid0 = 0, rid1 = 0;
+  uint32_t rpos = 0u;
+  if (ids) {
+    rid0 = p.row_ids[min(row_lo, pr.M - 1)];
+    rid1 = p.row_ids[min(row_lo + 8, pr.M - 1)];
+    rpos = (row_lo < p.row_pos_n ? 0x3333u : 0u) | (row_lo + 8 < p.row_pos_n ? 0xCCCCu : 0u);
+  }
+  float rw0 = 1.f, rw1 = 1.f;
+  if (w) {
+    rw0 = p.row_w[min(row_lo, pr.M - 1)];
+    rw1 = p.row_w[min(row_lo + 8, pr.M - 1)];
+  }
+#pragma unroll
+  for (int c = 0; c < kTileN / 32; ++c) {
+    const float* v = acc + 16 * c;
+    const int col0 = col_base + 32 * c;
+    float cw[8];
+    if (w) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) cw[j] = p.col_w[min(col0 + 8 * (j >> 1) + c_lo + (j & 1), pr.N - 1)];
+    }
+    const bool slab_diag = diag && (gst.row0 < col0 + 32) && (col0 < gst.row0 + 16);
+    const bool slab_edge = edge && ((gst.row0 + 16 > pr.M) || (col0 + 32 > pr.N));
+    uint32_t pos = 0;
+    bool slab_pos = false;
+    if (ids) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int e1 = 0; e1 < 2; ++e1) {
+          const int col = col0 + 8 * j + c_lo + e1;
+          if (col < p.col_pos_n) {
+            const int64_t cid = p.col_ids[col];
+            pos |= static_cast<uint32_t>(cid == rid0) << (4 * j + e1);
+            pos |= static_cast<uint32_t>(cid == rid1) << (4 * j + 2 + e1);
+          }
+        }
+      }
+      pos &= rpos;
+      slab_pos = __any_sync(0xffffffffu, pos != 0u);
+    }
+    // the series / exact choice is made per slab inside (distill_slab_series)
+    if (!slab_edge && !slab_diag && !slab_pos)
+      distill_slab<false>(v, pbuf, c, t_eff, bias, tl, bl, p.distill_lambda, row_lo, col0, c_lo, pr.M, pr.N, sg, gst,
+                          p.g_scale, p.g_diag, false, 0u, w, cw, rw0, rw1, acc_sp, acc_g, acc_gs);
+    else
+      distill_slab<true>(v, pbuf, c, t_eff, bias, tl, bl, p.distill_lambda, row_lo, col0, c_lo, pr.M, pr.N, sg, gst,
+                         p.g_scale, p.g_diag, slab_diag, pos, w, cw, rw0, rw1, acc_sp, acc_g, acc_gs);
+  }
+  kahan_add(s_sp, c_sp, acc_sp);
+  kahan_add(s_g, c_g, acc_g);
+  kahan_add(s_gs, c_gs, acc_gs);
+}
+
 // -------------------------------------------------------------------------------------------------
 // The kernel
 // -------------------------------------------------------------------------------------------------
@@ -643,6 +821,9 @@ __device__ __forceinline__ void mma_loop_f8(float (&sum)[64], float (&acc)[64], 
 // kWeights: the loss kernel with per-sample weights (SIGLIP_OPT_SAMPLE_WEIGHTS); its own instantiation for the same
 // reason, composing with kIds and kMetrics.
 // kTileNT: columns of a tile. 256 (kWideTileN) exists for the out kernel with 16-bit operands only (no split-K).
+// kMode = kModeDistill: the loss kernel of a distillation step, its own instantiation (kDistillStages, 128-column
+// tiles): the teacher's k-blocks of every tile first (tmA1 / tmB1), its probabilities in shared memory, then the
+// student's k-loop and the soft-target epilogue (distill_epilogue); ids, weights and metrics are runtime options there.
 template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false,
           bool kWeights = false, int kTileNT = kTileN>
 __global__ void __launch_bounds__(kNumThreads, 1)
@@ -656,6 +837,8 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
   static_assert(!kWeights || kMode == kModeLoss, "sample weights are a loss-kernel option");
   static_assert(kTileNT == kTileN || (kTileNT == kWideTileN && kMode == kModeOut && !kF8),
                 "256-column tiles: out kernel, 16-bit operands");
+  static_assert(kMode != kModeDistill || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
+                "the distillation kernel takes ids, weights and metrics as runtime options");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -684,6 +867,10 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
     prefetch_tmap(&tmA0);
     prefetch_tmap(&tmB0);
     if (p.nprob > 1) {
+      prefetch_tmap(&tmA1);
+      prefetch_tmap(&tmB1);
+    }
+    if constexpr (kMode == kModeDistill) {
       prefetch_tmap(&tmA1);
       prefetch_tmap(&tmB1);
     }
@@ -724,7 +911,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
     // wave and must survive the sigma operand streaming through the 50 MB L2 once per pass. The sigma operand itself
     // keeps normal priority: the column tiles of a row panel read the same lines a little apart in time.
     const uint64_t pol_b = l2_policy_evict_last();
-    const uint64_t pol_a = (kMode == kModeLoss) ? pol_b : l2_policy_evict_normal();
+    const uint64_t pol_a = (kMode != kModeOut) ? pol_b : l2_policy_evict_normal();
     for (int t = cluster_id; t < total_tiles; t += num_clusters) {
       const TileCoord tc = decode_tile<kCS>(p, t, static_cast<int>(crank));
       const Problem& pr = p.prob[tc.prob];
@@ -738,6 +925,31 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       const int a_mn = pr.a_mn, b_mn = pr.b_mn;
       int kb0, kb1;
       item_k_range(p, tc, num_kb, kb0, kb1);
+      if constexpr (kMode == kModeDistill) {
+        // the teacher's k-blocks of the tile first (both K-major, K = D_T), through the same ring
+        constexpr int kRows = kTileN / kCS;
+        const int num_kb_t = (p.k_teacher + kBlockK - 1) / kBlockK;
+        for (int kb = 0; kb < num_kb_t; ++kb) {
+          mbar_wait(empty0 + 8u * stage, phase ^ 1u, p.dbg, 1, t, kb, 0, p.wait_stats ? &w_empty : nullptr);
+          if (elect_one_sync()) {
+            const uint32_t sA = smem_base + stage * C::kStageBytes;
+            const uint32_t sB = sA + C::kABytes;
+            const uint32_t fb = full0 + 8u * stage;
+            mbar_arrive_expect_tx(fb, C::kStageBytes);
+            tma_load_2d_hint(&tmA1, fb, sA, kb * kBlockK, m_idx, pol_a);
+            const uint32_t dst = sB + crank * (kRows * 128);
+            if constexpr (kCS == 1)
+              tma_load_2d_hint(&tmB1, fb, dst, kb * kBlockK, n_idx, pol_b);
+            else
+              tma_load_2d_mcast(&tmB1, fb, dst, kb * kBlockK, n_idx + static_cast<int>(crank) * kRows, kMcMask);
+          }
+          __syncwarp();
+          if (++stage == C::kStages) {
+            stage = 0;
+            phase ^= 1u;
+          }
+        }
+      }
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(empty0 + 8u * stage, phase ^ 1u, p.dbg, 1, t, kb, 0, p.wait_stats ? &w_empty : nullptr);
         if (elect_one_sync()) {
@@ -790,11 +1002,21 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
     const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // first fragment row (the second is r_lo + 8)
     const int c_lo = 2 * (lane & 3);                // first fragment column of every 8-column group
     const float t_exact = expf(load_t_prime(p));
-    const float bias = (kMode == kModeLoss) ? *p.bias : 0.f;
+    const float bias = (kMode != kModeOut) ? *p.bias : 0.f;
     // loss kernel: z = t_eff * acc + b with t_eff = t * s_scale (the accumulator is 2^8 <img, txt> for fp16 x 16 operands)
-    const float s_scale = (kMode == kModeLoss && p.s_scale != 0.f) ? p.s_scale : 1.0f;
+    const float s_scale = (kMode != kModeOut && p.s_scale != 0.f) ? p.s_scale : 1.0f;
     const float t_eff = t_exact * s_scale;
     const float tl = t_eff * kLog2e, bl = bias * kLog2e;
+    // distillation: the teacher's z^T = t_T s^T + b_T (its accumulator is 2^8 s^T for fp16 x 16 operands)
+    float tT_eff = 0.f, bias_T = 0.f, tT_l = 0.f, bT_l = 0.f;
+    uint32_t pbuf = 0;
+    if constexpr (kMode == kModeDistill) {
+      tT_eff = expf(*p.t_prime_T) * (p.teacher_f16 ? 1.0f / 256.0f : 1.0f);
+      bias_T = *p.bias_T;
+      tT_l = tT_eff * kLog2e;
+      bT_l = bias_T * kLog2e;
+      pbuf = bar_base + 1024u;   // behind the barrier block (Cfg::kPBytes)
+    }
     // per-thread running sums over the tiles of this CTA: compensated fp32 (Kahan); fp64 only at the very end
     float s_sp = 0.f, s_g = 0.f, s_gs = 0.f, c_sp = 0.f, c_g = 0.f, c_gs = 0.f;
     long long w_full = 0;
@@ -839,11 +1061,38 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
         const uint32_t b_adv = pr.b_mn ? (kMmaK * 128u) >> 4 : 32u >> 4;
         const uint64_t adesc0 = make_smem_desc_sw128(smem_base + static_cast<uint32_t>(wg) * 8192u, a_lbo, 1024u);
         const uint64_t bdesc0 = make_smem_desc_sw128(smem_base + C::kABytes, b_lbo, 1024u);
+        if constexpr (kMode == kModeDistill) {
+          // s^T of the tile over the teacher's k-blocks, then p = sigma(t_T s^T + b_T) into this thread's slots. The
+          // student's k-loop below starts from zero (its first wgmma does not accumulate); the producer is already
+          // streaming its operands while the conversion runs.
+          const int num_kb_t = (p.k_teacher + kBlockK - 1) / kBlockK;
+          if (p.teacher_f16)
+            mma_loop<1, 0, 0, kCS, C::kStageBytes, kTileN>(acc, 0, num_kb_t, stage, phase, C::kStages, adesc0, bdesc0,
+                                                           a_adv, b_adv, full0, empty0, lane, p.dbg, t, w_full_p);
+          else
+            mma_loop<0, 0, 0, kCS, C::kStageBytes, kTileN>(acc, 0, num_kb_t, stage, phase, C::kStages, adesc0, bdesc0,
+                                                           a_adv, b_adv, full0, empty0, lane, p.dbg, t, w_full_p);
+#pragma unroll
+          for (int c = 0; c < kTileN / 32; ++c) {
+            const bool series = distill_slab_series(acc + 16 * c, tT_eff, bias_T);
+#pragma unroll
+            for (int i = 16 * c; i < 16 * c + 16; ++i) {
+              const float pv = distill_sigma(acc[i], tT_eff, bias_T, tT_l, bT_l, series);
+              asm volatile("st.shared.f32 [%0], %1;" ::"r"(distill_p_addr(pbuf, i)), "f"(pv) : "memory");
+            }
+          }
+        }
 #define SIGLIP_MMA_LOOP(T, TA, TB)                                                                                  \
   mma_loop<T, TA, TB, kCS, C::kStageBytes, kTileNT>(acc, kb0, kb1, stage, phase, C::kStages, adesc0, bdesc0, a_adv, \
                                                     b_adv, full0, empty0, lane, p.dbg, t, w_full_p)
         const int sel = pr.a_mn * 2 + pr.b_mn;
-        if (fp8) {
+        if constexpr (kMode == kModeDistill) {
+          // the loss operands (student and teacher) are always K-major: no MN-major variants in this instantiation
+          if (pr.ab_f16)
+            SIGLIP_MMA_LOOP(1, 0, 0);
+          else
+            SIGLIP_MMA_LOOP(0, 0, 0);
+        } else if (fp8) {
           // kF8 instantiation only (launch_gemm routes 8-bit operands there): the result lands in acc8
           if constexpr (kF8)
             mma_loop_f8<kCS, C::kStageBytes>(acc8, acc, kb0, kb1, stage, phase, C::kStages, adesc0, bdesc0, full0,
@@ -868,7 +1117,10 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       if (p.aux_trace != nullptr && threadIdx.x == 0 && t == cluster_id && blockIdx.x == 0)
         p.aux_trace[6] = globaltimer_ns();                                   // first tile's MMAs done (CTA 0)
 
-      if constexpr (kMode == kModeLoss) {
+      if constexpr (kMode == kModeDistill) {
+        distill_epilogue(p, acc, pbuf, &tmG, staging_base, warp, wg, lane, row0, col_base, row_lo, c_lo, pr, t_eff, bias,
+                         tl, bl, g_store_policy, s_sp, c_sp, s_g, c_g, s_gs, c_gs);
+      } else if constexpr (kMode == kModeLoss) {
         // argmax keys first, on the raw accumulator: whichever path each slab then takes below
         if constexpr (kMetrics) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
         float acc_sp = 0.f, acc_g = 0.f, acc_gs = 0.f;
@@ -1069,7 +1321,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       p.wait_stats[8ll * blockIdx.x + 1] = static_cast<unsigned long long>(w_full);
       p.wait_stats[8ll * blockIdx.x + 3] = static_cast<unsigned long long>(clock_cycles() - c_start);
     }
-    if constexpr (kMode == kModeLoss) {
+    if constexpr (kMode != kModeOut) {
       // all sigma slabs of this warp must be in global memory before the kernel ends
       if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
       // fixed-order reduction: lanes -> warp -> consumer warps -> one slot per CTA (summed later in slot order)
@@ -1678,7 +1930,7 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
                 const CUtensorMap* tmG, const KernelParams& p, int num_sms, cudaStream_t stream) {
   using C = Cfg<kMode, kStages, kTileNT>;
   auto kern = siglip_gemm_kernel<kMode, kStages, kCS, kF8, kIds && kMode == kModeLoss, kMetrics && kMode == kModeLoss,
-                                 kWeights && kMode == kModeLoss, kTileNT>;
+                                 kWeights && kMode == kModeLoss, kTileNT>;   // kModeDistill: runtime options
   static bool attr_set = false;
   cudaError_t e = cudaSuccess;
   if (!attr_set) {
@@ -1747,7 +1999,7 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
   // a loss launch keeps the grid of the largest chunk of its forward (KernelParams::grid_n): CTA i owns partial slot i
   // in every chunk, and the CTAs without a tile only carry their slot forward
   int grid_tiles = total_tiles;
-  if (kMode == kModeLoss && pl.grid_n > pl.prob[0].N)
+  if (kMode != kModeOut && pl.grid_n > pl.prob[0].N)
     grid_tiles = pl.prob[0].tiles_m * ((pl.grid_n + kTileN - 1) / kTileN);
   if (clusters > grid_tiles) clusters = grid_tiles;
   if (clusters < 1) clusters = 1;
@@ -1845,6 +2097,13 @@ int launch_gemm(int cta_group, int mode, int stages, int mcast, int tile_n, cons
     }
   }
   if (tile_n != kTileN) return static_cast<int>(cudaErrorInvalidValue);
+  if (mode == kModeLoss && p.k_teacher > 0) {   // distillation: kModeDistill, kDistillStages whatever `stages` asks
+    switch (cluster_size(cta_group, mcast)) {
+      case 4: return launch_impl<kModeDistill, kDistillStages, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      case 2: return launch_impl<kModeDistill, kDistillStages, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      default: return launch_impl<kModeDistill, kDistillStages, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+    }
+  }
   switch (cluster_size(cta_group, mcast)) {
     case 4:
       if (mode == kModeLoss) SIGLIP_LAUNCH_STAGES(kModeLoss, 4);

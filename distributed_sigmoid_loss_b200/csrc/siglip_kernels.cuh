@@ -150,9 +150,24 @@ struct KernelParams {
   // and read only by the kIds instantiations: the row twin of col_pos_n.
   int row_pos_n;   // loss kernel, kIds: rows that carry ids (row_ids has this many entries): the paired images, or all
                    // of them under SIGLIP_OPT_EXTRA_IMAGE_IDS. Rows past it never match
+  // Distillation from a frozen teacher (siglip_set_teacher). Appended last like the fields above. k_teacher > 0 selects
+  // the distillation loss kernel (kModeDistill, its own instantiation): every tile first contracts the teacher's image
+  // rows (tmA1) with the teacher's text chunk (tmB1) over k_teacher, turns s^T into p = sigma(t_T s^T + b_T), then runs
+  // the student's k-loop; the target of pair (i, j) is q = (1 - lambda) y + lambda p. In that kernel ids (row_ids),
+  // weights (row_w) and metric keys (row_keys) are runtime options.
+  int k_teacher;              // D_T (multiple of 8); 0 = no teacher
+  int teacher_f16;            // teacher operands are fp16(x * 16) instead of bf16
+  const float* t_prime_T;     // fp32 device scalars: t_T = exp(t'_T), b_T
+  const float* bias_T;
+  float distill_lambda;       // in (0, 1]
 };
 
-enum KernelMode { kModeLoss = 0, kModeOut = 1 };
+// kModeDistill: the loss kernel of a distillation step (KernelParams::k_teacher > 0), its own instantiation
+enum KernelMode { kModeLoss = 0, kModeOut = 1, kModeDistill = 2 };
+
+// Pipeline depth of the distillation loss kernel: 4 stages of 32 KiB leave room for the 64 KiB of teacher
+// probabilities (fp32, 128 x 128 per CTA) next to the sigma staging buffers.
+constexpr int kDistillStages = 4;
 
 constexpr int kTileCols = 128;   // columns of a tile (wgmma N); a CTA computes 128 rows of it
 constexpr int kWideTileCols = 256;   // the gradient kernel's wide tiles (out mode, 16-bit operands, no split-K)

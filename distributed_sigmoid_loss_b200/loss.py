@@ -48,14 +48,25 @@ class SigmoidLossEngine:
 
     def __init__(self, batch: int, dim: int, device: torch.device, group=None, cta_group: int = 2,
                  overlap_pull: bool = True, rank_world: Optional[Tuple[int, int]] = None, loopback: bool = False,
-                 batch_per_rank=None, texts_per_rank=None, images_per_rank=None):
+                 batch_per_rank=None, texts_per_rank=None, images_per_rank=None, teacher_dim: int = 0):
         self._L = _capi.lib()
         if not torch.cuda.is_available() or self._L.siglip_device_count() == 0:
             raise RuntimeError("distributed_sigmoid_loss_b200 needs an sm_90 (H100) device; there is no CPU fallback")
         self.batch, self.dim, self.device, self.group = batch, dim, torch.device(device), group
         self.rank, self.world = rank_world if rank_world is not None else _group_rank_world(group)
         h = ctypes.c_void_p()
-        if images_per_rank is not None:
+        self.teacher_dim = int(teacher_dim)
+        if self.teacher_dim and (images_per_rank is not None or texts_per_rank is not None):
+            raise RuntimeError("a distillation engine (teacher_dim > 0) takes no extra texts or images")
+        if self.teacher_dim:
+            # distillation: the teacher width is part of the exported allocation (siglip_ctx_create_distill)
+            bpr = [int(b) for b in batch_per_rank] if batch_per_rank is not None else [batch] * self.world
+            if len(bpr) != self.world or bpr[self.rank] != batch:
+                raise RuntimeError(f"batch_per_rank {bpr} must list one batch per rank and hold {batch} at rank {self.rank}")
+            _capi.check(self._L.siglip_ctx_create_distill(ctypes.byref(h), self.device.index or 0, self.rank, self.world,
+                                                          (ctypes.c_int * self.world)(*bpr), dim, self.teacher_dim))
+            self.batch_per_rank = bpr
+        elif images_per_rank is not None:
             # extra images: rank p holds images_per_rank[p] >= its batch images, the paired ones first, then its extras
             # (siglip_ctx_create_extras); every rank passes the same three lists
             bpr = [int(b) for b in batch_per_rank] if batch_per_rank is not None else [batch] * self.world
@@ -144,6 +155,56 @@ class SigmoidLossEngine:
 
     def debug_set_text_chunk(self, chunk: int, txt: torch.Tensor) -> None:
         _capi.check(self._L.siglip_debug_set_text_chunk(self._h, chunk, txt.data_ptr(), self._stream()))
+
+    def set_teacher(self, timg: torch.Tensor, ttxt: torch.Tensor, t_prime: torch.Tensor, bias: torch.Tensor,
+                    lam: float) -> None:
+        """SIGLIP_OPT_DISTILL: the teacher of the NEXT step. timg / ttxt: [B, teacher_dim] contiguous, 16-byte aligned,
+        both bf16 or both float16 holding 16*x (see teacher_operand); t_prime / bias: 1-element fp32 tensors on the
+        engine's device (t_T = exp(t_prime)); lam in (0, 1]. Only the pointers are recorded: the tensors must stay alive
+        until the step is enqueued."""
+        for x in (timg, ttxt):
+            if x.device != self.device or x.dtype not in (torch.bfloat16, torch.float16) or not x.is_contiguous() or \
+                    tuple(x.shape) != (self.batch, self.teacher_dim):
+                raise RuntimeError(f"teacher operands must be contiguous bf16 (or fp16 x16) [{self.batch}, "
+                                   f"{self.teacher_dim}] tensors on {self.device}, got {tuple(x.shape)} {x.dtype}")
+        if timg.dtype != ttxt.dtype:
+            raise RuntimeError("teacher image and text operands must use the same 16-bit format")
+        for x in (t_prime, bias):
+            if x.dtype != torch.float32 or x.numel() != 1 or x.device != self.device:
+                raise RuntimeError("teacher scalars must be 1-element fp32 tensors on the engine's device")
+        _capi.check(self._L.siglip_set_teacher(self._h, timg.data_ptr(), ttxt.data_ptr(),
+                                               int(timg.dtype == torch.float16), t_prime.data_ptr(), bias.data_ptr(),
+                                               float(lam)))
+
+    def teacher_operand(self, x: torch.Tensor, normalize: bool) -> torch.Tensor:
+        """A teacher embedding [B, teacher_dim] in the kernels' operand format, by the student's rules: bf16 as it is,
+        anything else through the fp32 conversion to float16 holding 16*x; normalize=True L2-normalises it first."""
+        hi = x.dtype != torch.bfloat16
+        if normalize:
+            if x.dtype not in (torch.float32, torch.bfloat16):
+                x = x.float()
+            x = _aligned(x)
+            out = torch.empty(x.shape[0], self.teacher_dim, device=self.device,
+                              dtype=torch.float16 if hi else torch.bfloat16)
+            inv = torch.empty(x.shape[0], device=self.device, dtype=torch.float32)
+            with torch.cuda.device(self.device):
+                _capi.check(self._L.siglip_teacher_normalize_fwd(self._h, x.shape[0], x.data_ptr(),
+                                                                 int(x.dtype == torch.bfloat16), out.data_ptr(),
+                                                                 inv.data_ptr(), int(hi), self._stream()))
+            return out
+        if not hi:
+            return _aligned(x)
+        x = _aligned(x.float())
+        out = torch.empty(x.shape[0], self.teacher_dim, device=self.device, dtype=torch.float16)
+        with torch.cuda.device(self.device):
+            _capi.check(self._L.siglip_teacher_convert_f32(self._h, x.shape[0], x.data_ptr(), out.data_ptr(), 1,
+                                                           self._stream()))
+        return out
+
+    def debug_set_teacher_text_chunk(self, chunk: int, ttxt: torch.Tensor) -> None:
+        """Loopback: the teacher text of chunk `chunk` ([B_c, teacher_dim], the teacher's operand format) as its owner
+        would have published it."""
+        _capi.check(self._L.siglip_debug_set_teacher_text_chunk(self._h, chunk, ttxt.data_ptr(), self._stream()))
 
     def set_sample_ids(self, ids: torch.Tensor) -> None:
         """SIGLIP_OPT_SAMPLE_IDS: this rank's sample ids ([B] int64, contiguous, on the engine's device) for the NEXT
@@ -527,12 +588,14 @@ class _SigmoidLossFn(torch.autograd.Function):
     of the forward by the backward's generation guard does not arm them again (they belong to the first run).
     weights: (image_weights [R] or None, text_weights [T] or None) fp32 (SIGLIP_OPT_SAMPLE_WEIGHTS engines), set before
     every step the engine runs for this call, like the ids.
-    extra_img_ids: [R - B] int64 ids of the extra images (SIGLIP_OPT_EXTRA_IMAGE_IDS engines), set along with ids."""
+    extra_img_ids: [R - B] int64 ids of the extra images (SIGLIP_OPT_EXTRA_IMAGE_IDS engines), set along with ids.
+    teacher: (teacher_image, teacher_text, teacher_t_prime, teacher_bias, lambda) of a distillation step
+    (SIGLIP_OPT_DISTILL engines): constants, no gradient flows to them; set before every step like the ids."""
 
     @staticmethod
     def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool = False, fused: bool = False,
                 ids: Optional[torch.Tensor] = None, metrics=None, extra_ids: Optional[torch.Tensor] = None, weights=None,
-                extra_img_ids: Optional[torch.Tensor] = None):
+                extra_img_ids: Optional[torch.Tensor] = None, teacher=None):
         need_grad = any(ctx.needs_input_grad[:4])
         raw = None
         # bf16 callers: bf16 operands (what autograd would multiply). Anything wider (the reference's own test feeds
@@ -566,7 +629,15 @@ class _SigmoidLossFn(torch.autograd.Function):
             b = b.to(device=img.device, dtype=torch.float32)
         b = b.reshape(1)
         ctx.fused = bool(fused and need_grad)
+        if teacher is not None:
+            timg, ttxt, ttp, tbias, lam = teacher
+            teacher = (engine.teacher_operand(timg.detach(), normalize), engine.teacher_operand(ttxt.detach(), normalize),
+                       ttp.detach().to(device=img.device, dtype=torch.float32).reshape(1),
+                       tbias.detach().to(device=img.device, dtype=torch.float32).reshape(1), lam)
+            engine.set_teacher(*teacher)
         ctx.ids, ctx.extra_ids, ctx.weights, ctx.extra_img_ids = ids, extra_ids, weights, extra_img_ids
+        # the split schedule's backward may have to re-run the forward with the same teacher; the fused one never does
+        ctx.teacher = None if ctx.fused else teacher
         if ids is not None:
             engine.set_sample_ids(ids)
         if extra_ids is not None:
@@ -632,6 +703,8 @@ class _SigmoidLossFn(torch.autograd.Function):
                     eng.set_extra_image_ids(ctx.extra_img_ids)
                 if ctx.weights is not None:
                     eng.set_sample_weights(*ctx.weights)
+                if ctx.teacher is not None:
+                    eng.set_teacher(*ctx.teacher)
                 eng.forward(img_b, txt_b, tp, b, True)
                 ctx.gen = eng.saved_generation
             if ctx.normalize:
@@ -648,14 +721,16 @@ class _SigmoidLossFn(torch.autograd.Function):
                 gt = dtxt.to(tdt) if ctx.needs_input_grad[1] else None
         gp = dtp.reshape(pshape).to(device=pdev, dtype=pdt) if ctx.needs_input_grad[2] else None
         gb = db.reshape(bshape).to(device=bdev, dtype=bdt) if ctx.needs_input_grad[3] else None
-        return gi, gt, gp, gb, None, None, None, None, None, None, None, None
+        return gi, gt, gp, gb, None, None, None, None, None, None, None, None, None
 
 
 class _EngineCache:
     def __init__(self, group=None, cta_group: int = 2, overlap_pull: bool = True, sync_scalar_grads: bool = False,
                  bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
-                 extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0):
+                 extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
+                 distill: Optional[float] = None):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
+        self.distill = distill
         self.extra_images = extra_images
         self.sample_weights = sample_weights
         self.sync_scalar_grads, self.bidir = sync_scalar_grads, bidir
@@ -663,10 +738,10 @@ class _EngineCache:
         self.batch_per_rank = batch_per_rank
         self.hard_negatives = hard_negatives
         self.extra_texts = extra_texts
-        self._engines: Dict[Tuple[int, int, int], SigmoidLossEngine] = {}
+        self._engines: Dict[Tuple[int, int, int, int], SigmoidLossEngine] = {}
 
-    def get(self, batch: int, dim: int, device: torch.device) -> SigmoidLossEngine:
-        key = (device.index if device.index is not None else torch.cuda.current_device(), batch, dim)
+    def get(self, batch: int, dim: int, device: torch.device, teacher_dim: int = 0) -> SigmoidLossEngine:
+        key = (device.index if device.index is not None else torch.cuda.current_device(), batch, dim, teacher_dim)
         eng = self._engines.get(key)
         if eng is None:
             dev = torch.device("cuda", key[0])
@@ -681,7 +756,8 @@ class _EngineCache:
                 # every rank holds the same number K of extra images: R_p = B_p + K
                 ipr = [int(b) + self.extra_images for b in bpr]
             eng = SigmoidLossEngine(batch, dim, dev, self.group, self.cta_group, self.overlap_pull,
-                                    batch_per_rank=self.batch_per_rank, texts_per_rank=tpr, images_per_rank=ipr)
+                                    batch_per_rank=self.batch_per_rank, texts_per_rank=tpr, images_per_rank=ipr,
+                                    teacher_dim=teacher_dim)
             if self.sync_scalar_grads:
                 eng.set_option(_capi.SIGLIP_OPT_SYNC_SCALAR_GRADS, 1)
             if self.bidir:
@@ -694,6 +770,8 @@ class _EngineCache:
                 eng.set_option(_capi.SIGLIP_OPT_EXTRA_IMAGE_IDS, 1)
             if self.sample_weights:
                 eng.set_option(_capi.SIGLIP_OPT_SAMPLE_WEIGHTS, 1)
+            if self.distill is not None:
+                eng.set_option(_capi.SIGLIP_OPT_DISTILL, 1)
             self._engines[key] = eng
         return eng
 
@@ -858,6 +936,56 @@ def _with_negatives(text_embeddings: torch.Tensor, negative_text) -> torch.Tenso
     return text_embeddings if negative_text is None else torch.cat([text_embeddings, negative_text])
 
 
+def _validate_distill(distill, hard_negatives: int, extra_texts: int, extra_images: int) -> Optional[float]:
+    """distill=lambda of a module: None (off) or a float in (0, 1], the weight of the teacher's probabilities in the
+    targets. The extras of hard_negatives / extra_texts / extra_images would need teacher embeddings of their own."""
+    if distill is None:
+        return None
+    if isinstance(distill, bool) or not isinstance(distill, (int, float)) or not 0.0 < float(distill) <= 1.0:
+        raise RuntimeError(f"distill must be a float in (0, 1] (the weight of the teacher's probabilities), got "
+                           f"{distill!r}")
+    for name, k in (("hard_negatives", hard_negatives), ("extra_texts", extra_texts), ("extra_images", extra_images)):
+        if k:
+            raise RuntimeError(f"distill cannot be combined with {name}: its extra embeddings would need teacher "
+                               f"embeddings of their own")
+    return float(distill)
+
+
+def _teacher_of(distill: Optional[float], image_embeddings: torch.Tensor, names, values):
+    """The teacher arguments of a forward: all four required with distill, refused without. teacher_image and
+    teacher_text are floating [B, D_T] tensors (the same shape, D_T may differ from the students' width) and the two
+    scalars 1-element floating tensors, all on the embeddings' device, none requiring grad: the teacher is a constant
+    and a gradient with respect to it is never computed. Returns (timg, ttxt, scale, bias, lambda) with D_T zero-padded
+    to a multiple of 8, or None. Raises before any GPU work."""
+    if distill is None:
+        for n, x in zip(names, values):
+            if x is not None:
+                raise RuntimeError(f"{n} given, but the loss was built without distill=lambda")
+        return None
+    for n, x in zip(names, values):
+        if x is None:
+            raise RuntimeError(f"distill={distill}: forward needs {', '.join(names)}")
+        if not isinstance(x, torch.Tensor) or not x.is_floating_point():
+            raise RuntimeError(f"{n} must be a floating-point tensor, got "
+                               f"{x.dtype if isinstance(x, torch.Tensor) else type(x).__name__}")
+        if x.requires_grad:
+            raise RuntimeError(f"{n} requires grad, but the teacher is frozen and no gradient flows to it: pass "
+                               f"{n}.detach()")
+        if x.device != image_embeddings.device:
+            raise RuntimeError(f"{n} is on {x.device}, the embeddings on {image_embeddings.device}")
+    timg, ttxt, tscale, tbias = values
+    rows = image_embeddings.shape[0] if image_embeddings.dim() >= 1 else None
+    for n, x in zip(names[:2], (timg, ttxt)):
+        if x.dim() != 2 or x.shape[0] != rows or x.shape[1] < 1:
+            raise RuntimeError(f"{n} must have shape [{rows}, teacher_dim], got {tuple(x.shape)}")
+    if timg.shape != ttxt.shape:
+        raise RuntimeError(f"{names[0]} {tuple(timg.shape)} and {names[1]} {tuple(ttxt.shape)} must have the same shape")
+    for n, x in zip(names[2:], (tscale, tbias)):
+        if x.numel() != 1:
+            raise RuntimeError(f"{n} must be a 0-dim (1-element) tensor, got shape {tuple(x.shape)}")
+    return (_pad_dim(timg), _pad_dim(ttxt), tscale, tbias, distill)
+
+
 def _validate_return_metrics(return_metrics) -> None:
     if not isinstance(return_metrics, bool):
         raise RuntimeError(f"return_metrics must be a bool, got {type(return_metrics).__name__}")
@@ -964,17 +1092,30 @@ class DDPSigmoidLoss(nn.Module):
     an extra is a t2i miss unless that image carries the text's id; with ids ``i2t_index`` is ``[B + K]`` and covers the
     extras (an extra whose id matches no text is always an i2t miss). Composes with ``hard_negatives`` /
     ``extra_texts``. Collective: every rank uses the same K.
+
+    ``distill=lambda`` in (0, 1]: distillation from a frozen teacher. Every ``forward`` also takes ``teacher_image`` and
+    ``teacher_text`` ([B, D_T], D_T may differ from D) and the teacher's ``teacher_t_prime`` / ``teacher_bias`` (0-dim
+    device tensors, the module's own convention). The target of pair (i, j) becomes
+    ``q = (1 − λ) y + λ σ(exp(t'_T) <timg_i, ttxt_j> + b_T)`` with y the hard label, and the loss
+    ``(1/B) Σ w (softplus(z) − q z)``; λ = 1 is pure distillation. The teacher similarities are computed inside the loss
+    kernel, tile by tile, and never stored; the teacher texts travel with the student texts. Teacher tensors follow the
+    student's input rules (bf16 as is, fp32 through the fp16 conversion, ``normalize_inputs`` normalises them too) and
+    must not require grad. Composes with ``multi_positive``, ``sample_weights``, ``return_metrics`` (the metrics rank the
+    student's logits), ``batch_per_rank``, ``sync_scalar_grads`` and both schedules; not with ``hard_negatives``,
+    ``extra_texts`` or ``extra_images``. Collective: every rank uses the same λ and D_T.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
                  normalize_inputs: bool = False, sync_scalar_grads: bool = False, fused_step: Optional[bool] = None,
                  batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
-                 extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0) -> None:
+                 extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
+                 distill: Optional[float] = None) -> None:
         super().__init__()
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_images = _validate_hard_negatives(extra_images, "extra_images")
         extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
         sample_weights = _validate_sample_weights(sample_weights)
+        distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images)
         self.t_prime = nn.Parameter(torch.tensor(math.log(10), dtype=torch.float64))
         self.bias = nn.Parameter(torch.tensor(-10.0))
         self.gpu_batch_size = gpu_batch_size
@@ -998,20 +1139,32 @@ class DDPSigmoidLoss(nn.Module):
         self.sample_weights = sample_weights
         # extension: extra images per rank (hard-negative images, or with ids several images per caption)
         self.extra_images = extra_images
+        # extension: distillation from a frozen teacher (soft targets from the teacher's embeddings)
+        self.distill = distill
         self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank,
                                    multi_positive=multi_positive, hard_negatives=hard_negatives,
-                                   extra_texts=extra_texts, sample_weights=sample_weights, extra_images=extra_images)
+                                   extra_texts=extra_texts, sample_weights=sample_weights, extra_images=extra_images,
+                                   distill=distill)
 
-    def engine_for(self, batch: int, dim: int, device: torch.device) -> SigmoidLossEngine:
-        return self._cache.get(batch, (dim + 7) // 8 * 8, device)
+    def engine_for(self, batch: int, dim: int, device: torch.device, teacher_dim: int = 0) -> SigmoidLossEngine:
+        """The engine forward() uses for these shapes. A module built with distill=lambda needs the teacher's width
+        (teacher_dim, padded to a multiple of 8 like dim)."""
+        if (self.distill is not None) != (teacher_dim > 0):
+            raise RuntimeError("engine_for: pass teacher_dim > 0 exactly when the loss was built with distill=lambda")
+        return self._cache.get(batch, (dim + 7) // 8 * 8, device, (teacher_dim + 7) // 8 * 8)
 
     def forward(self, image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, *,
                 negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
                 return_metrics: bool = False, extra_text: Optional[torch.Tensor] = None,
                 extra_text_ids: Optional[torch.Tensor] = None, image_weights: Optional[torch.Tensor] = None,
                 text_weights: Optional[torch.Tensor] = None, extra_image: Optional[torch.Tensor] = None,
-                extra_image_ids: Optional[torch.Tensor] = None):
+                extra_image_ids: Optional[torch.Tensor] = None, teacher_image: Optional[torch.Tensor] = None,
+                teacher_text: Optional[torch.Tensor] = None, teacher_t_prime: Optional[torch.Tensor] = None,
+                teacher_bias: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
+        teacher = _teacher_of(self.distill, image_embeddings,
+                              ("teacher_image", "teacher_text", "teacher_t_prime", "teacher_bias"),
+                              (teacher_image, teacher_text, teacher_t_prime, teacher_bias))
         ids = _validate_ids(sample_ids, self.multi_positive, image_embeddings)
         _validate_negatives(text_embeddings, negative_text, self.hard_negatives)
         _validate_negatives(text_embeddings, extra_text, self.extra_texts, "extra_text", "extra_texts")
@@ -1024,11 +1177,12 @@ class DDPSigmoidLoss(nn.Module):
         text_embeddings = _with_negatives(_with_negatives(text_embeddings, negative_text), extra_text)
         image_embeddings = _with_negatives(image_embeddings, extra_image)
         image_embeddings, text_embeddings = _pad_dim(image_embeddings), _pad_dim(text_embeddings)
-        eng = self._cache.get(self.gpu_batch_size, image_embeddings.shape[1], image_embeddings.device)
+        eng = self._cache.get(self.gpu_batch_size, image_embeddings.shape[1], image_embeddings.device,
+                              teacher[0].shape[1] if teacher is not None else 0)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
         loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
-                                    self.normalize_inputs, fused, ids, bufs, extra_ids, weights, ximg_ids)
+                                    self.normalize_inputs, fused, ids, bufs, extra_ids, weights, ximg_ids, teacher)
         return (loss, _metric_dict(bufs)) if return_metrics else loss
 
 
@@ -1049,18 +1203,22 @@ class SigLipLoss(nn.Module):
     ``sample_weights=True``: every forward takes ``image_weights`` [B] and ``text_weights`` [B + K] (or None for ones),
     per-sample loss weights in [0, 1] as in ``DDPSigmoidLoss``. ``extra_images=K``: every forward takes ``extra_image``
     [K, D] (and with ``multi_positive`` ``extra_image_ids`` [K]), hard-negative images or further images of a caption as
-    in ``DDPSigmoidLoss``; ``image_weights`` then has B + K entries."""
+    in ``DDPSigmoidLoss``; ``image_weights`` then has B + K entries. ``distill=lambda``: every forward takes
+    ``teacher_image`` / ``teacher_text`` [B, D_T] and ``teacher_logit_scale`` / ``teacher_logit_bias`` (0-dim, the
+    convention of ``logit_scale`` / ``logit_bias``), distillation from a frozen teacher as in ``DDPSigmoidLoss``."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
                  multi_positive: bool = False, hard_negatives: int = 0, extra_texts: int = 0,
-                 sample_weights: bool = False, extra_images: int = 0):
+                 sample_weights: bool = False, extra_images: int = 0, distill: Optional[float] = None):
         super().__init__()
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_images = _validate_hard_negatives(extra_images, "extra_images")
         extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
         sample_weights = _validate_sample_weights(sample_weights)
+        distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images)
+        self.distill = distill
         self.cache_labels, self.rank, self.world_size, self.bidir = cache_labels, rank, world_size, bidir
         self.use_horovod = use_horovod
         self.fused_step = fused_step
@@ -1071,15 +1229,20 @@ class SigLipLoss(nn.Module):
         self.extra_images = extra_images
         self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive,
                                    hard_negatives=hard_negatives, extra_texts=extra_texts, sample_weights=sample_weights,
-                                   extra_images=extra_images)
+                                   extra_images=extra_images, distill=distill)
 
     def forward(self, image_features, text_features, logit_scale, logit_bias, output_dict: bool = False, *,
                 negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
                 return_metrics: bool = False, extra_text: Optional[torch.Tensor] = None,
                 extra_text_ids: Optional[torch.Tensor] = None, image_weights: Optional[torch.Tensor] = None,
                 text_weights: Optional[torch.Tensor] = None, extra_image: Optional[torch.Tensor] = None,
-                extra_image_ids: Optional[torch.Tensor] = None):
+                extra_image_ids: Optional[torch.Tensor] = None, teacher_image: Optional[torch.Tensor] = None,
+                teacher_text: Optional[torch.Tensor] = None, teacher_logit_scale: Optional[torch.Tensor] = None,
+                teacher_logit_bias: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
+        teacher = _teacher_of(self.distill, image_features,
+                              ("teacher_image", "teacher_text", "teacher_logit_scale", "teacher_logit_bias"),
+                              (teacher_image, teacher_text, teacher_logit_scale, teacher_logit_bias))
         ids = _validate_ids(sample_ids, self.multi_positive, image_features)
         _validate_negatives(text_features, negative_text, self.hard_negatives)
         _validate_negatives(text_features, extra_text, self.extra_texts, "extra_text", "extra_texts")
@@ -1093,7 +1256,8 @@ class SigLipLoss(nn.Module):
         text_features = _with_negatives(_with_negatives(text_features, negative_text), extra_text)
         image_features = _with_negatives(image_features, extra_image)
         image_features, text_features = _pad_dim(image_features), _pad_dim(text_features)
-        eng = self._cache.get(batch, image_features.shape[1], image_features.device)
+        eng = self._cache.get(batch, image_features.shape[1], image_features.device,
+                              teacher[0].shape[1] if teacher is not None else 0)
         if (eng.rank, eng.world) != (self.rank, self.world_size):
             raise RuntimeError(
                 f"SigLipLoss(rank={self.rank}, world_size={self.world_size}) does not match the process group "
@@ -1103,6 +1267,6 @@ class SigLipLoss(nn.Module):
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
         loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs,
-                                    extra_ids, weights, ximg_ids)
+                                    extra_ids, weights, ximg_ids, teacher)
         out = {"contrastive_loss": loss} if output_dict else loss
         return (out, _metric_dict(bufs)) if return_metrics else out

@@ -137,6 +137,17 @@ enum {
                                       hard-negative image. Without this option an extra image matches no id. The loss
                                       still divides by B_r. Needs SIGLIP_OPT_SAMPLE_IDS on (else SIGLIP_ERR_STATE);
                                       turning that option off clears this one. Collective: set on all ranks. Default 0 */
+  SIGLIP_OPT_DISTILL = 25, /* 1: distillation from a frozen teacher (siglip_ctx_create_distill contexts only, else
+                              SIGLIP_ERR_STATE). The target of pair (i, j) becomes
+                                q_ij = (1 - lambda) y_ij + lambda sigma(t_T <timg_i, ttxt_j> + b_T)
+                              (y in {0, 1}: the labels the other options give) and rank r's loss
+                                (1/B_r) sum_ij w_ij (softplus(z_ij) - q_ij z_ij).
+                              The teacher similarities are computed tile by tile inside the loss kernel and never
+                              stored; the teacher texts travel with the student texts. Every step needs
+                              siglip_set_teacher since the previous step (else SIGLIP_ERR_STATE before any launch).
+                              Composes with SIGLIP_OPT_SAMPLE_IDS, SIGLIP_OPT_SAMPLE_WEIGHTS, metrics, bidir and
+                              uneven batches; unavailable with hard negatives / extra texts / extra images and in the
+                              host-buffer entries. The gradient kernels are unchanged. Collective. Default 0 */
   SIGLIP_OPT_AUX_TRACE = 18 /* 1: record globaltimer stamps of the auxiliary warps of CTA 0 for every launch (start,
                                last peer flag seen, jobs done, end of launch); read with siglip_ctx_aux_trace */
 };
@@ -205,6 +216,26 @@ int siglip_ctx_create_texts(siglip_ctx** out, int device, int rank, int world, c
  */
 int siglip_ctx_create_extras(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank,
                              const int* images_per_rank, const int* texts_per_rank, int D);
+
+/*
+ * Same as siglip_ctx_create_uneven, for distillation (SIGLIP_OPT_DISTILL): D_teacher is the width of the teacher's
+ * embeddings (a positive multiple of 8; it may differ from D). The gathered teacher text ([world][max B, D_teacher]
+ * bf16 or fp16 x 16) is part of the exported text allocation, sized here because options are set after the handle
+ * exchange; every rank passes the same list and D_teacher (handle import refuses a peer whose D_teacher differs).
+ * D_teacher = 0 is exactly siglip_ctx_create_uneven.
+ */
+int siglip_ctx_create_distill(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank, int D,
+                              int D_teacher);
+
+/*
+ * SIGLIP_OPT_DISTILL: the teacher of the NEXT step. timg [B, D_teacher] and ttxt [B, D_teacher] are this rank's teacher
+ * embeddings, both bf16 (teacher_f16 = 0) or both fp16(x * 16) (teacher_f16 = 1, the fp32-input format), 16-byte
+ * aligned; t_prime_T / bias_T are fp32 device scalars (t_T = exp(t_prime_T)); lambda in (0, 1]. Only the pointers are
+ * recorded (like siglip_request_metrics): the buffers must hold their values when the step runs on its stream, and a
+ * single-rank step stays capturable into a CUDA graph. No gradient flows to the teacher.
+ */
+int siglip_set_teacher(siglip_ctx* ctx, const void* timg, const void* ttxt, int teacher_f16, const float* t_prime_T,
+                       const float* bias_T, float lambda);
 
 int siglip_ctx_set_option(siglip_ctx* ctx, int option, int value);
 
@@ -427,6 +458,17 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
  */
 int siglip_debug_loopback(siglip_ctx* ctx);
 int siglip_debug_set_text_chunk(siglip_ctx* ctx, int chunk, const void* txt_dev, void* cuda_stream);
+
+/* The teacher twin of siglip_debug_set_text_chunk (SIGLIP_OPT_DISTILL): the teacher text of chunk `chunk`
+ * ([batch of that rank, D_teacher] in the teacher's format) as its owner would have published it. */
+int siglip_debug_set_teacher_text_chunk(siglip_ctx* ctx, int chunk, const void* ttxt_dev, void* cuda_stream);
+
+/* The teacher's operand formats (width D_teacher): siglip_convert_f32_rows and siglip_normalize_fwd_rows over `rows`
+ * rows of teacher embeddings, with the format given by f16 (1: fp16(16 x), 0: bf16). Forward only. */
+int siglip_teacher_convert_f32(siglip_ctx* ctx, int rows, const float* x_f32, void* out_16bit, int f16,
+                               void* cuda_stream);
+int siglip_teacher_normalize_fwd(siglip_ctx* ctx, int rows, const void* x, int in_bf16, void* xhat, float* inv_norm,
+                                 int f16, void* cuda_stream);
 int siglip_debug_get_slot(siglip_ctx* ctx, int chunk, float* out_dev, void* cuda_stream);
 /* The ids twin of siglip_debug_set_text_chunk (SIGLIP_OPT_SAMPLE_IDS): the sample ids of text chunk `chunk`
  * ([batch of that rank] int64 device buffer: its paired texts only; [T of that rank] under SIGLIP_OPT_EXTRA_TEXT_IDS:

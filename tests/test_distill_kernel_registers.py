@@ -1,0 +1,31 @@
+"""The three distillation loss kernels of the built library (siglip_gemm_kernel<kModeDistill = 2, 4 stages, cluster
+1 / 2 / 4>) use 167 registers per thread and spill nothing to local memory (DESIGN.md, "Distillation from a teacher")."""
+import os
+import re
+import shutil
+import subprocess
+
+import pytest
+
+from distributed_sigmoid_loss_b200 import _capi
+
+
+def test_distill_kernels_use_167_registers_and_no_spills():
+    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    if not os.path.exists(exe) or not os.path.exists(_capi.LIB_PATH):
+        pytest.skip("needs cuobjdump and the built library")
+    out = subprocess.run([exe, "-res-usage", _capi.LIB_PATH], check=True, capture_output=True, text=True).stdout
+    usage, name = {}, None
+    for line in out.splitlines():
+        m = re.search(r"Function (\S+):", line)
+        if m:
+            name = m.group(1)
+            continue
+        if name is not None and "REG:" in line:
+            usage[name] = line
+            name = None
+    distill = {n: u for n, u in usage.items() if re.search(r"siglip_gemm_kernelILi2ELi4ELi[124]E", n)}
+    assert len(distill) == 3, sorted(distill)
+    for n, u in distill.items():
+        assert re.search(r"\bREG:167\b", u), (n, u)
+        assert re.search(r"\bLOCAL:0\b", u), (n, u)

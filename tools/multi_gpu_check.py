@@ -58,6 +58,10 @@ def main() -> int:
                     help="also check per-sample loss weights against the float64 oracle: random weights with zeros on "
                          "every rank, the text weights travelling with the text, uneven batches, with and without sample "
                          "ids and hard negatives, fused and split")
+    ap.add_argument("--distill", action="store_true",
+                    help="also check distillation from a frozen teacher against the float64 oracle: the teacher text "
+                         "travelling with the student text through the peer pulls, a teacher width different from the "
+                         "student's, uneven batches, with and without sample ids and weights, fused and split")
     ap.add_argument("--soak", type=int, default=0,
                     help="N > 0: that many back-to-back steps at the --batch/--dim shape mixing the fused step, the split "
                          "API and forward-only calls; same inputs, so every step of a kind must reproduce its first result "
@@ -496,6 +500,53 @@ def main() -> int:
                     l2.backward()
                     torch.cuda.synchronize()
                     report(f"weights {fused} B={Bs} K={K} ids={with_ids} D={D} rep{rep}", dict(
+                        loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
+                        dimg=rel_f(a.grad.float().cpu(), torch.from_numpy(mine["dimg"])),
+                        dtxt=rel_f(b.grad.float().cpu(), dtxt_ref),
+                        dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
+                        db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
+
+    # ---- distillation: each rank's teacher text travels with its text through the peer pulls ----------------------
+    if args.distill:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from distill_oracle import closed_form_distill
+        from sample_weights_oracle import label_blocks
+        Bs = [160 + 24 * r for r in range(world)]
+        D, DT, tp, bias, ttp, tbias, lam = 136, 72, math.log(10.0), -8.0, math.log(20.0), -6.0, 0.7
+        g = torch.Generator().manual_seed(5555)
+        unit = lambda n, d: torch.nn.functional.normalize(torch.randn(n, d, generator=g)).to(torch.bfloat16)  # noqa: E731
+        for with_ids, with_w in ((False, False), (True, True)):
+            imgs, texts = [unit(b, D) for b in Bs], [unit(b, D) for b in Bs]
+            timgs, ttexts = [unit(b, DT) for b in Bs], [unit(b, DT) for b in Bs]
+            ids = list(torch.split(torch.randint(0, 200, (sum(Bs),), generator=g), Bs)) if with_ids else None
+            iws = [torch.rand(b, generator=g) for b in Bs] if with_w else None
+            tws = [torch.rand(b, generator=g) for b in Bs] if with_w else None
+            f = lambda xs: None if xs is None else [x.double().numpy() for x in xs]  # noqa: E731
+            ref = closed_form_distill(f(imgs), f(texts), tp, bias, f(timgs), f(ttexts), ttp, tbias, lam, f(iws), f(tws),
+                                      label_blocks(Bs, Bs, f(ids)))
+            mine = ref[rank]
+            dtxt_ref = torch.from_numpy(sum(ref[r]["contrib"][rank] for r in range(world)))
+            img, txt = imgs[rank].to(dev), texts[rank].to(dev)
+            for fused in (None, False):
+                modx = DDPSigmoidLoss(Bs[rank], fused_step=fused, batch_per_rank=Bs, multi_positive=with_ids,
+                                      sample_weights=with_w, distill=lam).to(dev)
+                with torch.no_grad():
+                    modx.t_prime.fill_(tp)
+                    modx.bias.fill_(bias)
+                for rep in range(2):
+                    modx.zero_grad()
+                    # fp32 student inputs (fp16 operands, fp32 gradients), bf16 teacher: two operand formats in one step
+                    a, b = (x.float().requires_grad_(True) for x in (img, txt))
+                    kw = dict(teacher_image=timgs[rank].to(dev), teacher_text=ttexts[rank].to(dev),
+                              teacher_t_prime=torch.tensor(ttp, device=dev), teacher_bias=torch.tensor(tbias, device=dev))
+                    if with_ids:
+                        kw["sample_ids"] = ids[rank].to(dev)
+                    if with_w:
+                        kw.update(image_weights=iws[rank].to(dev), text_weights=tws[rank].to(dev))
+                    l2 = modx(a, b, **kw)
+                    l2.backward()
+                    torch.cuda.synchronize()
+                    report(f"distill {fused} B={Bs} D={D} D_T={DT} ids={with_ids} weights={with_w} rep{rep}", dict(
                         loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
                         dimg=rel_f(a.grad.float().cpu(), torch.from_numpy(mine["dimg"])),
                         dtxt=rel_f(b.grad.float().cpu(), dtxt_ref),
