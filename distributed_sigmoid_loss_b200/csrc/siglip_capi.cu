@@ -130,7 +130,8 @@ constexpr int kMaxWorld = 32;
 //   0 text of forward #n is in place        1 dtxt contribution of backward #n, gradient slot j is complete
 //   2 forward #n finished pulling everyone's text     3 backward #n finished reading everyone's contributions
 //   4 (dt', dbias) of backward #n are in the owner's mailbox (SIGLIP_OPT_SYNC_SCALAR_GRADS)
-//   5 the retrieval-metric partials of forward #n are in place (siglip_request_metrics)
+//   5 the retrieval-metric and per-sample-loss partials of forward #n are in place (siglip_request_metrics,
+//     siglip_request_sample_losses)
 constexpr int kFlagKinds = 6;
 // the mailbox (2 floats) lives behind the flag counters, in the same peer-mapped allocation
 constexpr int kMailboxOffset = kFlagKinds * kMaxWorld;
@@ -236,6 +237,11 @@ struct siglip_ctx {
   int64_t* m_i2t = nullptr;
   int64_t* m_t2i = nullptr;
   unsigned long long* mkeys_step = nullptr;  // key block of the step being issued (null: no metrics this step)
+  // per-sample losses (siglip_request_sample_losses), armed for the next step only
+  bool losses_armed = false;
+  float* l_img = nullptr;                // [R] image_loss output
+  float* l_txt = nullptr;                // [T] text_loss output
+  unsigned long long* lsum_step = nullptr;  // fixed-point block of the step being issued (null: no per-sample losses)
   // diagnostics, read from the environment once at context creation (see include/siglip_b200.h)
   bool dbg_no_gstore = false, dbg_no_cvt = false, dbg_loss_waitstats = false;
   // workspaces
@@ -249,6 +255,9 @@ struct siglip_ctx {
   unsigned long long* mkeys[2] = {};     // per step parity: [world][Tmax] column argmax partials of every text chunk
                                          // over my images, then [Rmax] row keys, then [Emax] my extra-image ids (world > 1
                                          // under SIGLIP_OPT_EXTRA_IMAGE_IDS). world > 1: behind ids_all (exported)
+  unsigned long long* lsum[2] = {};      // per step parity: [world][Tmax] column sums of every text chunk over my images,
+                                         // [Rmax] row sums, then the same layout again for the poison bits
+                                         // (lsum_block). world > 1: behind the gathered teacher text (exported)
   float* w_all = nullptr;                // [world][w_stride] text weights of every chunk (world > 1): behind the metric
                                          // keys in the exported allocation, sized at creation whatever the options
   float* w_in = nullptr;                 // [w_stride] my text weights, then [R] my image weights, clamped into [0, 1];
@@ -269,6 +278,7 @@ struct siglip_ctx {
   float* loop_mailboxes = nullptr;       // loopback only: [world][2] stand-ins for the peers' (dt', dbias) mailboxes
   float* loop_zero = nullptr;            // loopback only: [world][Tmax, D] zeros standing in for the peers' contribution slots
   unsigned long long* loop_keys = nullptr;  // loopback only: [world][Tmax] the peers' column partials of my chunk
+  unsigned long long* loop_lsums = nullptr;  // loopback only: [world] blocks standing in for the peers' loss partials
   int64_t* loop_xids = nullptr;          // loopback only: [world][Emax] the peers' published extra-image ids
   float* scalars = nullptr;              // [24] device scalars: host API staging, saved dt'/dbias of the last forward
   unsigned long long* aux_trace = nullptr;  // [kTraceLaunches][16] globaltimer stamps (SIGLIP_OPT_AUX_TRACE)
@@ -287,6 +297,7 @@ struct siglip_ctx {
   unsigned int** signal_ptrs_dev = nullptr;  // [kFlagKinds][world]
   const float** mailbox_ptrs_dev = nullptr;  // [world] every rank's (dt', dbias) mailbox
   const unsigned long long** mkey_ptrs_dev = nullptr;  // [2][world] every rank's column partial of my chunk, per parity
+  const unsigned long long** lsum_ptrs_dev = nullptr;  // [2][world] every rank's loss column partial of my chunk
   const int64_t** xid_ptrs_dev = nullptr;    // [2][world] every rank's published extra-image ids, per parity
   unsigned int n_fwd = 0, n_bwd = 0;         // forward / backward passes issued (flag counters)
   unsigned int prewait3 = 0;                 // highest n for which "peers finished backward n" has been waited for
@@ -364,6 +375,8 @@ inline size_t chunk_ids_bytes(const siglip_ctx* c, int rank) {
 // ids and weights of step s are given once: a step in ids / weights mode consumes them (all checked before anything is
 // launched or consumed)
 int take_ids(siglip_ctx* c) {
+  if (c->losses_armed && c->distill)
+    return fail(SIGLIP_ERR_STATE, "per-sample losses are unavailable under SIGLIP_OPT_DISTILL");
   if (c->sample_ids && !c->ids_set)
     return fail(SIGLIP_ERR_STATE,
                 "SIGLIP_OPT_SAMPLE_IDS is on but siglip_set_sample_ids was not called since the previous step");
@@ -450,6 +463,63 @@ inline const void* teacher_chunk(const siglip_ctx* c, int cidx) {
   return (cidx == c->rank) ? c->t_txt : static_cast<const void*>(c->ttxt_all + cidx * teacher_stride(c));
 }
 
+// ---- per-sample losses (siglip_request_sample_losses) ----
+// 64-bit words from a fixed-point sum to its poison word: [world][Tmax] column sums (the loss kernel writes one per text
+// of every chunk), then [Rmax] row sums
+inline size_t lsum_half(const siglip_ctx* c) { return static_cast<size_t>(c->world) * c->Tmax + c->Rmax; }
+// words per step parity: the sums, then the poison words in the same layout
+inline size_t lsum_block(const siglip_ctx* c) { return 2 * lsum_half(c); }
+inline size_t lsum_rows(const siglip_ctx* c) { return static_cast<size_t>(c->world) * c->Tmax; }
+// byte offset of the two blocks in the exported text allocation: behind the gathered teacher text (which is empty
+// without a teacher), so that no earlier offset moves
+inline size_t lsum_offset(const siglip_ctx* c) {
+  return teacher_offset(c) + teacher_stride(c) * c->world * sizeof(__nv_bfloat16);
+}
+
+// A step with per-sample losses starts: the block of the step's parity is zeroed by one memset. The block is written
+// by the step's loss kernels and read by the peers after flag kind 5 of the step, like the metric keys, and
+// double-buffered by parity for the same reason (DESIGN.md, "Per-sample losses").
+int take_sample_losses(siglip_ctx* c, unsigned int s, cudaStream_t st) {
+  c->lsum_step = nullptr;
+  if (!c->losses_armed) return 0;
+  c->losses_armed = false;
+  c->lsum_step = c->lsum[s & 1u];
+  CK(cudaMemsetAsync(c->lsum_step, 0, lsum_block(c) * sizeof(unsigned long long), st));
+  c->launches++;
+  return 0;
+}
+// After the step's last loss kernel (and the metrics finalisation, if armed): combine the column sums of my chunk
+// (W > 1: with every rank's, after flag kind 5, which this kernel raises unless the metrics finalisation did) and
+// decode both sides into the caller's buffers.
+int finalize_sample_losses(siglip_ctx* c, unsigned int s, bool signal, cudaStream_t st) {
+  if (c->lsum_step == nullptr) return 0;
+  const int W = c->world;
+  siglip::SampleLossArgs a;
+  memset(&a, 0, sizeof(a));
+  a.rows = c->lsum_step + lsum_rows(c);
+  a.col_own = c->lsum_step + static_cast<size_t>(c->rank) * c->Tmax;
+  a.poison = static_cast<long long>(lsum_half(c));
+  a.R = c->R;
+  a.T = c->T;
+  a.rank = c->rank;
+  a.world = W;
+  a.signal = signal ? 1 : 0;
+  a.image_loss = c->l_img;
+  a.text_loss = c->l_txt;
+  if (W > 1) {
+    a.col_peers = c->lsum_ptrs_dev + static_cast<size_t>(s & 1u) * W;
+    a.sig_ptrs = c->signal_ptrs_dev + 5 * W;
+    a.flags_local = c->flags + 5 * kMaxWorld;
+    a.value = s;
+    a.timeout_ns = peer_timeout_ns(c);
+  }
+  a.dbg = c->dbg_dev;
+  c->lsum_step = nullptr;
+  CKI(siglip::launch_sample_loss_finalize(a, st));
+  c->launches++;
+  return 0;
+}
+
 // A metrics step starts (armed by siglip_request_metrics for this step only): the key block of the step's parity is
 // zeroed, so that no max of an earlier step survives. Double-buffered by parity: a peer may still read my partials of
 // step n in its finalisation while my step n + 1 writes; by step n + 2 that read is over (DESIGN.md, "In-batch
@@ -512,6 +582,15 @@ int finalize_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
   CKI(siglip::launch_metrics_finalize(a, st));
   c->launches++;
   return 0;
+}
+
+// The step's detached outputs, after its last loss kernel: the metrics, then the per-sample losses (which raise flag
+// kind 5 themselves when no metrics finalisation did)
+int finalize_step_outputs(siglip_ctx* c, unsigned int s, cudaStream_t st) {
+  const bool metrics = c->mkeys_step != nullptr;
+  int rc;
+  if ((rc = finalize_metrics(c, s, st))) return rc;
+  return finalize_sample_losses(c, s, !metrics, st);
 }
 
 // Sigma operand + fp16 text copy number i, allocated on first use. The fused step needs two (own chunk, chunk in
@@ -674,6 +753,11 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
     p.col_keys = c->mkeys_step + static_cast<size_t>(cidx) * c->Tmax;
     p.row_off = c->off[c->rank];
     p.col_off = c->toff[cidx];
+  }
+  if (c->lsum_step != nullptr) {   // a per-sample-loss step: the kModeSampleLoss kernel adds the row / column sums
+    p.sl_rows = c->lsum_step + lsum_rows(c);
+    p.sl_cols = c->lsum_step + static_cast<size_t>(cidx) * c->Tmax;
+    p.sl_poison = static_cast<long long>(lsum_half(c));
   }
   p.partials = c->partials;
   p.accumulate_partials = first ? 0 : 1;  // the first chunk of a forward overwrites every slot of the grid
@@ -1011,6 +1095,7 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
   const size_t stride = chunk_stride(c);
   const unsigned int s = ++c->n_fwd;
   if ((rc = take_metrics(c, s, st))) return rc;
+  if ((rc = take_sample_losses(c, s, st))) return rc;
   // the saved state is being overwritten (a forward without save still replaces my gathered text slot, which the
   // backward of a multi-rank job reads for the positive-pair term); valid again once a saving forward is enqueued
   if (save || c->world > 1) c->gen = 0;
@@ -1063,7 +1148,7 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
   if (W > 1) {
     if ((rc = signal_peers(c, 2, s, st))) return rc;
   }
-  if ((rc = finalize_metrics(c, s, st))) return rc;
+  if ((rc = finalize_step_outputs(c, s, st))) return rc;
   CK(cudaGetLastError());
   if (save) {
     c->saved_f16 = c->input_f16;
@@ -1190,6 +1275,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   const unsigned int base = (n - 1) * static_cast<unsigned int>(W);
   const bool ik = c->inkernel_sync != 0;
   if ((rc = take_metrics(c, s, st))) return rc;
+  if ((rc = take_sample_losses(c, s, st))) return rc;
   c->gen = 0;                       // the sigma operands of a split forward (if any) are overwritten
   c->saved_f16 = c->input_f16;
   if ((rc = ensure_g(c, 0))) return rc;
@@ -1338,7 +1424,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
     if ((rc = run_grad_chunk(c, 0, true, img, own_txt, c->T, t_prime, grad_out, o, aux, end, st))) return rc;
     if (W > 1 && !ik && (rc = signal_peers(c, 3, n, st))) return rc;
   }
-  if ((rc = finalize_metrics(c, s, st))) return rc;
+  if ((rc = finalize_step_outputs(c, s, st))) return rc;
   if (W > 1 && c->sync_scalar_grads) {
     CKI(siglip::launch_allreduce_scalars(c->scalars + kSavedScalars, grad_out,
                                          reinterpret_cast<float*>(c->flags + kMailboxOffset), c->mailbox_ptrs_dev,
@@ -1491,14 +1577,18 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     const size_t w_bytes = static_cast<size_t>(world) * c->w_stride * sizeof(float);
     // a distillation context also gathers the teacher text there (nothing without a teacher)
     const size_t t_bytes = teacher_stride(c) * world * sizeof(__nv_bfloat16);
-    CK(alloc(reinterpret_cast<void**>(&c->txt_all),
-             stride * world * sizeof(__nv_bfloat16) + world * ids_slot_bytes + mkeys_bytes + w_bytes + t_bytes));
+    // and the per-sample-loss partials behind that (sized whatever the options: a peer's offsets cannot depend on them)
+    const size_t l_bytes = 2 * lsum_block(c) * sizeof(unsigned long long);
+    CK(alloc(reinterpret_cast<void**>(&c->txt_all), stride * world * sizeof(__nv_bfloat16) + world * ids_slot_bytes +
+                                                        mkeys_bytes + w_bytes + t_bytes + l_bytes));
     c->ids_all = reinterpret_cast<int64_t*>(c->txt_all + stride * world);   // 16-byte aligned: D % 8 == 0
     c->mkeys[0] = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(c->txt_all) + mkeys_offset(c));
     c->mkeys[1] = c->mkeys[0] + mkeys_block(c);
     c->w_all = reinterpret_cast<float*>(reinterpret_cast<char*>(c->txt_all) + weights_offset(c));
     if (DT > 0)
       c->ttxt_all = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<char*>(c->txt_all) + teacher_offset(c));
+    c->lsum[0] = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(c->txt_all) + lsum_offset(c));
+    c->lsum[1] = c->lsum[0] + lsum_block(c);
     CK(alloc(reinterpret_cast<void**>(&c->slots), stride * world * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dimg_acc), static_cast<size_t>(c->R) * D * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dtxt_acc), static_cast<size_t>(c->T) * D * sizeof(float)));
@@ -1507,6 +1597,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     CK(alloc(reinterpret_cast<void**>(&c->signal_ptrs_dev), kFlagKinds * world * sizeof(unsigned int*)));
     CK(alloc(reinterpret_cast<void**>(&c->mailbox_ptrs_dev), world * sizeof(float*)));
     CK(alloc(reinterpret_cast<void**>(&c->mkey_ptrs_dev), 2 * world * sizeof(unsigned long long*)));
+    CK(alloc(reinterpret_cast<void**>(&c->lsum_ptrs_dev), 2 * world * sizeof(unsigned long long*)));
     if (c->ximg) CK(alloc(reinterpret_cast<void**>(&c->xid_ptrs_dev), 2 * world * sizeof(int64_t*)));
     const float* fin[2] = {c->dtxt_acc, c->slots + rank * stride};
     CK(cudaMemcpy(c->final_ptrs_dev, fin, sizeof(fin), cudaMemcpyHostToDevice));
@@ -1750,6 +1841,18 @@ static int publish_peer_tables(siglip_ctx* c) {
       if (c->loopback && p != c->rank) mk[q * c->world + p] = c->loop_keys + static_cast<size_t>(p) * c->Tmax;
     }
   CK(cudaMemcpy(c->mkey_ptrs_dev, mk.data(), mk.size() * sizeof(unsigned long long*), cudaMemcpyHostToDevice));
+  // every rank's loss column partial of my chunk, per step parity (loopback: the stand-ins
+  // siglip_debug_set_peer_sample_loss_partials seeds, with their poison words at the same distance)
+  std::vector<const unsigned long long*> ls(2 * c->world);
+  for (int q = 0; q < 2; ++q)
+    for (int p = 0; p < c->world; ++p) {
+      const unsigned long long* blk =
+          reinterpret_cast<const unsigned long long*>(reinterpret_cast<const char*>(c->peer_txt[p]) + lsum_offset(c)) +
+          q * lsum_block(c);
+      if (c->loopback && p != c->rank) blk = c->loop_lsums + static_cast<size_t>(p) * lsum_block(c);
+      ls[q * c->world + p] = blk + static_cast<size_t>(c->rank) * c->Tmax;
+    }
+  CK(cudaMemcpy(c->lsum_ptrs_dev, ls.data(), ls.size() * sizeof(unsigned long long*), cudaMemcpyHostToDevice));
   if (c->xid_ptrs_dev != nullptr) {
     // every rank's published extra-image ids, per step parity (loopback: the stand-ins
     // siglip_debug_set_peer_extra_image_ids seeds)
@@ -1924,6 +2027,45 @@ int siglip_request_metrics(siglip_ctx* c, float* top1, int64_t* i2t_index, int64
   return 0;
 }
 
+int siglip_request_sample_losses(siglip_ctx* c, float* image_loss, float* text_loss) {
+  if (c == nullptr || image_loss == nullptr || text_loss == nullptr)
+    return fail(SIGLIP_ERR_INVALID, "null argument (image_loss and text_loss are required)");
+  if (c->distill)
+    return fail(SIGLIP_ERR_STATE, "per-sample losses are unavailable under SIGLIP_OPT_DISTILL");
+  if (c->lsum[0] == nullptr) {
+    // one rank: the blocks are allocated on the first request, as the metric keys are (and apart from them), so a
+    // context that never asks holds exactly the workspace it held without them; allowed inside a CUDA-graph capture
+    const size_t bytes = 2 * lsum_block(c) * sizeof(unsigned long long);
+    CK(cudaSetDevice(c->device));
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    CK(cudaThreadExchangeStreamCaptureMode(&mode));
+    unsigned long long* words = nullptr;
+    const cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&words), bytes);
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    CK(e);
+    c->lsum[0] = words;
+    c->lsum[1] = words + lsum_block(c);
+    c->workspace_bytes += bytes;
+  }
+  c->l_img = image_loss;
+  c->l_txt = text_loss;
+  c->losses_armed = true;
+  return 0;
+}
+
+int siglip_debug_set_peer_sample_loss_partials(siglip_ctx* c, int peer, const int64_t* partials_dev,
+                                               void* cuda_stream) {
+  if (c == nullptr || partials_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->loopback || peer < 0 || peer >= c->world || peer == c->rank)
+    return fail(SIGLIP_ERR_INVALID,
+                "siglip_debug_set_peer_sample_loss_partials needs a loopback context and a peer rank != own rank");
+  CK(cudaSetDevice(c->device));
+  CK(cudaMemcpyAsync(c->loop_lsums + static_cast<size_t>(peer) * lsum_block(c) + static_cast<size_t>(c->rank) * c->Tmax,
+                     partials_dev, static_cast<size_t>(c->T) * sizeof(int64_t), cudaMemcpyDeviceToDevice,
+                     static_cast<cudaStream_t>(cuda_stream)));
+  return 0;
+}
+
 int siglip_debug_set_peer_metric_keys(siglip_ctx* c, int peer, const uint64_t* keys_dev, void* cuda_stream) {
   if (c == nullptr || keys_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (!c->loopback || peer < 0 || peer >= c->world || peer == c->rank)
@@ -2038,6 +2180,9 @@ int siglip_host_submit_grads(siglip_ctx* c, const void* img_host, const void* tx
                 "(siglip_ctx_create_extras with images_per_rank != batch_per_rank)");
   if (c->metrics_armed)
     return fail(SIGLIP_ERR_STATE, "the host-buffer entries return no retrieval metrics: siglip_request_metrics is armed");
+  if (c->losses_armed)
+    return fail(SIGLIP_ERR_STATE,
+                "the host-buffer entries return no per-sample losses: siglip_request_sample_losses is armed");
   if (c->sample_weights)
     return fail(SIGLIP_ERR_STATE,
                 "the host-buffer entries take no sample weights: unavailable under SIGLIP_OPT_SAMPLE_WEIGHTS");
@@ -2185,6 +2330,8 @@ int siglip_debug_loopback(siglip_ctx* c) {
     CK(cudaMemset(c->loop_mailboxes, 0, 2 * kMaxWorld * sizeof(float)));
     CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_keys), static_cast<size_t>(c->world) * c->Tmax * 8));
     CK(cudaMemset(c->loop_keys, 0, static_cast<size_t>(c->world) * c->Tmax * 8));
+    CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_lsums), static_cast<size_t>(c->world) * lsum_block(c) * 8));
+    CK(cudaMemset(c->loop_lsums, 0, static_cast<size_t>(c->world) * lsum_block(c) * 8));
     if (c->Emax > 0) {
       CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_xids), static_cast<size_t>(c->world) * c->Emax * 8));
       CK(cudaMemset(c->loop_xids, 0, static_cast<size_t>(c->world) * c->Emax * 8));
@@ -2539,6 +2686,9 @@ void free_ctx(siglip_ctx* c) {
   cudaFree(c->loop_keys);
   if (c->world == 1) cudaFree(c->mkeys[0]);   // world > 1: part of txt_all
   cudaFree(c->mkey_ptrs_dev);
+  cudaFree(c->loop_lsums);
+  if (c->world == 1) cudaFree(c->lsum[0]);    // world > 1: part of txt_all
+  cudaFree(c->lsum_ptrs_dev);
   cudaFree(c->scalars);
   cudaFree(c->aux_trace);
   cudaFree(c->splitk_ws);

@@ -285,11 +285,13 @@ __device__ __forceinline__ float slab_w(int i, const float* cw, float rw0, float
 // is bound by the MUFU and FMA pipes.
 // kW (SIGLIP_OPT_SAMPLE_WEIGHTS): element i has weight slab_w(i, cw, rw0, rw1); it scales e where e multiplies into both
 // terms, so a weight of exactly 1 leaves every value bit-identical to the unweighted path.
-template <bool kW = false>
+// kL (per-sample losses, kModeSampleLoss): element i's term w softplus(z), computed next to the fmaf chain of the sum
+// (which it leaves untouched), is added to lrow[row half] and lcol[2 j + e1] (the thread's 2 rows and 8 columns).
+template <bool kW = false, bool kL = false>
 __device__ __forceinline__ void loss_slab_fast(const float* v, float tl, float bl, int col0, bool store_g,
                                                const GStore& gst, float gscale, float& acc_sp, float& acc_g,
                                                float& acc_gs, const float* cw = nullptr, float rw0 = 1.f,
-                                               float rw1 = 1.f) {
+                                               float rw1 = 1.f, float* lrow = nullptr, float* lcol = nullptr) {
   uint32_t packed[8];
   float a_sp = 0.f, a_g = 0.f, a_gs = 0.f;
   float g_prev = 0.f;
@@ -307,6 +309,11 @@ __device__ __forceinline__ void loss_slab_fast(const float* v, float tl, float b
     float l = fmaf(e, 0.33333334f, -0.5f);               // log1p(e) / e = 1 - e/2 + e^2/3    [- e^3/4 < 1e-6 dropped]
     l = fmaf(e, l, 1.0f);
     a_sp = fmaf(ew, l, a_sp);
+    if constexpr (kL) {
+      const float term = ew * l;
+      lrow[(i >> 1) & 1] += term;
+      lcol[2 * (i >> 2) + (i & 1)] += term;
+    }
     a_g += g;
     a_gs = fmaf(g, s, a_gs);
     // element i = 4 j + e': row half e' >> 1, column e' & 1 -> packed[2 j + (e' >> 1)]
@@ -325,11 +332,13 @@ __device__ __forceinline__ void loss_slab_fast(const float* v, float tl, float b
 // General path. row_lo: global row of this thread's first fragment row; col0: global column of the slab; c_lo as above.
 // pos (kMask only): bit i set = element i is a positive pair by sample id (SIGLIP_OPT_SAMPLE_IDS); 0 without ids.
 // kW: element i's weight multiplies its three terms once its label is applied (x * 1 == x: unit weights change no bit).
-template <bool kMask, bool kW = false>
+// kL: element i's term (sp once masked and weighted) is also added to lrow / lcol as in loss_slab_fast.
+template <bool kMask, bool kW = false, bool kL = false>
 __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int row_lo, int col0, int c_lo, int nrows,
                                           int ncols, bool store_g, const GStore& gst, float gscale, float* g_diag,
                                           bool on_diag, uint32_t pos, float& acc_sp, float& acc_g, float& acc_gs,
-                                          const float* cw = nullptr, float rw0 = 1.f, float rw1 = 1.f) {
+                                          const float* cw = nullptr, float rw0 = 1.f, float rw1 = 1.f,
+                                          float* lrow = nullptr, float* lcol = nullptr) {
   uint32_t packed[8];
   float g_prev = 0.f;
 #pragma unroll
@@ -374,6 +383,10 @@ __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int 
       g_store *= w;
     }
     acc_sp += sp;
+    if constexpr (kL) {
+      lrow[(i >> 1) & 1] += sp;
+      lcol[2 * (i >> 2) + (i & 1)] += sp;
+    }
     acc_g += g;
     acc_gs = fmaf(g, s, acc_gs);
     if (i & 1)
@@ -810,6 +823,145 @@ __device__ __forceinline__ void distill_epilogue(const KernelParams& p, const fl
 }
 
 // -------------------------------------------------------------------------------------------------
+// Per-sample losses (kModeSampleLoss): row and column sums of the terms w_ij softplus(-y_ij z_ij) the loss adds up, from
+// the same per-element values (loss_slab_fast / loss_slab with kL). Every partial is rounded once to a 64-bit
+// fixed-point word (value * 2^32) and added with red.add.u64: integer addition is associative, so the sums depend only
+// on the 128 x 128 tile and 16-row slab geometry, never on the order of the atomics, the cluster shape or the schedule.
+// Every term is >= 0 (softplus, weights in [0, 1]). A partial that is not below kSampleLossMaxPartial (too large, +inf
+// or NaN) is never added as a number: it ORs a poison bit into the word sl_poison words behind, which the finalisation
+// decodes into +inf (1) or NaN (2).
+// -------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void red_add_u64(unsigned long long* p, unsigned long long v) {
+  asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+
+__device__ __forceinline__ void red_or_b64(unsigned long long* p, unsigned long long v) {
+  asm volatile("red.relaxed.gpu.global.or.b64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+
+// v * 2^32 is exact in fp32 and below 2^48, so the conversion to an integer does not round
+__device__ __forceinline__ void sample_loss_add(unsigned long long* w, long long poison, float v) {
+  if (v < kSampleLossMaxPartial) {   // false for NaN and +inf
+    const unsigned long long q = __float2ull_rn(v * 4294967296.0f);
+    if (q != 0ull) red_add_u64(w, q);
+  } else {
+    red_or_b64(w + poison, (v != v) ? 2ull : 1ull);
+  }
+}
+
+// The loss epilogue of kModeSampleLoss. The three sums, g_diag and the stored sigma operand are those of the kModeLoss
+// epilogue bit for bit: the same slab functions and path choices, with unit weights when the step has none (x * 1 == x)
+// and the ids and metric keys as runtime options. On top:
+//   rows:    each thread sums its two fragment rows over the tile's 4 slabs, the quad adds its 4 threads (shfl_xor 1, 2),
+//            one red.add per row and tile;
+//   columns: per slab, the thread's 2 rows of each of its 8 columns, then a reduce-scatter over the warp's 8 row groups
+//            (lanes xor 16, 8, 4, as in tile_metrics) that leaves lane l with column q = l >> 2 of its lane % 4 group,
+//            one red.add per lane and slab.
+// Rows >= M and columns >= N add nothing (their terms are masked to 0 and their words do not exist).
+__device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, const float (&acc)[kTileN / 2],
+                                                     const CUtensorMap* tmG, uint32_t staging_base, int warp, int wg,
+                                                     int lane, int row0, int col_base, int row_lo, int c_lo,
+                                                     const Problem& pr, float t_eff, float bias, float tl, float bl,
+                                                     uint64_t policy, float& s_sp, float& c_sp, float& s_g, float& c_g,
+                                                     float& s_gs, float& c_gs) {
+  if (p.row_keys != nullptr) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
+  float acc_sp = 0.f, acc_g = 0.f, acc_gs = 0.f;
+  const bool edge = (row0 + kBlockM > pr.M) || (col_base + kTileN > pr.N);
+  const bool diag = p.own_chunk && (row0 == col_base);
+  const bool sg = p.store_g != 0;
+  GStore gst;
+  gst.tmap = tmG;
+  gst.stage = staging_base + static_cast<uint32_t>(warp) * kStagingBytesPerWarp;
+  gst.row0 = row0 + wg * 64 + (warp & 3) * 16;
+  gst.lane = lane;
+  gst.policy = policy;
+  const bool ids = p.row_ids != nullptr, w = p.row_w != nullptr;
+  int64_t rid0 = 0, rid1 = 0;
+  uint32_t rpos = 0u;
+  if (ids) {
+    rid0 = p.row_ids[min(row_lo, pr.M - 1)];
+    rid1 = p.row_ids[min(row_lo + 8, pr.M - 1)];
+    rpos = (row_lo < p.row_pos_n ? 0x3333u : 0u) | (row_lo + 8 < p.row_pos_n ? 0xCCCCu : 0u);
+  }
+  float rw0 = 1.f, rw1 = 1.f;
+  if (w) {
+    rw0 = p.row_w[min(row_lo, pr.M - 1)];
+    rw1 = p.row_w[min(row_lo + 8, pr.M - 1)];
+  }
+  float lrow[2] = {0.f, 0.f};
+#pragma unroll
+  for (int c = 0; c < kTileN / 32; ++c) {
+    const float* v = acc + 16 * c;
+    const int col0 = col_base + 32 * c;
+    float cw[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) cw[j] = w ? p.col_w[min(col0 + 8 * (j >> 1) + c_lo + (j & 1), pr.N - 1)] : 1.f;
+    const bool slab_diag = diag && (gst.row0 < col0 + 32) && (col0 < gst.row0 + 16);
+    const bool slab_edge = edge && ((gst.row0 + 16 > pr.M) || (col0 + 32 > pr.N));
+    uint32_t pos = 0;
+    bool slab_pos = false;
+    if (ids) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int e1 = 0; e1 < 2; ++e1) {
+          const int col = col0 + 8 * j + c_lo + e1;
+          if (col < p.col_pos_n) {
+            const int64_t cid = p.col_ids[col];
+            pos |= static_cast<uint32_t>(cid == rid0) << (4 * j + e1);
+            pos |= static_cast<uint32_t>(cid == rid1) << (4 * j + 2 + e1);
+          }
+        }
+      }
+      pos &= rpos;
+      slab_pos = __any_sync(0xffffffffu, pos != 0u);
+    }
+    float lcol[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (!slab_edge && !slab_diag && !slab_pos) {
+      float smax = v[0];
+#pragma unroll
+      for (int j = 1; j < 16; ++j) smax = fmaxf(smax, v[j]);
+      const bool fast = __all_sync(0xffffffffu, fmaf(smax, t_eff, bias) < kFastZ);
+      if (fast)
+        loss_slab_fast<true, true>(v, tl, bl, col0, sg, gst, p.g_scale, acc_sp, acc_g, acc_gs, cw, rw0, rw1, lrow,
+                                   lcol);
+      else
+        loss_slab<false, true, true>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag,
+                                     false, 0u, acc_sp, acc_g, acc_gs, cw, rw0, rw1, lrow, lcol);
+    } else {
+      loss_slab<true, true, true>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag,
+                                  slab_diag, pos, acc_sp, acc_g, acc_gs, cw, rw0, rw1, lrow, lcol);
+    }
+    // reduce-scatter: after the step over lane bit m, lcol[0 .. h) holds the columns q = k + (bit m of lane ? h : 0)
+#pragma unroll
+    for (int h = 4, m = 16; h >= 1; h >>= 1, m >>= 1) {
+      const bool hi = (lane & m) != 0;
+#pragma unroll
+      for (int k = 0; k < h; ++k) {
+        const float send = hi ? lcol[k] : lcol[k + h];
+        const float keep = hi ? lcol[k + h] : lcol[k];
+        lcol[k] = keep + __shfl_xor_sync(0xffffffffu, send, m);
+      }
+    }
+    const int q = lane >> 2;
+    const int col = col0 + 8 * (q >> 1) + c_lo + (q & 1);
+    if (col < pr.N) sample_loss_add(p.sl_cols + col, p.sl_poison, lcol[0]);
+  }
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1) {
+    lrow[0] += __shfl_xor_sync(0xffffffffu, lrow[0], o);
+    lrow[1] += __shfl_xor_sync(0xffffffffu, lrow[1], o);
+  }
+  if ((lane & 3) == 0) {
+    if (row_lo < pr.M) sample_loss_add(p.sl_rows + row_lo, p.sl_poison, lrow[0]);
+    if (row_lo + 8 < pr.M) sample_loss_add(p.sl_rows + row_lo + 8, p.sl_poison, lrow[1]);
+  }
+  kahan_add(s_sp, c_sp, acc_sp);
+  kahan_add(s_g, c_g, acc_g);
+  kahan_add(s_gs, c_gs, acc_gs);
+}
+
+// -------------------------------------------------------------------------------------------------
 // The kernel
 // -------------------------------------------------------------------------------------------------
 // kF8: the out kernel of the 8-bit measurement path (its own instantiation: the extra fp32 result registers of
@@ -824,6 +976,9 @@ __device__ __forceinline__ void distill_epilogue(const KernelParams& p, const fl
 // kMode = kModeDistill: the loss kernel of a distillation step, its own instantiation (kDistillStages, 128-column
 // tiles): the teacher's k-blocks of every tile first (tmA1 / tmB1), its probabilities in shared memory, then the
 // student's k-loop and the soft-target epilogue (distill_epilogue); ids, weights and metrics are runtime options there.
+// kMode = kModeSampleLoss: the loss kernel of a step with per-sample losses, its own instantiation (both stage counts,
+// 128-column tiles, K-major operands): the kModeLoss epilogue plus the fixed-point row / column sums
+// (sample_loss_epilogue); ids, weights and metrics are runtime options there.
 template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false,
           bool kWeights = false, int kTileNT = kTileN>
 __global__ void __launch_bounds__(kNumThreads, 1)
@@ -839,6 +994,8 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
                 "256-column tiles: out kernel, 16-bit operands");
   static_assert(kMode != kModeDistill || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
                 "the distillation kernel takes ids, weights and metrics as runtime options");
+  static_assert(kMode != kModeSampleLoss || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
+                "the per-sample-loss kernel takes ids, weights and metrics as runtime options");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -1086,7 +1243,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
   mma_loop<T, TA, TB, kCS, C::kStageBytes, kTileNT>(acc, kb0, kb1, stage, phase, C::kStages, adesc0, bdesc0, a_adv, \
                                                     b_adv, full0, empty0, lane, p.dbg, t, w_full_p)
         const int sel = pr.a_mn * 2 + pr.b_mn;
-        if constexpr (kMode == kModeDistill) {
+        if constexpr (kMode == kModeDistill || kMode == kModeSampleLoss) {
           // the loss operands (student and teacher) are always K-major: no MN-major variants in this instantiation
           if (pr.ab_f16)
             SIGLIP_MMA_LOOP(1, 0, 0);
@@ -1120,6 +1277,9 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       if constexpr (kMode == kModeDistill) {
         distill_epilogue(p, acc, pbuf, &tmG, staging_base, warp, wg, lane, row0, col_base, row_lo, c_lo, pr, t_eff, bias,
                          tl, bl, g_store_policy, s_sp, c_sp, s_g, c_g, s_gs, c_gs);
+      } else if constexpr (kMode == kModeSampleLoss) {
+        sample_loss_epilogue(p, acc, &tmG, staging_base, warp, wg, lane, row0, col_base, row_lo, c_lo, pr, t_eff, bias,
+                             tl, bl, g_store_policy, s_sp, c_sp, s_g, c_g, s_gs, c_gs);
       } else if constexpr (kMode == kModeLoss) {
         // argmax keys first, on the raw accumulator: whichever path each slab then takes below
         if constexpr (kMetrics) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
@@ -1797,6 +1957,67 @@ __global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const
   if (tid < 2) a.top1[tid] = static_cast<float>(hits[tid]) / static_cast<float>(tid == 0 ? ni : nt);
 }
 
+// Finalisation of the per-sample losses (SampleLossArgs). Like metrics_finalize_kernel it never triggers
+// griddepcontrol.launch_dependents, and at W > 1 it reads the peers' partials of the step only after their flag kind 5
+// of the step: the same words at the same points of the step as the metric keys (DESIGN.md, "Per-sample losses").
+constexpr int kSampleLossThreads = 1024;
+
+__device__ __forceinline__ float sample_loss_decode(unsigned long long sum, unsigned long long poison) {
+  if (poison & 2ull) return __int_as_float(0x7fffffff);
+  if (poison & 1ull) return INFINITY;
+  return static_cast<float>(static_cast<double>(sum) * (1.0 / kSampleLossScale));
+}
+
+__global__ void __launch_bounds__(kSampleLossThreads) sample_loss_finalize_kernel(const SampleLossArgs a) {
+  const int tid = threadIdx.x;
+  if (a.world > 1) {
+    if (tid < a.world) {
+      if (a.signal) {
+        __threadfence_system();   // my partials (written by the step's loss kernels) before the flag
+        asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(a.sig_ptrs[tid]), "r"(a.value) : "memory");
+      }
+      uint64_t t0 = 0;
+      uint32_t spins = 0;
+      while (true) {
+        unsigned int v;
+        asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(a.flags_local + tid) : "memory");
+        if (v >= a.value) break;
+        if ((++spins & 0xffu) == 0) {
+          const uint64_t now = globaltimer_ns();
+          if (t0 == 0) t0 = now;
+          if (now - t0 > a.timeout_ns) {
+            if (a.dbg != nullptr) {
+              a.dbg->block = tid;
+              a.dbg->aux0 = v;
+              a.dbg->aux1 = a.value;
+              a.dbg->code = 10;
+              __threadfence_system();
+            }
+            __trap();
+          }
+        }
+      }
+      __threadfence();   // order the other threads' peer reads after the observed flags
+    }
+    __syncthreads();
+  }
+  for (int i = tid; i < a.R; i += kSampleLossThreads) a.image_loss[i] = sample_loss_decode(a.rows[i], a.rows[i + a.poison]);
+  for (int i = tid; i < a.T; i += kSampleLossThreads) {
+    unsigned long long sum = a.col_own[i], poison = a.col_own[i + a.poison];
+    if (a.world > 1) {
+      for (int q = 0; q < a.world; ++q) {   // integer sums: the rank order is only for definiteness
+        if (q == a.rank) continue;
+        unsigned long long v, b;
+        asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(a.col_peers[q] + i) : "memory");
+        asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(b) : "l"(a.col_peers[q] + i + a.poison) : "memory");
+        sum += v;
+        poison |= b;
+      }
+    }
+    a.text_loss[i] = sample_loss_decode(sum, poison);
+  }
+}
+
 // -------------------------------------------------------------------------------------------------
 // L2 normalisation fused around the loss (SURVEY.md §8f-1: the step the reference's callers run right before it,
 // test_distributed_sigmoid_loss.py:99-101). One warp per row; HBM-bound: coalesced 16-byte accesses, fp32 math.
@@ -2104,6 +2325,20 @@ int launch_gemm(int cta_group, int mode, int stages, int mcast, int tile_n, cons
       default: return launch_impl<kModeDistill, kDistillStages, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
     }
   }
+  if (mode == kModeLoss && p.sl_rows != nullptr) {   // per-sample losses: kModeSampleLoss, 4 or 6 stages
+    const bool s4 = stages == 4;
+    switch (cluster_size(cta_group, mcast)) {
+      case 4:
+        return s4 ? launch_impl<kModeSampleLoss, 4, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeSampleLoss, 6, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      case 2:
+        return s4 ? launch_impl<kModeSampleLoss, 4, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeSampleLoss, 6, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      default:
+        return s4 ? launch_impl<kModeSampleLoss, 4, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeSampleLoss, 6, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+    }
+  }
   switch (cluster_size(cta_group, mcast)) {
     case 4:
       if (mode == kModeLoss) SIGLIP_LAUNCH_STAGES(kModeLoss, 4);
@@ -2190,6 +2425,11 @@ int launch_clamp_weights(const float* src_a, float* dst_a, int na, const float* 
 
 int launch_metrics_finalize(const MetricsArgs& a, cudaStream_t stream) {
   metrics_finalize_kernel<<<1, kMetricsThreads, 0, stream>>>(a);
+  return static_cast<int>(cudaGetLastError());
+}
+
+int launch_sample_loss_finalize(const SampleLossArgs& a, cudaStream_t stream) {
+  sample_loss_finalize_kernel<<<1, kSampleLossThreads, 0, stream>>>(a);
   return static_cast<int>(cudaGetLastError());
 }
 

@@ -160,10 +160,26 @@ struct KernelParams {
   const float* t_prime_T;     // fp32 device scalars: t_T = exp(t'_T), b_T
   const float* bias_T;
   float distill_lambda;       // in (0, 1]
+  // Per-sample losses (siglip_request_sample_losses). Appended last like the fields above. Non-null sl_rows selects the
+  // kModeSampleLoss loss kernel: besides the three sums it adds every tile's row sums and every 16-row slab's column
+  // sums of the terms w_ij softplus(-y_ij z_ij) into 64-bit fixed-point words (value * 2^32, red.add.u64), so that the
+  // result does not depend on the order of the atomics. A partial that is not finite or >= kSampleLossMaxPartial ORs a
+  // poison bit (1: too large or +inf, 2: NaN) into the word sl_poison words behind its sum instead.
+  unsigned long long* sl_rows;   // [M]: sums of this rank's images over the chunk's texts
+  unsigned long long* sl_cols;   // [N]: sums of the chunk's texts over this rank's images
+  long long sl_poison;           // distance in words from a sum to its poison word
 };
 
 // kModeDistill: the loss kernel of a distillation step (KernelParams::k_teacher > 0), its own instantiation
-enum KernelMode { kModeLoss = 0, kModeOut = 1, kModeDistill = 2 };
+// kModeSampleLoss: the loss kernel of a step with per-sample losses (KernelParams::sl_rows != null), its own
+// instantiation; ids, weights and metric keys are runtime options in it
+enum KernelMode { kModeLoss = 0, kModeOut = 1, kModeDistill = 2, kModeSampleLoss = 3 };
+
+// Per-sample losses: fixed-point scale of the 64-bit sums, and the largest partial (one tile's row sum over 128
+// columns, or one 16-row slab's column sum) that is added as a number. 2^16 * 2^32 per partial keeps the unsigned sum
+// of up to 2^16 partials per sample (a global batch of up to 2^20 images and 2^23 texts) inside 64 bits.
+constexpr double kSampleLossScale = 4294967296.0;        // 2^32
+constexpr float kSampleLossMaxPartial = 65536.0f;        // 2^16
 
 // Pipeline depth of the distillation loss kernel: 4 stages of 32 KiB leave room for the 64 KiB of teacher
 // probabilities (fp32, 128 x 128 per CTA) next to the sigma staging buffers.
@@ -258,6 +274,27 @@ struct MetricsArgs {
   DebugRecord* dbg;
 };
 int launch_metrics_finalize(const MetricsArgs& a, cudaStream_t stream);
+
+// Finalisation of a per-sample-loss step (one block, after the step's last loss kernel, and after the metrics
+// finalisation when both are armed). W > 1: unless the metrics finalisation already did, publish flag kind 5 to every
+// rank; then wait for every rank's flag kind 5 of the step and add the W ranks' fixed-point partials of my chunk in rank
+// order (relaxed system-scope loads). Decode rows into image_loss [R] and columns into text_loss [T].
+struct SampleLossArgs {
+  const unsigned long long* rows;              // [R] local row sums (poison words sl_poison words behind)
+  const unsigned long long* col_own;           // [T] my partial of my chunk
+  const unsigned long long* const* col_peers;  // [world] every rank's partial of my chunk (world > 1; own entry unused)
+  long long poison;                            // distance in words from a sum to its poison word (same on every rank)
+  int R, T, rank, world;
+  int signal;                                  // 1: raise flag kind 5 here (no metrics finalisation in this step)
+  float* image_loss;
+  float* text_loss;
+  unsigned int* const* sig_ptrs;               // [world] flag kind 5 of every rank (world > 1)
+  const volatile unsigned int* flags_local;    // my flag kind 5 row
+  unsigned int value;
+  unsigned long long timeout_ns;
+  DebugRecord* dbg;
+};
+int launch_sample_loss_finalize(const SampleLossArgs& a, cudaStream_t stream);
 int launch_wait_flags(const volatile unsigned int* flags, int n, unsigned int value, unsigned long long timeout_ns,
                       DebugRecord* dbg, cudaStream_t stream);
 

@@ -295,6 +295,28 @@ class SigmoidLossEngine:
             raise RuntimeError(f"peer metric keys must be a contiguous int64 [{n}] tensor on {self.device}")
         _capi.check(self._L.siglip_debug_set_peer_metric_keys(self._h, peer, keys.data_ptr(), self._stream()))
 
+    def request_sample_losses(self, image_loss: torch.Tensor, text_loss: torch.Tensor) -> None:
+        """Arm the per-sample losses of the NEXT step (siglip_request_sample_losses): image_loss fp32 [R] (the paired
+        images, then the extra images) and text_loss fp32 [T] (the paired texts, then the extras), contiguous on the
+        engine's device. image_loss[i] is the sum of w_ij softplus(-y_ij z_ij) over every text of the global batch,
+        text_loss[j] the same sum over every image of the global batch (no 1/B). Nothing is read on the host; the step
+        writes them on its stream. Refused under distillation."""
+        for name, x, n in (("image_loss", image_loss, self.images), ("text_loss", text_loss, self.texts)):
+            if not isinstance(x, torch.Tensor) or x.dtype != torch.float32 or tuple(x.shape) != (n,) or \
+                    not x.is_contiguous() or x.device != self.device:
+                raise RuntimeError(f"{name} must be a contiguous fp32 [{n}] tensor on {self.device}")
+        _capi.check(self._L.siglip_request_sample_losses(self._h, image_loss.data_ptr(), text_loss.data_ptr()))
+
+    def debug_set_peer_sample_loss_partials(self, peer: int, partials: torch.Tensor) -> None:
+        """Loopback: the per-sample-loss column partials ([T] int64 fixed-point words, value * 2^32) standing in for peer
+        `peer`'s partial of this rank's text chunk."""
+        n = self.texts
+        if partials.dtype != torch.int64 or tuple(partials.shape) != (n,) or not partials.is_contiguous() or \
+                partials.device != self.device:
+            raise RuntimeError(f"peer sample-loss partials must be a contiguous int64 [{n}] tensor on {self.device}")
+        _capi.check(self._L.siglip_debug_set_peer_sample_loss_partials(self._h, peer, partials.data_ptr(),
+                                                                       self._stream()))
+
     @property
     def metric_images(self) -> int:
         """Images of this rank that i2t ranks: the paired ones, or all R under SIGLIP_OPT_EXTRA_IMAGE_IDS."""
@@ -590,12 +612,14 @@ class _SigmoidLossFn(torch.autograd.Function):
     every step the engine runs for this call, like the ids.
     extra_img_ids: [R - B] int64 ids of the extra images (SIGLIP_OPT_EXTRA_IMAGE_IDS engines), set along with ids.
     teacher: (teacher_image, teacher_text, teacher_t_prime, teacher_bias, lambda) of a distillation step
-    (SIGLIP_OPT_DISTILL engines): constants, no gradient flows to them; set before every step like the ids."""
+    (SIGLIP_OPT_DISTILL engines): constants, no gradient flows to them; set before every step like the ids.
+    sample_losses: (image_loss [R], text_loss [T]) fp32 output buffers: the per-sample losses of this call's step are
+    armed. Like the metrics, a re-run of the forward by the backward's generation guard does not arm them again."""
 
     @staticmethod
     def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool = False, fused: bool = False,
                 ids: Optional[torch.Tensor] = None, metrics=None, extra_ids: Optional[torch.Tensor] = None, weights=None,
-                extra_img_ids: Optional[torch.Tensor] = None, teacher=None):
+                extra_img_ids: Optional[torch.Tensor] = None, teacher=None, sample_losses=None):
         need_grad = any(ctx.needs_input_grad[:4])
         raw = None
         # bf16 callers: bf16 operands (what autograd would multiply). Anything wider (the reference's own test feeds
@@ -648,6 +672,8 @@ class _SigmoidLossFn(torch.autograd.Function):
             engine.set_sample_weights(*weights)
         if metrics is not None:
             engine.request_metrics(*metrics)
+        if sample_losses is not None:
+            engine.request_sample_losses(*sample_losses)
         if ctx.fused:
             # gradients in the dtype autograd would return for these inputs (fp32 when a projection follows)
             gdt = torch.bfloat16 if (not hi and not normalize) else torch.float32
@@ -721,7 +747,7 @@ class _SigmoidLossFn(torch.autograd.Function):
                 gt = dtxt.to(tdt) if ctx.needs_input_grad[1] else None
         gp = dtp.reshape(pshape).to(device=pdev, dtype=pdt) if ctx.needs_input_grad[2] else None
         gb = db.reshape(bshape).to(device=bdev, dtype=bdt) if ctx.needs_input_grad[3] else None
-        return gi, gt, gp, gb, None, None, None, None, None, None, None, None, None
+        return gi, gt, gp, gb, None, None, None, None, None, None, None, None, None, None
 
 
 class _EngineCache:
@@ -999,6 +1025,29 @@ def _metric_buffers(batch: int, device: torch.device, texts: Optional[int] = Non
             torch.empty(batch if texts is None else texts, device=device, dtype=torch.int64))
 
 
+def _validate_return_sample_losses(return_sample_losses, distill) -> None:
+    if not isinstance(return_sample_losses, bool):
+        raise RuntimeError(f"return_sample_losses must be a bool, got {type(return_sample_losses).__name__}")
+    if return_sample_losses and distill is not None:
+        raise RuntimeError("return_sample_losses is unavailable with distill: the distillation loss kernel does not "
+                           "compute per-sample losses")
+
+
+def _sample_loss_buffers(eng) -> Tuple[torch.Tensor, torch.Tensor]:
+    return (torch.empty(eng.images, device=eng.device, dtype=torch.float32),
+            torch.empty(eng.texts, device=eng.device, dtype=torch.float32))
+
+
+def _with_outputs(out, metric_bufs, loss_bufs):
+    """(out), (out, metrics), (out, sample_losses) or (out, metrics, sample_losses), as the caller asked."""
+    extra = []
+    if metric_bufs is not None:
+        extra.append(_metric_dict(metric_bufs))
+    if loss_bufs is not None:
+        extra.append({"image_loss": loss_bufs[0], "text_loss": loss_bufs[1]})
+    return (out, *extra) if extra else out
+
+
 def _metric_dict(bufs) -> Dict[str, torch.Tensor]:
     """The in-batch retrieval metrics of a step, as device tensors (no host synchronisation): top-1 rates of this rank's
     images / texts (0-dim fp32) and the global index of each one's best match (int64 [B])."""
@@ -1103,6 +1152,16 @@ class DDPSigmoidLoss(nn.Module):
     must not require grad. Composes with ``multi_positive``, ``sample_weights``, ``return_metrics`` (the metrics rank the
     student's logits), ``batch_per_rank``, ``sync_scalar_grads`` and both schedules; not with ``hard_negatives``,
     ``extra_texts`` or ``extra_images``. Collective: every rank uses the same λ and D_T.
+
+    ``forward(..., return_sample_losses=True)`` returns ``(loss, sample_losses)``, or ``(loss, metrics, sample_losses)``
+    with ``return_metrics``: ``image_loss`` ([R] fp32, the paired images then the extra images) holds, for each image
+    of this rank, the sum of its pair terms ``w · softplus(−y z)`` over every text of the global batch, and
+    ``text_loss`` ([T] fp32, captions then ``negative_text`` / ``extra_text``) the same sum for each text over every
+    image of the global batch. No 1/B is applied, so ``loss == image_loss.sum() / B`` up to rounding, and a sample of
+    weight 0 reports exactly 0. The loss kernels add them up from the terms they already compute, in 64-bit fixed point,
+    so they are bitwise reproducible; loss, gradients and metrics are unchanged. Device tensors, no host
+    synchronisation, not differentiable; works under ``torch.no_grad()`` (data selection over a super-batch). Not with
+    ``distill``. Collective: every rank asks on the same steps.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
@@ -1160,8 +1219,9 @@ class DDPSigmoidLoss(nn.Module):
                 text_weights: Optional[torch.Tensor] = None, extra_image: Optional[torch.Tensor] = None,
                 extra_image_ids: Optional[torch.Tensor] = None, teacher_image: Optional[torch.Tensor] = None,
                 teacher_text: Optional[torch.Tensor] = None, teacher_t_prime: Optional[torch.Tensor] = None,
-                teacher_bias: Optional[torch.Tensor] = None):
+                teacher_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False):
         _validate_return_metrics(return_metrics)
+        _validate_return_sample_losses(return_sample_losses, self.distill)
         teacher = _teacher_of(self.distill, image_embeddings,
                               ("teacher_image", "teacher_text", "teacher_t_prime", "teacher_bias"),
                               (teacher_image, teacher_text, teacher_t_prime, teacher_bias))
@@ -1181,9 +1241,11 @@ class DDPSigmoidLoss(nn.Module):
                               teacher[0].shape[1] if teacher is not None else 0)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
+        lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
         loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
-                                    self.normalize_inputs, fused, ids, bufs, extra_ids, weights, ximg_ids, teacher)
-        return (loss, _metric_dict(bufs)) if return_metrics else loss
+                                    self.normalize_inputs, fused, ids, bufs, extra_ids, weights, ximg_ids, teacher,
+                                    lbufs)
+        return _with_outputs(loss, bufs, lbufs)
 
 
 SigmoidLoss = DDPSigmoidLoss
@@ -1205,7 +1267,10 @@ class SigLipLoss(nn.Module):
     [K, D] (and with ``multi_positive`` ``extra_image_ids`` [K]), hard-negative images or further images of a caption as
     in ``DDPSigmoidLoss``; ``image_weights`` then has B + K entries. ``distill=lambda``: every forward takes
     ``teacher_image`` / ``teacher_text`` [B, D_T] and ``teacher_logit_scale`` / ``teacher_logit_bias`` (0-dim, the
-    convention of ``logit_scale`` / ``logit_bias``), distillation from a frozen teacher as in ``DDPSigmoidLoss``."""
+    convention of ``logit_scale`` / ``logit_bias``), distillation from a frozen teacher as in ``DDPSigmoidLoss``.
+    ``return_sample_losses=True``: also returns the per-sample losses of ``DDPSigmoidLoss`` (``image_loss`` [R],
+    ``text_loss`` [T]) as the last element, after the metrics when both are asked; like the metrics they stay out of
+    the ``output_dict``."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
@@ -1238,8 +1303,9 @@ class SigLipLoss(nn.Module):
                 text_weights: Optional[torch.Tensor] = None, extra_image: Optional[torch.Tensor] = None,
                 extra_image_ids: Optional[torch.Tensor] = None, teacher_image: Optional[torch.Tensor] = None,
                 teacher_text: Optional[torch.Tensor] = None, teacher_logit_scale: Optional[torch.Tensor] = None,
-                teacher_logit_bias: Optional[torch.Tensor] = None):
+                teacher_logit_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False):
         _validate_return_metrics(return_metrics)
+        _validate_return_sample_losses(return_sample_losses, self.distill)
         teacher = _teacher_of(self.distill, image_features,
                               ("teacher_image", "teacher_text", "teacher_logit_scale", "teacher_logit_bias"),
                               (teacher_image, teacher_text, teacher_logit_scale, teacher_logit_bias))
@@ -1266,7 +1332,8 @@ class SigLipLoss(nn.Module):
             logit_bias = torch.zeros((), device=image_features.device)
         fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
+        lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
         loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs,
-                                    extra_ids, weights, ximg_ids, teacher)
+                                    extra_ids, weights, ximg_ids, teacher, lbufs)
         out = {"contrastive_loss": loss} if output_dict else loss
-        return (out, _metric_dict(bufs)) if return_metrics else out
+        return _with_outputs(out, bufs, lbufs)

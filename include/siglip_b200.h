@@ -390,6 +390,28 @@ int siglip_set_sample_weights(siglip_ctx* ctx, const float* image_w, const float
  */
 int siglip_request_metrics(siglip_ctx* ctx, float* top1, int64_t* i2t_index, int64_t* t2i_index);
 
+/* Per-sample losses of the NEXT siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd only (detached statistics, fp32):
+ *   image_loss[i] (i < R: paired images, then extra images) = sum over every text of the global batch (all ranks,
+ *                 hard negatives / extra texts included) of w_ij * l_ij
+ *   text_loss[j]  (j < T: paired texts, then extras)        = sum over every image of the global batch (all ranks,
+ *                 extra images included) of w_ij * l_ij
+ * where l_ij = softplus(-y_ij z_ij) is exactly the pair's term of the loss, with the labels the options give, and w_ij
+ * its weight (1 without SIGLIP_OPT_SAMPLE_WEIGHTS). No 1/B: the rank's loss is image_loss.sum() / B up to rounding, and
+ * a sample of weight 0 reports exactly 0. Each partial (a 128-column tile of a row, a 16-row slab of a column) is added
+ * as a 64-bit fixed-point number (value * 2^32), so the results are bitwise reproducible whatever the cluster shape,
+ * stage count, schedule or order of the atomics. A partial that is not finite or not below 2^16 makes its sample
+ * report +inf (NaN for a NaN term).
+ * image_loss: [R] fp32 device buffer, text_loss: [T] fp32 device buffer, both required. Loss, gradients and the
+ * retrieval metrics are bit-identical to the same step without the request.
+ * Cost: the step's loss kernels run their own instantiation (kModeSampleLoss), which also adds the row and column sums,
+ * plus two launches (a memset of the step's fixed-point words and a one-block finalisation kernel). Workspace: two
+ * parities of [world * Tmax + Rmax] sums plus as many poison words, 64-bit each; on a single-rank context
+ * 32 * (T + R) bytes allocated by the first call (also allowed inside a capture), on a multi-rank context part of the
+ * exported text allocation from creation. This call only records the pointers, so a single-rank step stays capturable.
+ * Collective: every rank arms the same steps. Returns SIGLIP_ERR_STATE under SIGLIP_OPT_DISTILL; the host-buffer entries
+ * return SIGLIP_ERR_STATE while armed. */
+int siglip_request_sample_losses(siglip_ctx* ctx, float* image_loss, float* text_loss);
+
 /* Forward only (torch.no_grad / evaluation): siglip_forward with save_for_backward = 0. */
 int siglip_fwd(siglip_ctx* ctx, const void* img, const void* txt, const float* t_prime, const float* bias,
                float* loss, void* cuda_stream);
@@ -485,6 +507,11 @@ int siglip_debug_set_mailbox(siglip_ctx* ctx, int peer, float dt_prime, float db
  * (0xFFFFFFFF - global image index), 0 = no candidate), so
  * that the cross-rank combine of a metrics step sees candidates the kernel did not produce itself. */
 int siglip_debug_set_peer_metric_keys(siglip_ctx* ctx, int peer, const uint64_t* keys_dev, void* cuda_stream);
+/* Loopback only: seed the per-sample-loss column partials of this rank's text chunk that stand in for peer rank
+ * `peer`'s ([T] 64-bit fixed-point words, value * 2^32), so that the cross-rank sum of a per-sample-loss step adds
+ * numbers the kernel did not produce itself. */
+int siglip_debug_set_peer_sample_loss_partials(siglip_ctx* ctx, int peer, const int64_t* partials_dev,
+                                               void* cuda_stream);
 /* Loopback only (SIGLIP_OPT_EXTRA_IMAGE_IDS): seed the extra-image ids that stand in for what peer rank `peer` publishes
  * in a metrics step ([R_peer - B_peer] int64 device buffer), so that a t2i winner among its extra images is judged by
  * ids the test chose. */

@@ -62,6 +62,10 @@ def main() -> int:
                     help="also check distillation from a frozen teacher against the float64 oracle: the teacher text "
                          "travelling with the student text through the peer pulls, a teacher width different from the "
                          "student's, uneven batches, with and without sample ids and weights, fused and split")
+    ap.add_argument("--sample-losses", action="store_true",
+                    help="also check the per-sample losses (return_sample_losses=True) against the float64 oracle: "
+                         "text_loss combines every rank's column partials of the own chunk, uneven batches, hard "
+                         "negatives, ids and weights, fused / split / forward-only, and the cross-rank sum identity")
     ap.add_argument("--soak", type=int, default=0,
                     help="N > 0: that many back-to-back steps at the --batch/--dim shape mixing the fused step, the split "
                          "API and forward-only calls; same inputs, so every step of a kind must reproduce its first result "
@@ -301,6 +305,63 @@ def main() -> int:
                     t2i_index=float((gt != res["t2i_index"])[ok_t].mean()),
                     i2t_top1=abs(float(top1[0]) - hi.mean()), t2i_top1=abs(float(top1[1]) - ht.mean()),
                     unclear_rows=float(1.0 - min(ok_i.mean(), ok_t.mean())) / 50), tol=1e-6)
+            eng.close()
+
+    # ---- per-sample losses: the column sums of my chunk add every rank's fixed-point partials after flag kind 5; the
+    # totals over ranks of image_loss and text_loss agree --------------------------------------------------------------
+    if args.sample_losses:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from extra_images_oracle import label_blocks
+        from sample_losses_oracle import sample_losses
+        from distributed_sigmoid_loss_b200 import SigmoidLossEngine
+        Bs = [160 + 24 * r for r in range(world)]
+        Ts = [b + 8 + 4 * r for r, b in enumerate(Bs)]
+        D, tp, bias = 136, math.log(10.0), -8.0
+        g = torch.Generator().manual_seed(777)
+        imgs = [torch.nn.functional.normalize(torch.randn(b, D, generator=g)).to(torch.bfloat16) for b in Bs]
+        txts = [torch.nn.functional.normalize(torch.randn(t, D, generator=g)).to(torch.bfloat16) for t in Ts]
+        idss = [torch.randint(0, sum(Bs) // 2, (b,), generator=g) for b in Bs]
+        wis = [torch.rand(b, generator=g) * (torch.rand(b, generator=g) > 0.2) for b in Bs]
+        wts = [torch.rand(t, generator=g) * (torch.rand(t, generator=g) > 0.2) for t in Ts]
+        for with_ids in (False, True):
+            labels = label_blocks(Bs, Bs, Ts, [x.numpy() for x in idss] if with_ids else None)
+            ref = sample_losses([x.float().numpy() for x in imgs], [x.float().numpy() for x in txts], Bs, tp, bias,
+                                labels, [x.numpy() for x in wis], [x.numpy() for x in wts])
+            eng = SigmoidLossEngine(Bs[rank], D, dev, batch_per_rank=Bs, texts_per_rank=Ts)
+            if with_ids:
+                eng.set_option(_capi.SIGLIP_OPT_SAMPLE_IDS, 1)
+            eng.set_option(_capi.SIGLIP_OPT_SAMPLE_WEIGHTS, 1)
+            tpt, bt = torch.tensor([tp], device=dev), torch.tensor([bias], device=dev)
+            img, txt = imgs[rank].to(dev), txts[rank].to(dev)
+            for sched in ("fused", "split", "fwd", "fused"):
+                il = torch.empty(Bs[rank], device=dev)
+                tl = torch.empty(Ts[rank], device=dev)
+                if with_ids:
+                    eng.set_sample_ids(idss[rank].to(dev))
+                eng.set_sample_weights(wis[rank].to(dev), wts[rank].to(dev))
+                eng.request_sample_losses(il, tl)
+                if sched == "fused":
+                    loss = eng.fwd_bwd(img, txt, tpt, bt)[0]
+                elif sched == "split":
+                    loss = eng.forward(img, txt, tpt, bt, True)
+                    eng.backward(img, txt, tpt, None)
+                else:
+                    loss = eng.fwd(img, txt, tpt, bt)
+                torch.cuda.synchronize()
+                tot = torch.tensor([il.double().sum(), tl.double().sum()], device=dev)
+                dist.all_reduce(tot)
+                want_i, want_t = ref[rank]["image_loss"], ref[rank]["text_loss"]
+
+                def max_rel(got, want):
+                    got = got.double().cpu().numpy()
+                    keep = want > 0
+                    return float(np.max(np.abs(got[keep] - want[keep]) / want[keep]))
+
+                report(f"sample losses ids={with_ids} {sched} B={Bs} T={Ts}", dict(
+                    image_loss=max_rel(il, want_i), text_loss=max_rel(tl, want_t),
+                    zero_weights=float((il.cpu()[wis[rank] == 0] != 0).any() or (tl.cpu()[wts[rank] == 0] != 0).any()),
+                    loss_identity=abs(float(il.double().sum()) / Bs[rank] - float(loss)) / abs(float(loss)),
+                    cross_rank_sums=abs(float(tot[0] - tot[1])) / float(tot[0])), tol=1e-3)
             eng.close()
 
     # ---- hard-negative captions: every rank's extras are pulled with its text and scored against every image; their
