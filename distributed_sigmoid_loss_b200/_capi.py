@@ -31,6 +31,8 @@ EXPORTED_SYMBOLS = (
     "siglip_teacher_normalize_fwd",
     "siglip_ctx_set_option",
     "siglip_ctx_workspace_bytes",
+    "siglip_sigma_panel_rows",
+    "siglip_ctx_sigma_panels",
     "siglip_ctx_handle_bytes",
     "siglip_ctx_export_handles",
     "siglip_ctx_import_handles",
@@ -105,6 +107,7 @@ SIGLIP_OPT_EXTRA_TEXT_IDS = 22
 SIGLIP_OPT_SAMPLE_WEIGHTS = 23
 SIGLIP_OPT_EXTRA_IMAGE_IDS = 24
 SIGLIP_OPT_DISTILL = 25
+SIGLIP_OPT_SIGMA_BUDGET_MIB = 26
 
 _lib: Optional[ctypes.CDLL] = None
 
@@ -148,6 +151,10 @@ def lib() -> ctypes.CDLL:
     L.siglip_ctx_set_option.restype = ci
     L.siglip_ctx_workspace_bytes.argtypes = [vp]
     L.siglip_ctx_workspace_bytes.restype = cs
+    L.siglip_sigma_panel_rows.argtypes = [ci, ci, ci, ci, ci, ci, ctypes.POINTER(ci)]
+    L.siglip_sigma_panel_rows.restype = ci
+    L.siglip_ctx_sigma_panels.argtypes = [vp, ci, ctypes.POINTER(ci), ctypes.POINTER(ci), ctypes.POINTER(ci)]
+    L.siglip_ctx_sigma_panels.restype = ci
     L.siglip_ctx_handle_bytes.restype = cs
     L.siglip_ctx_export_handles.argtypes = [vp, vp, cs]
     L.siglip_ctx_export_handles.restype = ci

@@ -263,6 +263,8 @@ struct siglip_ctx {
   float* w_in = nullptr;                 // [w_stride] my text weights, then [R] my image weights, clamped into [0, 1];
                                          // allocated by the first siglip_set_sample_weights
   int w_stride = 0;                      // Tmax rounded up to 4: every slot is a whole number of 16-byte vectors
+  int sigma_budget_mib = 0;              // SIGLIP_OPT_SIGMA_BUDGET_MIB: bound of the sigma operands (0: none)
+  int g_rows[kMaxWorld] = {};            // rows of each allocated sigma operand (Rp, or a panel height under a budget)
   __nv_bfloat16* G[kMaxWorld] = {};      // [Rp, Tp] sigma operands (fp16 bits x kGScale), diagonal zeroed, allocated on
                                          // first use: fused step 2 (own chunk + the chunk in flight), split API one per chunk
   __nv_bfloat16* img16 = nullptr;        // [R, D] fp16 (x kXScale) images: B operand of the dtxt contraction
@@ -595,25 +597,90 @@ int finalize_step_outputs(siglip_ctx* c, unsigned int s, cudaStream_t st) {
 
 // Sigma operand + fp16 text copy number i, allocated on first use. The fused step needs two (own chunk, chunk in
 // flight), the split forward / backward API one per text chunk (they all live from the forward to the backward).
-int ensure_g(siglip_ctx* c, int i) {
-  if (c->G[i] != nullptr) return 0;
-  const size_t gbytes = static_cast<size_t>(c->Rp) * c->Tp * sizeof(__nv_bfloat16);
+// rows: rows of the operand (0: Rp, the whole batch; a panel height under SIGLIP_OPT_SIGMA_BUDGET_MIB). An operand of
+// another height is released first.
+void release_g(siglip_ctx* c, int i) {
+  if (c->G[i] == nullptr) return;
+  cudaFree(c->G[i]);
+  cudaFree(c->txt16[i]);
+  c->workspace_bytes -= static_cast<size_t>(c->g_rows[i]) * c->Tp * sizeof(__nv_bfloat16) +
+                        chunk_stride(c) * sizeof(__nv_bfloat16);
+  c->G[i] = nullptr;
+  c->txt16[i] = nullptr;
+  c->g_rows[i] = 0;
+}
+
+int ensure_g(siglip_ctx* c, int i, int rows = 0, cudaError_t* err = nullptr) {
+  if (rows == 0) rows = c->Rp;
+  if (c->G[i] != nullptr && c->g_rows[i] == rows) return 0;
+  release_g(c, i);
+  const size_t gbytes = static_cast<size_t>(rows) * c->Tp * sizeof(__nv_bfloat16);
   const size_t tbytes = chunk_stride(c) * sizeof(__nv_bfloat16);
   cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&c->G[i]), gbytes);
   if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&c->txt16[i]), tbytes);
   if (e != cudaSuccess) {
     cudaGetLastError();
+    if (err != nullptr) *err = e;
     if (c->G[i]) cudaFree(c->G[i]);
     c->G[i] = nullptr;
     char buf[256];
     snprintf(buf, sizeof(buf),
              "sigma operand %d needs %.2f GiB more device memory (B = %d: %d x %d 16-bit per text chunk kept for the "
-             "backward; siglip_fwd_bwd needs 2 of them, the split forward/backward API one per rank): %s",
-             i, static_cast<double>(gbytes + tbytes) / (1024.0 * 1024.0 * 1024.0), c->Bmax, c->Rp, c->Tp,
+             "backward; siglip_fwd_bwd needs 2 of them, the split forward/backward API one per rank; "
+             "SIGLIP_OPT_SIGMA_BUDGET_MIB bounds them by running siglip_fwd_bwd in row panels): %s",
+             i, static_cast<double>(gbytes + tbytes) / (1024.0 * 1024.0 * 1024.0), c->Bmax, rows, c->Tp,
              cudaGetErrorString(e));
     return fail(SIGLIP_ERR_CUDA, buf);
   }
+  c->g_rows[i] = rows;
   c->workspace_bytes += gbytes + tbytes;
+  return 0;
+}
+
+// ---- row panels (SIGLIP_OPT_SIGMA_BUDGET_MIB) ----
+// The sigma operands of a step under a budget: `nbuf` buffers of buf_rows x Tp 16-bit, the R rows of the rank scored
+// in panels of `rows` (a multiple of the cluster's 128 x cluster_size rows; the last one may be shorter). A budget that
+// holds nbuf whole [Rp, Tp] operands (or none set) gives the unbounded layout: one panel of R rows in Rp-row buffers.
+// Depends on the budget, the shapes and the cluster configuration only, never on free memory.
+struct Panels {
+  int rows = 0;       // panel height (0: the budget is below one minimal panel)
+  int n = 1;          // panels
+  int buf_rows = 0;   // rows of each sigma buffer
+};
+Panels sigma_panels(int R, int Rp, int Tp, int nbuf, int unit, long long budget_mib) {
+  Panels pn;
+  const long long row_bytes = static_cast<long long>(nbuf) * Tp * static_cast<long long>(sizeof(__nv_bfloat16));
+  const long long budget = budget_mib * 1024ll * 1024ll;
+  if (budget_mib <= 0 || static_cast<long long>(Rp) * row_bytes <= budget) {
+    pn.rows = R;
+    pn.buf_rows = Rp;
+    return pn;
+  }
+  const long long P = budget / row_bytes / unit * unit;   // < Rp here
+  if (P == 0) return pn;
+  pn.buf_rows = static_cast<int>(P);
+  pn.rows = P < R ? static_cast<int>(P) : R;
+  pn.n = ceil_div(R, pn.rows);
+  return pn;
+}
+// bytes of the smallest budget that runs: nbuf buffers of one minimal panel
+inline long long sigma_min_bytes(int Tp, int nbuf, int unit) {
+  return static_cast<long long>(nbuf) * unit * Tp * static_cast<long long>(sizeof(__nv_bfloat16));
+}
+// sigma buffers of the fused step: the own chunk's (kept to the end) and the one in flight at W > 1, one at W = 1
+inline int fused_buffers(const siglip_ctx* c) { return c->world > 1 ? 2 : 1; }
+inline int panel_unit(const siglip_ctx* c) { return 128 * siglip::cluster_size(c->cta_group, c->mcast); }
+int step_panels(siglip_ctx* c, int nbuf, Panels* out) {
+  *out = sigma_panels(c->R, c->Rp, c->Tp, nbuf, panel_unit(c), c->sigma_budget_mib);
+  if (out->rows == 0) {
+    char buf[256];
+    snprintf(buf, sizeof(buf),
+             "SIGLIP_OPT_SIGMA_BUDGET_MIB = %d is below one minimal sigma panel: %d buffer(s) of %d x %d 16-bit need "
+             "%.1f MiB",
+             c->sigma_budget_mib, nbuf, panel_unit(c), c->Tp,
+             static_cast<double>(sigma_min_bytes(c->Tp, nbuf, panel_unit(c))) / (1024.0 * 1024.0));
+    return fail(SIGLIP_ERR_INVALID, buf);
+  }
   return 0;
 }
 
@@ -676,24 +743,41 @@ struct FinJob {   // last chunk of a forward: the loss kernel's last CTA writes 
   float* dbias = nullptr;
 };
 
+// Rows [r0, r0 + rows) of this rank scored against columns [c0, c0 + cols) of a text chunk: a row panel of
+// SIGLIP_OPT_SIGMA_BUDGET_MIB (the default is the whole chunk). Every row- and column-indexed pointer of the launch is
+// offset by the window's origin, so the kernels see a matrix of their own: the own chunk's positives sit at local
+// row == local column only when r0 == c0.
+struct Window {
+  int r0 = 0, rows = -1;   // -1: all R rows
+  int c0 = 0, cols = -1;   // -1: the columns from c0 to the end of the chunk
+};
+
 // The loss kernel over one text chunk (Bn rows, owner's batch): S = img @ txt_c^T on wgmma, fused
 // scale/bias/log-sigmoid/reduce. save: also write the sigma operand G[gi] (+ g_diag on the own chunk); the fp16 copies
 // the gradient kernel needs are auxiliary jobs built by the caller.
 // cidx: owner rank of the chunk; col_ids: sample ids of the chunk (null = positional labels).
 int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const void* img, const __nv_bfloat16* txt_c,
                    int Bn, const int64_t* col_ids, const float* t_prime, const float* bias, bool save, const AuxList& aux,
-                   const FinJob* fin, const EndSignal& end, cudaStream_t st) {
+                   const FinJob* fin, const EndSignal& end, cudaStream_t st, const Window& win = Window()) {
   const int cg = c->cta_group;
   int rc;
-  if ((rc = ensure_g(c, save ? gi : 0))) return rc;
-  __nv_bfloat16* G = c->G[save ? gi : 0];
+  const int gidx = save ? gi : 0;
+  if (c->G[gidx] == nullptr && (rc = ensure_g(c, gidx))) return rc;
+  const int r0 = win.r0, c0 = win.c0;
+  const int M = win.rows < 0 ? c->R : win.rows;
+  Bn = win.cols < 0 ? Bn - c0 : win.cols;   // from here on: the window's columns
+  img = static_cast<const char*>(img) + static_cast<size_t>(r0) * c->D * sizeof(__nv_bfloat16);
+  txt_c += static_cast<size_t>(c0) * c->D;
+  __nv_bfloat16* G = c->G[gidx] + c0;
   CUtensorMap tmA, tmB, tmG;
-  if ((rc = encode_operand(&tmA, img, c->R, c->D, c->D, 0, 128))) return rc;
+  if ((rc = encode_operand(&tmA, img, M, c->D, c->D, 0, 128))) return rc;
   const int mc = c->mcast;
   if ((rc = encode_operand(&tmB, txt_c, Bn, c->D, c->D, 0, siglip::b_box_rows_kmajor(siglip::cluster_size(cg, mc)))))
     return rc;
   // store map of the sigma operand: [R, Bn] inside the padded [Rp, Tp] buffer, one 16-row x 32-column slab per TMA store
-  if ((rc = encode_bf16_2d(&tmG, G, (uint64_t)Bn, (uint64_t)c->R, (uint64_t)c->Tp, 32, 16,
+  // (a panel: [rows, cols] at column c0 of a buffer of panel height)
+  const int g_rows = M < c->g_rows[gidx] ? M : c->g_rows[gidx];
+  if ((rc = encode_bf16_2d(&tmG, G, (uint64_t)Bn, (uint64_t)g_rows, (uint64_t)c->Tp, 32, 16,
                            CU_TENSOR_MAP_SWIZZLE_64B)))
     return rc;
   KernelParams p;
@@ -701,8 +785,10 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
   // distillation: the teacher's images and text chunk are the second operand pair (K = DT), same boxes as the student's
   CUtensorMap tmTA = tmA, tmTB = tmB;
   if (c->distill) {
-    if ((rc = encode_operand(&tmTA, c->t_img, c->R, c->DT, c->DT, 0, 128))) return rc;
-    if ((rc = encode_operand(&tmTB, teacher_chunk(c, cidx), Bn, c->DT, c->DT, 0,
+    const __nv_bfloat16* t_img = static_cast<const __nv_bfloat16*>(c->t_img) + static_cast<size_t>(r0) * c->DT;
+    const __nv_bfloat16* t_txt = static_cast<const __nv_bfloat16*>(teacher_chunk(c, cidx)) + static_cast<size_t>(c0) * c->DT;
+    if ((rc = encode_operand(&tmTA, t_img, M, c->DT, c->DT, 0, 128))) return rc;
+    if ((rc = encode_operand(&tmTB, t_txt, Bn, c->DT, c->DT, 0,
                              siglip::b_box_rows_kmajor(siglip::cluster_size(cg, mc)))))
       return rc;
     p.k_teacher = c->DT;
@@ -716,7 +802,7 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
   p.prob[0].ab_f16 = c->input_f16;
   p.s_scale = c->input_f16 ? 1.0f / (kXScale * kXScale) : 1.0f;
   // rows: my images, the paired ones and then the extras; the loss still divides by the paired batch
-  p.prob[0].M = c->R;
+  p.prob[0].M = M;
   p.prob[0].N = Bn;
   p.prob[0].K = c->D;
   p.t_prime = t_prime;
@@ -724,39 +810,40 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
   p.inv_b = 1.0f / static_cast<float>(c->B);
   p.G = G;
   p.ldg = c->Tp;
-  p.g_diag = c->g_diag;
+  p.g_diag = c->g_diag + r0;
   // the own chunk's positives are its first B columns (row == col < M); the hard negatives behind them never are. With
   // extra images and extra texts on this rank, row == col would also meet them: the own chunk then takes its positives
   // from ids, bounded to the first B rows and columns (iota ids for positional labels), and leaves g_diag alone
   p.own_chunk = (own && !c->own_pos_ids) ? 1 : 0;
   p.store_g = save ? 1 : 0;
   p.g_scale = kGScale;
+  auto rest = [](int n, int o) { return n > o ? n - o : 0; };   // entries of an id list past a window's origin
   if (col_ids != nullptr) {
-    p.row_ids = row_ids(c);
-    p.col_ids = col_ids;
+    p.row_ids = row_ids(c) + r0;
+    p.col_ids = col_ids + c0;
     // the chunk's ids cover its paired texts, and under SIGLIP_OPT_EXTRA_TEXT_IDS its extras too
-    p.col_pos_n = chunk_id_count(c, cidx);
+    p.col_pos_n = rest(chunk_id_count(c, cidx), c0);
     // the rows' ids cover the paired images, and under SIGLIP_OPT_EXTRA_IMAGE_IDS the extras too
-    p.row_pos_n = row_id_count(c);
+    p.row_pos_n = rest(row_id_count(c), r0);
   } else if (own && c->own_pos_ids) {
-    p.row_ids = c->iota;
-    p.col_ids = c->iota;
-    p.col_pos_n = c->B;
-    p.row_pos_n = c->B;
+    p.row_ids = c->iota + r0;
+    p.col_ids = c->iota + c0;
+    p.col_pos_n = rest(c->B, c0);
+    p.row_pos_n = rest(c->B, r0);
   }
   if (c->sample_weights) {   // the kWeights instantiation: w_ij = image weight i x text weight j of the chunk
-    p.row_w = image_weights(c);
-    p.col_w = chunk_weights(c, cidx);
+    p.row_w = image_weights(c) + r0;
+    p.col_w = chunk_weights(c, cidx) + c0;
   }
   if (c->mkeys_step != nullptr) {   // a metrics step: the kMetrics instantiation reduces the argmax keys
-    p.row_keys = c->mkeys_step + mkeys_rows(c);
-    p.col_keys = c->mkeys_step + static_cast<size_t>(cidx) * c->Tmax;
-    p.row_off = c->off[c->rank];
-    p.col_off = c->toff[cidx];
+    p.row_keys = c->mkeys_step + mkeys_rows(c) + r0;
+    p.col_keys = c->mkeys_step + static_cast<size_t>(cidx) * c->Tmax + c0;
+    p.row_off = c->off[c->rank] + r0;
+    p.col_off = c->toff[cidx] + c0;
   }
   if (c->lsum_step != nullptr) {   // a per-sample-loss step: the kModeSampleLoss kernel adds the row / column sums
-    p.sl_rows = c->lsum_step + lsum_rows(c);
-    p.sl_cols = c->lsum_step + static_cast<size_t>(cidx) * c->Tmax;
+    p.sl_rows = c->lsum_step + lsum_rows(c) + r0;
+    p.sl_cols = c->lsum_step + static_cast<size_t>(cidx) * c->Tmax + c0;
     p.sl_poison = static_cast<long long>(lsum_half(c));
   }
   p.partials = c->partials;
@@ -862,21 +949,33 @@ int grad_tile_cols(const siglip_ctx* c, int M0, int M1) {
   return 18 * waves(siglip::kWideTileCols) <= 10 * waves(siglip::kTileCols) ? siglip::kWideTileCols : siglip::kTileCols;
 }
 
+// A row panel of the gradient launch (SIGLIP_OPT_SIGMA_BUDGET_MIB): the sigma panel of rows [r0, r0 + rows) in buffer
+// gb, the chunk's fp16 text in txt16[tb]. dimg takes rows [r0, r0 + rows) (its positive-pair term too, on the own
+// chunk); dtxt sums over the panel's rows, and takes the positive-pair term of all B rows only when fix_dtxt (the last
+// own-chunk launch, after every panel's g_diag is written). The default is the whole chunk in buffer gi.
+struct GradPanel {
+  int gb = -1, tb = -1;   // -1: gi
+  int r0 = 0, rows = -1;  // -1: all R rows
+  bool fix_dtxt = true;
+};
+
 int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_bfloat16* txt_own, int Bn,
                    const float* t_prime, const float* grad_out, const GradOut& o, const AuxList& aux,
-                   const EndSignal& end, cudaStream_t st) {
+                   const EndSignal& end, cudaStream_t st, const GradPanel& gp = GradPanel()) {
   const int cg = c->cta_group;
-  const int tile_n = grad_tile_cols(c, c->R, Bn);
+  const int gb = gp.gb < 0 ? gi : gp.gb, tb = gp.tb < 0 ? gi : gp.tb;
+  const int r0 = gp.r0, M = gp.rows < 0 ? c->R : gp.rows;
+  const int tile_n = grad_tile_cols(c, M, Bn);
   const int bk = siglip::b_box_k_mnmajor(siglip::cluster_size(cg, c->mcast), tile_n);
   CUtensorMap tmA0, tmB0, tmA1, tmB1;
   int rc;
-  if (c->G[gi] == nullptr) return fail(SIGLIP_ERR_STATE, "gradient kernel without a saved sigma operand");
+  if (c->G[gb] == nullptr) return fail(SIGLIP_ERR_STATE, "gradient kernel without a saved sigma operand");
   // G is [R, Bn]: the MN-major map of the dtxt problem reads R k-rows of it and the image copy R rows; TMA fills the
-  // boxes past R with zeros, so a partial last k block adds nothing
-  if ((rc = encode_operand(&tmA0, c->G[gi], c->R, Bn, c->Tp, 0, 128))) return rc;
-  if ((rc = encode_operand(&tmB0, c->txt16[gi], c->D, Bn, c->D, 1, 0, bk))) return rc;
-  if ((rc = encode_operand(&tmA1, c->G[gi], Bn, c->R, c->Tp, 1, 0))) return rc;
-  if ((rc = encode_operand(&tmB1, c->img16, c->D, c->R, c->D, 1, 0, bk))) return rc;
+  // boxes past R with zeros, so a partial last k block adds nothing (a panel: rows [r0, r0 + M) of both)
+  if ((rc = encode_operand(&tmA0, c->G[gb], M, Bn, c->Tp, 0, 128))) return rc;
+  if ((rc = encode_operand(&tmB0, c->txt16[tb], c->D, Bn, c->D, 1, 0, bk))) return rc;
+  if ((rc = encode_operand(&tmA1, c->G[gb], Bn, M, c->Tp, 1, 0))) return rc;
+  if ((rc = encode_operand(&tmB1, c->img16 + static_cast<size_t>(r0) * c->D, c->D, M, c->D, 1, 0, bk))) return rc;
   KernelParams p;
   memset(&p, 0, sizeof(p));
   p.nprob = 2;
@@ -892,16 +991,19 @@ int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_
     pr.fix_f16 = c->saved_f16;
     pr.fix_mat_scale = c->saved_f16 ? 1.0f / kXScale : 1.0f;
   }
-  p.prob[0].M = c->R;
+  const size_t row_off = static_cast<size_t>(r0) * c->D;   // dimg elements before the panel
+  p.prob[0].M = M;
   p.prob[0].K = Bn;
   p.prob[0].a_mn = 0;
-  p.prob[0].out = o.dimg_out;
+  p.prob[0].out = static_cast<char*>(o.dimg_out) + row_off * (o.dimg_bf16 ? sizeof(__nv_bfloat16) : sizeof(float));
   p.prob[0].out_bf16 = o.dimg_bf16 ? 1 : 0;
-  p.prob[0].add_src = o.dimg_add;
+  p.prob[0].add_src = o.dimg_add != nullptr ? o.dimg_add + row_off : nullptr;
   p.prob[0].ld_add = c->D;
-  p.prob[0].fix_mat = (own && !c->own_pos_ids) ? txt_own : nullptr;
+  if (p.prob[0].fix_vec != nullptr) p.prob[0].fix_vec += r0;
+  p.prob[0].fix_mat = (own && !c->own_pos_ids) ? txt_own + row_off : nullptr;
+  if (!gp.fix_dtxt) p.prob[1].fix_vec = nullptr;
   p.prob[1].M = Bn;
-  p.prob[1].K = c->R;
+  p.prob[1].K = M;
   p.prob[1].a_mn = 1;
   p.prob[1].out = o.dtxt_out;
   p.prob[1].out_bf16 = o.dtxt_bf16 ? 1 : 0;
@@ -911,8 +1013,12 @@ int run_grad_chunk(siglip_ctx* c, int gi, bool own, const void* img, const __nv_
   p.p1_wait_flag = o.dtxt_add_flag;
   p.p1_wait_value = o.dtxt_add_value;
   // g_diag and both fix matrices hold this rank's B rows; the dtxt rows of the own chunk's hard negatives (B .. Bn) and
-  // the dimg rows of its extra images (B .. R) have no positive-pair term
-  p.fix_rows = c->B;
+  // the dimg rows of its extra images (B .. R) have no positive-pair term. A panel past row 0 has B - r0 of them and no
+  // dtxt term (the caller's choice above): the field covers the dimg problem alone
+  // (a chunk other than the own one has no positive-pair term at all)
+  if (p.prob[1].fix_vec != nullptr && r0 != 0)
+    return fail(SIGLIP_ERR_INVALID, "a gradient panel past row 0 cannot take the dtxt positive term");
+  p.fix_rows = c->B > r0 ? c->B - r0 : 0;
   if (o.sc_dt_prime != nullptr || o.sc_dbias != nullptr) {
     p.sc_saved = c->scalars + kSavedScalars;
     p.sc_dt_prime = o.sc_dt_prime;
@@ -1089,6 +1195,28 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
   if ((rc = check_call(c, img, txt, t_prime, st))) return rc;
   if (bias == nullptr || loss == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if ((rc = check_dbg(c, "siglip forward (previous launch)"))) return rc;
+  if (c->sigma_budget_mib > 0) {
+    Panels pn;
+    if (save) {
+      // the split API keeps one whole operand per chunk until the backward: no panels
+      pn = sigma_panels(c->R, c->Rp, c->Tp, c->world, panel_unit(c), c->sigma_budget_mib);
+      if (pn.n > 1 || pn.buf_rows != c->Rp) {
+        char buf[320];
+        snprintf(buf, sizeof(buf),
+                 "siglip_forward with save_for_backward keeps %d sigma operands of %d x %d 16-bit (%.2f GiB) until "
+                 "the backward, more than SIGLIP_OPT_SIGMA_BUDGET_MIB = %d: use siglip_fwd_bwd, which runs in row panels",
+                 c->world, c->Rp, c->Tp,
+                 static_cast<double>(c->world) * c->Rp * c->Tp * sizeof(__nv_bfloat16) / (1024.0 * 1024.0 * 1024.0),
+                 c->sigma_budget_mib);
+        return fail(SIGLIP_ERR_STATE, buf);
+      }
+    } else if (c->G[0] == nullptr) {
+      // a forward without save writes no sigma: one panel-sized buffer backs the (unused) store map
+      if ((rc = step_panels(c, 1, &pn))) return rc;
+      CK(cudaSetDevice(c->device));
+      if ((rc = ensure_g(c, 0, pn.buf_rows))) return rc;
+    }
+  }
   if ((rc = take_ids(c))) return rc;
   CK(cudaSetDevice(c->device));
   const int W = c->world, r = c->rank;
@@ -1258,6 +1386,16 @@ int backward_impl(siglip_ctx* c, const void* img, const void* txt, const float* 
 // (text pulls inside L(k-1), progressive fold inside G(j+1)) is unchanged, but every flag is waited for / raised INSIDE
 // these kernels (auxiliary warps, last-CTA tickets): a multi-rank step is exactly 2W launches, like a single-rank one.
 // The last gradient launch adds the folded peer contributions in its dtxt epilogue, so there is no reduction kernel.
+//
+// Under SIGLIP_OPT_SIGMA_BUDGET_MIB the rows are scored in np panels of P rows (DESIGN.md, "Row panels"): every sigma
+// operand holds one panel, and each chunk runs L G per panel (index k.p below). Panel 0 of the own chunk keeps the
+// role of L0 / G0, so the exchange keeps its shape:
+//   W > 1:  L0.0  [L0.p G0.p]p=np-1..1  [L1.p G1.p]p=0..np-1  ...  [L(W-1).p G(W-1).p]  G0.0
+//   W = 1:        [L0.p G0.p]p=np-1..1  L0.0 G0.0          (one buffer: nothing is in flight)
+// Flag 1 of a remote chunk is raised by its last panel's gradient launch; its earlier panels add into the slot. The
+// own panels past 0 sum their dtxt into a local partial (slot `rank`, which no peer reads in this step, or dtxt_acc at
+// W = 1) that enters the first fold, and G0.0 adds the positive-pair term of all B rows to dtxt. With one panel the
+// launches are exactly the unbounded step's.
 // ---------------------------------------------------------------------------------------------------------------
 int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_prime, const float* bias, float* loss,
                const float* grad_out, void* dimg, void* dtxt, float* dt_prime, float* dbias, cudaStream_t st) {
@@ -1266,9 +1404,13 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   if (bias == nullptr || loss == nullptr || dimg == nullptr || dtxt == nullptr)
     return fail(SIGLIP_ERR_INVALID, "null argument");
   if ((rc = check_dbg(c, "siglip_fwd_bwd (previous launch)"))) return rc;
+  Panels pn;
+  if ((rc = step_panels(c, fused_buffers(c), &pn))) return rc;
   if ((rc = take_ids(c))) return rc;
   CK(cudaSetDevice(c->device));
   const int W = c->world, r = c->rank;
+  const int np = pn.n, P = pn.rows;
+  auto prow = [&](int p) { return c->R - p * P < P ? c->R - p * P : P; };
   const size_t stride = chunk_stride(c);
   const unsigned int s = ++c->n_fwd;
   const unsigned int n = ++c->n_bwd;
@@ -1278,8 +1420,15 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   if ((rc = take_sample_losses(c, s, st))) return rc;
   c->gen = 0;                       // the sigma operands of a split forward (if any) are overwritten
   c->saved_f16 = c->input_f16;
-  if ((rc = ensure_g(c, 0))) return rc;
-  if (W > 1 && (rc = ensure_g(c, 1))) return rc;
+  if ((rc = ensure_g(c, 0, pn.buf_rows))) return rc;
+  if (W > 1 && (rc = ensure_g(c, 1, pn.buf_rows))) return rc;
+  if (W == 1 && np > 1 && c->dtxt_acc == nullptr) {
+    const size_t bytes = static_cast<size_t>(c->T) * c->D * sizeof(float);
+    CK(cudaMalloc(reinterpret_cast<void**>(&c->dtxt_acc), bytes));
+    c->workspace_bytes += bytes;
+  }
+  // dtxt of the own panels past 0 (fp32, [T, D]), added to the fold chain (W > 1) or by G0.0 (W = 1)
+  float* own_part = (np > 1) ? ((W > 1) ? c->slots + r * stride : c->dtxt_acc) : nullptr;
   const __nv_bfloat16* own_txt = reinterpret_cast<const __nv_bfloat16*>(txt);
   const size_t own_bytes = static_cast<size_t>(c->T) * c->D * sizeof(__nv_bfloat16);
   FinJob fin;
@@ -1292,9 +1441,11 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   // Distillation adds a teacher publish and a teacher pull to L0 (up to 8 jobs with ids and weights): the own text's
   // conversion and the flag-3 wait move to L1 as well. G0, their first consumer, and G1 run behind L1.
   const bool l0_work_in_l1 = W > 1 && ik && c->distill;
+  // with panels, those jobs go to the launch behind L0.0, the first own panel's loss kernel (G0.p reads them)
+  const bool moved_to_l1 = np == 1;
 
   // ---- L0: own chunk. Its auxiliary warps also publish my text to the peers and start the first pull ----
-  {
+  if (W > 1 || np == 1) {
     AuxList aux;
     if (W > 1) {
       if (ik) {
@@ -1341,19 +1492,22 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       c->prewait3 = n - 1;
       add_pull_job(c, aux, step_owner(c, r, 1), s);
     }
+    Window w0;
+    w0.rows = prow(0);
     if ((rc = run_loss_chunk(c, 0, r, true, true, img, own_txt, c->T, chunk_ids(c, r), t_prime, bias, true, aux,
-                             (W == 1) ? &fin : nullptr, EndSignal(), st)))
+                             (W == 1) ? &fin : nullptr, EndSignal(), st, w0)))
       return rc;
   }
   if (W > 1) own_txt = c->txt_all + r * stride;   // the copy the peers see (same bytes)
-  // ---- remote chunks: L_k then G_k (gradient slot j = k) ----
-  for (int k = 1; k < W; ++k) {
-    const int cidx = step_owner(c, r, k);
-    const __nv_bfloat16* txt_c = c->txt_all + cidx * stride;
-    {
-      AuxList aux;
-      add_cvt_jobs(c, aux, 1, k == 1 && img_cvt_in_l1, img, txt_c, c->Ts[cidx]);
-      if (k == 1 && l0_work_in_l1) {
+  // ---- own panels past 0: L0.p G0.p in the buffer of the chunks in flight (W = 1: the only buffer) ----
+  for (int p = np - 1; p >= 1; --p) {
+    const int p0 = p * P, rows = prow(p), gb = (W > 1) ? 1 : 0;
+    const bool first_launch = (W == 1 && p == np - 1);
+    AuxList aux;
+    if (first_launch) add_cvt_jobs(c, aux, 0, true, img, own_txt, c->T);
+    if (W > 1 && p == np - 1) {
+      if (img_cvt_in_l1) add_img_cvt_job(c, aux, img);
+      if (l0_work_in_l1) {
         add_cvt_jobs(c, aux, 0, false, img, reinterpret_cast<const __nv_bfloat16*>(txt), c->T);
         siglip::AuxJob& w3 = aux.add(siglip::kAuxWaitOnly);
         w3.wait_flags = c->flags + 3 * kMaxWorld;
@@ -1361,25 +1515,85 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
         w3.wait_value = n - 1;
         w3.site = 13;
       }
-      if (k + 1 < W) add_pull_job(c, aux, step_owner(c, r, k + 1), s);
-      const bool lastL = (k == W - 1);
+    }
+    // The panel's positives sit in columns [p0, p0 + rows): scored with the own-chunk diagonal in a window that starts
+    // at column p0, the columns before it in a second launch without one. iota ids (own_pos_ids) and rows past B need
+    // one launch.
+    const bool own_rows = p0 < c->B;
+    Window w;
+    w.r0 = p0;
+    w.rows = rows;
+    if (own_rows && !c->own_pos_ids) {
+      w.c0 = p0;
+      if ((rc = run_loss_chunk(c, gb, r, true, first_launch, img, own_txt, c->T, chunk_ids(c, r), t_prime, bias, true,
+                               aux, nullptr, EndSignal(), st, w)))
+        return rc;
+      w.c0 = 0;
+      w.cols = p0;
+      if ((rc = run_loss_chunk(c, gb, r, false, false, img, own_txt, c->T, chunk_ids(c, r), t_prime, bias, true,
+                               AuxList(), nullptr, EndSignal(), st, w)))
+        return rc;
+    } else if ((rc = run_loss_chunk(c, gb, r, own_rows, first_launch, img, own_txt, c->T, chunk_ids(c, r), t_prime,
+                                    bias, true, aux, nullptr, EndSignal(), st, w))) {
+      return rc;
+    }
+    GradOut o;
+    o.dimg_out = (W > 1) ? static_cast<void*>(c->dimg_acc) : dimg;   // W = 1: these rows are final
+    o.dimg_bf16 = W == 1 && c->grad_bf16;
+    o.dtxt_out = own_part;
+    o.dtxt_add = (p == np - 1) ? nullptr : own_part;
+    GradPanel gp;
+    gp.gb = gb;
+    gp.tb = 0;
+    gp.r0 = p0;
+    gp.rows = rows;
+    gp.fix_dtxt = false;
+    if ((rc = run_grad_chunk(c, gb, true, img, own_txt, c->T, t_prime, grad_out, o, AuxList(), EndSignal(), st, gp)))
+      return rc;
+  }
+  // ---- remote chunks: L_k then G_k (gradient slot j = k) ----
+  for (int k = 1; k < W; ++k) {
+    const int cidx = step_owner(c, r, k);
+    const __nv_bfloat16* txt_c = c->txt_all + cidx * stride;
+   for (int p = 0; p < np; ++p) {
+    const int p0 = p * P;
+    {
+      AuxList aux;
+      if (p == 0) add_cvt_jobs(c, aux, 1, k == 1 && img_cvt_in_l1 && moved_to_l1, img, txt_c, c->Ts[cidx]);
+      if (p == 0 && k == 1 && l0_work_in_l1 && moved_to_l1) {
+        add_cvt_jobs(c, aux, 0, false, img, reinterpret_cast<const __nv_bfloat16*>(txt), c->T);
+        siglip::AuxJob& w3 = aux.add(siglip::kAuxWaitOnly);
+        w3.wait_flags = c->flags + 3 * kMaxWorld;
+        w3.wait_n = W;
+        w3.wait_value = n - 1;
+        w3.site = 13;
+      }
+      if (p == 0 && k + 1 < W) add_pull_job(c, aux, step_owner(c, r, k + 1), s);
+      const bool lastL = (k == W - 1) && (p == np - 1);
       EndSignal end = (lastL && ik) ? end_signal(c, 2, s) : EndSignal();   // "I have pulled everyone's text"
+      Window w;
+      w.r0 = p0;
+      w.rows = prow(p);
       if ((rc = run_loss_chunk(c, 1, cidx, false, false, img, txt_c, c->Ts[cidx], chunk_ids(c, cidx), t_prime, bias, true,
-                               aux, lastL ? &fin : nullptr, end, st)))
+                               aux, lastL ? &fin : nullptr, end, st, w)))
         return rc;
       if (lastL && !ik && (rc = signal_peers(c, 2, s, st))) return rc;
     }
     const int j = k;
+    // dimg rows of a panel past 0 were started by their own panel, and the last chunk finishes them
+    const bool rows_final = p > 0 && k == W - 1;
     GradOut o;
-    o.dimg_add = (j > 1) ? c->dimg_acc : nullptr;
-    o.dimg_out = c->dimg_acc;
+    o.dimg_add = (j > 1 || p > 0) ? c->dimg_acc : nullptr;
+    o.dimg_out = rows_final ? dimg : static_cast<void*>(c->dimg_acc);
+    o.dimg_bf16 = rows_final && c->grad_bf16;
     o.dtxt_out = c->slots + cidx * stride;
+    o.dtxt_add = (p > 0) ? c->slots + cidx * stride : nullptr;   // the chunk's earlier panels
     AuxList aux;
-    if (j >= 2) {
+    if (j >= 2 && p == 0) {
       const int pr = ((r - step_offset(c, j - 1)) % W + W) % W;
       siglip::AuxJob& f = aux.add(siglip::kAuxFold);
       f.src = reinterpret_cast<const uint4*>(c->peer_slots[pr] + r * stride);
-      f.src2 = (j == 2) ? nullptr : reinterpret_cast<const uint4*>(c->dtxt_acc);
+      f.src2 = reinterpret_cast<const uint4*>((j == 2) ? own_part : c->dtxt_acc);
       f.dst = reinterpret_cast<uint4*>(c->dtxt_acc);
       f.n16 = static_cast<unsigned long long>(c->T) * c->D * sizeof(float) / 16;
       f.wait_flags = c->flags + 1 * kMaxWorld + pr;
@@ -1387,9 +1601,24 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       f.wait_value = base + static_cast<unsigned int>(j - 1);
       f.site = 7;
     }
-    EndSignal end = ik ? end_signal(c, 1, base + static_cast<unsigned int>(j)) : EndSignal();
-    if ((rc = run_grad_chunk(c, 1, false, img, own_txt, c->Ts[cidx], t_prime, grad_out, o, aux, end, st))) return rc;
-    if (!ik && (rc = signal_peers(c, 1, base + static_cast<unsigned int>(j), st))) return rc;
+    // "my contribution to owner cidx is complete": its last panel only
+    const bool lastG = p == np - 1;
+    EndSignal end = (ik && lastG) ? end_signal(c, 1, base + static_cast<unsigned int>(j)) : EndSignal();
+    GradPanel gp;
+    gp.r0 = p0;
+    gp.rows = prow(p);
+    if ((rc = run_grad_chunk(c, 1, false, img, own_txt, c->Ts[cidx], t_prime, grad_out, o, aux, end, st, gp)))
+      return rc;
+    if (!ik && lastG && (rc = signal_peers(c, 1, base + static_cast<unsigned int>(j), st))) return rc;
+   }
+  }
+  // ---- W = 1 with panels: L0.0 last, in the buffer G0.0 reads ----
+  if (W == 1 && np > 1) {
+    Window w0;
+    w0.rows = prow(0);
+    if ((rc = run_loss_chunk(c, 0, r, true, false, img, own_txt, c->T, chunk_ids(c, r), t_prime, bias, true, AuxList(),
+                             &fin, EndSignal(), st, w0)))
+      return rc;
   }
   // ---- G0: own chunk, gradient slot W. Folds the last remote contribution and adds the folded sum in its epilogue ----
   {
@@ -1404,7 +1633,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       const int pr = ((r - step_offset(c, W - 1)) % W + W) % W;
       siglip::AuxJob& f = aux.add(siglip::kAuxFold);
       f.src = reinterpret_cast<const uint4*>(c->peer_slots[pr] + r * stride);
-      f.src2 = (W == 2) ? nullptr : reinterpret_cast<const uint4*>(c->dtxt_acc);
+      f.src2 = reinterpret_cast<const uint4*>((W == 2) ? own_part : c->dtxt_acc);
       f.dst = reinterpret_cast<uint4*>(c->dtxt_acc);
       f.n16 = static_cast<unsigned long long>(c->T) * c->D * sizeof(float) / 16;
       f.wait_flags = c->flags + 1 * kMaxWorld + pr;
@@ -1416,12 +1645,16 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       o.dtxt_add = c->dtxt_acc;
       o.dtxt_add_flag = c->sync_words + kSyncFoldDone;
       o.dtxt_add_value = n;
+    } else if (np > 1) {
+      o.dtxt_add = own_part;   // W = 1: the own panels past 0, written by the launches before this one
     }
     const bool scalars_here = !(W > 1 && c->sync_scalar_grads);
     o.sc_dt_prime = scalars_here ? dt_prime : nullptr;
     o.sc_dbias = scalars_here ? dbias : nullptr;
     EndSignal end = (W > 1 && ik) ? end_signal(c, 3, n) : EndSignal();   // "I have read everyone's contributions"
-    if ((rc = run_grad_chunk(c, 0, true, img, own_txt, c->T, t_prime, grad_out, o, aux, end, st))) return rc;
+    GradPanel gp;
+    gp.rows = prow(0);
+    if ((rc = run_grad_chunk(c, 0, true, img, own_txt, c->T, t_prime, grad_out, o, aux, end, st, gp))) return rc;
     if (W > 1 && !ik && (rc = signal_peers(c, 3, n, st))) return rc;
   }
   if ((rc = finalize_step_outputs(c, s, st))) return rc;
@@ -1609,8 +1842,17 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   c->peer_slots[rank] = c->slots;
   c->peer_flags[rank] = c->flags;
   c->workspace_bytes = total;
-  int rc = ensure_g(c, 0);
-  if (rc) return rc;
+  // The first sigma operand is allocated here when the device holds it. When the device is out of memory for it, the
+  // context is created all the same and the first step allocates what it needs: a batch whose whole operand exceeds
+  // the device runs under SIGLIP_OPT_SIGMA_BUDGET_MIB, and an unbounded step reports the shortfall there. Any other
+  // failure fails the creation.
+  {
+    cudaError_t ge = cudaSuccess;
+    if (int grc = ensure_g(c, 0, 0, &ge)) {
+      if (ge != cudaErrorMemoryAllocation) return grc;
+      g_last_error.clear();
+    }
+  }
   CK(cudaDeviceSynchronize());
   guard.c = nullptr;
   *out = c;
@@ -1680,6 +1922,14 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL needs a context created with siglip_ctx_create_distill");
       c->distill = value ? 1 : 0;
       c->teacher_set = false;
+      return 0;
+    case SIGLIP_OPT_SIGMA_BUDGET_MIB:
+      if (value < 0) return fail(SIGLIP_ERR_INVALID, "the sigma budget must be >= 0 MiB (0: unbounded)");
+      c->sigma_budget_mib = value;
+      // the operands are allocated again, at the height the next step needs
+      CK(cudaSetDevice(c->device));
+      for (int i = 0; i < kMaxWorld; ++i) release_g(c, i);
+      c->gen = 0;
       return 0;
     case SIGLIP_OPT_CTA_GROUP:
       if (value != 1 && value != 2) return fail(SIGLIP_ERR_INVALID, "cta_group must be 1 or 2");
@@ -1784,6 +2034,25 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
 }
 
 size_t siglip_ctx_workspace_bytes(const siglip_ctx* c) { return c ? c->workspace_bytes : 0; }
+
+int siglip_ctx_sigma_panels(const siglip_ctx* c, int buffers, int* panel_rows, int* panels, int* whole) {
+  if (c == nullptr || buffers < 0 || buffers > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "invalid argument");
+  const Panels pn = sigma_panels(c->R, c->Rp, c->Tp, buffers ? buffers : fused_buffers(c), panel_unit(c),
+                                 c->sigma_budget_mib);
+  if (panel_rows != nullptr) *panel_rows = pn.rows;
+  if (panels != nullptr) *panels = pn.rows ? pn.n : 0;
+  if (whole != nullptr) *whole = (pn.rows == c->R && pn.buf_rows == c->Rp) ? 1 : 0;
+  return 0;
+}
+
+int siglip_sigma_panel_rows(int rows, int rows_padded, int cols_padded, int buffers, int cluster_rows, int budget_mib,
+                            int* buffer_rows) {
+  if (rows < 1 || rows_padded < rows || cols_padded < 1 || buffers < 1 || cluster_rows < 1 || budget_mib < 0)
+    return -fail(SIGLIP_ERR_INVALID, "siglip_sigma_panel_rows: invalid argument");
+  const Panels pn = sigma_panels(rows, rows_padded, cols_padded, buffers, cluster_rows, budget_mib);
+  if (buffer_rows != nullptr) *buffer_rows = pn.buf_rows;
+  return pn.rows;
+}
 
 size_t siglip_ctx_handle_bytes(void) { return sizeof(IpcBlob); }
 

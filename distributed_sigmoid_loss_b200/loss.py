@@ -145,6 +145,25 @@ class SigmoidLossEngine:
         if option == _capi.SIGLIP_OPT_EXTRA_IMAGE_IDS or (option == _capi.SIGLIP_OPT_SAMPLE_IDS and not value):
             self.extra_image_ids = bool(value)
 
+    def set_sigma_budget(self, sigma_budget_bytes: Optional[int]) -> None:
+        """SIGLIP_OPT_SIGMA_BUDGET_MIB: bound the 16-bit sigma operands to sigma_budget_bytes (rounded down to MiB; None
+        or 0: unbounded). Fused steps then run in row panels (see the option in include/siglip_b200.h)."""
+        mib = _sigma_budget_mib(sigma_budget_bytes)
+        self.set_option(_capi.SIGLIP_OPT_SIGMA_BUDGET_MIB, mib)
+        self.sigma_budget_mib = mib
+
+    def split_fits_budget(self) -> bool:
+        """Whether the split forward / backward (W whole sigma operands kept until the backward) fits the budget."""
+        return self.sigma_panels(self.world)[2]
+
+    def sigma_panels(self, buffers: int = 0) -> Tuple[int, int, bool]:
+        """(panel rows, panels, whole) of the budget for `buffers` sigma operands (0: the fused step's); panel rows 0
+        means the budget is below one minimal panel, whole that it holds the whole operands (siglip_ctx_sigma_panels)."""
+        rows, n, whole = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        _capi.check(self._L.siglip_ctx_sigma_panels(self._h, int(buffers), ctypes.byref(rows), ctypes.byref(n),
+                                                    ctypes.byref(whole)))
+        return rows.value, n.value, bool(whole.value)
+
     def kernel_times(self):
         """(loss_ms, loss_launches, grad_ms, grad_launches) since the last call; needs SIGLIP_OPT_KERNEL_TIMING."""
         lm, gm = ctypes.c_double(), ctypes.c_double()
@@ -754,8 +773,9 @@ class _EngineCache:
     def __init__(self, group=None, cta_group: int = 2, overlap_pull: bool = True, sync_scalar_grads: bool = False,
                  bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
                  extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
-                 distill: Optional[float] = None):
+                 distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
+        self.sigma_budget_bytes = sigma_budget_bytes
         self.distill = distill
         self.extra_images = extra_images
         self.sample_weights = sample_weights
@@ -798,8 +818,35 @@ class _EngineCache:
                 eng.set_option(_capi.SIGLIP_OPT_SAMPLE_WEIGHTS, 1)
             if self.distill is not None:
                 eng.set_option(_capi.SIGLIP_OPT_DISTILL, 1)
+            if self.sigma_budget_bytes:
+                eng.set_sigma_budget(self.sigma_budget_bytes)
             self._engines[key] = eng
         return eng
+
+
+def _sigma_budget_mib(sigma_budget_bytes) -> int:
+    if sigma_budget_bytes is None:
+        return 0
+    if isinstance(sigma_budget_bytes, bool) or not isinstance(sigma_budget_bytes, int) or sigma_budget_bytes < 0:
+        raise ValueError(f"sigma_budget_bytes must be None or an int >= 0, got {sigma_budget_bytes!r}")
+    mib = sigma_budget_bytes >> 20
+    if sigma_budget_bytes and mib == 0:
+        raise ValueError(f"sigma_budget_bytes = {sigma_budget_bytes} is below 1 MiB")
+    return mib
+
+
+def _fused_under_budget(eng, fused_step: Optional[bool]) -> bool:
+    """The schedule of a step: the module's choice, except that under a sigma budget every step takes the fused step
+    (the split forward keeps W whole operands); an explicit fused_step=False that the budget cannot hold raises here,
+    before any GPU work."""
+    fused = (eng.world > 1) if fused_step is None else bool(fused_step)
+    if getattr(eng, "sigma_budget_mib", 0):
+        if fused_step is None:
+            fused = True
+        elif not fused and not eng.split_fits_budget():
+            raise ValueError("fused_step=False keeps one whole sigma operand per rank until the backward, more than "
+                             "sigma_budget_bytes: use fused_step=None or True, which runs in row panels")
+    return fused
 
 
 _ID_DTYPES = (torch.int8, torch.uint8, torch.int16, torch.int32, torch.int64)
@@ -1168,8 +1215,9 @@ class DDPSigmoidLoss(nn.Module):
                  normalize_inputs: bool = False, sync_scalar_grads: bool = False, fused_step: Optional[bool] = None,
                  batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
                  extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
-                 distill: Optional[float] = None) -> None:
+                 distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None) -> None:
         super().__init__()
+        _sigma_budget_mib(sigma_budget_bytes)
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_images = _validate_hard_negatives(extra_images, "extra_images")
         extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
@@ -1203,7 +1251,9 @@ class DDPSigmoidLoss(nn.Module):
         self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank,
                                    multi_positive=multi_positive, hard_negatives=hard_negatives,
                                    extra_texts=extra_texts, sample_weights=sample_weights, extra_images=extra_images,
-                                   distill=distill)
+                                   distill=distill, sigma_budget_bytes=sigma_budget_bytes)
+        # extension: bound of the 16-bit sigma operands; steps then run in row panels (memory O(budget), not O(B^2))
+        self.sigma_budget_bytes = sigma_budget_bytes
 
     def engine_for(self, batch: int, dim: int, device: torch.device, teacher_dim: int = 0) -> SigmoidLossEngine:
         """The engine forward() uses for these shapes. A module built with distill=lambda needs the teacher's width
@@ -1239,7 +1289,7 @@ class DDPSigmoidLoss(nn.Module):
         image_embeddings, text_embeddings = _pad_dim(image_embeddings), _pad_dim(text_embeddings)
         eng = self._cache.get(self.gpu_batch_size, image_embeddings.shape[1], image_embeddings.device,
                               teacher[0].shape[1] if teacher is not None else 0)
-        fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
+        fused = _fused_under_budget(eng, self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
         lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
         loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
@@ -1275,8 +1325,10 @@ class SigLipLoss(nn.Module):
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
                  multi_positive: bool = False, hard_negatives: int = 0, extra_texts: int = 0,
-                 sample_weights: bool = False, extra_images: int = 0, distill: Optional[float] = None):
+                 sample_weights: bool = False, extra_images: int = 0, distill: Optional[float] = None,
+                 sigma_budget_bytes: Optional[int] = None):
         super().__init__()
+        _sigma_budget_mib(sigma_budget_bytes)
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_images = _validate_hard_negatives(extra_images, "extra_images")
@@ -1294,7 +1346,9 @@ class SigLipLoss(nn.Module):
         self.extra_images = extra_images
         self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive,
                                    hard_negatives=hard_negatives, extra_texts=extra_texts, sample_weights=sample_weights,
-                                   extra_images=extra_images, distill=distill)
+                                   extra_images=extra_images, distill=distill, sigma_budget_bytes=sigma_budget_bytes)
+        # bound of the 16-bit sigma operands; steps then run in row panels (as on DDPSigmoidLoss)
+        self.sigma_budget_bytes = sigma_budget_bytes
 
     def forward(self, image_features, text_features, logit_scale, logit_bias, output_dict: bool = False, *,
                 negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
@@ -1330,7 +1384,7 @@ class SigLipLoss(nn.Module):
                 f"(rank={eng.rank}, world_size={eng.world})")
         if logit_bias is None:
             logit_bias = torch.zeros((), device=image_features.device)
-        fused = (eng.world > 1) if self.fused_step is None else bool(self.fused_step)
+        fused = _fused_under_budget(eng, self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
         lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
         loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs,

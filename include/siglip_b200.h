@@ -148,9 +148,44 @@ enum {
                               Composes with SIGLIP_OPT_SAMPLE_IDS, SIGLIP_OPT_SAMPLE_WEIGHTS, metrics, bidir and
                               uneven batches; unavailable with hard negatives / extra texts / extra images and in the
                               host-buffer entries. The gradient kernels are unchanged. Collective. Default 0 */
+  SIGLIP_OPT_SIGMA_BUDGET_MIB = 26, /* bound, in MiB, of the 16-bit sigma operands (the one buffer that grows with B^2).
+                                       0 (default): none, every step as before. Otherwise siglip_fwd_bwd scores the
+                                       rank's R rows in row panels of P rows, P the largest multiple of
+                                       128 x cluster_size (SIGLIP_OPT_CTA_GROUP x SIGLIP_OPT_MCAST) whose buffers fit:
+                                       2 buffers of [P, Tp] at W > 1, 1 at W = 1 (siglip_sigma_panel_rows). A budget that
+                                       holds the whole operands runs the unbounded step unchanged; one below a minimal
+                                       panel is refused (SIGLIP_ERR_INVALID, with the minimum). P depends on the budget,
+                                       the shapes and the cluster options, never on free memory. Composes with every
+                                       other option. Retrieval metrics and per-sample losses are bit-identical to the
+                                       unbounded step, and so is dimg at W = 1 without split-K. At W > 1 the dimg rows
+                                       of panels past 0 add the own chunk's term first rather than last, and split-K
+                                       slices a panel's ragged wave differently: dimg then agrees up to fp32 summation
+                                       order, as loss / dtxt / dt' / dbias always do (DESIGN.md, "Row panels"). siglip_fwd / siglip_forward without save allocate one
+                                       panel at most; siglip_forward with save keeps W whole operands until the backward
+                                       and returns SIGLIP_ERR_STATE when they exceed the budget. The host-buffer entries
+                                       run siglip_fwd_bwd and so run under the budget. Setting it releases the operands
+                                       (and any forward saved for backward). Per rank; default 0 */
   SIGLIP_OPT_AUX_TRACE = 18 /* 1: record globaltimer stamps of the auxiliary warps of CTA 0 for every launch (start,
                                last peer flag seen, jobs done, end of launch); read with siglip_ctx_aux_trace */
 };
+
+/*
+ * Panel height of SIGLIP_OPT_SIGMA_BUDGET_MIB, without a device: `rows` (R) rows of a rank, sigma operands of
+ * `rows_padded` x `cols_padded` (Rp x Tp, max R and max T rounded up to 256) 16-bit elements, `buffers` of them (2 at
+ * W > 1, 1 at W = 1), panels a multiple of `cluster_rows` (128 x cluster size). Returns the panel height: `rows` when one
+ * panel covers the rank (budget 0, or one that holds the whole operands), 0 when the budget is below one minimal panel,
+ * -SIGLIP_ERR_INVALID for invalid arguments. *buffer_rows (optional) receives the rows of each allocated operand.
+ */
+int siglip_sigma_panel_rows(int rows, int rows_padded, int cols_padded, int buffers, int cluster_rows, int budget_mib,
+                            int* buffer_rows);
+
+/*
+ * The same rule for a context's shapes, cluster options and budget: `buffers` sigma operands (0: what siglip_fwd_bwd
+ * keeps, 2 at W > 1 and 1 at W = 1; the world size: what siglip_forward with save keeps). *panel_rows gets the panel
+ * height (0: below one minimal panel), *panels the number of panels, *whole 1 when the budget holds the whole operands
+ * (the unbounded layout). Any output may be null. Host only.
+ */
+int siglip_ctx_sigma_panels(const siglip_ctx* c, int buffers, int* panel_rows, int* panels, int* whole);
 
 /* Library / build identification: "siglip_b200 <version> sm_90a". */
 const char* siglip_version(void);
@@ -168,6 +203,9 @@ int siglip_device_count(void);
  * flags); the [Bp, Bp] 16-bit sigma operands and the fp16 text copies that go with them are allocated on first use: two for
  * the fused step whatever the world size, one per rank for the split forward / backward API (an allocation failure there
  * says how many GiB were needed). On any failure nothing stays allocated. `device` is the CUDA device ordinal.
+ * The first sigma operand is allocated at creation when the device holds it; when it runs out of memory for it, the
+ * context is created all the same and the first step allocates what it needs (under SIGLIP_OPT_SIGMA_BUDGET_MIB: one
+ * panel's worth) or reports the shortfall.
  */
 int siglip_ctx_create(siglip_ctx** out, int device, int rank, int world, int B, int D);
 

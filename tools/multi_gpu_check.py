@@ -66,6 +66,10 @@ def main() -> int:
                     help="also check the per-sample losses (return_sample_losses=True) against the float64 oracle: "
                          "text_loss combines every rank's column partials of the own chunk, uneven batches, hard "
                          "negatives, ids and weights, fused / split / forward-only, and the cross-rank sum identity")
+    ap.add_argument("--row-panels", action="store_true",
+                    help="also check the fused step in row panels (sigma_budget_bytes forcing several panels) against "
+                         "the float64 closed form and against the unbounded step on the same peers: uneven batches "
+                         "(DDPSigmoidLoss), bidir (SigLipLoss), two steps each")
     ap.add_argument("--soak", type=int, default=0,
                     help="N > 0: that many back-to-back steps at the --batch/--dim shape mixing the fused step, the split "
                          "API and forward-only calls; same inputs, so every step of a kind must reproduce its first result "
@@ -309,6 +313,47 @@ def main() -> int:
 
     # ---- per-sample losses: the column sums of my chunk add every rank's fixed-point partials after flag kind 5; the
     # totals over ranks of image_loss and text_loss agree --------------------------------------------------------------
+    if args.row_panels:
+        from distributed_sigmoid_loss_b200 import SigLipLoss
+        for (Bs, D, bidir) in ([[1000 - 100 * (p % 3) for p in range(world)], 136, False],
+                               [[960] * world, 264, True]):   # SigLipLoss: equal batches
+            B = Bs[rank]
+            off = [sum(Bs[:p]) for p in range(world + 1)]
+            g = torch.Generator().manual_seed(7)
+            img_all = torch.nn.functional.normalize(torch.randn(off[-1], D, generator=g)).to(torch.bfloat16)
+            txt_all = torch.nn.functional.normalize(img_all.float() + 0.6 * torch.randn(off[-1], D, generator=g))
+            txt_all = txt_all.to(torch.bfloat16)
+            img = img_all[off[rank]:off[rank + 1]].to(dev).contiguous()
+            txt = txt_all[off[rank]:off[rank + 1]].to(dev).contiguous()
+            tpt, bt = torch.tensor([math.log(10.0)], device=dev), torch.tensor([-10.0], device=dev)
+            outs = []
+            for budget in (None, 1 << 20):
+                mod = (SigLipLoss(rank=rank, world_size=world, bidir=True, sigma_budget_bytes=budget) if bidir else
+                       DDPSigmoidLoss(B, batch_per_rank=Bs, sigma_budget_bytes=budget)).to(dev)
+                eng = mod._cache.get(B, D, dev)
+                if budget:
+                    rows, n, _ = eng.sigma_panels()
+                    assert n >= 2, (rows, n)
+                for rep in range(2):
+                    out = [x.clone() for x in eng.fwd_bwd(img, txt, tpt, bt)]
+                torch.cuda.synchronize()
+                outs.append(out)
+            # every rank's loss over its rows: the closed form over the global batch (uneven: per-rank blocks)
+            x, y = img_all.double(), txt_all.double()
+            z = 10.0 * (x[off[rank]:off[rank + 1]] @ y.T) - 10.0
+            lab = -torch.ones_like(z)
+            lab[torch.arange(B), off[rank] + torch.arange(B)] = 1.0
+            loss_ref = float(torch.nn.functional.softplus(-lab * z).sum() / B)
+            gz = -lab * torch.sigmoid(-lab * z) * 10.0 / B
+            dimg_ref = gz @ y
+            unb, pan = outs
+            report(f"row panels W={world} Bs={Bs} D={D} bidir={bidir} vs float64", dict(
+                loss=abs(float(pan[0]) - loss_ref) / abs(loss_ref),
+                dimg=rel_f(pan[1].cpu(), dimg_ref.float())))
+            report(f"row panels W={world} Bs={Bs} D={D} bidir={bidir} vs unbounded",
+                   {k: rel_f(a.cpu().float(), b.cpu().float()) for k, a, b in
+                    zip(("loss", "dimg", "dtxt", "dt_prime", "dbias"), pan, unb)}, tol=1e-5)
+
     if args.sample_losses:
         sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
         from extra_images_oracle import label_blocks
