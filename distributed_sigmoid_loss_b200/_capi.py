@@ -48,6 +48,7 @@ EXPORTED_SYMBOLS = (
     "siglip_set_sample_weights",
     "siglip_request_metrics",
     "siglip_request_sample_losses",
+    "siglip_request_topk",
     "siglip_fwd_bwd_host",
     "siglip_convert_f32",
     "siglip_host_submit",
@@ -71,6 +72,7 @@ EXPORTED_SYMBOLS = (
     "siglip_debug_set_mailbox",
     "siglip_debug_set_peer_metric_keys",
     "siglip_debug_set_peer_sample_loss_partials",
+    "siglip_debug_set_peer_topk_keys",
     "siglip_debug_set_peer_extra_image_ids",
     "siglip_ctx_aux_trace",
     "siglip_ctx_destroy",
@@ -248,6 +250,10 @@ def lib() -> ctypes.CDLL:
     L.siglip_request_sample_losses.restype = ci
     L.siglip_debug_set_peer_sample_loss_partials.argtypes = [vp, ci, vp, vp]
     L.siglip_debug_set_peer_sample_loss_partials.restype = ci
+    L.siglip_request_topk.argtypes = [vp, ci, vp, vp, vp]
+    L.siglip_request_topk.restype = ci
+    L.siglip_debug_set_peer_topk_keys.argtypes = [vp, ci, vp, vp]
+    L.siglip_debug_set_peer_topk_keys.restype = ci
     L.siglip_ctx_launch_count.argtypes = [vp]
     L.siglip_ctx_launch_count.restype = ctypes.c_ulonglong
     L.siglip_debug_gemm.argtypes = [ci, ci, ci, ci, ci, vp, ctypes.c_longlong, ci, vp, ctypes.c_longlong, ci, vp,

@@ -242,6 +242,16 @@ struct siglip_ctx {
   float* l_img = nullptr;                // [R] image_loss output
   float* l_txt = nullptr;                // [T] text_loss output
   unsigned long long* lsum_step = nullptr;  // fixed-point block of the step being issued (null: no per-sample losses)
+  // top-K retrieval (siglip_request_topk), armed for the next step only; K = 1 runs the metrics path
+  bool topk_armed = false;
+  int topk_k = 0;
+  float* k_recall = nullptr;             // [2k]
+  int64_t* k_i2t = nullptr;              // [ni, k] or null
+  int64_t* k_t2i = nullptr;              // [nt, k] or null
+  bool metrics_step = false;             // the step being issued writes the siglip_request_metrics outputs
+  bool topk1_step = false;               // the step being issued writes K = 1 outputs from the metric keys
+  bool topk_step = false;                // the step being issued fills the K > 1 lists (tk_cols / tk_rows of its parity)
+  unsigned int topk_par = 0;             // ... whose parity is this
   // diagnostics, read from the environment once at context creation (see include/siglip_b200.h)
   bool dbg_no_gstore = false, dbg_no_cvt = false, dbg_loss_waitstats = false;
   // workspaces
@@ -258,6 +268,10 @@ struct siglip_ctx {
   unsigned long long* lsum[2] = {};      // per step parity: [world][Tmax] column sums of every text chunk over my images,
                                          // [Rmax] row sums, then the same layout again for the poison bits
                                          // (lsum_block). world > 1: behind the gathered teacher text (exported)
+  unsigned long long* tk_cols[2] = {};   // per step parity: [world][Tmax][kTopKMax] top-K column lists of every text
+                                         // chunk over my images. world > 1: behind the loss partials (exported);
+                                         // world == 1: allocated by the first siglip_request_topk
+  unsigned long long* tk_rows[2] = {};   // per step parity: [Rmax][kTopKMax] row lists; allocated by the first request
   float* w_all = nullptr;                // [world][w_stride] text weights of every chunk (world > 1): behind the metric
                                          // keys in the exported allocation, sized at creation whatever the options
   float* w_in = nullptr;                 // [w_stride] my text weights, then [R] my image weights, clamped into [0, 1];
@@ -281,6 +295,7 @@ struct siglip_ctx {
   float* loop_zero = nullptr;            // loopback only: [world][Tmax, D] zeros standing in for the peers' contribution slots
   unsigned long long* loop_keys = nullptr;  // loopback only: [world][Tmax] the peers' column partials of my chunk
   unsigned long long* loop_lsums = nullptr;  // loopback only: [world] blocks standing in for the peers' loss partials
+  unsigned long long* loop_topk = nullptr;   // loopback only: [world][Tmax][kTopKMax] the peers' column lists of my chunk
   int64_t* loop_xids = nullptr;          // loopback only: [world][Emax] the peers' published extra-image ids
   float* scalars = nullptr;              // [24] device scalars: host API staging, saved dt'/dbias of the last forward
   unsigned long long* aux_trace = nullptr;  // [kTraceLaunches][16] globaltimer stamps (SIGLIP_OPT_AUX_TRACE)
@@ -300,6 +315,7 @@ struct siglip_ctx {
   const float** mailbox_ptrs_dev = nullptr;  // [world] every rank's (dt', dbias) mailbox
   const unsigned long long** mkey_ptrs_dev = nullptr;  // [2][world] every rank's column partial of my chunk, per parity
   const unsigned long long** lsum_ptrs_dev = nullptr;  // [2][world] every rank's loss column partial of my chunk
+  const unsigned long long** tk_ptrs_dev = nullptr;    // [2][world] every rank's top-K column lists of my chunk
   const int64_t** xid_ptrs_dev = nullptr;    // [2][world] every rank's published extra-image ids, per parity
   unsigned int n_fwd = 0, n_bwd = 0;         // forward / backward passes issued (flag counters)
   unsigned int prewait3 = 0;                 // highest n for which "peers finished backward n" has been waited for
@@ -379,6 +395,8 @@ inline size_t chunk_ids_bytes(const siglip_ctx* c, int rank) {
 int take_ids(siglip_ctx* c) {
   if (c->losses_armed && c->distill)
     return fail(SIGLIP_ERR_STATE, "per-sample losses are unavailable under SIGLIP_OPT_DISTILL");
+  if (c->topk_armed && c->distill)
+    return fail(SIGLIP_ERR_STATE, "top-K retrieval is unavailable under SIGLIP_OPT_DISTILL");
   if (c->sample_ids && !c->ids_set)
     return fail(SIGLIP_ERR_STATE,
                 "SIGLIP_OPT_SAMPLE_IDS is on but siglip_set_sample_ids was not called since the previous step");
@@ -423,6 +441,7 @@ inline unsigned long long peer_timeout_ns(const siglip_ctx* c) {
 
 // ---- retrieval metrics (siglip_request_metrics) ----
 static_assert(siglip::kMetricsMaxWorld == kMaxWorld, "the finalisation kernel takes one batch offset per rank");
+static_assert(siglip::kTopKMax == SIGLIP_TOPK_MAX, "the top-K lists have SIGLIP_TOPK_MAX slots");
 // 64-bit words per step parity: [world][Tmax] column partials (the loss kernel writes one per text of the chunk; the
 // finalisation reads the paired ones), then [Rmax] row keys, then [Emax] extra-image ids of this rank (published for the
 // peers' t2i hit test under SIGLIP_OPT_EXTRA_IMAGE_IDS). Without extra images: [Bmax] row keys and nothing behind.
@@ -526,9 +545,13 @@ int finalize_sample_losses(siglip_ctx* c, unsigned int s, bool signal, cudaStrea
 // zeroed, so that no max of an earlier step survives. Double-buffered by parity: a peer may still read my partials of
 // step n in its finalisation while my step n + 1 writes; by step n + 2 that read is over (DESIGN.md, "In-batch
 // retrieval metrics").
+// A top-K request with K = 1 takes this path too (its outputs are the metric keys'), with or without a metrics request.
 int take_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
   c->mkeys_step = nullptr;
-  if (!c->metrics_armed) return 0;
+  c->topk1_step = c->topk_armed && c->topk_k == 1;
+  if (c->topk1_step) c->topk_armed = false;
+  c->metrics_step = c->metrics_armed;
+  if (!c->metrics_armed && !c->topk1_step) return 0;
   c->metrics_armed = false;
   c->mkeys_step = c->mkeys[s & 1u];
   CK(cudaMemsetAsync(c->mkeys_step, 0, mkeys_block(c) * sizeof(unsigned long long), st));
@@ -541,15 +564,10 @@ int take_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
   }
   return 0;
 }
-// After the step's last loss kernel: combine the keys (W > 1: with every rank's partials of my chunk, flag kind 5) and
-// write the indices and the top-1 rates.
-int finalize_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
-  if (c->mkeys_step == nullptr) return 0;
+// The finalisation arguments of step s: batches, hit rules and flags (shared with the top-K finalisation)
+void fill_metrics_args(const siglip_ctx* c, unsigned int s, siglip::MetricsArgs& a) {
   const int W = c->world;
-  siglip::MetricsArgs a;
   memset(&a, 0, sizeof(a));
-  a.row_keys = c->mkeys_step + mkeys_rows(c);
-  a.col_own = c->mkeys_step + static_cast<size_t>(c->rank) * c->Tmax;
   a.B = c->B;
   a.R = c->R;
   a.rank = c->rank;
@@ -569,30 +587,95 @@ int finalize_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
     a.extra_image_ids = c->extra_image_ids;
     if (W > 1 && c->xid_ptrs_dev != nullptr) a.xids_peers = c->xid_ptrs_dev + static_cast<size_t>(s & 1u) * W;
   }
-  a.top1 = c->m_top1;
-  a.i2t = c->m_i2t;
-  a.t2i = c->m_t2i;
   if (W > 1) {
-    a.col_peers = c->mkey_ptrs_dev + static_cast<size_t>(s & 1u) * W;
     a.sig_ptrs = c->signal_ptrs_dev + 5 * W;
     a.flags_local = c->flags + 5 * kMaxWorld;
     a.value = s;
     a.timeout_ns = peer_timeout_ns(c);
   }
   a.dbg = c->dbg_dev;
+}
+
+// After the step's last loss kernel: combine the keys (W > 1: with every rank's partials of my chunk, flag kind 5) and
+// write the indices and the top-1 rates.
+int finalize_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
+  if (c->mkeys_step == nullptr) return 0;
+  siglip::MetricsArgs a;
+  fill_metrics_args(c, s, a);
+  a.row_keys = c->mkeys_step + mkeys_rows(c);
+  a.col_own = c->mkeys_step + static_cast<size_t>(c->rank) * c->Tmax;
+  if (c->world > 1) a.col_peers = c->mkey_ptrs_dev + static_cast<size_t>(s & 1u) * c->world;
   c->mkeys_step = nullptr;
-  CKI(siglip::launch_metrics_finalize(a, st));
+  // once per set of outputs: siglip_request_metrics', then a K = 1 top-K request's (the same keys; a second raise of
+  // flag kind 5 with the same value changes nothing)
+  for (int out = 0; out < 2; ++out) {
+    if (!(out == 0 ? c->metrics_step : c->topk1_step)) continue;
+    a.top1 = out == 0 ? c->m_top1 : c->k_recall;
+    a.i2t = out == 0 ? c->m_i2t : c->k_i2t;
+    a.t2i = out == 0 ? c->m_t2i : c->k_t2i;
+    CKI(siglip::launch_metrics_finalize(a, st));
+    c->launches++;
+  }
+  c->metrics_step = c->topk1_step = false;
+  return 0;
+}
+
+// ---- top-K retrieval (siglip_request_topk, K > 1) ----
+inline size_t topk_cols_words(const siglip_ctx* c) { return static_cast<size_t>(c->world) * c->Tmax * siglip::kTopKMax; }
+inline size_t topk_rows_words(const siglip_ctx* c) { return static_cast<size_t>(c->Rmax) * siglip::kTopKMax; }
+// byte offset of the two column-list blocks in the exported text allocation: behind the per-sample-loss partials
+inline size_t topk_offset(const siglip_ctx* c) { return lsum_offset(c) + 2 * lsum_block(c) * sizeof(unsigned long long); }
+
+// A top-K step starts: the lists of the step's parity are zeroed (two memsets). Written by the step's loss kernels and
+// read by the peers after flag kind 5 of the step, double-buffered by parity like the metric keys.
+int take_topk(siglip_ctx* c, unsigned int s, cudaStream_t st) {
+  c->topk_step = false;
+  if (!c->topk_armed) return 0;   // (K = 1 was taken by take_metrics)
+  c->topk_armed = false;
+  c->topk_step = true;
+  c->topk_par = s & 1u;
+  CK(cudaMemsetAsync(c->tk_cols[s & 1u], 0, topk_cols_words(c) * sizeof(unsigned long long), st));
+  CK(cudaMemsetAsync(c->tk_rows[s & 1u], 0, topk_rows_words(c) * sizeof(unsigned long long), st));
+  c->launches += 2;
+  if (c->world > 1 && c->sample_ids && c->extra_image_ids && c->R > c->B) {
+    // my extra images' ids for the peers' t2i hit test, where take_metrics publishes them (the same words, if both)
+    CK(cudaMemcpyAsync(c->mkeys[s & 1u] + mkeys_xids(c), c->rids + c->B,
+                       static_cast<size_t>(c->R - c->B) * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
+  }
+  return 0;
+}
+
+// After the metrics finalisation (if any): merge the column lists of my chunk (W > 1: with every rank's, after flag
+// kind 5, which this kernel raises unless the metrics finalisation did), decode both sides and count the recalls.
+int finalize_topk(siglip_ctx* c, unsigned int s, bool signal, cudaStream_t st) {
+  if (!c->topk_step) return 0;
+  const int W = c->world;
+  siglip::TopKArgs a;
+  memset(&a, 0, sizeof(a));
+  fill_metrics_args(c, s, a.m);
+  a.rows = c->tk_rows[s & 1u];
+  a.col_own = c->tk_cols[s & 1u] + static_cast<size_t>(c->rank) * c->Tmax * siglip::kTopKMax;
+  if (W > 1) a.col_peers = c->tk_ptrs_dev + static_cast<size_t>(s & 1u) * W;
+  a.k = c->topk_k;
+  a.signal = signal ? 1 : 0;
+  a.recall = c->k_recall;
+  a.i2t = c->k_i2t;
+  a.t2i = c->k_t2i;
+  c->topk_step = false;
+  CKI(siglip::launch_topk_finalize(a, st));
   c->launches++;
   return 0;
 }
 
-// The step's detached outputs, after its last loss kernel: the metrics, then the per-sample losses (which raise flag
-// kind 5 themselves when no metrics finalisation did)
+// The step's detached outputs, after its last loss kernel: the metrics, then the top-K lists, then the per-sample
+// losses; the first finalisation at W > 1 raises flag kind 5
 int finalize_step_outputs(siglip_ctx* c, unsigned int s, cudaStream_t st) {
   const bool metrics = c->mkeys_step != nullptr;
+  const bool topk = c->topk_step;
   int rc;
   if ((rc = finalize_metrics(c, s, st))) return rc;
-  return finalize_sample_losses(c, s, !metrics, st);
+  if ((rc = finalize_topk(c, s, !metrics, st))) return rc;
+  return finalize_sample_losses(c, s, !metrics && !topk, st);
 }
 
 // Sigma operand + fp16 text copy number i, allocated on first use. The fused step needs two (own chunk, chunk in
@@ -845,6 +928,13 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
     p.sl_rows = c->lsum_step + lsum_rows(c) + r0;
     p.sl_cols = c->lsum_step + static_cast<size_t>(cidx) * c->Tmax + c0;
     p.sl_poison = static_cast<long long>(lsum_half(c));
+  }
+  if (c->topk_step) {   // a top-K step (K > 1): the kModeTopK kernel fills the row / column lists
+    p.tk_rows = c->tk_rows[c->topk_par] + static_cast<size_t>(r0) * siglip::kTopKMax;
+    p.tk_cols = c->tk_cols[c->topk_par] + (static_cast<size_t>(cidx) * c->Tmax + c0) * siglip::kTopKMax;
+    p.tk_k = c->topk_k;
+    p.row_off = c->off[c->rank] + r0;
+    p.col_off = c->toff[cidx] + c0;
   }
   p.partials = c->partials;
   p.accumulate_partials = first ? 0 : 1;  // the first chunk of a forward overwrites every slot of the grid
@@ -1224,6 +1314,7 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
   const unsigned int s = ++c->n_fwd;
   if ((rc = take_metrics(c, s, st))) return rc;
   if ((rc = take_sample_losses(c, s, st))) return rc;
+  if ((rc = take_topk(c, s, st))) return rc;
   // the saved state is being overwritten (a forward without save still replaces my gathered text slot, which the
   // backward of a multi-rank job reads for the positive-pair term); valid again once a saving forward is enqueued
   if (save || c->world > 1) c->gen = 0;
@@ -1418,6 +1509,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   const bool ik = c->inkernel_sync != 0;
   if ((rc = take_metrics(c, s, st))) return rc;
   if ((rc = take_sample_losses(c, s, st))) return rc;
+  if ((rc = take_topk(c, s, st))) return rc;
   c->gen = 0;                       // the sigma operands of a split forward (if any) are overwritten
   c->saved_f16 = c->input_f16;
   if ((rc = ensure_g(c, 0, pn.buf_rows))) return rc;
@@ -1812,8 +1904,10 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     const size_t t_bytes = teacher_stride(c) * world * sizeof(__nv_bfloat16);
     // and the per-sample-loss partials behind that (sized whatever the options: a peer's offsets cannot depend on them)
     const size_t l_bytes = 2 * lsum_block(c) * sizeof(unsigned long long);
+    // and the top-K column lists behind those (sized whatever the options, for the same reason)
+    const size_t k_bytes = 2 * topk_cols_words(c) * sizeof(unsigned long long);
     CK(alloc(reinterpret_cast<void**>(&c->txt_all), stride * world * sizeof(__nv_bfloat16) + world * ids_slot_bytes +
-                                                        mkeys_bytes + w_bytes + t_bytes + l_bytes));
+                                                        mkeys_bytes + w_bytes + t_bytes + l_bytes + k_bytes));
     c->ids_all = reinterpret_cast<int64_t*>(c->txt_all + stride * world);   // 16-byte aligned: D % 8 == 0
     c->mkeys[0] = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(c->txt_all) + mkeys_offset(c));
     c->mkeys[1] = c->mkeys[0] + mkeys_block(c);
@@ -1822,6 +1916,8 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
       c->ttxt_all = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<char*>(c->txt_all) + teacher_offset(c));
     c->lsum[0] = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(c->txt_all) + lsum_offset(c));
     c->lsum[1] = c->lsum[0] + lsum_block(c);
+    c->tk_cols[0] = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(c->txt_all) + topk_offset(c));
+    c->tk_cols[1] = c->tk_cols[0] + topk_cols_words(c);
     CK(alloc(reinterpret_cast<void**>(&c->slots), stride * world * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dimg_acc), static_cast<size_t>(c->R) * D * sizeof(float)));
     CK(alloc(reinterpret_cast<void**>(&c->dtxt_acc), static_cast<size_t>(c->T) * D * sizeof(float)));
@@ -1831,6 +1927,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     CK(alloc(reinterpret_cast<void**>(&c->mailbox_ptrs_dev), world * sizeof(float*)));
     CK(alloc(reinterpret_cast<void**>(&c->mkey_ptrs_dev), 2 * world * sizeof(unsigned long long*)));
     CK(alloc(reinterpret_cast<void**>(&c->lsum_ptrs_dev), 2 * world * sizeof(unsigned long long*)));
+    CK(alloc(reinterpret_cast<void**>(&c->tk_ptrs_dev), 2 * world * sizeof(unsigned long long*)));
     if (c->ximg) CK(alloc(reinterpret_cast<void**>(&c->xid_ptrs_dev), 2 * world * sizeof(int64_t*)));
     const float* fin[2] = {c->dtxt_acc, c->slots + rank * stride};
     CK(cudaMemcpy(c->final_ptrs_dev, fin, sizeof(fin), cudaMemcpyHostToDevice));
@@ -2122,6 +2219,18 @@ static int publish_peer_tables(siglip_ctx* c) {
       ls[q * c->world + p] = blk + static_cast<size_t>(c->rank) * c->Tmax;
     }
   CK(cudaMemcpy(c->lsum_ptrs_dev, ls.data(), ls.size() * sizeof(unsigned long long*), cudaMemcpyHostToDevice));
+  // every rank's top-K column lists of my chunk, per step parity (loopback: the stand-ins
+  // siglip_debug_set_peer_topk_keys seeds)
+  std::vector<const unsigned long long*> tk(2 * c->world);
+  for (int q = 0; q < 2; ++q)
+    for (int p = 0; p < c->world; ++p) {
+      const unsigned long long* blk =
+          reinterpret_cast<const unsigned long long*>(reinterpret_cast<const char*>(c->peer_txt[p]) + topk_offset(c)) +
+          q * topk_cols_words(c) + static_cast<size_t>(c->rank) * c->Tmax * siglip::kTopKMax;
+      if (c->loopback && p != c->rank) blk = c->loop_topk + static_cast<size_t>(p) * c->Tmax * siglip::kTopKMax;
+      tk[q * c->world + p] = blk;
+    }
+  CK(cudaMemcpy(c->tk_ptrs_dev, tk.data(), tk.size() * sizeof(unsigned long long*), cudaMemcpyHostToDevice));
   if (c->xid_ptrs_dev != nullptr) {
     // every rank's published extra-image ids, per step parity (loopback: the stand-ins
     // siglip_debug_set_peer_extra_image_ids seeds)
@@ -2322,6 +2431,49 @@ int siglip_request_sample_losses(siglip_ctx* c, float* image_loss, float* text_l
   return 0;
 }
 
+int siglip_request_topk(siglip_ctx* c, int k, float* recall, int64_t* i2t_topk, int64_t* t2i_topk) {
+  if (c == nullptr || recall == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument (recall is required)");
+  if (k < 1 || k > SIGLIP_TOPK_MAX) return fail(SIGLIP_ERR_INVALID, "k must be in 1 .. SIGLIP_TOPK_MAX");
+  if (c->distill) return fail(SIGLIP_ERR_STATE, "top-K retrieval is unavailable under SIGLIP_OPT_DISTILL");
+  if (k > 1 && c->tk_rows[0] == nullptr) {
+    // the row lists (and on one rank the column lists ahead of them) are allocated by the first request, so a context
+    // that never asks holds exactly the workspace it held without them; allowed inside a CUDA-graph capture
+    const size_t cols = (c->world == 1) ? 2 * topk_cols_words(c) : 0;
+    const size_t bytes = (cols + 2 * topk_rows_words(c)) * sizeof(unsigned long long);
+    CK(cudaSetDevice(c->device));
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    CK(cudaThreadExchangeStreamCaptureMode(&mode));
+    unsigned long long* words = nullptr;
+    const cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&words), bytes);
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    CK(e);
+    if (c->world == 1) {
+      c->tk_cols[0] = words + 2 * topk_rows_words(c);   // behind the row lists, which free_ctx releases
+      c->tk_cols[1] = c->tk_cols[0] + topk_cols_words(c);
+    }
+    c->tk_rows[0] = words;
+    c->tk_rows[1] = words + topk_rows_words(c);
+    c->workspace_bytes += bytes;
+  }
+  c->topk_k = k;
+  c->k_recall = recall;
+  c->k_i2t = i2t_topk;
+  c->k_t2i = t2i_topk;
+  c->topk_armed = true;
+  return 0;
+}
+
+int siglip_debug_set_peer_topk_keys(siglip_ctx* c, int peer, const uint64_t* keys_dev, void* cuda_stream) {
+  if (c == nullptr || keys_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->loopback || peer < 0 || peer >= c->world || peer == c->rank)
+    return fail(SIGLIP_ERR_INVALID, "siglip_debug_set_peer_topk_keys needs a loopback context and a peer rank != own rank");
+  CK(cudaSetDevice(c->device));
+  CK(cudaMemcpyAsync(c->loop_topk + static_cast<size_t>(peer) * c->Tmax * siglip::kTopKMax, keys_dev,
+                     static_cast<size_t>(c->T) * siglip::kTopKMax * sizeof(uint64_t), cudaMemcpyDeviceToDevice,
+                     static_cast<cudaStream_t>(cuda_stream)));
+  return 0;
+}
+
 int siglip_debug_set_peer_sample_loss_partials(siglip_ctx* c, int peer, const int64_t* partials_dev,
                                                void* cuda_stream) {
   if (c == nullptr || partials_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
@@ -2452,6 +2604,8 @@ int siglip_host_submit_grads(siglip_ctx* c, const void* img_host, const void* tx
   if (c->losses_armed)
     return fail(SIGLIP_ERR_STATE,
                 "the host-buffer entries return no per-sample losses: siglip_request_sample_losses is armed");
+  if (c->topk_armed)
+    return fail(SIGLIP_ERR_STATE, "the host-buffer entries return no top-K lists: siglip_request_topk is armed");
   if (c->sample_weights)
     return fail(SIGLIP_ERR_STATE,
                 "the host-buffer entries take no sample weights: unavailable under SIGLIP_OPT_SAMPLE_WEIGHTS");
@@ -2601,6 +2755,8 @@ int siglip_debug_loopback(siglip_ctx* c) {
     CK(cudaMemset(c->loop_keys, 0, static_cast<size_t>(c->world) * c->Tmax * 8));
     CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_lsums), static_cast<size_t>(c->world) * lsum_block(c) * 8));
     CK(cudaMemset(c->loop_lsums, 0, static_cast<size_t>(c->world) * lsum_block(c) * 8));
+    CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_topk), topk_cols_words(c) * 8));
+    CK(cudaMemset(c->loop_topk, 0, topk_cols_words(c) * 8));
     if (c->Emax > 0) {
       CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_xids), static_cast<size_t>(c->world) * c->Emax * 8));
       CK(cudaMemset(c->loop_xids, 0, static_cast<size_t>(c->world) * c->Emax * 8));
@@ -2958,6 +3114,9 @@ void free_ctx(siglip_ctx* c) {
   cudaFree(c->loop_lsums);
   if (c->world == 1) cudaFree(c->lsum[0]);    // world > 1: part of txt_all
   cudaFree(c->lsum_ptrs_dev);
+  cudaFree(c->loop_topk);
+  cudaFree(c->tk_rows[0]);                    // allocated by the first request (world == 1: with the column lists)
+  cudaFree(c->tk_ptrs_dev);
   cudaFree(c->scalars);
   cudaFree(c->aux_trace);
   cudaFree(c->splitk_ws);

@@ -576,6 +576,121 @@ __device__ __forceinline__ void tile_metrics(const float (&acc)[64], int row_lo,
   }
 }
 
+// -------------------------------------------------------------------------------------------------
+// Top-K retrieval (kModeTopK): per row and per column a list of kTopKMax 64-bit keys (the metric keys above), sorted
+// best first, of which the first K are filled; 0 = empty slot. A candidate c enters with a chain of atomic maxima:
+// for s = 0 .. K-1, old = atom.max(&list[s], c), and if old < c the displaced key old is carried on instead; the chain
+// ends when the carried key is 0. Every atomic keeps the larger key and carries the smaller, so no key is lost or
+// duplicated, slots never decrease, and the list stays sorted; the keys are distinct, so whatever the order of the
+// atomics the final list is exactly the top K of its candidates (DESIGN.md, "Top-K retrieval").
+// Prefilter: a candidate not above the list's K-th slot cannot enter. That slot is read once per fragment row and tile
+// and once per column and 32-column slab with a plain relaxed load (a stale value is a lower bound: slots only grow),
+// and raised by what each chain learns (the key carried out of slot K-1 is below that slot).
+// -------------------------------------------------------------------------------------------------
+__device__ __forceinline__ unsigned long long atom_max_u64(unsigned long long* p, unsigned long long v) {
+  unsigned long long old;
+  asm volatile("atom.relaxed.gpu.global.max.u64 %0, [%1], %2;" : "=l"(old) : "l"(p), "l"(v) : "memory");
+  return old;
+}
+
+// volatile, so that it is read anew on every tile (consecutive tiles of a CTA share their rows: a pure load would be
+// hoisted out of the tile loop); no memory clobber, so a slab's 8 loads issue back to back ahead of its chains
+__device__ __forceinline__ unsigned long long topk_floor(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p));
+  return v;
+}
+
+// Insert c into a list of k slots. Returns a key below the final list[k - 1], or 0 when the chain ended early.
+__device__ __forceinline__ unsigned long long topk_insert(unsigned long long* list, int k, unsigned long long c) {
+  for (int s = 0; s < k; ++s) {
+    const unsigned long long old = atom_max_u64(list + s, c);
+    if (old < c) {
+      c = old;
+      if (c == 0ull) return 0ull;
+    }
+  }
+  return c;
+}
+
+// Rows: the concurrent clusters of a step work on the tiles of one row panel (the schedule is row-major), so a row's
+// list has no useful floor yet when most of its tiles arrive. Each quad therefore selects its row's keys of the tile
+// best first, one per round (round r: the quad's largest key below the one of round r - 1, shfl_xor 1, 2), and its
+// first thread inserts it; the rounds stop at the list's floor, or after K. Columns, per 32-column slab: each thread
+// offers its 2 rows of each of its 8 columns (a column's tiles arrive panel after panel, behind an established floor).
+// Rows >= M and columns >= N are never candidates.
+__device__ __forceinline__ void tile_topk(const float (&acc)[64], int row_lo, int col_base, int c_lo, int M, int N,
+                                          int lane, const KernelParams& p) {
+  const int k = p.tk_k;
+  const bool v0 = row_lo < M, v1 = row_lo + 8 < M;
+  const int lead = lane & ~3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const bool valid = h ? v1 : v0;
+    const int row = min(row_lo + 8 * h, M - 1);
+    unsigned long long thr = valid ? topk_floor(p.tk_rows + static_cast<size_t>(row) * kTopKMax + k - 1) : ~0ull;
+    thr = __shfl_sync(0xffffffffu, thr, lead);   // one floor per quad
+    // the previous round's key as (value, column): the scan compares the accumulator in place (64-bit keys of all 32
+    // elements would be hoisted out of the rounds into registers); equal values order by column as the keys do
+    // (+inf, -1): no bound in round 0; (-inf, INT_MAX): nothing selected. A NaN logit compares false and is never
+    // selected here (the row side of a non-finite step is undefined)
+    float bv = INFINITY;
+    int bc = -1;
+    for (int r = 0; r < k; ++r) {
+      float cv = -INFINITY;
+      int cc = 0x7fffffff;
+#pragma unroll
+      for (int i = 0; i < 64; ++i) {
+        if (((i >> 1) & 1) != h) continue;
+        const int col = col_base + 8 * (i >> 2) + c_lo + (i & 1);
+        const float v = acc[i];
+        if (col < N && (v < bv || (v == bv && col > bc)) && (v > cv || (v == cv && col < cc))) {
+          cv = v;
+          cc = col;
+        }
+      }
+      unsigned long long best = (cc != 0x7fffffff) ? metric_key(cv, p.col_off + cc) : 0ull;
+      best = max_u64(best, __shfl_xor_sync(0xffffffffu, best, 1));
+      best = max_u64(best, __shfl_xor_sync(0xffffffffu, best, 2));
+      const bool go = best > thr;   // the same in the 4 threads of a quad
+      if (!__any_sync(0xffffffffu, go)) break;
+      if (go && lane == lead) thr = max_u64(thr, topk_insert(p.tk_rows + static_cast<size_t>(row) * kTopKMax, k, best));
+      thr = __shfl_sync(0xffffffffu, thr, lead);
+      if (go) {   // the next round looks below the key just taken
+        const uint32_t ord = static_cast<uint32_t>(best >> 32);
+        bv = __uint_as_float(ord ^ ((ord >> 31) ? 0x80000000u : 0xFFFFFFFFu));
+        bc = static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(best)) - p.col_off;
+      } else {    // a quad that stopped offers nothing more
+        bv = -INFINITY;
+        bc = 0x7fffffff;
+      }
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < kTileN / 32; ++c) {
+    unsigned long long thr[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const int col = col_base + 32 * c + 8 * (q >> 1) + c_lo + (q & 1);
+      thr[q] = (col < N) ? topk_floor(p.tk_cols + static_cast<size_t>(col) * kTopKMax + k - 1) : ~0ull;
+    }
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const int col = col_base + 32 * c + 8 * (q >> 1) + c_lo + (q & 1);
+      unsigned long long* list = p.tk_cols + static_cast<size_t>(min(col, N - 1)) * kTopKMax;
+      const int i = 16 * c + 4 * (q >> 1) + (q & 1);
+      if (v0) {
+        const unsigned long long key = metric_key(acc[i], p.row_off + row_lo);
+        if (key > thr[q]) thr[q] = max_u64(thr[q], topk_insert(list, k, key));
+      }
+      if (v1) {
+        const unsigned long long key = metric_key(acc[i + 2], p.row_off + row_lo + 8);
+        if (key > thr[q]) topk_insert(list, k, key);
+      }
+    }
+  }
+}
+
 // Epilogue of the out kernel: one row of the fragment (h = 0: row_lo, 1: row_lo + 8), kN / 8 column pairs (16 for
 // 128-column tiles, 32 for 256-column ones).
 //   val = scale * (acc * acc_scale + fix * x[row, col]) (+ add_src[row, col]);  written as fp32 or bf16
@@ -858,6 +973,9 @@ __device__ __forceinline__ void sample_loss_add(unsigned long long* w, long long
 //            (lanes xor 16, 8, 4, as in tile_metrics) that leaves lane l with column q = l >> 2 of its lane % 4 group,
 //            one red.add per lane and slab.
 // Rows >= M and columns >= N add nothing (their terms are masked to 0 and their words do not exist).
+// kTopK (kModeTopK): the top-K insertion (tile_topk) runs first, after the argmax keys, and the fixed-point sums are a
+// runtime option (p.sl_rows); the three sums, g_diag and the sigma operand are unchanged.
+template <bool kTopK = false>
 __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, const float (&acc)[kTileN / 2],
                                                      const CUtensorMap* tmG, uint32_t staging_base, int warp, int wg,
                                                      int lane, int row0, int col_base, int row_lo, int c_lo,
@@ -865,6 +983,8 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
                                                      uint64_t policy, float& s_sp, float& c_sp, float& s_g, float& c_g,
                                                      float& s_gs, float& c_gs) {
   if (p.row_keys != nullptr) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
+  if constexpr (kTopK) tile_topk(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
+  const bool sl = !kTopK || p.sl_rows != nullptr;
   float acc_sp = 0.f, acc_g = 0.f, acc_gs = 0.f;
   const bool edge = (row0 + kBlockM > pr.M) || (col_base + kTileN > pr.N);
   const bool diag = p.own_chunk && (row0 == col_base);
@@ -932,27 +1052,29 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
       loss_slab<true, true, true>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag,
                                   slab_diag, pos, acc_sp, acc_g, acc_gs, cw, rw0, rw1, lrow, lcol);
     }
-    // reduce-scatter: after the step over lane bit m, lcol[0 .. h) holds the columns q = k + (bit m of lane ? h : 0)
+    if (sl) {
+      // reduce-scatter: after the step over lane bit m, lcol[0 .. h) holds the columns q = k + (bit m of lane ? h : 0)
 #pragma unroll
-    for (int h = 4, m = 16; h >= 1; h >>= 1, m >>= 1) {
-      const bool hi = (lane & m) != 0;
+      for (int h = 4, m = 16; h >= 1; h >>= 1, m >>= 1) {
+        const bool hi = (lane & m) != 0;
 #pragma unroll
-      for (int k = 0; k < h; ++k) {
-        const float send = hi ? lcol[k] : lcol[k + h];
-        const float keep = hi ? lcol[k + h] : lcol[k];
-        lcol[k] = keep + __shfl_xor_sync(0xffffffffu, send, m);
+        for (int k = 0; k < h; ++k) {
+          const float send = hi ? lcol[k] : lcol[k + h];
+          const float keep = hi ? lcol[k + h] : lcol[k];
+          lcol[k] = keep + __shfl_xor_sync(0xffffffffu, send, m);
+        }
       }
+      const int q = lane >> 2;
+      const int col = col0 + 8 * (q >> 1) + c_lo + (q & 1);
+      if (col < pr.N) sample_loss_add(p.sl_cols + col, p.sl_poison, lcol[0]);
     }
-    const int q = lane >> 2;
-    const int col = col0 + 8 * (q >> 1) + c_lo + (q & 1);
-    if (col < pr.N) sample_loss_add(p.sl_cols + col, p.sl_poison, lcol[0]);
   }
 #pragma unroll
   for (int o = 1; o <= 2; o <<= 1) {
     lrow[0] += __shfl_xor_sync(0xffffffffu, lrow[0], o);
     lrow[1] += __shfl_xor_sync(0xffffffffu, lrow[1], o);
   }
-  if ((lane & 3) == 0) {
+  if (sl && (lane & 3) == 0) {
     if (row_lo < pr.M) sample_loss_add(p.sl_rows + row_lo, p.sl_poison, lrow[0]);
     if (row_lo + 8 < pr.M) sample_loss_add(p.sl_rows + row_lo + 8, p.sl_poison, lrow[1]);
   }
@@ -979,6 +1101,8 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
 // kMode = kModeSampleLoss: the loss kernel of a step with per-sample losses, its own instantiation (both stage counts,
 // 128-column tiles, K-major operands): the kModeLoss epilogue plus the fixed-point row / column sums
 // (sample_loss_epilogue); ids, weights and metrics are runtime options there.
+// kMode = kModeTopK: the loss kernel of a top-K step, its own instantiation like kModeSampleLoss: the top-K insertion
+// (tile_topk), then the kModeSampleLoss epilogue; ids, weights, metrics and the per-sample-loss sums are runtime options.
 template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false,
           bool kWeights = false, int kTileNT = kTileN>
 __global__ void __launch_bounds__(kNumThreads, 1)
@@ -996,6 +1120,8 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
                 "the distillation kernel takes ids, weights and metrics as runtime options");
   static_assert(kMode != kModeSampleLoss || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
                 "the per-sample-loss kernel takes ids, weights and metrics as runtime options");
+  static_assert(kMode != kModeTopK || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
+                "the top-K kernel takes ids, weights, metrics and per-sample losses as runtime options");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -1243,7 +1369,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
   mma_loop<T, TA, TB, kCS, C::kStageBytes, kTileNT>(acc, kb0, kb1, stage, phase, C::kStages, adesc0, bdesc0, a_adv, \
                                                     b_adv, full0, empty0, lane, p.dbg, t, w_full_p)
         const int sel = pr.a_mn * 2 + pr.b_mn;
-        if constexpr (kMode == kModeDistill || kMode == kModeSampleLoss) {
+        if constexpr (kMode == kModeDistill || kMode == kModeSampleLoss || kMode == kModeTopK) {
           // the loss operands (student and teacher) are always K-major: no MN-major variants in this instantiation
           if (pr.ab_f16)
             SIGLIP_MMA_LOOP(1, 0, 0);
@@ -1280,6 +1406,9 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       } else if constexpr (kMode == kModeSampleLoss) {
         sample_loss_epilogue(p, acc, &tmG, staging_base, warp, wg, lane, row0, col_base, row_lo, c_lo, pr, t_eff, bias,
                              tl, bl, g_store_policy, s_sp, c_sp, s_g, c_g, s_gs, c_gs);
+      } else if constexpr (kMode == kModeTopK) {
+        sample_loss_epilogue<true>(p, acc, &tmG, staging_base, warp, wg, lane, row0, col_base, row_lo, c_lo, pr, t_eff,
+                                   bias, tl, bl, g_store_policy, s_sp, c_sp, s_g, c_g, s_gs, c_gs);
       } else if constexpr (kMode == kModeLoss) {
         // argmax keys first, on the raw accumulator: whichever path each slab then takes below
         if constexpr (kMetrics) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
@@ -2018,6 +2147,141 @@ __global__ void __launch_bounds__(kSampleLossThreads) sample_loss_finalize_kerne
   }
 }
 
+// Finalisation of a top-K step (TopKArgs). Like metrics_finalize_kernel it never triggers
+// griddepcontrol.launch_dependents, and at W > 1 it reads the peers' lists of the step only after their flag kind 5 of
+// the step: the same protocol as the metric keys (DESIGN.md, "Top-K retrieval").
+constexpr int kTopKThreads = 1024;
+
+__global__ void __launch_bounds__(kTopKThreads) topk_finalize_kernel(const TopKArgs t) {
+  const MetricsArgs& a = t.m;
+  // first[side][s]: samples whose first hit is at rank s (s = K: no hit among the K)
+  __shared__ unsigned int first[2][kTopKMax + 1];
+  const int tid = threadIdx.x;
+  if (tid < 2 * (kTopKMax + 1)) first[tid / (kTopKMax + 1)][tid % (kTopKMax + 1)] = 0u;
+  if (a.world > 1) {
+    if (tid < a.world) {
+      if (t.signal) {
+        __threadfence_system();   // my lists (written by the step's loss kernels) before the flag
+        asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(a.sig_ptrs[tid]), "r"(a.value) : "memory");
+      }
+      uint64_t t0 = 0;
+      uint32_t spins = 0;
+      while (true) {
+        unsigned int v;
+        asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(a.flags_local + tid) : "memory");
+        if (v >= a.value) break;
+        if ((++spins & 0xffu) == 0) {
+          const uint64_t now = globaltimer_ns();
+          if (t0 == 0) t0 = now;
+          if (now - t0 > a.timeout_ns) {
+            if (a.dbg != nullptr) {
+              a.dbg->block = tid;
+              a.dbg->aux0 = v;
+              a.dbg->aux1 = a.value;
+              a.dbg->code = 10;
+              __threadfence_system();
+            }
+            __trap();
+          }
+        }
+      }
+      __threadfence();   // order the other threads' peer reads after the observed flags
+    }
+  }
+  __syncthreads();
+  const int K = t.k;
+  // the images and texts ranked, as in metrics_finalize_kernel
+  const int nt = a.extra_ids ? a.T : a.B;
+  const int ni = a.extra_image_ids ? a.R : a.B;
+  const int n = ni > nt ? ni : nt;
+  unsigned int cnt[2][kTopKMax + 1] = {};   // per thread, by first-hit rank (K: none)
+  for (int i = tid; i < n; i += kTopKThreads) {
+    unsigned long long key[kTopKMax];
+    if (i < ni) {
+#pragma unroll
+      for (int s = 0; s < kTopKMax; ++s) key[s] = (s < K) ? t.rows[static_cast<size_t>(i) * kTopKMax + s] : 0ull;
+      int f = K;
+#pragma unroll
+      for (int s = 0; s < kTopKMax; ++s) {
+        if (s < K) {
+          const int j = key_index(key[s]);
+          if (t.i2t) t.i2t[static_cast<size_t>(i) * K + s] = j;
+          if (f == K && j >= 0 && metrics_i2t_hit(a, i, j)) f = s;
+        }
+      }
+#pragma unroll
+      for (int s = 0; s <= kTopKMax; ++s) cnt[0][s] += (f == s);
+    }
+    if (i >= nt) continue;
+    if (a.world == 1) {
+#pragma unroll
+      for (int s = 0; s < kTopKMax; ++s) key[s] = (s < K) ? t.col_own[static_cast<size_t>(i) * kTopKMax + s] : 0ull;
+    } else {
+      // K-way merge of the W sorted lists (keys of different ranks are distinct: each covers that rank's images): the
+      // head of every list is kept, and only the list whose head was taken is read again
+      int head[kMetricsMaxWorld] = {};
+      unsigned long long hv[kMetricsMaxWorld];
+      auto load = [&](int q) -> unsigned long long {
+        if (head[q] >= K) return 0ull;
+        const size_t o = static_cast<size_t>(i) * kTopKMax + head[q];
+        if (q == a.rank) return t.col_own[o];
+        unsigned long long v;
+        asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(t.col_peers[q] + o) : "memory");
+        return v;
+      };
+      for (int q = 0; q < a.world; ++q) hv[q] = load(q);
+#pragma unroll
+      for (int s = 0; s < kTopKMax; ++s) {
+        unsigned long long best = 0ull;
+        int bq = -1;
+        if (s < K) {
+          for (int q = 0; q < a.world; ++q) {
+            if (hv[q] > best) {
+              best = hv[q];
+              bq = q;
+            }
+          }
+          if (bq >= 0) {
+            ++head[bq];
+            hv[bq] = load(bq);
+          }
+        }
+        key[s] = best;
+      }
+    }
+    int f = K;
+#pragma unroll
+    for (int s = 0; s < kTopKMax; ++s) {
+      if (s < K) {
+        const int g = key_index(key[s]);
+        if (t.t2i) t.t2i[static_cast<size_t>(i) * K + s] = g;
+        if (f == K && g >= 0 && metrics_t2i_hit(a, i, g)) f = s;
+      }
+    }
+#pragma unroll
+    for (int s = 0; s <= kTopKMax; ++s) cnt[1][s] += (f == s);
+  }
+  // integer counts: the sum does not depend on the order
+#pragma unroll
+  for (int d = 0; d < 2; ++d) {
+#pragma unroll
+    for (int s = 0; s <= kTopKMax; ++s) {
+      unsigned int v = cnt[d][s];
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if ((tid & 31) == 0 && v != 0u) atomicAdd(&first[d][s], v);
+    }
+  }
+  __syncthreads();
+  // recall@k = (samples with their first hit at a rank < k) / samples: integer counts, as the top-1 rate
+  if (tid < 2) {
+    unsigned int hits = 0u;
+    for (int s = 0; s < K; ++s) {
+      hits += first[tid][s];
+      t.recall[tid * K + s] = static_cast<float>(hits) / static_cast<float>(tid == 0 ? ni : nt);
+    }
+  }
+}
+
 // -------------------------------------------------------------------------------------------------
 // L2 normalisation fused around the loss (SURVEY.md §8f-1: the step the reference's callers run right before it,
 // test_distributed_sigmoid_loss.py:99-101). One warp per row; HBM-bound: coalesced 16-byte accesses, fp32 math.
@@ -2325,6 +2589,20 @@ int launch_gemm(int cta_group, int mode, int stages, int mcast, int tile_n, cons
       default: return launch_impl<kModeDistill, kDistillStages, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
     }
   }
+  if (mode == kModeLoss && p.tk_rows != nullptr) {   // top-K (with or without per-sample losses): kModeTopK
+    const bool s4 = stages == 4;
+    switch (cluster_size(cta_group, mcast)) {
+      case 4:
+        return s4 ? launch_impl<kModeTopK, 4, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeTopK, 6, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      case 2:
+        return s4 ? launch_impl<kModeTopK, 4, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeTopK, 6, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      default:
+        return s4 ? launch_impl<kModeTopK, 4, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeTopK, 6, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+    }
+  }
   if (mode == kModeLoss && p.sl_rows != nullptr) {   // per-sample losses: kModeSampleLoss, 4 or 6 stages
     const bool s4 = stages == 4;
     switch (cluster_size(cta_group, mcast)) {
@@ -2430,6 +2708,11 @@ int launch_metrics_finalize(const MetricsArgs& a, cudaStream_t stream) {
 
 int launch_sample_loss_finalize(const SampleLossArgs& a, cudaStream_t stream) {
   sample_loss_finalize_kernel<<<1, kSampleLossThreads, 0, stream>>>(a);
+  return static_cast<int>(cudaGetLastError());
+}
+
+int launch_topk_finalize(const TopKArgs& a, cudaStream_t stream) {
+  topk_finalize_kernel<<<1, kTopKThreads, 0, stream>>>(a);
   return static_cast<int>(cudaGetLastError());
 }
 

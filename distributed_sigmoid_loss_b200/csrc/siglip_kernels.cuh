@@ -168,12 +168,24 @@ struct KernelParams {
   unsigned long long* sl_rows;   // [M]: sums of this rank's images over the chunk's texts
   unsigned long long* sl_cols;   // [N]: sums of the chunk's texts over this rank's images
   long long sl_poison;           // distance in words from a sum to its poison word
+  // Top-K retrieval (siglip_request_topk, K > 1). Appended last like the fields above. Non-null tk_rows selects the
+  // kModeTopK loss kernel: besides the kModeSampleLoss epilogue (whose sums are then optional) it inserts every
+  // candidate key above a list's current K-th entry into that row's / column's sorted list of kTopKMax slots with a
+  // chain of atomic maxima (tile_topk). Keys as row_keys / col_keys, global indices from row_off / col_off.
+  unsigned long long* tk_rows;   // [M][kTopKMax]: the best texts of each image of this rank
+  unsigned long long* tk_cols;   // [N][kTopKMax]: the best images of each text of the chunk, over this rank's images
+  int tk_k;                      // K in 2 .. kTopKMax: slots of each list that are filled
 };
 
 // kModeDistill: the loss kernel of a distillation step (KernelParams::k_teacher > 0), its own instantiation
 // kModeSampleLoss: the loss kernel of a step with per-sample losses (KernelParams::sl_rows != null), its own
 // instantiation; ids, weights and metric keys are runtime options in it
-enum KernelMode { kModeLoss = 0, kModeOut = 1, kModeDistill = 2, kModeSampleLoss = 3 };
+// kModeTopK: the loss kernel of a top-K step (KernelParams::tk_rows != null), its own instantiation; ids, weights,
+// metric keys and per-sample-loss sums are runtime options in it
+enum KernelMode { kModeLoss = 0, kModeOut = 1, kModeDistill = 2, kModeSampleLoss = 3, kModeTopK = 4 };
+
+// Top-K retrieval: slots of every list (SIGLIP_TOPK_MAX), whatever K the step asks
+constexpr int kTopKMax = 10;
 
 // Per-sample losses: fixed-point scale of the 64-bit sums, and the largest partial (one tile's row sum over 128
 // columns, or one 16-row slab's column sum) that is added as a number. 2^16 * 2^32 per partial keeps the unsigned sum
@@ -295,6 +307,24 @@ struct SampleLossArgs {
   DebugRecord* dbg;
 };
 int launch_sample_loss_finalize(const SampleLossArgs& a, cudaStream_t stream);
+
+// Finalisation of a top-K step with K > 1 (one block, after the metrics finalisation when both are armed, before the
+// per-sample losses). W > 1: unless the metrics finalisation already did, publish flag kind 5 to every rank; then wait
+// for every rank's flag kind 5 of the step and merge the W sorted column lists of each of my texts (relaxed
+// system-scope loads). Decode the lists into global indices and count, per side, the samples whose first hit is at
+// each rank, for recall@k. m carries the hit rules and the flags as for the metrics (its key pointers are unused).
+struct TopKArgs {
+  MetricsArgs m;
+  const unsigned long long* rows;              // [R][kTopKMax] local row lists
+  const unsigned long long* col_own;           // [T][kTopKMax] my lists of my chunk
+  const unsigned long long* const* col_peers;  // [world] every rank's lists of my chunk (world > 1; own entry unused)
+  int k;
+  int signal;                                  // 1: raise flag kind 5 here (no metrics finalisation in this step)
+  float* recall;                               // [2k]: i2t, then t2i
+  int64_t* i2t;                                // [ni][k] or null
+  int64_t* t2i;                                // [nt][k] or null
+};
+int launch_topk_finalize(const TopKArgs& a, cudaStream_t stream);
 int launch_wait_flags(const volatile unsigned int* flags, int n, unsigned int value, unsigned long long timeout_ns,
                       DebugRecord* dbg, cudaStream_t stream);
 

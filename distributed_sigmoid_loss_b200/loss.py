@@ -22,6 +22,9 @@ import torch.nn as nn
 
 from . import _capi
 
+# Largest K of the top-K in-batch retrieval (SIGLIP_TOPK_MAX in include/siglip_b200.h)
+TOPK_MAX = 10
+
 
 def _group_rank_world(group) -> Tuple[int, int]:
     if dist.is_available() and dist.is_initialized():
@@ -313,6 +316,36 @@ class SigmoidLossEngine:
                 keys.device != self.device:
             raise RuntimeError(f"peer metric keys must be a contiguous int64 [{n}] tensor on {self.device}")
         _capi.check(self._L.siglip_debug_set_peer_metric_keys(self._h, peer, keys.data_ptr(), self._stream()))
+
+    def request_topk(self, k: int, recall: torch.Tensor, i2t_topk: Optional[torch.Tensor] = None,
+                     t2i_topk: Optional[torch.Tensor] = None) -> None:
+        """Arm the top-K in-batch retrieval of the NEXT step (siglip_request_topk), k in 1 .. TOPK_MAX: recall fp32 [2k]
+        (i2t recall@1..k, then t2i), i2t_topk int64 [metric_images, k] and t2i_topk int64 [metric_texts, k] (global
+        indices, best first, -1 past the candidates) or None, all contiguous on the engine's device. Nothing is read on
+        the host; the step writes them on its stream. Refused under distillation."""
+        if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= TOPK_MAX:
+            raise RuntimeError(f"k must be an int in 1 .. {TOPK_MAX}, got {k!r}")
+        bufs = (("recall", recall, torch.float32, (2 * k,)),
+                ("i2t_topk", i2t_topk, torch.int64, (self.metric_images, k)),
+                ("t2i_topk", t2i_topk, torch.int64, (self.metric_texts, k)))
+        for name, x, dt, shape in bufs:
+            if x is None and name != "recall":
+                continue
+            if not isinstance(x, torch.Tensor) or x.dtype != dt or tuple(x.shape) != shape or not x.is_contiguous() \
+                    or x.device != self.device:
+                raise RuntimeError(f"{name} must be a contiguous {dt} {list(shape)} tensor on {self.device}")
+        _capi.check(self._L.siglip_request_topk(self._h, k, recall.data_ptr(),
+                                                i2t_topk.data_ptr() if i2t_topk is not None else None,
+                                                t2i_topk.data_ptr() if t2i_topk is not None else None))
+
+    def debug_set_peer_topk_keys(self, peer: int, keys: torch.Tensor) -> None:
+        """Loopback: the top-K column lists ([T, TOPK_MAX] int64 holding the 64-bit keys, each row sorted best first and
+        0-padded) standing in for peer `peer`'s lists of this rank's text chunk."""
+        shape = (self.texts, TOPK_MAX)
+        if keys.dtype != torch.int64 or tuple(keys.shape) != shape or not keys.is_contiguous() or \
+                keys.device != self.device:
+            raise RuntimeError(f"peer top-K keys must be a contiguous int64 {list(shape)} tensor on {self.device}")
+        _capi.check(self._L.siglip_debug_set_peer_topk_keys(self._h, peer, keys.data_ptr(), self._stream()))
 
     def request_sample_losses(self, image_loss: torch.Tensor, text_loss: torch.Tensor) -> None:
         """Arm the per-sample losses of the NEXT step (siglip_request_sample_losses): image_loss fp32 [R] (the paired
@@ -690,7 +723,9 @@ class _SigmoidLossFn(torch.autograd.Function):
         if weights is not None:
             engine.set_sample_weights(*weights)
         if metrics is not None:
-            engine.request_metrics(*metrics)
+            engine.request_metrics(*metrics[:3])
+            if len(metrics) > 3:   # metrics_topk = K > 1: (K, recall, i2t_topk, t2i_topk) follow
+                engine.request_topk(*metrics[3:])
         if sample_losses is not None:
             engine.request_sample_losses(*sample_losses)
         if ctx.fused:
@@ -1097,9 +1132,37 @@ def _with_outputs(out, metric_bufs, loss_bufs):
 
 def _metric_dict(bufs) -> Dict[str, torch.Tensor]:
     """The in-batch retrieval metrics of a step, as device tensors (no host synchronisation): top-1 rates of this rank's
-    images / texts (0-dim fp32) and the global index of each one's best match (int64 [B])."""
-    top1, i2t, t2i = bufs
-    return {"i2t_top1": top1[0], "t2i_top1": top1[1], "i2t_index": i2t, "t2i_index": t2i}
+    images / texts (0-dim fp32) and the global index of each one's best match (int64 [B]); with metrics_topk = K > 1
+    also each one's K best matches (int64 [n, K]) and recall@1..K (fp32 [K]) per direction."""
+    top1, i2t, t2i = bufs[:3]
+    out = {"i2t_top1": top1[0], "t2i_top1": top1[1], "i2t_index": i2t, "t2i_index": t2i}
+    if len(bufs) > 3:
+        k, recall, i2t_topk, t2i_topk = bufs[3:]
+        out.update({"i2t_topk": i2t_topk, "t2i_topk": t2i_topk, "i2t_recall": recall[:k], "t2i_recall": recall[k:]})
+    return out
+
+
+def _validate_metrics_topk(metrics_topk, return_metrics, distill) -> int:
+    """K of a forward's top-K retrieval (None: 1, the top-1 metrics alone)."""
+    if metrics_topk is None:
+        return 1
+    if isinstance(metrics_topk, bool) or not isinstance(metrics_topk, int) or not 1 <= metrics_topk <= TOPK_MAX:
+        raise RuntimeError(f"metrics_topk must be an int in 1 .. {TOPK_MAX}, got {metrics_topk!r}")
+    if not return_metrics:
+        raise RuntimeError("metrics_topk needs return_metrics=True")
+    if distill is not None:
+        raise RuntimeError("metrics_topk is unavailable with distill: the distillation loss kernel does not rank the "
+                           "top K")
+    return metrics_topk
+
+
+def _topk_buffers(eng, k: int, bufs):
+    """The metric buffers, followed by (K, recall [2K], i2t_topk [ni, K], t2i_topk [nt, K]) when K > 1."""
+    if bufs is None or k == 1:
+        return bufs
+    return (*bufs, k, torch.empty(2 * k, device=eng.device, dtype=torch.float32),
+            torch.empty(eng.metric_images, k, device=eng.device, dtype=torch.int64),
+            torch.empty(eng.metric_texts, k, device=eng.device, dtype=torch.int64))
 
 
 def _validate(image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, expect_batch: Optional[int]) -> None:
@@ -1209,6 +1272,14 @@ class DDPSigmoidLoss(nn.Module):
     so they are bitwise reproducible; loss, gradients and metrics are unchanged. Device tensors, no host
     synchronisation, not differentiable; works under ``torch.no_grad()`` (data selection over a super-batch). Not with
     ``distill``. Collective: every rank asks on the same steps.
+
+    ``forward(..., return_metrics=True, metrics_topk=K)``, K in 1 .. 10: with K > 1 the metrics dict also holds
+    ``i2t_topk`` ([ni, K] int64: each ranked image's K best texts over the global batch, global indices, best first,
+    ties to the lower index, −1 past the candidates), ``t2i_topk`` ([nt, K]: each ranked text's K best images) and
+    ``i2t_recall`` / ``t2i_recall`` ([K] fp32: the fraction with a hit among the first k, k = 1 .. K, by the hit rules of
+    the top-1 metrics). ``recall[0]`` and column 0 are the top-1 rate and index bit for bit; loss and gradients are
+    unchanged. K = 1 or None returns today's dict. Not with ``distill``; works under ``torch.no_grad()`` (evaluation,
+    mining). Collective: every rank asks the same K on the same steps.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
@@ -1269,9 +1340,11 @@ class DDPSigmoidLoss(nn.Module):
                 text_weights: Optional[torch.Tensor] = None, extra_image: Optional[torch.Tensor] = None,
                 extra_image_ids: Optional[torch.Tensor] = None, teacher_image: Optional[torch.Tensor] = None,
                 teacher_text: Optional[torch.Tensor] = None, teacher_t_prime: Optional[torch.Tensor] = None,
-                teacher_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False):
+                teacher_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False,
+                metrics_topk: Optional[int] = None):
         _validate_return_metrics(return_metrics)
         _validate_return_sample_losses(return_sample_losses, self.distill)
+        topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill)
         teacher = _teacher_of(self.distill, image_embeddings,
                               ("teacher_image", "teacher_text", "teacher_t_prime", "teacher_bias"),
                               (teacher_image, teacher_text, teacher_t_prime, teacher_bias))
@@ -1291,6 +1364,7 @@ class DDPSigmoidLoss(nn.Module):
                               teacher[0].shape[1] if teacher is not None else 0)
         fused = _fused_under_budget(eng, self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
+        bufs = _topk_buffers(eng, topk, bufs)
         lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
         loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
                                     self.normalize_inputs, fused, ids, bufs, extra_ids, weights, ximg_ids, teacher,
@@ -1357,9 +1431,11 @@ class SigLipLoss(nn.Module):
                 text_weights: Optional[torch.Tensor] = None, extra_image: Optional[torch.Tensor] = None,
                 extra_image_ids: Optional[torch.Tensor] = None, teacher_image: Optional[torch.Tensor] = None,
                 teacher_text: Optional[torch.Tensor] = None, teacher_logit_scale: Optional[torch.Tensor] = None,
-                teacher_logit_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False):
+                teacher_logit_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False,
+                metrics_topk: Optional[int] = None):
         _validate_return_metrics(return_metrics)
         _validate_return_sample_losses(return_sample_losses, self.distill)
+        topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill)
         teacher = _teacher_of(self.distill, image_features,
                               ("teacher_image", "teacher_text", "teacher_logit_scale", "teacher_logit_bias"),
                               (teacher_image, teacher_text, teacher_logit_scale, teacher_logit_bias))
@@ -1386,6 +1462,7 @@ class SigLipLoss(nn.Module):
             logit_bias = torch.zeros((), device=image_features.device)
         fused = _fused_under_budget(eng, self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
+        bufs = _topk_buffers(eng, topk, bufs)
         lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
         loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs,
                                     extra_ids, weights, ximg_ids, teacher, lbufs)

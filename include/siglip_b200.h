@@ -450,6 +450,31 @@ int siglip_request_metrics(siglip_ctx* ctx, float* top1, int64_t* i2t_index, int
  * return SIGLIP_ERR_STATE while armed. */
 int siglip_request_sample_losses(siglip_ctx* ctx, float* image_loss, float* text_loss);
 
+/* Largest K of siglip_request_topk. */
+#define SIGLIP_TOPK_MAX 10
+
+/* Top-K in-batch retrieval of the NEXT siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd only (detached):
+ *   i2t_topk[i, s] (i < the images siglip_request_metrics ranks) = global index of image i's (s+1)-th best text over
+ *                  the global batch, t2i_topk[j, s] the same for text j's images; -1 past the candidates there are
+ *   recall[k - 1] (k = 1 .. K) = fraction of those images with a hit among their first k texts, recall[K + k - 1] the
+ *                  same for the texts (hits as in siglip_request_metrics: the pair, a shared id, extras by their ids)
+ * The ranking is the metrics' own: the key (order-preserving bits of s) << 32 | (0xFFFFFFFF - global index), so ties
+ * go to the lower index, recall[0] / recall[K] equal the top-1 rates bit for bit, column 0 equals the top-1 indices,
+ * and the lists for K are the first K entries of the lists for any larger K. Bitwise reproducible whatever the cluster
+ * shape, stage count, schedule, row panels or order of the atomics.
+ * k in 1 .. SIGLIP_TOPK_MAX; recall: [2k] fp32 device buffer (required), i2t_topk [ni, k] and t2i_topk [nt, k] int64
+ * device buffers or NULL. Loss, gradients, the retrieval metrics and the per-sample losses are bit-identical to the same
+ * step without the request; composes with siglip_request_metrics and siglip_request_sample_losses.
+ * Cost: k = 1 runs the metrics path. k > 1 runs the step's loss kernels in their own instantiation, which inserts
+ * every logit above a list's current K-th key into per-row and per-column sorted lists, plus two memsets and a
+ * one-block finalisation kernel. Workspace: two parities of [world * Tmax] column lists and [Rmax] row lists of
+ * SIGLIP_TOPK_MAX 64-bit keys each; the row lists (and on a single-rank context the column lists) are allocated by the
+ * first call (also allowed inside a capture), the column lists of a multi-rank context are part of the exported text
+ * allocation from creation. This call only records the pointers.
+ * Collective: every rank arms the same steps with the same k. Returns SIGLIP_ERR_INVALID for k out of range or a null
+ * recall, SIGLIP_ERR_STATE under SIGLIP_OPT_DISTILL; the host-buffer entries return SIGLIP_ERR_STATE while armed. */
+int siglip_request_topk(siglip_ctx* ctx, int k, float* recall, int64_t* i2t_topk, int64_t* t2i_topk);
+
 /* Forward only (torch.no_grad / evaluation): siglip_forward with save_for_backward = 0. */
 int siglip_fwd(siglip_ctx* ctx, const void* img, const void* txt, const float* t_prime, const float* bias,
                float* loss, void* cuda_stream);
@@ -545,6 +570,10 @@ int siglip_debug_set_mailbox(siglip_ctx* ctx, int peer, float dt_prime, float db
  * (0xFFFFFFFF - global image index), 0 = no candidate), so
  * that the cross-rank combine of a metrics step sees candidates the kernel did not produce itself. */
 int siglip_debug_set_peer_metric_keys(siglip_ctx* ctx, int peer, const uint64_t* keys_dev, void* cuda_stream);
+/* Loopback only: seed the top-K column lists of this rank's text chunk that stand in for peer rank `peer`'s
+ * ([T, SIGLIP_TOPK_MAX] 64-bit keys as in siglip_debug_set_peer_metric_keys, each row sorted best first and 0-padded),
+ * so that the cross-rank merge of a top-K step sees lists the kernel did not produce itself. */
+int siglip_debug_set_peer_topk_keys(siglip_ctx* ctx, int peer, const uint64_t* keys_dev, void* cuda_stream);
 /* Loopback only: seed the per-sample-loss column partials of this rank's text chunk that stand in for peer rank
  * `peer`'s ([T] 64-bit fixed-point words, value * 2^32), so that the cross-rank sum of a per-sample-loss step adds
  * numbers the kernel did not produce itself. */

@@ -66,6 +66,10 @@ def main() -> int:
                     help="also check the per-sample losses (return_sample_losses=True) against the float64 oracle: "
                          "text_loss combines every rank's column partials of the own chunk, uneven batches, hard "
                          "negatives, ids and weights, fused / split / forward-only, and the cross-rank sum identity")
+    ap.add_argument("--metrics-topk", action="store_true",
+                    help="also check the top-K retrieval (metrics_topk=10) against the float64 oracle on exact "
+                         "small-integer embeddings: t2i merges every rank's column lists of the own chunk, uneven "
+                         "batches, hard negatives, ids with duplicates, fused / split / forward-only")
     ap.add_argument("--row-panels", action="store_true",
                     help="also check the fused step in row panels (sigma_budget_bytes forcing several panels) against "
                          "the float64 closed form and against the unbounded step on the same peers: uneven batches "
@@ -407,6 +411,50 @@ def main() -> int:
                     zero_weights=float((il.cpu()[wis[rank] == 0] != 0).any() or (tl.cpu()[wts[rank] == 0] != 0).any()),
                     loss_identity=abs(float(il.double().sum()) / Bs[rank] - float(loss)) / abs(float(loss)),
                     cross_rank_sums=abs(float(tot[0] - tot[1])) / float(tot[0])), tol=1e-3)
+            eng.close()
+
+    if args.metrics_topk:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from retrieval_topk_oracle import recall_counts, topk_retrieval
+        from distributed_sigmoid_loss_b200 import SigmoidLossEngine
+        Bs = [160 + 24 * r for r in range(world)]
+        Ts = [b + 8 + 4 * r for r, b in enumerate(Bs)]
+        D, K = 136, 10
+        gn = np.random.default_rng(4242)
+        # small integers / 8: exact bf16 operands, exact fp32 logits, so the lists compare exactly (ties included)
+        base = [gn.integers(-2, 3, (b, D)) for b in Bs]
+        imgs = [torch.from_numpy(x / 8).to(torch.bfloat16) for x in base]
+        txts = [torch.from_numpy(np.concatenate([x + gn.integers(-1, 2, x.shape), gn.integers(-2, 3, (t - b, D))]) / 8)
+                .to(torch.bfloat16) for x, b, t in zip(base, Bs, Ts)]
+        idss = [gn.integers(0, sum(Bs) // 2, b).astype(np.int64) for b in Bs]
+        for with_ids in (False, True):
+            ref = topk_retrieval([x.double().numpy() for x in imgs], [x.double().numpy() for x in txts], Bs, K,
+                                 img_ids=idss if with_ids else None, txt_ids=idss if with_ids else None)[rank]
+            eng = SigmoidLossEngine(Bs[rank], D, dev, batch_per_rank=Bs, texts_per_rank=Ts)
+            if with_ids:
+                eng.set_option(_capi.SIGLIP_OPT_SAMPLE_IDS, 1)
+            tpt, bt = torch.tensor([math.log(10.0)], device=dev), torch.tensor([-8.0], device=dev)
+            img, txt = imgs[rank].to(dev), txts[rank].to(dev)
+            for sched in ("fused", "split", "fwd", "fused"):
+                recall = torch.empty(2 * K, device=dev)
+                i2t = torch.empty(Bs[rank], K, device=dev, dtype=torch.int64)
+                t2i = torch.empty(Bs[rank], K, device=dev, dtype=torch.int64)
+                if with_ids:
+                    eng.set_sample_ids(torch.from_numpy(idss[rank]).to(dev))
+                eng.request_topk(K, recall, i2t, t2i)
+                if sched == "fused":
+                    eng.fwd_bwd(img, txt, tpt, bt)
+                elif sched == "split":
+                    eng.forward(img, txt, tpt, bt, True)
+                    eng.backward(img, txt, tpt, None)
+                else:
+                    eng.fwd(img, txt, tpt, bt)
+                torch.cuda.synchronize()
+                want = np.concatenate([recall_counts(ref["i2t_first"], K), recall_counts(ref["t2i_first"], K)])
+                report(f"top-K ids={with_ids} {sched} B={Bs} T={Ts}", dict(
+                    i2t_lists=float((i2t.cpu().numpy() != ref["i2t_topk"]).mean()),
+                    t2i_lists=float((t2i.cpu().numpy() != ref["t2i_topk"]).mean()),
+                    recall=float(np.abs(recall.cpu().numpy() - want).max())), tol=0.0)
             eng.close()
 
     # ---- hard-negative captions: every rank's extras are pulled with its text and scored against every image; their
