@@ -46,6 +46,7 @@ EXPORTED_SYMBOLS = (
     "siglip_set_extra_text_ids",
     "siglip_set_extra_image_ids",
     "siglip_set_sample_weights",
+    "siglip_set_groups",
     "siglip_request_metrics",
     "siglip_request_sample_losses",
     "siglip_request_topk",
@@ -69,6 +70,7 @@ EXPORTED_SYMBOLS = (
     "siglip_debug_get_slot",
     "siglip_debug_set_chunk_ids",
     "siglip_debug_set_chunk_weights",
+    "siglip_debug_set_chunk_groups",
     "siglip_debug_set_mailbox",
     "siglip_debug_set_peer_metric_keys",
     "siglip_debug_set_peer_sample_loss_partials",
@@ -110,6 +112,7 @@ SIGLIP_OPT_SAMPLE_WEIGHTS = 23
 SIGLIP_OPT_EXTRA_IMAGE_IDS = 24
 SIGLIP_OPT_DISTILL = 25
 SIGLIP_OPT_SIGMA_BUDGET_MIB = 26
+SIGLIP_OPT_EXCLUDE_GROUPS = 27
 
 _lib: Optional[ctypes.CDLL] = None
 
@@ -242,6 +245,10 @@ def lib() -> ctypes.CDLL:
     L.siglip_set_sample_weights.restype = ci
     L.siglip_debug_set_chunk_weights.argtypes = [vp, ci, vp, vp]
     L.siglip_debug_set_chunk_weights.restype = ci
+    L.siglip_set_groups.argtypes = [vp, vp, vp, vp]
+    L.siglip_set_groups.restype = ci
+    L.siglip_debug_set_chunk_groups.argtypes = [vp, ci, vp, vp]
+    L.siglip_debug_set_chunk_groups.restype = ci
     L.siglip_request_metrics.argtypes = [vp, vp, vp, vp]
     L.siglip_request_metrics.restype = ci
     L.siglip_debug_set_peer_metric_keys.argtypes = [vp, ci, vp, vp]

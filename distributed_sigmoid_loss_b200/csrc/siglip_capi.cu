@@ -218,6 +218,9 @@ struct siglip_ctx {
   bool extra_ids_set = false;            // siglip_set_extra_text_ids was called since the previous step
   int sample_weights = 0;                // SIGLIP_OPT_SAMPLE_WEIGHTS: per-sample loss weights (collective)
   bool weights_set = false;              // siglip_set_sample_weights was called since the previous step
+  int exclude_groups = 0;                // SIGLIP_OPT_EXCLUDE_GROUPS: same-group pairs are excluded (collective)
+  bool groups_set = false;               // siglip_set_groups was called since the previous step
+  bool ids_grp = false;                  // ids_in has its group halves (allocated when the mode is first turned on)
   // distillation (siglip_ctx_create_distill, SIGLIP_OPT_DISTILL)
   int DT = 0;                            // teacher width D_teacher (0: a context without a teacher)
   int distill = 0;                       // SIGLIP_OPT_DISTILL (collective)
@@ -257,9 +260,11 @@ struct siglip_ctx {
   // workspaces
   __nv_bfloat16* txt_all = nullptr;      // [world][Tmax, D] bf16; slot `rank` is what the peers pull (world > 1),
                                          // followed by ids_all in the same (IPC-exported) allocation
-  int64_t* ids_all = nullptr;            // [world][ids_stride] ids of every text chunk (world > 1)
+  int64_t* ids_all = nullptr;            // [world][2 ids_stride] ids, then text groups, of every text chunk (world > 1)
   int64_t* ids_in = nullptr;             // [ids_stride] this rank's ids for the next step: B sample ids
-                                         // (siglip_set_sample_ids), then K extra-text ids (siglip_set_extra_text_ids)
+                                         // (siglip_set_sample_ids), then K extra-text ids (siglip_set_extra_text_ids);
+                                         // once SIGLIP_OPT_EXCLUDE_GROUPS has been on, followed by [ids_stride] text
+                                         // groups and [R] image groups (siglip_set_groups), laid out like a slot
   int ids_stride = 0;                    // Tmax rounded up to even: every slot is a whole number of 16-byte vectors.
                                          // Fixed at creation (options are set after the handle exchange)
   unsigned long long* mkeys[2] = {};     // per step parity: [world][Tmax] column argmax partials of every text chunk
@@ -374,21 +379,38 @@ inline size_t chunk_stride(const siglip_ctx* c) { return static_cast<size_t>(c->
 
 // Sample ids of text chunk `cidx` as the loss kernel reads them (null outside SIGLIP_OPT_SAMPLE_IDS): the caller's ids
 // for the own chunk, the gathered copy for the others.
+// Every slot of ids_all is [ids_stride] ids, then [ids_stride] text groups (SIGLIP_OPT_EXCLUDE_GROUPS), fixed at
+// creation: the groups ride every copy of the ids, which then moves the whole slot.
+inline size_t ids_slot(const siglip_ctx* c) { return 2 * static_cast<size_t>(c->ids_stride); }
 inline const int64_t* chunk_ids(const siglip_ctx* c, int cidx) {
   if (!c->sample_ids) return nullptr;
-  return (cidx == c->rank) ? c->ids_in : c->ids_all + static_cast<size_t>(cidx) * c->ids_stride;
+  return (cidx == c->rank) ? c->ids_in : c->ids_all + static_cast<size_t>(cidx) * ids_slot(c);
 }
 // Rank o's published ids slot, seen through its exported text allocation (they sit behind its [world][Tmax, D] text)
 inline const int64_t* peer_ids(const siglip_ctx* c, int o) {
   return reinterpret_cast<const int64_t*>(c->peer_txt[o] + c->world * chunk_stride(c)) +
-         static_cast<size_t>(o) * c->ids_stride;
+         static_cast<size_t>(o) * ids_slot(c);
 }
+// ---- excluded groups (SIGLIP_OPT_EXCLUDE_GROUPS) ----
+// Text groups of chunk `cidx` as the loss kernel reads them (null outside the mode): the group half of my ids_in for
+// the own chunk, of the gathered slot for the others. Image groups are local, behind my text groups: they never travel.
+inline const int64_t* chunk_groups(const siglip_ctx* c, int cidx) {
+  if (!c->exclude_groups) return nullptr;
+  return ((cidx == c->rank) ? c->ids_in : c->ids_all + static_cast<size_t>(cidx) * ids_slot(c)) + c->ids_stride;
+}
+inline const int64_t* image_groups(const siglip_ctx* c) { return c->exclude_groups ? c->ids_in + ids_slot(c) : nullptr; }
+// the ids copies of the exchange run in ids mode or groups mode; under groups mode they move the whole slot
+inline bool ids_travel(const siglip_ctx* c) { return c->sample_ids || c->exclude_groups; }
 // the sample ids of a rank (siglip_set_sample_ids)
 inline size_t ids_bytes(const siglip_ctx* c, int rank) { return static_cast<size_t>(c->Bs[rank]) * sizeof(int64_t); }
 // the ids of a text chunk as the exchange moves them: its paired texts', and under SIGLIP_OPT_EXTRA_TEXT_IDS its extras'
 inline int chunk_id_count(const siglip_ctx* c, int rank) { return c->extra_text_ids ? c->Ts[rank] : c->Bs[rank]; }
 inline size_t chunk_ids_bytes(const siglip_ctx* c, int rank) {
   return static_cast<size_t>(chunk_id_count(c, rank)) * sizeof(int64_t);
+}
+// bytes one ids copy of the exchange moves: the chunk's ids, or the whole slot (ids and text groups) under groups mode
+inline size_t ids_copy_bytes(const siglip_ctx* c, int rank) {
+  return c->exclude_groups ? ids_slot(c) * sizeof(int64_t) : chunk_ids_bytes(c, rank);
 }
 // ids and weights of step s are given once: a step in ids / weights mode consumes them (all checked before anything is
 // launched or consumed)
@@ -411,6 +433,10 @@ int take_ids(siglip_ctx* c) {
                 "SIGLIP_OPT_SAMPLE_WEIGHTS is on but siglip_set_sample_weights was not called since the previous step");
   if (c->distill && !c->teacher_set)
     return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is on but siglip_set_teacher was not called since the previous step");
+  if (c->exclude_groups && !c->groups_set)
+    return fail(SIGLIP_ERR_STATE,
+                "SIGLIP_OPT_EXCLUDE_GROUPS is on but siglip_set_groups was not called since the previous step");
+  c->groups_set = false;
   c->teacher_set = false;
   c->ids_set = false;
   c->extra_ids_set = false;
@@ -453,7 +479,7 @@ inline size_t mkeys_xids(const siglip_ctx* c) { return static_cast<size_t>(c->wo
 inline size_t mkeys_rows(const siglip_ctx* c) { return static_cast<size_t>(c->world) * c->Tmax; }
 // byte offset of the two key blocks in the exported text allocation: behind the gathered text and ids
 inline size_t mkeys_offset(const siglip_ctx* c) {
-  return chunk_stride(c) * c->world * sizeof(__nv_bfloat16) + static_cast<size_t>(c->world) * c->ids_stride * sizeof(int64_t);
+  return chunk_stride(c) * c->world * sizeof(__nv_bfloat16) + static_cast<size_t>(c->world) * ids_slot(c) * sizeof(int64_t);
 }
 // byte offset of the text-weight slots in the exported text allocation: behind the two key blocks
 inline size_t weights_offset(const siglip_ctx* c) {
@@ -582,7 +608,7 @@ void fill_metrics_args(const siglip_ctx* c, unsigned int s, siglip::MetricsArgs&
     a.ids_own = c->ids_in;
     a.row_ids = row_ids(c);
     a.ids_all = c->ids_all;
-    a.ids_stride = c->ids_stride;
+    a.ids_stride = static_cast<int>(ids_slot(c));
     a.extra_ids = c->extra_text_ids;
     a.extra_image_ids = c->extra_image_ids;
     if (W > 1 && c->xid_ptrs_dev != nullptr) a.xids_peers = c->xid_ptrs_dev + static_cast<size_t>(s & 1u) * W;
@@ -918,6 +944,11 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
     p.row_w = image_weights(c) + r0;
     p.col_w = chunk_weights(c, cidx) + c0;
   }
+  if (c->exclude_groups) {   // the kModeGroups kernel: same-group pairs that are not positives are excluded
+    p.row_grp = image_groups(c) + r0;
+    p.col_grp = chunk_groups(c, cidx) + c0;
+    p.grp_rows = rest(c->R, r0);
+  }
   if (c->mkeys_step != nullptr) {   // a metrics step: the kMetrics instantiation reduces the argmax keys
     p.row_keys = c->mkeys_step + mkeys_rows(c) + r0;
     p.col_keys = c->mkeys_step + static_cast<size_t>(cidx) * c->Tmax + c0;
@@ -1198,13 +1229,13 @@ void add_pull_job(siglip_ctx* c, AuxList& aux, int o, unsigned int s) {
   j.wait_n = 1;
   j.wait_value = s;
   j.site = 5;
-  if (c->sample_ids) {
-    // the chunk's ids ride the same flag: the owner published them before its text signal, and every CTA has
-    // observed that flag in the job above before it runs this one
+  if (ids_travel(c)) {
+    // the chunk's ids (and text groups) ride the same flag: the owner published them before its text signal, and
+    // every CTA has observed that flag in the job above before it runs this one
     siglip::AuxJob& ji = aux.add(siglip::kAuxCopy);
     ji.src = reinterpret_cast<const uint4*>(peer_ids(c, o));
-    ji.dst = reinterpret_cast<uint4*>(c->ids_all + static_cast<size_t>(o) * c->ids_stride);
-    ji.n16 = (chunk_ids_bytes(c, o) + 15) / 16;   // within the slot: ids_stride is even
+    ji.dst = reinterpret_cast<uint4*>(c->ids_all + static_cast<size_t>(o) * ids_slot(c));
+    ji.n16 = (ids_copy_bytes(c, o) + 15) / 16;   // within the slot: ids_stride is even
   }
   if (c->sample_weights) {
     // the chunk's text weights ride the same flag, like its ids
@@ -1251,8 +1282,8 @@ void add_weights_publish_job(siglip_ctx* c, AuxList& aux, unsigned int s) {
 void add_ids_publish_job(siglip_ctx* c, AuxList& aux, unsigned int s) {
   siglip::AuxJob& j = aux.add(siglip::kAuxCopy);
   j.src = reinterpret_cast<const uint4*>(c->ids_in);
-  j.dst = reinterpret_cast<uint4*>(c->ids_all + static_cast<size_t>(c->rank) * c->ids_stride);
-  j.n16 = (chunk_ids_bytes(c, c->rank) + 15) / 16;
+  j.dst = reinterpret_cast<uint4*>(c->ids_all + static_cast<size_t>(c->rank) * ids_slot(c));
+  j.n16 = (ids_copy_bytes(c, c->rank) + 15) / 16;
   j.wait_flags = c->flags + 2 * kMaxWorld;
   j.wait_n = c->world;
   j.wait_value = s - 1;
@@ -1261,9 +1292,9 @@ void add_ids_publish_job(siglip_ctx* c, AuxList& aux, unsigned int s) {
 
 // the same publishes (ids, text weights) as stream copies (split forward, helper-kernel variant of the fused step)
 int copy_own_chunk_data(siglip_ctx* c, cudaStream_t st) {
-  if (c->sample_ids)
-    CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(c->rank) * c->ids_stride, c->ids_in,
-                       chunk_ids_bytes(c, c->rank), cudaMemcpyDeviceToDevice, st));
+  if (ids_travel(c))
+    CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(c->rank) * ids_slot(c), c->ids_in,
+                       ids_copy_bytes(c, c->rank), cudaMemcpyDeviceToDevice, st));
   if (c->sample_weights)
     CK(cudaMemcpyAsync(c->w_all + static_cast<size_t>(c->rank) * c->w_stride, c->w_in, chunk_weights_bytes(c, c->rank),
                        cudaMemcpyDeviceToDevice, st));
@@ -1349,9 +1380,9 @@ int forward_impl(siglip_ctx* c, const void* img, const void* txt, const float* t
         if ((rc = wait_one(c, 0, nxt, s, st))) return rc;
         CK(cudaMemcpyAsync(c->txt_all + nxt * stride, c->peer_txt[nxt] + nxt * stride,
                            static_cast<size_t>(c->Ts[nxt]) * c->D * sizeof(__nv_bfloat16), cudaMemcpyDefault, st));
-        if (c->sample_ids)
-          CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(nxt) * c->ids_stride, peer_ids(c, nxt),
-                             chunk_ids_bytes(c, nxt), cudaMemcpyDefault, st));
+        if (ids_travel(c))
+          CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(nxt) * ids_slot(c), peer_ids(c, nxt),
+                             ids_copy_bytes(c, nxt), cudaMemcpyDefault, st));
         if (c->sample_weights)
           CK(cudaMemcpyAsync(c->w_all + static_cast<size_t>(nxt) * c->w_stride, peer_weights(c, nxt),
                              chunk_weights_bytes(c, nxt), cudaMemcpyDefault, st));
@@ -1529,7 +1560,8 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   fin.dbias = c->scalars + kSavedScalars + 1;
   // With ids and weights, L0 would carry 9 jobs (3 publishes, 2 conversions, the flag-3 wait, 3 pulls) of
   // kMaxAuxJobs = 8: the image conversion then runs in L1 instead (its first reader is G1, behind L1).
-  const bool img_cvt_in_l1 = W > 1 && ik && ((c->sample_ids && c->sample_weights) || c->distill);
+  // (Groups mode runs the same ids jobs, so it counts as ids here.)
+  const bool img_cvt_in_l1 = W > 1 && ik && ((ids_travel(c) && c->sample_weights) || c->distill);
   // Distillation adds a teacher publish and a teacher pull to L0 (up to 8 jobs with ids and weights): the own text's
   // conversion and the flag-3 wait move to L1 as well. G0, their first consumer, and G1 run behind L1.
   const bool l0_work_in_l1 = W > 1 && ik && c->distill;
@@ -1545,7 +1577,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
         // then "text of forward s in place" (flag 0) goes to every rank once all CTAs have copied their share. My
         // ids (sample-id mode) and text weights (weights mode) are copied by jobs before it: each CTA finishes them
         // before the text job's ticket, so the same signal covers them.
-        if (c->sample_ids) add_ids_publish_job(c, aux, s);
+        if (ids_travel(c)) add_ids_publish_job(c, aux, s);
         if (c->sample_weights) add_weights_publish_job(c, aux, s);
         if (c->distill) add_teacher_publish_job(c, aux, s);
         siglip::AuxJob& cp = aux.add(siglip::kAuxCopy);
@@ -1906,7 +1938,8 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     const size_t l_bytes = 2 * lsum_block(c) * sizeof(unsigned long long);
     // and the top-K column lists behind those (sized whatever the options, for the same reason)
     const size_t k_bytes = 2 * topk_cols_words(c) * sizeof(unsigned long long);
-    CK(alloc(reinterpret_cast<void**>(&c->txt_all), stride * world * sizeof(__nv_bfloat16) + world * ids_slot_bytes +
+    // (every ids slot has a text-group half: SIGLIP_OPT_EXCLUDE_GROUPS may be set after the handle exchange too)
+    CK(alloc(reinterpret_cast<void**>(&c->txt_all), stride * world * sizeof(__nv_bfloat16) + world * 2 * ids_slot_bytes +
                                                         mkeys_bytes + w_bytes + t_bytes + l_bytes + k_bytes));
     c->ids_all = reinterpret_cast<int64_t*>(c->txt_all + stride * world);   // 16-byte aligned: D % 8 == 0
     c->mkeys[0] = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(c->txt_all) + mkeys_offset(c));
@@ -2017,9 +2050,33 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
     case SIGLIP_OPT_DISTILL:
       if (value && c->DT == 0)
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL needs a context created with siglip_ctx_create_distill");
+      if (value && c->exclude_groups)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is unavailable under SIGLIP_OPT_EXCLUDE_GROUPS");
       c->distill = value ? 1 : 0;
       c->teacher_set = false;
       return 0;
+    case SIGLIP_OPT_EXCLUDE_GROUPS: {
+      if (value && c->distill)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_EXCLUDE_GROUPS is unavailable under SIGLIP_OPT_DISTILL");
+      if (value && !c->ids_grp) {
+        // ids_in grows its group halves ([ids_stride] text groups, [R] image groups) on first use, so a context that
+        // never turns the mode on holds the workspace it held without it. Its ids are kept (they may be set already).
+        CK(cudaSetDevice(c->device));
+        CK(cudaDeviceSynchronize());   // no launch in flight reads the old buffer
+        const size_t bytes = (ids_slot(c) + static_cast<size_t>(c->R)) * sizeof(int64_t);
+        int64_t* buf = nullptr;
+        CK(cudaMalloc(reinterpret_cast<void**>(&buf), bytes));
+        CK(cudaMemset(buf, 0, bytes));
+        CK(cudaMemcpy(buf, c->ids_in, static_cast<size_t>(c->ids_stride) * sizeof(int64_t), cudaMemcpyDeviceToDevice));
+        CK(cudaFree(c->ids_in));
+        c->ids_in = buf;
+        c->ids_grp = true;
+        c->workspace_bytes += bytes - static_cast<size_t>(c->ids_stride) * sizeof(int64_t);
+      }
+      c->exclude_groups = value ? 1 : 0;
+      c->groups_set = false;
+      return 0;
+    }
     case SIGLIP_OPT_SIGMA_BUDGET_MIB:
       if (value < 0) return fail(SIGLIP_ERR_INVALID, "the sigma budget must be >= 0 MiB (0: unbounded)");
       c->sigma_budget_mib = value;
@@ -2379,6 +2436,20 @@ int siglip_set_sample_weights(siglip_ctx* c, const float* image_w, const float* 
   return 0;
 }
 
+int siglip_set_groups(siglip_ctx* c, const int64_t* image_groups, const int64_t* text_groups, void* cuda_stream) {
+  if (c == nullptr || image_groups == nullptr || text_groups == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->exclude_groups) return fail(SIGLIP_ERR_STATE, "siglip_set_groups needs SIGLIP_OPT_EXCLUDE_GROUPS = 1");
+  CK(cudaSetDevice(c->device));
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  // my text groups go to the group half of my slot (published with my ids), my image groups behind it
+  CK(cudaMemcpyAsync(c->ids_in + c->ids_stride, text_groups, static_cast<size_t>(c->T) * sizeof(int64_t),
+                     cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(c->ids_in + ids_slot(c), image_groups, static_cast<size_t>(c->R) * sizeof(int64_t),
+                     cudaMemcpyDeviceToDevice, st));
+  c->groups_set = true;
+  return 0;
+}
+
 int siglip_request_metrics(siglip_ctx* c, float* top1, int64_t* i2t_index, int64_t* t2i_index) {
   if (c == nullptr || top1 == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument (top1 is required)");
   if (c->mkeys[0] == nullptr) {
@@ -2611,6 +2682,9 @@ int siglip_host_submit_grads(siglip_ctx* c, const void* img_host, const void* tx
                 "the host-buffer entries take no sample weights: unavailable under SIGLIP_OPT_SAMPLE_WEIGHTS");
   if (c->distill)
     return fail(SIGLIP_ERR_STATE, "the host-buffer entries take no teacher: unavailable under SIGLIP_OPT_DISTILL");
+  if (c->exclude_groups)
+    return fail(SIGLIP_ERR_STATE,
+                "the host-buffer entries take no group ids: unavailable under SIGLIP_OPT_EXCLUDE_GROUPS");
   const bool with_grads = dimg_host_bf16 != nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   CK(cudaSetDevice(c->device));
@@ -2821,8 +2895,18 @@ int siglip_teacher_normalize_fwd(siglip_ctx* c, int rows, const void* x, int in_
 int siglip_debug_set_chunk_ids(siglip_ctx* c, int chunk, const int64_t* ids_dev, void* cuda_stream) {
   if (c == nullptr || ids_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
-  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * c->ids_stride, ids_dev, chunk_ids_bytes(c, chunk),
+  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * ids_slot(c), ids_dev, chunk_ids_bytes(c, chunk),
                      cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
+  return 0;
+}
+
+int siglip_debug_set_chunk_groups(siglip_ctx* c, int chunk, const int64_t* groups_dev, void* cuda_stream) {
+  if (c == nullptr || groups_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
+  // the group half of the chunk's slot, where its owner's ids publish puts them
+  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * ids_slot(c) + c->ids_stride, groups_dev,
+                     static_cast<size_t>(c->Ts[chunk]) * sizeof(int64_t), cudaMemcpyDeviceToDevice,
+                     static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
 

@@ -333,12 +333,14 @@ __device__ __forceinline__ void loss_slab_fast(const float* v, float tl, float b
 // pos (kMask only): bit i set = element i is a positive pair by sample id (SIGLIP_OPT_SAMPLE_IDS); 0 without ids.
 // kW: element i's weight multiplies its three terms once its label is applied (x * 1 == x: unit weights change no bit).
 // kL: element i's term (sp once masked and weighted) is also added to lrow / lcol as in loss_slab_fast.
-template <bool kMask, bool kW = false, bool kL = false>
+// kX (kModeGroups, with kMask): excl bit i set = element i is an excluded pair (same group, not a positive): its sp, g
+// and stored sigma are 0, so it adds nothing anywhere. A positive is never excluded (the label tests come first).
+template <bool kMask, bool kW = false, bool kL = false, bool kX = false>
 __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int row_lo, int col0, int c_lo, int nrows,
                                           int ncols, bool store_g, const GStore& gst, float gscale, float* g_diag,
                                           bool on_diag, uint32_t pos, float& acc_sp, float& acc_g, float& acc_gs,
                                           const float* cw = nullptr, float rw0 = 1.f, float rw1 = 1.f,
-                                          float* lrow = nullptr, float* lcol = nullptr) {
+                                          float* lrow = nullptr, float* lcol = nullptr, uint32_t excl = 0u) {
   uint32_t packed[8];
   float g_prev = 0.f;
 #pragma unroll
@@ -371,6 +373,10 @@ __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int 
         sp = fmaxf(-z, 0.f) + l;                       // g * 2^14 in [-16384, 0) goes into the fp16 operand
         g = -((z >= 0.f) ? e * r : r);
         g_store = g;
+      } else if (kX && ((excl >> i) & 1u)) {           // excluded pair (same group): neither pulled nor pushed
+        sp = 0.f;
+        g = 0.f;
+        g_store = 0.f;
       }
       sp = valid ? sp : 0.f;
       g = valid ? g : 0.f;
@@ -975,7 +981,11 @@ __device__ __forceinline__ void sample_loss_add(unsigned long long* w, long long
 // Rows >= M and columns >= N add nothing (their terms are masked to 0 and their words do not exist).
 // kTopK (kModeTopK): the top-K insertion (tile_topk) runs first, after the argmax keys, and the fixed-point sums are a
 // runtime option (p.sl_rows); the three sums, g_diag and the sigma operand are unchanged.
-template <bool kTopK = false>
+// kGroups (kModeGroups): excluded same-group pairs (p.row_grp / p.col_grp). Once per tile the groups of the thread's two
+// fragment rows, once per slab those of its 8 columns (clamped like the ids); the excl bits of the matching elements
+// that are not positives, and a warp vote: a slab with an excluded element takes the masked path, which zeroes it, and
+// every other slab keeps the path it takes without groups. Top-K lists and the per-sample sums are runtime options.
+template <bool kTopK = false, bool kGroups = false>
 __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, const float (&acc)[kTileN / 2],
                                                      const CUtensorMap* tmG, uint32_t staging_base, int warp, int wg,
                                                      int lane, int row0, int col_base, int row_lo, int c_lo,
@@ -983,8 +993,12 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
                                                      uint64_t policy, float& s_sp, float& c_sp, float& s_g, float& c_g,
                                                      float& s_gs, float& c_gs) {
   if (p.row_keys != nullptr) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
-  if constexpr (kTopK) tile_topk(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
-  const bool sl = !kTopK || p.sl_rows != nullptr;
+  if constexpr (kTopK) {
+    tile_topk(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
+  } else if constexpr (kGroups) {
+    if (p.tk_rows != nullptr) tile_topk(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
+  }
+  const bool sl = (!kTopK && !kGroups) || p.sl_rows != nullptr;
   float acc_sp = 0.f, acc_g = 0.f, acc_gs = 0.f;
   const bool edge = (row0 + kBlockM > pr.M) || (col_base + kTileN > pr.N);
   const bool diag = p.own_chunk && (row0 == col_base);
@@ -1007,6 +1021,13 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
   if (w) {
     rw0 = p.row_w[min(row_lo, pr.M - 1)];
     rw1 = p.row_w[min(row_lo + 8, pr.M - 1)];
+  }
+  int64_t rg0 = -1, rg1 = -1;
+  uint32_t rgrp = 0u;   // excl bits of the rows that have a group (>= 0, within grp_rows)
+  if constexpr (kGroups) {
+    rg0 = p.row_grp[min(row_lo, p.grp_rows - 1)];
+    rg1 = p.row_grp[min(row_lo + 8, p.grp_rows - 1)];
+    rgrp = (row_lo < p.grp_rows && rg0 >= 0 ? 0x3333u : 0u) | (row_lo + 8 < p.grp_rows && rg1 >= 0 ? 0xCCCCu : 0u);
   }
   float lrow[2] = {0.f, 0.f};
 #pragma unroll
@@ -1036,8 +1057,24 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
       pos &= rpos;
       slab_pos = __any_sync(0xffffffffu, pos != 0u);
     }
+    uint32_t excl = 0u;
+    bool slab_excl = false;
+    if constexpr (kGroups) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int e1 = 0; e1 < 2; ++e1) {
+          // a column beyond N reads column N - 1: it only lies in edge slabs, which mask it
+          const int64_t cg = p.col_grp[min(col0 + 8 * j + c_lo + e1, pr.N - 1)];
+          excl |= static_cast<uint32_t>(cg == rg0) << (4 * j + e1);
+          excl |= static_cast<uint32_t>(cg == rg1) << (4 * j + 2 + e1);
+        }
+      }
+      excl &= rgrp & ~pos;   // the own diagonal is tested before excl in loss_slab (slab_diag takes that path anyway)
+      slab_excl = __any_sync(0xffffffffu, excl != 0u);
+    }
     float lcol[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (!slab_edge && !slab_diag && !slab_pos) {
+    if (!slab_edge && !slab_diag && !slab_pos && !slab_excl) {
       float smax = v[0];
 #pragma unroll
       for (int j = 1; j < 16; ++j) smax = fmaxf(smax, v[j]);
@@ -1049,8 +1086,9 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
         loss_slab<false, true, true>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag,
                                      false, 0u, acc_sp, acc_g, acc_gs, cw, rw0, rw1, lrow, lcol);
     } else {
-      loss_slab<true, true, true>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag,
-                                  slab_diag, pos, acc_sp, acc_g, acc_gs, cw, rw0, rw1, lrow, lcol);
+      loss_slab<true, true, true, kGroups>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale,
+                                           p.g_diag, slab_diag, pos, acc_sp, acc_g, acc_gs, cw, rw0, rw1, lrow, lcol,
+                                           excl);
     }
     if (sl) {
       // reduce-scatter: after the step over lane bit m, lcol[0 .. h) holds the columns q = k + (bit m of lane ? h : 0)
@@ -1103,6 +1141,9 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
 // (sample_loss_epilogue); ids, weights and metrics are runtime options there.
 // kMode = kModeTopK: the loss kernel of a top-K step, its own instantiation like kModeSampleLoss: the top-K insertion
 // (tile_topk), then the kModeSampleLoss epilogue; ids, weights, metrics and the per-sample-loss sums are runtime options.
+// kMode = kModeGroups: the loss kernel of a step that excludes same-group pairs, its own instantiation like
+// kModeSampleLoss: its epilogue with the group comparisons (sample_loss_epilogue<false, true>); ids, weights, metrics,
+// the per-sample-loss sums and the top-K lists are runtime options.
 template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false,
           bool kWeights = false, int kTileNT = kTileN>
 __global__ void __launch_bounds__(kNumThreads, 1)
@@ -1122,6 +1163,8 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
                 "the per-sample-loss kernel takes ids, weights and metrics as runtime options");
   static_assert(kMode != kModeTopK || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
                 "the top-K kernel takes ids, weights, metrics and per-sample losses as runtime options");
+  static_assert(kMode != kModeGroups || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
+                "the excluded-groups kernel takes ids, weights, metrics, per-sample losses and top-K as runtime options");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -1369,7 +1412,8 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
   mma_loop<T, TA, TB, kCS, C::kStageBytes, kTileNT>(acc, kb0, kb1, stage, phase, C::kStages, adesc0, bdesc0, a_adv, \
                                                     b_adv, full0, empty0, lane, p.dbg, t, w_full_p)
         const int sel = pr.a_mn * 2 + pr.b_mn;
-        if constexpr (kMode == kModeDistill || kMode == kModeSampleLoss || kMode == kModeTopK) {
+        if constexpr (kMode == kModeDistill || kMode == kModeSampleLoss || kMode == kModeTopK ||
+                      kMode == kModeGroups) {
           // the loss operands (student and teacher) are always K-major: no MN-major variants in this instantiation
           if (pr.ab_f16)
             SIGLIP_MMA_LOOP(1, 0, 0);
@@ -1409,6 +1453,9 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       } else if constexpr (kMode == kModeTopK) {
         sample_loss_epilogue<true>(p, acc, &tmG, staging_base, warp, wg, lane, row0, col_base, row_lo, c_lo, pr, t_eff,
                                    bias, tl, bl, g_store_policy, s_sp, c_sp, s_g, c_g, s_gs, c_gs);
+      } else if constexpr (kMode == kModeGroups) {
+        sample_loss_epilogue<false, true>(p, acc, &tmG, staging_base, warp, wg, lane, row0, col_base, row_lo, c_lo, pr,
+                                          t_eff, bias, tl, bl, g_store_policy, s_sp, c_sp, s_g, c_g, s_gs, c_gs);
       } else if constexpr (kMode == kModeLoss) {
         // argmax keys first, on the raw accumulator: whichever path each slab then takes below
         if constexpr (kMetrics) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
@@ -2587,6 +2634,20 @@ int launch_gemm(int cta_group, int mode, int stages, int mcast, int tile_n, cons
       case 4: return launch_impl<kModeDistill, kDistillStages, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
       case 2: return launch_impl<kModeDistill, kDistillStages, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
       default: return launch_impl<kModeDistill, kDistillStages, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+    }
+  }
+  if (mode == kModeLoss && p.col_grp != nullptr) {   // excluded groups (with any other option): kModeGroups
+    const bool s4 = stages == 4;
+    switch (cluster_size(cta_group, mcast)) {
+      case 4:
+        return s4 ? launch_impl<kModeGroups, 4, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeGroups, 6, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      case 2:
+        return s4 ? launch_impl<kModeGroups, 4, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeGroups, 6, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      default:
+        return s4 ? launch_impl<kModeGroups, 4, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeGroups, 6, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
     }
   }
   if (mode == kModeLoss && p.tk_rows != nullptr) {   // top-K (with or without per-sample losses): kModeTopK

@@ -175,6 +175,12 @@ struct KernelParams {
   unsigned long long* tk_rows;   // [M][kTopKMax]: the best texts of each image of this rank
   unsigned long long* tk_cols;   // [N][kTopKMax]: the best images of each text of the chunk, over this rank's images
   int tk_k;                      // K in 2 .. kTopKMax: slots of each list that are filled
+  // Excluded pairs from group ids (SIGLIP_OPT_EXCLUDE_GROUPS). Appended last like the fields above. Non-null col_grp
+  // selects the kModeGroups loss kernel: a pair (i, j) that is not a positive and whose groups match
+  // (row_grp[i] == col_grp[j] >= 0) contributes 0 to the sums, the sigma operand and the per-sample sums.
+  const int64_t* row_grp;        // [grp_rows]: groups of this rank's images (rows of the launch)
+  const int64_t* col_grp;        // [N]: groups of the texts of the chunk being scored
+  int grp_rows;                  // rows that carry a group (row_grp has this many entries); rows past it match nothing
 };
 
 // kModeDistill: the loss kernel of a distillation step (KernelParams::k_teacher > 0), its own instantiation
@@ -182,7 +188,9 @@ struct KernelParams {
 // instantiation; ids, weights and metric keys are runtime options in it
 // kModeTopK: the loss kernel of a top-K step (KernelParams::tk_rows != null), its own instantiation; ids, weights,
 // metric keys and per-sample-loss sums are runtime options in it
-enum KernelMode { kModeLoss = 0, kModeOut = 1, kModeDistill = 2, kModeSampleLoss = 3, kModeTopK = 4 };
+// kModeGroups: the loss kernel of a step with excluded same-group pairs (KernelParams::col_grp != null), its own
+// instantiation; ids, weights, metric keys, per-sample-loss sums and top-K lists are runtime options in it
+enum KernelMode { kModeLoss = 0, kModeOut = 1, kModeDistill = 2, kModeSampleLoss = 3, kModeTopK = 4, kModeGroups = 5 };
 
 // Top-K retrieval: slots of every list (SIGLIP_TOPK_MAX), whatever K the step asks
 constexpr int kTopKMax = 10;

@@ -280,6 +280,21 @@ class SigmoidLossEngine:
             raise RuntimeError(f"sample weights must be a contiguous fp32 [{n}] tensor on {self.device} (or None), got "
                                f"{tuple(w.shape)} {w.dtype} on {w.device}")
 
+    def set_groups(self, image_groups: torch.Tensor, text_groups: torch.Tensor) -> None:
+        """SIGLIP_OPT_EXCLUDE_GROUPS: this rank's image groups ([R] int64: the paired images, then the extra images) and
+        text groups ([T] int64: the paired texts, then the extras), contiguous on the engine's device, for the NEXT step.
+        Copied on the current stream like set_sample_ids; a negative group matches nothing."""
+        self._check_ids(image_groups, self.images)
+        self._check_ids(text_groups, self.texts)
+        with torch.cuda.device(self.device):
+            _capi.check(self._L.siglip_set_groups(self._h, image_groups.data_ptr(), text_groups.data_ptr(),
+                                                  self._stream()))
+
+    def debug_set_chunk_groups(self, chunk: int, groups: torch.Tensor) -> None:
+        """Loopback: the text groups of chunk `chunk` ([T_c] int64) as its owner would have published them."""
+        self._check_ids(groups, self.texts_per_rank[chunk])
+        _capi.check(self._L.siglip_debug_set_chunk_groups(self._h, chunk, groups.data_ptr(), self._stream()))
+
     def debug_set_chunk_ids(self, chunk: int, ids: torch.Tensor) -> None:
         """Loopback: the ids of text chunk `chunk` as its owner would have published them: its sample ids ([B_c]), or
         under SIGLIP_OPT_EXTRA_TEXT_IDS the ids of all its texts ([T_c])."""
@@ -666,12 +681,14 @@ class _SigmoidLossFn(torch.autograd.Function):
     teacher: (teacher_image, teacher_text, teacher_t_prime, teacher_bias, lambda) of a distillation step
     (SIGLIP_OPT_DISTILL engines): constants, no gradient flows to them; set before every step like the ids.
     sample_losses: (image_loss [R], text_loss [T]) fp32 output buffers: the per-sample losses of this call's step are
-    armed. Like the metrics, a re-run of the forward by the backward's generation guard does not arm them again."""
+    armed. Like the metrics, a re-run of the forward by the backward's generation guard does not arm them again.
+    groups: (image_groups [R], text_groups [T]) int64 (SIGLIP_OPT_EXCLUDE_GROUPS engines), set before every step the
+    engine runs for this call, like the ids."""
 
     @staticmethod
     def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool = False, fused: bool = False,
                 ids: Optional[torch.Tensor] = None, metrics=None, extra_ids: Optional[torch.Tensor] = None, weights=None,
-                extra_img_ids: Optional[torch.Tensor] = None, teacher=None, sample_losses=None):
+                extra_img_ids: Optional[torch.Tensor] = None, teacher=None, sample_losses=None, groups=None):
         need_grad = any(ctx.needs_input_grad[:4])
         raw = None
         # bf16 callers: bf16 operands (what autograd would multiply). Anything wider (the reference's own test feeds
@@ -712,6 +729,7 @@ class _SigmoidLossFn(torch.autograd.Function):
                        tbias.detach().to(device=img.device, dtype=torch.float32).reshape(1), lam)
             engine.set_teacher(*teacher)
         ctx.ids, ctx.extra_ids, ctx.weights, ctx.extra_img_ids = ids, extra_ids, weights, extra_img_ids
+        ctx.groups = groups
         # the split schedule's backward may have to re-run the forward with the same teacher; the fused one never does
         ctx.teacher = None if ctx.fused else teacher
         if ids is not None:
@@ -722,6 +740,8 @@ class _SigmoidLossFn(torch.autograd.Function):
             engine.set_extra_image_ids(extra_img_ids)
         if weights is not None:
             engine.set_sample_weights(*weights)
+        if groups is not None:
+            engine.set_groups(*groups)
         if metrics is not None:
             engine.request_metrics(*metrics[:3])
             if len(metrics) > 3:   # metrics_topk = K > 1: (K, recall, i2t_topk, t2i_topk) follow
@@ -783,6 +803,8 @@ class _SigmoidLossFn(torch.autograd.Function):
                     eng.set_extra_image_ids(ctx.extra_img_ids)
                 if ctx.weights is not None:
                     eng.set_sample_weights(*ctx.weights)
+                if ctx.groups is not None:
+                    eng.set_groups(*ctx.groups)
                 if ctx.teacher is not None:
                     eng.set_teacher(*ctx.teacher)
                 eng.forward(img_b, txt_b, tp, b, True)
@@ -801,15 +823,17 @@ class _SigmoidLossFn(torch.autograd.Function):
                 gt = dtxt.to(tdt) if ctx.needs_input_grad[1] else None
         gp = dtp.reshape(pshape).to(device=pdev, dtype=pdt) if ctx.needs_input_grad[2] else None
         gb = db.reshape(bshape).to(device=bdev, dtype=bdt) if ctx.needs_input_grad[3] else None
-        return gi, gt, gp, gb, None, None, None, None, None, None, None, None, None, None
+        return gi, gt, gp, gb, None, None, None, None, None, None, None, None, None, None, None
 
 
 class _EngineCache:
     def __init__(self, group=None, cta_group: int = 2, overlap_pull: bool = True, sync_scalar_grads: bool = False,
                  bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
                  extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
-                 distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None):
+                 distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None,
+                 exclude_groups: bool = False):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
+        self.exclude_groups = exclude_groups
         self.sigma_budget_bytes = sigma_budget_bytes
         self.distill = distill
         self.extra_images = extra_images
@@ -853,6 +877,8 @@ class _EngineCache:
                 eng.set_option(_capi.SIGLIP_OPT_SAMPLE_WEIGHTS, 1)
             if self.distill is not None:
                 eng.set_option(_capi.SIGLIP_OPT_DISTILL, 1)
+            if self.exclude_groups:
+                eng.set_option(_capi.SIGLIP_OPT_EXCLUDE_GROUPS, 1)
             if self.sigma_budget_bytes:
                 eng.set_sigma_budget(self.sigma_budget_bytes)
             self._engines[key] = eng
@@ -1036,6 +1062,49 @@ def _weights_of(sample_weights: bool, image_weights, text_weights, image_embeddi
     tw = _validate_weights(text_weights, sample_weights, nt + extras if nt is not None else None, "text_weights",
                            text_embeddings.device)
     return (iw, tw) if sample_weights else None
+
+
+def _validate_exclude_groups(exclude_groups, distill) -> bool:
+    """exclude_groups of a module: a bool, and not together with distill (the distillation loss kernel has no group
+    comparisons)."""
+    if not isinstance(exclude_groups, bool):
+        raise RuntimeError(f"exclude_groups must be a bool, got {type(exclude_groups).__name__}")
+    if exclude_groups and distill is not None:
+        raise RuntimeError("exclude_groups cannot be combined with distill: the distillation loss kernel does not "
+                           "exclude pairs")
+    return exclude_groups
+
+
+def _validate_group_ids(groups, n: Optional[int], name: str, what: str, device: torch.device) -> torch.Tensor:
+    if groups is None:
+        raise RuntimeError(f"exclude_groups=True: forward needs {name} ([{n}] integer tensor, one group per {what[:-1]})")
+    if not isinstance(groups, torch.Tensor) or groups.dtype not in _ID_DTYPES:
+        raise RuntimeError(f"{name} must be an integer tensor, got "
+                           f"{groups.dtype if isinstance(groups, torch.Tensor) else type(groups)}")
+    if groups.dim() != 1 or groups.shape[0] != n:
+        raise RuntimeError(f"{name} must have shape [{n}] (one group per {what[:-1]}), got {tuple(groups.shape)}")
+    if groups.device != device:
+        raise RuntimeError(f"{name} are on {groups.device}, the {what} on {device}")
+    return groups.to(torch.int64).contiguous()
+
+
+def _groups_of(exclude_groups: bool, image_groups, text_groups, image_embeddings: torch.Tensor,
+               text_embeddings: torch.Tensor, extras: int, extra_images: int):
+    """image_groups / text_groups of a forward: both required with exclude_groups, refused without. The images are the
+    paired ones followed by the extra images ([B + K_img]), the texts the paired ones followed by the hard negatives or
+    extra texts ([B + K]). Returns them as contiguous int64, or None. Raises before any GPU work."""
+    if not exclude_groups:
+        for name, v in (("image_groups", image_groups), ("text_groups", text_groups)):
+            if v is not None:
+                raise RuntimeError(f"{name} given, but the loss was built without exclude_groups=True")
+        return None
+    ni = image_embeddings.shape[0] if image_embeddings.dim() >= 1 else None
+    nt = text_embeddings.shape[0] if text_embeddings.dim() >= 1 else None
+    gi = _validate_group_ids(image_groups, ni + extra_images if ni is not None else None, "image_groups", "images",
+                             image_embeddings.device)
+    gt = _validate_group_ids(text_groups, nt + extras if nt is not None else None, "text_groups", "texts",
+                             text_embeddings.device)
+    return gi, gt
 
 
 def _with_negatives(text_embeddings: torch.Tensor, negative_text) -> torch.Tensor:
@@ -1280,13 +1349,24 @@ class DDPSigmoidLoss(nn.Module):
     the top-1 metrics). ``recall[0]`` and column 0 are the top-1 rate and index bit for bit; loss and gradients are
     unchanged. K = 1 or None returns today's dict. Not with ``distill``; works under ``torch.no_grad()`` (evaluation,
     mining). Collective: every rank asks the same K on the same steps.
+
+    ``exclude_groups=True``: every ``forward`` also takes ``image_groups`` ([B + K_img] integers: the paired images, then
+    ``extra_image``) and ``text_groups`` ([B + K] integers: the captions, then ``negative_text`` / ``extra_text``) on the
+    embeddings' device; a negative group is "no group". A pair that is positive by the other options stays positive;
+    any other pair whose image and text share a group (on any rank) is excluded: it adds exactly 0 to the loss, the
+    gradients, ``t_prime.grad`` / ``bias.grad`` and the per-sample losses, neither pulled together nor pushed apart
+    (near-duplicates, dedup clusters, class labels: in-batch false negatives). The loss still divides by B. Unique groups
+    give exactly the step without the option. Retrieval metrics and top-K lists are unchanged: every pair stays a
+    candidate; the lists hold global indices, so a caller can look the groups up. Works with or without
+    ``multi_positive``; not with ``distill``. Collective: set on every rank.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
                  normalize_inputs: bool = False, sync_scalar_grads: bool = False, fused_step: Optional[bool] = None,
                  batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
                  extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
-                 distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None) -> None:
+                 distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None,
+                 exclude_groups: bool = False) -> None:
         super().__init__()
         _sigma_budget_mib(sigma_budget_bytes)
         hard_negatives = _validate_hard_negatives(hard_negatives)
@@ -1294,6 +1374,7 @@ class DDPSigmoidLoss(nn.Module):
         extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
         sample_weights = _validate_sample_weights(sample_weights)
         distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images)
+        exclude_groups = _validate_exclude_groups(exclude_groups, distill)
         self.t_prime = nn.Parameter(torch.tensor(math.log(10), dtype=torch.float64))
         self.bias = nn.Parameter(torch.tensor(-10.0))
         self.gpu_batch_size = gpu_batch_size
@@ -1319,10 +1400,13 @@ class DDPSigmoidLoss(nn.Module):
         self.extra_images = extra_images
         # extension: distillation from a frozen teacher (soft targets from the teacher's embeddings)
         self.distill = distill
+        # extension: same-group pairs excluded from the loss (in-batch false negatives made neutral)
+        self.exclude_groups = exclude_groups
         self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank,
                                    multi_positive=multi_positive, hard_negatives=hard_negatives,
                                    extra_texts=extra_texts, sample_weights=sample_weights, extra_images=extra_images,
-                                   distill=distill, sigma_budget_bytes=sigma_budget_bytes)
+                                   distill=distill, sigma_budget_bytes=sigma_budget_bytes,
+                                   exclude_groups=exclude_groups)
         # extension: bound of the 16-bit sigma operands; steps then run in row panels (memory O(budget), not O(B^2))
         self.sigma_budget_bytes = sigma_budget_bytes
 
@@ -1341,7 +1425,8 @@ class DDPSigmoidLoss(nn.Module):
                 extra_image_ids: Optional[torch.Tensor] = None, teacher_image: Optional[torch.Tensor] = None,
                 teacher_text: Optional[torch.Tensor] = None, teacher_t_prime: Optional[torch.Tensor] = None,
                 teacher_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False,
-                metrics_topk: Optional[int] = None):
+                metrics_topk: Optional[int] = None, image_groups: Optional[torch.Tensor] = None,
+                text_groups: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
         _validate_return_sample_losses(return_sample_losses, self.distill)
         topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill)
@@ -1356,6 +1441,8 @@ class DDPSigmoidLoss(nn.Module):
         ximg_ids = _validate_extra_image_ids(extra_image_ids, self.extra_images, self.multi_positive, image_embeddings)
         weights = _weights_of(self.sample_weights, image_weights, text_weights, image_embeddings, text_embeddings,
                               self.hard_negatives + self.extra_texts, self.extra_images)
+        groups = _groups_of(self.exclude_groups, image_groups, text_groups, image_embeddings, text_embeddings,
+                            self.hard_negatives + self.extra_texts, self.extra_images)
         _validate(image_embeddings, text_embeddings, self.gpu_batch_size)
         text_embeddings = _with_negatives(_with_negatives(text_embeddings, negative_text), extra_text)
         image_embeddings = _with_negatives(image_embeddings, extra_image)
@@ -1368,7 +1455,7 @@ class DDPSigmoidLoss(nn.Module):
         lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
         loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
                                     self.normalize_inputs, fused, ids, bufs, extra_ids, weights, ximg_ids, teacher,
-                                    lbufs)
+                                    lbufs, groups)
         return _with_outputs(loss, bufs, lbufs)
 
 
@@ -1394,13 +1481,14 @@ class SigLipLoss(nn.Module):
     convention of ``logit_scale`` / ``logit_bias``), distillation from a frozen teacher as in ``DDPSigmoidLoss``.
     ``return_sample_losses=True``: also returns the per-sample losses of ``DDPSigmoidLoss`` (``image_loss`` [R],
     ``text_loss`` [T]) as the last element, after the metrics when both are asked; like the metrics they stay out of
-    the ``output_dict``."""
+    the ``output_dict``. ``exclude_groups=True``: every forward takes ``image_groups`` [B + K_img] and ``text_groups``
+    [B + K], and same-group pairs that are not positives are excluded from the loss, as in ``DDPSigmoidLoss``."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
                  multi_positive: bool = False, hard_negatives: int = 0, extra_texts: int = 0,
                  sample_weights: bool = False, extra_images: int = 0, distill: Optional[float] = None,
-                 sigma_budget_bytes: Optional[int] = None):
+                 sigma_budget_bytes: Optional[int] = None, exclude_groups: bool = False):
         super().__init__()
         _sigma_budget_mib(sigma_budget_bytes)
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
@@ -1409,7 +1497,9 @@ class SigLipLoss(nn.Module):
         extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
         sample_weights = _validate_sample_weights(sample_weights)
         distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images)
+        exclude_groups = _validate_exclude_groups(exclude_groups, distill)
         self.distill = distill
+        self.exclude_groups = exclude_groups
         self.cache_labels, self.rank, self.world_size, self.bidir = cache_labels, rank, world_size, bidir
         self.use_horovod = use_horovod
         self.fused_step = fused_step
@@ -1420,7 +1510,8 @@ class SigLipLoss(nn.Module):
         self.extra_images = extra_images
         self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive,
                                    hard_negatives=hard_negatives, extra_texts=extra_texts, sample_weights=sample_weights,
-                                   extra_images=extra_images, distill=distill, sigma_budget_bytes=sigma_budget_bytes)
+                                   extra_images=extra_images, distill=distill, sigma_budget_bytes=sigma_budget_bytes,
+                                   exclude_groups=exclude_groups)
         # bound of the 16-bit sigma operands; steps then run in row panels (as on DDPSigmoidLoss)
         self.sigma_budget_bytes = sigma_budget_bytes
 
@@ -1432,7 +1523,8 @@ class SigLipLoss(nn.Module):
                 extra_image_ids: Optional[torch.Tensor] = None, teacher_image: Optional[torch.Tensor] = None,
                 teacher_text: Optional[torch.Tensor] = None, teacher_logit_scale: Optional[torch.Tensor] = None,
                 teacher_logit_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False,
-                metrics_topk: Optional[int] = None):
+                metrics_topk: Optional[int] = None, image_groups: Optional[torch.Tensor] = None,
+                text_groups: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
         _validate_return_sample_losses(return_sample_losses, self.distill)
         topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill)
@@ -1447,6 +1539,8 @@ class SigLipLoss(nn.Module):
         ximg_ids = _validate_extra_image_ids(extra_image_ids, self.extra_images, self.multi_positive, image_features)
         weights = _weights_of(self.sample_weights, image_weights, text_weights, image_features, text_features,
                               self.hard_negatives + self.extra_texts, self.extra_images)
+        groups = _groups_of(self.exclude_groups, image_groups, text_groups, image_features, text_features,
+                            self.hard_negatives + self.extra_texts, self.extra_images)
         _validate(image_features, text_features, None)
         batch = image_features.shape[0]
         text_features = _with_negatives(_with_negatives(text_features, negative_text), extra_text)
@@ -1465,6 +1559,6 @@ class SigLipLoss(nn.Module):
         bufs = _topk_buffers(eng, topk, bufs)
         lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
         loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs,
-                                    extra_ids, weights, ximg_ids, teacher, lbufs)
+                                    extra_ids, weights, ximg_ids, teacher, lbufs, groups)
         out = {"contrastive_loss": loss} if output_dict else loss
         return _with_outputs(out, bufs, lbufs)

@@ -165,6 +165,16 @@ enum {
                                        and returns SIGLIP_ERR_STATE when they exceed the budget. The host-buffer entries
                                        run siglip_fwd_bwd and so run under the budget. Setting it releases the operands
                                        (and any forward saved for backward). Per rank; default 0 */
+  SIGLIP_OPT_EXCLUDE_GROUPS = 27, /* 1: pairs of the same group are excluded from the loss. Every image (paired, then
+                                     extra: [R_r]) and every text (paired, then extra: [T_r]) carries an int64 group id;
+                                     a negative id is "no group". A pair that the other options make positive stays
+                                     positive; any other pair (i, j) with image_group[i] == text_group[j] >= 0 adds
+                                     exactly 0 to the loss, the sigma operand, dt' / dbias, dimg / dtxt and the
+                                     per-sample losses (the loss still divides by B_r). Metrics and top-K lists are
+                                     unchanged. Every step needs siglip_set_groups since the previous step (else
+                                     SIGLIP_ERR_STATE before any launch); the text groups travel to the other ranks with
+                                     the text. Unavailable with SIGLIP_OPT_DISTILL and in the host-buffer entries
+                                     (SIGLIP_ERR_STATE). Collective. Default 0 */
   SIGLIP_OPT_AUX_TRACE = 18 /* 1: record globaltimer stamps of the auxiliary warps of CTA 0 for every launch (start,
                                last peer flag seen, jobs done, end of launch); read with siglip_ctx_aux_trace */
 };
@@ -403,6 +413,16 @@ int siglip_set_extra_image_ids(siglip_ctx* ctx, const int64_t* ids_dev, void* cu
 int siglip_set_sample_weights(siglip_ctx* ctx, const float* image_w, const float* text_w, void* cuda_stream);
 
 /*
+ * SIGLIP_OPT_EXCLUDE_GROUPS: the group ids of this rank's images (image_groups, [R_r] int64 device buffer: its paired
+ * images, then its extra images) and texts (text_groups, [T_r]: its paired texts, then its extras) for the NEXT
+ * siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd call. Stream-ordered copies into the context: nothing is read on
+ * the host, and a single-rank step with groups can be captured into a CUDA graph, the copies with it. In the mode a step
+ * without this call since the previous step returns SIGLIP_ERR_STATE before launching anything; outside it this call
+ * returns SIGLIP_ERR_STATE.
+ */
+int siglip_set_groups(siglip_ctx* ctx, const int64_t* image_groups, const int64_t* text_groups, void* cuda_stream);
+
+/*
  * In-batch retrieval metrics of the NEXT siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd call (that step only),
  * computed from the logits the loss kernels already hold in registers, without a second similarity GEMM:
  *   i2t_index[i] = argmax_j s_ij over all sum(T) texts, for each of this rank's B images (global text index; with hard
@@ -559,6 +579,9 @@ int siglip_debug_get_slot(siglip_ctx* ctx, int chunk, float* out_dev, void* cuda
  * ([batch of that rank] int64 device buffer: its paired texts only; [T of that rank] under SIGLIP_OPT_EXTRA_TEXT_IDS:
  * its paired texts, then its extras) as the "peer" would have published them. */
 int siglip_debug_set_chunk_ids(siglip_ctx* ctx, int chunk, const int64_t* ids_dev, void* cuda_stream);
+/* The groups twin (SIGLIP_OPT_EXCLUDE_GROUPS): the text groups of chunk `chunk` ([T of that rank] int64 device buffer)
+ * as the "peer" would have published them. */
+int siglip_debug_set_chunk_groups(siglip_ctx* ctx, int chunk, const int64_t* groups_dev, void* cuda_stream);
 /* The weights twin (SIGLIP_OPT_SAMPLE_WEIGHTS): the text weights of chunk `chunk` ([T of that rank] fp32 device buffer,
  * or NULL = ones), clamped like siglip_set_sample_weights, as the "peer" would have published them. */
 int siglip_debug_set_chunk_weights(siglip_ctx* ctx, int chunk, const float* text_w_dev, void* cuda_stream);

@@ -70,6 +70,9 @@ def main() -> int:
                     help="also check the top-K retrieval (metrics_topk=10) against the float64 oracle on exact "
                          "small-integer embeddings: t2i merges every rank's column lists of the own chunk, uneven "
                          "batches, hard negatives, ids with duplicates, fused / split / forward-only")
+    ap.add_argument("--exclude-groups", action="store_true",
+                    help="also check excluded same-group pairs (exclude_groups=True) against the float64 oracle, with "
+                         "and without ids and with hard negatives, on both schedules")
     ap.add_argument("--row-panels", action="store_true",
                     help="also check the fused step in row panels (sigma_budget_bytes forcing several panels) against "
                          "the float64 closed form and against the unbounded step on the same peers: uneven batches "
@@ -654,6 +657,55 @@ def main() -> int:
                     l2.backward()
                     torch.cuda.synchronize()
                     report(f"weights {fused} B={Bs} K={K} ids={with_ids} D={D} rep{rep}", dict(
+                        loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
+                        dimg=rel_f(a.grad.float().cpu(), torch.from_numpy(mine["dimg"])),
+                        dtxt=rel_f(b.grad.float().cpu(), dtxt_ref),
+                        dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
+                        db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
+
+    # ---- excluded groups: each rank's text groups travel with its ids through the peer pulls ------------------------
+    if args.exclude_groups:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from exclude_groups_oracle import closed_form_groups, clustered, group_labels
+        from sample_weights_oracle import label_blocks
+        Bs = [160 + 24 * r for r in range(world)]
+        D, tp, bias, n_groups = 136, math.log(10.0), -5.0, 7
+        rng = np.random.default_rng(5555)
+        for K, with_ids in ((0, False), (0, True), (37, False)):
+            Ts = [b + K for b in Bs]
+            tgs = [rng.integers(0, n_groups, t) for t in Ts]
+            igs = [tg[:b].copy() for tg, b in zip(tgs, Bs)]   # image i shares text i's group
+            imgs = [torch.from_numpy(clustered(ig, D, n_groups, 1, 10 + r)).to(torch.bfloat16) for r, ig in enumerate(igs)]
+            texts = [torch.from_numpy(clustered(tg, D, n_groups, 1, 50 + r)).to(torch.bfloat16) for r, tg in enumerate(tgs)]
+            for gr in igs + tgs:
+                gr[rng.random(len(gr)) < 0.2] = -1
+            ids = [torch.from_numpy(rng.integers(0, 200, b)) for b in Bs] if with_ids else None
+            f = lambda xs: [x.double().numpy() for x in xs]  # noqa: E731
+            labels = group_labels(label_blocks(Bs, Ts, [x.numpy() for x in ids] if ids else None), igs, tgs)
+            ref = closed_form_groups(f(imgs), f(texts), tp, bias, labels, Bs)
+            mine = ref[rank]
+            dtxt_ref = torch.from_numpy(sum(ref[r]["contrib"][rank] for r in range(world)))
+            img, txt = imgs[rank].to(dev), texts[rank].to(dev)
+            for fused in (None, False):
+                modx = DDPSigmoidLoss(Bs[rank], fused_step=fused, batch_per_rank=Bs, multi_positive=with_ids,
+                                      hard_negatives=K, exclude_groups=True).to(dev)
+                with torch.no_grad():
+                    modx.t_prime.fill_(tp)
+                    modx.bias.fill_(bias)
+                for rep in range(2):
+                    modx.zero_grad()
+                    a, b = (x.float().requires_grad_(True) for x in (img, txt))
+                    kw = dict(image_groups=torch.from_numpy(igs[rank]).to(dev),
+                              text_groups=torch.from_numpy(tgs[rank]).to(dev))
+                    if with_ids:
+                        kw["sample_ids"] = ids[rank].to(dev)
+                    if K:
+                        l2 = modx(a, b[:Bs[rank]], negative_text=b[Bs[rank]:], **kw)
+                    else:
+                        l2 = modx(a, b, **kw)
+                    l2.backward()
+                    torch.cuda.synchronize()
+                    report(f"exclude groups {fused} B={Bs} K={K} ids={with_ids} D={D} rep{rep}", dict(
                         loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
                         dimg=rel_f(a.grad.float().cpu(), torch.from_numpy(mine["dimg"])),
                         dtxt=rel_f(b.grad.float().cpu(), dtxt_ref),
