@@ -74,6 +74,7 @@ EXPORTED_SYMBOLS = (
     "siglip_debug_set_mailbox",
     "siglip_debug_set_peer_metric_keys",
     "siglip_debug_set_peer_sample_loss_partials",
+    "siglip_debug_set_peer_sample_loss_poison",
     "siglip_debug_set_peer_topk_keys",
     "siglip_debug_set_peer_extra_image_ids",
     "siglip_ctx_aux_trace",
@@ -257,6 +258,8 @@ def lib() -> ctypes.CDLL:
     L.siglip_request_sample_losses.restype = ci
     L.siglip_debug_set_peer_sample_loss_partials.argtypes = [vp, ci, vp, vp]
     L.siglip_debug_set_peer_sample_loss_partials.restype = ci
+    L.siglip_debug_set_peer_sample_loss_poison.argtypes = [vp, ci, vp, vp]
+    L.siglip_debug_set_peer_sample_loss_poison.restype = ci
     L.siglip_request_topk.argtypes = [vp, ci, vp, vp, vp]
     L.siglip_request_topk.restype = ci
     L.siglip_debug_set_peer_topk_keys.argtypes = [vp, ci, vp, vp]

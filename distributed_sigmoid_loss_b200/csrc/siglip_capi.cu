@@ -2558,6 +2558,20 @@ int siglip_debug_set_peer_sample_loss_partials(siglip_ctx* c, int peer, const in
   return 0;
 }
 
+int siglip_debug_set_peer_sample_loss_poison(siglip_ctx* c, int peer, const int64_t* poison_dev, void* cuda_stream) {
+  if (c == nullptr || poison_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->loopback || peer < 0 || peer >= c->world || peer == c->rank)
+    return fail(SIGLIP_ERR_INVALID,
+                "siglip_debug_set_peer_sample_loss_poison needs a loopback context and a peer rank != own rank");
+  CK(cudaSetDevice(c->device));
+  // the poison words sit lsum_half words behind the sums siglip_debug_set_peer_sample_loss_partials seeds
+  CK(cudaMemcpyAsync(c->loop_lsums + static_cast<size_t>(peer) * lsum_block(c) + lsum_half(c) +
+                         static_cast<size_t>(c->rank) * c->Tmax,
+                     poison_dev, static_cast<size_t>(c->T) * sizeof(int64_t), cudaMemcpyDeviceToDevice,
+                     static_cast<cudaStream_t>(cuda_stream)));
+  return 0;
+}
+
 int siglip_debug_set_peer_metric_keys(siglip_ctx* c, int peer, const uint64_t* keys_dev, void* cuda_stream) {
   if (c == nullptr || keys_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (!c->loopback || peer < 0 || peer >= c->world || peer == c->rank)

@@ -85,6 +85,19 @@ __device__ __forceinline__ uint32_t pack_16x2(float lo, float hi) {
   return r;
 }
 
+// fp16(lo * scale), fp16(hi * scale) in one word (low half = lo), scale > 0: the operand conversions. A finite value
+// saturates at +-65504 (.satfinite: what clamping to the fp16 range before cvt.rn gave, product overflow included), NaN
+// stays NaN, and +-inf stays +-inf, so a non-finite embedding entry reaches the loss and the gradients. .satfinite maps
+// +-inf to +-65504 (0x7bff / 0xfbff), one below the infinities' bits (0x7c00 / 0xfc00): an infinite input adds that one.
+// A clamp with fminf / fmaxf would return the non-NaN operand and turn NaN into -65504.
+__device__ __forceinline__ uint32_t pack_f16x2_scaled(float lo, float hi, float scale) {
+  uint32_t r;
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi * scale), "f"(lo * scale));
+  const uint32_t inf_lo = (__float_as_uint(lo) & 0x7fffffffu) == 0x7f800000u;
+  const uint32_t inf_hi = (__float_as_uint(hi) & 0x7fffffffu) == 0x7f800000u;
+  return r + inf_lo + (inf_hi << 16);
+}
+
 __device__ __forceinline__ void named_barrier_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -1768,9 +1781,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
           uint32_t o[4];
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
-            const float lo = fminf(fmaxf(__uint_as_float(w[q] << 16) * sc, -65504.f), 65504.f);
-            const float hi = fminf(fmaxf(__uint_as_float(w[q] & 0xffff0000u) * sc, -65504.f), 65504.f);
-            o[q] = pack_16x2<true>(lo, hi);
+            o[q] = pack_f16x2_scaled(__uint_as_float(w[q] << 16), __uint_as_float(w[q] & 0xffff0000u), sc);
           }
           return make_uint4(o[0], o[1], o[2], o[3]);
         };
@@ -2362,15 +2373,11 @@ __device__ __forceinline__ void store8(void* base, size_t idx8, const float (&v)
   }
 }
 
-// fp16(v * scale), clamped to the fp16 range: the operand format of the fp32-input path
+// fp16(v * scale), finite values clamped to the fp16 range, NaN and +-inf kept: the operand format of the fp32-input path
 __device__ __forceinline__ void store8_f16(void* base, size_t idx8, const float (&v)[8], float scale) {
   uint32_t o[4];
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const float lo = fminf(fmaxf(v[2 * q] * scale, -65504.f), 65504.f);
-    const float hi = fminf(fmaxf(v[2 * q + 1] * scale, -65504.f), 65504.f);
-    o[q] = pack_16x2<true>(lo, hi);
-  }
+  for (int q = 0; q < 4; ++q) o[q] = pack_f16x2_scaled(v[2 * q], v[2 * q + 1], scale);
   reinterpret_cast<uint4*>(base)[idx8] = make_uint4(o[0], o[1], o[2], o[3]);
 }
 

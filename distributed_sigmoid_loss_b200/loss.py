@@ -384,6 +384,15 @@ class SigmoidLossEngine:
         _capi.check(self._L.siglip_debug_set_peer_sample_loss_partials(self._h, peer, partials.data_ptr(),
                                                                        self._stream()))
 
+    def debug_set_peer_sample_loss_poison(self, peer: int, poison: torch.Tensor) -> None:
+        """Loopback: the poison words ([T] int64; 1: a +inf or too large partial, 2: a NaN partial, 0: none) that go with
+        peer `peer`'s seeded partials; they stay until seeded again."""
+        n = self.texts
+        if poison.dtype != torch.int64 or tuple(poison.shape) != (n,) or not poison.is_contiguous() or \
+                poison.device != self.device:
+            raise RuntimeError(f"peer sample-loss poison must be a contiguous int64 [{n}] tensor on {self.device}")
+        _capi.check(self._L.siglip_debug_set_peer_sample_loss_poison(self._h, peer, poison.data_ptr(), self._stream()))
+
     @property
     def metric_images(self) -> int:
         """Images of this rank that i2t ranks: the paired ones, or all R under SIGLIP_OPT_EXTRA_IMAGE_IDS."""
@@ -1264,7 +1273,9 @@ class DDPSigmoidLoss(nn.Module):
     ``nn.Parameter``s with the reference's state_dict keys; hand them to the optimizer (README.md:20).
     Embeddings are expected L2-normalised by the caller (distributed_sigmoid_loss.py:20); with
     ``normalize_inputs=False`` values must satisfy |x| <= 4094 (the gradient kernels consume fp16(16 x) copies;
-    unit-norm embeddings are six orders of magnitude inside that).
+    unit-norm embeddings are six orders of magnitude inside that). NaN and ±inf in the embeddings, ``t_prime`` or
+    ``bias`` are never turned into finite values: the loss and each gradient element are non-finite where autograd of
+    the reference is, so ``torch.amp.GradScaler`` skips the step of a tower that overflowed under autocast.
     Every rank of ``group`` must call ``forward`` the same number of times (collective, like all_gather).
 
     Limits (also reported by the C library when violated): all ranks of ``group`` must be GPUs of ONE node with NVLink /

@@ -14,6 +14,9 @@
  * row-major [T, D] one (T = B unless the context was created with siglip_ctx_create_texts / _extras: then this rank's T
  * texts are its B paired captions followed by its hard negatives), 16-byte aligned, D % 8 == 0. `dimg` [R, D] and
  * `dtxt` [T, D] are row-major fp32 (or bf16 with SIGLIP_OPT_GRAD_BF16). Scalars are fp32 device scalars.
+ * Non-finite inputs: NaN and +-inf embedding entries, t' and bias reach every output they touch (every conversion to an
+ * operand format keeps them), so each output element is non-finite where float64 autograd of the loss on the same
+ * operand values is (NaN and inf are not told apart), and per-sample losses are NaN or +inf as documented there.
  */
 #ifndef SIGLIP_B200_H_
 #define SIGLIP_B200_H_
@@ -602,6 +605,10 @@ int siglip_debug_set_peer_topk_keys(siglip_ctx* ctx, int peer, const uint64_t* k
  * numbers the kernel did not produce itself. */
 int siglip_debug_set_peer_sample_loss_partials(siglip_ctx* ctx, int peer, const int64_t* partials_dev,
                                                void* cuda_stream);
+/* Loopback only: seed the poison words that go with those partials ([T] 64-bit words, bit 0: a partial that was +inf
+ * or not below 2^16, bit 1: a NaN partial; 0: none), so that the cross-rank OR of a per-sample-loss step sees poison the
+ * kernel did not produce itself. They stay until seeded again. */
+int siglip_debug_set_peer_sample_loss_poison(siglip_ctx* ctx, int peer, const int64_t* poison_dev, void* cuda_stream);
 /* Loopback only (SIGLIP_OPT_EXTRA_IMAGE_IDS): seed the extra-image ids that stand in for what peer rank `peer` publishes
  * in a metrics step ([R_peer - B_peer] int64 device buffer), so that a t2i winner among its extra images is judged by
  * ids the test chose. */

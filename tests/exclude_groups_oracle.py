@@ -86,21 +86,88 @@ def text_loss_of(res: List[Dict], c: int) -> np.ndarray:
     return sum(x["text_part"][c] for x in res)
 
 
-def torch_loss(img, txt, t_prime, bias, y, image_w=None, text_w=None, normalize: bool = False, batch=None):
-    """A direct torch restatement of one rank's loss over the whole text set (img [R, D], txt [T, D], y [R, T] in
-    {+1, -1, 0}): sum over the pairs with |y| = 1 of a_i c_j softplus(-y z) / B. Differentiable in every input."""
+def torch_terms(img, txt, t_prime, bias, y, image_w=None, text_w=None, normalize: bool = False, teacher=None):
+    """The pair terms of ``torch_loss`` ([R, T]): a_i c_j |y| softplus(-y z). teacher = (timg, ttxt, t'_T, b_T, lambda)
+    gives the distillation terms a_i c_j (softplus(z) - q z) instead, q = (1 - lambda) [y = 1] + lambda sigma(exp(t'_T)
+    <timg_i, ttxt_j> + b_T) (normalize=True normalises the teacher rows too; no gradient flows to the teacher).
+    Non-finite inputs propagate as autograd propagates them; the rows and columns of the per-sample losses are the row
+    and column sums of these terms."""
     import torch
 
+    F = torch.nn.functional
     if normalize:
-        img, txt = torch.nn.functional.normalize(img, dim=-1), torch.nn.functional.normalize(txt, dim=-1)
+        img, txt = F.normalize(img, dim=-1), F.normalize(txt, dim=-1)
     z = torch.exp(t_prime) * (img @ txt.T) + bias
     w = y.abs()
     if image_w is not None:
         w = w * image_w[:, None]
     if text_w is not None:
         w = w * text_w[None, :]
+    if teacher is not None:
+        timg, ttxt, ttp, tb, lam = teacher
+        if normalize:
+            timg, ttxt = F.normalize(timg, dim=-1), F.normalize(ttxt, dim=-1)
+        p = torch.sigmoid(torch.exp(torch.as_tensor(ttp, dtype=z.dtype)) * (timg @ ttxt.T) + tb).detach()
+        q = (1.0 - lam) * (y > 0).to(z.dtype) + lam * p
+        return w * (F.softplus(z) - q * z)
     ys = torch.where(y == 0, -torch.ones_like(y), y)
-    return (w * torch.nn.functional.softplus(-ys * z)).sum() / (img.shape[0] if batch is None else batch)
+    return w * F.softplus(-ys * z)
+
+
+def torch_loss(img, txt, t_prime, bias, y, image_w=None, text_w=None, normalize: bool = False, batch=None,
+               teacher=None):
+    """A direct torch restatement of one rank's loss over the whole text set (img [R, D], txt [T, D], y [R, T] in
+    {+1, -1, 0}): sum over the pairs with |y| = 1 of a_i c_j softplus(-y z) / B (teacher: the distillation terms of
+    ``torch_terms``). Differentiable in every input."""
+    terms = torch_terms(img, txt, t_prime, bias, y, image_w, text_w, normalize, teacher)
+    return terms.sum() / (img.shape[0] if batch is None else batch)
+
+
+def operand_values(x):
+    """The values the kernels consume for an embedding tensor x, as float64: bf16 entries as they are; fp32 / fp16
+    entries rounded through fp16(16 x) / 16, saturated at +-4094 (65504 / 16) outside the supported range; NaN and +-inf
+    kept as they are."""
+    import torch
+
+    x64 = x.detach().double()
+    if x.dtype == torch.bfloat16:
+        return x64
+    r = (x.detach().float() * 16.0).clamp(-65504.0, 65504.0).half().double() / 16.0
+    return torch.where(torch.isfinite(x64), r, x64)
+
+
+ROW_PARTIAL_COLS = 128   # a row's per-sample-loss partial: one loss tile's columns of one text chunk
+COL_PARTIAL_ROWS = 16    # a column's partial: one warp's 16 rows of one loss tile
+MAX_PARTIAL = 2.0 ** 16
+
+
+def _partial_class(parts) -> np.ndarray:
+    """Per sample (axis 0 of parts, partials along axis 1): 2 for a NaN partial, 1 for a +inf or >= 2^16 one, else 0."""
+    nan = np.isnan(parts).any(axis=1)
+    big = (np.nan_to_num(parts, nan=0.0, posinf=np.inf) >= MAX_PARTIAL).any(axis=1)
+    return np.where(nan, 2, np.where(big, 1, 0))
+
+
+def sample_loss_classes(terms, chunk_texts, rows: Optional[int] = None) -> Dict[str, np.ndarray]:
+    """What the per-sample losses of one rank hold, from its pair terms ([R, sum T_c] float64, chunks side by side):
+    image_loss[i] is NaN if one of its row partials (ROW_PARTIAL_COLS columns of a chunk) is NaN, +inf if one is +inf
+    or not below 2^16, else the row sum; text_loss_part[j] (this rank's share of text j's loss) the same over column
+    partials of COL_PARTIAL_ROWS rows. rows: the rows that belong to the step (default: all)."""
+    terms = np.asarray(terms, np.float64)
+    R = terms.shape[0] if rows is None else rows
+    terms = terms[:R]
+    rparts, lo = [], 0
+    for T in chunk_texts:
+        for c0 in range(lo, lo + T, ROW_PARTIAL_COLS):
+            rparts.append(terms[:, c0:min(c0 + ROW_PARTIAL_COLS, lo + T)].sum(axis=1))
+        lo += T
+    cparts = [terms[r0:r0 + COL_PARTIAL_ROWS].sum(axis=0) for r0 in range(0, R, COL_PARTIAL_ROWS)]
+
+    def decode(total, cls):
+        return np.where(cls == 2, np.nan, np.where(cls == 1, np.inf, total))
+
+    return dict(image_loss=decode(terms.sum(axis=1), _partial_class(np.stack(rparts, axis=1))),
+                text_loss_part=decode(terms.sum(axis=0), _partial_class(np.stack(cparts, axis=1))))
 
 
 def clustered(groups, D: int, n_clusters: int, seed: int, noise_seed: int, spread: float = 0.7) -> np.ndarray:

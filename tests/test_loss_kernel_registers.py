@@ -36,3 +36,5 @@ def test_loss_kernels_keep_168_registers_and_no_spills():
     for n, u in loss.items():
         assert re.search(r"\bREG:168\b", u), (n, u)
         assert re.search(r"\bLOCAL:0\b", u), (n, u)
+        # the kernel's own 16-byte frame: a register spill goes to the stack and grows it (LOCAL stays 0)
+        assert re.search(r"\bSTACK:16\b", u), (n, u)

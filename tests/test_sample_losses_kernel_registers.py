@@ -30,3 +30,5 @@ def test_sample_loss_kernels_use_168_registers_and_no_spills():
     for n, u in kern.items():
         assert re.search(r"\bREG:168\b", u), (n, u)
         assert re.search(r"\bLOCAL:0\b", u), (n, u)
+        # the kernel's own 16-byte frame: a register spill goes to the stack and grows it (LOCAL stays 0)
+        assert re.search(r"\bSTACK:16\b", u), (n, u)
