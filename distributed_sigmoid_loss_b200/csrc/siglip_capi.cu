@@ -1628,7 +1628,14 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
     const int p0 = p * P, rows = prow(p), gb = (W > 1) ? 1 : 0;
     const bool first_launch = (W == 1 && p == np - 1);
     AuxList aux;
-    if (first_launch) add_cvt_jobs(c, aux, 0, true, img, own_txt, c->T);
+    if (first_launch) {
+      add_cvt_jobs(c, aux, 0, true, img, own_txt, c->T);
+      // A loss launch's grid follows its panel's row tiles, and this shortest panel runs first: its CTAs overwrite
+      // their partial slots only. L0.0, the largest panel, runs last and adds into every slot, so the slots past this
+      // launch's grid would carry the previous step's sums into this step's loss, dt' and dbias.
+      CK(cudaMemsetAsync(c->partials, 0, static_cast<size_t>(c->num_sms) * 4 * sizeof(double), st));
+      c->launches++;
+    }
     if (W > 1 && p == np - 1) {
       if (img_cvt_in_l1) add_img_cvt_job(c, aux, img);
       if (l0_work_in_l1) {
@@ -2450,25 +2457,30 @@ int siglip_set_groups(siglip_ctx* c, const int64_t* image_groups, const int64_t*
   return 0;
 }
 
+// one rank: the key blocks are allocated on the first request that reduces argmax keys (siglip_request_metrics, or
+// siglip_request_topk with K = 1), so a context that never asks holds exactly the workspace it held without them.
+// (world > 1: they are part of the exported text allocation.) The allocation is not a stream operation; the relaxed
+// capture mode lets a first request inside a CUDA-graph capture make it, as PyTorch's caching allocator does.
+static int ensure_metric_keys(siglip_ctx* c) {
+  if (c->mkeys[0] != nullptr) return 0;
+  const size_t bytes = 2 * mkeys_block(c) * sizeof(unsigned long long);
+  CK(cudaSetDevice(c->device));
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  CK(cudaThreadExchangeStreamCaptureMode(&mode));
+  unsigned long long* keys = nullptr;
+  const cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&keys), bytes);
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  CK(e);
+  c->mkeys[0] = keys;
+  c->mkeys[1] = keys + mkeys_block(c);
+  c->workspace_bytes += bytes;
+  return 0;
+}
+
 int siglip_request_metrics(siglip_ctx* c, float* top1, int64_t* i2t_index, int64_t* t2i_index) {
   if (c == nullptr || top1 == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument (top1 is required)");
-  if (c->mkeys[0] == nullptr) {
-    // one rank: the key blocks are allocated on the first request, so a context that never asks for metrics holds
-    // exactly the workspace it held without them. (world > 1: they are part of the exported text allocation.) The
-    // allocation is not a stream operation; the relaxed capture mode lets a first request inside a CUDA-graph capture
-    // make it, as PyTorch's caching allocator does.
-    const size_t bytes = 2 * mkeys_block(c) * sizeof(unsigned long long);
-    CK(cudaSetDevice(c->device));
-    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
-    CK(cudaThreadExchangeStreamCaptureMode(&mode));
-    unsigned long long* keys = nullptr;
-    const cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&keys), bytes);
-    cudaThreadExchangeStreamCaptureMode(&mode);
-    CK(e);
-    c->mkeys[0] = keys;
-    c->mkeys[1] = keys + mkeys_block(c);
-    c->workspace_bytes += bytes;
-  }
+  int rc;
+  if ((rc = ensure_metric_keys(c))) return rc;
   c->m_top1 = top1;
   c->m_i2t = i2t_index;
   c->m_t2i = t2i_index;
@@ -2506,6 +2518,8 @@ int siglip_request_topk(siglip_ctx* c, int k, float* recall, int64_t* i2t_topk, 
   if (c == nullptr || recall == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument (recall is required)");
   if (k < 1 || k > SIGLIP_TOPK_MAX) return fail(SIGLIP_ERR_INVALID, "k must be in 1 .. SIGLIP_TOPK_MAX");
   if (c->distill) return fail(SIGLIP_ERR_STATE, "top-K retrieval is unavailable under SIGLIP_OPT_DISTILL");
+  int rc;
+  if (k == 1 && (rc = ensure_metric_keys(c))) return rc;   // K = 1 runs the metrics path on the argmax keys
   if (k > 1 && c->tk_rows[0] == nullptr) {
     // the row lists (and on one rank the column lists ahead of them) are allocated by the first request, so a context
     // that never asks holds exactly the workspace it held without them; allowed inside a CUDA-graph capture

@@ -1,0 +1,454 @@
+"""The loss step's options in combination: a table of cells and a composed float64 oracle — test infrastructure, never
+the product path.
+
+Every cell turns on a set of options (sample ids, extra texts / images with or without ids, weights, excluded groups, a
+teacher, per-sample losses, metrics, top-K) and picks the engine configuration it runs under (W, bidir, schedule, row
+panels, INPUT_F16, gradient tile width, stages, cluster shape). ``route`` restates how ``launch_gemm`` picks the loss
+kernel for each launch of the step, so the table's coverage of kernel instantiations and runtime branches is derived,
+not claimed. ``oracle`` composes the single-feature oracles (no new loss math); ``retrieval`` and ``peer_stand_ins``
+give the exact retrieval results and what the loopback hooks need to stand in for the other ranks.
+
+Planted data: every embedding entry is a small integer / 8, so the bf16 and fp16(16 x) operands are exact and every fp32
+logit equals its float64 value; retrieval is compared exactly. Samples are integer cluster centres (one per group) plus
+an integer vector per sample id plus sparse noise: duplicate ids are near-duplicates, captions and extras lie near their
+image, and same-group negatives have sigma(z) ~ 0.12 at t = 5, bias = -6 (against ~0.003 for the other negatives), so
+the excluded pairs carry weight while a flipped label still moves a step's loss by more than 20x the tolerance."""
+from __future__ import annotations
+
+import dataclasses
+import itertools
+import math
+from dataclasses import dataclass
+from typing import Dict, List, Optional
+
+import numpy as np
+
+from distill_oracle import closed_form_distill
+from exclude_groups_oracle import closed_form_groups, group_labels, text_loss_of
+from extra_images_oracle import label_blocks
+from retrieval_metrics_oracle import key_as_int64, metric_key
+from retrieval_topk_oracle import recall_counts, topk_retrieval
+from sample_losses_oracle import fixed_point_partial
+
+TP, BIAS = math.log(5.0), -6.0
+TTP, TBIAS, LAM = math.log(3.0), -2.0, 0.6   # the teacher's t', bias and the distillation weight lambda
+TOL = 1e-3
+KMAX = 10   # SIGLIP_TOPK_MAX: the width of a peer's seeded top-K column lists
+D, DT = 136, 72
+N_GROUPS = 10
+
+MODES = ("loss", "sample_loss", "topk", "groups", "distill")
+CONTEXTS = ("plain", "hn", "xt", "xi", "xin", "both")
+SCHEDS = ("fused", "split", "fwd")
+CLUSTERS = {1: [(1, 1)], 2: [(2, 1), (1, 2)], 4: [(2, 2)]}   # cluster size -> (cta_group, mcast)
+DISTILL_STAGES = 4   # kDistillStages: the distillation kernel runs 4 stages whatever the request
+
+# per-rank paired batches, extra texts and extra images of each world size (uneven, ragged past 256 at W = 1); the
+# panel cells use larger batches so that a budget of a few MiB splits the rows into several panels
+SHAPES = {1: ((300,), (37,), (23,)), 2: ((200, 136), (29, 41), (17, 30)), 3: ((136, 200, 160), (19, 0, 33), (9, 27, 13))}
+PANEL_SHAPES = {1: ((700,), (60,), (48,)), 2: ((600, 520), (40, 72), (24, 36)),
+                3: ((520, 456, 600), (8, 40, 0), (36, 12, 20))}
+
+
+@dataclass(frozen=True)
+class Options:
+    """What a step computes. Extra-text / extra-image ids need sample ids; a teacher takes none of the extras, groups,
+    per-sample losses or top-K (the documented refusals)."""
+    ids: bool = False
+    xtexts: bool = False     # extra texts: hard negatives, or with xt_ids further captions
+    ximages: bool = False    # extra images: hard negatives, or with xi_ids further images of a caption
+    xt_ids: bool = False
+    xi_ids: bool = False
+    weights: bool = False
+    groups: bool = False
+    teacher: bool = False
+    metrics: bool = False    # siglip_request_metrics (top-1)
+    losses: bool = False     # siglip_request_sample_losses
+    topk: int = 0            # siglip_request_topk's K; K = 1 runs the metrics path
+
+    @property
+    def context(self) -> str:
+        if self.xtexts and self.ximages:
+            return "both"
+        if self.xtexts:
+            return "xt" if self.xt_ids else "hn"
+        if self.ximages:
+            return "xi" if self.xi_ids else "xin"
+        return "plain"
+
+    @property
+    def keys(self) -> bool:
+        """The step reduces argmax keys (row_keys): a metrics request or a K = 1 top-K request."""
+        return self.metrics or self.topk == 1
+
+    def valid(self) -> bool:
+        if (self.xt_ids and not (self.ids and self.xtexts)) or (self.xi_ids and not (self.ids and self.ximages)):
+            return False
+        return not (self.teacher and (self.xtexts or self.ximages or self.groups or self.losses or self.topk > 1))
+
+    def removals(self) -> Dict[str, "Options"]:
+        """Each option this step turns on that changes its labels, weights or targets, switched off on its own (with
+        what it needs: ids take the extras' ids along)."""
+        r = dataclasses.replace
+        out = {}
+        if self.xtexts:
+            out["extra texts"] = r(self, xtexts=False, xt_ids=False)
+        if self.ximages:
+            out["extra images"] = r(self, ximages=False, xi_ids=False)
+        if self.ids:
+            out["ids"] = r(self, ids=False, xt_ids=False, xi_ids=False)
+        if self.xt_ids:
+            out["extra text ids"] = r(self, xt_ids=False)
+        if self.xi_ids:
+            out["extra image ids"] = r(self, xi_ids=False)
+        if self.weights:
+            out["weights"] = r(self, weights=False)
+        if self.groups:
+            out["groups"] = r(self, groups=False)
+        if self.teacher:
+            out["teacher"] = r(self, teacher=False)
+        return out
+
+
+@dataclass(frozen=True)
+class Cell:
+    opts: Options
+    W: int
+    r: int
+    bidir: bool
+    sched: str
+    panels: bool
+    f16: bool
+    tile_n: int
+    stages: int
+    cg: int
+    mcast: int
+    seed: int
+
+    @property
+    def mode(self) -> str:
+        return mode_of(self.opts)
+
+    @property
+    def cluster(self) -> int:
+        return self.cg * self.mcast
+
+    @property
+    def name(self) -> str:
+        o = self.opts
+        on = [k for k in ("ids", "xt_ids", "xi_ids", "weights", "groups", "teacher", "metrics", "losses")
+              if getattr(o, k)]
+        on += [f"k{o.topk}"] if o.topk else []
+        return (f"{self.seed:03d}-{self.mode}-{o.context}-{'+'.join(on) or 'none'}-W{self.W}r{self.r}"
+                f"{'-bidir' if self.bidir else ''}-{self.sched}{'-panels' if self.panels else ''}"
+                f"{'-f16' if self.f16 else ''}-t{self.tile_n}-s{self.stages}-cg{self.cg}m{self.mcast}")
+
+    def shapes(self):
+        """(Bs, Rs, Ts) of every rank, as the step sees them."""
+        Bs, K, E = (PANEL_SHAPES if self.panels else SHAPES)[self.W]
+        Ts = tuple(b + (k if self.opts.xtexts else 0) for b, k in zip(Bs, K))
+        Rs = tuple(b + (e if self.opts.ximages else 0) for b, e in zip(Bs, E))
+        return Bs, Rs, Ts
+
+    def budget_mib(self, cluster: Optional[int] = None) -> int:
+        """The smallest SIGLIP_OPT_SIGMA_BUDGET_MIB that runs the fused step in more than one row panel (0: no panels),
+        for the cell's cluster size or another one (siglip_ctx_sigma_panels: panels of whole 128-row cluster blocks)."""
+        if not self.panels:
+            return 0
+        Bs, Rs, Ts = self.shapes()
+        rp, tp = _round_up(max(Rs), 256), _round_up(max(Ts), 256)
+        nbuf, unit = (2 if self.W > 1 else 1), 128 * (cluster or self.cluster)
+        for mib in range(1, 64):
+            rows = mib * 2 ** 20 // (nbuf * tp * 2) // unit * unit
+            if rows and rp * nbuf * tp * 2 > mib * 2 ** 20 and Rs[self.r] > rows:
+                return mib
+        raise AssertionError(f"{self.name}: no budget splits the rows into panels")
+
+
+def _round_up(x, m):
+    return (x + m - 1) // m * m
+
+
+def mode_of(o: Options) -> str:
+    """The loss kernel launch_gemm selects (csrc/siglip_kernels.cu): distillation first, then groups, top-K (K > 1),
+    per-sample losses, and otherwise the plain loss kernel."""
+    if o.teacher:
+        return "distill"
+    if o.groups:
+        return "groups"
+    if o.topk > 1:
+        return "topk"
+    if o.losses:
+        return "sample_loss"
+    return "loss"
+
+
+def route(cell: Cell):
+    """The loss-kernel launches of the cell's step, one per text chunk: (instantiation, runtime options) pairs.
+    An instantiation is (mode, stages, cluster size[, ids, metrics, weights]) — kModeLoss compiles its three options in,
+    the other modes take them at run time. ids is on for a chunk whose labels come from ids: True for every chunk with
+    sample ids, "iota" for the own chunk of a rank with extras of both kinds under positional labels (the positional
+    pairs as iota ids: the same branch, fed differently)."""
+    o = cell.opts
+    mode = mode_of(o)
+    stages = DISTILL_STAGES if mode == "distill" else cell.stages
+    out = set()
+    for c in range(cell.W):
+        ids = True if o.ids else ("iota" if c == cell.r and o.xtexts and o.ximages else False)
+        if mode == "loss":
+            out.add(((mode, stages, cell.cluster, ids, o.keys, o.weights), ()))
+            continue
+        rt = dict(ids=ids, weights=o.weights, metrics=o.keys)
+        if mode in ("topk", "groups"):
+            rt["losses"] = o.losses
+        if mode == "groups":
+            rt["topk"] = o.topk > 1
+        out.add(((mode, stages, cell.cluster), tuple(sorted(rt.items()))))
+    return out
+
+
+def runtime_options(mode: str) -> List[str]:
+    return {"loss": [], "sample_loss": ["ids", "metrics", "weights"], "topk": ["ids", "losses", "metrics", "weights"],
+            "groups": ["ids", "losses", "metrics", "topk", "weights"], "distill": ["ids", "metrics", "weights"]}[mode]
+
+
+def instantiations(mode: str):
+    """Every loss-kernel instantiation launch_gemm can select for a mode."""
+    if mode == "distill":
+        return {(mode, DISTILL_STAGES, cs) for cs in CLUSTERS}
+    base = {(mode, st, cs) for st in (4, 6) for cs in CLUSTERS}
+    if mode != "loss":
+        return base
+    return {b + f for b in base for f in itertools.product((False, True), repeat=3)}
+
+
+def axis_values(mode: str) -> Dict[str, tuple]:
+    """The values of every other axis a mode can be paired with (distillation takes no extras)."""
+    return dict(context=("plain",) if mode == "distill" else CONTEXTS, W=(1, 2, 3), bidir=(False, True), sched=SCHEDS,
+                panels=(False, True), f16=(False, True), tile_n=(128, 256), stages=(4, 6), cluster=(1, 2, 4))
+
+
+def axis_of(cell: Cell, axis: str):
+    return cell.opts.context if axis == "context" else getattr(cell, axis)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the table
+# ---------------------------------------------------------------------------------------------------------------------
+def _combos(names):
+    return [dict(zip(names, v)) for v in itertools.product((False, True), repeat=len(names))]
+
+
+def _mode_rows():
+    """(mode, runtime options, stages, cluster) of every cell: the 48 kModeLoss instantiations, and for every other mode
+    each combination of its runtime options once, cycling through its instantiations."""
+    rows = []
+    for f in _combos(["ids", "metrics", "weights"]):
+        for st in (4, 6):
+            for cs in (1, 2, 4):
+                rows.append(("loss", f, st, cs))
+    for mode in ("sample_loss", "topk", "groups", "distill"):
+        for i, f in enumerate(_combos(runtime_options(mode))):
+            rows.append((mode, f, (4, 6)[(i // 3) % 2], (1, 2, 4)[i % 3]))
+    return rows
+
+
+def _lru_pick(order, ok):
+    """The least recently picked value of `order` that satisfies ok; it moves to the back."""
+    v = next(x for x in order if ok(x))
+    order.remove(v)
+    order.append(v)
+    return v
+
+
+def build_table() -> List[Cell]:
+    cells, counters = [], {}
+    for seed, (mode, f, stages, cs) in enumerate(_mode_rows()):
+        j = counters.setdefault(mode, [0, {}])
+        i, cyc = j[0], j[1]
+        j[0] += 1
+        ids = f.get("ids", False)
+        W = (1, 2, 3)[i % 3]
+        ctx = "plain" if mode == "distill" else _lru_pick(
+            cyc.setdefault("ctx", list(CONTEXTS)),
+            lambda c: (ids or c not in ("xt", "xi")) and (ids or W > 1 or c != "both"))
+        panels = i % 4 == 3
+        sched = "fused" if panels else _lru_pick(cyc.setdefault("sched", list(SCHEDS)), lambda s: True)
+        cg, mcast = CLUSTERS[cs][(i // 2) % len(CLUSTERS[cs])]
+        metrics = f.get("metrics", False)
+        o = Options(ids=ids, xtexts=ctx in ("hn", "xt", "both"), ximages=ctx in ("xi", "xin", "both"),
+                    xt_ids=ids and ctx in ("xt", "both"), xi_ids=ids and ctx in ("xi", "both"),
+                    weights=f.get("weights", False), groups=mode == "groups", teacher=mode == "distill",
+                    # a metrics cell of the modes without a top-K option asks for it as a K = 1 top-K request every
+                    # other time: the same keys, a second set of outputs
+                    metrics=metrics and not (mode in ("loss", "sample_loss") and i % 2),
+                    losses=f.get("losses", False) or mode == "sample_loss",
+                    topk=(5 if mode == "topk" else 3 if f.get("topk") else
+                          1 if metrics and mode in ("loss", "sample_loss") and i % 2 else 0))
+        assert o.valid(), o
+        cells.append(Cell(o, W, i % W, W > 1 and (i // 3) % 2 == 1, sched, panels, (i + i // 4) % 2 == 1,
+                          (128, 256)[(i // 2 + i // 8) % 2], stages, cg, mcast, seed))
+    return cells
+
+
+TABLE = build_table()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# planted data
+# ---------------------------------------------------------------------------------------------------------------------
+@dataclass
+class Problem:
+    """Every rank's embeddings and per-sample inputs for the cell's shapes with all extras present (float64 values of
+    integers / 8); an Options picks which of them a step uses."""
+    Bs: tuple
+    Rs: tuple
+    Ts: tuple
+    imgs: list        # [R_r, D]
+    txts: list        # [T_r, D]
+    ids: list         # [B_r] int64
+    xt_ids: list      # [T_r - B_r]
+    xi_ids: list      # [R_r - B_r]
+    iw: list          # [R_r] fp32 values
+    tw: list          # [T_r]
+    ig: list          # [R_r] int64, -1: no group
+    tg: list          # [T_r]
+    timgs: list       # [B_r, DT] teacher
+    ttxts: list
+
+    def view(self, o: Options):
+        """(Bs, Rs, Ts, imgs, txts) of the step: the extras a step without them does not have are cut off."""
+        Rs = self.Rs if o.ximages else self.Bs
+        Ts = self.Ts if o.xtexts else self.Bs
+        return (self.Bs, Rs, Ts, [x[:n] for x, n in zip(self.imgs, Rs)], [x[:n] for x, n in zip(self.txts, Ts)])
+
+
+def planted(cell: Cell) -> Problem:
+    Bs, K, E = (PANEL_SHAPES if cell.panels else SHAPES)[cell.W]
+    Rs = tuple(b + e for b, e in zip(Bs, E))
+    Ts = tuple(b + k for b, k in zip(Bs, K))
+    g = np.random.default_rng(1000 + cell.seed)
+    centres = g.choice([-1, 0, 1], (N_GROUPS, D), p=[0.2, 0.6, 0.2])
+    n_ids = max(8, sum(Bs) // 2)                       # duplicates within and across ranks
+    id_vec = g.choice([-1, 0, 1], (n_ids, D), p=[0.3, 0.4, 0.3])
+    id_grp = g.integers(0, N_GROUPS, n_ids)
+
+    def near(idv):
+        idv = np.asarray(idv, np.int64)
+        return (centres[id_grp[idv]] + id_vec[idv] + g.choice([-1, 0, 1], (len(idv), D), p=[0.1, 0.8, 0.1])) / 8.0
+
+    def groups_of(idv):
+        gr = id_grp[np.asarray(idv, np.int64)].astype(np.int64)
+        gr[g.random(len(gr)) < 0.2] = -1
+        return gr
+
+    def weights(n):
+        w = g.random(n).astype(np.float32)
+        w[g.random(n) < 0.2] = 0.0
+        return w
+
+    P = dict(imgs=[], txts=[], ids=[], xt_ids=[], xi_ids=[], iw=[], tw=[], ig=[], tg=[], timgs=[], ttxts=[])
+    for b, r_, t_ in zip(Bs, Rs, Ts):
+        ids = g.integers(0, n_ids, b)
+        # extras: a text (image) near a sample of the global id pool; a fifth of the extra images carry a fresh id
+        xt = g.integers(0, n_ids, t_ - b)
+        xi = g.integers(0, n_ids, r_ - b)
+        xi_content = xi.copy()
+        fresh = g.random(r_ - b) < 0.2
+        xi[fresh] = 10 ** 6 + g.integers(0, 10 ** 6, int(fresh.sum()))
+        P["ids"].append(ids.astype(np.int64))
+        P["xt_ids"].append(xt.astype(np.int64))
+        P["xi_ids"].append(xi.astype(np.int64))
+        P["imgs"].append(np.concatenate([near(ids), near(xi_content)]))
+        P["txts"].append(np.concatenate([near(ids), near(xt)]))
+        P["iw"].append(weights(r_))
+        P["tw"].append(weights(t_))
+        P["ig"].append(np.concatenate([groups_of(ids), groups_of(xi_content)]))
+        P["tg"].append(np.concatenate([groups_of(ids), groups_of(xt)]))
+        timg = g.integers(-2, 3, (b, DT))
+        P["timgs"].append(timg / 8.0)
+        P["ttxts"].append((timg + g.choice([-1, 0, 1], (b, DT), p=[0.2, 0.6, 0.2])) / 8.0)
+    return Problem(Bs, Rs, Ts, **P)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the composed oracle
+# ---------------------------------------------------------------------------------------------------------------------
+def labels(P: Problem, o: Options):
+    Bs, Rs, Ts, _, _ = P.view(o)
+    lab = label_blocks(Bs, Rs, Ts, P.ids if o.ids else None, P.xt_ids if o.xt_ids else None,
+                       P.xi_ids if o.xi_ids else None)
+    if o.groups:
+        lab = group_labels(lab, [x[:n] for x, n in zip(P.ig, Rs)], [x[:n] for x, n in zip(P.tg, Ts)])
+    return lab
+
+
+def oracle(P: Problem, o: Options) -> List[Dict]:
+    """Per rank: loss, dimg [R_r, D], contrib[c] [T_c, D], dt_prime, dbias; without a teacher also image_loss [R_r],
+    text_part[c] (this rank's column sums over chunk c) and text_loss [T_r] (every rank's column sums of its chunk)."""
+    Bs, Rs, Ts, imgs, txts = P.view(o)
+    iw = [x[:n].astype(np.float64) for x, n in zip(P.iw, Rs)] if o.weights else None
+    tw = [x[:n].astype(np.float64) for x, n in zip(P.tw, Ts)] if o.weights else None
+    lab = labels(P, o)
+    if o.teacher:
+        return closed_form_distill(imgs, txts, TP, BIAS, P.timgs, P.ttxts, TTP, TBIAS, LAM, iw, tw, lab)
+    res = closed_form_groups(imgs, txts, TP, BIAS, lab, Bs, iw, tw)
+    for r, x in enumerate(res):
+        x["text_loss"] = text_loss_of(res, r)
+    return res
+
+
+def retrieval(P: Problem, o: Options, k: int) -> List[Dict]:
+    """Per rank: top-K lists and recall (topk_retrieval), and the top-1 outputs they contain: i2t_index / t2i_index
+    (column 0) and top1 = (i2t, t2i) rates as the kernels count them. Weights and groups play no part; i2t ranks all
+    R_r images only under extra-image ids, t2i all T_r texts only under extra-text ids."""
+    Bs, Rs, Ts, imgs, txts = P.view(o)
+    img_ids = txt_ids = None
+    if o.ids:
+        img_ids = [np.concatenate([a, b]) if o.xi_ids else a for a, b in zip(P.ids, P.xi_ids)]
+        txt_ids = [np.concatenate([a, b]) if o.xt_ids else a for a, b in zip(P.ids, P.xt_ids)]
+    out = topk_retrieval(imgs, txts, Bs, max(k, 1), img_ids, txt_ids, rank_all_images=o.xi_ids,
+                         rank_all_texts=o.xt_ids)
+    for x in out:
+        x["i2t_index"], x["t2i_index"] = x["i2t_topk"][:, 0].copy(), x["t2i_topk"][:, 0].copy()
+        x["top1"] = np.array([recall_counts(x["i2t_first"], 1)[0], recall_counts(x["t2i_first"], 1)[0]], np.float32)
+        x["recall_f32"] = np.concatenate([recall_counts(x["i2t_first"], max(k, 1)),
+                                          recall_counts(x["t2i_first"], max(k, 1))])
+    return out
+
+
+def peer_stand_ins(P: Problem, o: Options, r: int, res: Optional[List[Dict]], ret: Optional[List[Dict]],
+                   f16: bool = False):
+    """What each peer p != r publishes for rank r's chunk: metric_keys (its column argmax keys, [B_r], [T_r] under
+    extra-text ids), topk_keys ([T_r, KMAX] sorted, 0-padded), partials (fixed-point words of its column sums, [T_r]) and
+    xi_ids (its extra-image ids, under extra-image ids). The keys hold the loss kernel's accumulator: <img, txt>, or
+    2^8 <img, txt> for fp16(16 x) operands (f16), as every rank of an INPUT_F16 job computes them."""
+    acc = 256.0 if f16 else 1.0
+    Bs, Rs, Ts, _, _ = P.view(o)
+    out = {}
+    for p in range(len(Bs)):
+        if p == r:
+            continue
+        d = {}
+        if ret is not None:
+            S, off, toff = ret[r]["S"], ret[r]["off"], ret[r]["toff"]
+            keys = np.zeros((Ts[r], KMAX), np.int64)
+            for j in range(Ts[r]):
+                col = S[off[p]:off[p + 1], toff[r] + j]
+                order = np.lexsort((np.arange(len(col)), -col))[:KMAX]
+                keys[j, :len(order)] = [key_as_int64(metric_key(acc * col[i], off[p] + i)) for i in order]
+            d["topk_keys"] = keys
+            d["metric_keys"] = keys[:Ts[r] if o.xt_ids else Bs[r], 0].copy()
+        if res is not None and "text_part" in res[p]:
+            d["partials"] = np.array([fixed_point_partial(v)[0] for v in res[p]["text_part"][r]], np.int64)
+        if o.xi_ids:
+            d["xi_ids"] = P.xi_ids[p][:Rs[p] - Bs[p]]
+        out[p] = d
+    return out
+
+
+def rel(a, b) -> float:
+    """The suite's norm-and-max relative error (test_gpu_exclude_groups._rel) in numpy."""
+    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
+    return max(float(np.linalg.norm(a - b) / (np.linalg.norm(b) + 1e-300)),
+               float(np.abs(a - b).max() / (np.abs(b).max() + 1e-300)))
