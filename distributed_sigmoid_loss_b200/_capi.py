@@ -47,6 +47,8 @@ EXPORTED_SYMBOLS = (
     "siglip_set_extra_image_ids",
     "siglip_set_sample_weights",
     "siglip_set_groups",
+    "siglip_ctx_create_labels",
+    "siglip_set_label_sets",
     "siglip_request_metrics",
     "siglip_request_sample_losses",
     "siglip_request_topk",
@@ -71,6 +73,8 @@ EXPORTED_SYMBOLS = (
     "siglip_debug_set_chunk_ids",
     "siglip_debug_set_chunk_weights",
     "siglip_debug_set_chunk_groups",
+    "siglip_debug_set_chunk_label_sets",
+    "siglip_debug_set_peer_extra_image_label_sets",
     "siglip_debug_set_mailbox",
     "siglip_debug_set_peer_metric_keys",
     "siglip_debug_set_peer_sample_loss_partials",
@@ -114,6 +118,8 @@ SIGLIP_OPT_EXTRA_IMAGE_IDS = 24
 SIGLIP_OPT_DISTILL = 25
 SIGLIP_OPT_SIGMA_BUDGET_MIB = 26
 SIGLIP_OPT_EXCLUDE_GROUPS = 27
+SIGLIP_OPT_LABEL_SETS = 28
+SIGLIP_MAX_LABELS = 4
 
 _lib: Optional[ctypes.CDLL] = None
 
@@ -250,6 +256,15 @@ def lib() -> ctypes.CDLL:
     L.siglip_set_groups.restype = ci
     L.siglip_debug_set_chunk_groups.argtypes = [vp, ci, vp, vp]
     L.siglip_debug_set_chunk_groups.restype = ci
+    L.siglip_ctx_create_labels.argtypes = [ctypes.POINTER(vp), ci, ci, ci, ctypes.POINTER(ci), ctypes.POINTER(ci),
+                                           ctypes.POINTER(ci), ci, ci]
+    L.siglip_ctx_create_labels.restype = ci
+    L.siglip_set_label_sets.argtypes = [vp, vp, vp, vp, vp]
+    L.siglip_set_label_sets.restype = ci
+    L.siglip_debug_set_chunk_label_sets.argtypes = [vp, ci, vp, vp]
+    L.siglip_debug_set_chunk_label_sets.restype = ci
+    L.siglip_debug_set_peer_extra_image_label_sets.argtypes = [vp, ci, vp, vp]
+    L.siglip_debug_set_peer_extra_image_label_sets.restype = ci
     L.siglip_request_metrics.argtypes = [vp, vp, vp, vp]
     L.siglip_request_metrics.restype = ci
     L.siglip_debug_set_peer_metric_keys.argtypes = [vp, ci, vp, vp]

@@ -155,7 +155,8 @@ struct IpcBlob {
   int Tmax;
   int R;      // images of the rank (B + its extra images)
   int Rmax;
-  char host[60];
+  char host[56];
+  int M;           // labels per set (siglip_ctx_create_labels; 0: none); inside the 64 bytes the host name had before
   int D_teacher;   // width of the gathered teacher text (0: none); inside the 64 bytes the host name had before
 };
 
@@ -221,6 +222,11 @@ struct siglip_ctx {
   int exclude_groups = 0;                // SIGLIP_OPT_EXCLUDE_GROUPS: same-group pairs are excluded (collective)
   bool groups_set = false;               // siglip_set_groups was called since the previous step
   bool ids_grp = false;                  // ids_in has its group halves (allocated when the mode is first turned on)
+  // label sets (siglip_ctx_create_labels, SIGLIP_OPT_LABEL_SETS)
+  int LM = 0;                            // labels per set M, 1 .. SIGLIP_MAX_LABELS (0: a context without label sets)
+  int label_sets = 0;                    // SIGLIP_OPT_LABEL_SETS (collective)
+  bool sets_set = false;                 // siglip_set_label_sets was called since the previous step
+  int64_t* lrows = nullptr;              // [R][LM] the sets of my images: the paired ones, then the extras. Never exported
   // distillation (siglip_ctx_create_distill, SIGLIP_OPT_DISTILL)
   int DT = 0;                            // teacher width D_teacher (0: a context without a teacher)
   int distill = 0;                       // SIGLIP_OPT_DISTILL (collective)
@@ -260,7 +266,8 @@ struct siglip_ctx {
   // workspaces
   __nv_bfloat16* txt_all = nullptr;      // [world][Tmax, D] bf16; slot `rank` is what the peers pull (world > 1),
                                          // followed by ids_all in the same (IPC-exported) allocation
-  int64_t* ids_all = nullptr;            // [world][2 ids_stride] ids, then text groups, of every text chunk (world > 1)
+  int64_t* ids_all = nullptr;            // [world][ids_slot] ids (or label sets), then text groups, of every text chunk
+                                         // (world > 1)
   int64_t* ids_in = nullptr;             // [ids_stride] this rank's ids for the next step: B sample ids
                                          // (siglip_set_sample_ids), then K extra-text ids (siglip_set_extra_text_ids);
                                          // once SIGLIP_OPT_EXCLUDE_GROUPS has been on, followed by [ids_stride] text
@@ -380,8 +387,12 @@ inline size_t chunk_stride(const siglip_ctx* c) { return static_cast<size_t>(c->
 // Sample ids of text chunk `cidx` as the loss kernel reads them (null outside SIGLIP_OPT_SAMPLE_IDS): the caller's ids
 // for the own chunk, the gathered copy for the others.
 // Every slot of ids_all is [ids_stride] ids, then [ids_stride] text groups (SIGLIP_OPT_EXCLUDE_GROUPS), fixed at
-// creation: the groups ride every copy of the ids, which then moves the whole slot.
-inline size_t ids_slot(const siglip_ctx* c) { return 2 * static_cast<size_t>(c->ids_stride); }
+// creation: the groups ride every copy of the ids, which then moves the whole slot. In a context with label sets the
+// ids half is [ids_stride][M] set words (SIGLIP_OPT_LABEL_SETS: text l's set at l * M), the groups behind them.
+inline size_t set_words(const siglip_ctx* c) {
+  return static_cast<size_t>(c->ids_stride) * static_cast<size_t>(c->LM > 0 ? c->LM : 1);
+}
+inline size_t ids_slot(const siglip_ctx* c) { return set_words(c) + static_cast<size_t>(c->ids_stride); }
 inline const int64_t* chunk_ids(const siglip_ctx* c, int cidx) {
   if (!c->sample_ids) return nullptr;
   return (cidx == c->rank) ? c->ids_in : c->ids_all + static_cast<size_t>(cidx) * ids_slot(c);
@@ -396,11 +407,18 @@ inline const int64_t* peer_ids(const siglip_ctx* c, int o) {
 // the own chunk, of the gathered slot for the others. Image groups are local, behind my text groups: they never travel.
 inline const int64_t* chunk_groups(const siglip_ctx* c, int cidx) {
   if (!c->exclude_groups) return nullptr;
-  return ((cidx == c->rank) ? c->ids_in : c->ids_all + static_cast<size_t>(cidx) * ids_slot(c)) + c->ids_stride;
+  return ((cidx == c->rank) ? c->ids_in : c->ids_all + static_cast<size_t>(cidx) * ids_slot(c)) + set_words(c);
 }
 inline const int64_t* image_groups(const siglip_ctx* c) { return c->exclude_groups ? c->ids_in + ids_slot(c) : nullptr; }
-// the ids copies of the exchange run in ids mode or groups mode; under groups mode they move the whole slot
-inline bool ids_travel(const siglip_ctx* c) { return c->sample_ids || c->exclude_groups; }
+// ---- label sets (SIGLIP_OPT_LABEL_SETS) ----
+// Text sets of chunk `cidx` as the loss kernel reads them (null outside the mode): the set half of my ids_in for the
+// own chunk, of the gathered slot for the others. Image sets are local (lrows): they never travel.
+inline const int64_t* chunk_sets(const siglip_ctx* c, int cidx) {
+  if (!c->label_sets) return nullptr;
+  return (cidx == c->rank) ? c->ids_in : c->ids_all + static_cast<size_t>(cidx) * ids_slot(c);
+}
+// the ids copies of the exchange run in ids, groups or label-set mode; under the last two they move the whole slot
+inline bool ids_travel(const siglip_ctx* c) { return c->sample_ids || c->exclude_groups || c->label_sets; }
 // the sample ids of a rank (siglip_set_sample_ids)
 inline size_t ids_bytes(const siglip_ctx* c, int rank) { return static_cast<size_t>(c->Bs[rank]) * sizeof(int64_t); }
 // the ids of a text chunk as the exchange moves them: its paired texts', and under SIGLIP_OPT_EXTRA_TEXT_IDS its extras'
@@ -410,7 +428,7 @@ inline size_t chunk_ids_bytes(const siglip_ctx* c, int rank) {
 }
 // bytes one ids copy of the exchange moves: the chunk's ids, or the whole slot (ids and text groups) under groups mode
 inline size_t ids_copy_bytes(const siglip_ctx* c, int rank) {
-  return c->exclude_groups ? ids_slot(c) * sizeof(int64_t) : chunk_ids_bytes(c, rank);
+  return (c->exclude_groups || c->label_sets) ? ids_slot(c) * sizeof(int64_t) : chunk_ids_bytes(c, rank);
 }
 // ids and weights of step s are given once: a step in ids / weights mode consumes them (all checked before anything is
 // launched or consumed)
@@ -436,6 +454,10 @@ int take_ids(siglip_ctx* c) {
   if (c->exclude_groups && !c->groups_set)
     return fail(SIGLIP_ERR_STATE,
                 "SIGLIP_OPT_EXCLUDE_GROUPS is on but siglip_set_groups was not called since the previous step");
+  if (c->label_sets && !c->sets_set)
+    return fail(SIGLIP_ERR_STATE,
+                "SIGLIP_OPT_LABEL_SETS is on but siglip_set_label_sets was not called since the previous step");
+  c->sets_set = false;
   c->groups_set = false;
   c->teacher_set = false;
   c->ids_set = false;
@@ -470,13 +492,19 @@ static_assert(siglip::kMetricsMaxWorld == kMaxWorld, "the finalisation kernel ta
 static_assert(siglip::kTopKMax == SIGLIP_TOPK_MAX, "the top-K lists have SIGLIP_TOPK_MAX slots");
 // 64-bit words per step parity: [world][Tmax] column partials (the loss kernel writes one per text of the chunk; the
 // finalisation reads the paired ones), then [Rmax] row keys, then [Emax] extra-image ids of this rank (published for the
-// peers' t2i hit test under SIGLIP_OPT_EXTRA_IMAGE_IDS). Without extra images: [Bmax] row keys and nothing behind.
+// peers' t2i hit test under SIGLIP_OPT_EXTRA_IMAGE_IDS; [Emax][M] extra-image sets in a context with label sets).
+// Without extra images: [Bmax] row keys and nothing behind.
 inline size_t mkeys_block(const siglip_ctx* c) {
-  return static_cast<size_t>(c->world) * c->Tmax + static_cast<size_t>(c->Rmax) + static_cast<size_t>(c->Emax);
+  return static_cast<size_t>(c->world) * c->Tmax + static_cast<size_t>(c->Rmax) +
+         static_cast<size_t>(c->Emax) * static_cast<size_t>(c->LM > 0 ? c->LM : 1);
 }
 // offset of the published extra-image ids in a key block
 inline size_t mkeys_xids(const siglip_ctx* c) { return static_cast<size_t>(c->world) * c->Tmax + c->Rmax; }
 inline size_t mkeys_rows(const siglip_ctx* c) { return static_cast<size_t>(c->world) * c->Tmax; }
+// words per peer of the loopback stand-ins of the published extra-image ids (or sets)
+inline size_t loop_xids_stride(const siglip_ctx* c) {
+  return static_cast<size_t>(c->Emax) * static_cast<size_t>(c->LM > 0 ? c->LM : 1);
+}
 // byte offset of the two key blocks in the exported text allocation: behind the gathered text and ids
 inline size_t mkeys_offset(const siglip_ctx* c) {
   return chunk_stride(c) * c->world * sizeof(__nv_bfloat16) + static_cast<size_t>(c->world) * ids_slot(c) * sizeof(int64_t);
@@ -588,6 +616,10 @@ int take_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
     CK(cudaMemcpyAsync(c->mkeys_step + mkeys_xids(c), c->rids + c->B,
                        static_cast<size_t>(c->R - c->B) * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
   }
+  if (c->world > 1 && c->label_sets && c->R > c->B) {   // my extra images' sets, in the same words
+    CK(cudaMemcpyAsync(c->mkeys_step + mkeys_xids(c), c->lrows + static_cast<size_t>(c->B) * c->LM,
+                       static_cast<size_t>(c->R - c->B) * c->LM * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
+  }
   return 0;
 }
 // The finalisation arguments of step s: batches, hit rules and flags (shared with the top-K finalisation)
@@ -621,6 +653,18 @@ void fill_metrics_args(const siglip_ctx* c, unsigned int s, siglip::MetricsArgs&
   }
   a.dbg = c->dbg_dev;
 }
+// The label-set hit rule of step s (SIGLIP_OPT_LABEL_SETS): my sets, the gathered text sets and the peers' published
+// extra-image sets
+void fill_label_set_args(const siglip_ctx* c, unsigned int s, siglip::LabelSetArgs& l) {
+  memset(&l, 0, sizeof(l));
+  l.row_sets = c->lrows;
+  l.text_own = c->ids_in;
+  l.text_all = c->ids_all;
+  l.slot = static_cast<long long>(ids_slot(c));
+  if (c->world > 1 && c->xid_ptrs_dev != nullptr)
+    l.xsets_peers = c->xid_ptrs_dev + static_cast<size_t>(s & 1u) * c->world;
+  l.m = c->LM;
+}
 
 // After the step's last loss kernel: combine the keys (W > 1: with every rank's partials of my chunk, flag kind 5) and
 // write the indices and the top-1 rates.
@@ -639,7 +683,13 @@ int finalize_metrics(siglip_ctx* c, unsigned int s, cudaStream_t st) {
     a.top1 = out == 0 ? c->m_top1 : c->k_recall;
     a.i2t = out == 0 ? c->m_i2t : c->k_i2t;
     a.t2i = out == 0 ? c->m_t2i : c->k_t2i;
-    CKI(siglip::launch_metrics_finalize(a, st));
+    if (c->label_sets) {
+      siglip::LabelSetArgs l;
+      fill_label_set_args(c, s, l);
+      CKI(siglip::launch_metrics_finalize_labels(a, l, st));
+    } else {
+      CKI(siglip::launch_metrics_finalize(a, st));
+    }
     c->launches++;
   }
   c->metrics_step = c->topk1_step = false;
@@ -668,6 +718,10 @@ int take_topk(siglip_ctx* c, unsigned int s, cudaStream_t st) {
     CK(cudaMemcpyAsync(c->mkeys[s & 1u] + mkeys_xids(c), c->rids + c->B,
                        static_cast<size_t>(c->R - c->B) * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
   }
+  if (c->world > 1 && c->label_sets && c->R > c->B) {   // my extra images' sets, as take_metrics publishes them
+    CK(cudaMemcpyAsync(c->mkeys[s & 1u] + mkeys_xids(c), c->lrows + static_cast<size_t>(c->B) * c->LM,
+                       static_cast<size_t>(c->R - c->B) * c->LM * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
+  }
   return 0;
 }
 
@@ -688,7 +742,13 @@ int finalize_topk(siglip_ctx* c, unsigned int s, bool signal, cudaStream_t st) {
   a.i2t = c->k_i2t;
   a.t2i = c->k_t2i;
   c->topk_step = false;
-  CKI(siglip::launch_topk_finalize(a, st));
+  if (c->label_sets) {
+    siglip::LabelSetArgs l;
+    fill_label_set_args(c, s, l);
+    CKI(siglip::launch_topk_finalize_labels(a, l, st));
+  } else {
+    CKI(siglip::launch_topk_finalize(a, st));
+  }
   c->launches++;
   return 0;
 }
@@ -948,6 +1008,11 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
     p.row_grp = image_groups(c) + r0;
     p.col_grp = chunk_groups(c, cidx) + c0;
     p.grp_rows = rest(c->R, r0);
+  }
+  if (c->label_sets) {   // the kModeLabels kernel: pairs whose sets share a label are positives too
+    p.row_lab = c->lrows + static_cast<size_t>(r0) * c->LM;
+    p.col_lab = chunk_sets(c, cidx) + static_cast<size_t>(c0) * c->LM;
+    p.lab_m = c->LM;
   }
   if (c->mkeys_step != nullptr) {   // a metrics step: the kMetrics instantiation reduces the argmax keys
     p.row_keys = c->mkeys_step + mkeys_rows(c) + r0;
@@ -1827,7 +1892,7 @@ int siglip_device_count(void) {
 // Bs[p]: rank p's batch; Rs[p] >= Bs[p]: its images (paired ones first, then its extra images); Ts[p] >= Bs[p]: its
 // texts (paired ones first, then its hard negatives). Every argument is checked before the first CUDA call.
 static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, const int* Bs, const int* Rs,
-                           const int* Ts, int D, int DT = 0) {
+                           const int* Ts, int D, int DT = 0, int LM = 0) {
   if (out == nullptr) return fail(SIGLIP_ERR_INVALID, "out is null");
   *out = nullptr;
   if (world < 1 || world > kMaxWorld || rank < 0 || rank >= world)
@@ -1846,6 +1911,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   }
   if (D < 8 || (D % 8) != 0) return fail(SIGLIP_ERR_INVALID, "need D a positive multiple of 8");
   if (DT < 0 || (DT % 8) != 0) return fail(SIGLIP_ERR_INVALID, "need D_teacher a positive multiple of 8 (0: no teacher)");
+  if (LM < 0 || LM > SIGLIP_MAX_LABELS) return fail(SIGLIP_ERR_INVALID, "need 1 <= M <= SIGLIP_MAX_LABELS labels per set");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     cudaGetLastError();
@@ -1884,6 +1950,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   c->own_pos_ids = c->R > c->B && c->T > c->B;
   c->D = D;
   c->DT = DT;
+  c->LM = LM;
   c->Bp = round_up(Bmax, 256);
   c->Tp = round_up(Tmax, 256);
   c->Rp = round_up(Rmax, 256);
@@ -1923,7 +1990,15 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
   // cannot depend on it); without extras this is Bmax rounded up, as it was before they existed
   c->ids_stride = round_up(Tmax, 2);
   const size_t ids_slot_bytes = static_cast<size_t>(c->ids_stride) * sizeof(int64_t);
-  CK(alloc(reinterpret_cast<void**>(&c->ids_in), ids_slot_bytes));
+  if (LM > 0) {
+    // a context with label sets holds its whole slot from the start (sets, text groups, then [R] image groups), and
+    // its images' sets
+    CK(alloc(reinterpret_cast<void**>(&c->ids_in), (ids_slot(c) + static_cast<size_t>(c->R)) * sizeof(int64_t)));
+    c->ids_grp = true;
+    CK(alloc(reinterpret_cast<void**>(&c->lrows), static_cast<size_t>(c->R) * LM * sizeof(int64_t)));
+  } else {
+    CK(alloc(reinterpret_cast<void**>(&c->ids_in), ids_slot_bytes));
+  }
   if (c->R > c->B) CK(alloc(reinterpret_cast<void**>(&c->rids), static_cast<size_t>(c->R) * sizeof(int64_t)));
   if (c->own_pos_ids) {
     const int n = c->R > c->T ? c->R : c->T;
@@ -1946,7 +2021,7 @@ static int ctx_create_impl(siglip_ctx** out, int device, int rank, int world, co
     // and the top-K column lists behind those (sized whatever the options, for the same reason)
     const size_t k_bytes = 2 * topk_cols_words(c) * sizeof(unsigned long long);
     // (every ids slot has a text-group half: SIGLIP_OPT_EXCLUDE_GROUPS may be set after the handle exchange too)
-    CK(alloc(reinterpret_cast<void**>(&c->txt_all), stride * world * sizeof(__nv_bfloat16) + world * 2 * ids_slot_bytes +
+    CK(alloc(reinterpret_cast<void**>(&c->txt_all), stride * world * sizeof(__nv_bfloat16) + world * ids_slot(c) * 8 +
                                                         mkeys_bytes + w_bytes + t_bytes + l_bytes + k_bytes));
     c->ids_all = reinterpret_cast<int64_t*>(c->txt_all + stride * world);   // 16-byte aligned: D % 8 == 0
     c->mkeys[0] = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(c->txt_all) + mkeys_offset(c));
@@ -2032,6 +2107,15 @@ int siglip_ctx_create_distill(siglip_ctx** out, int device, int rank, int world,
   return ctx_create_impl(out, device, rank, world, batch_per_rank, batch_per_rank, batch_per_rank, D, D_teacher);
 }
 
+int siglip_ctx_create_labels(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank,
+                             const int* images_per_rank, const int* texts_per_rank, int D, int M) {
+  if (batch_per_rank == nullptr || images_per_rank == nullptr || texts_per_rank == nullptr)
+    return fail(SIGLIP_ERR_INVALID, "batch_per_rank / images_per_rank / texts_per_rank is null");
+  if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
+  if (M < 1 || M > SIGLIP_MAX_LABELS) return fail(SIGLIP_ERR_INVALID, "need 1 <= M <= SIGLIP_MAX_LABELS labels per set");
+  return ctx_create_impl(out, device, rank, world, batch_per_rank, images_per_rank, texts_per_rank, D, 0, M);
+}
+
 int siglip_set_teacher(siglip_ctx* c, const void* timg, const void* ttxt, int teacher_f16, const float* t_prime_T,
                        const float* bias_T, float lambda) {
   if (c == nullptr || timg == nullptr || ttxt == nullptr || t_prime_T == nullptr || bias_T == nullptr)
@@ -2059,6 +2143,8 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL needs a context created with siglip_ctx_create_distill");
       if (value && c->exclude_groups)
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is unavailable under SIGLIP_OPT_EXCLUDE_GROUPS");
+      if (value && c->label_sets)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is unavailable under SIGLIP_OPT_LABEL_SETS");
       c->distill = value ? 1 : 0;
       c->teacher_set = false;
       return 0;
@@ -2084,6 +2170,16 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
       c->groups_set = false;
       return 0;
     }
+    case SIGLIP_OPT_LABEL_SETS:
+      if (value && c->LM == 0)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_LABEL_SETS needs a context created with siglip_ctx_create_labels");
+      if (value && (c->sample_ids || c->extra_text_ids || c->extra_image_ids))
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_LABEL_SETS replaces sample ids: turn SIGLIP_OPT_SAMPLE_IDS off first");
+      if (value && c->distill)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_LABEL_SETS is unavailable under SIGLIP_OPT_DISTILL");
+      c->label_sets = value ? 1 : 0;
+      c->sets_set = false;
+      return 0;
     case SIGLIP_OPT_SIGMA_BUDGET_MIB:
       if (value < 0) return fail(SIGLIP_ERR_INVALID, "the sigma budget must be >= 0 MiB (0: unbounded)");
       c->sigma_budget_mib = value;
@@ -2127,6 +2223,8 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
       c->sync_scalar_grads = value ? 1 : 0;
       return 0;
     case SIGLIP_OPT_SAMPLE_IDS:
+      if (value && c->label_sets)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_SAMPLE_IDS is unavailable under SIGLIP_OPT_LABEL_SETS");
       c->sample_ids = value ? 1 : 0;
       c->ids_set = false;
       if (!c->sample_ids) c->extra_text_ids = c->extra_image_ids = 0;   // the extras' ids extend the sample ids
@@ -2134,12 +2232,16 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
       c->ximg_ids_set = false;
       return 0;
     case SIGLIP_OPT_EXTRA_IMAGE_IDS:
+      if (value && c->label_sets)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_EXTRA_IMAGE_IDS is unavailable under SIGLIP_OPT_LABEL_SETS");
       if (value && !c->sample_ids)
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_EXTRA_IMAGE_IDS needs SIGLIP_OPT_SAMPLE_IDS on first");
       c->extra_image_ids = value ? 1 : 0;
       c->ximg_ids_set = false;
       return 0;
     case SIGLIP_OPT_EXTRA_TEXT_IDS:
+      if (value && c->label_sets)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_EXTRA_TEXT_IDS is unavailable under SIGLIP_OPT_LABEL_SETS");
       if (value && !c->sample_ids)
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_EXTRA_TEXT_IDS needs SIGLIP_OPT_SAMPLE_IDS on first");
       c->extra_text_ids = value ? 1 : 0;
@@ -2237,6 +2339,7 @@ int siglip_ctx_export_handles(siglip_ctx* c, void* out_bytes, size_t capacity) {
   b.R = c->R;
   b.Rmax = c->Rmax;
   b.D_teacher = c->DT;
+  b.M = c->LM;
   if (gethostname(b.host, sizeof(b.host) - 1) != 0) b.host[0] = 0;
   memcpy(out_bytes, &b, sizeof(b));
   return 0;
@@ -2304,7 +2407,8 @@ static int publish_peer_tables(siglip_ctx* c) {
         xi[q * c->world + p] = reinterpret_cast<const int64_t*>(
             reinterpret_cast<const unsigned long long*>(reinterpret_cast<const char*>(c->peer_txt[p]) + mkeys_offset(c)) +
             q * mkeys_block(c) + mkeys_xids(c));
-        if (c->loopback && p != c->rank) xi[q * c->world + p] = c->loop_xids + static_cast<size_t>(p) * c->Emax;
+        if (c->loopback && p != c->rank)
+          xi[q * c->world + p] = c->loop_xids + static_cast<size_t>(p) * loop_xids_stride(c);
       }
     CK(cudaMemcpy(c->xid_ptrs_dev, xi.data(), xi.size() * sizeof(int64_t*), cudaMemcpyHostToDevice));
   }
@@ -2338,6 +2442,10 @@ int siglip_ctx_import_handles(siglip_ctx* c, const void* all_ranks_bytes, size_t
       return fail(SIGLIP_ERR_INVALID,
                   "peer context has a different D_teacher than this rank: every rank must be created with the same "
                   "siglip_ctx_create_distill arguments");
+    if (b.M != c->LM)
+      return fail(SIGLIP_ERR_INVALID,
+                  "peer context has a different label-set width M than this rank: every rank must be created with the "
+                  "same siglip_ctx_create_labels M");
     if (p == c->rank) continue;
     char me[sizeof(b.host)] = {0};
     if (gethostname(me, sizeof(me) - 1) != 0) me[0] = 0;
@@ -2449,11 +2557,38 @@ int siglip_set_groups(siglip_ctx* c, const int64_t* image_groups, const int64_t*
   CK(cudaSetDevice(c->device));
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   // my text groups go to the group half of my slot (published with my ids), my image groups behind it
-  CK(cudaMemcpyAsync(c->ids_in + c->ids_stride, text_groups, static_cast<size_t>(c->T) * sizeof(int64_t),
+  CK(cudaMemcpyAsync(c->ids_in + set_words(c), text_groups, static_cast<size_t>(c->T) * sizeof(int64_t),
                      cudaMemcpyDeviceToDevice, st));
   CK(cudaMemcpyAsync(c->ids_in + ids_slot(c), image_groups, static_cast<size_t>(c->R) * sizeof(int64_t),
                      cudaMemcpyDeviceToDevice, st));
   c->groups_set = true;
+  return 0;
+}
+
+int siglip_set_label_sets(siglip_ctx* c, const int64_t* sample_labels, const int64_t* extra_text_labels,
+                          const int64_t* extra_image_labels, void* cuda_stream) {
+  if (c == nullptr || sample_labels == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->label_sets) return fail(SIGLIP_ERR_STATE, "siglip_set_label_sets needs SIGLIP_OPT_LABEL_SETS = 1");
+  CK(cudaSetDevice(c->device));
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  const size_t m = static_cast<size_t>(c->LM), w = sizeof(int64_t);
+  // a sample's set belongs to its image (my rows) and to its paired text (the set half of my slot, published)
+  CK(cudaMemcpyAsync(c->lrows, sample_labels, c->B * m * w, cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(c->ids_in, sample_labels, c->B * m * w, cudaMemcpyDeviceToDevice, st));
+  // extras without sets (null) get empty ones: all bytes 0xff is -1 in every slot
+  if (c->T > c->B) {
+    if (extra_text_labels != nullptr)
+      CK(cudaMemcpyAsync(c->ids_in + c->B * m, extra_text_labels, (c->T - c->B) * m * w, cudaMemcpyDeviceToDevice, st));
+    else
+      CK(cudaMemsetAsync(c->ids_in + c->B * m, 0xff, (c->T - c->B) * m * w, st));
+  }
+  if (c->R > c->B) {
+    if (extra_image_labels != nullptr)
+      CK(cudaMemcpyAsync(c->lrows + c->B * m, extra_image_labels, (c->R - c->B) * m * w, cudaMemcpyDeviceToDevice, st));
+    else
+      CK(cudaMemsetAsync(c->lrows + c->B * m, 0xff, (c->R - c->B) * m * w, st));
+  }
+  c->sets_set = true;
   return 0;
 }
 
@@ -2592,8 +2727,10 @@ int siglip_debug_set_peer_metric_keys(siglip_ctx* c, int peer, const uint64_t* k
     return fail(SIGLIP_ERR_INVALID,
                 "siglip_debug_set_peer_metric_keys needs a loopback context and a peer rank != own rank");
   CK(cudaSetDevice(c->device));
+  // the keys of the texts the finalisation ranks: all T under label sets (their t2i ranks every text)
+  const int n = c->label_sets ? c->T : chunk_id_count(c, c->rank);
   CK(cudaMemcpyAsync(c->loop_keys + static_cast<size_t>(peer) * c->Tmax, keys_dev,
-                     static_cast<size_t>(chunk_id_count(c, c->rank)) * sizeof(unsigned long long),
+                     static_cast<size_t>(n) * sizeof(unsigned long long),
                      cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
@@ -2607,7 +2744,22 @@ int siglip_debug_set_peer_extra_image_ids(siglip_ctx* c, int peer, const int64_t
   if (e == 0) return 0;
   if (ids_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   CK(cudaSetDevice(c->device));
-  CK(cudaMemcpyAsync(c->loop_xids + static_cast<size_t>(peer) * c->Emax, ids_dev, e * sizeof(int64_t),
+  CK(cudaMemcpyAsync(c->loop_xids + static_cast<size_t>(peer) * loop_xids_stride(c), ids_dev, e * sizeof(int64_t),
+                     cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
+  return 0;
+}
+
+int siglip_debug_set_peer_extra_image_label_sets(siglip_ctx* c, int peer, const int64_t* sets_dev, void* cuda_stream) {
+  if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->loopback || peer < 0 || peer >= c->world || peer == c->rank || c->LM == 0)
+    return fail(SIGLIP_ERR_INVALID,
+                "siglip_debug_set_peer_extra_image_label_sets needs a loopback labels context and a peer rank != own "
+                "rank");
+  const size_t e = static_cast<size_t>(c->Rs[peer] - c->Bs[peer]) * c->LM;
+  if (e == 0) return 0;
+  if (sets_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(c->device));
+  CK(cudaMemcpyAsync(c->loop_xids + static_cast<size_t>(peer) * loop_xids_stride(c), sets_dev, e * sizeof(int64_t),
                      cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
@@ -2713,6 +2865,9 @@ int siglip_host_submit_grads(siglip_ctx* c, const void* img_host, const void* tx
   if (c->exclude_groups)
     return fail(SIGLIP_ERR_STATE,
                 "the host-buffer entries take no group ids: unavailable under SIGLIP_OPT_EXCLUDE_GROUPS");
+  if (c->label_sets)
+    return fail(SIGLIP_ERR_STATE,
+                "the host-buffer entries take no label sets: unavailable under SIGLIP_OPT_LABEL_SETS");
   const bool with_grads = dimg_host_bf16 != nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   CK(cudaSetDevice(c->device));
@@ -2860,8 +3015,8 @@ int siglip_debug_loopback(siglip_ctx* c) {
     CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_topk), topk_cols_words(c) * 8));
     CK(cudaMemset(c->loop_topk, 0, topk_cols_words(c) * 8));
     if (c->Emax > 0) {
-      CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_xids), static_cast<size_t>(c->world) * c->Emax * 8));
-      CK(cudaMemset(c->loop_xids, 0, static_cast<size_t>(c->world) * c->Emax * 8));
+      CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_xids), static_cast<size_t>(c->world) * loop_xids_stride(c) * 8));
+      CK(cudaMemset(c->loop_xids, 0, static_cast<size_t>(c->world) * loop_xids_stride(c) * 8));
     }
   }
   for (int p = 0; p < c->world; ++p) {
@@ -2932,8 +3087,19 @@ int siglip_debug_set_chunk_groups(siglip_ctx* c, int chunk, const int64_t* group
   if (c == nullptr || groups_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
   // the group half of the chunk's slot, where its owner's ids publish puts them
-  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * ids_slot(c) + c->ids_stride, groups_dev,
+  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * ids_slot(c) + set_words(c), groups_dev,
                      static_cast<size_t>(c->Ts[chunk]) * sizeof(int64_t), cudaMemcpyDeviceToDevice,
+                     static_cast<cudaStream_t>(cuda_stream)));
+  return 0;
+}
+
+int siglip_debug_set_chunk_label_sets(siglip_ctx* c, int chunk, const int64_t* sets_dev, void* cuda_stream) {
+  if (c == nullptr || sets_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
+  if (c->LM == 0) return fail(SIGLIP_ERR_STATE, "siglip_debug_set_chunk_label_sets needs a context with label sets");
+  // the set half of the chunk's slot, where its owner's ids publish puts them
+  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * ids_slot(c), sets_dev,
+                     static_cast<size_t>(c->Ts[chunk]) * c->LM * sizeof(int64_t), cudaMemcpyDeviceToDevice,
                      static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
@@ -3207,6 +3373,7 @@ void free_ctx(siglip_ctx* c) {
   cudaFree(c->rids);
   cudaFree(c->iota);
   cudaFree(c->loop_xids);
+  cudaFree(c->lrows);
   cudaFree(c->xid_ptrs_dev);
   cudaFree(c->w_in);   // w_all: part of txt_all
   cudaFree(c->img16);

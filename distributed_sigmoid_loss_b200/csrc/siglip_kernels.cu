@@ -998,7 +998,13 @@ __device__ __forceinline__ void sample_loss_add(unsigned long long* w, long long
 // fragment rows, once per slab those of its 8 columns (clamped like the ids); the excl bits of the matching elements
 // that are not positives, and a warp vote: a slab with an excluded element takes the masked path, which zeroes it, and
 // every other slab keeps the path it takes without groups. Top-K lists and the per-sample sums are runtime options.
-template <bool kTopK = false, bool kGroups = false>
+// kLabels (kModeLabels): positives from label sets (p.row_lab / p.col_lab, p.lab_m labels each). Once per tile, before
+// the slab loop, each of the thread's two fragment rows' set is compared with the sets of its 32 columns (lab_m^2 64-bit
+// compares per element; rolled loops, so that no set stays in registers across the loop), together with the id
+// positives of the own chunk (own_pos_ids); the 64 pos bits are the only state the slab loop carries. There they form
+// pos before the warp vote: a slab with a positive takes the masked path, every other slab keeps its path. Groups
+// (tested after these positives), top-K lists and the per-sample sums are runtime options.
+template <bool kTopK = false, bool kGroups = false, bool kLabels = false>
 __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, const float (&acc)[kTileN / 2],
                                                      const CUtensorMap* tmG, uint32_t staging_base, int warp, int wg,
                                                      int lane, int row0, int col_base, int row_lo, int c_lo,
@@ -1008,10 +1014,12 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
   if (p.row_keys != nullptr) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
   if constexpr (kTopK) {
     tile_topk(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
-  } else if constexpr (kGroups) {
+  } else if constexpr (kGroups || kLabels) {
     if (p.tk_rows != nullptr) tile_topk(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
   }
-  const bool sl = (!kTopK && !kGroups) || p.sl_rows != nullptr;
+  const bool sl = (!kTopK && !kGroups && !kLabels) || p.sl_rows != nullptr;
+  // excluded groups: always in kModeGroups, a runtime option in kModeLabels
+  const bool grp = kGroups || (kLabels && p.col_grp != nullptr);
   float acc_sp = 0.f, acc_g = 0.f, acc_gs = 0.f;
   const bool edge = (row0 + kBlockM > pr.M) || (col_base + kTileN > pr.N);
   const bool diag = p.own_chunk && (row0 == col_base);
@@ -1025,7 +1033,7 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
   const bool ids = p.row_ids != nullptr, w = p.row_w != nullptr;
   int64_t rid0 = 0, rid1 = 0;
   uint32_t rpos = 0u;
-  if (ids) {
+  if (!kLabels && ids) {   // kLabels: the id positives are part of lpos below
     rid0 = p.row_ids[min(row_lo, pr.M - 1)];
     rid1 = p.row_ids[min(row_lo + 8, pr.M - 1)];
     rpos = (row_lo < p.row_pos_n ? 0x3333u : 0u) | (row_lo + 8 < p.row_pos_n ? 0xCCCCu : 0u);
@@ -1037,10 +1045,55 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
   }
   int64_t rg0 = -1, rg1 = -1;
   uint32_t rgrp = 0u;   // excl bits of the rows that have a group (>= 0, within grp_rows)
-  if constexpr (kGroups) {
+  if ((kGroups || kLabels) && grp) {
     rg0 = p.row_grp[min(row_lo, p.grp_rows - 1)];
     rg1 = p.row_grp[min(row_lo + 8, p.grp_rows - 1)];
     rgrp = (row_lo < p.grp_rows && rg0 >= 0 ? 0x3333u : 0u) | (row_lo + 8 < p.grp_rows && rg1 >= 0 ? 0xCCCCu : 0u);
+  }
+  // Label-set positives of the tile's 4 slabs, before the slab loop: the sets of the two fragment rows live in registers
+  // only here, next to the accumulator, and the loop carries the 16 pos bits of each slab in one 64-bit word. Rows past
+  // M read row M - 1 and columns past N column N - 1: they only lie in edge slabs, which mask them. An empty slot (< 0)
+  // and a row slot past lab_m never match, since only column labels >= 0 are compared.
+  uint64_t lpos = 0ull;
+  if constexpr (kLabels) {
+    // one fragment row at a time (rows 0 and 8 of the thread's pair) and one slab at a time, not unrolled: one set and
+    // one slab's columns are in registers at a time
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+      int64_t rl[kMaxLabels];
+      const int64_t* rs = p.row_lab + static_cast<size_t>(min(row_lo + 8 * h, pr.M - 1)) * p.lab_m;
+#pragma unroll
+      for (int k = 0; k < kMaxLabels; ++k) rl[k] = (k < p.lab_m) ? rs[k] : -1;
+      // the positional positives of an own chunk whose extras make them id positives (iota ids, own_pos_ids), with the
+      // bounds of the ids path
+      const bool rid_ok = ids && row_lo + 8 * h < p.row_pos_n;
+      const int64_t rid = rid_ok ? p.row_ids[min(row_lo + 8 * h, pr.M - 1)] : 0;
+#pragma unroll 1
+      for (int c = 0; c < kTileN / 32; ++c) {
+        uint32_t lp = 0u;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+#pragma unroll
+          for (int e1 = 0; e1 < 2; ++e1) {
+            const int col = col_base + 32 * c + 8 * j + c_lo + e1;
+            const int64_t* cs = p.col_lab + static_cast<size_t>(min(col, pr.N - 1)) * p.lab_m;
+            bool hit = rid_ok && col < p.col_pos_n && p.col_ids[col] == rid;
+#pragma unroll
+            for (int k = 0; k < kMaxLabels; ++k) {
+              if (k < p.lab_m) {
+                const int64_t cl = cs[k];
+                if (cl >= 0) {
+#pragma unroll
+                  for (int q = 0; q < kMaxLabels; ++q) hit |= cl == rl[q];
+                }
+              }
+            }
+            lp |= static_cast<uint32_t>(hit) << (4 * j + 2 * h + e1);
+          }
+        }
+        lpos |= static_cast<uint64_t>(lp) << (16 * c);
+      }
+    }
   }
   float lrow[2] = {0.f, 0.f};
 #pragma unroll
@@ -1054,7 +1107,7 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
     const bool slab_edge = edge && ((gst.row0 + 16 > pr.M) || (col0 + 32 > pr.N));
     uint32_t pos = 0;
     bool slab_pos = false;
-    if (ids) {
+    if (!kLabels && ids) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
 #pragma unroll
@@ -1070,9 +1123,13 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
       pos &= rpos;
       slab_pos = __any_sync(0xffffffffu, pos != 0u);
     }
+    if constexpr (kLabels) {
+      pos |= static_cast<uint32_t>(lpos >> (16 * c)) & 0xFFFFu;
+      slab_pos = __any_sync(0xffffffffu, pos != 0u);
+    }
     uint32_t excl = 0u;
     bool slab_excl = false;
-    if constexpr (kGroups) {
+    if ((kGroups || kLabels) && grp) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
 #pragma unroll
@@ -1099,9 +1156,9 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
         loss_slab<false, true, true>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag,
                                      false, 0u, acc_sp, acc_g, acc_gs, cw, rw0, rw1, lrow, lcol);
     } else {
-      loss_slab<true, true, true, kGroups>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale,
-                                           p.g_diag, slab_diag, pos, acc_sp, acc_g, acc_gs, cw, rw0, rw1, lrow, lcol,
-                                           excl);
+      loss_slab<true, true, true, kGroups || kLabels>(v, t_eff, bias, row_lo, col0, c_lo, pr.M, pr.N, sg, gst,
+                                                      p.g_scale, p.g_diag, slab_diag, pos, acc_sp, acc_g, acc_gs, cw,
+                                                      rw0, rw1, lrow, lcol, excl);
     }
     if (sl) {
       // reduce-scatter: after the step over lane bit m, lcol[0 .. h) holds the columns q = k + (bit m of lane ? h : 0)
@@ -1157,6 +1214,9 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
 // kMode = kModeGroups: the loss kernel of a step that excludes same-group pairs, its own instantiation like
 // kModeSampleLoss: its epilogue with the group comparisons (sample_loss_epilogue<false, true>); ids, weights, metrics,
 // the per-sample-loss sums and the top-K lists are runtime options.
+// kMode = kModeLabels: the loss kernel of a step with label sets, its own instantiation like kModeGroups: its epilogue
+// with the set intersections (sample_loss_epilogue<false, false, true>); ids, weights, metrics, the per-sample-loss
+// sums, the top-K lists and excluded groups are runtime options.
 template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false,
           bool kWeights = false, int kTileNT = kTileN>
 __global__ void __launch_bounds__(kNumThreads, 1)
@@ -1178,6 +1238,8 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
                 "the top-K kernel takes ids, weights, metrics and per-sample losses as runtime options");
   static_assert(kMode != kModeGroups || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
                 "the excluded-groups kernel takes ids, weights, metrics, per-sample losses and top-K as runtime options");
+  static_assert(kMode != kModeLabels || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
+                "the label-set kernel takes its other options at run time");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -1426,7 +1488,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
                                                     b_adv, full0, empty0, lane, p.dbg, t, w_full_p)
         const int sel = pr.a_mn * 2 + pr.b_mn;
         if constexpr (kMode == kModeDistill || kMode == kModeSampleLoss || kMode == kModeTopK ||
-                      kMode == kModeGroups) {
+                      kMode == kModeGroups || kMode == kModeLabels) {
           // the loss operands (student and teacher) are always K-major: no MN-major variants in this instantiation
           if (pr.ab_f16)
             SIGLIP_MMA_LOOP(1, 0, 0);
@@ -1469,6 +1531,10 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       } else if constexpr (kMode == kModeGroups) {
         sample_loss_epilogue<false, true>(p, acc, &tmG, staging_base, warp, wg, lane, row0, col_base, row_lo, c_lo, pr,
                                           t_eff, bias, tl, bl, g_store_policy, s_sp, c_sp, s_g, c_g, s_gs, c_gs);
+      } else if constexpr (kMode == kModeLabels) {
+        sample_loss_epilogue<false, false, true>(p, acc, &tmG, staging_base, warp, wg, lane, row0, col_base, row_lo,
+                                                 c_lo, pr, t_eff, bias, tl, bl, g_store_policy, s_sp, c_sp, s_g, c_g,
+                                                 s_gs, c_gs);
       } else if constexpr (kMode == kModeLoss) {
         // argmax keys first, on the raw accumulator: whichever path each slab then takes below
         if constexpr (kMetrics) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
@@ -2066,11 +2132,75 @@ __device__ __forceinline__ bool metrics_t2i_hit(const MetricsArgs& a, int i, int
   return id == a.ids_own[i];
 }
 
+// ---- label sets (SIGLIP_OPT_LABEL_SETS): the hit rule of the kLabels finalisations ----
+// Do the set x (kMaxLabels entries, -1 past m) and the m labels at y share a label >= 0? kPeer: y lies in a peer's
+// memory and is read with relaxed system-scope loads.
+template <bool kPeer = false>
+__device__ __forceinline__ bool label_sets_meet(const int64_t (&x)[kMaxLabels], const int64_t* y, int m) {
+  bool hit = false;
+  for (int k = 0; k < m; ++k) {
+    int64_t v;
+    if constexpr (kPeer)
+      asm volatile("ld.relaxed.sys.global.s64 %0, [%1];" : "=l"(v) : "l"(y + k) : "memory");
+    else
+      v = y[k];
+    if (v < 0) continue;
+#pragma unroll
+    for (int q = 0; q < kMaxLabels; ++q) hit |= v == x[q];
+  }
+  return hit;
+}
+__device__ __forceinline__ void label_set_load(int64_t (&x)[kMaxLabels], const int64_t* s, int m) {
+#pragma unroll
+  for (int k = 0; k < kMaxLabels; ++k) x[k] = k < m ? s[k] : -1;
+}
+// the sets of text l of rank o as this rank holds them: its own, or the gathered copy
+__device__ __forceinline__ const int64_t* label_text_set(const MetricsArgs& a, const LabelSetArgs& l, int o, int t) {
+  return ((o == a.rank) ? l.text_own : l.text_all + static_cast<size_t>(o) * l.slot) + static_cast<size_t>(t) * l.m;
+}
+// Is global text j a hit for my image i? The positional pair, or a text whose set meets the image's.
+__device__ __forceinline__ bool labels_i2t_hit(const MetricsArgs& a, const LabelSetArgs& l, int i, int j) {
+  const int o = metrics_owner(a, a.toff, j);
+  const int t = j - a.toff[o];
+  if (o == a.rank && t == i && i < a.B) return true;
+  int64_t x[kMaxLabels];
+  label_set_load(x, l.row_sets + static_cast<size_t>(i) * l.m, l.m);
+  return label_sets_meet(x, label_text_set(a, l, o, t), l.m);
+}
+// Is global image g a hit for my text i? The positional pair, or an image whose set meets the text's: a paired image
+// shares its paired text's set (the gathered copy), an extra image of a peer is read from the sets that peer published.
+__device__ __forceinline__ bool labels_t2i_hit(const MetricsArgs& a, const LabelSetArgs& l, int i, int g) {
+  const int o = metrics_owner(a, a.off, g);
+  const int r = g - a.off[o];
+  if (o == a.rank && r == i && i < a.B) return true;
+  int64_t x[kMaxLabels];
+  label_set_load(x, l.text_own + static_cast<size_t>(i) * l.m, l.m);
+  if (o == a.rank) return label_sets_meet(x, l.row_sets + static_cast<size_t>(r) * l.m, l.m);
+  if (r < a.bs[o]) return label_sets_meet(x, label_text_set(a, l, o, r), l.m);
+  return label_sets_meet<true>(x, l.xsets_peers[o] + static_cast<size_t>(r - a.bs[o]) * l.m, l.m);
+}
+template <bool kLabels>
+__device__ __forceinline__ bool finalize_i2t_hit(const MetricsArgs& a, const LabelSetArgs& l, int i, int j) {
+  if constexpr (kLabels)
+    return labels_i2t_hit(a, l, i, j);
+  else
+    return metrics_i2t_hit(a, i, j);
+}
+template <bool kLabels>
+__device__ __forceinline__ bool finalize_t2i_hit(const MetricsArgs& a, const LabelSetArgs& l, int i, int g) {
+  if constexpr (kLabels)
+    return labels_t2i_hit(a, l, i, g);
+  else
+    return metrics_t2i_hit(a, i, g);
+}
+
 __device__ __forceinline__ int key_index(unsigned long long k) {
   return k == 0ull ? -1 : static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(k));
 }
 
-__global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const MetricsArgs a) {
+// kLabels: the hit rule of a label-set step (LabelSetArgs); the kernel without it is metrics_finalize_kernel below
+template <bool kLabels>
+__device__ __forceinline__ void metrics_finalize(const MetricsArgs& a, const LabelSetArgs& l) {
   __shared__ unsigned int hits[2];
   const int tid = threadIdx.x;
   if (tid < 2) hits[tid] = 0u;
@@ -2104,18 +2234,18 @@ __global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const
   }
   __syncthreads();
   unsigned int h_i2t = 0, h_t2i = 0;
-  // column partials are read for the paired texts (i < B), and under extra_ids for every text of this rank (i < T);
-  // otherwise the extras' column keys are computed but never read
-  const int nt = a.extra_ids ? a.T : a.B;
-  // images ranked by i2t: the paired ones, and under extra_image_ids every image of this rank (row keys of the extras
-  // are computed but never read otherwise)
-  const int ni = a.extra_image_ids ? a.R : a.B;
+  // column partials are read for the paired texts (i < B), and under extra_ids or label sets for every text of this
+  // rank (i < T); otherwise the extras' column keys are computed but never read
+  const int nt = (kLabels || a.extra_ids) ? a.T : a.B;
+  // images ranked by i2t: the paired ones, and under extra_image_ids or label sets every image of this rank (row keys
+  // of the extras are computed but never read otherwise)
+  const int ni = (kLabels || a.extra_image_ids) ? a.R : a.B;
   const int n = ni > nt ? ni : nt;
   for (int i = tid; i < n; i += kMetricsThreads) {
     if (i < ni) {
       const int j = key_index(a.row_keys[i]);   // best text of my image i, over all texts including the extras
       if (a.i2t) a.i2t[i] = j;
-      if (j >= 0) h_i2t += metrics_i2t_hit(a, i, j);
+      if (j >= 0) h_i2t += finalize_i2t_hit<kLabels>(a, l, i, j);
     }
     if (i >= nt) continue;
     unsigned long long k = a.col_own[i];
@@ -2129,7 +2259,7 @@ __global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const
     }
     const int g = key_index(k);               // best image of my text i
     if (a.t2i) a.t2i[i] = g;
-    if (g >= 0) h_t2i += metrics_t2i_hit(a, i, g);
+    if (g >= 0) h_t2i += finalize_t2i_hit<kLabels>(a, l, i, g);
   }
   // integer counts: the sum does not depend on the order
   for (int o = 16; o > 0; o >>= 1) {
@@ -2142,6 +2272,14 @@ __global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const
   }
   __syncthreads();
   if (tid < 2) a.top1[tid] = static_cast<float>(hits[tid]) / static_cast<float>(tid == 0 ? ni : nt);
+}
+
+__global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_kernel(const MetricsArgs a) {
+  metrics_finalize<false>(a, LabelSetArgs{});
+}
+__global__ void __launch_bounds__(kMetricsThreads) metrics_finalize_labels_kernel(const MetricsArgs a,
+                                                                                  const LabelSetArgs l) {
+  metrics_finalize<true>(a, l);
 }
 
 // Finalisation of the per-sample losses (SampleLossArgs). Like metrics_finalize_kernel it never triggers
@@ -2210,7 +2348,9 @@ __global__ void __launch_bounds__(kSampleLossThreads) sample_loss_finalize_kerne
 // the step: the same protocol as the metric keys (DESIGN.md, "Top-K retrieval").
 constexpr int kTopKThreads = 1024;
 
-__global__ void __launch_bounds__(kTopKThreads) topk_finalize_kernel(const TopKArgs t) {
+// kLabels: the hit rule of a label-set step (LabelSetArgs); the kernel without it is topk_finalize_kernel below
+template <bool kLabels>
+__device__ __forceinline__ void topk_finalize(const TopKArgs& t, const LabelSetArgs& l) {
   const MetricsArgs& a = t.m;
   // first[side][s]: samples whose first hit is at rank s (s = K: no hit among the K)
   __shared__ unsigned int first[2][kTopKMax + 1];
@@ -2248,9 +2388,9 @@ __global__ void __launch_bounds__(kTopKThreads) topk_finalize_kernel(const TopKA
   }
   __syncthreads();
   const int K = t.k;
-  // the images and texts ranked, as in metrics_finalize_kernel
-  const int nt = a.extra_ids ? a.T : a.B;
-  const int ni = a.extra_image_ids ? a.R : a.B;
+  // the images and texts ranked, as in metrics_finalize
+  const int nt = (kLabels || a.extra_ids) ? a.T : a.B;
+  const int ni = (kLabels || a.extra_image_ids) ? a.R : a.B;
   const int n = ni > nt ? ni : nt;
   unsigned int cnt[2][kTopKMax + 1] = {};   // per thread, by first-hit rank (K: none)
   for (int i = tid; i < n; i += kTopKThreads) {
@@ -2264,7 +2404,7 @@ __global__ void __launch_bounds__(kTopKThreads) topk_finalize_kernel(const TopKA
         if (s < K) {
           const int j = key_index(key[s]);
           if (t.i2t) t.i2t[static_cast<size_t>(i) * K + s] = j;
-          if (f == K && j >= 0 && metrics_i2t_hit(a, i, j)) f = s;
+          if (f == K && j >= 0 && finalize_i2t_hit<kLabels>(a, l, i, j)) f = s;
         }
       }
 #pragma unroll
@@ -2313,7 +2453,7 @@ __global__ void __launch_bounds__(kTopKThreads) topk_finalize_kernel(const TopKA
       if (s < K) {
         const int g = key_index(key[s]);
         if (t.t2i) t.t2i[static_cast<size_t>(i) * K + s] = g;
-        if (f == K && g >= 0 && metrics_t2i_hit(a, i, g)) f = s;
+        if (f == K && g >= 0 && finalize_t2i_hit<kLabels>(a, l, i, g)) f = s;
       }
     }
 #pragma unroll
@@ -2338,6 +2478,13 @@ __global__ void __launch_bounds__(kTopKThreads) topk_finalize_kernel(const TopKA
       t.recall[tid * K + s] = static_cast<float>(hits) / static_cast<float>(tid == 0 ? ni : nt);
     }
   }
+}
+
+__global__ void __launch_bounds__(kTopKThreads) topk_finalize_kernel(const TopKArgs t) {
+  topk_finalize<false>(t, LabelSetArgs{});
+}
+__global__ void __launch_bounds__(kTopKThreads) topk_finalize_labels_kernel(const TopKArgs t, const LabelSetArgs l) {
+  topk_finalize<true>(t, l);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -2643,6 +2790,20 @@ int launch_gemm(int cta_group, int mode, int stages, int mcast, int tile_n, cons
       default: return launch_impl<kModeDistill, kDistillStages, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
     }
   }
+  if (mode == kModeLoss && p.col_lab != nullptr) {   // label sets (with any option but distillation): kModeLabels
+    const bool s4 = stages == 4;
+    switch (cluster_size(cta_group, mcast)) {
+      case 4:
+        return s4 ? launch_impl<kModeLabels, 4, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeLabels, 6, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      case 2:
+        return s4 ? launch_impl<kModeLabels, 4, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeLabels, 6, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      default:
+        return s4 ? launch_impl<kModeLabels, 4, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeLabels, 6, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+    }
+  }
   if (mode == kModeLoss && p.col_grp != nullptr) {   // excluded groups (with any other option): kModeGroups
     const bool s4 = stages == 4;
     switch (cluster_size(cta_group, mcast)) {
@@ -2774,6 +2935,11 @@ int launch_metrics_finalize(const MetricsArgs& a, cudaStream_t stream) {
   return static_cast<int>(cudaGetLastError());
 }
 
+int launch_metrics_finalize_labels(const MetricsArgs& a, const LabelSetArgs& l, cudaStream_t stream) {
+  metrics_finalize_labels_kernel<<<1, kMetricsThreads, 0, stream>>>(a, l);
+  return static_cast<int>(cudaGetLastError());
+}
+
 int launch_sample_loss_finalize(const SampleLossArgs& a, cudaStream_t stream) {
   sample_loss_finalize_kernel<<<1, kSampleLossThreads, 0, stream>>>(a);
   return static_cast<int>(cudaGetLastError());
@@ -2781,6 +2947,11 @@ int launch_sample_loss_finalize(const SampleLossArgs& a, cudaStream_t stream) {
 
 int launch_topk_finalize(const TopKArgs& a, cudaStream_t stream) {
   topk_finalize_kernel<<<1, kTopKThreads, 0, stream>>>(a);
+  return static_cast<int>(cudaGetLastError());
+}
+
+int launch_topk_finalize_labels(const TopKArgs& a, const LabelSetArgs& l, cudaStream_t stream) {
+  topk_finalize_labels_kernel<<<1, kTopKThreads, 0, stream>>>(a, l);
   return static_cast<int>(cudaGetLastError());
 }
 

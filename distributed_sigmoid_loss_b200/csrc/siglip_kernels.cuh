@@ -181,6 +181,13 @@ struct KernelParams {
   const int64_t* row_grp;        // [grp_rows]: groups of this rank's images (rows of the launch)
   const int64_t* col_grp;        // [N]: groups of the texts of the chunk being scored
   int grp_rows;                  // rows that carry a group (row_grp has this many entries); rows past it match nothing
+  // Multi-label positives from label sets (SIGLIP_OPT_LABEL_SETS). Appended last like the fields above. Non-null
+  // col_lab selects the kModeLabels loss kernel: a pair (i, j) is also a positive when the sets row_lab[i] and col_lab[j]
+  // share a label >= 0 (negative entries are empty slots). Groups, ids, weights, metric keys, per-sample sums and top-K
+  // lists stay runtime options there; excluded groups apply after these positives.
+  const int64_t* row_lab;        // [M][lab_m]: the sets of this rank's images (rows of the launch)
+  const int64_t* col_lab;        // [N][lab_m]: the sets of the texts of the chunk being scored
+  int lab_m;                     // labels per set, 1 .. kMaxLabels
 };
 
 // kModeDistill: the loss kernel of a distillation step (KernelParams::k_teacher > 0), its own instantiation
@@ -190,7 +197,20 @@ struct KernelParams {
 // metric keys and per-sample-loss sums are runtime options in it
 // kModeGroups: the loss kernel of a step with excluded same-group pairs (KernelParams::col_grp != null), its own
 // instantiation; ids, weights, metric keys, per-sample-loss sums and top-K lists are runtime options in it
-enum KernelMode { kModeLoss = 0, kModeOut = 1, kModeDistill = 2, kModeSampleLoss = 3, kModeTopK = 4, kModeGroups = 5 };
+// kModeLabels: the loss kernel of a step with label sets (KernelParams::col_lab != null), its own instantiation; ids,
+// weights, metric keys, per-sample-loss sums, top-K lists and excluded groups are runtime options in it
+enum KernelMode {
+  kModeLoss = 0,
+  kModeOut = 1,
+  kModeDistill = 2,
+  kModeSampleLoss = 3,
+  kModeTopK = 4,
+  kModeGroups = 5,
+  kModeLabels = 6
+};
+
+// Label sets: labels per set at most (SIGLIP_MAX_LABELS)
+constexpr int kMaxLabels = 4;
 
 // Top-K retrieval: slots of every list (SIGLIP_TOPK_MAX), whatever K the step asks
 constexpr int kTopKMax = 10;
@@ -333,6 +353,22 @@ struct TopKArgs {
   int64_t* t2i;                                // [nt][k] or null
 };
 int launch_topk_finalize(const TopKArgs& a, cudaStream_t stream);
+
+// The hit rule of a label-set step (SIGLIP_OPT_LABEL_SETS) for the metrics and top-K finalisations: a hit is the
+// positional pair (my image i and my paired text i, i < B) or a pair whose sets share a label >= 0. i2t ranks all R
+// images and t2i all T texts. These launches run their own instantiation of the finalisation kernels; the MetricsArgs
+// id fields are unused.
+struct LabelSetArgs {
+  const int64_t* row_sets;                     // [R][m] the sets of this rank's images: paired, then extra
+  const int64_t* text_own;                     // [T][m] the sets of this rank's texts: paired, then extra
+  const int64_t* text_all;                     // [world][slot]: every chunk's text sets, gathered in this step
+  long long slot;                              // words between two chunks' sets in text_all
+  const int64_t* const* xsets_peers;           // [world] every rank's published extra-image sets ([E_o][m]) of this
+                                               // step (world > 1 with extra images; own entry unused)
+  int m;                                       // labels per set
+};
+int launch_metrics_finalize_labels(const MetricsArgs& a, const LabelSetArgs& l, cudaStream_t stream);
+int launch_topk_finalize_labels(const TopKArgs& a, const LabelSetArgs& l, cudaStream_t stream);
 int launch_wait_flags(const volatile unsigned int* flags, int n, unsigned int value, unsigned long long timeout_ns,
                       DebugRecord* dbg, cudaStream_t stream);
 

@@ -24,6 +24,8 @@ from . import _capi
 
 # Largest K of the top-K in-batch retrieval (SIGLIP_TOPK_MAX in include/siglip_b200.h)
 TOPK_MAX = 10
+# labels per set at most (SIGLIP_MAX_LABELS): multi_label=M takes 1 <= M <= MAX_LABELS
+MAX_LABELS = 4
 
 
 def _group_rank_world(group) -> Tuple[int, int]:
@@ -51,7 +53,8 @@ class SigmoidLossEngine:
 
     def __init__(self, batch: int, dim: int, device: torch.device, group=None, cta_group: int = 2,
                  overlap_pull: bool = True, rank_world: Optional[Tuple[int, int]] = None, loopback: bool = False,
-                 batch_per_rank=None, texts_per_rank=None, images_per_rank=None, teacher_dim: int = 0):
+                 batch_per_rank=None, texts_per_rank=None, images_per_rank=None, teacher_dim: int = 0,
+                 labels: int = 0):
         self._L = _capi.lib()
         if not torch.cuda.is_available() or self._L.siglip_device_count() == 0:
             raise RuntimeError("distributed_sigmoid_loss_b200 needs an sm_90 (H100) device; there is no CPU fallback")
@@ -61,7 +64,19 @@ class SigmoidLossEngine:
         self.teacher_dim = int(teacher_dim)
         if self.teacher_dim and (images_per_rank is not None or texts_per_rank is not None):
             raise RuntimeError("a distillation engine (teacher_dim > 0) takes no extra texts or images")
-        if self.teacher_dim:
+        self.labels = int(labels)   # labels per set of a label-set engine (siglip_ctx_create_labels), 0: none
+        if self.labels and self.teacher_dim:
+            raise RuntimeError("a label-set engine (labels > 0) takes no teacher")
+        if self.labels:
+            # label sets: the sets' width is part of the exported allocation (siglip_ctx_create_labels)
+            bpr, ipr, tpr = self._extras_lists(batch, batch_per_rank, images_per_rank, texts_per_rank)
+            _capi.check(self._L.siglip_ctx_create_labels(ctypes.byref(h), self.device.index or 0, self.rank, self.world,
+                                                         (ctypes.c_int * self.world)(*bpr),
+                                                         (ctypes.c_int * self.world)(*ipr),
+                                                         (ctypes.c_int * self.world)(*tpr), dim, self.labels))
+            self.batch_per_rank, self.images_per_rank, self.texts_per_rank = bpr, ipr, tpr
+            images_per_rank, texts_per_rank = ipr, tpr
+        elif self.teacher_dim:
             # distillation: the teacher width is part of the exported allocation (siglip_ctx_create_distill)
             bpr = [int(b) for b in batch_per_rank] if batch_per_rank is not None else [batch] * self.world
             if len(bpr) != self.world or bpr[self.rank] != batch:
@@ -72,15 +87,7 @@ class SigmoidLossEngine:
         elif images_per_rank is not None:
             # extra images: rank p holds images_per_rank[p] >= its batch images, the paired ones first, then its extras
             # (siglip_ctx_create_extras); every rank passes the same three lists
-            bpr = [int(b) for b in batch_per_rank] if batch_per_rank is not None else [batch] * self.world
-            ipr = [int(r) for r in images_per_rank]
-            tpr = [int(t) for t in texts_per_rank] if texts_per_rank is not None else list(bpr)
-            if len(bpr) != self.world or bpr[self.rank] != batch or len(ipr) != self.world or len(tpr) != self.world:
-                raise RuntimeError(f"batch_per_rank {bpr} / images_per_rank {ipr} / texts_per_rank {tpr} must list one "
-                                   f"entry per rank and hold batch {batch} at rank {self.rank}")
-            if any(r < b for r, b in zip(ipr, bpr)) or any(t < b for t, b in zip(tpr, bpr)):
-                raise RuntimeError(f"images_per_rank {ipr} and texts_per_rank {tpr} must be >= batch_per_rank {bpr} on "
-                                   f"every rank")
+            bpr, ipr, tpr = self._extras_lists(batch, batch_per_rank, images_per_rank, texts_per_rank)
             _capi.check(self._L.siglip_ctx_create_extras(ctypes.byref(h), self.device.index or 0, self.rank, self.world,
                                                          (ctypes.c_int * self.world)(*bpr),
                                                          (ctypes.c_int * self.world)(*ipr),
@@ -121,6 +128,7 @@ class SigmoidLossEngine:
         self.images = self.images_per_rank[self.rank]   # rows of img / dimg: the batch plus this rank's extra images
         self.extra_text_ids = False   # SIGLIP_OPT_EXTRA_TEXT_IDS: every text of a chunk carries an id (see set_option)
         self.extra_image_ids = False  # SIGLIP_OPT_EXTRA_IMAGE_IDS: every image of this rank carries an id
+        self.label_sets = False       # SIGLIP_OPT_LABEL_SETS: every sample, extra text and extra image carries a set
         self._h = h
         _capi.check(self._L.siglip_ctx_set_option(h, _capi.SIGLIP_OPT_CTA_GROUP, int(cta_group)))
         _capi.check(self._L.siglip_ctx_set_option(h, _capi.SIGLIP_OPT_OVERLAP_PULL, int(bool(overlap_pull))))
@@ -129,6 +137,21 @@ class SigmoidLossEngine:
                 _capi.check(self._L.siglip_debug_loopback(h))
             else:
                 self._exchange_handles()
+
+    def _extras_lists(self, batch: int, batch_per_rank, images_per_rank, texts_per_rank):
+        """(batch_per_rank, images_per_rank, texts_per_rank) of an engine created with extras or label sets: one entry
+        per rank (None: the batch on every rank, and no extras), this rank's batch at its index, and images and texts
+        at least the batch on every rank."""
+        bpr = [int(b) for b in batch_per_rank] if batch_per_rank is not None else [batch] * self.world
+        ipr = [int(r) for r in images_per_rank] if images_per_rank is not None else list(bpr)
+        tpr = [int(t) for t in texts_per_rank] if texts_per_rank is not None else list(bpr)
+        if len(bpr) != self.world or bpr[self.rank] != batch or len(ipr) != self.world or len(tpr) != self.world:
+            raise RuntimeError(f"batch_per_rank {bpr} / images_per_rank {ipr} / texts_per_rank {tpr} must list one "
+                               f"entry per rank and hold batch {batch} at rank {self.rank}")
+        if any(r < b for r, b in zip(ipr, bpr)) or any(t < b for t, b in zip(tpr, bpr)):
+            raise RuntimeError(f"images_per_rank {ipr} and texts_per_rank {tpr} must be >= batch_per_rank {bpr} on "
+                               f"every rank")
+        return bpr, ipr, tpr
 
     # -- peer bootstrap: replaces the reference's reliance on the process group for every step ------------
     def _exchange_handles(self) -> None:
@@ -147,6 +170,8 @@ class SigmoidLossEngine:
             self.extra_text_ids = bool(value)   # the library clears the extras' ids with the sample ids
         if option == _capi.SIGLIP_OPT_EXTRA_IMAGE_IDS or (option == _capi.SIGLIP_OPT_SAMPLE_IDS and not value):
             self.extra_image_ids = bool(value)
+        if option == _capi.SIGLIP_OPT_LABEL_SETS:
+            self.label_sets = bool(value)
 
     def set_sigma_budget(self, sigma_budget_bytes: Optional[int]) -> None:
         """SIGLIP_OPT_SIGMA_BUDGET_MIB: bound the 16-bit sigma operands to sigma_budget_bytes (rounded down to MiB; None
@@ -295,6 +320,39 @@ class SigmoidLossEngine:
         self._check_ids(groups, self.texts_per_rank[chunk])
         _capi.check(self._L.siglip_debug_set_chunk_groups(self._h, chunk, groups.data_ptr(), self._stream()))
 
+    def set_label_sets(self, sample_labels: torch.Tensor, extra_text_labels: Optional[torch.Tensor] = None,
+                       extra_image_labels: Optional[torch.Tensor] = None) -> None:
+        """SIGLIP_OPT_LABEL_SETS: this rank's label sets for the NEXT step, contiguous int64 on the engine's device:
+        sample_labels [B, M] (image i and paired text i), extra_text_labels [T - B, M] and extra_image_labels [R - B, M],
+        or None for empty sets. Copied on the current stream like set_sample_ids; a negative entry is an empty slot."""
+        self._check_sets(sample_labels, self.batch)
+        for x, n in ((extra_text_labels, self.texts - self.batch), (extra_image_labels, self.images - self.batch)):
+            if x is not None:
+                self._check_sets(x, n)
+        with torch.cuda.device(self.device):
+            _capi.check(self._L.siglip_set_label_sets(
+                self._h, sample_labels.data_ptr(),
+                extra_text_labels.data_ptr() if extra_text_labels is not None else None,
+                extra_image_labels.data_ptr() if extra_image_labels is not None else None, self._stream()))
+
+    def debug_set_chunk_label_sets(self, chunk: int, sets: torch.Tensor) -> None:
+        """Loopback: the text sets of chunk `chunk` ([T_c, M] int64) as its owner would have published them."""
+        self._check_sets(sets, self.texts_per_rank[chunk])
+        _capi.check(self._L.siglip_debug_set_chunk_label_sets(self._h, chunk, sets.data_ptr(), self._stream()))
+
+    def debug_set_peer_extra_image_label_sets(self, peer: int, sets: torch.Tensor) -> None:
+        """Loopback: the extra-image sets ([R_peer - B_peer, M] int64) standing in for what peer `peer` publishes in a
+        metrics or top-K step."""
+        self._check_sets(sets, self.images_per_rank[peer] - self.batch_per_rank[peer])
+        _capi.check(self._L.siglip_debug_set_peer_extra_image_label_sets(self._h, peer, sets.data_ptr(),
+                                                                         self._stream()))
+
+    def _check_sets(self, sets: torch.Tensor, n: int) -> None:
+        if sets.dtype != torch.int64 or tuple(sets.shape) != (n, self.labels) or not sets.is_contiguous() or \
+                sets.device != self.device:
+            raise RuntimeError(f"label sets must be a contiguous int64 [{n}, {self.labels}] tensor on {self.device}, "
+                               f"got {tuple(sets.shape)} {sets.dtype} on {sets.device}")
+
     def debug_set_chunk_ids(self, chunk: int, ids: torch.Tensor) -> None:
         """Loopback: the ids of text chunk `chunk` as its owner would have published them: its sample ids ([B_c]), or
         under SIGLIP_OPT_EXTRA_TEXT_IDS the ids of all its texts ([T_c])."""
@@ -395,13 +453,15 @@ class SigmoidLossEngine:
 
     @property
     def metric_images(self) -> int:
-        """Images of this rank that i2t ranks: the paired ones, or all R under SIGLIP_OPT_EXTRA_IMAGE_IDS."""
-        return self.images if self.extra_image_ids else self.batch
+        """Images of this rank that i2t ranks: the paired ones, or all R under SIGLIP_OPT_EXTRA_IMAGE_IDS or
+        SIGLIP_OPT_LABEL_SETS."""
+        return self.images if (self.extra_image_ids or self.label_sets) else self.batch
 
     @property
     def metric_texts(self) -> int:
-        """Texts of this rank that t2i ranks: the paired ones, or all T under SIGLIP_OPT_EXTRA_TEXT_IDS."""
-        return self.texts if self.extra_text_ids else self.batch
+        """Texts of this rank that t2i ranks: the paired ones, or all T under SIGLIP_OPT_EXTRA_TEXT_IDS or
+        SIGLIP_OPT_LABEL_SETS."""
+        return self.texts if (self.extra_text_ids or self.label_sets) else self.batch
 
     def debug_get_slot(self, chunk: int) -> torch.Tensor:
         out = torch.empty(self.texts_per_rank[chunk], self.dim, device=self.device, dtype=torch.float32)
@@ -692,12 +752,15 @@ class _SigmoidLossFn(torch.autograd.Function):
     sample_losses: (image_loss [R], text_loss [T]) fp32 output buffers: the per-sample losses of this call's step are
     armed. Like the metrics, a re-run of the forward by the backward's generation guard does not arm them again.
     groups: (image_groups [R], text_groups [T]) int64 (SIGLIP_OPT_EXCLUDE_GROUPS engines), set before every step the
-    engine runs for this call, like the ids."""
+    engine runs for this call, like the ids.
+    label_sets: (sample_labels [B, M], extra_text_labels [T - B, M] or None, extra_image_labels [R - B, M] or None) int64
+    (SIGLIP_OPT_LABEL_SETS engines), set before every step the engine runs for this call, like the ids."""
 
     @staticmethod
     def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool = False, fused: bool = False,
                 ids: Optional[torch.Tensor] = None, metrics=None, extra_ids: Optional[torch.Tensor] = None, weights=None,
-                extra_img_ids: Optional[torch.Tensor] = None, teacher=None, sample_losses=None, groups=None):
+                extra_img_ids: Optional[torch.Tensor] = None, teacher=None, sample_losses=None, groups=None,
+                label_sets=None):
         need_grad = any(ctx.needs_input_grad[:4])
         raw = None
         # bf16 callers: bf16 operands (what autograd would multiply). Anything wider (the reference's own test feeds
@@ -739,6 +802,7 @@ class _SigmoidLossFn(torch.autograd.Function):
             engine.set_teacher(*teacher)
         ctx.ids, ctx.extra_ids, ctx.weights, ctx.extra_img_ids = ids, extra_ids, weights, extra_img_ids
         ctx.groups = groups
+        ctx.label_sets = label_sets
         # the split schedule's backward may have to re-run the forward with the same teacher; the fused one never does
         ctx.teacher = None if ctx.fused else teacher
         if ids is not None:
@@ -751,6 +815,8 @@ class _SigmoidLossFn(torch.autograd.Function):
             engine.set_sample_weights(*weights)
         if groups is not None:
             engine.set_groups(*groups)
+        if label_sets is not None:
+            engine.set_label_sets(*label_sets)
         if metrics is not None:
             engine.request_metrics(*metrics[:3])
             if len(metrics) > 3:   # metrics_topk = K > 1: (K, recall, i2t_topk, t2i_topk) follow
@@ -814,6 +880,8 @@ class _SigmoidLossFn(torch.autograd.Function):
                     eng.set_sample_weights(*ctx.weights)
                 if ctx.groups is not None:
                     eng.set_groups(*ctx.groups)
+                if ctx.label_sets is not None:
+                    eng.set_label_sets(*ctx.label_sets)
                 if ctx.teacher is not None:
                     eng.set_teacher(*ctx.teacher)
                 eng.forward(img_b, txt_b, tp, b, True)
@@ -832,7 +900,7 @@ class _SigmoidLossFn(torch.autograd.Function):
                 gt = dtxt.to(tdt) if ctx.needs_input_grad[1] else None
         gp = dtp.reshape(pshape).to(device=pdev, dtype=pdt) if ctx.needs_input_grad[2] else None
         gb = db.reshape(bshape).to(device=bdev, dtype=bdt) if ctx.needs_input_grad[3] else None
-        return gi, gt, gp, gb, None, None, None, None, None, None, None, None, None, None, None
+        return gi, gt, gp, gb, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 class _EngineCache:
@@ -840,9 +908,10 @@ class _EngineCache:
                  bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
                  extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
                  distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None,
-                 exclude_groups: bool = False):
+                 exclude_groups: bool = False, multi_label: int = 0):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
         self.exclude_groups = exclude_groups
+        self.multi_label = multi_label
         self.sigma_budget_bytes = sigma_budget_bytes
         self.distill = distill
         self.extra_images = extra_images
@@ -871,14 +940,16 @@ class _EngineCache:
                 ipr = [int(b) + self.extra_images for b in bpr]
             eng = SigmoidLossEngine(batch, dim, dev, self.group, self.cta_group, self.overlap_pull,
                                     batch_per_rank=self.batch_per_rank, texts_per_rank=tpr, images_per_rank=ipr,
-                                    teacher_dim=teacher_dim)
+                                    teacher_dim=teacher_dim, labels=self.multi_label)
             if self.sync_scalar_grads:
                 eng.set_option(_capi.SIGLIP_OPT_SYNC_SCALAR_GRADS, 1)
             if self.bidir:
                 eng.set_option(_capi.SIGLIP_OPT_BIDIR, 1)
             if self.multi_positive:
                 eng.set_option(_capi.SIGLIP_OPT_SAMPLE_IDS, 1)
-            if self.extra_texts:
+            if self.multi_label:
+                eng.set_option(_capi.SIGLIP_OPT_LABEL_SETS, 1)
+            if self.extra_texts and not self.multi_label:
                 eng.set_option(_capi.SIGLIP_OPT_EXTRA_TEXT_IDS, 1)   # needs the sample ids on first
             if self.extra_images and self.multi_positive:
                 eng.set_option(_capi.SIGLIP_OPT_EXTRA_IMAGE_IDS, 1)
@@ -1114,6 +1185,66 @@ def _groups_of(exclude_groups: bool, image_groups, text_groups, image_embeddings
     gt = _validate_group_ids(text_groups, nt + extras if nt is not None else None, "text_groups", "texts",
                              text_embeddings.device)
     return gi, gt
+
+
+def _validate_multi_label(multi_label, multi_positive: bool, distill) -> int:
+    """multi_label=M of a module: None or 0 (off), or the labels per set, 1 .. MAX_LABELS. Label sets replace the ids of
+    multi_positive, and the distillation loss kernel has no label sets."""
+    if multi_label is None:
+        return 0
+    if isinstance(multi_label, bool) or not isinstance(multi_label, int) or not 0 <= multi_label <= MAX_LABELS:
+        raise RuntimeError(f"multi_label must be None or an int in 1 .. {MAX_LABELS} (labels per set), got "
+                           f"{multi_label!r}")
+    if multi_label and multi_positive:
+        raise RuntimeError("multi_label cannot be combined with multi_positive: label sets replace the sample ids "
+                           "(M = 1 with the ids as labels is multi_positive)")
+    if multi_label and distill is not None:
+        raise RuntimeError("multi_label cannot be combined with distill: the distillation loss kernel has no label sets")
+    return multi_label
+
+
+def _validate_label_set(labels, n: Optional[int], m: int, name: str, what: str, device: torch.device) -> torch.Tensor:
+    if labels is None:
+        raise RuntimeError(f"multi_label={m}: forward needs {name} ([{n}, {m}] integer tensor, one label set per "
+                           f"{what})")
+    if not isinstance(labels, torch.Tensor) or labels.dtype not in _ID_DTYPES:
+        raise RuntimeError(f"{name} must be an integer tensor, got "
+                           f"{labels.dtype if isinstance(labels, torch.Tensor) else type(labels)}")
+    if labels.dim() != 2 or tuple(labels.shape) != (n, m):
+        raise RuntimeError(f"{name} must have shape [{n}, {m}] (one set of {m} labels per {what}), got "
+                           f"{tuple(labels.shape)}")
+    if labels.device != device:
+        raise RuntimeError(f"{name} are on {labels.device}, the embeddings on {device}")
+    return labels.to(torch.int64).contiguous()
+
+
+def _label_sets_of(multi_label: int, sample_labels, extra_text_labels, extra_image_labels,
+                   image_embeddings: torch.Tensor, extra_texts: int, extra_images: int):
+    """sample_labels [B, M] / extra_text_labels [K, M] / extra_image_labels [K_img, M] of a forward: the sample sets are
+    required with multi_label, the extra texts' with extra_texts = K > 0 and the extra images' with extra_images =
+    K_img > 0; every one is refused otherwise (hard negatives get empty sets). A negative label is an empty slot.
+    Returns (sample, extra text or None, extra image or None) as contiguous int64, or None. Raises before any GPU
+    work."""
+    given = (("sample_labels", sample_labels), ("extra_text_labels", extra_text_labels),
+             ("extra_image_labels", extra_image_labels))
+    if not multi_label:
+        for name, v in given:
+            if v is not None:
+                raise RuntimeError(f"{name} given, but the loss was built without multi_label=M")
+        return None
+    if extra_texts == 0 and extra_text_labels is not None:
+        raise RuntimeError("extra_text_labels given, but the loss was built without extra_texts=K (hard negatives have "
+                           "empty label sets)")
+    if extra_images == 0 and extra_image_labels is not None:
+        raise RuntimeError("extra_image_labels given, but the loss was built without extra_images=K")
+    dev = image_embeddings.device
+    nb = image_embeddings.shape[0] if image_embeddings.dim() >= 1 else None
+    ls = _validate_label_set(sample_labels, nb, multi_label, "sample_labels", "sample", dev)
+    lt = _validate_label_set(extra_text_labels, extra_texts, multi_label, "extra_text_labels", "extra text",
+                             dev) if extra_texts else None
+    li = _validate_label_set(extra_image_labels, extra_images, multi_label, "extra_image_labels", "extra image",
+                             dev) if extra_images else None
+    return ls, lt, li
 
 
 def _with_negatives(text_embeddings: torch.Tensor, negative_text) -> torch.Tensor:
@@ -1370,6 +1501,17 @@ class DDPSigmoidLoss(nn.Module):
     give exactly the step without the option. Retrieval metrics and top-K lists are unchanged: every pair stays a
     candidate; the lists hold global indices, so a caller can look the groups up. Works with or without
     ``multi_positive``; not with ``distill``. Collective: set on every rank.
+
+    ``multi_label=M`` (1 <= M <= 4): multi-label positives. Every ``forward`` takes ``sample_labels`` ([B, M] integers:
+    the label set of sample i, shared by image i and caption i; a negative entry is an empty slot, duplicates are
+    allowed) on the embeddings' device, and with ``extra_texts=K`` / ``extra_images=K`` also ``extra_text_labels`` /
+    ``extra_image_labels`` ([K, M]). ``hard_negatives`` get empty sets. A pair is positive iff it is a sample's own
+    pair or its image's and text's sets share a label >= 0 (on any rank): an image labelled {golden retriever, dog} is
+    a positive for the prompts "a photo of a dog" ({dog}) and "a photo of a golden retriever"; a poodle image ({poodle,
+    dog}) only for the first. Every other pair is negative; the loss still divides by B. M = 1 with labels >= 0 is
+    ``multi_positive`` with those ids. Retrieval metrics and top-K lists count a hit by the same rule and rank every
+    image and text of the rank (extras included). Composes with every option but ``multi_positive`` and ``distill``;
+    ``exclude_groups`` applies after these positives. Collective: the same M on every rank.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
@@ -1377,12 +1519,14 @@ class DDPSigmoidLoss(nn.Module):
                  batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
                  extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
                  distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None,
-                 exclude_groups: bool = False) -> None:
+                 exclude_groups: bool = False, multi_label: Optional[int] = None) -> None:
         super().__init__()
         _sigma_budget_mib(sigma_budget_bytes)
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_images = _validate_hard_negatives(extra_images, "extra_images")
-        extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
+        multi_label = _validate_multi_label(multi_label, multi_positive, distill)
+        # extra texts carry ids under multi_positive, label sets under multi_label
+        extra_texts = _validate_extra_texts(extra_texts, multi_positive or bool(multi_label), hard_negatives)
         sample_weights = _validate_sample_weights(sample_weights)
         distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images)
         exclude_groups = _validate_exclude_groups(exclude_groups, distill)
@@ -1413,11 +1557,13 @@ class DDPSigmoidLoss(nn.Module):
         self.distill = distill
         # extension: same-group pairs excluded from the loss (in-batch false negatives made neutral)
         self.exclude_groups = exclude_groups
+        # extension: multi-label positives from per-sample label sets (0: off)
+        self.multi_label = multi_label
         self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank,
                                    multi_positive=multi_positive, hard_negatives=hard_negatives,
                                    extra_texts=extra_texts, sample_weights=sample_weights, extra_images=extra_images,
                                    distill=distill, sigma_budget_bytes=sigma_budget_bytes,
-                                   exclude_groups=exclude_groups)
+                                   exclude_groups=exclude_groups, multi_label=multi_label)
         # extension: bound of the 16-bit sigma operands; steps then run in row panels (memory O(budget), not O(B^2))
         self.sigma_budget_bytes = sigma_budget_bytes
 
@@ -1437,7 +1583,8 @@ class DDPSigmoidLoss(nn.Module):
                 teacher_text: Optional[torch.Tensor] = None, teacher_t_prime: Optional[torch.Tensor] = None,
                 teacher_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False,
                 metrics_topk: Optional[int] = None, image_groups: Optional[torch.Tensor] = None,
-                text_groups: Optional[torch.Tensor] = None):
+                text_groups: Optional[torch.Tensor] = None, sample_labels: Optional[torch.Tensor] = None,
+                extra_text_labels: Optional[torch.Tensor] = None, extra_image_labels: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
         _validate_return_sample_losses(return_sample_losses, self.distill)
         topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill)
@@ -1447,13 +1594,16 @@ class DDPSigmoidLoss(nn.Module):
         ids = _validate_ids(sample_ids, self.multi_positive, image_embeddings)
         _validate_negatives(text_embeddings, negative_text, self.hard_negatives)
         _validate_negatives(text_embeddings, extra_text, self.extra_texts, "extra_text", "extra_texts")
-        extra_ids = _validate_extra_text_ids(extra_text_ids, self.extra_texts, text_embeddings)
+        extra_ids = _validate_extra_text_ids(extra_text_ids, 0 if self.multi_label else self.extra_texts,
+                                             text_embeddings)
         _validate_negatives(image_embeddings, extra_image, self.extra_images, "extra_image", "extra_images", "images")
         ximg_ids = _validate_extra_image_ids(extra_image_ids, self.extra_images, self.multi_positive, image_embeddings)
         weights = _weights_of(self.sample_weights, image_weights, text_weights, image_embeddings, text_embeddings,
                               self.hard_negatives + self.extra_texts, self.extra_images)
         groups = _groups_of(self.exclude_groups, image_groups, text_groups, image_embeddings, text_embeddings,
                             self.hard_negatives + self.extra_texts, self.extra_images)
+        label_sets = _label_sets_of(self.multi_label, sample_labels, extra_text_labels, extra_image_labels,
+                                    image_embeddings, self.extra_texts, self.extra_images)
         _validate(image_embeddings, text_embeddings, self.gpu_batch_size)
         text_embeddings = _with_negatives(_with_negatives(text_embeddings, negative_text), extra_text)
         image_embeddings = _with_negatives(image_embeddings, extra_image)
@@ -1466,7 +1616,7 @@ class DDPSigmoidLoss(nn.Module):
         lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
         loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
                                     self.normalize_inputs, fused, ids, bufs, extra_ids, weights, ximg_ids, teacher,
-                                    lbufs, groups)
+                                    lbufs, groups, label_sets)
         return _with_outputs(loss, bufs, lbufs)
 
 
@@ -1493,24 +1643,30 @@ class SigLipLoss(nn.Module):
     ``return_sample_losses=True``: also returns the per-sample losses of ``DDPSigmoidLoss`` (``image_loss`` [R],
     ``text_loss`` [T]) as the last element, after the metrics when both are asked; like the metrics they stay out of
     the ``output_dict``. ``exclude_groups=True``: every forward takes ``image_groups`` [B + K_img] and ``text_groups``
-    [B + K], and same-group pairs that are not positives are excluded from the loss, as in ``DDPSigmoidLoss``."""
+    [B + K], and same-group pairs that are not positives are excluded from the loss, as in ``DDPSigmoidLoss``.
+    ``multi_label=M``: every forward takes ``sample_labels`` [B, M] (and ``extra_text_labels`` / ``extra_image_labels``
+    [K, M] with ``extra_texts`` / ``extra_images``), and pairs whose label sets meet are positives, as in
+    ``DDPSigmoidLoss``."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
                  multi_positive: bool = False, hard_negatives: int = 0, extra_texts: int = 0,
                  sample_weights: bool = False, extra_images: int = 0, distill: Optional[float] = None,
-                 sigma_budget_bytes: Optional[int] = None, exclude_groups: bool = False):
+                 sigma_budget_bytes: Optional[int] = None, exclude_groups: bool = False,
+                 multi_label: Optional[int] = None):
         super().__init__()
         _sigma_budget_mib(sigma_budget_bytes)
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_images = _validate_hard_negatives(extra_images, "extra_images")
-        extra_texts = _validate_extra_texts(extra_texts, multi_positive, hard_negatives)
+        multi_label = _validate_multi_label(multi_label, multi_positive, distill)
+        extra_texts = _validate_extra_texts(extra_texts, multi_positive or bool(multi_label), hard_negatives)
         sample_weights = _validate_sample_weights(sample_weights)
         distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images)
         exclude_groups = _validate_exclude_groups(exclude_groups, distill)
         self.distill = distill
         self.exclude_groups = exclude_groups
+        self.multi_label = multi_label
         self.cache_labels, self.rank, self.world_size, self.bidir = cache_labels, rank, world_size, bidir
         self.use_horovod = use_horovod
         self.fused_step = fused_step
@@ -1522,7 +1678,7 @@ class SigLipLoss(nn.Module):
         self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive,
                                    hard_negatives=hard_negatives, extra_texts=extra_texts, sample_weights=sample_weights,
                                    extra_images=extra_images, distill=distill, sigma_budget_bytes=sigma_budget_bytes,
-                                   exclude_groups=exclude_groups)
+                                   exclude_groups=exclude_groups, multi_label=multi_label)
         # bound of the 16-bit sigma operands; steps then run in row panels (as on DDPSigmoidLoss)
         self.sigma_budget_bytes = sigma_budget_bytes
 
@@ -1535,7 +1691,8 @@ class SigLipLoss(nn.Module):
                 teacher_text: Optional[torch.Tensor] = None, teacher_logit_scale: Optional[torch.Tensor] = None,
                 teacher_logit_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False,
                 metrics_topk: Optional[int] = None, image_groups: Optional[torch.Tensor] = None,
-                text_groups: Optional[torch.Tensor] = None):
+                text_groups: Optional[torch.Tensor] = None, sample_labels: Optional[torch.Tensor] = None,
+                extra_text_labels: Optional[torch.Tensor] = None, extra_image_labels: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
         _validate_return_sample_losses(return_sample_losses, self.distill)
         topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill)
@@ -1545,13 +1702,15 @@ class SigLipLoss(nn.Module):
         ids = _validate_ids(sample_ids, self.multi_positive, image_features)
         _validate_negatives(text_features, negative_text, self.hard_negatives)
         _validate_negatives(text_features, extra_text, self.extra_texts, "extra_text", "extra_texts")
-        extra_ids = _validate_extra_text_ids(extra_text_ids, self.extra_texts, text_features)
+        extra_ids = _validate_extra_text_ids(extra_text_ids, 0 if self.multi_label else self.extra_texts, text_features)
         _validate_negatives(image_features, extra_image, self.extra_images, "extra_image", "extra_images", "images")
         ximg_ids = _validate_extra_image_ids(extra_image_ids, self.extra_images, self.multi_positive, image_features)
         weights = _weights_of(self.sample_weights, image_weights, text_weights, image_features, text_features,
                               self.hard_negatives + self.extra_texts, self.extra_images)
         groups = _groups_of(self.exclude_groups, image_groups, text_groups, image_features, text_features,
                             self.hard_negatives + self.extra_texts, self.extra_images)
+        label_sets = _label_sets_of(self.multi_label, sample_labels, extra_text_labels, extra_image_labels,
+                                    image_features, self.extra_texts, self.extra_images)
         _validate(image_features, text_features, None)
         batch = image_features.shape[0]
         text_features = _with_negatives(_with_negatives(text_features, negative_text), extra_text)
@@ -1570,6 +1729,6 @@ class SigLipLoss(nn.Module):
         bufs = _topk_buffers(eng, topk, bufs)
         lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
         loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs,
-                                    extra_ids, weights, ximg_ids, teacher, lbufs, groups)
+                                    extra_ids, weights, ximg_ids, teacher, lbufs, groups, label_sets)
         out = {"contrastive_loss": loss} if output_dict else loss
         return _with_outputs(out, bufs, lbufs)

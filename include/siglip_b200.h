@@ -178,6 +178,21 @@ enum {
                                      SIGLIP_ERR_STATE before any launch); the text groups travel to the other ranks with
                                      the text. Unavailable with SIGLIP_OPT_DISTILL and in the host-buffer entries
                                      (SIGLIP_ERR_STATE). Collective. Default 0 */
+  SIGLIP_OPT_LABEL_SETS = 28, /* 1: multi-label positives (siglip_ctx_create_labels contexts only, else
+                                 SIGLIP_ERR_STATE). Every sample carries a set of M int64 labels (a negative entry is an
+                                 empty slot; duplicates are allowed), shared by its image and its paired text; extra
+                                 texts and extra images carry their own. Pair (image i, text j) is positive iff it is the
+                                 own-chunk positional pair (i == j < B_r on the own chunk) or the two sets share a label
+                                 >= 0; every other pair is negative. Loss and gradients keep their formulas (the loss
+                                 divides by B_r); the own diagonal keeps its fp32 term, other positives go through the
+                                 sigma operand like id positives. M = 1 with labels >= 0 is SIGLIP_OPT_SAMPLE_IDS with
+                                 those ids (under ids, -1 is an ordinary id; here it is an empty slot). Excluded groups
+                                 apply after these positives. Metrics and top-K lists count a hit by the same rule and
+                                 rank all R_r images (i2t) and all T_r texts (t2i). Every step needs siglip_set_label_sets
+                                 since the previous step (else SIGLIP_ERR_STATE before any launch); the text sets travel
+                                 to the other ranks with the text. Unavailable with SIGLIP_OPT_SAMPLE_IDS,
+                                 SIGLIP_OPT_EXTRA_TEXT_IDS, SIGLIP_OPT_EXTRA_IMAGE_IDS, SIGLIP_OPT_DISTILL and in the
+                                 host-buffer entries (SIGLIP_ERR_STATE). Collective. Default 0 */
   SIGLIP_OPT_AUX_TRACE = 18 /* 1: record globaltimer stamps of the auxiliary warps of CTA 0 for every launch (start,
                                last peer flag seen, jobs done, end of launch); read with siglip_ctx_aux_trace */
 };
@@ -277,6 +292,19 @@ int siglip_ctx_create_extras(siglip_ctx** out, int device, int rank, int world, 
  */
 int siglip_ctx_create_distill(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank, int D,
                               int D_teacher);
+
+/* Labels per set at most (siglip_ctx_create_labels) */
+#define SIGLIP_MAX_LABELS 4
+
+/*
+ * Same as siglip_ctx_create_extras, for label sets (SIGLIP_OPT_LABEL_SETS): every sample, extra text and extra image
+ * carries a set of M labels, 1 <= M <= SIGLIP_MAX_LABELS. The gathered text sets ([world][T_max, M] int64, followed by
+ * the text groups) are part of the exported text allocation, sized here because options are set after the handle
+ * exchange; every rank passes the same lists and M (handle import refuses a peer whose M differs). A context created
+ * any other way keeps its layout, and SIGLIP_OPT_LABEL_SETS returns SIGLIP_ERR_STATE there.
+ */
+int siglip_ctx_create_labels(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank,
+                             const int* images_per_rank, const int* texts_per_rank, int D, int M);
 
 /*
  * SIGLIP_OPT_DISTILL: the teacher of the NEXT step. timg [B, D_teacher] and ttxt [B, D_teacher] are this rank's teacher
@@ -424,6 +452,17 @@ int siglip_set_sample_weights(siglip_ctx* ctx, const float* image_w, const float
  * returns SIGLIP_ERR_STATE.
  */
 int siglip_set_groups(siglip_ctx* ctx, const int64_t* image_groups, const int64_t* text_groups, void* cuda_stream);
+
+/*
+ * SIGLIP_OPT_LABEL_SETS: the label sets of this rank for the NEXT siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd
+ * call, int64 device buffers, M labels per row: sample_labels [B, M] (image i and paired text i), extra_text_labels
+ * [T - B, M] or NULL (empty sets: pure hard negatives) and extra_image_labels [R - B, M] or NULL (empty sets).
+ * Stream-ordered copies into the context: nothing is read on the host, and a single-rank step with label sets can be
+ * captured into a CUDA graph, the copies with it. In the mode a step without this call since the previous step returns
+ * SIGLIP_ERR_STATE before launching anything; outside it this call returns SIGLIP_ERR_STATE.
+ */
+int siglip_set_label_sets(siglip_ctx* ctx, const int64_t* sample_labels, const int64_t* extra_text_labels,
+                          const int64_t* extra_image_labels, void* cuda_stream);
 
 /*
  * In-batch retrieval metrics of the NEXT siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd call (that step only),
@@ -585,6 +624,9 @@ int siglip_debug_set_chunk_ids(siglip_ctx* ctx, int chunk, const int64_t* ids_de
 /* The groups twin (SIGLIP_OPT_EXCLUDE_GROUPS): the text groups of chunk `chunk` ([T of that rank] int64 device buffer)
  * as the "peer" would have published them. */
 int siglip_debug_set_chunk_groups(siglip_ctx* ctx, int chunk, const int64_t* groups_dev, void* cuda_stream);
+/* The label-set twin (SIGLIP_OPT_LABEL_SETS): the text sets of chunk `chunk` ([T of that rank, M] int64 device buffer:
+ * its paired texts' sets, then its extras') as the "peer" would have published them. */
+int siglip_debug_set_chunk_label_sets(siglip_ctx* ctx, int chunk, const int64_t* sets_dev, void* cuda_stream);
 /* The weights twin (SIGLIP_OPT_SAMPLE_WEIGHTS): the text weights of chunk `chunk` ([T of that rank] fp32 device buffer,
  * or NULL = ones), clamped like siglip_set_sample_weights, as the "peer" would have published them. */
 int siglip_debug_set_chunk_weights(siglip_ctx* ctx, int chunk, const float* text_w_dev, void* cuda_stream);
@@ -592,9 +634,9 @@ int siglip_debug_set_chunk_weights(siglip_ctx* ctx, int chunk, const float* text
  * SIGLIP_OPT_SYNC_SCALAR_GRADS can be checked against numbers the kernel did not produce itself. */
 int siglip_debug_set_mailbox(siglip_ctx* ctx, int peer, float dt_prime, float dbias);
 /* Loopback only: seed the column argmax partials of this rank's text chunk that stand in for peer rank `peer`'s
- * ([B] 64-bit keys, [T] under SIGLIP_OPT_EXTRA_TEXT_IDS: (order-preserving fp32 bits of s) << 32 |
- * (0xFFFFFFFF - global image index), 0 = no candidate), so
- * that the cross-rank combine of a metrics step sees candidates the kernel did not produce itself. */
+ * ([B] 64-bit keys, [T] under SIGLIP_OPT_EXTRA_TEXT_IDS or SIGLIP_OPT_LABEL_SETS: (order-preserving fp32 bits of
+ * s) << 32 | (0xFFFFFFFF - global image index), 0 = no candidate), so that the cross-rank combine of a metrics step
+ * sees candidates the kernel did not produce itself. */
 int siglip_debug_set_peer_metric_keys(siglip_ctx* ctx, int peer, const uint64_t* keys_dev, void* cuda_stream);
 /* Loopback only: seed the top-K column lists of this rank's text chunk that stand in for peer rank `peer`'s
  * ([T, SIGLIP_TOPK_MAX] 64-bit keys as in siglip_debug_set_peer_metric_keys, each row sorted best first and 0-padded),
@@ -613,6 +655,9 @@ int siglip_debug_set_peer_sample_loss_poison(siglip_ctx* ctx, int peer, const in
  * in a metrics step ([R_peer - B_peer] int64 device buffer), so that a t2i winner among its extra images is judged by
  * ids the test chose. */
 int siglip_debug_set_peer_extra_image_ids(siglip_ctx* ctx, int peer, const int64_t* ids_dev, void* cuda_stream);
+/* The label-set twin: the sets of rank `peer`'s extra images ([E_peer, M] int64 device buffer) as that peer would have
+ * published them for a metrics or top-K step (SIGLIP_OPT_LABEL_SETS). */
+int siglip_debug_set_peer_extra_image_label_sets(siglip_ctx* ctx, int peer, const int64_t* sets_dev, void* cuda_stream);
 /* With SIGLIP_OPT_AUX_TRACE: device-synchronise and copy out 16 globaltimer stamps (ns) per launch since the last call:
  * [0..2] auxiliary warps of CTA 0: start, last peer flag observed (0 = no wait), jobs done; [3] launch end as seen by
  * the last CTA; [4] kernel entry (CTA 0); [5] set-up done (barriers); [6] MMAs of the first tile done (CTA 0);

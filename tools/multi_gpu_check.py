@@ -73,6 +73,9 @@ def main() -> int:
     ap.add_argument("--exclude-groups", action="store_true",
                     help="also check excluded same-group pairs (exclude_groups=True) against the float64 oracle, with "
                          "and without ids and with hard negatives, on both schedules")
+    ap.add_argument("--label-sets", action="store_true",
+                    help="also check multi-label positives (multi_label=M) against the float64 oracle, with extra texts "
+                         "and extra images carrying label sets")
     ap.add_argument("--row-panels", action="store_true",
                     help="also check the fused step in row panels (sigma_budget_bytes forcing several panels) against "
                          "the float64 closed form and against the unbounded step on the same peers: uneven batches "
@@ -706,6 +709,83 @@ def main() -> int:
                     l2.backward()
                     torch.cuda.synchronize()
                     report(f"exclude groups {fused} B={Bs} K={K} ids={with_ids} D={D} rep{rep}", dict(
+                        loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
+                        dimg=rel_f(a.grad.float().cpu(), torch.from_numpy(mine["dimg"])),
+                        dtxt=rel_f(b.grad.float().cpu(), dtxt_ref),
+                        dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
+                        db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
+
+    # ---- label sets: each rank's text sets travel with its ids slot through the peer pulls -------------------------
+    if args.label_sets:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from exclude_groups_oracle import clustered
+        from label_sets_oracle import closed_form_sets, dense_labels, topk_retrieval_sets
+        Bs = [160 + 24 * r for r in range(world)]
+        D, tp, bias = 136, math.log(10.0), -5.0
+        rng = np.random.default_rng(6666)
+        for M, K, E in ((1, 0, 0), (4, 29, 0), (2, 0, 17)):
+            Ts, Rs = [b + K for b in Bs], [b + E for b in Bs]
+            ss = [rng.integers(0, 12, (b, M)) for b in Bs]
+            for s_ in ss:
+                s_[rng.random(s_.shape) < 0.3] = -1
+            tsets = [np.concatenate([s_, rng.integers(-1, 12, (K, M))]) for s_ in ss]
+            isets = [np.concatenate([s_, rng.integers(-1, 12, (E, M))]) for s_ in ss]
+            key = lambda x: np.where(x[:, 0] >= 0, x[:, 0], 99)  # noqa: E731
+            imgs = [torch.from_numpy(clustered(key(x), D, 13, 1, 10 + r)).to(torch.bfloat16) for r, x in enumerate(isets)]
+            texts = [torch.from_numpy(clustered(key(x), D, 13, 1, 50 + r)).to(torch.bfloat16) for r, x in enumerate(tsets)]
+            f = lambda xs: [x.double().numpy() for x in xs]  # noqa: E731
+            ref = closed_form_sets(f(imgs), f(texts), tp, bias, isets, tsets, Bs)
+            mine = ref[rank]
+            dtxt_ref = torch.from_numpy(sum(ref[r]["contrib"][rank] for r in range(world)))
+            img, txt = imgs[rank].to(dev), texts[rank].to(dev)
+            B = Bs[rank]
+            for fused in (None, False):
+                modx = DDPSigmoidLoss(B, fused_step=fused, batch_per_rank=Bs, multi_label=M, extra_texts=K,
+                                      extra_images=E).to(dev)
+                with torch.no_grad():
+                    modx.t_prime.fill_(tp)
+                    modx.bias.fill_(bias)
+                for rep in range(2):
+                    modx.zero_grad()
+                    a, b = (x.float().requires_grad_(True) for x in (img, txt))
+                    kw = dict(sample_labels=torch.from_numpy(isets[rank][:B]).to(dev))
+                    if K:
+                        kw.update(extra_text=b[B:], extra_text_labels=torch.from_numpy(tsets[rank][B:]).to(dev))
+                    if E:
+                        kw.update(extra_image=a[B:], extra_image_labels=torch.from_numpy(isets[rank][B:]).to(dev))
+                    kq = 3
+                    if rep == 0:   # retrieval over the real peers: published text and extra-image sets
+                        l2, met = modx(a[:B], b[:B], return_metrics=True, metrics_topk=kq, **kw)
+                    else:
+                        l2 = modx(a[:B], b[:B], **kw)
+                    l2.backward()
+                    torch.cuda.synchronize()
+                    if rep == 0:
+                        exp = topk_retrieval_sets(f(imgs), f(texts), Bs, kq, isets, tsets)[rank]
+                        Y = dense_labels(isets, tsets, Bs) > 0
+                        o, to = exp["off"][rank], exp["toff"][rank]
+                        got_i = met["i2t_topk"].cpu().numpy()
+                        got_t = met["t2i_topk"].cpu().numpy()
+
+                        def clear(v):
+                            top = np.sort(v)[::-1][:kq + 1]
+                            return float(np.min(top[:-1] - top[1:])) > 1e-4
+
+                        ci = np.array([clear(exp["S"][o + i]) for i in range(len(got_i))])
+                        ct = np.array([clear(exp["S"][:, to + j]) for j in range(len(got_t))])
+                        fi = np.array([next((q for q, j in enumerate(row) if Y[o + i, j]), kq)
+                                       for i, row in enumerate(got_i)])
+                        ft = np.array([next((q for q, g in enumerate(row) if Y[g, to + j]), kq)
+                                       for j, row in enumerate(got_t)])
+                        rec = np.concatenate([met["i2t_recall"].cpu().numpy(), met["t2i_recall"].cpu().numpy()])
+                        want = [np.float32(np.count_nonzero(x < q)) / np.float32(len(x)) for x in (fi, ft)
+                                for q in range(1, kq + 1)]
+                        report(f"label sets retrieval B={Bs} M={M} K={K} E={E}", dict(
+                            i2t_lists=float((got_i[ci] != exp["i2t_topk"][ci]).any(axis=1).mean()),
+                            t2i_lists=float((got_t[ct] != exp["t2i_topk"][ct]).any(axis=1).mean()),
+                            unclear=float(max(0.8 - ci.mean(), 0.8 - ct.mean(), 0.0)),
+                            recall=float(np.abs(rec - np.array(want, np.float32)).max())), tol=0.0)
+                    report(f"label sets {fused} B={Bs} M={M} K={K} E={E} D={D} rep{rep}", dict(
                         loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
                         dimg=rel_f(a.grad.float().cpu(), torch.from_numpy(mine["dimg"])),
                         dtxt=rel_f(b.grad.float().cpu(), dtxt_ref),
