@@ -49,6 +49,7 @@ EXPORTED_SYMBOLS = (
     "siglip_set_groups",
     "siglip_ctx_create_labels",
     "siglip_set_label_sets",
+    "siglip_set_focal",
     "siglip_request_metrics",
     "siglip_request_sample_losses",
     "siglip_request_topk",
@@ -119,6 +120,7 @@ SIGLIP_OPT_DISTILL = 25
 SIGLIP_OPT_SIGMA_BUDGET_MIB = 26
 SIGLIP_OPT_EXCLUDE_GROUPS = 27
 SIGLIP_OPT_LABEL_SETS = 28
+SIGLIP_OPT_FOCAL = 29
 SIGLIP_MAX_LABELS = 4
 
 _lib: Optional[ctypes.CDLL] = None
@@ -261,6 +263,8 @@ def lib() -> ctypes.CDLL:
     L.siglip_ctx_create_labels.restype = ci
     L.siglip_set_label_sets.argtypes = [vp, vp, vp, vp, vp]
     L.siglip_set_label_sets.restype = ci
+    L.siglip_set_focal.argtypes = [vp, ctypes.c_float, ctypes.c_float]
+    L.siglip_set_focal.restype = ci
     L.siglip_debug_set_chunk_label_sets.argtypes = [vp, ci, vp, vp]
     L.siglip_debug_set_chunk_label_sets.restype = ci
     L.siglip_debug_set_peer_extra_image_label_sets.argtypes = [vp, ci, vp, vp]

@@ -227,6 +227,11 @@ struct siglip_ctx {
   int label_sets = 0;                    // SIGLIP_OPT_LABEL_SETS (collective)
   bool sets_set = false;                 // siglip_set_label_sets was called since the previous step
   int64_t* lrows = nullptr;              // [R][LM] the sets of my images: the paired ones, then the extras. Never exported
+  // focal pair loss (SIGLIP_OPT_FOCAL): gamma and alpha are kernel parameters, kept until siglip_set_focal changes them
+  int focal = 0;                         // SIGLIP_OPT_FOCAL (collective)
+  bool focal_set = false;                // siglip_set_focal has been called
+  float focal_gamma = 0.0f;
+  float focal_alpha = -1.0f;             // < 0: no alpha
   // distillation (siglip_ctx_create_distill, SIGLIP_OPT_DISTILL)
   int DT = 0;                            // teacher width D_teacher (0: a context without a teacher)
   int distill = 0;                       // SIGLIP_OPT_DISTILL (collective)
@@ -457,6 +462,8 @@ int take_ids(siglip_ctx* c) {
   if (c->label_sets && !c->sets_set)
     return fail(SIGLIP_ERR_STATE,
                 "SIGLIP_OPT_LABEL_SETS is on but siglip_set_label_sets was not called since the previous step");
+  if (c->focal && !c->focal_set)
+    return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_FOCAL is on but siglip_set_focal was never called");
   c->sets_set = false;
   c->groups_set = false;
   c->teacher_set = false;
@@ -1013,6 +1020,11 @@ int run_loss_chunk(siglip_ctx* c, int gi, int cidx, bool own, bool first, const 
     p.row_lab = c->lrows + static_cast<size_t>(r0) * c->LM;
     p.col_lab = chunk_sets(c, cidx) + static_cast<size_t>(c0) * c->LM;
     p.lab_m = c->LM;
+  }
+  if (c->focal) {   // the kModeFocal kernel: focal terms, every other option at run time
+    p.focal = 1;
+    p.focal_gamma = c->focal_gamma;
+    p.focal_alpha = c->focal_alpha;
   }
   if (c->mkeys_step != nullptr) {   // a metrics step: the kMetrics instantiation reduces the argmax keys
     p.row_keys = c->mkeys_step + mkeys_rows(c) + r0;
@@ -2145,6 +2157,8 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is unavailable under SIGLIP_OPT_EXCLUDE_GROUPS");
       if (value && c->label_sets)
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is unavailable under SIGLIP_OPT_LABEL_SETS");
+      if (value && c->focal)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is unavailable under SIGLIP_OPT_FOCAL");
       c->distill = value ? 1 : 0;
       c->teacher_set = false;
       return 0;
@@ -2179,6 +2193,11 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_LABEL_SETS is unavailable under SIGLIP_OPT_DISTILL");
       c->label_sets = value ? 1 : 0;
       c->sets_set = false;
+      return 0;
+    case SIGLIP_OPT_FOCAL:
+      if (value && c->distill)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_FOCAL is unavailable under SIGLIP_OPT_DISTILL");
+      c->focal = value ? 1 : 0;
       return 0;
     case SIGLIP_OPT_SIGMA_BUDGET_MIB:
       if (value < 0) return fail(SIGLIP_ERR_INVALID, "the sigma budget must be >= 0 MiB (0: unbounded)");
@@ -2592,6 +2611,18 @@ int siglip_set_label_sets(siglip_ctx* c, const int64_t* sample_labels, const int
   return 0;
 }
 
+int siglip_set_focal(siglip_ctx* c, float gamma, float alpha) {
+  if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "ctx is null");
+  if (!c->focal) return fail(SIGLIP_ERR_STATE, "siglip_set_focal needs SIGLIP_OPT_FOCAL = 1");
+  // |g| < 1.44 for gamma <= 8, so g * kGScale stays inside the fp16 sigma operand (DESIGN.md, "Focal pair loss")
+  if (!(gamma >= 0.0f && gamma <= 8.0f)) return fail(SIGLIP_ERR_INVALID, "focal gamma must be finite and in [0, 8]");
+  if (alpha != alpha || alpha > 1.0f) return fail(SIGLIP_ERR_INVALID, "focal alpha must be in [0, 1], or < 0 for none");
+  c->focal_gamma = gamma;
+  c->focal_alpha = alpha < 0.0f ? -1.0f : alpha;
+  c->focal_set = true;
+  return 0;
+}
+
 // one rank: the key blocks are allocated on the first request that reduces argmax keys (siglip_request_metrics, or
 // siglip_request_topk with K = 1), so a context that never asks holds exactly the workspace it held without them.
 // (world > 1: they are part of the exported text allocation.) The allocation is not a stream operation; the relaxed
@@ -2868,6 +2899,8 @@ int siglip_host_submit_grads(siglip_ctx* c, const void* img_host, const void* tx
   if (c->label_sets)
     return fail(SIGLIP_ERR_STATE,
                 "the host-buffer entries take no label sets: unavailable under SIGLIP_OPT_LABEL_SETS");
+  if (c->focal)
+    return fail(SIGLIP_ERR_STATE, "the host-buffer entries compute the SigLIP loss: unavailable under SIGLIP_OPT_FOCAL");
   const bool with_grads = dimg_host_bf16 != nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   CK(cudaSetDevice(c->device));

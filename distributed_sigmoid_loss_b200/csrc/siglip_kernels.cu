@@ -417,6 +417,93 @@ __device__ __forceinline__ void loss_slab(const float* v, float t, float b, int 
 }
 
 // -------------------------------------------------------------------------------------------------
+// Focal pair loss (kModeFocal). With m = z for a negative and m = -z for a positive (the logit of the wrong answer):
+//   term = a_t sigma(m)^gamma softplus(m),   dterm/dm = a_t sigma(m)^gamma (gamma sigma(-m) softplus(m) + sigma(m)),
+//   g = dterm/dz = dterm/dm for a negative, -dterm/dm for a positive,
+// with sigma(m)^gamma = exp(-gamma softplus(-m)) from the softplus the term computes anyway: one more ex2 per element.
+// The general path forms neither sigma(m) nor 1 - sigma(m) by a subtraction; the series path's 1 - sigma(z), with
+// sigma(z) < 2^-6, does not cancel. gamma = 0 gives the SigLIP terms. Every element
+// takes its weight (1 without weights) and adds its term to lrow / lcol, as loss_slab with kW and kL.
+// -------------------------------------------------------------------------------------------------
+// Series path: every element of the slab is a negative with z < kFastZ (the vote of loss_slab_fast), so e = exp(z) <
+// 2^-6, sigma(z) and softplus(z) = log1p(e) take the series of loss_slab_fast, and sigma(z)^gamma = exp(gamma (z -
+// log1p(e))) reuses the exponent of e: one more ex2 than loss_slab_fast.
+__device__ __forceinline__ void focal_slab_fast(const float* v, float tl, float bl, float gamma, float a_neg, int col0,
+                                                bool store_g, const GStore& gst, float gscale, float& acc_sp,
+                                                float& acc_g, float& acc_gs, const float* cw, float rw0, float rw1,
+                                                float* lrow, float* lcol) {
+  uint32_t packed[8];
+  float g_prev = 0.f;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const float s = v[i];
+    const float x = fmaf(s, tl, bl);                     // z log2(e)
+    const float e = ex2_approx(x);                       // exp(z), z < kFastZ
+    const float sig = e * fmaf(e, e - 1.0f, 1.0f);       // sigma(z) = e (1 - e + e^2)
+    const float l = e * fmaf(e, fmaf(e, 0.33333334f, -0.5f), 1.0f);   // softplus(z) = e (1 - e/2 + e^2/3)
+    const float pw = ex2_approx(gamma * fmaf(-l, kLog2e, x));         // sigma(z)^gamma
+    const float aw = a_neg * slab_w(i, cw, rw0, rw1) * pw;
+    const float term = aw * l;
+    const float g = aw * fmaf(gamma * (1.0f - sig), l, sig);
+    acc_sp += term;
+    lrow[(i >> 1) & 1] += term;
+    lcol[2 * (i >> 2) + (i & 1)] += term;
+    acc_g += g;
+    acc_gs = fmaf(g, s, acc_gs);
+    if (i & 1)
+      packed[2 * (i >> 2) + ((i >> 1) & 1)] = pack_16x2<true>(g_prev, g * gscale);
+    else
+      g_prev = g * gscale;
+  }
+  if (store_g) store_g_slab(gst, col0, packed);
+}
+
+// General path: any z, the labels, masks and exclusions of loss_slab<true, true, true, true> (pos, excl, the own
+// diagonal into g_diag, rows / columns past the problem masked to 0).
+__device__ __forceinline__ void focal_slab(const float* v, float t, float b, float gamma, float a_pos, float a_neg,
+                                           int row_lo, int col0, int c_lo, int nrows, int ncols, bool store_g,
+                                           const GStore& gst, float gscale, float* g_diag, bool on_diag, uint32_t pos,
+                                           uint32_t excl, float& acc_sp, float& acc_g, float& acc_gs, const float* cw,
+                                           float rw0, float rw1, float* lrow, float* lcol) {
+  uint32_t packed[8];
+  float g_prev = 0.f;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const int row = row_lo + 8 * ((i >> 1) & 1);
+    const int col = col0 + 8 * (i >> 2) + c_lo + (i & 1);
+    const float s = v[i];
+    const float z = fmaf(s, t, b);
+    const float e = ex2_approx(-fabsf(z) * kLog2e);    // exp(-|z|) in (0, 1]
+    const float l = e * log1p_over_e(e);               // log1p(exp(-|z|))
+    const float r = rcp_approx(1.0f + e);              // sigma(|z|)
+    const bool dg = on_diag && row == col;             // the own diagonal: its term goes to g_diag
+    const bool y = dg || ((pos >> i) & 1u);
+    const float m = y ? -z : z;
+    const float pm = (m >= 0.f) ? r : e * r;           // sigma(m)
+    const float qm = (m >= 0.f) ? e * r : r;           // sigma(-m) = 1 - sigma(m)
+    const float spm = fmaxf(m, 0.f) + l;               // softplus(m)
+    const float pw = ex2_approx(-gamma * kLog2e * (fmaxf(-m, 0.f) + l));   // sigma(m)^gamma = exp(-gamma softplus(-m))
+    const bool valid = (row < nrows) && (col < ncols) && (y || !((excl >> i) & 1u));   // a positive is never excluded
+    const float aw = valid ? (y ? a_pos : a_neg) * slab_w(i, cw, rw0, rw1) * pw : 0.f;
+    const float sp = valid ? aw * spm : 0.f;
+    const float gm = valid ? aw * fmaf(gamma * qm, spm, pm) : 0.f;
+    const float g = y ? -gm : gm;
+    if (dg && store_g && valid) g_diag[row] = g;
+    const float g_store = dg ? 0.f : g;                // the own diagonal stays out of the 16-bit operand
+    acc_sp += sp;
+    lrow[(i >> 1) & 1] += sp;
+    lcol[2 * (i >> 2) + (i & 1)] += sp;
+    acc_g += g;
+    acc_gs = fmaf(g, s, acc_gs);
+    if (i & 1)
+      packed[2 * (i >> 2) + ((i >> 1) & 1)] = pack_16x2<true>(g_prev, g_store * gscale);
+    else
+      g_prev = g_store * gscale;
+  }
+  if (store_g) store_g_slab(gst, col0, packed);
+}
+
+// -------------------------------------------------------------------------------------------------
 // Distillation (kModeDistill). Per element, with p the teacher's probability of the pair and y its hard label:
 //   q = (1 - lambda) y + lambda p,   term = softplus(z) - q z,   g = sigma(z) - q      (times the pair's weight)
 // sigma and softplus take the series of loss_slab_fast in a 16x32 slab whose z are all < kFastZ (warp vote, as in the
@@ -1004,7 +1091,9 @@ __device__ __forceinline__ void sample_loss_add(unsigned long long* w, long long
 // positives of the own chunk (own_pos_ids); the 64 pos bits are the only state the slab loop carries. There they form
 // pos before the warp vote: a slab with a positive takes the masked path, every other slab keeps its path. Groups
 // (tested after these positives), top-K lists and the per-sample sums are runtime options.
-template <bool kTopK = false, bool kGroups = false, bool kLabels = false>
+// kFocal (kModeFocal): the focal terms (focal_slab_fast / focal_slab) in place of the SigLIP ones, on the same slab
+// geometry and path votes; label sets (as kLabels), ids, groups, top-K lists and the per-sample sums are runtime options.
+template <bool kTopK = false, bool kGroups = false, bool kLabels = false, bool kFocal = false>
 __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, const float (&acc)[kTileN / 2],
                                                      const CUtensorMap* tmG, uint32_t staging_base, int warp, int wg,
                                                      int lane, int row0, int col_base, int row_lo, int c_lo,
@@ -1014,12 +1103,18 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
   if (p.row_keys != nullptr) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
   if constexpr (kTopK) {
     tile_topk(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
-  } else if constexpr (kGroups || kLabels) {
+  } else if constexpr (kGroups || kLabels || kFocal) {
     if (p.tk_rows != nullptr) tile_topk(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
   }
-  const bool sl = (!kTopK && !kGroups && !kLabels) || p.sl_rows != nullptr;
-  // excluded groups: always in kModeGroups, a runtime option in kModeLabels
-  const bool grp = kGroups || (kLabels && p.col_grp != nullptr);
+  const bool sl = (!kTopK && !kGroups && !kLabels && !kFocal) || p.sl_rows != nullptr;
+  // excluded groups: always in kModeGroups, a runtime option in kModeLabels and kModeFocal
+  const bool grp = kGroups || ((kLabels || kFocal) && p.col_grp != nullptr);
+  // label-set positives: always in kModeLabels, a runtime option in kModeFocal
+  const bool lab = kLabels || (kFocal && p.col_lab != nullptr);
+  // focal: gamma and the weights a_t of the positives and the negatives (both 1 without alpha)
+  const float gamma = kFocal ? p.focal_gamma : 0.f;
+  const bool alpha = kFocal && p.focal_alpha >= 0.f;
+  const float a_pos = alpha ? p.focal_alpha : 1.f, a_neg = alpha ? 1.f - p.focal_alpha : 1.f;
   float acc_sp = 0.f, acc_g = 0.f, acc_gs = 0.f;
   const bool edge = (row0 + kBlockM > pr.M) || (col_base + kTileN > pr.N);
   const bool diag = p.own_chunk && (row0 == col_base);
@@ -1033,7 +1128,7 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
   const bool ids = p.row_ids != nullptr, w = p.row_w != nullptr;
   int64_t rid0 = 0, rid1 = 0;
   uint32_t rpos = 0u;
-  if (!kLabels && ids) {   // kLabels: the id positives are part of lpos below
+  if (!lab && ids) {   // label sets: the id positives are part of lpos below
     rid0 = p.row_ids[min(row_lo, pr.M - 1)];
     rid1 = p.row_ids[min(row_lo + 8, pr.M - 1)];
     rpos = (row_lo < p.row_pos_n ? 0x3333u : 0u) | (row_lo + 8 < p.row_pos_n ? 0xCCCCu : 0u);
@@ -1045,7 +1140,7 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
   }
   int64_t rg0 = -1, rg1 = -1;
   uint32_t rgrp = 0u;   // excl bits of the rows that have a group (>= 0, within grp_rows)
-  if ((kGroups || kLabels) && grp) {
+  if ((kGroups || kLabels || kFocal) && grp) {
     rg0 = p.row_grp[min(row_lo, p.grp_rows - 1)];
     rg1 = p.row_grp[min(row_lo + 8, p.grp_rows - 1)];
     rgrp = (row_lo < p.grp_rows && rg0 >= 0 ? 0x3333u : 0u) | (row_lo + 8 < p.grp_rows && rg1 >= 0 ? 0xCCCCu : 0u);
@@ -1055,7 +1150,7 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
   // M read row M - 1 and columns past N column N - 1: they only lie in edge slabs, which mask them. An empty slot (< 0)
   // and a row slot past lab_m never match, since only column labels >= 0 are compared.
   uint64_t lpos = 0ull;
-  if constexpr (kLabels) {
+  if ((kLabels || kFocal) && lab) {
     // one fragment row at a time (rows 0 and 8 of the thread's pair) and one slab at a time, not unrolled: one set and
     // one slab's columns are in registers at a time
 #pragma unroll 1
@@ -1107,7 +1202,7 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
     const bool slab_edge = edge && ((gst.row0 + 16 > pr.M) || (col0 + 32 > pr.N));
     uint32_t pos = 0;
     bool slab_pos = false;
-    if (!kLabels && ids) {
+    if (!lab && ids) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
 #pragma unroll
@@ -1123,13 +1218,13 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
       pos &= rpos;
       slab_pos = __any_sync(0xffffffffu, pos != 0u);
     }
-    if constexpr (kLabels) {
+    if ((kLabels || kFocal) && lab) {
       pos |= static_cast<uint32_t>(lpos >> (16 * c)) & 0xFFFFu;
       slab_pos = __any_sync(0xffffffffu, pos != 0u);
     }
     uint32_t excl = 0u;
     bool slab_excl = false;
-    if ((kGroups || kLabels) && grp) {
+    if ((kGroups || kLabels || kFocal) && grp) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
 #pragma unroll
@@ -1144,7 +1239,22 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
       slab_excl = __any_sync(0xffffffffu, excl != 0u);
     }
     float lcol[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (!slab_edge && !slab_diag && !slab_pos && !slab_excl) {
+    if constexpr (kFocal) {
+      // the series path for the slabs the SigLIP kernels send down loss_slab_fast, the general path for all others
+      bool fast = false;
+      if (!slab_edge && !slab_diag && !slab_pos && !slab_excl) {
+        float smax = v[0];
+#pragma unroll
+        for (int j = 1; j < 16; ++j) smax = fmaxf(smax, v[j]);
+        fast = __all_sync(0xffffffffu, fmaf(smax, t_eff, bias) < kFastZ);
+      }
+      if (fast)
+        focal_slab_fast(v, tl, bl, gamma, a_neg, col0, sg, gst, p.g_scale, acc_sp, acc_g, acc_gs, cw, rw0, rw1, lrow,
+                        lcol);
+      else
+        focal_slab(v, t_eff, bias, gamma, a_pos, a_neg, row_lo, col0, c_lo, pr.M, pr.N, sg, gst, p.g_scale, p.g_diag,
+                   slab_diag, pos, excl, acc_sp, acc_g, acc_gs, cw, rw0, rw1, lrow, lcol);
+    } else if (!slab_edge && !slab_diag && !slab_pos && !slab_excl) {
       float smax = v[0];
 #pragma unroll
       for (int j = 1; j < 16; ++j) smax = fmaxf(smax, v[j]);
@@ -1217,6 +1327,9 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
 // kMode = kModeLabels: the loss kernel of a step with label sets, its own instantiation like kModeGroups: its epilogue
 // with the set intersections (sample_loss_epilogue<false, false, true>); ids, weights, metrics, the per-sample-loss
 // sums, the top-K lists and excluded groups are runtime options.
+// kMode = kModeFocal: the loss kernel of a focal step, its own instantiation like kModeLabels: its epilogue with the
+// focal terms (sample_loss_epilogue<false, false, false, true>); ids, label sets, weights, metrics, the per-sample-loss
+// sums, the top-K lists and excluded groups are runtime options.
 template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false,
           bool kWeights = false, int kTileNT = kTileN>
 __global__ void __launch_bounds__(kNumThreads, 1)
@@ -1240,6 +1353,8 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
                 "the excluded-groups kernel takes ids, weights, metrics, per-sample losses and top-K as runtime options");
   static_assert(kMode != kModeLabels || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
                 "the label-set kernel takes its other options at run time");
+  static_assert(kMode != kModeFocal || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
+                "the focal kernel takes its other options at run time");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -1488,7 +1603,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
                                                     b_adv, full0, empty0, lane, p.dbg, t, w_full_p)
         const int sel = pr.a_mn * 2 + pr.b_mn;
         if constexpr (kMode == kModeDistill || kMode == kModeSampleLoss || kMode == kModeTopK ||
-                      kMode == kModeGroups || kMode == kModeLabels) {
+                      kMode == kModeGroups || kMode == kModeLabels || kMode == kModeFocal) {
           // the loss operands (student and teacher) are always K-major: no MN-major variants in this instantiation
           if (pr.ab_f16)
             SIGLIP_MMA_LOOP(1, 0, 0);
@@ -1535,6 +1650,10 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
         sample_loss_epilogue<false, false, true>(p, acc, &tmG, staging_base, warp, wg, lane, row0, col_base, row_lo,
                                                  c_lo, pr, t_eff, bias, tl, bl, g_store_policy, s_sp, c_sp, s_g, c_g,
                                                  s_gs, c_gs);
+      } else if constexpr (kMode == kModeFocal) {
+        sample_loss_epilogue<false, false, false, true>(p, acc, &tmG, staging_base, warp, wg, lane, row0, col_base,
+                                                        row_lo, c_lo, pr, t_eff, bias, tl, bl, g_store_policy, s_sp,
+                                                        c_sp, s_g, c_g, s_gs, c_gs);
       } else if constexpr (kMode == kModeLoss) {
         // argmax keys first, on the raw accumulator: whichever path each slab then takes below
         if constexpr (kMetrics) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
@@ -2788,6 +2907,20 @@ int launch_gemm(int cta_group, int mode, int stages, int mcast, int tile_n, cons
       case 4: return launch_impl<kModeDistill, kDistillStages, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
       case 2: return launch_impl<kModeDistill, kDistillStages, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
       default: return launch_impl<kModeDistill, kDistillStages, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+    }
+  }
+  if (mode == kModeLoss && p.focal) {   // focal terms (with any option but distillation): kModeFocal
+    const bool s4 = stages == 4;
+    switch (cluster_size(cta_group, mcast)) {
+      case 4:
+        return s4 ? launch_impl<kModeFocal, 4, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeFocal, 6, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      case 2:
+        return s4 ? launch_impl<kModeFocal, 4, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeFocal, 6, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+      default:
+        return s4 ? launch_impl<kModeFocal, 4, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream)
+                  : launch_impl<kModeFocal, 6, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
     }
   }
   if (mode == kModeLoss && p.col_lab != nullptr) {   // label sets (with any option but distillation): kModeLabels

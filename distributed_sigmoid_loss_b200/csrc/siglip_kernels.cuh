@@ -188,6 +188,13 @@ struct KernelParams {
   const int64_t* row_lab;        // [M][lab_m]: the sets of this rank's images (rows of the launch)
   const int64_t* col_lab;        // [N][lab_m]: the sets of the texts of the chunk being scored
   int lab_m;                     // labels per set, 1 .. kMaxLabels
+  // Focal pair loss (SIGLIP_OPT_FOCAL, siglip_set_focal). Appended last like the fields above. focal != 0 selects the
+  // kModeFocal loss kernel: pair (i, j) with target y, p = sigma(z), p_t = y ? p : 1 - p and a_t = y ? alpha : 1 - alpha
+  // (1 without alpha) adds a_t (1 - p_t)^gamma softplus(-(2y - 1) z) and stores its derivative in z. Ids, label sets,
+  // weights, excluded groups, metric keys, per-sample sums and top-K lists stay runtime options there.
+  int focal;
+  float focal_gamma;             // in [0, 8]
+  float focal_alpha;             // in [0, 1]; < 0: no alpha (a_t = 1)
 };
 
 // kModeDistill: the loss kernel of a distillation step (KernelParams::k_teacher > 0), its own instantiation
@@ -199,6 +206,8 @@ struct KernelParams {
 // instantiation; ids, weights, metric keys, per-sample-loss sums and top-K lists are runtime options in it
 // kModeLabels: the loss kernel of a step with label sets (KernelParams::col_lab != null), its own instantiation; ids,
 // weights, metric keys, per-sample-loss sums, top-K lists and excluded groups are runtime options in it
+// kModeFocal: the loss kernel of a focal step (KernelParams::focal != 0), its own instantiation; ids, label sets,
+// weights, metric keys, per-sample-loss sums, top-K lists and excluded groups are runtime options in it
 enum KernelMode {
   kModeLoss = 0,
   kModeOut = 1,
@@ -206,7 +215,8 @@ enum KernelMode {
   kModeSampleLoss = 3,
   kModeTopK = 4,
   kModeGroups = 5,
-  kModeLabels = 6
+  kModeLabels = 6,
+  kModeFocal = 7
 };
 
 // Label sets: labels per set at most (SIGLIP_MAX_LABELS)

@@ -335,6 +335,11 @@ class SigmoidLossEngine:
                 extra_text_labels.data_ptr() if extra_text_labels is not None else None,
                 extra_image_labels.data_ptr() if extra_image_labels is not None else None, self._stream()))
 
+    def set_focal(self, gamma: float, alpha: Optional[float] = None) -> None:
+        """SIGLIP_OPT_FOCAL: gamma in [0, 8] and alpha in [0, 1] (None: no alpha) of the focal pair loss, for every later
+        step until the next call. Host-side only: nothing is launched."""
+        _capi.check(self._L.siglip_set_focal(self._h, float(gamma), -1.0 if alpha is None else float(alpha)))
+
     def debug_set_chunk_label_sets(self, chunk: int, sets: torch.Tensor) -> None:
         """Loopback: the text sets of chunk `chunk` ([T_c, M] int64) as its owner would have published them."""
         self._check_sets(sets, self.texts_per_rank[chunk])
@@ -908,8 +913,9 @@ class _EngineCache:
                  bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
                  extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
                  distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None,
-                 exclude_groups: bool = False, multi_label: int = 0):
+                 exclude_groups: bool = False, multi_label: int = 0, focal=None):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
+        self.focal = focal   # (gamma, alpha or None), or None
         self.exclude_groups = exclude_groups
         self.multi_label = multi_label
         self.sigma_budget_bytes = sigma_budget_bytes
@@ -959,6 +965,9 @@ class _EngineCache:
                 eng.set_option(_capi.SIGLIP_OPT_DISTILL, 1)
             if self.exclude_groups:
                 eng.set_option(_capi.SIGLIP_OPT_EXCLUDE_GROUPS, 1)
+            if self.focal is not None:
+                eng.set_option(_capi.SIGLIP_OPT_FOCAL, 1)
+                eng.set_focal(*self.focal)
             if self.sigma_budget_bytes:
                 eng.set_sigma_budget(self.sigma_budget_bytes)
             self._engines[key] = eng
@@ -1253,6 +1262,25 @@ def _with_negatives(text_embeddings: torch.Tensor, negative_text) -> torch.Tenso
     return text_embeddings if negative_text is None else torch.cat([text_embeddings, negative_text])
 
 
+def _validate_focal(focal_gamma, focal_alpha, distill):
+    """focal_gamma / focal_alpha of a module: None (off), or gamma a finite number in [0, 8] and alpha None or a number
+    in [0, 1]. |g| < 1.44 for gamma <= 8 keeps every pair derivative inside the fp16 sigma operand. Not with distill:
+    the distillation loss kernel has no focal terms. Returns (gamma, alpha) or None."""
+    def number(x):
+        return not isinstance(x, bool) and isinstance(x, (int, float))
+    if focal_gamma is None:
+        if focal_alpha is not None:
+            raise RuntimeError("focal_alpha given, but the loss was built without focal_gamma")
+        return None
+    if not number(focal_gamma) or not 0.0 <= float(focal_gamma) <= 8.0:   # NaN fails the comparison
+        raise RuntimeError(f"focal_gamma must be None or a number in [0, 8], got {focal_gamma!r}")
+    if focal_alpha is not None and (not number(focal_alpha) or not 0.0 <= float(focal_alpha) <= 1.0):
+        raise RuntimeError(f"focal_alpha must be None or a number in [0, 1], got {focal_alpha!r}")
+    if distill is not None:
+        raise RuntimeError("focal_gamma cannot be combined with distill: the distillation loss kernel has no focal terms")
+    return float(focal_gamma), (None if focal_alpha is None else float(focal_alpha))
+
+
 def _validate_distill(distill, hard_negatives: int, extra_texts: int, extra_images: int) -> Optional[float]:
     """distill=lambda of a module: None (off) or a float in (0, 1], the weight of the teacher's probabilities in the
     targets. The extras of hard_negatives / extra_texts / extra_images would need teacher embeddings of their own."""
@@ -1512,6 +1540,16 @@ class DDPSigmoidLoss(nn.Module):
     ``multi_positive`` with those ids. Retrieval metrics and top-K lists count a hit by the same rule and rank every
     image and text of the rank (extras included). Composes with every option but ``multi_positive`` and ``distill``;
     ``exclude_groups`` applies after these positives. Collective: the same M on every rank.
+
+    ``focal_gamma=gamma`` (0 <= gamma <= 8) and ``focal_alpha=alpha`` (None, or 0 <= alpha <= 1): torchvision's
+    ``sigmoid_focal_loss`` over every pair of the global batch. With p = σ(z), target y from whatever labels the other
+    options give, ``p_t = p`` if y = 1 else ``1 − p`` and ``a_t = alpha`` if y = 1 else ``1 − alpha`` (1 without
+    alpha), pair (i, j) adds ``w · a_t (1 − p_t)^gamma · softplus(−(2y − 1) z)``, and the loss still divides by B: easy
+    pairs, the bulk of the negatives, are down-weighted. gamma = 0 without alpha is the SigLIP loss. The terms are
+    computed in the loss kernel, without the ``[B, W·B]`` logits. Excluded pairs stay 0, per-sample losses report the
+    focal terms, retrieval metrics are unchanged. Derivatives below about 2⁻²⁸ lose precision in the fp16 operand of
+    dimg / dtxt (DESIGN.md, "Focal pair loss"). Composes with every option but ``distill``. Collective: the same values
+    on every rank.
     """
 
     def __init__(self, gpu_batch_size: int, group=None, cta_group: int = 2, overlap_pull: bool = True,
@@ -1519,7 +1557,8 @@ class DDPSigmoidLoss(nn.Module):
                  batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
                  extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
                  distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None,
-                 exclude_groups: bool = False, multi_label: Optional[int] = None) -> None:
+                 exclude_groups: bool = False, multi_label: Optional[int] = None,
+                 focal_gamma: Optional[float] = None, focal_alpha: Optional[float] = None) -> None:
         super().__init__()
         _sigma_budget_mib(sigma_budget_bytes)
         hard_negatives = _validate_hard_negatives(hard_negatives)
@@ -1530,6 +1569,7 @@ class DDPSigmoidLoss(nn.Module):
         sample_weights = _validate_sample_weights(sample_weights)
         distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images)
         exclude_groups = _validate_exclude_groups(exclude_groups, distill)
+        focal = _validate_focal(focal_gamma, focal_alpha, distill)
         self.t_prime = nn.Parameter(torch.tensor(math.log(10), dtype=torch.float64))
         self.bias = nn.Parameter(torch.tensor(-10.0))
         self.gpu_batch_size = gpu_batch_size
@@ -1559,11 +1599,13 @@ class DDPSigmoidLoss(nn.Module):
         self.exclude_groups = exclude_groups
         # extension: multi-label positives from per-sample label sets (0: off)
         self.multi_label = multi_label
+        # extension: the focal pair loss (torchvision's sigmoid_focal_loss), (gamma, alpha) or None
+        self.focal = focal
         self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank,
                                    multi_positive=multi_positive, hard_negatives=hard_negatives,
                                    extra_texts=extra_texts, sample_weights=sample_weights, extra_images=extra_images,
                                    distill=distill, sigma_budget_bytes=sigma_budget_bytes,
-                                   exclude_groups=exclude_groups, multi_label=multi_label)
+                                   exclude_groups=exclude_groups, multi_label=multi_label, focal=focal)
         # extension: bound of the 16-bit sigma operands; steps then run in row panels (memory O(budget), not O(B^2))
         self.sigma_budget_bytes = sigma_budget_bytes
 
@@ -1646,14 +1688,15 @@ class SigLipLoss(nn.Module):
     [B + K], and same-group pairs that are not positives are excluded from the loss, as in ``DDPSigmoidLoss``.
     ``multi_label=M``: every forward takes ``sample_labels`` [B, M] (and ``extra_text_labels`` / ``extra_image_labels``
     [K, M] with ``extra_texts`` / ``extra_images``), and pairs whose label sets meet are positives, as in
-    ``DDPSigmoidLoss``."""
+    ``DDPSigmoidLoss``. ``focal_gamma`` / ``focal_alpha``: the focal pair loss of ``DDPSigmoidLoss``."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
                  multi_positive: bool = False, hard_negatives: int = 0, extra_texts: int = 0,
                  sample_weights: bool = False, extra_images: int = 0, distill: Optional[float] = None,
                  sigma_budget_bytes: Optional[int] = None, exclude_groups: bool = False,
-                 multi_label: Optional[int] = None):
+                 multi_label: Optional[int] = None, focal_gamma: Optional[float] = None,
+                 focal_alpha: Optional[float] = None):
         super().__init__()
         _sigma_budget_mib(sigma_budget_bytes)
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
@@ -1664,6 +1707,8 @@ class SigLipLoss(nn.Module):
         sample_weights = _validate_sample_weights(sample_weights)
         distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images)
         exclude_groups = _validate_exclude_groups(exclude_groups, distill)
+        focal = _validate_focal(focal_gamma, focal_alpha, distill)
+        self.focal = focal
         self.distill = distill
         self.exclude_groups = exclude_groups
         self.multi_label = multi_label
@@ -1678,7 +1723,7 @@ class SigLipLoss(nn.Module):
         self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive,
                                    hard_negatives=hard_negatives, extra_texts=extra_texts, sample_weights=sample_weights,
                                    extra_images=extra_images, distill=distill, sigma_budget_bytes=sigma_budget_bytes,
-                                   exclude_groups=exclude_groups, multi_label=multi_label)
+                                   exclude_groups=exclude_groups, multi_label=multi_label, focal=focal)
         # bound of the 16-bit sigma operands; steps then run in row panels (as on DDPSigmoidLoss)
         self.sigma_budget_bytes = sigma_budget_bytes
 

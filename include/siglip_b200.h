@@ -193,6 +193,16 @@ enum {
                                  to the other ranks with the text. Unavailable with SIGLIP_OPT_SAMPLE_IDS,
                                  SIGLIP_OPT_EXTRA_TEXT_IDS, SIGLIP_OPT_EXTRA_IMAGE_IDS, SIGLIP_OPT_DISTILL and in the
                                  host-buffer entries (SIGLIP_ERR_STATE). Collective. Default 0 */
+  SIGLIP_OPT_FOCAL = 29, /* 1: the focal pair loss (torchvision's sigmoid_focal_loss) in place of the SigLIP term. Pair
+                            (i, j) with target y (from whatever labels the other options give), p = sigma(z),
+                            p_t = y ? p : 1 - p and a_t = y ? alpha : 1 - alpha (1 without alpha) adds
+                            w a_t (1 - p_t)^gamma softplus(-(2y - 1) z) to the loss (still divided by B_r), and the
+                            gradients, dt' and dbias follow. gamma = 0 without alpha is the SigLIP loss. Excluded pairs
+                            stay 0; metrics and top-K lists are unchanged; per-sample losses sum the focal terms. gamma
+                            and alpha come from siglip_set_focal: a step in the mode before that call returns
+                            SIGLIP_ERR_STATE before any launch. Unavailable with SIGLIP_OPT_DISTILL and in the
+                            host-buffer entries (SIGLIP_ERR_STATE). Collective: every rank sets the same option and
+                            values (not checked). Default 0 */
   SIGLIP_OPT_AUX_TRACE = 18 /* 1: record globaltimer stamps of the auxiliary warps of CTA 0 for every launch (start,
                                last peer flag seen, jobs done, end of launch); read with siglip_ctx_aux_trace */
 };
@@ -463,6 +473,15 @@ int siglip_set_groups(siglip_ctx* ctx, const int64_t* image_groups, const int64_
  */
 int siglip_set_label_sets(siglip_ctx* ctx, const int64_t* sample_labels, const int64_t* extra_text_labels,
                           const int64_t* extra_image_labels, void* cuda_stream);
+
+/*
+ * SIGLIP_OPT_FOCAL: gamma (finite, 0 <= gamma <= 8) and alpha (0 <= alpha <= 1, or < 0 for none) of the focal pair loss.
+ * Checks and records the two values on the host, launches nothing (a single-rank step stays capturable into a CUDA
+ * graph), and they hold for every later step until the next call. Every rank must set the same values: they are not
+ * compared across ranks. Returns SIGLIP_ERR_INVALID for values out of range (NaN included) and SIGLIP_ERR_STATE
+ * outside the mode.
+ */
+int siglip_set_focal(siglip_ctx* ctx, float gamma, float alpha);
 
 /*
  * In-batch retrieval metrics of the NEXT siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd call (that step only),

@@ -76,6 +76,9 @@ def main() -> int:
     ap.add_argument("--label-sets", action="store_true",
                     help="also check multi-label positives (multi_label=M) against the float64 oracle, with extra texts "
                          "and extra images carrying label sets")
+    ap.add_argument("--focal", action="store_true",
+                    help="also check the focal pair loss (focal_gamma / focal_alpha) against the float64 oracle, "
+                         "positional, with label sets and extras, and with weights and excluded groups")
     ap.add_argument("--row-panels", action="store_true",
                     help="also check the fused step in row panels (sigma_budget_bytes forcing several panels) against "
                          "the float64 closed form and against the unbounded step on the same peers: uneven batches "
@@ -791,6 +794,74 @@ def main() -> int:
                         dtxt=rel_f(b.grad.float().cpu(), dtxt_ref),
                         dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
                         db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
+
+    # ---- focal pair loss: gamma and alpha are kernel parameters; the exchange is the one of the options it rides ----
+    if args.focal:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from exclude_groups_oracle import clustered, group_labels
+        from focal_oracle import closed_form_focal
+        from label_sets_oracle import set_labels
+        Bs = [160 + 24 * r for r in range(world)]
+        D, tp, bias = 136, math.log(10.0), -5.0
+        rng = np.random.default_rng(7777)
+        for gamma, alpha, M, K, E, extra in ((2.0, 0.25, 0, 0, 0, False), (5.0, None, 2, 29, 17, False),
+                                             (0.5, 0.25, 0, 0, 0, True)):
+            Ts, Rs = [b + K for b in Bs], [b + E for b in Bs]
+            ss = [rng.integers(-1, 12, (b, max(M, 1))) for b in Bs]
+            tsets = [np.concatenate([s_, rng.integers(-1, 12, (K, max(M, 1)))]) for s_ in ss]
+            isets = [np.concatenate([s_, rng.integers(-1, 12, (E, max(M, 1)))]) for s_ in ss]
+            key = lambda x: np.where(x[:, 0] >= 0, x[:, 0], 99)  # noqa: E731
+            imgs = [torch.from_numpy(clustered(key(x), D, 13, 1, 20 + r)).to(torch.bfloat16) for r, x in enumerate(isets)]
+            texts = [torch.from_numpy(clustered(key(x), D, 13, 1, 60 + r)).to(torch.bfloat16) for r, x in enumerate(tsets)]
+            f = lambda xs: [x.double().numpy() for x in xs]  # noqa: E731
+            if M:
+                lab = set_labels(isets, tsets, Bs)
+            else:
+                lab = [[np.where((np.arange(Rs[r])[:, None] == np.arange(Ts[c])[None, :]) & (r == c), 1.0, -1.0)
+                        for c in range(world)] for r in range(world)]
+            iws = tws = igs = tgs = None
+            if extra:   # weights and excluded groups
+                iws = [rng.random(r_) for r_ in Rs]
+                tws = [rng.random(t_) for t_ in Ts]
+                igs = [rng.integers(-1, 6, r_) for r_ in Rs]
+                tgs = [rng.integers(-1, 6, t_) for t_ in Ts]
+                lab = group_labels(lab, igs, tgs)
+            ref = closed_form_focal(f(imgs), f(texts), tp, bias, lab, gamma, alpha, Bs, iws, tws)
+            mine = ref[rank]
+            dtxt_ref = torch.from_numpy(sum(ref[r]["contrib"][rank] for r in range(world)))
+            img, txt = imgs[rank].to(dev), texts[rank].to(dev)
+            B = Bs[rank]
+            for fused in (None, False):
+                modx = DDPSigmoidLoss(B, fused_step=fused, batch_per_rank=Bs, multi_label=M or None, extra_texts=K,
+                                      extra_images=E, sample_weights=extra, exclude_groups=extra, focal_gamma=gamma,
+                                      focal_alpha=alpha).to(dev)
+                with torch.no_grad():
+                    modx.t_prime.fill_(tp)
+                    modx.bias.fill_(bias)
+                for rep in range(2):
+                    modx.zero_grad()
+                    a, b = (x.float().requires_grad_(True) for x in (img, txt))
+                    kw = {}
+                    if M:
+                        kw["sample_labels"] = torch.from_numpy(isets[rank][:B]).to(dev)
+                    if K:
+                        kw.update(extra_text=b[B:], extra_text_labels=torch.from_numpy(tsets[rank][B:]).to(dev))
+                    if E:
+                        kw.update(extra_image=a[B:], extra_image_labels=torch.from_numpy(isets[rank][B:]).to(dev))
+                    if extra:
+                        kw.update(image_weights=torch.from_numpy(iws[rank]).float().to(dev),
+                                  text_weights=torch.from_numpy(tws[rank]).float().to(dev),
+                                  image_groups=torch.from_numpy(igs[rank]).to(dev),
+                                  text_groups=torch.from_numpy(tgs[rank]).to(dev))
+                    l2 = modx(a[:B] if E else a, b[:B] if K else b, **kw)
+                    l2.backward()
+                    torch.cuda.synchronize()
+                    report(f"focal {fused} gamma={gamma} alpha={alpha} B={Bs} M={M} K={K} E={E} w/g={extra} rep{rep}",
+                           dict(loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
+                                dimg=rel_f(a.grad.float().cpu(), torch.from_numpy(mine["dimg"])),
+                                dtxt=rel_f(b.grad.float().cpu(), dtxt_ref),
+                                dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
+                                db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
 
     # ---- distillation: each rank's teacher text travels with its text through the peer pulls ----------------------
     if args.distill:
