@@ -48,6 +48,7 @@ EXPORTED_SYMBOLS = (
     "siglip_set_sample_weights",
     "siglip_set_groups",
     "siglip_ctx_create_labels",
+    "siglip_ctx_create_distill_extras",
     "siglip_set_label_sets",
     "siglip_set_focal",
     "siglip_request_metrics",
@@ -261,6 +262,9 @@ def lib() -> ctypes.CDLL:
     L.siglip_ctx_create_labels.argtypes = [ctypes.POINTER(vp), ci, ci, ci, ctypes.POINTER(ci), ctypes.POINTER(ci),
                                            ctypes.POINTER(ci), ci, ci]
     L.siglip_ctx_create_labels.restype = ci
+    L.siglip_ctx_create_distill_extras.argtypes = [ctypes.POINTER(vp), ci, ci, ci, ctypes.POINTER(ci),
+                                                   ctypes.POINTER(ci), ctypes.POINTER(ci), ci, ci, ci]
+    L.siglip_ctx_create_distill_extras.restype = ci
     L.siglip_set_label_sets.argtypes = [vp, vp, vp, vp, vp]
     L.siglip_set_label_sets.restype = ci
     L.siglip_set_focal.argtypes = [vp, ctypes.c_float, ctypes.c_float]

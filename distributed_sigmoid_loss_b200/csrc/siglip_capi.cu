@@ -234,6 +234,9 @@ struct siglip_ctx {
   float focal_alpha = -1.0f;             // < 0: no alpha
   // distillation (siglip_ctx_create_distill, SIGLIP_OPT_DISTILL)
   int DT = 0;                            // teacher width D_teacher (0: a context without a teacher)
+  // siglip_ctx_create_distill_extras: distillation composes with per-sample losses, top-K, groups and label sets. A
+  // siglip_ctx_create_distill context keeps refusing them, as it always has
+  bool distill_opts = false;
   int distill = 0;                       // SIGLIP_OPT_DISTILL (collective)
   bool teacher_set = false;              // siglip_set_teacher was called since the previous step
   const void* t_img = nullptr;           // [B, DT] teacher images of the step (caller's buffer)
@@ -438,10 +441,12 @@ inline size_t ids_copy_bytes(const siglip_ctx* c, int rank) {
 // ids and weights of step s are given once: a step in ids / weights mode consumes them (all checked before anything is
 // launched or consumed)
 int take_ids(siglip_ctx* c) {
-  if (c->losses_armed && c->distill)
-    return fail(SIGLIP_ERR_STATE, "per-sample losses are unavailable under SIGLIP_OPT_DISTILL");
-  if (c->topk_armed && c->distill)
-    return fail(SIGLIP_ERR_STATE, "top-K retrieval is unavailable under SIGLIP_OPT_DISTILL");
+  if (c->losses_armed && c->distill && !c->distill_opts)
+    return fail(SIGLIP_ERR_STATE, "per-sample losses are unavailable under SIGLIP_OPT_DISTILL on a "
+                                  "siglip_ctx_create_distill context (siglip_ctx_create_distill_extras takes them)");
+  if (c->topk_armed && c->distill && !c->distill_opts)
+    return fail(SIGLIP_ERR_STATE, "top-K retrieval is unavailable under SIGLIP_OPT_DISTILL on a "
+                                  "siglip_ctx_create_distill context (siglip_ctx_create_distill_extras takes it)");
   if (c->sample_ids && !c->ids_set)
     return fail(SIGLIP_ERR_STATE,
                 "SIGLIP_OPT_SAMPLE_IDS is on but siglip_set_sample_ids was not called since the previous step");
@@ -526,10 +531,11 @@ inline const float* peer_weights(const siglip_ctx* c, int o) {
          static_cast<size_t>(o) * c->w_stride;
 }
 // ---- distillation (SIGLIP_OPT_DISTILL) ----
-// elements between consecutive teacher text chunks of ttxt_all
-inline size_t teacher_stride(const siglip_ctx* c) { return static_cast<size_t>(c->Bmax) * c->DT; }
+// elements between consecutive teacher text chunks of ttxt_all: a chunk holds all T texts of its rank, paired then
+// extras, as the student's does (without extra texts T = B, the layout it had before extras could have a teacher)
+inline size_t teacher_stride(const siglip_ctx* c) { return static_cast<size_t>(c->Tmax) * c->DT; }
 inline size_t teacher_chunk_bytes(const siglip_ctx* c, int rank) {
-  return static_cast<size_t>(c->Bs[rank]) * c->DT * sizeof(__nv_bfloat16);
+  return static_cast<size_t>(c->Ts[rank]) * c->DT * sizeof(__nv_bfloat16);
 }
 // byte offset of the gathered teacher text in the exported text allocation: behind the text weights
 inline size_t teacher_offset(const siglip_ctx* c) {
@@ -2112,20 +2118,37 @@ int siglip_ctx_create_extras(siglip_ctx** out, int device, int rank, int world, 
   return ctx_create_impl(out, device, rank, world, batch_per_rank, images_per_rank, texts_per_rank, D);
 }
 
+// The public creation entries with a teacher or label sets: the lists are checked, then ctx_create_impl
+static int ctx_create_checked(siglip_ctx** out, int device, int rank, int world, const int* Bs, const int* Rs,
+                              const int* Ts, int D, int DT, int M, bool distill_opts = false) {
+  if (Bs == nullptr || Rs == nullptr || Ts == nullptr)
+    return fail(SIGLIP_ERR_INVALID, "batch_per_rank / images_per_rank / texts_per_rank is null");
+  if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
+  if (M < 0 || M > SIGLIP_MAX_LABELS)
+    return fail(SIGLIP_ERR_INVALID, "need 1 <= M <= SIGLIP_MAX_LABELS labels per set (0: no label sets)");
+  const int rc = ctx_create_impl(out, device, rank, world, Bs, Rs, Ts, D, DT, M);
+  if (rc == 0) (*out)->distill_opts = distill_opts;
+  return rc;
+}
+
 int siglip_ctx_create_distill(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank, int D,
                               int D_teacher) {
   if (batch_per_rank == nullptr) return fail(SIGLIP_ERR_INVALID, "batch_per_rank is null");
-  if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
-  return ctx_create_impl(out, device, rank, world, batch_per_rank, batch_per_rank, batch_per_rank, D, D_teacher);
+  return ctx_create_checked(out, device, rank, world, batch_per_rank, batch_per_rank, batch_per_rank, D, D_teacher, 0);
 }
 
 int siglip_ctx_create_labels(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank,
                              const int* images_per_rank, const int* texts_per_rank, int D, int M) {
-  if (batch_per_rank == nullptr || images_per_rank == nullptr || texts_per_rank == nullptr)
-    return fail(SIGLIP_ERR_INVALID, "batch_per_rank / images_per_rank / texts_per_rank is null");
-  if (world < 1 || world > kMaxWorld) return fail(SIGLIP_ERR_INVALID, "rank/world out of range (world <= 32)");
   if (M < 1 || M > SIGLIP_MAX_LABELS) return fail(SIGLIP_ERR_INVALID, "need 1 <= M <= SIGLIP_MAX_LABELS labels per set");
-  return ctx_create_impl(out, device, rank, world, batch_per_rank, images_per_rank, texts_per_rank, D, 0, M);
+  return ctx_create_checked(out, device, rank, world, batch_per_rank, images_per_rank, texts_per_rank, D, 0, M);
+}
+
+int siglip_ctx_create_distill_extras(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank,
+                                     const int* images_per_rank, const int* texts_per_rank, int D, int D_teacher,
+                                     int M) {
+  if (D_teacher < 8) return fail(SIGLIP_ERR_INVALID, "need D_teacher a positive multiple of 8");
+  return ctx_create_checked(out, device, rank, world, batch_per_rank, images_per_rank, texts_per_rank, D, D_teacher, M,
+                            true);
 }
 
 int siglip_set_teacher(siglip_ctx* c, const void* timg, const void* ttxt, int teacher_f16, const float* t_prime_T,
@@ -2152,19 +2175,20 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
   switch (option) {
     case SIGLIP_OPT_DISTILL:
       if (value && c->DT == 0)
-        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL needs a context created with siglip_ctx_create_distill");
-      if (value && c->exclude_groups)
-        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is unavailable under SIGLIP_OPT_EXCLUDE_GROUPS");
-      if (value && c->label_sets)
-        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is unavailable under SIGLIP_OPT_LABEL_SETS");
+        return fail(SIGLIP_ERR_STATE,
+                    "SIGLIP_OPT_DISTILL needs a context created with siglip_ctx_create_distill(_extras)");
+      if (value && c->exclude_groups && !c->distill_opts)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is unavailable under SIGLIP_OPT_EXCLUDE_GROUPS on a "
+                                      "siglip_ctx_create_distill context (siglip_ctx_create_distill_extras takes both)");
       if (value && c->focal)
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_DISTILL is unavailable under SIGLIP_OPT_FOCAL");
       c->distill = value ? 1 : 0;
       c->teacher_set = false;
       return 0;
     case SIGLIP_OPT_EXCLUDE_GROUPS: {
-      if (value && c->distill)
-        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_EXCLUDE_GROUPS is unavailable under SIGLIP_OPT_DISTILL");
+      if (value && c->distill && !c->distill_opts)
+        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_EXCLUDE_GROUPS is unavailable under SIGLIP_OPT_DISTILL on a "
+                                      "siglip_ctx_create_distill context (siglip_ctx_create_distill_extras takes both)");
       if (value && !c->ids_grp) {
         // ids_in grows its group halves ([ids_stride] text groups, [R] image groups) on first use, so a context that
         // never turns the mode on holds the workspace it held without it. Its ids are kept (they may be set already).
@@ -2186,11 +2210,10 @@ int siglip_ctx_set_option(siglip_ctx* c, int option, int value) {
     }
     case SIGLIP_OPT_LABEL_SETS:
       if (value && c->LM == 0)
-        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_LABEL_SETS needs a context created with siglip_ctx_create_labels");
+        return fail(SIGLIP_ERR_STATE,
+                    "SIGLIP_OPT_LABEL_SETS needs a context created with siglip_ctx_create_labels or with M > 0");
       if (value && (c->sample_ids || c->extra_text_ids || c->extra_image_ids))
         return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_LABEL_SETS replaces sample ids: turn SIGLIP_OPT_SAMPLE_IDS off first");
-      if (value && c->distill)
-        return fail(SIGLIP_ERR_STATE, "SIGLIP_OPT_LABEL_SETS is unavailable under SIGLIP_OPT_DISTILL");
       c->label_sets = value ? 1 : 0;
       c->sets_set = false;
       return 0;
@@ -2657,8 +2680,9 @@ int siglip_request_metrics(siglip_ctx* c, float* top1, int64_t* i2t_index, int64
 int siglip_request_sample_losses(siglip_ctx* c, float* image_loss, float* text_loss) {
   if (c == nullptr || image_loss == nullptr || text_loss == nullptr)
     return fail(SIGLIP_ERR_INVALID, "null argument (image_loss and text_loss are required)");
-  if (c->distill)
-    return fail(SIGLIP_ERR_STATE, "per-sample losses are unavailable under SIGLIP_OPT_DISTILL");
+  if (c->distill && !c->distill_opts)
+    return fail(SIGLIP_ERR_STATE, "per-sample losses are unavailable under SIGLIP_OPT_DISTILL on a "
+                                  "siglip_ctx_create_distill context (siglip_ctx_create_distill_extras takes them)");
   if (c->lsum[0] == nullptr) {
     // one rank: the blocks are allocated on the first request, as the metric keys are (and apart from them), so a
     // context that never asks holds exactly the workspace it held without them; allowed inside a CUDA-graph capture
@@ -2683,7 +2707,9 @@ int siglip_request_sample_losses(siglip_ctx* c, float* image_loss, float* text_l
 int siglip_request_topk(siglip_ctx* c, int k, float* recall, int64_t* i2t_topk, int64_t* t2i_topk) {
   if (c == nullptr || recall == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument (recall is required)");
   if (k < 1 || k > SIGLIP_TOPK_MAX) return fail(SIGLIP_ERR_INVALID, "k must be in 1 .. SIGLIP_TOPK_MAX");
-  if (c->distill) return fail(SIGLIP_ERR_STATE, "top-K retrieval is unavailable under SIGLIP_OPT_DISTILL");
+  if (c->distill && !c->distill_opts)
+    return fail(SIGLIP_ERR_STATE, "top-K retrieval is unavailable under SIGLIP_OPT_DISTILL on a "
+                                  "siglip_ctx_create_distill context (siglip_ctx_create_distill_extras takes it)");
   int rc;
   if (k == 1 && (rc = ensure_metric_keys(c))) return rc;   // K = 1 runs the metrics path on the argmax keys
   if (k > 1 && c->tk_rows[0] == nullptr) {

@@ -43,6 +43,9 @@ constexpr int kStagingBytesPerWarp = 1024;  // one 16x32 16-bit slab, 64-byte ro
 constexpr int kWideTileN = kWideTileCols;
 constexpr int kWideStages = 4;
 
+// the loss-kernel modes that contract the teacher's operands (tmA1 / tmB1) before the student's
+__host__ __device__ constexpr bool teacher_mode(int mode) { return mode == kModeDistill || mode == kModeDistillOpts; }
+
 template <int kMode, int kStagesT, int kTileNT = kTileN>
 struct Cfg {
   static constexpr int kABytes = kBlockM * kBlockK * 2;            // 16 KiB
@@ -50,8 +53,8 @@ struct Cfg {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = kStagesT;
   static constexpr int kStagingBytes = (kMode != kModeOut) ? kNumEpiWarps * kStagingBytesPerWarp : 0;
-  // kModeDistill: the teacher's probabilities (fp32, one 128 x 128 tile) follow the barrier block
-  static constexpr int kPBytes = (kMode == kModeDistill) ? kBlockM * kTileNT * 4 : 0;
+  // kModeDistill, kModeDistillOpts: the teacher's probabilities (fp32, one 128 x 128 tile) follow the barrier block
+  static constexpr int kPBytes = teacher_mode(kMode) ? kBlockM * kTileNT * 4 : 0;
   static constexpr int kSmemBytes =
       kStages * kStageBytes + kStagingBytes + 1024 /*barriers, reduction*/ + kPBytes + 1024 /*alignment slack*/;
   static_assert(kSmemBytes <= 232448, "exceeds the 227 KB of shared memory a CTA may use");
@@ -546,14 +549,18 @@ __device__ __forceinline__ uint32_t distill_p_addr(uint32_t pbuf, int i) {
 }
 
 // One 16x32 slab of the distillation epilogue. kMask: rows / columns past the matrix are dropped and labels are applied
-// (the own-chunk diagonal, whose g goes to g_diag in fp32, and the pos bits of sample ids); without it y = 0.
-// w: per-sample weights (cw / rw0 / rw1 as in slab_w) when non-zero.
-template <bool kMask>
+// (the own-chunk diagonal, whose g goes to g_diag in fp32, and the pos bits of sample ids or label sets); without it
+// y = 0. w: per-sample weights (cw / rw0 / rw1 as in slab_w) when non-zero.
+// kL (kModeDistillOpts): element i's term, once weighted and masked, is also added to lrow / lcol as in loss_slab.
+// kX (kModeDistillOpts, with kMask): excl bit i set = element i is an excluded pair (same group, not a positive): it is
+// masked like a pair past the matrix, so its term, g and stored sigma are 0 whatever its teacher probability.
+template <bool kMask, bool kL = false, bool kX = false>
 __device__ __forceinline__ void distill_slab(const float* v, uint32_t pbuf, int c, float t, float b, float tl, float bl,
                                              float lambda, int row_lo, int col0, int c_lo, int nrows, int ncols,
                                              bool store_g, const GStore& gst, float gscale, float* g_diag, bool on_diag,
                                              uint32_t pos, bool w, const float* cw, float rw0, float rw1,
-                                             float& acc_sp, float& acc_g, float& acc_gs) {
+                                             float& acc_sp, float& acc_g, float& acc_gs, float* lrow = nullptr,
+                                             float* lcol = nullptr, uint32_t excl = 0u) {
   uint32_t packed[8];
   float g_prev = 0.f;
   const float one_minus = 1.0f - lambda;
@@ -574,6 +581,7 @@ __device__ __forceinline__ void distill_slab(const float* v, uint32_t pbuf, int 
       valid = (row < nrows) && (col < ncols);
       own_diag = on_diag && row == col;
       y = (own_diag || ((pos >> i) & 1u)) ? 1.0f : 0.f;
+      if constexpr (kX) valid = valid && (own_diag || !((excl >> i) & 1u));   // excl never holds a pos bit
     }
     const float q = fmaf(lambda, pt, one_minus * y);
     float sp = ((z >= 0.f) ? (1.0f - q) * z : -q * z) + l;   // softplus(z) - q z without cancelling at q = 1
@@ -594,6 +602,10 @@ __device__ __forceinline__ void distill_slab(const float* v, uint32_t pbuf, int 
       g_store = valid ? g_store : 0.f;
     }
     acc_sp += sp;
+    if constexpr (kL) {
+      lrow[(i >> 1) & 1] += sp;
+      lcol[2 * (i >> 2) + (i & 1)] += sp;
+    }
     acc_g += g;
     acc_gs = fmaf(g, s, acc_gs);
     if (i & 1)
@@ -1093,24 +1105,28 @@ __device__ __forceinline__ void sample_loss_add(unsigned long long* w, long long
 // (tested after these positives), top-K lists and the per-sample sums are runtime options.
 // kFocal (kModeFocal): the focal terms (focal_slab_fast / focal_slab) in place of the SigLIP ones, on the same slab
 // geometry and path votes; label sets (as kLabels), ids, groups, top-K lists and the per-sample sums are runtime options.
-template <bool kTopK = false, bool kGroups = false, bool kLabels = false, bool kFocal = false>
+// kDistill (kModeDistillOpts): the soft-target terms of distillation (distill_slab, the teacher's probabilities in pbuf)
+// on the slab geometry and path choice of distill_epilogue, as runtime options everything kFocal takes. Without groups,
+// label sets and the per-sample sums, the three sums, g_diag and the sigma operand are those of distill_epilogue bit
+// for bit: a slab takes distill_slab<false> or <true> exactly when distill_epilogue does.
+template <bool kTopK = false, bool kGroups = false, bool kLabels = false, bool kFocal = false, bool kDistill = false>
 __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, const float (&acc)[kTileN / 2],
                                                      const CUtensorMap* tmG, uint32_t staging_base, int warp, int wg,
                                                      int lane, int row0, int col_base, int row_lo, int c_lo,
                                                      const Problem& pr, float t_eff, float bias, float tl, float bl,
                                                      uint64_t policy, float& s_sp, float& c_sp, float& s_g, float& c_g,
-                                                     float& s_gs, float& c_gs) {
+                                                     float& s_gs, float& c_gs, uint32_t pbuf = 0u) {
   if (p.row_keys != nullptr) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
   if constexpr (kTopK) {
     tile_topk(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
-  } else if constexpr (kGroups || kLabels || kFocal) {
+  } else if constexpr (kGroups || kLabels || kFocal || kDistill) {
     if (p.tk_rows != nullptr) tile_topk(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
   }
-  const bool sl = (!kTopK && !kGroups && !kLabels && !kFocal) || p.sl_rows != nullptr;
-  // excluded groups: always in kModeGroups, a runtime option in kModeLabels and kModeFocal
-  const bool grp = kGroups || ((kLabels || kFocal) && p.col_grp != nullptr);
-  // label-set positives: always in kModeLabels, a runtime option in kModeFocal
-  const bool lab = kLabels || (kFocal && p.col_lab != nullptr);
+  const bool sl = (!kTopK && !kGroups && !kLabels && !kFocal && !kDistill) || p.sl_rows != nullptr;
+  // excluded groups: always in kModeGroups, a runtime option in kModeLabels, kModeFocal and kModeDistillOpts
+  const bool grp = kGroups || ((kLabels || kFocal || kDistill) && p.col_grp != nullptr);
+  // label-set positives: always in kModeLabels, a runtime option in kModeFocal and kModeDistillOpts
+  const bool lab = kLabels || ((kFocal || kDistill) && p.col_lab != nullptr);
   // focal: gamma and the weights a_t of the positives and the negatives (both 1 without alpha)
   const float gamma = kFocal ? p.focal_gamma : 0.f;
   const bool alpha = kFocal && p.focal_alpha >= 0.f;
@@ -1140,7 +1156,7 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
   }
   int64_t rg0 = -1, rg1 = -1;
   uint32_t rgrp = 0u;   // excl bits of the rows that have a group (>= 0, within grp_rows)
-  if ((kGroups || kLabels || kFocal) && grp) {
+  if ((kGroups || kLabels || kFocal || kDistill) && grp) {
     rg0 = p.row_grp[min(row_lo, p.grp_rows - 1)];
     rg1 = p.row_grp[min(row_lo + 8, p.grp_rows - 1)];
     rgrp = (row_lo < p.grp_rows && rg0 >= 0 ? 0x3333u : 0u) | (row_lo + 8 < p.grp_rows && rg1 >= 0 ? 0xCCCCu : 0u);
@@ -1150,7 +1166,7 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
   // M read row M - 1 and columns past N column N - 1: they only lie in edge slabs, which mask them. An empty slot (< 0)
   // and a row slot past lab_m never match, since only column labels >= 0 are compared.
   uint64_t lpos = 0ull;
-  if ((kLabels || kFocal) && lab) {
+  if ((kLabels || kFocal || kDistill) && lab) {
     // one fragment row at a time (rows 0 and 8 of the thread's pair) and one slab at a time, not unrolled: one set and
     // one slab's columns are in registers at a time
 #pragma unroll 1
@@ -1218,13 +1234,13 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
       pos &= rpos;
       slab_pos = __any_sync(0xffffffffu, pos != 0u);
     }
-    if ((kLabels || kFocal) && lab) {
+    if ((kLabels || kFocal || kDistill) && lab) {
       pos |= static_cast<uint32_t>(lpos >> (16 * c)) & 0xFFFFu;
       slab_pos = __any_sync(0xffffffffu, pos != 0u);
     }
     uint32_t excl = 0u;
     bool slab_excl = false;
-    if ((kGroups || kLabels || kFocal) && grp) {
+    if ((kGroups || kLabels || kFocal || kDistill) && grp) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
 #pragma unroll
@@ -1239,7 +1255,17 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
       slab_excl = __any_sync(0xffffffffu, excl != 0u);
     }
     float lcol[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if constexpr (kFocal) {
+    if constexpr (kDistill) {
+      // the series / exact choice is made per slab inside (distill_slab_series)
+      if (!slab_edge && !slab_diag && !slab_pos && !slab_excl)
+        distill_slab<false, true>(v, pbuf, c, t_eff, bias, tl, bl, p.distill_lambda, row_lo, col0, c_lo, pr.M, pr.N,
+                                  sg, gst, p.g_scale, p.g_diag, false, 0u, w, cw, rw0, rw1, acc_sp, acc_g, acc_gs, lrow,
+                                  lcol);
+      else
+        distill_slab<true, true, true>(v, pbuf, c, t_eff, bias, tl, bl, p.distill_lambda, row_lo, col0, c_lo, pr.M,
+                                       pr.N, sg, gst, p.g_scale, p.g_diag, slab_diag, pos, w, cw, rw0, rw1, acc_sp,
+                                       acc_g, acc_gs, lrow, lcol, excl);
+    } else if constexpr (kFocal) {
       // the series path for the slabs the SigLIP kernels send down loss_slab_fast, the general path for all others
       bool fast = false;
       if (!slab_edge && !slab_diag && !slab_pos && !slab_excl) {
@@ -1330,6 +1356,10 @@ __device__ __forceinline__ void sample_loss_epilogue(const KernelParams& p, cons
 // kMode = kModeFocal: the loss kernel of a focal step, its own instantiation like kModeLabels: its epilogue with the
 // focal terms (sample_loss_epilogue<false, false, false, true>); ids, label sets, weights, metrics, the per-sample-loss
 // sums, the top-K lists and excluded groups are runtime options.
+// kMode = kModeDistillOpts: the loss kernel of a distillation step with per-sample losses, top-K lists, excluded groups
+// or label sets, its own instantiation like kModeDistill: its teacher pass, then the kModeFocal epilogue with the
+// soft-target terms (sample_loss_epilogue<false, false, false, false, true>); every option kModeFocal takes is a
+// runtime option.
 template <int kMode, int kStagesT, int kCS, bool kF8 = false, bool kIds = false, bool kMetrics = false,
           bool kWeights = false, int kTileNT = kTileN>
 __global__ void __launch_bounds__(kNumThreads, 1)
@@ -1355,6 +1385,8 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
                 "the label-set kernel takes its other options at run time");
   static_assert(kMode != kModeFocal || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
                 "the focal kernel takes its other options at run time");
+  static_assert(kMode != kModeDistillOpts || (!kF8 && !kIds && !kMetrics && !kWeights && kTileNT == kTileN),
+                "the distillation kernel with options takes its other options at run time");
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned stage bases
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -1386,7 +1418,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       prefetch_tmap(&tmA1);
       prefetch_tmap(&tmB1);
     }
-    if constexpr (kMode == kModeDistill) {
+    if constexpr (teacher_mode(kMode)) {
       prefetch_tmap(&tmA1);
       prefetch_tmap(&tmB1);
     }
@@ -1441,7 +1473,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
       const int a_mn = pr.a_mn, b_mn = pr.b_mn;
       int kb0, kb1;
       item_k_range(p, tc, num_kb, kb0, kb1);
-      if constexpr (kMode == kModeDistill) {
+      if constexpr (teacher_mode(kMode)) {
         // the teacher's k-blocks of the tile first (both K-major, K = D_T), through the same ring
         constexpr int kRows = kTileN / kCS;
         const int num_kb_t = (p.k_teacher + kBlockK - 1) / kBlockK;
@@ -1526,7 +1558,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
     // distillation: the teacher's z^T = t_T s^T + b_T (its accumulator is 2^8 s^T for fp16 x 16 operands)
     float tT_eff = 0.f, bias_T = 0.f, tT_l = 0.f, bT_l = 0.f;
     uint32_t pbuf = 0;
-    if constexpr (kMode == kModeDistill) {
+    if constexpr (teacher_mode(kMode)) {
       tT_eff = expf(*p.t_prime_T) * (p.teacher_f16 ? 1.0f / 256.0f : 1.0f);
       bias_T = *p.bias_T;
       tT_l = tT_eff * kLog2e;
@@ -1577,7 +1609,7 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
         const uint32_t b_adv = pr.b_mn ? (kMmaK * 128u) >> 4 : 32u >> 4;
         const uint64_t adesc0 = make_smem_desc_sw128(smem_base + static_cast<uint32_t>(wg) * 8192u, a_lbo, 1024u);
         const uint64_t bdesc0 = make_smem_desc_sw128(smem_base + C::kABytes, b_lbo, 1024u);
-        if constexpr (kMode == kModeDistill) {
+        if constexpr (teacher_mode(kMode)) {
           // s^T of the tile over the teacher's k-blocks, then p = sigma(t_T s^T + b_T) into this thread's slots. The
           // student's k-loop below starts from zero (its first wgmma does not accumulate); the producer is already
           // streaming its operands while the conversion runs.
@@ -1602,8 +1634,8 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
   mma_loop<T, TA, TB, kCS, C::kStageBytes, kTileNT>(acc, kb0, kb1, stage, phase, C::kStages, adesc0, bdesc0, a_adv, \
                                                     b_adv, full0, empty0, lane, p.dbg, t, w_full_p)
         const int sel = pr.a_mn * 2 + pr.b_mn;
-        if constexpr (kMode == kModeDistill || kMode == kModeSampleLoss || kMode == kModeTopK ||
-                      kMode == kModeGroups || kMode == kModeLabels || kMode == kModeFocal) {
+        if constexpr (teacher_mode(kMode) || kMode == kModeSampleLoss || kMode == kModeTopK || kMode == kModeGroups ||
+                      kMode == kModeLabels || kMode == kModeFocal) {
           // the loss operands (student and teacher) are always K-major: no MN-major variants in this instantiation
           if (pr.ab_f16)
             SIGLIP_MMA_LOOP(1, 0, 0);
@@ -1654,6 +1686,10 @@ siglip_gemm_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_consta
         sample_loss_epilogue<false, false, false, true>(p, acc, &tmG, staging_base, warp, wg, lane, row0, col_base,
                                                         row_lo, c_lo, pr, t_eff, bias, tl, bl, g_store_policy, s_sp,
                                                         c_sp, s_g, c_g, s_gs, c_gs);
+      } else if constexpr (kMode == kModeDistillOpts) {
+        sample_loss_epilogue<false, false, false, false, true>(p, acc, &tmG, staging_base, warp, wg, lane, row0,
+                                                               col_base, row_lo, c_lo, pr, t_eff, bias, tl, bl,
+                                                               g_store_policy, s_sp, c_sp, s_g, c_g, s_gs, c_gs, pbuf);
       } else if constexpr (kMode == kModeLoss) {
         // argmax keys first, on the raw accumulator: whichever path each slab then takes below
         if constexpr (kMetrics) tile_metrics(acc, row_lo, col_base, c_lo, pr.M, pr.N, lane, p);
@@ -2877,6 +2913,12 @@ size_t gemm_smem_bytes(int mode) {
 // the five tensor maps and the parameter block travel as kernel parameters: keep them inside the classic 4 KiB limit
 static_assert(5 * sizeof(CUtensorMap) + sizeof(KernelParams) <= 4096, "kernel parameters exceed 4 KiB");
 
+// Distillation with per-sample losses, top-K, groups or label sets: kModeDistillOpts at kDistillStages. Defined behind
+// launch_gemm, so that its three kernels come after every other kernel in the module, whose code stays as it was.
+static int launch_distill_opts(int cluster, const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensorMap* tmA1,
+                               const CUtensorMap* tmB1, const CUtensorMap* tmG, const KernelParams& p, int num_sms,
+                               cudaStream_t stream);
+
 int launch_gemm(int cta_group, int mode, int stages, int mcast, int tile_n, const CUtensorMap* tmA0,
                 const CUtensorMap* tmB0, const CUtensorMap* tmA1, const CUtensorMap* tmB1, const CUtensorMap* tmG,
                 const KernelParams& p, int num_sms, cudaStream_t stream) {
@@ -2902,6 +2944,9 @@ int launch_gemm(int cta_group, int mode, int stages, int mcast, int tile_n, cons
     }
   }
   if (tile_n != kTileN) return static_cast<int>(cudaErrorInvalidValue);
+  if (mode == kModeLoss && p.k_teacher > 0 &&
+      (p.sl_rows != nullptr || p.tk_rows != nullptr || p.col_grp != nullptr || p.col_lab != nullptr))
+    return launch_distill_opts(cluster_size(cta_group, mcast), tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
   if (mode == kModeLoss && p.k_teacher > 0) {   // distillation: kModeDistill, kDistillStages whatever `stages` asks
     switch (cluster_size(cta_group, mcast)) {
       case 4: return launch_impl<kModeDistill, kDistillStages, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
@@ -3097,6 +3142,16 @@ int launch_wait_flags(const volatile unsigned int* flags, int n, unsigned int va
                       DebugRecord* dbg, cudaStream_t stream) {
   wait_flags_kernel<<<1, 32, 0, stream>>>(flags, n, value, timeout_ns, dbg);
   return static_cast<int>(cudaGetLastError());
+}
+
+static int launch_distill_opts(int cluster, const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensorMap* tmA1,
+                               const CUtensorMap* tmB1, const CUtensorMap* tmG, const KernelParams& p, int num_sms,
+                               cudaStream_t stream) {
+  switch (cluster) {
+    case 4: return launch_impl<kModeDistillOpts, kDistillStages, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+    case 2: return launch_impl<kModeDistillOpts, kDistillStages, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+    default: return launch_impl<kModeDistillOpts, kDistillStages, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+  }
 }
 
 }  // namespace siglip

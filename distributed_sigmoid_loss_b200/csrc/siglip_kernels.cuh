@@ -154,7 +154,8 @@ struct KernelParams {
   // the distillation loss kernel (kModeDistill, its own instantiation): every tile first contracts the teacher's image
   // rows (tmA1) with the teacher's text chunk (tmB1) over k_teacher, turns s^T into p = sigma(t_T s^T + b_T), then runs
   // the student's k-loop; the target of pair (i, j) is q = (1 - lambda) y + lambda p. In that kernel ids (row_ids),
-  // weights (row_w) and metric keys (row_keys) are runtime options.
+  // weights (row_w) and metric keys (row_keys) are runtime options. With sl_rows, tk_rows, col_grp or col_lab set as
+  // well, the launch runs kModeDistillOpts, which takes all of those as runtime options too.
   int k_teacher;              // D_T (multiple of 8); 0 = no teacher
   int teacher_f16;            // teacher operands are fp16(x * 16) instead of bf16
   const float* t_prime_T;     // fp32 device scalars: t_T = exp(t'_T), b_T
@@ -208,6 +209,10 @@ struct KernelParams {
 // weights, metric keys, per-sample-loss sums, top-K lists and excluded groups are runtime options in it
 // kModeFocal: the loss kernel of a focal step (KernelParams::focal != 0), its own instantiation; ids, label sets,
 // weights, metric keys, per-sample-loss sums, top-K lists and excluded groups are runtime options in it
+// kModeDistillOpts: the loss kernel of a distillation step with per-sample losses, top-K lists, excluded groups or label
+// sets (k_teacher > 0 and any of sl_rows, tk_rows, col_grp, col_lab), its own instantiation; the teacher pass of
+// kModeDistill, then the soft-target terms in the kModeFocal epilogue; ids, label sets, weights, excluded groups, metric
+// keys, per-sample-loss sums and top-K lists are runtime options in it
 enum KernelMode {
   kModeLoss = 0,
   kModeOut = 1,
@@ -216,7 +221,8 @@ enum KernelMode {
   kModeTopK = 4,
   kModeGroups = 5,
   kModeLabels = 6,
-  kModeFocal = 7
+  kModeFocal = 7,
+  kModeDistillOpts = 8
 };
 
 // Label sets: labels per set at most (SIGLIP_MAX_LABELS)

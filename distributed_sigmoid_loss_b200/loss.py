@@ -54,7 +54,7 @@ class SigmoidLossEngine:
     def __init__(self, batch: int, dim: int, device: torch.device, group=None, cta_group: int = 2,
                  overlap_pull: bool = True, rank_world: Optional[Tuple[int, int]] = None, loopback: bool = False,
                  batch_per_rank=None, texts_per_rank=None, images_per_rank=None, teacher_dim: int = 0,
-                 labels: int = 0):
+                 labels: int = 0, distill_options: bool = False):
         self._L = _capi.lib()
         if not torch.cuda.is_available() or self._L.siglip_device_count() == 0:
             raise RuntimeError("distributed_sigmoid_loss_b200 needs an sm_90 (H100) device; there is no CPU fallback")
@@ -62,12 +62,26 @@ class SigmoidLossEngine:
         self.rank, self.world = rank_world if rank_world is not None else _group_rank_world(group)
         h = ctypes.c_void_p()
         self.teacher_dim = int(teacher_dim)
-        if self.teacher_dim and (images_per_rank is not None or texts_per_rank is not None):
-            raise RuntimeError("a distillation engine (teacher_dim > 0) takes no extra texts or images")
         self.labels = int(labels)   # labels per set of a label-set engine (siglip_ctx_create_labels), 0: none
-        if self.labels and self.teacher_dim:
-            raise RuntimeError("a label-set engine (labels > 0) takes no teacher")
-        if self.labels:
+        # distill_options: a teacher together with extras, label sets, per-sample losses, top-K and groups
+        # (siglip_ctx_create_distill_extras); without it a distillation engine refuses them, as it always has
+        if distill_options and not self.teacher_dim:
+            raise RuntimeError("distill_options=True needs teacher_dim > 0")
+        if self.teacher_dim and not distill_options and (images_per_rank is not None or texts_per_rank is not None):
+            raise RuntimeError("a distillation engine (teacher_dim > 0) takes no extra texts or images without "
+                               "distill_options=True")
+        if self.labels and self.teacher_dim and not distill_options:
+            raise RuntimeError("a label-set engine (labels > 0) takes no teacher without distill_options=True")
+        if distill_options:
+            # every text and image of a rank has a teacher row
+            bpr, ipr, tpr = self._extras_lists(batch, batch_per_rank, images_per_rank, texts_per_rank)
+            _capi.check(self._L.siglip_ctx_create_distill_extras(
+                ctypes.byref(h), self.device.index or 0, self.rank, self.world, (ctypes.c_int * self.world)(*bpr),
+                (ctypes.c_int * self.world)(*ipr), (ctypes.c_int * self.world)(*tpr), dim, self.teacher_dim,
+                self.labels))
+            self.batch_per_rank, self.images_per_rank, self.texts_per_rank = bpr, ipr, tpr
+            images_per_rank, texts_per_rank = ipr, tpr
+        elif self.labels:
             # label sets: the sets' width is part of the exported allocation (siglip_ctx_create_labels)
             bpr, ipr, tpr = self._extras_lists(batch, batch_per_rank, images_per_rank, texts_per_rank)
             _capi.check(self._L.siglip_ctx_create_labels(ctypes.byref(h), self.device.index or 0, self.rank, self.world,
@@ -205,14 +219,14 @@ class SigmoidLossEngine:
 
     def set_teacher(self, timg: torch.Tensor, ttxt: torch.Tensor, t_prime: torch.Tensor, bias: torch.Tensor,
                     lam: float) -> None:
-        """SIGLIP_OPT_DISTILL: the teacher of the NEXT step. timg / ttxt: [B, teacher_dim] contiguous, 16-byte aligned,
-        both bf16 or both float16 holding 16*x (see teacher_operand); t_prime / bias: 1-element fp32 tensors on the
-        engine's device (t_T = exp(t_prime)); lam in (0, 1]. Only the pointers are recorded: the tensors must stay alive
-        until the step is enqueued."""
-        for x in (timg, ttxt):
+        """SIGLIP_OPT_DISTILL: the teacher of the NEXT step. timg: [images, teacher_dim], ttxt: [texts, teacher_dim]
+        (paired rows, then extras, like the student's), contiguous, 16-byte aligned, both bf16 or both float16 holding
+        16*x (see teacher_operand); t_prime / bias: 1-element fp32 tensors on the engine's device (t_T = exp(t_prime));
+        lam in (0, 1]. Only the pointers are recorded: the tensors must stay alive until the step is enqueued."""
+        for x, rows in ((timg, self.images), (ttxt, self.texts)):
             if x.device != self.device or x.dtype not in (torch.bfloat16, torch.float16) or not x.is_contiguous() or \
-                    tuple(x.shape) != (self.batch, self.teacher_dim):
-                raise RuntimeError(f"teacher operands must be contiguous bf16 (or fp16 x16) [{self.batch}, "
+                    tuple(x.shape) != (rows, self.teacher_dim):
+                raise RuntimeError(f"teacher operands must be contiguous bf16 (or fp16 x16) [{rows}, "
                                    f"{self.teacher_dim}] tensors on {self.device}, got {tuple(x.shape)} {x.dtype}")
         if timg.dtype != ttxt.dtype:
             raise RuntimeError("teacher image and text operands must use the same 16-bit format")
@@ -249,8 +263,8 @@ class SigmoidLossEngine:
         return out
 
     def debug_set_teacher_text_chunk(self, chunk: int, ttxt: torch.Tensor) -> None:
-        """Loopback: the teacher text of chunk `chunk` ([B_c, teacher_dim], the teacher's operand format) as its owner
-        would have published it."""
+        """Loopback: the teacher text of chunk `chunk` ([T_c, teacher_dim], the teacher's operand format: paired texts,
+        then extras) as its owner would have published it."""
         _capi.check(self._L.siglip_debug_set_teacher_text_chunk(self._h, chunk, ttxt.data_ptr(), self._stream()))
 
     def set_sample_ids(self, ids: torch.Tensor) -> None:
@@ -400,7 +414,7 @@ class SigmoidLossEngine:
         """Arm the top-K in-batch retrieval of the NEXT step (siglip_request_topk), k in 1 .. TOPK_MAX: recall fp32 [2k]
         (i2t recall@1..k, then t2i), i2t_topk int64 [metric_images, k] and t2i_topk int64 [metric_texts, k] (global
         indices, best first, -1 past the candidates) or None, all contiguous on the engine's device. Nothing is read on
-        the host; the step writes them on its stream. Refused under distillation."""
+        the host; the step writes them on its stream. Refused under distillation without distill_options."""
         if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= TOPK_MAX:
             raise RuntimeError(f"k must be an int in 1 .. {TOPK_MAX}, got {k!r}")
         bufs = (("recall", recall, torch.float32, (2 * k,)),
@@ -430,7 +444,8 @@ class SigmoidLossEngine:
         images, then the extra images) and text_loss fp32 [T] (the paired texts, then the extras), contiguous on the
         engine's device. image_loss[i] is the sum of w_ij softplus(-y_ij z_ij) over every text of the global batch,
         text_loss[j] the same sum over every image of the global batch (no 1/B). Nothing is read on the host; the step
-        writes them on its stream. Refused under distillation."""
+        writes them on its stream. Refused under distillation without distill_options; with it the terms are
+        w_ij (softplus(z_ij) - q_ij z_ij)."""
         for name, x, n in (("image_loss", image_loss, self.images), ("text_loss", text_loss, self.texts)):
             if not isinstance(x, torch.Tensor) or x.dtype != torch.float32 or tuple(x.shape) != (n,) or \
                     not x.is_contiguous() or x.device != self.device:
@@ -913,8 +928,9 @@ class _EngineCache:
                  bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
                  extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
                  distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None,
-                 exclude_groups: bool = False, multi_label: int = 0, focal=None):
+                 exclude_groups: bool = False, multi_label: int = 0, focal=None, distill_options: bool = False):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
+        self.distill_options = distill_options
         self.focal = focal   # (gamma, alpha or None), or None
         self.exclude_groups = exclude_groups
         self.multi_label = multi_label
@@ -946,7 +962,8 @@ class _EngineCache:
                 ipr = [int(b) + self.extra_images for b in bpr]
             eng = SigmoidLossEngine(batch, dim, dev, self.group, self.cta_group, self.overlap_pull,
                                     batch_per_rank=self.batch_per_rank, texts_per_rank=tpr, images_per_rank=ipr,
-                                    teacher_dim=teacher_dim, labels=self.multi_label)
+                                    teacher_dim=teacher_dim, labels=self.multi_label,
+                                    distill_options=self.distill_options and teacher_dim > 0)
             if self.sync_scalar_grads:
                 eng.set_option(_capi.SIGLIP_OPT_SYNC_SCALAR_GRADS, 1)
             if self.bidir:
@@ -1154,13 +1171,13 @@ def _weights_of(sample_weights: bool, image_weights, text_weights, image_embeddi
 
 
 def _validate_exclude_groups(exclude_groups, distill) -> bool:
-    """exclude_groups of a module: a bool, and not together with distill (the distillation loss kernel has no group
-    comparisons)."""
+    """exclude_groups of a module: a bool, and not together with distill unless distill_options=True (distill: the
+    module's distill_closed)."""
     if not isinstance(exclude_groups, bool):
         raise RuntimeError(f"exclude_groups must be a bool, got {type(exclude_groups).__name__}")
     if exclude_groups and distill is not None:
         raise RuntimeError("exclude_groups cannot be combined with distill: the distillation loss kernel does not "
-                           "exclude pairs")
+                           "exclude pairs (distill_options=True runs the one that does)")
     return exclude_groups
 
 
@@ -1198,7 +1215,7 @@ def _groups_of(exclude_groups: bool, image_groups, text_groups, image_embeddings
 
 def _validate_multi_label(multi_label, multi_positive: bool, distill) -> int:
     """multi_label=M of a module: None or 0 (off), or the labels per set, 1 .. MAX_LABELS. Label sets replace the ids of
-    multi_positive, and the distillation loss kernel has no label sets."""
+    multi_positive, and need distill_options=True under distill (distill: the module's distill_closed)."""
     if multi_label is None:
         return 0
     if isinstance(multi_label, bool) or not isinstance(multi_label, int) or not 0 <= multi_label <= MAX_LABELS:
@@ -1208,7 +1225,8 @@ def _validate_multi_label(multi_label, multi_positive: bool, distill) -> int:
         raise RuntimeError("multi_label cannot be combined with multi_positive: label sets replace the sample ids "
                            "(M = 1 with the ids as labels is multi_positive)")
     if multi_label and distill is not None:
-        raise RuntimeError("multi_label cannot be combined with distill: the distillation loss kernel has no label sets")
+        raise RuntimeError("multi_label cannot be combined with distill: the distillation loss kernel has no label sets "
+                           "(distill_options=True runs the one that has)")
     return multi_label
 
 
@@ -1281,33 +1299,47 @@ def _validate_focal(focal_gamma, focal_alpha, distill):
     return float(focal_gamma), (None if focal_alpha is None else float(focal_alpha))
 
 
-def _validate_distill(distill, hard_negatives: int, extra_texts: int, extra_images: int) -> Optional[float]:
+def _validate_distill(distill, hard_negatives: int, extra_texts: int, extra_images: int,
+                      distill_options=False) -> Optional[float]:
     """distill=lambda of a module: None (off) or a float in (0, 1], the weight of the teacher's probabilities in the
-    targets. The extras of hard_negatives / extra_texts / extra_images would need teacher embeddings of their own."""
+    targets. The extras of hard_negatives / extra_texts / extra_images need teacher embeddings of their own, which
+    only distill_options=True takes (a bool, and only with distill)."""
+    if not isinstance(distill_options, bool):
+        raise RuntimeError(f"distill_options must be a bool, got {type(distill_options).__name__}")
+    if distill_options and distill is None:
+        raise RuntimeError("distill_options=True needs distill=lambda")
     if distill is None:
         return None
     if isinstance(distill, bool) or not isinstance(distill, (int, float)) or not 0.0 < float(distill) <= 1.0:
         raise RuntimeError(f"distill must be a float in (0, 1] (the weight of the teacher's probabilities), got "
                            f"{distill!r}")
     for name, k in (("hard_negatives", hard_negatives), ("extra_texts", extra_texts), ("extra_images", extra_images)):
-        if k:
+        if k and not distill_options:
             raise RuntimeError(f"distill cannot be combined with {name}: its extra embeddings would need teacher "
-                               f"embeddings of their own")
+                               f"embeddings of their own (distill_options=True takes them)")
     return float(distill)
 
 
-def _teacher_of(distill: Optional[float], image_embeddings: torch.Tensor, names, values):
+def _teacher_of(distill: Optional[float], image_embeddings: torch.Tensor, names, values, extras=()):
     """The teacher arguments of a forward: all four required with distill, refused without. teacher_image and
     teacher_text are floating [B, D_T] tensors (the same shape, D_T may differ from the students' width) and the two
     scalars 1-element floating tensors, all on the embeddings' device, none requiring grad: the teacher is a constant
-    and a gradient with respect to it is never computed. Returns (timg, ttxt, scale, bias, lambda) with D_T zero-padded
-    to a multiple of 8, or None. Raises before any GPU work."""
+    and a gradient with respect to it is never computed. extras: (name, tensor, K, "text" or "image") of the teacher's
+    rows for the student's extras (teacher_negative_text, teacher_extra_text, teacher_extra_image): each required
+    exactly when its K > 0, a [K, D_T] tensor checked like the others and of its paired tensor's dtype, appended to
+    teacher_text or teacher_image in the student's order. Returns (timg, ttxt, scale, bias, lambda) with D_T
+    zero-padded to a multiple of 8, or None. Raises before any GPU work."""
     if distill is None:
-        for n, x in zip(names, values):
+        for n, x in list(zip(names, values)) + [(e[0], e[1]) for e in extras]:
             if x is not None:
                 raise RuntimeError(f"{n} given, but the loss was built without distill=lambda")
         return None
-    for n, x in zip(names, values):
+    for n, x, k, _ in extras:
+        if (x is not None) != (k > 0):
+            raise RuntimeError(f"{n} given, but the loss has no such extras" if x is not None else
+                               f"distill={distill}: forward needs {n} ([{k}, teacher_dim], the teacher's rows of the "
+                               f"extras)")
+    for n, x in list(zip(names, values)) + [(e[0], e[1]) for e in extras if e[1] is not None]:
         if x is None:
             raise RuntimeError(f"distill={distill}: forward needs {', '.join(names)}")
         if not isinstance(x, torch.Tensor) or not x.is_floating_point():
@@ -1328,7 +1360,26 @@ def _teacher_of(distill: Optional[float], image_embeddings: torch.Tensor, names,
     for n, x in zip(names[2:], (tscale, tbias)):
         if x.numel() != 1:
             raise RuntimeError(f"{n} must be a 0-dim (1-element) tensor, got shape {tuple(x.shape)}")
+    for n, x, k, side in extras:
+        if x is None:
+            continue
+        paired = ttxt if side == "text" else timg
+        if x.dim() != 2 or tuple(x.shape) != (k, timg.shape[1]):
+            raise RuntimeError(f"{n} must have shape [{k}, {timg.shape[1]}] (teacher_dim), got {tuple(x.shape)}")
+        if x.dtype != paired.dtype:
+            raise RuntimeError(f"{n} is {x.dtype}, the paired teacher {side}s {paired.dtype}: use one dtype")
+        if side == "text":
+            ttxt = torch.cat([ttxt, x])
+        else:
+            timg = torch.cat([timg, x])
     return (_pad_dim(timg), _pad_dim(ttxt), tscale, tbias, distill)
+
+
+def _teacher_extras(mod, negative_text, extra_text, extra_image):
+    """The teacher-extras argument of _teacher_of for a module (DDPSigmoidLoss or SigLipLoss)."""
+    return (("teacher_negative_text", negative_text, mod.hard_negatives, "text"),
+            ("teacher_extra_text", extra_text, mod.extra_texts, "text"),
+            ("teacher_extra_image", extra_image, mod.extra_images, "image"))
 
 
 def _validate_return_metrics(return_metrics) -> None:
@@ -1345,11 +1396,12 @@ def _metric_buffers(batch: int, device: torch.device, texts: Optional[int] = Non
 
 
 def _validate_return_sample_losses(return_sample_losses, distill) -> None:
+    """distill: the module's distill_closed."""
     if not isinstance(return_sample_losses, bool):
         raise RuntimeError(f"return_sample_losses must be a bool, got {type(return_sample_losses).__name__}")
     if return_sample_losses and distill is not None:
         raise RuntimeError("return_sample_losses is unavailable with distill: the distillation loss kernel does not "
-                           "compute per-sample losses")
+                           "compute per-sample losses (distill_options=True runs the one that does)")
 
 
 def _sample_loss_buffers(eng) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -1380,7 +1432,7 @@ def _metric_dict(bufs) -> Dict[str, torch.Tensor]:
 
 
 def _validate_metrics_topk(metrics_topk, return_metrics, distill) -> int:
-    """K of a forward's top-K retrieval (None: 1, the top-1 metrics alone)."""
+    """K of a forward's top-K retrieval (None: 1, the top-1 metrics alone). distill: the module's distill_closed."""
     if metrics_topk is None:
         return 1
     if isinstance(metrics_topk, bool) or not isinstance(metrics_topk, int) or not 1 <= metrics_topk <= TOPK_MAX:
@@ -1389,7 +1441,7 @@ def _validate_metrics_topk(metrics_topk, return_metrics, distill) -> int:
         raise RuntimeError("metrics_topk needs return_metrics=True")
     if distill is not None:
         raise RuntimeError("metrics_topk is unavailable with distill: the distillation loss kernel does not rank the "
-                           "top K")
+                           "top K (distill_options=True runs the one that does)")
     return metrics_topk
 
 
@@ -1498,9 +1550,16 @@ class DDPSigmoidLoss(nn.Module):
     ``(1/B) Σ w (softplus(z) − q z)``; λ = 1 is pure distillation. The teacher similarities are computed inside the loss
     kernel, tile by tile, and never stored; the teacher texts travel with the student texts. Teacher tensors follow the
     student's input rules (bf16 as is, fp32 through the fp16 conversion, ``normalize_inputs`` normalises them too) and
-    must not require grad. Composes with ``multi_positive``, ``sample_weights``, ``return_metrics`` (the metrics rank the
-    student's logits), ``batch_per_rank``, ``sync_scalar_grads`` and both schedules; not with ``hard_negatives``,
-    ``extra_texts`` or ``extra_images``. Collective: every rank uses the same λ and D_T.
+    must not require grad. Composes with ``multi_positive``, ``sample_weights``, ``return_metrics``, ``batch_per_rank``,
+    ``sync_scalar_grads`` and both schedules. With ``distill_options=True`` it composes with every option but
+    ``focal_gamma`` (the metrics and top-K lists rank the student's logits; per-sample losses sum the terms
+    ``w (softplus(z) − q z)``; an excluded pair adds 0); without it, ``hard_negatives``, ``extra_texts``,
+    ``extra_images``, ``exclude_groups``, ``multi_label``, ``return_sample_losses`` and ``metrics_topk`` > 1 are
+    refused, as they always were. With the flag and
+    ``hard_negatives`` / ``extra_texts`` / ``extra_images`` every ``forward`` also takes the teacher's rows of the extras,
+    ``teacher_negative_text`` / ``teacher_extra_text`` / ``teacher_extra_image`` ([K, D_T], the same rules); a hard
+    negative's target is ``λ σ(teacher logit)``, so a teacher that cannot tell it from the true caption pulls it up.
+    Collective: every rank uses the same λ and D_T.
 
     ``forward(..., return_sample_losses=True)`` returns ``(loss, sample_losses)``, or ``(loss, metrics, sample_losses)``
     with ``return_metrics``: ``image_loss`` ([R] fp32, the paired images then the extra images) holds, for each image
@@ -1509,16 +1568,16 @@ class DDPSigmoidLoss(nn.Module):
     image of the global batch. No 1/B is applied, so ``loss == image_loss.sum() / B`` up to rounding, and a sample of
     weight 0 reports exactly 0. The loss kernels add them up from the terms they already compute, in 64-bit fixed point,
     so they are bitwise reproducible; loss, gradients and metrics are unchanged. Device tensors, no host
-    synchronisation, not differentiable; works under ``torch.no_grad()`` (data selection over a super-batch). Not with
-    ``distill``. Collective: every rank asks on the same steps.
+    synchronisation, not differentiable; works under ``torch.no_grad()`` (data selection over a super-batch). Under
+    ``distill`` they sum the distillation terms ``w (softplus(z) − q z)``. Collective: every rank asks on the same
+    steps.
 
     ``forward(..., return_metrics=True, metrics_topk=K)``, K in 1 .. 10: with K > 1 the metrics dict also holds
     ``i2t_topk`` ([ni, K] int64: each ranked image's K best texts over the global batch, global indices, best first,
     ties to the lower index, −1 past the candidates), ``t2i_topk`` ([nt, K]: each ranked text's K best images) and
     ``i2t_recall`` / ``t2i_recall`` ([K] fp32: the fraction with a hit among the first k, k = 1 .. K, by the hit rules of
     the top-1 metrics). ``recall[0]`` and column 0 are the top-1 rate and index bit for bit; loss and gradients are
-    unchanged. K = 1 or None returns today's dict. Not with ``distill``; works under ``torch.no_grad()`` (evaluation,
-    mining). Collective: every rank asks the same K on the same steps.
+    unchanged. K = 1 or None returns today's dict. Works under ``torch.no_grad()`` (evaluation, mining). Collective: every rank asks the same K on the same steps.
 
     ``exclude_groups=True``: every ``forward`` also takes ``image_groups`` ([B + K_img] integers: the paired images, then
     ``extra_image``) and ``text_groups`` ([B + K] integers: the captions, then ``negative_text`` / ``extra_text``) on the
@@ -1528,7 +1587,8 @@ class DDPSigmoidLoss(nn.Module):
     (near-duplicates, dedup clusters, class labels: in-batch false negatives). The loss still divides by B. Unique groups
     give exactly the step without the option. Retrieval metrics and top-K lists are unchanged: every pair stays a
     candidate; the lists hold global indices, so a caller can look the groups up. Works with or without
-    ``multi_positive``; not with ``distill``. Collective: set on every rank.
+    ``multi_positive`` and with ``distill`` (an excluded pair adds 0 whatever its teacher probability). Collective: set
+    on every rank.
 
     ``multi_label=M`` (1 <= M <= 4): multi-label positives. Every ``forward`` takes ``sample_labels`` ([B, M] integers:
     the label set of sample i, shared by image i and caption i; a negative entry is an empty slot, duplicates are
@@ -1538,7 +1598,7 @@ class DDPSigmoidLoss(nn.Module):
     a positive for the prompts "a photo of a dog" ({dog}) and "a photo of a golden retriever"; a poodle image ({poodle,
     dog}) only for the first. Every other pair is negative; the loss still divides by B. M = 1 with labels >= 0 is
     ``multi_positive`` with those ids. Retrieval metrics and top-K lists count a hit by the same rule and rank every
-    image and text of the rank (extras included). Composes with every option but ``multi_positive`` and ``distill``;
+    image and text of the rank (extras included). Composes with every option but ``multi_positive``;
     ``exclude_groups`` applies after these positives. Collective: the same M on every rank.
 
     ``focal_gamma=gamma`` (0 <= gamma <= 8) and ``focal_alpha=alpha`` (None, or 0 <= alpha <= 1): torchvision's
@@ -1558,17 +1618,21 @@ class DDPSigmoidLoss(nn.Module):
                  extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
                  distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None,
                  exclude_groups: bool = False, multi_label: Optional[int] = None,
-                 focal_gamma: Optional[float] = None, focal_alpha: Optional[float] = None) -> None:
+                 focal_gamma: Optional[float] = None, focal_alpha: Optional[float] = None,
+                 distill_options: bool = False) -> None:
         super().__init__()
         _sigma_budget_mib(sigma_budget_bytes)
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_images = _validate_hard_negatives(extra_images, "extra_images")
-        multi_label = _validate_multi_label(multi_label, multi_positive, distill)
+        # distill_closed: what the option checks refuse, distill=lambda without distill_options (None otherwise)
+        closed = None if distill_options is True else distill
+        multi_label = _validate_multi_label(multi_label, multi_positive, closed)
         # extra texts carry ids under multi_positive, label sets under multi_label
         extra_texts = _validate_extra_texts(extra_texts, multi_positive or bool(multi_label), hard_negatives)
         sample_weights = _validate_sample_weights(sample_weights)
-        distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images)
-        exclude_groups = _validate_exclude_groups(exclude_groups, distill)
+        distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images, distill_options)
+        self.distill_closed = None if distill_options else distill
+        exclude_groups = _validate_exclude_groups(exclude_groups, self.distill_closed)
         focal = _validate_focal(focal_gamma, focal_alpha, distill)
         self.t_prime = nn.Parameter(torch.tensor(math.log(10), dtype=torch.float64))
         self.bias = nn.Parameter(torch.tensor(-10.0))
@@ -1605,7 +1669,8 @@ class DDPSigmoidLoss(nn.Module):
                                    multi_positive=multi_positive, hard_negatives=hard_negatives,
                                    extra_texts=extra_texts, sample_weights=sample_weights, extra_images=extra_images,
                                    distill=distill, sigma_budget_bytes=sigma_budget_bytes,
-                                   exclude_groups=exclude_groups, multi_label=multi_label, focal=focal)
+                                   exclude_groups=exclude_groups, multi_label=multi_label, focal=focal,
+                                   distill_options=distill_options)
         # extension: bound of the 16-bit sigma operands; steps then run in row panels (memory O(budget), not O(B^2))
         self.sigma_budget_bytes = sigma_budget_bytes
 
@@ -1626,13 +1691,17 @@ class DDPSigmoidLoss(nn.Module):
                 teacher_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False,
                 metrics_topk: Optional[int] = None, image_groups: Optional[torch.Tensor] = None,
                 text_groups: Optional[torch.Tensor] = None, sample_labels: Optional[torch.Tensor] = None,
-                extra_text_labels: Optional[torch.Tensor] = None, extra_image_labels: Optional[torch.Tensor] = None):
+                extra_text_labels: Optional[torch.Tensor] = None, extra_image_labels: Optional[torch.Tensor] = None,
+                teacher_negative_text: Optional[torch.Tensor] = None,
+                teacher_extra_text: Optional[torch.Tensor] = None,
+                teacher_extra_image: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
-        _validate_return_sample_losses(return_sample_losses, self.distill)
-        topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill)
+        _validate_return_sample_losses(return_sample_losses, self.distill_closed)
+        topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill_closed)
         teacher = _teacher_of(self.distill, image_embeddings,
                               ("teacher_image", "teacher_text", "teacher_t_prime", "teacher_bias"),
-                              (teacher_image, teacher_text, teacher_t_prime, teacher_bias))
+                              (teacher_image, teacher_text, teacher_t_prime, teacher_bias),
+                              _teacher_extras(self, teacher_negative_text, teacher_extra_text, teacher_extra_image))
         ids = _validate_ids(sample_ids, self.multi_positive, image_embeddings)
         _validate_negatives(text_embeddings, negative_text, self.hard_negatives)
         _validate_negatives(text_embeddings, extra_text, self.extra_texts, "extra_text", "extra_texts")
@@ -1681,7 +1750,8 @@ class SigLipLoss(nn.Module):
     [K, D] (and with ``multi_positive`` ``extra_image_ids`` [K]), hard-negative images or further images of a caption as
     in ``DDPSigmoidLoss``; ``image_weights`` then has B + K entries. ``distill=lambda``: every forward takes
     ``teacher_image`` / ``teacher_text`` [B, D_T] and ``teacher_logit_scale`` / ``teacher_logit_bias`` (0-dim, the
-    convention of ``logit_scale`` / ``logit_bias``), distillation from a frozen teacher as in ``DDPSigmoidLoss``.
+    convention of ``logit_scale`` / ``logit_bias``), distillation from a frozen teacher as in ``DDPSigmoidLoss``, with
+    ``teacher_negative_text`` / ``teacher_extra_text`` / ``teacher_extra_image`` [K, D_T] for the extras.
     ``return_sample_losses=True``: also returns the per-sample losses of ``DDPSigmoidLoss`` (``image_loss`` [R],
     ``text_loss`` [T]) as the last element, after the metrics when both are asked; like the metrics they stay out of
     the ``output_dict``. ``exclude_groups=True``: every forward takes ``image_groups`` [B + K_img] and ``text_groups``
@@ -1696,17 +1766,19 @@ class SigLipLoss(nn.Module):
                  sample_weights: bool = False, extra_images: int = 0, distill: Optional[float] = None,
                  sigma_budget_bytes: Optional[int] = None, exclude_groups: bool = False,
                  multi_label: Optional[int] = None, focal_gamma: Optional[float] = None,
-                 focal_alpha: Optional[float] = None):
+                 focal_alpha: Optional[float] = None, distill_options: bool = False):
         super().__init__()
         _sigma_budget_mib(sigma_budget_bytes)
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_images = _validate_hard_negatives(extra_images, "extra_images")
-        multi_label = _validate_multi_label(multi_label, multi_positive, distill)
+        closed = None if distill_options is True else distill   # as on DDPSigmoidLoss
+        multi_label = _validate_multi_label(multi_label, multi_positive, closed)
         extra_texts = _validate_extra_texts(extra_texts, multi_positive or bool(multi_label), hard_negatives)
         sample_weights = _validate_sample_weights(sample_weights)
-        distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images)
-        exclude_groups = _validate_exclude_groups(exclude_groups, distill)
+        distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images, distill_options)
+        self.distill_closed = None if distill_options else distill
+        exclude_groups = _validate_exclude_groups(exclude_groups, self.distill_closed)
         focal = _validate_focal(focal_gamma, focal_alpha, distill)
         self.focal = focal
         self.distill = distill
@@ -1723,7 +1795,8 @@ class SigLipLoss(nn.Module):
         self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive,
                                    hard_negatives=hard_negatives, extra_texts=extra_texts, sample_weights=sample_weights,
                                    extra_images=extra_images, distill=distill, sigma_budget_bytes=sigma_budget_bytes,
-                                   exclude_groups=exclude_groups, multi_label=multi_label, focal=focal)
+                                   exclude_groups=exclude_groups, multi_label=multi_label, focal=focal,
+                                   distill_options=distill_options)
         # bound of the 16-bit sigma operands; steps then run in row panels (as on DDPSigmoidLoss)
         self.sigma_budget_bytes = sigma_budget_bytes
 
@@ -1737,13 +1810,17 @@ class SigLipLoss(nn.Module):
                 teacher_logit_bias: Optional[torch.Tensor] = None, return_sample_losses: bool = False,
                 metrics_topk: Optional[int] = None, image_groups: Optional[torch.Tensor] = None,
                 text_groups: Optional[torch.Tensor] = None, sample_labels: Optional[torch.Tensor] = None,
-                extra_text_labels: Optional[torch.Tensor] = None, extra_image_labels: Optional[torch.Tensor] = None):
+                extra_text_labels: Optional[torch.Tensor] = None, extra_image_labels: Optional[torch.Tensor] = None,
+                teacher_negative_text: Optional[torch.Tensor] = None,
+                teacher_extra_text: Optional[torch.Tensor] = None,
+                teacher_extra_image: Optional[torch.Tensor] = None):
         _validate_return_metrics(return_metrics)
-        _validate_return_sample_losses(return_sample_losses, self.distill)
-        topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill)
+        _validate_return_sample_losses(return_sample_losses, self.distill_closed)
+        topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill_closed)
         teacher = _teacher_of(self.distill, image_features,
                               ("teacher_image", "teacher_text", "teacher_logit_scale", "teacher_logit_bias"),
-                              (teacher_image, teacher_text, teacher_logit_scale, teacher_logit_bias))
+                              (teacher_image, teacher_text, teacher_logit_scale, teacher_logit_bias),
+                              _teacher_extras(self, teacher_negative_text, teacher_extra_text, teacher_extra_image))
         ids = _validate_ids(sample_ids, self.multi_positive, image_features)
         _validate_negatives(text_features, negative_text, self.hard_negatives)
         _validate_negatives(text_features, extra_text, self.extra_texts, "extra_text", "extra_texts")

@@ -140,17 +140,23 @@ enum {
                                       hard-negative image. Without this option an extra image matches no id. The loss
                                       still divides by B_r. Needs SIGLIP_OPT_SAMPLE_IDS on (else SIGLIP_ERR_STATE);
                                       turning that option off clears this one. Collective: set on all ranks. Default 0 */
-  SIGLIP_OPT_DISTILL = 25, /* 1: distillation from a frozen teacher (siglip_ctx_create_distill contexts only, else
-                              SIGLIP_ERR_STATE). The target of pair (i, j) becomes
+  SIGLIP_OPT_DISTILL = 25, /* 1: distillation from a frozen teacher (siglip_ctx_create_distill and
+                              siglip_ctx_create_distill_extras contexts only, else SIGLIP_ERR_STATE). The target of pair (i, j) becomes
                                 q_ij = (1 - lambda) y_ij + lambda sigma(t_T <timg_i, ttxt_j> + b_T)
-                              (y in {0, 1}: the labels the other options give) and rank r's loss
+                              (y in {0, 1}: the labels the other options give; 0 for a hard negative) and rank r's
+                              loss
                                 (1/B_r) sum_ij w_ij (softplus(z_ij) - q_ij z_ij).
-                              The teacher similarities are computed tile by tile inside the loss kernel and never
-                              stored; the teacher texts travel with the student texts. Every step needs
-                              siglip_set_teacher since the previous step (else SIGLIP_ERR_STATE before any launch).
-                              Composes with SIGLIP_OPT_SAMPLE_IDS, SIGLIP_OPT_SAMPLE_WEIGHTS, metrics, bidir and
-                              uneven batches; unavailable with hard negatives / extra texts / extra images and in the
-                              host-buffer entries. The gradient kernels are unchanged. Collective. Default 0 */
+                              An extra text or image takes its teacher probability from its own teacher row. An
+                              excluded pair (SIGLIP_OPT_EXCLUDE_GROUPS) adds exactly 0. The teacher similarities are
+                              computed tile by tile inside the loss kernel and never stored; the teacher texts travel
+                              with the student texts. Every step needs siglip_set_teacher since the previous step (else
+                              SIGLIP_ERR_STATE before any launch). Composes with ids, weights, metrics, row panels,
+                              bidir and uneven batches. On a siglip_ctx_create_distill_extras context it also composes
+                              with extras, excluded groups, label sets, per-sample losses and top-K; a
+                              siglip_ctx_create_distill context refuses those (SIGLIP_ERR_STATE). Never with
+                              SIGLIP_OPT_FOCAL, nor in the host-buffer entries. Per-sample losses sum the terms w_ij (softplus(z_ij) - q_ij z_ij) >= 0; metrics
+                              and top-K rank the student's logits. The gradient kernels are unchanged. Collective.
+                              Default 0 */
   SIGLIP_OPT_SIGMA_BUDGET_MIB = 26, /* bound, in MiB, of the 16-bit sigma operands (the one buffer that grows with B^2).
                                        0 (default): none, every step as before. Otherwise siglip_fwd_bwd scores the
                                        rank's R rows in row panels of P rows, P the largest multiple of
@@ -176,10 +182,11 @@ enum {
                                      per-sample losses (the loss still divides by B_r). Metrics and top-K lists are
                                      unchanged. Every step needs siglip_set_groups since the previous step (else
                                      SIGLIP_ERR_STATE before any launch); the text groups travel to the other ranks with
-                                     the text. Unavailable with SIGLIP_OPT_DISTILL and in the host-buffer entries
-                                     (SIGLIP_ERR_STATE). Collective. Default 0 */
-  SIGLIP_OPT_LABEL_SETS = 28, /* 1: multi-label positives (siglip_ctx_create_labels contexts only, else
-                                 SIGLIP_ERR_STATE). Every sample carries a set of M int64 labels (a negative entry is an
+                                     the text. Unavailable with SIGLIP_OPT_DISTILL on a siglip_ctx_create_distill
+                                     context, and in the host-buffer entries (SIGLIP_ERR_STATE). Collective.
+                                     Default 0 */
+  SIGLIP_OPT_LABEL_SETS = 28, /* 1: multi-label positives (siglip_ctx_create_labels contexts and
+                                 siglip_ctx_create_distill_extras contexts with M > 0 only, else SIGLIP_ERR_STATE). Every sample carries a set of M int64 labels (a negative entry is an
                                  empty slot; duplicates are allowed), shared by its image and its paired text; extra
                                  texts and extra images carry their own. Pair (image i, text j) is positive iff it is the
                                  own-chunk positional pair (i == j < B_r on the own chunk) or the two sets share a label
@@ -191,8 +198,8 @@ enum {
                                  rank all R_r images (i2t) and all T_r texts (t2i). Every step needs siglip_set_label_sets
                                  since the previous step (else SIGLIP_ERR_STATE before any launch); the text sets travel
                                  to the other ranks with the text. Unavailable with SIGLIP_OPT_SAMPLE_IDS,
-                                 SIGLIP_OPT_EXTRA_TEXT_IDS, SIGLIP_OPT_EXTRA_IMAGE_IDS, SIGLIP_OPT_DISTILL and in the
-                                 host-buffer entries (SIGLIP_ERR_STATE). Collective. Default 0 */
+                                 SIGLIP_OPT_EXTRA_TEXT_IDS, SIGLIP_OPT_EXTRA_IMAGE_IDS and in the host-buffer entries
+                                 (SIGLIP_ERR_STATE). Collective. Default 0 */
   SIGLIP_OPT_FOCAL = 29, /* 1: the focal pair loss (torchvision's sigmoid_focal_loss) in place of the SigLIP term. Pair
                             (i, j) with target y (from whatever labels the other options give), p = sigma(z),
                             p_t = y ? p : 1 - p and a_t = y ? alpha : 1 - alpha (1 without alpha) adds
@@ -317,8 +324,22 @@ int siglip_ctx_create_labels(siglip_ctx** out, int device, int rank, int world, 
                              const int* images_per_rank, const int* texts_per_rank, int D, int M);
 
 /*
- * SIGLIP_OPT_DISTILL: the teacher of the NEXT step. timg [B, D_teacher] and ttxt [B, D_teacher] are this rank's teacher
- * embeddings, both bf16 (teacher_f16 = 0) or both fp16(x * 16) (teacher_f16 = 1, the fp32-input format), 16-byte
+ * A context that holds everything at once: a teacher of width D_teacher (a positive multiple of 8, as in
+ * siglip_ctx_create_distill), extra texts and extra images (as in siglip_ctx_create_extras) and, for M in
+ * 1 .. SIGLIP_MAX_LABELS, label sets (as in siglip_ctx_create_labels; M = 0: none). The gathered teacher text is
+ * [world][T_max, D_teacher]: every text of a rank, paired then extras, has a teacher row. Handle import refuses a peer
+ * whose D_teacher or M differs. Under SIGLIP_OPT_DISTILL such a context takes per-sample losses, top-K, excluded
+ * groups and label sets, which a siglip_ctx_create_distill context refuses. siglip_ctx_create_distill has the layout
+ * of this entry with images = texts = batch and M = 0, and siglip_ctx_create_labels that of this entry without a
+ * teacher.
+ */
+int siglip_ctx_create_distill_extras(siglip_ctx** out, int device, int rank, int world, const int* batch_per_rank,
+                                     const int* images_per_rank, const int* texts_per_rank, int D, int D_teacher,
+                                     int M);
+
+/*
+ * SIGLIP_OPT_DISTILL: the teacher of the NEXT step. timg [R, D_teacher] and ttxt [T, D_teacher] are this rank's teacher
+ * embeddings in the order of the student's (paired rows, then extras; R = T = B without extras), both bf16 (teacher_f16 = 0) or both fp16(x * 16) (teacher_f16 = 1, the fp32-input format), 16-byte
  * aligned; t_prime_T / bias_T are fp32 device scalars (t_T = exp(t_prime_T)); lambda in (0, 1]. Only the pointers are
  * recorded (like siglip_request_metrics): the buffers must hold their values when the step runs on its stream, and a
  * single-rank step stays capturable into a CUDA graph. No gradient flows to the teacher.
@@ -527,8 +548,9 @@ int siglip_request_metrics(siglip_ctx* ctx, float* top1, int64_t* i2t_index, int
  * parities of [world * Tmax + Rmax] sums plus as many poison words, 64-bit each; on a single-rank context
  * 32 * (T + R) bytes allocated by the first call (also allowed inside a capture), on a multi-rank context part of the
  * exported text allocation from creation. This call only records the pointers, so a single-rank step stays capturable.
- * Collective: every rank arms the same steps. Returns SIGLIP_ERR_STATE under SIGLIP_OPT_DISTILL; the host-buffer entries
- * return SIGLIP_ERR_STATE while armed. */
+ * Collective: every rank arms the same steps. Under SIGLIP_OPT_DISTILL the sums are those of the distillation
+ * terms; a siglip_ctx_create_distill context returns SIGLIP_ERR_STATE there (siglip_ctx_create_distill_extras takes
+ * them). The host-buffer entries return SIGLIP_ERR_STATE while armed. */
 int siglip_request_sample_losses(siglip_ctx* ctx, float* image_loss, float* text_loss);
 
 /* Largest K of siglip_request_topk. */
@@ -553,7 +575,8 @@ int siglip_request_sample_losses(siglip_ctx* ctx, float* image_loss, float* text
  * first call (also allowed inside a capture), the column lists of a multi-rank context are part of the exported text
  * allocation from creation. This call only records the pointers.
  * Collective: every rank arms the same steps with the same k. Returns SIGLIP_ERR_INVALID for k out of range or a null
- * recall, SIGLIP_ERR_STATE under SIGLIP_OPT_DISTILL; the host-buffer entries return SIGLIP_ERR_STATE while armed. */
+ * recall, SIGLIP_ERR_STATE under SIGLIP_OPT_DISTILL on a siglip_ctx_create_distill context (a
+ * siglip_ctx_create_distill_extras context takes it); the host-buffer entries return SIGLIP_ERR_STATE while armed. */
 int siglip_request_topk(siglip_ctx* ctx, int k, float* recall, int64_t* i2t_topk, int64_t* t2i_topk);
 
 /* Forward only (torch.no_grad / evaluation): siglip_forward with save_for_backward = 0. */
@@ -626,7 +649,8 @@ int siglip_debug_loopback(siglip_ctx* ctx);
 int siglip_debug_set_text_chunk(siglip_ctx* ctx, int chunk, const void* txt_dev, void* cuda_stream);
 
 /* The teacher twin of siglip_debug_set_text_chunk (SIGLIP_OPT_DISTILL): the teacher text of chunk `chunk`
- * ([batch of that rank, D_teacher] in the teacher's format) as its owner would have published it. */
+ * ([T of that rank, D_teacher] in the teacher's format: paired texts, then extras) as its owner would have published
+ * it. */
 int siglip_debug_set_teacher_text_chunk(siglip_ctx* ctx, int chunk, const void* ttxt_dev, void* cuda_stream);
 
 /* The teacher's operand formats (width D_teacher): siglip_convert_f32_rows and siglip_normalize_fwd_rows over `rows`

@@ -62,6 +62,10 @@ def main() -> int:
                     help="also check distillation from a frozen teacher against the float64 oracle: the teacher text "
                          "travelling with the student text through the peer pulls, a teacher width different from the "
                          "student's, uneven batches, with and without sample ids and weights, fused and split")
+    ap.add_argument("--distill-options", action="store_true",
+                    help="also check distillation with the other options against the float64 oracle: hard negatives "
+                         "and label sets with extras (each with the teacher's rows of the extras travelling with the "
+                         "text), excluded groups and weights, per-sample losses, uneven batches, fused and split")
     ap.add_argument("--sample-losses", action="store_true",
                     help="also check the per-sample losses (return_sample_losses=True) against the float64 oracle: "
                          "text_loss combines every rank's column partials of the own chunk, uneven batches, hard "
@@ -909,6 +913,80 @@ def main() -> int:
                         dtxt=rel_f(b.grad.float().cpu(), dtxt_ref),
                         dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
                         db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"])))
+
+    # ---- distillation with the other options: the teacher's rows of the extras travel with the text ----------------
+    if args.distill_options:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))      # the oracle lives with the tests
+        from distill_options_oracle import closed_form_distill_options
+        from exclude_groups_oracle import group_labels
+        from extra_images_oracle import label_blocks as xlabel_blocks
+        from label_sets_oracle import set_labels
+        Bs = [160 + 24 * r for r in range(world)]
+        D, DT, tp, bias, ttp, tbias, lam = 136, 72, math.log(10.0), -8.0, math.log(20.0), -6.0, 0.6
+        g = torch.Generator().manual_seed(6666)
+        rng = np.random.default_rng(6666)
+        unit = lambda n, d: torch.nn.functional.normalize(torch.randn(n, d, generator=g)).to(torch.bfloat16)  # noqa: E731
+        for kind, K, E in (("negatives", 48, 0), ("sets", 29, 17)):
+            Ts, Rs = [b + K for b in Bs], [b + E for b in Bs]
+            imgs, texts = [unit(r_, D) for r_ in Rs], [unit(t_, D) for t_ in Ts]
+            timgs, ttexts = [unit(r_, DT) for r_ in Rs], [unit(t_, DT) for t_ in Ts]
+            if kind == "sets":
+                ss = [rng.integers(-1, 12, (b, 2)) for b in Bs]
+                tsets = [np.concatenate([s_, rng.integers(-1, 12, (K, 2))]) for s_ in ss]
+                isets = [np.concatenate([s_, rng.integers(-1, 12, (E, 2))]) for s_ in ss]
+                lab = set_labels(isets, tsets, Bs)
+            else:
+                lab = xlabel_blocks(Bs, Rs, Ts)
+            iws = [rng.random(r_) for r_ in Rs]
+            tws = [rng.random(t_) for t_ in Ts]
+            igs = [rng.integers(-1, 6, r_) for r_ in Rs]
+            tgs = [rng.integers(-1, 6, t_) for t_ in Ts]
+            lab = group_labels(lab, igs, tgs)
+            f = lambda xs: [x.double().numpy() for x in xs]  # noqa: E731
+            ref = closed_form_distill_options(f(imgs), f(texts), tp, bias, f(timgs), f(ttexts), ttp, tbias, lam, lab, Bs,
+                                              iws, tws)
+            mine = ref[rank]
+            dtxt_ref = torch.from_numpy(sum(ref[r]["contrib"][rank] for r in range(world)))
+            tl_ref = torch.from_numpy(sum(ref[r]["text_part"][rank] for r in range(world)))
+            img, txt = imgs[rank].to(dev), texts[rank].to(dev)
+            B = Bs[rank]
+            for fused in (None, False):
+                modx = DDPSigmoidLoss(B, fused_step=fused, batch_per_rank=Bs, multi_label=2 if kind == "sets" else None,
+                                      hard_negatives=K if kind == "negatives" else 0,
+                                      extra_texts=K if kind == "sets" else 0, extra_images=E, sample_weights=True,
+                                      exclude_groups=True, distill=lam, distill_options=True).to(dev)
+                with torch.no_grad():
+                    modx.t_prime.fill_(tp)
+                    modx.bias.fill_(bias)
+                for rep in range(2):
+                    modx.zero_grad()
+                    a, b = (x.float().requires_grad_(True) for x in (img, txt))
+                    ti, tt = timgs[rank].to(dev), ttexts[rank].to(dev)
+                    kw = dict(teacher_image=ti[:B], teacher_text=tt[:B], teacher_t_prime=torch.tensor(ttp, device=dev),
+                              teacher_bias=torch.tensor(tbias, device=dev),
+                              image_weights=torch.from_numpy(iws[rank]).float().to(dev),
+                              text_weights=torch.from_numpy(tws[rank]).float().to(dev),
+                              image_groups=torch.from_numpy(igs[rank]).to(dev),
+                              text_groups=torch.from_numpy(tgs[rank]).to(dev))
+                    if kind == "negatives":
+                        kw.update(negative_text=b[B:], teacher_negative_text=tt[B:])
+                    else:
+                        kw.update(sample_labels=torch.from_numpy(isets[rank][:B]).to(dev),
+                                  extra_text=b[B:], teacher_extra_text=tt[B:],
+                                  extra_text_labels=torch.from_numpy(tsets[rank][B:]).to(dev),
+                                  extra_image=a[B:], teacher_extra_image=ti[B:],
+                                  extra_image_labels=torch.from_numpy(isets[rank][B:]).to(dev))
+                    l2, sl = modx(a[:B] if E else a, b[:B], return_sample_losses=True, **kw)
+                    l2.backward()
+                    torch.cuda.synchronize()
+                    report(f"distill-options {kind} {fused} B={Bs} K={K} E={E} rep{rep}", dict(
+                        loss=abs(float(l2) - mine["loss"]) / abs(mine["loss"]),
+                        dimg=rel_f(a.grad.float().cpu(), torch.from_numpy(mine["dimg"])),
+                        dtxt=rel_f(b.grad.float().cpu(), dtxt_ref),
+                        dtp=abs(float(modx.t_prime.grad) - mine["dt_prime"]) / abs(mine["dt_prime"]),
+                        db=abs(float(modx.bias.grad) - mine["dbias"]) / abs(mine["dbias"]),
+                        image_loss=rel_f(sl["image_loss"].cpu(), torch.from_numpy(mine["image_loss"])),
+                        text_loss=rel_f(sl["text_loss"].cpu(), tl_ref)))
 
     # ---- larger: fp32 autograd; dtxt reference summed over ranks ------------------------------------------
     B, D, tp, bias = 2048, 768, math.log(10.0), -10.0
