@@ -1,47 +1,59 @@
 """The loss step's options in combination: a table of cells and a composed float64 oracle — test infrastructure, never
 the product path.
 
-Every cell turns on a set of options (sample ids, extra texts / images with or without ids, weights, excluded groups, a
-teacher, per-sample losses, metrics, top-K) and picks the engine configuration it runs under (W, bidir, schedule, row
-panels, INPUT_F16, gradient tile width, stages, cluster shape). ``route`` restates how ``launch_gemm`` picks the loss
-kernel for each launch of the step, so the table's coverage of kernel instantiations and runtime branches is derived,
-not claimed. ``oracle`` composes the single-feature oracles (no new loss math); ``retrieval`` and ``peer_stand_ins``
-give the exact retrieval results and what the loopback hooks need to stand in for the other ranks.
+Every cell turns on a set of options (sample ids or label sets, extra texts / images with or without ids or sets,
+weights, excluded groups, the focal terms or a teacher, per-sample losses, metrics, top-K) and picks the engine
+configuration it runs under (W, bidir, schedule, row panels, INPUT_F16, gradient tile width, stages, cluster shape).
+``route`` restates how ``launch_gemm`` picks the loss kernel for each launch of the step, so the table's coverage of
+kernel instantiations and runtime branches is derived, not claimed. ``oracle`` composes the single-feature oracles (no
+new loss math); ``retrieval`` and ``peer_stand_ins`` give the exact retrieval results and what the loopback hooks need to
+stand in for the other ranks.
 
 Planted data: every embedding entry is a small integer / 8, so the bf16 and fp16(16 x) operands are exact and every fp32
 logit equals its float64 value; retrieval is compared exactly. Samples are integer cluster centres (one per group) plus
 an integer vector per sample id plus sparse noise: duplicate ids are near-duplicates, captions and extras lie near their
 image, and same-group negatives have sigma(z) ~ 0.12 at t = 5, bias = -6 (against ~0.003 for the other negatives), so
-the excluded pairs carry weight while a flipped label still moves a step's loss by more than 20x the tolerance."""
+the excluded pairs carry weight while a flipped label still moves a step's loss by more than 20x the tolerance. A label
+set holds the sample's id and a few tags of a small pool (not the groups: a positive is never excluded). The teacher's
+rows are an integer vector per teacher key plus sparse noise, the key being the id except that ids 2k + 1 share 2k's:
+at t_T = 6, b_T = -10 its p is ~0.97 on the pairs with one key and ~1e-4 elsewhere, a sharp teacher (a low entropy
+floor under the loss) that knows matches the labels do not."""
 from __future__ import annotations
 
 import dataclasses
 import itertools
 import math
 from dataclasses import dataclass
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 
-from distill_oracle import closed_form_distill
+from distill_options_oracle import closed_form_distill_options
 from exclude_groups_oracle import closed_form_groups, group_labels, text_loss_of
 from extra_images_oracle import label_blocks
+from focal_oracle import closed_form_focal
+from label_sets_oracle import set_labels, topk_retrieval_sets
 from retrieval_metrics_oracle import key_as_int64, metric_key
 from retrieval_topk_oracle import recall_counts, topk_retrieval
 from sample_losses_oracle import fixed_point_partial
 
 TP, BIAS = math.log(5.0), -6.0
-TTP, TBIAS, LAM = math.log(3.0), -2.0, 0.6   # the teacher's t', bias and the distillation weight lambda
+TTP, TBIAS, LAM = math.log(6.0), -10.0, 0.6   # the teacher's t', bias and the distillation weight lambda
 TOL = 1e-3
 KMAX = 10   # SIGLIP_TOPK_MAX: the width of a peer's seeded top-K column lists
 D, DT = 136, 72
 N_GROUPS = 10
+MMAX = 4    # the widest label set a cell uses
+N_TAGS = 40
 
-MODES = ("loss", "sample_loss", "topk", "groups", "distill")
+MODES = ("loss", "sample_loss", "topk", "groups", "distill", "labels", "focal", "distill_opts")
 CONTEXTS = ("plain", "hn", "xt", "xi", "xin", "both")
 SCHEDS = ("fused", "split", "fwd")
 CLUSTERS = {1: [(1, 1)], 2: [(2, 1), (1, 2)], 4: [(2, 2)]}   # cluster size -> (cta_group, mcast)
-DISTILL_STAGES = 4   # kDistillStages: the distillation kernel runs 4 stages whatever the request
+DISTILL_STAGES = 4   # kDistillStages: both teacher kernels run 4 stages whatever the request
+SET_MODES = ("labels", "focal", "distill_opts")   # the modes whose steps can carry label sets
+# (gamma, alpha) of the focal cells; gamma 0 without alpha is the plain step
+FOCALS = tuple((g, a) for g in (0.5, 2.0, 5.0) for a in (None, 0.25))
 
 # per-rank paired batches, extra texts and extra images of each world size (uneven, ragged past 256 at W = 1); the
 # panel cells use larger batches so that a budget of a few MiB splits the rows into several panels
@@ -52,15 +64,19 @@ PANEL_SHAPES = {1: ((700,), (60,), (48,)), 2: ((600, 520), (40, 72), (24, 36)),
 
 @dataclass(frozen=True)
 class Options:
-    """What a step computes. Extra-text / extra-image ids need sample ids; a teacher takes none of the extras, groups,
-    per-sample losses or top-K (the documented refusals)."""
+    """What a step computes. Extra-text / extra-image ids need sample ids, extra-text / extra-image sets need label sets;
+    label sets take no ids, and the focal terms no teacher (the documented refusals)."""
     ids: bool = False
-    xtexts: bool = False     # extra texts: hard negatives, or with xt_ids further captions
-    ximages: bool = False    # extra images: hard negatives, or with xi_ids further images of a caption
+    xtexts: bool = False     # extra texts: hard negatives, or with xt_ids / xt_sets further captions
+    ximages: bool = False    # extra images: hard negatives, or with xi_ids / xi_sets further images of a caption
     xt_ids: bool = False
     xi_ids: bool = False
+    labels: int = 0          # M: label sets of M labels per sample (SIGLIP_OPT_LABEL_SETS), 0: none
+    xt_sets: bool = False    # the extra texts carry sets of their own (else the empty sets of hard negatives)
+    xi_sets: bool = False
     weights: bool = False
     groups: bool = False
+    focal: Optional[Tuple[float, Optional[float]]] = None   # (gamma, alpha) of SIGLIP_OPT_FOCAL
     teacher: bool = False
     metrics: bool = False    # siglip_request_metrics (top-1)
     losses: bool = False     # siglip_request_sample_losses
@@ -71,9 +87,9 @@ class Options:
         if self.xtexts and self.ximages:
             return "both"
         if self.xtexts:
-            return "xt" if self.xt_ids else "hn"
+            return "xt" if (self.xt_ids or self.xt_sets) else "hn"
         if self.ximages:
-            return "xi" if self.xi_ids else "xin"
+            return "xi" if (self.xi_ids or self.xi_sets) else "xin"
         return "plain"
 
     @property
@@ -84,27 +100,40 @@ class Options:
     def valid(self) -> bool:
         if (self.xt_ids and not (self.ids and self.xtexts)) or (self.xi_ids and not (self.ids and self.ximages)):
             return False
-        return not (self.teacher and (self.xtexts or self.ximages or self.groups or self.losses or self.topk > 1))
+        if (self.xt_sets and not (self.labels and self.xtexts)) or (self.xi_sets and not (self.labels and
+                                                                                           self.ximages)):
+            return False
+        if not 0 <= self.labels <= MMAX or (self.labels and self.ids):
+            return False
+        return not (self.focal is not None and self.teacher)
 
     def removals(self) -> Dict[str, "Options"]:
         """Each option this step turns on that changes its labels, weights or targets, switched off on its own (with
-        what it needs: ids take the extras' ids along)."""
+        what depends on it: ids take the extras' ids along, label sets the extras' sets)."""
         r = dataclasses.replace
         out = {}
         if self.xtexts:
-            out["extra texts"] = r(self, xtexts=False, xt_ids=False)
+            out["extra texts"] = r(self, xtexts=False, xt_ids=False, xt_sets=False)
         if self.ximages:
-            out["extra images"] = r(self, ximages=False, xi_ids=False)
+            out["extra images"] = r(self, ximages=False, xi_ids=False, xi_sets=False)
         if self.ids:
             out["ids"] = r(self, ids=False, xt_ids=False, xi_ids=False)
         if self.xt_ids:
             out["extra text ids"] = r(self, xt_ids=False)
         if self.xi_ids:
             out["extra image ids"] = r(self, xi_ids=False)
+        if self.labels:
+            out["label sets"] = r(self, labels=0, xt_sets=False, xi_sets=False)
+        if self.xt_sets:
+            out["extra text sets"] = r(self, xt_sets=False)
+        if self.xi_sets:
+            out["extra image sets"] = r(self, xi_sets=False)
         if self.weights:
             out["weights"] = r(self, weights=False)
         if self.groups:
             out["groups"] = r(self, groups=False)
+        if self.focal is not None:
+            out["focal"] = r(self, focal=None)
         if self.teacher:
             out["teacher"] = r(self, teacher=False)
         return out
@@ -136,8 +165,10 @@ class Cell:
     @property
     def name(self) -> str:
         o = self.opts
-        on = [k for k in ("ids", "xt_ids", "xi_ids", "weights", "groups", "teacher", "metrics", "losses")
-              if getattr(o, k)]
+        on = [k for k in ("ids", "xt_ids", "xi_ids", "xt_sets", "xi_sets", "weights", "groups", "teacher", "metrics",
+                          "losses") if getattr(o, k)]
+        on += [f"M{o.labels}"] if o.labels else []
+        on += [f"g{o.focal[0]:g}" + (f"a{o.focal[1]:g}" if o.focal[1] is not None else "")] if o.focal else []
         on += [f"k{o.topk}"] if o.topk else []
         return (f"{self.seed:03d}-{self.mode}-{o.context}-{'+'.join(on) or 'none'}-W{self.W}r{self.r}"
                 f"{'-bidir' if self.bidir else ''}-{self.sched}{'-panels' if self.panels else ''}"
@@ -170,10 +201,15 @@ def _round_up(x, m):
 
 
 def mode_of(o: Options) -> str:
-    """The loss kernel launch_gemm selects (csrc/siglip_kernels.cu): distillation first, then groups, top-K (K > 1),
-    per-sample losses, and otherwise the plain loss kernel."""
+    """The loss kernel launch_gemm selects (csrc/siglip_kernels.cu): a teacher with per-sample losses, top-K (K > 1),
+    groups or label sets runs kModeDistillOpts, any other teacher kModeDistill; then the focal terms, label sets, groups,
+    top-K, per-sample losses, and otherwise the plain loss kernel."""
     if o.teacher:
-        return "distill"
+        return "distill_opts" if (o.losses or o.topk > 1 or o.groups or o.labels) else "distill"
+    if o.focal is not None:
+        return "focal"
+    if o.labels:
+        return "labels"
     if o.groups:
         return "groups"
     if o.topk > 1:
@@ -187,34 +223,73 @@ def route(cell: Cell):
     """The loss-kernel launches of the cell's step, one per text chunk: (instantiation, runtime options) pairs.
     An instantiation is (mode, stages, cluster size[, ids, metrics, weights]) — kModeLoss compiles its three options in,
     the other modes take them at run time. ids is on for a chunk whose labels come from ids: True for every chunk with
-    sample ids, "iota" for the own chunk of a rank with extras of both kinds under positional labels (the positional
-    pairs as iota ids: the same branch, fed differently)."""
+    sample ids, "iota" for the own chunk of a rank that holds extras of both kinds (run_loss_chunk's own_pos_ids: the
+    positional pairs as iota ids, the same branch fed differently; under label sets the label-set pre-pass folds them into
+    the positives). sets is on for every chunk of a label-set step. A teacher step also records the context it runs in
+    (distill_extras_context): the distill-extras workspace puts the gathered teacher text, and what follows it, at other
+    offsets, so the same kModeDistill branch reads different addresses there."""
     o = cell.opts
     mode = mode_of(o)
-    stages = DISTILL_STAGES if mode == "distill" else cell.stages
+    stages = DISTILL_STAGES if mode in ("distill", "distill_opts") else cell.stages
+    Bs, Rs, Ts = cell.shapes()
+    own_pos_ids = Rs[cell.r] > Bs[cell.r] and Ts[cell.r] > Bs[cell.r]
     out = set()
     for c in range(cell.W):
-        ids = True if o.ids else ("iota" if c == cell.r and o.xtexts and o.ximages else False)
+        ids = True if o.ids else ("iota" if c == cell.r and own_pos_ids else False)
         if mode == "loss":
             out.add(((mode, stages, cell.cluster, ids, o.keys, o.weights), ()))
             continue
         rt = dict(ids=ids, weights=o.weights, metrics=o.keys)
-        if mode in ("topk", "groups"):
+        if mode in ("topk", "groups") + SET_MODES:
             rt["losses"] = o.losses
-        if mode == "groups":
+        if mode in ("groups",) + SET_MODES:
             rt["topk"] = o.topk > 1
+        if mode in SET_MODES:
+            rt["groups"] = o.groups
+        if mode in ("focal", "distill_opts"):
+            rt["sets"] = bool(o.labels)
+        if o.teacher:
+            rt["extras_ctx"] = distill_extras_context(cell)
         out.add(((mode, stages, cell.cluster), tuple(sorted(rt.items()))))
     return out
 
 
+def distill_extras_context(cell: Cell) -> bool:
+    """A teacher cell runs in a siglip_ctx_create_distill_extras context (distill_options=True) when it has extras or
+    kModeDistillOpts's options, and in a siglip_ctx_create_distill one otherwise."""
+    Bs, Rs, Ts = cell.shapes()
+    return cell.opts.teacher and (Rs != Bs or Ts != Bs or cell.mode == "distill_opts")
+
+
 def runtime_options(mode: str) -> List[str]:
+    """The runtime options a mode's kernel branches on. The label source of kModeFocal and kModeDistillOpts is ids or
+    sets (positions: neither); kModeLabels always has sets, and its iota ids are part of them."""
     return {"loss": [], "sample_loss": ["ids", "metrics", "weights"], "topk": ["ids", "losses", "metrics", "weights"],
-            "groups": ["ids", "losses", "metrics", "topk", "weights"], "distill": ["ids", "metrics", "weights"]}[mode]
+            "groups": ["ids", "losses", "metrics", "topk", "weights"],
+            "labels": ["groups", "losses", "metrics", "topk", "weights"],
+            "focal": ["groups", "ids", "losses", "metrics", "sets", "topk", "weights"],
+            "distill": ["ids", "metrics", "weights"],
+            "distill_opts": ["groups", "ids", "losses", "metrics", "sets", "topk", "weights"]}[mode]
+
+
+def runtime_combos(mode: str) -> List[Dict[str, bool]]:
+    """Every combination of the mode's runtime options a step can reach: no ids with sets, and a teacher step without
+    sets, groups, per-sample losses and top-K runs kModeDistill instead."""
+    names = runtime_options(mode)
+    out = []
+    for v in itertools.product((False, True), repeat=len(names)):
+        f = dict(zip(names, v))
+        if f.get("ids") and f.get("sets"):
+            continue
+        if mode == "distill_opts" and not (f["sets"] or f["groups"] or f["losses"] or f["topk"]):
+            continue
+        out.append(f)
+    return out
 
 
 def instantiations(mode: str):
     """Every loss-kernel instantiation launch_gemm can select for a mode."""
-    if mode == "distill":
+    if mode in ("distill", "distill_opts"):
         return {(mode, DISTILL_STAGES, cs) for cs in CLUSTERS}
     base = {(mode, st, cs) for st in (4, 6) for cs in CLUSTERS}
     if mode != "loss":
@@ -223,32 +298,44 @@ def instantiations(mode: str):
 
 
 def axis_values(mode: str) -> Dict[str, tuple]:
-    """The values of every other axis a mode can be paired with (distillation takes no extras)."""
-    return dict(context=("plain",) if mode == "distill" else CONTEXTS, W=(1, 2, 3), bidir=(False, True), sched=SCHEDS,
-                panels=(False, True), f16=(False, True), tile_n=(128, 256), stages=(4, 6), cluster=(1, 2, 4))
+    """The values of every other axis a mode can be paired with: the set width M for the modes that carry sets, and
+    (gamma, alpha) for the focal terms."""
+    out = dict(context=CONTEXTS, W=(1, 2, 3), bidir=(False, True), sched=SCHEDS, panels=(False, True),
+               f16=(False, True), tile_n=(128, 256), stages=(4, 6), cluster=(1, 2, 4))
+    if mode in SET_MODES:
+        out["M"] = tuple(range(1, MMAX + 1))
+    if mode == "focal":
+        out["focal"] = FOCALS
+    return out
 
 
 def axis_of(cell: Cell, axis: str):
-    return cell.opts.context if axis == "context" else getattr(cell, axis)
+    if axis == "context":
+        return cell.opts.context
+    if axis == "M":
+        return cell.opts.labels
+    if axis == "focal":
+        return cell.opts.focal
+    return getattr(cell, axis)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # the table
 # ---------------------------------------------------------------------------------------------------------------------
-def _combos(names):
-    return [dict(zip(names, v)) for v in itertools.product((False, True), repeat=len(names))]
-
-
 def _mode_rows():
     """(mode, runtime options, stages, cluster) of every cell: the 48 kModeLoss instantiations, and for every other mode
-    each combination of its runtime options once, cycling through its instantiations."""
+    each combination of its runtime options once, cycling through its instantiations. kModeDistill's combinations run
+    without extras (the cells the table had before a teacher took extras); one cell per other context follows them."""
     rows = []
-    for f in _combos(["ids", "metrics", "weights"]):
+    for f in runtime_combos("sample_loss"):   # ids, metrics, weights: kModeLoss's compiled-in options
         for st in (4, 6):
             for cs in (1, 2, 4):
                 rows.append(("loss", f, st, cs))
-    for mode in ("sample_loss", "topk", "groups", "distill"):
-        for i, f in enumerate(_combos(runtime_options(mode))):
+    for mode in MODES[1:]:
+        combos = runtime_combos(mode)
+        if mode == "distill":
+            combos += [dict(ids=True, metrics=k % 2 == 1, weights=k // 2 % 2 == 1) for k in range(len(CONTEXTS) - 1)]
+        for i, f in enumerate(combos):
             rows.append((mode, f, (4, 6)[(i // 3) % 2], (1, 2, 4)[i % 3]))
     return rows
 
@@ -268,24 +355,37 @@ def build_table() -> List[Cell]:
         i, cyc = j[0], j[1]
         j[0] += 1
         ids = f.get("ids", False)
+        sets = mode == "labels" or f.get("sets", False)
         W = (1, 2, 3)[i % 3]
-        ctx = "plain" if mode == "distill" else _lru_pick(
-            cyc.setdefault("ctx", list(CONTEXTS)),
-            lambda c: (ids or c not in ("xt", "xi")) and (ids or W > 1 or c != "both"))
+        # xt / xi: extras with ids or sets of their own; both at W = 1 under positional labels would run iota ids only
+        if mode == "distill":   # its runtime combinations without extras, then every other context once
+            ctx = "plain" if i < len(runtime_combos(mode)) else CONTEXTS[1 + i - len(runtime_combos(mode))]
+        else:
+            ctx = _lru_pick(cyc.setdefault("ctx", list(CONTEXTS)),
+                            lambda c: (ids or sets or c not in ("xt", "xi")) and (ids or sets or W > 1 or c != "both"))
         panels = i % 4 == 3
-        sched = "fused" if panels else _lru_pick(cyc.setdefault("sched", list(SCHEDS)), lambda s: True)
+        # the loss alone can move by less than 20x the tolerance when a label-set step has extras (the tag positives
+        # raise it, the same-id positives lower it, and the extras' pairs are few) or a teacher's step has sets or
+        # extras with ids (its soft targets): those cells check gradients too
+        own = ctx in ("xt", "xi", "both")
+        loss_only = not ((sets and ctx != "plain") or (mode in ("distill", "distill_opts") and (sets or (ids and own))))
+        sched = "fused" if panels else _lru_pick(cyc.setdefault("sched", list(SCHEDS)), lambda s: loss_only or s != "fwd")
         cg, mcast = CLUSTERS[cs][(i // 2) % len(CLUSTERS[cs])]
         metrics = f.get("metrics", False)
+        M = _lru_pick(cyc.setdefault("M", list(range(1, MMAX + 1))), lambda m: True) if sets else 0
+        focal = _lru_pick(cyc.setdefault("focal", list(FOCALS)), lambda x: True) if mode == "focal" else None
         o = Options(ids=ids, xtexts=ctx in ("hn", "xt", "both"), ximages=ctx in ("xi", "xin", "both"),
                     xt_ids=ids and ctx in ("xt", "both"), xi_ids=ids and ctx in ("xi", "both"),
-                    weights=f.get("weights", False), groups=mode == "groups", teacher=mode == "distill",
+                    labels=M, xt_sets=sets and ctx in ("xt", "both"), xi_sets=sets and ctx in ("xi", "both"),
+                    weights=f.get("weights", False), groups=mode == "groups" or f.get("groups", False),
+                    focal=focal, teacher=mode in ("distill", "distill_opts"),
                     # a metrics cell of the modes without a top-K option asks for it as a K = 1 top-K request every
                     # other time: the same keys, a second set of outputs
                     metrics=metrics and not (mode in ("loss", "sample_loss") and i % 2),
                     losses=f.get("losses", False) or mode == "sample_loss",
                     topk=(5 if mode == "topk" else 3 if f.get("topk") else
                           1 if metrics and mode in ("loss", "sample_loss") and i % 2 else 0))
-        assert o.valid(), o
+        assert o.valid() and mode_of(o) == mode, o
         cells.append(Cell(o, W, i % W, W > 1 and (i // 3) % 2 == 1, sched, panels, (i + i // 4) % 2 == 1,
                           (128, 256)[(i // 2 + i // 8) % 2], stages, cg, mcast, seed))
     return cells
@@ -313,14 +413,38 @@ class Problem:
     tw: list          # [T_r]
     ig: list          # [R_r] int64, -1: no group
     tg: list          # [T_r]
-    timgs: list       # [B_r, DT] teacher
-    ttxts: list
+    itags: list       # [R_r, MMAX] int64 tags of the label sets, -1: an empty slot
+    ttags: list       # [T_r, MMAX]
+    timgs: list       # [R_r, DT] teacher
+    ttxts: list       # [T_r, DT]
 
     def view(self, o: Options):
         """(Bs, Rs, Ts, imgs, txts) of the step: the extras a step without them does not have are cut off."""
         Rs = self.Rs if o.ximages else self.Bs
         Ts = self.Ts if o.xtexts else self.Bs
         return (self.Bs, Rs, Ts, [x[:n] for x, n in zip(self.imgs, Rs)], [x[:n] for x, n in zip(self.txts, Ts)])
+
+    def teacher(self, o: Options):
+        """(timgs [R_r, DT], ttxts [T_r, DT]) of the step."""
+        Bs, Rs, Ts, _, _ = self.view(o)
+        return [x[:n] for x, n in zip(self.timgs, Rs)], [x[:n] for x, n in zip(self.ttxts, Ts)]
+
+    def sets(self, o: Options):
+        """(image sets [R_r, M], text sets [T_r, M]) of a label-set step: the first M tag slots with the row's id
+        (sample id, then the extra's id) in slot row % M, and the empty sets that siglip_set_label_sets writes for
+        extras without sets of their own. A paired text's set is its image's."""
+        Bs, Rs, Ts, _, _ = self.view(o)
+        M = o.labels
+
+        def build(tags, ids, extra_ids, b, n, own):
+            s = tags[:n, :M].copy()
+            s[np.arange(n), np.arange(n) % M] = np.concatenate([ids, extra_ids])[:n]
+            if not own:
+                s[b:] = -1
+            return s
+
+        return ([build(*a, o.xi_sets) for a in zip(self.itags, self.ids, self.xi_ids, Bs, Rs)],
+                [build(*a, o.xt_sets) for a in zip(self.ttags, self.ids, self.xt_ids, Bs, Ts)])
 
 
 def planted(cell: Cell) -> Problem:
@@ -332,10 +456,15 @@ def planted(cell: Cell) -> Problem:
     n_ids = max(8, sum(Bs) // 2)                       # duplicates within and across ranks
     id_vec = g.choice([-1, 0, 1], (n_ids, D), p=[0.3, 0.4, 0.3])
     id_grp = g.integers(0, N_GROUPS, n_ids)
+    tkey_vec = g.integers(-2, 3, (n_ids, DT))   # the teacher's vector of each key
 
     def near(idv):
         idv = np.asarray(idv, np.int64)
         return (centres[id_grp[idv]] + id_vec[idv] + g.choice([-1, 0, 1], (len(idv), D), p=[0.1, 0.8, 0.1])) / 8.0
+
+    def tnear(idv):
+        idv = np.asarray(idv, np.int64)
+        return (tkey_vec[idv - (idv % 2 == 1)] + g.choice([-1, 0, 1], (len(idv), DT), p=[0.1, 0.8, 0.1])) / 8.0
 
     def groups_of(idv):
         gr = id_grp[np.asarray(idv, np.int64)].astype(np.int64)
@@ -347,7 +476,11 @@ def planted(cell: Cell) -> Problem:
         w[g.random(n) < 0.2] = 0.0
         return w
 
-    P = dict(imgs=[], txts=[], ids=[], xt_ids=[], xi_ids=[], iw=[], tw=[], ig=[], tg=[], timgs=[], ttxts=[])
+    def tags(n):
+        return np.where(g.random((n, MMAX)) < 0.15, 10 ** 7 + g.integers(0, N_TAGS, (n, MMAX)), -1).astype(np.int64)
+
+    P = dict(imgs=[], txts=[], ids=[], xt_ids=[], xi_ids=[], iw=[], tw=[], ig=[], tg=[], itags=[], ttags=[], timgs=[],
+             ttxts=[])
     for b, r_, t_ in zip(Bs, Rs, Ts):
         ids = g.integers(0, n_ids, b)
         # extras: a text (image) near a sample of the global id pool; a fifth of the extra images carry a fresh id
@@ -365,9 +498,11 @@ def planted(cell: Cell) -> Problem:
         P["tw"].append(weights(t_))
         P["ig"].append(np.concatenate([groups_of(ids), groups_of(xi_content)]))
         P["tg"].append(np.concatenate([groups_of(ids), groups_of(xt)]))
-        timg = g.integers(-2, 3, (b, DT))
-        P["timgs"].append(timg / 8.0)
-        P["ttxts"].append((timg + g.choice([-1, 0, 1], (b, DT), p=[0.2, 0.6, 0.2])) / 8.0)
+        ti = tags(r_)
+        P["itags"].append(ti)
+        P["ttags"].append(np.concatenate([ti[:b], tags(t_ - b)]))
+        P["timgs"].append(np.concatenate([tnear(ids), tnear(xi_content)]))
+        P["ttxts"].append(np.concatenate([tnear(ids), tnear(xt)]))
     return Problem(Bs, Rs, Ts, **P)
 
 
@@ -376,39 +511,49 @@ def planted(cell: Cell) -> Problem:
 # ---------------------------------------------------------------------------------------------------------------------
 def labels(P: Problem, o: Options):
     Bs, Rs, Ts, _, _ = P.view(o)
-    lab = label_blocks(Bs, Rs, Ts, P.ids if o.ids else None, P.xt_ids if o.xt_ids else None,
-                       P.xi_ids if o.xi_ids else None)
+    if o.labels:
+        lab = set_labels(*P.sets(o), Bs)
+    else:
+        lab = label_blocks(Bs, Rs, Ts, P.ids if o.ids else None, P.xt_ids if o.xt_ids else None,
+                           P.xi_ids if o.xi_ids else None)
     if o.groups:
         lab = group_labels(lab, [x[:n] for x, n in zip(P.ig, Rs)], [x[:n] for x, n in zip(P.tg, Ts)])
     return lab
 
 
 def oracle(P: Problem, o: Options) -> List[Dict]:
-    """Per rank: loss, dimg [R_r, D], contrib[c] [T_c, D], dt_prime, dbias; without a teacher also image_loss [R_r],
-    text_part[c] (this rank's column sums over chunk c) and text_loss [T_r] (every rank's column sums of its chunk)."""
+    """Per rank: loss, dimg [R_r, D], contrib[c] [T_c, D], dt_prime, dbias, image_loss [R_r], text_part[c] (this rank's
+    column sums over chunk c) and text_loss [T_r] (every rank's column sums of its chunk)."""
     Bs, Rs, Ts, imgs, txts = P.view(o)
     iw = [x[:n].astype(np.float64) for x, n in zip(P.iw, Rs)] if o.weights else None
     tw = [x[:n].astype(np.float64) for x, n in zip(P.tw, Ts)] if o.weights else None
     lab = labels(P, o)
     if o.teacher:
-        return closed_form_distill(imgs, txts, TP, BIAS, P.timgs, P.ttxts, TTP, TBIAS, LAM, iw, tw, lab)
-    res = closed_form_groups(imgs, txts, TP, BIAS, lab, Bs, iw, tw)
+        res = closed_form_distill_options(imgs, txts, TP, BIAS, *P.teacher(o), TTP, TBIAS, LAM, lab, Bs, iw, tw)
+    elif o.focal is not None:
+        res = closed_form_focal(imgs, txts, TP, BIAS, lab, o.focal[0], o.focal[1], Bs, iw, tw)
+    else:
+        res = closed_form_groups(imgs, txts, TP, BIAS, lab, Bs, iw, tw)
     for r, x in enumerate(res):
         x["text_loss"] = text_loss_of(res, r)
     return res
 
 
 def retrieval(P: Problem, o: Options, k: int) -> List[Dict]:
-    """Per rank: top-K lists and recall (topk_retrieval), and the top-1 outputs they contain: i2t_index / t2i_index
-    (column 0) and top1 = (i2t, t2i) rates as the kernels count them. Weights and groups play no part; i2t ranks all
-    R_r images only under extra-image ids, t2i all T_r texts only under extra-text ids."""
+    """Per rank: top-K lists and recall (topk_retrieval, or topk_retrieval_sets under label sets), and the top-1 outputs
+    they contain: i2t_index / t2i_index (column 0) and top1 = (i2t, t2i) rates as the kernels count them. Weights, groups,
+    the focal terms and a teacher play no part; i2t ranks all R_r images only under extra-image ids or label sets, t2i
+    all T_r texts only under extra-text ids or label sets."""
     Bs, Rs, Ts, imgs, txts = P.view(o)
-    img_ids = txt_ids = None
-    if o.ids:
-        img_ids = [np.concatenate([a, b]) if o.xi_ids else a for a, b in zip(P.ids, P.xi_ids)]
-        txt_ids = [np.concatenate([a, b]) if o.xt_ids else a for a, b in zip(P.ids, P.xt_ids)]
-    out = topk_retrieval(imgs, txts, Bs, max(k, 1), img_ids, txt_ids, rank_all_images=o.xi_ids,
-                         rank_all_texts=o.xt_ids)
+    if o.labels:
+        out = topk_retrieval_sets(imgs, txts, Bs, max(k, 1), *P.sets(o))
+    else:
+        img_ids = txt_ids = None
+        if o.ids:
+            img_ids = [np.concatenate([a, b]) if o.xi_ids else a for a, b in zip(P.ids, P.xi_ids)]
+            txt_ids = [np.concatenate([a, b]) if o.xt_ids else a for a, b in zip(P.ids, P.xt_ids)]
+        out = topk_retrieval(imgs, txts, Bs, max(k, 1), img_ids, txt_ids, rank_all_images=o.xi_ids,
+                             rank_all_texts=o.xt_ids)
     for x in out:
         x["i2t_index"], x["t2i_index"] = x["i2t_topk"][:, 0].copy(), x["t2i_topk"][:, 0].copy()
         x["top1"] = np.array([recall_counts(x["i2t_first"], 1)[0], recall_counts(x["t2i_first"], 1)[0]], np.float32)
@@ -420,11 +565,13 @@ def retrieval(P: Problem, o: Options, k: int) -> List[Dict]:
 def peer_stand_ins(P: Problem, o: Options, r: int, res: Optional[List[Dict]], ret: Optional[List[Dict]],
                    f16: bool = False):
     """What each peer p != r publishes for rank r's chunk: metric_keys (its column argmax keys, [B_r], [T_r] under
-    extra-text ids), topk_keys ([T_r, KMAX] sorted, 0-padded), partials (fixed-point words of its column sums, [T_r]) and
-    xi_ids (its extra-image ids, under extra-image ids). The keys hold the loss kernel's accumulator: <img, txt>, or
-    2^8 <img, txt> for fp16(16 x) operands (f16), as every rank of an INPUT_F16 job computes them."""
+    extra-text ids or label sets), topk_keys ([T_r, KMAX] sorted, 0-padded), partials (fixed-point words of its column
+    sums, [T_r]), xi_ids (its extra-image ids, under extra-image ids) and under label sets tsets (its text chunk's sets)
+    and xi_sets (its extra images' sets). The keys hold the loss kernel's accumulator: <img, txt>, or 2^8 <img, txt> for
+    fp16(16 x) operands (f16), as every rank of an INPUT_F16 job computes them."""
     acc = 256.0 if f16 else 1.0
     Bs, Rs, Ts, _, _ = P.view(o)
+    isets, tsets = P.sets(o) if o.labels else (None, None)
     out = {}
     for p in range(len(Bs)):
         if p == r:
@@ -438,11 +585,14 @@ def peer_stand_ins(P: Problem, o: Options, r: int, res: Optional[List[Dict]], re
                 order = np.lexsort((np.arange(len(col)), -col))[:KMAX]
                 keys[j, :len(order)] = [key_as_int64(metric_key(acc * col[i], off[p] + i)) for i in order]
             d["topk_keys"] = keys
-            d["metric_keys"] = keys[:Ts[r] if o.xt_ids else Bs[r], 0].copy()
-        if res is not None and "text_part" in res[p]:
+            d["metric_keys"] = keys[:Ts[r] if (o.xt_ids or o.labels) else Bs[r], 0].copy()
+        if res is not None:
             d["partials"] = np.array([fixed_point_partial(v)[0] for v in res[p]["text_part"][r]], np.int64)
         if o.xi_ids:
             d["xi_ids"] = P.xi_ids[p][:Rs[p] - Bs[p]]
+        if o.labels:
+            d["tsets"] = tsets[p]
+            d["xi_sets"] = isets[p][Bs[p]:]
         out[p] = d
     return out
 
