@@ -69,6 +69,7 @@ EXPORTED_SYMBOLS = (
     "siglip_ctx_launch_count",
     "siglip_debug_gemm",
     "siglip_debug_gemm_timed",
+    "siglip_debug_max_active_clusters",
     "siglip_debug_loopback",
     "siglip_debug_set_text_chunk",
     "siglip_debug_get_slot",
@@ -295,6 +296,8 @@ def lib() -> ctypes.CDLL:
     L.siglip_debug_gemm_timed.argtypes = [ci, ci, ci, ci, ci, vp, ctypes.c_longlong, ci, vp, ctypes.c_longlong, ci, vp,
                                           ctypes.c_longlong, ci, ctypes.POINTER(ctypes.c_float), vp]
     L.siglip_debug_gemm_timed.restype = ci
+    L.siglip_debug_max_active_clusters.argtypes = [ci, ci, ci, ci, ci]
+    L.siglip_debug_max_active_clusters.restype = ci
     L.siglip_ctx_destroy.argtypes = [vp]
     L.siglip_ctx_destroy.restype = None
     _lib = L
@@ -308,6 +311,14 @@ def last_error() -> str:
 def check(code: int) -> None:
     if code != SIGLIP_OK:
         raise SiglipError(code, last_error())
+
+
+def max_active_clusters(cta_group: int, mcast: int, tile_n: int, stages: int = 0, device: int = 0) -> int:
+    """Clusters of the persistent grid of a gradient-kernel launch on `device` (siglip_debug_max_active_clusters)."""
+    n = lib().siglip_debug_max_active_clusters(device, cta_group, mcast, tile_n, stages)
+    if n < 0:
+        raise SiglipError(-n, last_error())
+    return n
 
 
 def device_count() -> int:

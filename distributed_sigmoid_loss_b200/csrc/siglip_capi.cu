@@ -1595,8 +1595,10 @@ int backward_impl(siglip_ctx* c, const void* img, const void* txt, const float* 
 // Under SIGLIP_OPT_SIGMA_BUDGET_MIB the rows are scored in np panels of P rows (DESIGN.md, "Row panels"): every sigma
 // operand holds one panel, and each chunk runs L G per panel (index k.p below). Panel 0 of the own chunk keeps the
 // role of L0 / G0, so the exchange keeps its shape:
-//   W > 1:  L0.0  [L0.p G0.p]p=np-1..1  [L1.p G1.p]p=0..np-1  ...  [L(W-1).p G(W-1).p]  G0.0
+//   W > 1:  L0.0  [L0.p G0.p]p=np-1..1  [L1.p G1.p]p=0..np-1  ...  [L(W-1).p G(W-1).p]p=1..np-1,0  G0.0
 //   W = 1:        [L0.p G0.p]p=np-1..1  L0.0 G0.0          (one buffer: nothing is in flight)
+// The forward's last loss launch sums the partial slots of its own grid, which follows its panel's row tiles: it must
+// be a launch of panel 0, the largest, whose grid L0.0 set up. So the last chunk runs its panel 0 last (W = 1: L0.0).
 // Flag 1 of a remote chunk is raised by its last panel's gradient launch; its earlier panels add into the slot. The
 // own panels past 0 sum their dtxt into a local partial (slot `rank`, which no peer reads in this step, or dtxt_acc at
 // W = 1) that enters the first fold, and G0.0 adds the positive-pair term of all B rows to dtxt. With one panel the
@@ -1769,12 +1771,14 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
   for (int k = 1; k < W; ++k) {
     const int cidx = step_owner(c, r, k);
     const __nv_bfloat16* txt_c = c->txt_all + cidx * stride;
-   for (int p = 0; p < np; ++p) {
+   for (int q = 0; q < np; ++q) {
+    const int p = (k == W - 1) ? (q + 1) % np : q;   // the last chunk: panels 1 .. np-1, then 0
+    const bool first_p = q == 0, last_p = q == np - 1;
     const int p0 = p * P;
     {
       AuxList aux;
-      if (p == 0) add_cvt_jobs(c, aux, 1, k == 1 && img_cvt_in_l1 && moved_to_l1, img, txt_c, c->Ts[cidx]);
-      if (p == 0 && k == 1 && l0_work_in_l1 && moved_to_l1) {
+      if (first_p) add_cvt_jobs(c, aux, 1, k == 1 && img_cvt_in_l1 && moved_to_l1, img, txt_c, c->Ts[cidx]);
+      if (first_p && k == 1 && l0_work_in_l1 && moved_to_l1) {
         add_cvt_jobs(c, aux, 0, false, img, reinterpret_cast<const __nv_bfloat16*>(txt), c->T);
         siglip::AuxJob& w3 = aux.add(siglip::kAuxWaitOnly);
         w3.wait_flags = c->flags + 3 * kMaxWorld;
@@ -1782,8 +1786,8 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
         w3.wait_value = n - 1;
         w3.site = 13;
       }
-      if (p == 0 && k + 1 < W) add_pull_job(c, aux, step_owner(c, r, k + 1), s);
-      const bool lastL = (k == W - 1) && (p == np - 1);
+      if (first_p && k + 1 < W) add_pull_job(c, aux, step_owner(c, r, k + 1), s);
+      const bool lastL = (k == W - 1) && last_p;
       EndSignal end = (lastL && ik) ? end_signal(c, 2, s) : EndSignal();   // "I have pulled everyone's text"
       Window w;
       w.r0 = p0;
@@ -1801,9 +1805,9 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
     o.dimg_out = rows_final ? dimg : static_cast<void*>(c->dimg_acc);
     o.dimg_bf16 = rows_final && c->grad_bf16;
     o.dtxt_out = c->slots + cidx * stride;
-    o.dtxt_add = (p > 0) ? c->slots + cidx * stride : nullptr;   // the chunk's earlier panels
+    o.dtxt_add = first_p ? nullptr : c->slots + cidx * stride;   // the chunk's earlier panels
     AuxList aux;
-    if (j >= 2 && p == 0) {
+    if (j >= 2 && first_p) {
       const int pr = ((r - step_offset(c, j - 1)) % W + W) % W;
       siglip::AuxJob& f = aux.add(siglip::kAuxFold);
       f.src = reinterpret_cast<const uint4*>(c->peer_slots[pr] + r * stride);
@@ -1816,7 +1820,7 @@ int fused_impl(siglip_ctx* c, const void* img, const void* txt, const float* t_p
       f.site = 7;
     }
     // "my contribution to owner cidx is complete": its last panel only
-    const bool lastG = p == np - 1;
+    const bool lastG = last_p;
     EndSignal end = (ik && lastG) ? end_signal(c, 1, base + static_cast<unsigned int>(j)) : EndSignal();
     GradPanel gp;
     gp.r0 = p0;
@@ -3276,6 +3280,20 @@ int siglip_scale(siglip_ctx* c, const void* src, void* dst, size_t nbytes, int i
 
 unsigned long long siglip_ctx_launch_count(const siglip_ctx* c) { return c ? c->launches : 0ull; }
 
+int siglip_debug_max_active_clusters(int device, int cta_group, int mcast, int tile_n, int stages) {
+  if (cta_group != 1 && cta_group != 2) return -fail(SIGLIP_ERR_INVALID, "cta_group must be 1 or 2");
+  if (mcast != 1 && mcast != 2) return -fail(SIGLIP_ERR_INVALID, "mcast must be 1 or 2");
+  if (tile_n != siglip::kTileCols && tile_n != siglip::kWideTileCols)
+    return -fail(SIGLIP_ERR_INVALID, "tile_n must be 128 or 256");
+  if (stages != 0 && stages != 4 && stages != 6) return -fail(SIGLIP_ERR_INVALID, "stages must be 0 (default), 4 or 6");
+  if (siglip_device_count() == 0) return -fail(SIGLIP_ERR_NO_DEVICE, "no sm_90 device; no CPU fallback");
+  if (cudaSetDevice(device) != cudaSuccess) return -fail(SIGLIP_ERR_CUDA, "cudaSetDevice failed");
+  const int n = siglip::query_max_active_clusters(siglip::cluster_size(cta_group, mcast), tile_n,
+                                                  stages > 0 ? stages : siglip::default_stages(siglip::kModeOut));
+  if (n < 1) return -fail(SIGLIP_ERR_CUDA, "cannot read the device's multiprocessor count");
+  return n;
+}
+
 int siglip_debug_gemm(int device, int cta_group, int M, int N, int K, const void* A, long long lda, int a_mn,
                       const void* Bm, long long ldb, int b_mn, float* C, long long ldc, void* cuda_stream) {
   return siglip_debug_gemm_timed(device, cta_group, M, N, K, A, lda, a_mn, Bm, ldb, b_mn, C, ldc, 1, nullptr,
@@ -3341,18 +3359,18 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
+  const char* env_st = getenv("SIGLIP_DEBUG_STAGES");
+  const int stages = env_st ? atoi(env_st) : 0;
+  if (stages != 0 && stages != 4 && stages != 6) return fail(SIGLIP_ERR_INVALID, "SIGLIP_DEBUG_STAGES must be 4 or 6");
   int lrc = 0;
   unsigned long long* wstats = nullptr;
   if (getenv("SIGLIP_DEBUG_WAITSTATS")) {
     printf("[waitstats cg=%d] max co-resident clusters: %d (SMs %d)\n", cta_group,
-           siglip::query_max_active_clusters(siglip::cluster_size(cta_group, mcast)), num_sms);
+           siglip::query_max_active_clusters(siglip::cluster_size(cta_group, mcast), tile_n, stages), num_sms);
     CK(cudaMalloc(reinterpret_cast<void**>(&wstats), 8 * 256 * sizeof(unsigned long long)));
     CK(cudaMemsetAsync(wstats, 0, 8 * 256 * sizeof(unsigned long long), st));
     p.wait_stats = wstats;
   }
-  const char* env_st = getenv("SIGLIP_DEBUG_STAGES");
-  const int stages = env_st ? atoi(env_st) : 0;
-  if (stages != 0 && stages != 4 && stages != 6) return fail(SIGLIP_ERR_INVALID, "SIGLIP_DEBUG_STAGES must be 4 or 6");
   if (iters > 1)  // warm-up
     lrc = siglip::launch_gemm(cta_group, siglip::kModeOut, stages, mcast, tile_n, &tmA, &tmB, &tmA, &tmB, &tmA, p,
                               num_sms, st);

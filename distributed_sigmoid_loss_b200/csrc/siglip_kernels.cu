@@ -2852,33 +2852,52 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
 
 }  // namespace
 
-int query_max_active_clusters(int cluster) {
-  int n = -1, dev = 0, num_sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess ||
-      cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-    return n;
+namespace {
+// The persistent grid's cluster count of one out-kernel instantiation, as launch_impl derives it: the runtime's
+// co-resident clusters (num_sms / kCS when the query fails), at most num_sms / kCS.
+template <int kStages, int kCS, int kTileNT = kTileN>
+int out_kernel_clusters(int num_sms) {
+  auto kern = siglip_gemm_kernel<kModeOut, kStages, kCS, false, false, false, false, kTileNT>;
+  const int smem = Cfg<kModeOut, kStages, kTileNT>::kSmemBytes;
   cudaLaunchConfig_t cfg{};
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cluster;
+  attr[0].val.clusterDim.x = kCS;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   cfg.blockDim = dim3(kNumThreads);
-  cfg.gridDim = dim3((num_sms / cluster) * cluster);
-  cfg.dynamicSmemBytes = Cfg<kModeOut, 6>::kSmemBytes;
-  auto query = [&](auto kern) {
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cfg.dynamicSmemBytes);
-    cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
-  };
-  if (cluster == 4)
-    query(siglip_gemm_kernel<kModeOut, 6, 4>);
-  else if (cluster == 2)
-    query(siglip_gemm_kernel<kModeOut, 6, 2>);
-  else
-    query(siglip_gemm_kernel<kModeOut, 6, 1>);
-  return n;
+  cfg.gridDim = dim3((num_sms / kCS) * kCS);
+  cfg.dynamicSmemBytes = smem;
+  int n = 0;
+  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess ||
+      cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) {
+    cudaGetLastError();
+    n = num_sms / kCS;
+  }
+  return n < num_sms / kCS ? n : num_sms / kCS;
+}
+}  // namespace
+
+int query_max_active_clusters(int cluster, int tile_n, int stages) {
+  int dev = 0, num_sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return -1;
+  if (tile_n == kWideTileN) {   // every stage request maps to kWideStages, as in launch_gemm
+    if (cluster == 4) return out_kernel_clusters<kWideStages, 4, kWideTileN>(num_sms);
+    if (cluster == 2) return out_kernel_clusters<kWideStages, 2, kWideTileN>(num_sms);
+    return out_kernel_clusters<kWideStages, 1, kWideTileN>(num_sms);
+  }
+  if (stages == 4) {
+    if (cluster == 4) return out_kernel_clusters<4, 4>(num_sms);
+    if (cluster == 2) return out_kernel_clusters<4, 2>(num_sms);
+    return out_kernel_clusters<4, 1>(num_sms);
+  }
+  if (cluster == 4) return out_kernel_clusters<6, 4>(num_sms);
+  if (cluster == 2) return out_kernel_clusters<6, 2>(num_sms);
+  return out_kernel_clusters<6, 1>(num_sms);
 }
 
 int default_stages(int /*mode*/) { return 6; }

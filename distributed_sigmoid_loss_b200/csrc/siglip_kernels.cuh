@@ -256,7 +256,10 @@ inline int b_box_k_mnmajor(int cs, int tile_n = kTileCols) { return (cs == 4 && 
 // Dynamic shared memory needed by the default configuration of `mode`.
 size_t gemm_smem_bytes(int mode);
 int default_stages(int mode);
-int query_max_active_clusters(int cluster);  // co-resident clusters of the out kernel (diagnostic)
+// Clusters of the persistent grid of the out kernel with `cluster` CTAs per cluster, tile_n columns (kTileCols or
+// kWideTileCols) and `stages` (4, else 6; the wide tiles always have kWideStages): what launch_impl launches
+// (diagnostics and tests). -1 without a device.
+int query_max_active_clusters(int cluster, int tile_n = kTileCols, int stages = 6);
 
 // Launch the warp-specialised persistent kernel. `stages` <= 0 selects the default pipeline depth (4 or 6).
 // tmG: store map of the sigma operand (loss mode; 16-bit [B, B], box {32, 16}, 64B swizzle) — any valid map in out mode.

@@ -632,6 +632,15 @@ unsigned long long siglip_ctx_launch_count(const siglip_ctx* ctx);
 int siglip_debug_gemm(int device, int cta_group, int M, int N, int K, const void* A, long long lda, int a_mn,
                       const void* Bm, long long ldb, int b_mn, float* C, long long ldc, void* cuda_stream);
 
+/*
+ * Test hook: clusters of the persistent grid that a gradient-kernel launch (SIGLIP_OPT_CTA_GROUP cta_group,
+ * SIGLIP_OPT_MCAST mcast, column tiles tile_n = 128 or 256, SIGLIP_OPT_STAGES_GRAD stages = 0, 4 or 6; 256-column
+ * tiles always run 4 stages) gets on `device`: the runtime's co-resident clusters of that instantiation, at most
+ * SMs / cluster size. Split-K (SIGLIP_OPT_SPLIT_K) cuts the ragged last wave of that grid. Returns the count, or minus
+ * the status code.
+ */
+int siglip_debug_max_active_clusters(int device, int cta_group, int mcast, int tile_n, int stages);
+
 /* Same contraction launched `iters` times back to back (after one warm-up when iters > 1); *ms_per_iter receives
  * the CUDA-event time per launch. Used to tune the mainloop apart from the loss epilogue. */
 int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, const void* A, long long lda, int a_mn,

@@ -1063,17 +1063,20 @@ def test_peer_timeout_option_and_trace_hook():
 # ---------------------------------------------------------------------------------------------------------
 # split-K of the gradient kernel's ragged last wave; fp8 (wgmma e4m3) measurement path
 # ---------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("shape", [(4096, 768), (1000, 136), (2048, 1152), (520, 264), (8192, 768)])
+# Each shape leaves a ragged last wave that splits at cta_group 1 and 2 under every request here (S = 2 .. 4 on an H100
+# SXM: 132 single-CTA or 66 two-CTA co-resident clusters); tests/test_gpu_grad_matrix.py derives the split per cell
+@pytest.mark.parametrize("shape", [(3000, 384), (1000, 136), (2048, 1152), (1100, 264), (2200, 1024)])
 @pytest.mark.parametrize("cg", [1, 2])
 def test_split_k_is_deterministic_and_matches_unsplit(shape, cg):
     """SIGLIP_OPT_SPLIT_K: the tiles of a ragged last wave are cut into K-slices whose fp32 partial accumulators meet in
     a workspace and are added in slice order — bitwise repeatable, and equal to the unsplit result up to fp32
-    summation order."""
+    summation order. The unsplit run keeps the split's 128-column tiles, so that different bits prove a split."""
     from distributed_sigmoid_loss_b200 import _capi
     B, D = shape
     img, txt = _synth(B, D, seed=13)
     tp, b = _scal(math.log(10.0)), _scal(-10.0)
     eng = _engine(B, D, cg)
+    eng.set_option(_capi.SIGLIP_OPT_GRAD_TILE_N, 128)
     out = {}
     for sk in (0, -1, 2, 3):
         eng.set_option(_capi.SIGLIP_OPT_SPLIT_K, sk)
@@ -1087,6 +1090,7 @@ def test_split_k_is_deterministic_and_matches_unsplit(shape, cg):
     for sk in (-1, 2, 3):
         _check(f"dimg split {sk}", out[sk][0], out[0][0], tol=2e-6)
         _check(f"dtxt split {sk}", out[sk][1], out[0][1], tol=2e-6)
+        assert not torch.equal(out[sk][1], out[0][1]), f"split {sk}: the bits of the unsplit step, nothing was split"
     with pytest.raises(RuntimeError):
         eng.set_option(_capi.SIGLIP_OPT_SPLIT_K, 1)
     eng.close()
