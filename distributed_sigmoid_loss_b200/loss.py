@@ -20,7 +20,7 @@ import torch
 import torch.distributed as dist
 import torch.nn as nn
 
-from . import _capi
+from . import _capi, cross_node
 
 # Largest K of the top-K in-batch retrieval (SIGLIP_TOPK_MAX in include/siglip_b200.h)
 TOPK_MAX = 10
@@ -54,12 +54,15 @@ class SigmoidLossEngine:
     def __init__(self, batch: int, dim: int, device: torch.device, group=None, cta_group: int = 2,
                  overlap_pull: bool = True, rank_world: Optional[Tuple[int, int]] = None, loopback: bool = False,
                  batch_per_rank=None, texts_per_rank=None, images_per_rank=None, teacher_dim: int = 0,
-                 labels: int = 0, distill_options: bool = False):
+                 labels: int = 0, distill_options: bool = False, node_base: int = 0):
         self._L = _capi.lib()
         if not torch.cuda.is_available() or self._L.siglip_device_count() == 0:
             raise RuntimeError("distributed_sigmoid_loss_b200 needs an sm_90 (H100) device; there is no CPU fallback")
         self.batch, self.dim, self.device, self.group = batch, dim, torch.device(device), group
         self.rank, self.world = rank_world if rank_world is not None else _group_rank_world(group)
+        # a node context of a group that spans nodes: its ranks are group ranks node_base .. node_base + world - 1
+        self.node_base = int(node_base)
+        self.topology = None   # cross_node.Topology of such a context (set by the engine cache)
         h = ctypes.c_void_p()
         self.teacher_dim = int(teacher_dim)
         self.labels = int(labels)   # labels per set of a label-set engine (siglip_ctx_create_labels), 0: none
@@ -172,9 +175,11 @@ class SigmoidLossEngine:
         n = int(self._L.siglip_ctx_handle_bytes())
         buf = ctypes.create_string_buffer(n)
         _capi.check(self._L.siglip_ctx_export_handles(self._h, buf, n))
-        blobs = [None] * self.world
+        # gathered over the whole group (no sub-group to create); a node context keeps its node's blobs, in node-rank
+        # order
+        blobs = [None] * dist.get_world_size(self.group)
         dist.all_gather_object(blobs, bytes(buf.raw), group=self.group)
-        joined = b"".join(blobs)
+        joined = b"".join(blobs[self.node_base:self.node_base + self.world])
         _capi.check(self._L.siglip_ctx_import_handles(self._h, joined, n))
         dist.barrier(group=self.group)
 
@@ -642,6 +647,7 @@ class SigmoidLossEngine:
                      dimg_host: Optional[torch.Tensor] = None, dtxt_host: Optional[torch.Tensor] = None):
         """End-to-end step on HOST bf16 buffers (pinned recommended): H2D, step, D2H inside one C call.
         Returns (loss, dt_prime, dbias) as Python floats."""
+        self._refuse_host_across_nodes()
         self._check_host(img_host, txt_host)
         out = (ctypes.c_float * 3)()
         loss_p = ctypes.cast(out, ctypes.c_void_p).value
@@ -660,6 +666,7 @@ class SigmoidLossEngine:
         `dtxt_host` (CPU bf16 [B, D], pinned recommended) are given, of its bf16 gradients on a second copy stream;
         returns a ticket for ``host_wait``. At most two steps in flight; the host tensors must stay alive until the
         ticket is waited."""
+        self._refuse_host_across_nodes()
         self._check_host(img_host, txt_host)
         if (dimg_host is None) != (dtxt_host is None):
             raise RuntimeError("give both gradient host buffers or neither")
@@ -679,6 +686,11 @@ class SigmoidLossEngine:
         p = ctypes.cast(out, ctypes.c_void_p).value
         _capi.check(self._L.siglip_host_wait(self._h, ticket, p, p + 4, p + 8))
         return float(out[0]), float(out[1]), float(out[2])
+
+    def _refuse_host_across_nodes(self) -> None:
+        if self.topology is not None:
+            raise RuntimeError("the host-buffer entries are unavailable across nodes: the remote texts travel as "
+                               "device tensors of the module's forward")
 
     def _check_host(self, img_host: torch.Tensor, txt_host: torch.Tensor) -> None:
         for x in (img_host, txt_host):
@@ -928,8 +940,12 @@ class _EngineCache:
                  bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
                  extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
                  distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None,
-                 exclude_groups: bool = False, multi_label: int = 0, focal=None, distill_options: bool = False):
+                 exclude_groups: bool = False, multi_label: int = 0, focal=None, distill_options: bool = False,
+                 ranks_per_node: Optional[int] = None):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
+        self.ranks_per_node = ranks_per_node
+        self._topology = None   # cross_node.Topology of a group that spans nodes, found when the first engine is built
+        self._topology_known = False
         self.distill_options = distill_options
         self.focal = focal   # (gamma, alpha or None), or None
         self.exclude_groups = exclude_groups
@@ -950,6 +966,10 @@ class _EngineCache:
         eng = self._engines.get(key)
         if eng is None:
             dev = torch.device("cuda", key[0])
+            if not self._topology_known:
+                self._topology = cross_node.topology(self.group, self.ranks_per_node)
+                self._topology_known = True
+            topo = self._topology
             tpr = ipr = None
             extras = self.hard_negatives + self.extra_texts   # at most one of the two is non-zero
             rank, world = _group_rank_world(self.group)
@@ -960,10 +980,13 @@ class _EngineCache:
             if self.extra_images:
                 # every rank holds the same number K of extra images: R_p = B_p + K
                 ipr = [int(b) + self.extra_images for b in bpr]
-            eng = SigmoidLossEngine(batch, dim, dev, self.group, self.cta_group, self.overlap_pull,
-                                    batch_per_rank=self.batch_per_rank, texts_per_rank=tpr, images_per_rank=ipr,
-                                    teacher_dim=teacher_dim, labels=self.multi_label,
-                                    distill_options=self.distill_options and teacher_dim > 0)
+            if topo is None:
+                eng = SigmoidLossEngine(batch, dim, dev, self.group, self.cta_group, self.overlap_pull,
+                                        batch_per_rank=self.batch_per_rank, texts_per_rank=tpr, images_per_rank=ipr,
+                                        teacher_dim=teacher_dim, labels=self.multi_label,
+                                        distill_options=self.distill_options and teacher_dim > 0)
+            else:
+                eng = self._node_engine(topo, batch, dim, dev, [int(b) for b in bpr], extras, teacher_dim)
             if self.sync_scalar_grads:
                 eng.set_option(_capi.SIGLIP_OPT_SYNC_SCALAR_GRADS, 1)
             if self.bidir:
@@ -972,8 +995,9 @@ class _EngineCache:
                 eng.set_option(_capi.SIGLIP_OPT_SAMPLE_IDS, 1)
             if self.multi_label:
                 eng.set_option(_capi.SIGLIP_OPT_LABEL_SETS, 1)
-            if self.extra_texts and not self.multi_label:
-                eng.set_option(_capi.SIGLIP_OPT_EXTRA_TEXT_IDS, 1)   # needs the sample ids on first
+            if (self.extra_texts and not self.multi_label) or (topo is not None and self.multi_positive):
+                # needs the sample ids on first; across nodes the remote rows carry their owners' ids
+                eng.set_option(_capi.SIGLIP_OPT_EXTRA_TEXT_IDS, 1)
             if self.extra_images and self.multi_positive:
                 eng.set_option(_capi.SIGLIP_OPT_EXTRA_IMAGE_IDS, 1)
             if self.sample_weights:
@@ -988,6 +1012,24 @@ class _EngineCache:
             if self.sigma_budget_bytes:
                 eng.set_sigma_budget(self.sigma_budget_bytes)
             self._engines[key] = eng
+        return eng
+
+    def _node_engine(self, topo, batch: int, dim: int, dev: torch.device, bpr, extras: int,
+                     teacher_dim: int) -> SigmoidLossEngine:
+        """The context of this rank's node in a group that spans nodes: local rank l of L, every local rank holding its
+        own texts and those of its counterparts on the other nodes (cross_node)."""
+        cross_node.check_options(self.distill, self.multi_positive, self.hard_negatives)
+        if len(bpr) != topo.world:
+            raise RuntimeError(f"batch_per_rank {bpr} must list one batch per rank of the group ({topo.world})")
+        group_tpr = [b + extras for b in bpr]
+        base, L = topo.node_base, topo.ranks_per_node
+        node_bpr = bpr[base:base + L]
+        ipr = [b + self.extra_images for b in node_bpr] if self.extra_images else None
+        eng = SigmoidLossEngine(batch, dim, dev, self.group, self.cta_group, self.overlap_pull,
+                                rank_world=(topo.local, L), batch_per_rank=node_bpr,
+                                texts_per_rank=topo.node_texts_per_rank(group_tpr), images_per_rank=ipr,
+                                teacher_dim=teacher_dim, labels=self.multi_label, node_base=base)
+        eng.topology, eng.group_texts_per_rank = topo, group_tpr
         return eng
 
 
@@ -1470,6 +1512,56 @@ def _validate(image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, exp
         raise RuntimeError("distributed_sigmoid_loss_b200 runs on CUDA (sm_90a) tensors only; there is no CPU path")
 
 
+def _node_step(mod, eng, text, t_prime, bias, sync_scalars: bool, ids, extra_ids, weights, groups, label_sets):
+    """The inputs of a node context's step in a group that spans nodes (eng.topology set): this rank's text rows
+    [T, D] (captions, then extras) followed by its counterparts' rows, and the per-text data that rides with them:
+    the owners' ids (captions' sample ids, extra texts' ids) as extra-text ids, their text weights, text groups and
+    label sets (hard negatives: empty sets). Images and their data stay on their rank. Returns (text, t_prime, bias,
+    extra_ids, weights, groups, label_sets) for _SigmoidLossFn; t_prime / bias pass through the exchange so that
+    sync_scalar_grads averages their gradients over the nodes."""
+    topo, tpr, group = eng.topology, eng.group_texts_per_rank, eng.group
+    rows, B = text.shape[0], eng.batch
+    cols = []
+    if mod.multi_positive:
+        cols.append(ids if extra_ids is None else torch.cat([ids, extra_ids]))
+    if weights is not None:
+        tw = weights[1] if weights[1] is not None else torch.ones(rows, device=text.device, dtype=torch.float32)
+        cols.append(tw.view(torch.int32).to(torch.int64))   # the fp32 bits, exactly
+    if groups is not None:
+        cols.append(groups[1])
+    cols = [c.reshape(rows, 1) for c in cols]
+    if label_sets is not None:
+        ls, lt, li = label_sets
+        if lt is None:
+            lt = torch.full((rows - B, ls.shape[1]), -1, device=ls.device, dtype=torch.int64)
+        cols.append(torch.cat([ls, lt]))
+    text, t_prime, bias = cross_node.exchange_texts(text, t_prime, bias, topo, tpr, group, sync_scalars)
+    if cols:
+        own = torch.cat(cols, dim=1)
+        both = torch.cat([own, cross_node.send_rows(own, topo, tpr, group)])
+        c = 0
+        if mod.multi_positive:
+            extra_ids = both[B:, 0].contiguous()
+            c += 1
+        if weights is not None:
+            weights = (weights[0], both[:, c].to(torch.int32).view(torch.float32).contiguous())
+            c += 1
+        if groups is not None:
+            groups = (groups[0], both[:, c].contiguous())
+            c += 1
+        if label_sets is not None:
+            label_sets = (label_sets[0], both[B:, c:].contiguous(), label_sets[2])
+    return text, t_prime, bias, extra_ids, weights, groups, label_sets
+
+
+def _fold_text_loss(eng, lbufs, rows: int):
+    """Per-sample losses of a node context: text_loss of the own rows plus the other nodes' values for them."""
+    if lbufs is None or eng.topology is None:
+        return lbufs
+    tl = lbufs[1]
+    return lbufs[0], cross_node.return_rows(tl[rows:], tl[:rows], eng.topology, eng.group_texts_per_rank, eng.group)
+
+
 def _pad_dim(x: torch.Tensor) -> torch.Tensor:
     """Zero-pad the embedding dimension to a multiple of 8 (16-byte rows for TMA). Zero columns change no dot product;
     F.pad is differentiable, so the gradient comes back sliced to the caller's width."""
@@ -1489,10 +1581,21 @@ class DDPSigmoidLoss(nn.Module):
     the reference is, so ``torch.amp.GradScaler`` skips the step of a tower that overflowed under autocast.
     Every rank of ``group`` must call ``forward`` the same number of times (collective, like all_gather).
 
-    Limits (also reported by the C library when violated): all ranks of ``group`` must be GPUs of ONE node with NVLink /
-    P2P access to each other (the exchange is CUDA-IPC peer memory, not NCCL), at most 32 ranks; give a multi-node job a
-    per-node ``group``. A rank waiting for a peer inside a kernel gives up after ``SIGLIP_PEER_TIMEOUT_MS`` (default
-    10 minutes).
+    Limits (also reported by the C library when violated): the in-kernel exchange reaches the GPUs of ONE node with
+    NVLink / P2P access to each other (CUDA-IPC peer memory, not NCCL), at most 32 ranks per node; a group that spans
+    nodes goes through ``ranks_per_node`` below. A rank waiting for a peer inside a kernel gives up after
+    ``SIGLIP_PEER_TIMEOUT_MS`` (default 10 minutes).
+
+    ``ranks_per_node=L``: a ``group`` that spans nodes, each node a block of L consecutive ranks (rank g = n·L + l);
+    None derives L from the ranks' hostnames once, when the first engine is built (an error when one host's ranks are
+    not consecutive or the nodes differ in size). Every rank still gets the loss, gradients, ``t_prime.grad`` /
+    ``bias.grad`` and per-sample losses of the global batch: rank (n, l) scores the texts of ranks (n', l) of the other
+    nodes as extras of its node's context, moved by an ``all_to_all_single`` over ``group`` (NCCL or gloo) whose
+    backward returns their gradients, added in node order. Ids, text weights, text groups and label sets travel with
+    the texts. ``sync_scalar_grads`` averages over every rank of ``group``. ``text_loss`` adds the nodes' values in node
+    order in fp32: deterministic, not bitwise the one-node value. Across nodes ``return_metrics`` / ``metrics_topk``,
+    ``distill``, ``hard_negatives`` with ``multi_positive`` and the host-buffer entries are refused. L equal to the
+    group's size is the single-node path. Collective: every rank passes the same L.
 
     ``multi_positive=True``: every ``forward`` takes ``sample_ids`` ([B] integers, one per sample on this rank), and a pair
     is positive iff its image and text carry the same id — on any rank (repeated captions, several captions of one
@@ -1619,9 +1722,10 @@ class DDPSigmoidLoss(nn.Module):
                  distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None,
                  exclude_groups: bool = False, multi_label: Optional[int] = None,
                  focal_gamma: Optional[float] = None, focal_alpha: Optional[float] = None,
-                 distill_options: bool = False) -> None:
+                 distill_options: bool = False, ranks_per_node: Optional[int] = None) -> None:
         super().__init__()
         _sigma_budget_mib(sigma_budget_bytes)
+        ranks_per_node = cross_node.validate_ranks_per_node(ranks_per_node)
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_images = _validate_hard_negatives(extra_images, "extra_images")
         # distill_closed: what the option checks refuse, distill=lambda without distill_options (None otherwise)
@@ -1670,7 +1774,7 @@ class DDPSigmoidLoss(nn.Module):
                                    extra_texts=extra_texts, sample_weights=sample_weights, extra_images=extra_images,
                                    distill=distill, sigma_budget_bytes=sigma_budget_bytes,
                                    exclude_groups=exclude_groups, multi_label=multi_label, focal=focal,
-                                   distill_options=distill_options)
+                                   distill_options=distill_options, ranks_per_node=ranks_per_node)
         # extension: bound of the 16-bit sigma operands; steps then run in row panels (memory O(budget), not O(B^2))
         self.sigma_budget_bytes = sigma_budget_bytes
 
@@ -1721,14 +1825,20 @@ class DDPSigmoidLoss(nn.Module):
         image_embeddings, text_embeddings = _pad_dim(image_embeddings), _pad_dim(text_embeddings)
         eng = self._cache.get(self.gpu_batch_size, image_embeddings.shape[1], image_embeddings.device,
                               teacher[0].shape[1] if teacher is not None else 0)
+        t_prime, bias, rows = self.t_prime, self.bias, text_embeddings.shape[0]
+        if eng.topology is not None:
+            cross_node.check_forward(return_metrics)
+            text_embeddings, t_prime, bias, extra_ids, weights, groups, label_sets = _node_step(
+                self, eng, text_embeddings, t_prime, bias, self.sync_scalar_grads, ids, extra_ids, weights, groups,
+                label_sets)
         fused = _fused_under_budget(eng, self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
         bufs = _topk_buffers(eng, topk, bufs)
         lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
-        loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, self.t_prime, self.bias, eng,
+        loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, t_prime, bias, eng,
                                     self.normalize_inputs, fused, ids, bufs, extra_ids, weights, ximg_ids, teacher,
                                     lbufs, groups, label_sets)
-        return _with_outputs(loss, bufs, lbufs)
+        return _with_outputs(loss, bufs, _fold_text_loss(eng, lbufs, rows))
 
 
 SigmoidLoss = DDPSigmoidLoss
@@ -1758,7 +1868,9 @@ class SigLipLoss(nn.Module):
     [B + K], and same-group pairs that are not positives are excluded from the loss, as in ``DDPSigmoidLoss``.
     ``multi_label=M``: every forward takes ``sample_labels`` [B, M] (and ``extra_text_labels`` / ``extra_image_labels``
     [K, M] with ``extra_texts`` / ``extra_images``), and pairs whose label sets meet are positives, as in
-    ``DDPSigmoidLoss``. ``focal_gamma`` / ``focal_alpha``: the focal pair loss of ``DDPSigmoidLoss``."""
+    ``DDPSigmoidLoss``. ``focal_gamma`` / ``focal_alpha``: the focal pair loss of ``DDPSigmoidLoss``.
+    ``ranks_per_node``: a group that spans nodes, with the global-batch loss, as in ``DDPSigmoidLoss``; ``rank`` and
+    ``world_size`` are then the rank and size of the whole group."""
 
     def __init__(self, cache_labels: bool = False, rank: int = 0, world_size: int = 1, bidir: bool = True,
                  use_horovod: bool = False, group=None, cta_group: int = 2, fused_step: Optional[bool] = None,
@@ -1766,9 +1878,11 @@ class SigLipLoss(nn.Module):
                  sample_weights: bool = False, extra_images: int = 0, distill: Optional[float] = None,
                  sigma_budget_bytes: Optional[int] = None, exclude_groups: bool = False,
                  multi_label: Optional[int] = None, focal_gamma: Optional[float] = None,
-                 focal_alpha: Optional[float] = None, distill_options: bool = False):
+                 focal_alpha: Optional[float] = None, distill_options: bool = False,
+                 ranks_per_node: Optional[int] = None):
         super().__init__()
         _sigma_budget_mib(sigma_budget_bytes)
+        ranks_per_node = cross_node.validate_ranks_per_node(ranks_per_node)
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
         hard_negatives = _validate_hard_negatives(hard_negatives)
         extra_images = _validate_hard_negatives(extra_images, "extra_images")
@@ -1796,7 +1910,7 @@ class SigLipLoss(nn.Module):
                                    hard_negatives=hard_negatives, extra_texts=extra_texts, sample_weights=sample_weights,
                                    extra_images=extra_images, distill=distill, sigma_budget_bytes=sigma_budget_bytes,
                                    exclude_groups=exclude_groups, multi_label=multi_label, focal=focal,
-                                   distill_options=distill_options)
+                                   distill_options=distill_options, ranks_per_node=ranks_per_node)
         # bound of the 16-bit sigma operands; steps then run in row panels (as on DDPSigmoidLoss)
         self.sigma_budget_bytes = sigma_budget_bytes
 
@@ -1840,12 +1954,19 @@ class SigLipLoss(nn.Module):
         image_features, text_features = _pad_dim(image_features), _pad_dim(text_features)
         eng = self._cache.get(batch, image_features.shape[1], image_features.device,
                               teacher[0].shape[1] if teacher is not None else 0)
-        if (eng.rank, eng.world) != (self.rank, self.world_size):
+        topo = eng.topology
+        rank_world = (eng.rank, eng.world) if topo is None else (topo.rank, topo.world)
+        if rank_world != (self.rank, self.world_size):
             raise RuntimeError(
                 f"SigLipLoss(rank={self.rank}, world_size={self.world_size}) does not match the process group "
-                f"(rank={eng.rank}, world_size={eng.world})")
+                f"(rank={rank_world[0]}, world_size={rank_world[1]})")
         if logit_bias is None:
             logit_bias = torch.zeros((), device=image_features.device)
+        rows = text_features.shape[0]
+        if topo is not None:
+            cross_node.check_forward(return_metrics)
+            text_features, logit_scale, logit_bias, extra_ids, weights, groups, label_sets = _node_step(
+                self, eng, text_features, logit_scale, logit_bias, False, ids, extra_ids, weights, groups, label_sets)
         fused = _fused_under_budget(eng, self.fused_step)
         bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
         bufs = _topk_buffers(eng, topk, bufs)
@@ -1853,4 +1974,4 @@ class SigLipLoss(nn.Module):
         loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs,
                                     extra_ids, weights, ximg_ids, teacher, lbufs, groups, label_sets)
         out = {"contrastive_loss": loss} if output_dict else loss
-        return _with_outputs(out, bufs, lbufs)
+        return _with_outputs(out, bufs, _fold_text_loss(eng, lbufs, rows))
