@@ -17,7 +17,10 @@ the excluded pairs carry weight while a flipped label still moves a step's loss 
 set holds the sample's id and a few tags of a small pool (not the groups: a positive is never excluded). The teacher's
 rows are an integer vector per teacher key plus sparse noise, the key being the id except that ids 2k + 1 share 2k's:
 at t_T = 6, b_T = -10 its p is ~0.97 on the pairs with one key and ~1e-4 elsewhere, a sharp teacher (a low entropy
-floor under the loss) that knows matches the labels do not."""
+floor under the loss) that knows matches the labels do not.
+
+That data never votes the loss epilogue's series path (every free slab holds some z above kFastZ). COLD runs the same
+rows on planted_cold's data, where most slabs do (tests/slab_paths.py models each slab's path; cell_slabs applies it)."""
 from __future__ import annotations
 
 import dataclasses
@@ -153,6 +156,7 @@ class Cell:
     cg: int
     mcast: int
     seed: int
+    cold: bool = False   # planted_cold's data: the series path's family
 
     @property
     def mode(self) -> str:
@@ -172,7 +176,8 @@ class Cell:
         on += [f"k{o.topk}"] if o.topk else []
         return (f"{self.seed:03d}-{self.mode}-{o.context}-{'+'.join(on) or 'none'}-W{self.W}r{self.r}"
                 f"{'-bidir' if self.bidir else ''}-{self.sched}{'-panels' if self.panels else ''}"
-                f"{'-f16' if self.f16 else ''}-t{self.tile_n}-s{self.stages}-cg{self.cg}m{self.mcast}")
+                f"{'-f16' if self.f16 else ''}-t{self.tile_n}-s{self.stages}-cg{self.cg}m{self.mcast}"
+                f"{'-cold' if self.cold else ''}")
 
     def shapes(self):
         """(Bs, Rs, Ts) of every rank, as the step sees them."""
@@ -194,6 +199,15 @@ class Cell:
             if rows and rp * nbuf * tp * 2 > mib * 2 ** 20 and Rs[self.r] > rows:
                 return mib
         raise AssertionError(f"{self.name}: no budget splits the rows into panels")
+
+    def panel_rows(self) -> int:
+        """The rows of the step's panels under budget_mib() (sigma_panels): all R_r rows without panels."""
+        Bs, Rs, Ts = self.shapes()
+        if not self.panels:
+            return Rs[self.r]
+        unit = 128 * self.cluster
+        P = self.budget_mib() * 2 ** 20 // ((2 if self.W > 1 else 1) * _round_up(max(Ts), 256) * 2) // unit * unit
+        return min(P, Rs[self.r])
 
 
 def _round_up(x, m):
@@ -228,30 +242,35 @@ def route(cell: Cell):
     the positives). sets is on for every chunk of a label-set step. A teacher step also records the context it runs in
     (distill_extras_context): the distill-extras workspace puts the gathered teacher text, and what follows it, at other
     offsets, so the same kModeDistill branch reads different addresses there."""
+    return {chunk_route(cell, c) for c in range(cell.W)}
+
+
+def own_pos_ids(cell: Cell) -> bool:
+    """The rank holds extras of both kinds: its own chunk takes its positional positives from iota ids."""
+    Bs, Rs, Ts = cell.shapes()
+    return Rs[cell.r] > Bs[cell.r] and Ts[cell.r] > Bs[cell.r]
+
+
+def chunk_route(cell: Cell, c: int):
+    """The (instantiation, runtime options) of the loss launches over text chunk c (route)."""
     o = cell.opts
     mode = mode_of(o)
     stages = DISTILL_STAGES if mode in ("distill", "distill_opts") else cell.stages
-    Bs, Rs, Ts = cell.shapes()
-    own_pos_ids = Rs[cell.r] > Bs[cell.r] and Ts[cell.r] > Bs[cell.r]
-    out = set()
-    for c in range(cell.W):
-        ids = True if o.ids else ("iota" if c == cell.r and own_pos_ids else False)
-        if mode == "loss":
-            out.add(((mode, stages, cell.cluster, ids, o.keys, o.weights), ()))
-            continue
-        rt = dict(ids=ids, weights=o.weights, metrics=o.keys)
-        if mode in ("topk", "groups") + SET_MODES:
-            rt["losses"] = o.losses
-        if mode in ("groups",) + SET_MODES:
-            rt["topk"] = o.topk > 1
-        if mode in SET_MODES:
-            rt["groups"] = o.groups
-        if mode in ("focal", "distill_opts"):
-            rt["sets"] = bool(o.labels)
-        if o.teacher:
-            rt["extras_ctx"] = distill_extras_context(cell)
-        out.add(((mode, stages, cell.cluster), tuple(sorted(rt.items()))))
-    return out
+    ids = True if o.ids else ("iota" if c == cell.r and own_pos_ids(cell) else False)
+    if mode == "loss":
+        return (mode, stages, cell.cluster, ids, o.keys, o.weights), ()
+    rt = dict(ids=ids, weights=o.weights, metrics=o.keys)
+    if mode in ("topk", "groups") + SET_MODES:
+        rt["losses"] = o.losses
+    if mode in ("groups",) + SET_MODES:
+        rt["topk"] = o.topk > 1
+    if mode in SET_MODES:
+        rt["groups"] = o.groups
+    if mode in ("focal", "distill_opts"):
+        rt["sets"] = bool(o.labels)
+    if o.teacher:
+        rt["extras_ctx"] = distill_extras_context(cell)
+    return (mode, stages, cell.cluster), tuple(sorted(rt.items()))
 
 
 def distill_extras_context(cell: Cell) -> bool:
@@ -348,12 +367,17 @@ def _lru_pick(order, ok):
     return v
 
 
-def build_table() -> List[Cell]:
+def build_table(cold: bool = False) -> List[Cell]:
+    """The cells of every row of _mode_rows. cold: the same rows on planted_cold's data (seeds from COLD_SEED), without
+    kModeDistill's rows for the other contexts: they run its branches again, and the cold family is the minimal cover of
+    the instantiations and runtime combinations."""
     cells, counters = [], {}
     for seed, (mode, f, stages, cs) in enumerate(_mode_rows()):
         j = counters.setdefault(mode, [0, {}])
         i, cyc = j[0], j[1]
         j[0] += 1
+        if cold and mode == "distill" and i >= len(runtime_combos(mode)):
+            continue
         ids = f.get("ids", False)
         sets = mode == "labels" or f.get("sets", False)
         W = (1, 2, 3)[i % 3]
@@ -374,6 +398,10 @@ def build_table() -> List[Cell]:
         metrics = f.get("metrics", False)
         M = _lru_pick(cyc.setdefault("M", list(range(1, MMAX + 1))), lambda m: True) if sets else 0
         focal = _lru_pick(cyc.setdefault("focal", list(FOCALS)), lambda x: True) if mode == "focal" else None
+        if cold and focal is not None:
+            # gamma >= 2 leaves a series slab's terms below 2e-4 of every output and its sigma * 2^14 among fp16's
+            # subnormals, where the 16-bit operand, not the path, sets the error: the cold family runs gamma = 0.5
+            focal = (0.5, focal[1])
         o = Options(ids=ids, xtexts=ctx in ("hn", "xt", "both"), ximages=ctx in ("xi", "xin", "both"),
                     xt_ids=ids and ctx in ("xt", "both"), xi_ids=ids and ctx in ("xi", "both"),
                     labels=M, xt_sets=sets and ctx in ("xt", "both"), xi_sets=sets and ctx in ("xi", "both"),
@@ -387,11 +415,13 @@ def build_table() -> List[Cell]:
                           1 if metrics and mode in ("loss", "sample_loss") and i % 2 else 0))
         assert o.valid() and mode_of(o) == mode, o
         cells.append(Cell(o, W, i % W, W > 1 and (i // 3) % 2 == 1, sched, panels, (i + i // 4) % 2 == 1,
-                          (128, 256)[(i // 2 + i // 8) % 2], stages, cg, mcast, seed))
+                          (128, 256)[(i // 2 + i // 8) % 2], stages, cg, mcast, seed + COLD_SEED * cold, cold))
     return cells
 
 
+COLD_SEED = 500
 TABLE = build_table()
+COLD = build_table(cold=True)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -448,6 +478,8 @@ class Problem:
 
 
 def planted(cell: Cell) -> Problem:
+    if cell.cold:
+        return planted_cold(cell)
     Bs, K, E = (PANEL_SHAPES if cell.panels else SHAPES)[cell.W]
     Rs = tuple(b + e for b, e in zip(Bs, E))
     Ts = tuple(b + k for b, k in zip(Bs, K))
@@ -504,6 +536,140 @@ def planted(cell: Cell) -> Problem:
         P["timgs"].append(np.concatenate([tnear(ids), tnear(xi_content)]))
         P["ttxts"].append(np.concatenate([tnear(ids), tnear(xt)]))
     return Problem(Bs, Rs, Ts, **P)
+
+
+# Cold data: integer rows / 8, so U = 64 <img, txt> is an integer and z = 5 U / 64 - 6 (U < 23.04: z < kFastZ).
+COLD_BAND = 32                   # the first rows of each paired batch: duplicate ids, shared tags and groups
+COLD_POOL = 24                   # the ids of the bands
+COLD_SIG, COLD_COMMON = 96, 104  # dims [0, 96): a sample's signature, [96, 104): common to all, [104, D): planted pairs
+COLD_TSIG = 56                   # teacher dims [0, 56): signature, [56, DT): planted slabs
+COLD_TARGETS = (24, 36, 23)      # U of the planted pairs: just above kFastZ (-4.125), warm (-3.19), just below (-4.203)
+COLD_TEACHER_U = 96              # added to U_T over a planted teacher slab: z_T ~ -1, p ~ 0.27
+
+
+def planted_cold(cell: Cell) -> Problem:
+    """The cold family's data: most negatives at z ~ -6.2 .. -4.6, so that the series slabs carry a large part of the
+    loss, the gradients and each sample's loss. A sample is a signature of 32 entries +-1 over 96 dims (the one of its id,
+    so positives and extras with a band id have U = 40, z = -2.9) plus 8 common dims (U = 8 between all rows). Duplicate
+    ids, label-set tags and groups lie in the first COLD_BAND rows of each paired batch only, every other sample has an
+    id of its own; a half of the extras caption a band id. Then, against each chunk, rank r gets planted negatives of
+    U in COLD_TARGETS off the bands (one dim of their own each): general slabs off the diagonal and series slabs whose
+    max z lies 3e-3 below kFastZ, where the series truncation is largest. The teacher's rows are a signature of 6 entries
+    +-4 (z_T = -1 on pairs of one id, below -5.5 elsewhere) and, on some whole slabs of rank r, U_T + COLD_TEACHER_U:
+    a teacher that knows matches the labels do not, in slabs whose student votes either way. Weights as planted's."""
+    Bs, K, E = (PANEL_SHAPES if cell.panels else SHAPES)[cell.W]
+    Rs = tuple(b + e for b, e in zip(Bs, E))
+    Ts = tuple(b + k for b, k in zip(Bs, K))
+    g = np.random.default_rng(1000 + cell.seed)
+    sig, tsig = {}, {}
+    fresh = iter(range(10 ** 5, 10 ** 6))
+
+    def rows(idv):
+        out = np.zeros((len(idv), D), np.int64)
+        for n, k in enumerate(idv):
+            if k not in sig:
+                v = np.zeros(COLD_SIG, np.int64)
+                v[g.choice(COLD_SIG, 32, replace=False)] = g.choice([-1, 1], 32)
+                sig[k] = v
+            out[n, :COLD_SIG] = sig[k]
+        out[:, COLD_SIG:COLD_COMMON] = 1
+        return out
+
+    def trows(idv):
+        out = np.zeros((len(idv), DT), np.int64)
+        for n, k in enumerate(idv):
+            if k not in tsig:
+                v = np.zeros(COLD_TSIG, np.int64)
+                v[g.choice(COLD_TSIG, 6, replace=False)] = g.choice([-4, 4], 6)
+                tsig[k] = v
+            out[n, :COLD_TSIG] = tsig[k]
+        return out
+
+    def weights(n):
+        w = g.random(n).astype(np.float32)
+        w[g.random(n) < 0.2] = 0.0
+        return w
+
+    def band_or_fresh(n):
+        return np.array([g.integers(0, COLD_POOL) if g.random() < 0.5 else next(fresh) for _ in range(n)], np.int64)
+
+    P = dict(imgs=[], txts=[], ids=[], xt_ids=[], xi_ids=[], iw=[], tw=[], ig=[], tg=[], itags=[], ttags=[], timgs=[],
+             ttxts=[])
+    for b, r_, t_ in zip(Bs, Rs, Ts):
+        nb = min(COLD_BAND, b)
+        ids = np.concatenate([g.integers(0, COLD_POOL, nb), [next(fresh) for _ in range(b - nb)]]).astype(np.int64)
+        xt, xi_content = band_or_fresh(t_ - b), band_or_fresh(r_ - b)
+        xi = xi_content.copy()
+        new = g.random(r_ - b) < 0.2
+        xi[new] = 10 ** 6 + g.integers(0, 10 ** 6, int(new.sum()))
+        band = np.arange(b) < nb
+        grp = np.where(band, ids % 3, -1)
+        tags = np.where(band[:, None] & (g.random((b, MMAX)) < 0.3), 10 ** 7 + g.integers(0, 3, (b, MMAX)), -1)
+        P["ids"].append(ids)
+        P["xt_ids"].append(xt)
+        P["xi_ids"].append(xi)
+        P["imgs"].append(rows(np.concatenate([ids, xi_content])))
+        P["txts"].append(rows(np.concatenate([ids, xt])))
+        P["iw"].append(weights(r_))
+        P["tw"].append(weights(t_))
+        P["ig"].append(np.concatenate([grp, np.full(r_ - b, -1)]).astype(np.int64))
+        P["tg"].append(np.concatenate([grp, np.full(t_ - b, -1)]).astype(np.int64))
+        P["itags"].append(np.concatenate([tags, np.full((r_ - b, MMAX), -1)]).astype(np.int64))
+        P["ttags"].append(np.concatenate([tags, np.full((t_ - b, MMAX), -1)]).astype(np.int64))
+        P["timgs"].append(trows(np.concatenate([ids, xi_content])))
+        P["ttxts"].append(trows(np.concatenate([ids, xt])))
+    r, R = cell.r, Rs[cell.r]
+    img, timg = P["imgs"][r], P["timgs"][r]
+    n, nt = (D - COLD_COMMON) // cell.W, (DT - COLD_TSIG) // cell.W
+
+    def off_diagonal(c, i0, j0):   # not a slab on the own diagonal (slab_paths.classes)
+        return c != r or i0 // 128 != j0 // 128 or not (i0 < j0 + 32 and j0 < i0 + 16)
+
+    for c in range(cell.W):
+        txt, ttxt, T = P["txts"][c], P["ttxts"][c], Ts[c]
+        pairs = []
+        for k in range(n):
+            i = COLD_BAND + (k * (R - COLD_BAND)) // n + int(g.integers(0, (R - COLD_BAND) // n))
+            j = int(g.integers(COLD_BAND, T))
+            while not off_diagonal(c, i // 16 * 16, j // 32 * 32):
+                j = int(g.integers(COLD_BAND, T))
+            d = COLD_COMMON + c * n + k
+            img[i, d], txt[j, d] = 1, COLD_TARGETS[k % 3] - int(img[i] @ txt[j])
+            pairs.append((i // 16 * 16, j // 32 * 32))
+        for k in range(nt):
+            if k % 2 == 0:   # the slab of a planted pair: the student's vote goes either way
+                i0, j0 = pairs[k]
+            else:
+                i0, j0 = 16 * int(g.integers(COLD_BAND // 16, R // 16)), 32 * int(g.integers(COLD_BAND // 32, T // 32))
+                while not off_diagonal(c, i0, j0):
+                    j0 = 32 * int(g.integers(COLD_BAND // 32, T // 32))
+            d = COLD_TSIG + c * nt + k
+            timg[i0:i0 + 16, d], ttxt[j0:j0 + 32, d] = 8, COLD_TEACHER_U // 8
+    for key in ("imgs", "txts", "timgs", "ttxts"):
+        P[key] = [x / 8.0 for x in P[key]]
+    return Problem(Bs, Rs, Ts, **P)
+
+
+def cell_slabs(cell: Cell, P: Problem) -> List[Tuple[Tuple, "slab_paths.SlabMap"]]:
+    """(chunk_route, SlabMap) of every loss launch of rank r's step (slab_paths.windows): the slabs' classes from the
+    oracle's labels and the fp32 votes of the student (and of a teacher) on the planted logits."""
+    import slab_paths
+
+    o, r = cell.opts, cell.r
+    Bs, Rs, Ts, imgs, txts = P.view(o)
+    lab = labels(P, o)[r]
+    timgs, ttxts = P.teacher(o) if o.teacher else (None, None)
+    out = []
+    for c in range(cell.W):
+        route_c = chunk_route(cell, c)
+        for r0, rows, c0, cols, own in slab_paths.windows(Rs[r], Bs[r], Ts[c], c == r, own_pos_ids(cell),
+                                                          cell.panel_rows()):
+            win = (slice(r0, r0 + rows), slice(c0, c0 + cols))
+            s = imgs[r][win[0]] @ txts[c][win[1]].T
+            ts = timgs[r][win[0]] @ ttxts[c][win[1]].T if o.teacher else None
+            out.append((route_c, slab_paths.slab_map(s, lab[c][win], own, TP, BIAS, cell.f16, ts, TTP, TBIAS, c, r0,
+                                                      c0)))
+    return out
 
 
 # ---------------------------------------------------------------------------------------------------------------------

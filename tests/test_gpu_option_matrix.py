@@ -16,7 +16,10 @@ and every option but the focal terms, against float64 autograd.
 Observed on one H100 80GB HBM3 (700 W power limit): 424 tests (333 cells, their panel families and 14 module cases) in
 about 7 to 8.5 min of wall time; the largest relative errors, all within the 1e-3 tolerance: loss 6.3e-5, the cells' dimg
 and dtxt (own chunk and peer slots) 4.5e-4, dt' 9.5e-5, dbias 2.8e-4, per-sample losses of 1e-6 and above 3.3e-4;
-the modules' bf16 gradients 2.7e-3 (their tolerance: 4e-3)."""
+the modules' bf16 gradients 2.7e-3 (their tolerance: 4e-3). With the 328 cold cells (om.COLD, whose launches run the
+series path), on the same card at 700 W: 753 tests in 8 min 21 s of wall time; the cold cells' largest relative errors:
+loss 3.2e-7, dimg 4.2e-4, dtxt (own chunk and peer slots) 3.5e-4, dt' 5.9e-5, dbias 5.7e-5, per-sample losses of 1e-6
+and above 3.0e-5."""
 import dataclasses
 
 import numpy as np
@@ -43,7 +46,8 @@ def _report():
         print(f"option matrix: largest relative error of {k}: {OBSERVED[k]:.3e}")
 
 
-def _note(kind, err):
+def _note(kind, err, tag=""):
+    kind = ("cold cells: " if tag.endswith("-cold") or "-cold " in tag else "") + kind
     OBSERVED[kind] = max(OBSERVED.get(kind, 0.0), err)
 
 
@@ -57,7 +61,7 @@ def _scal(x):
 
 def _check(name, got, ref, tol=om.TOL):
     err = _rel(got, ref)
-    _note("dtxt (own chunk and peer slots)" if "chunk" in name else name.rsplit(" ", 1)[1], err)
+    _note("dtxt (own chunk and peer slots)" if "chunk" in name else name.rsplit(" ", 1)[1], err, name)
     assert err <= tol, f"{name}: relative error {err:.3e}"
 
 
@@ -72,7 +76,7 @@ def _check_sample_losses(tag, got, want, zero, words):
         assert zero.any() and (g[zero] == 0).all(), f"{tag}: a weight-0 sample is not exactly 0"
     big = w >= 1e-6
     if big.any():
-        _note(f"{tag.rsplit(' ', 1)[1]} (samples >= 1e-6)", float(np.max(np.abs(g - w)[big] / w[big])))
+        _note(f"{tag.rsplit(' ', 1)[1]} (samples >= 1e-6)", float(np.max(np.abs(g - w)[big] / w[big])), tag)
     excess = np.abs(g - w) - (om.TOL * w + words * WORD)
     assert excess.max() <= 0, f"{tag}: sample {int(excess.argmax())} {g[excess.argmax()]:.6e} vs {w[excess.argmax()]:.6e}"
 
@@ -299,7 +303,7 @@ def _run(cell, **variant):
     return RESULTS[key]
 
 
-@pytest.mark.parametrize("cell", om.TABLE, ids=lambda c: c.name)
+@pytest.mark.parametrize("cell", om.TABLE + om.COLD, ids=lambda c: c.name)
 def test_cell_matches_the_composed_oracle(cell):
     _run(cell)
 

@@ -2,8 +2,11 @@
 non-distillation option on, with the focal terms and every other non-teacher option, and with a teacher and every option
 but the focal terms; its reduction to the single-feature oracles; every cell's sensitivity to each option it turns on;
 the table's coverage of the loss kernel's instantiations and runtime branches; the table's modes against the loss modes
-launch_gemm dispatches to; and the exactness of the planted logits."""
+launch_gemm dispatches to; the exactness of the planted logits; and the series path: the slab model of
+tests/slab_paths.py, the cold family's coverage of every instantiation and runtime combination in series slabs, and
+each cold cell's sensitivity to a bug local to its series slabs."""
 import dataclasses
+import functools
 import math
 import pathlib
 import re
@@ -13,6 +16,7 @@ import pytest
 import torch
 
 import option_matrix as om
+import slab_paths as sp
 from distill_oracle import closed_form_distill
 from distill_options_oracle import closed_form_distill_options
 from exclude_groups_oracle import closed_form_groups, group_labels, torch_loss, torch_terms
@@ -402,3 +406,299 @@ def test_planted_operands_and_logits_are_exact(W, panels):
     z = math.exp(om.TP) * (P.imgs[0] @ P.txts[0].T) + om.BIAS
     same = P.ig[0][:, None] == P.tg[0][None, :]
     assert (1 / (1 + np.exp(-z[(lab < 0) & same]))).mean() > 0.1
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the series path: the slab model (tests/slab_paths.py) and the cold family
+# ---------------------------------------------------------------------------------------------------------------------
+@functools.lru_cache(maxsize=None)
+def _slabs(cell):
+    return om.cell_slabs(cell, om.planted(cell))
+
+
+def _student_series(cell, m):
+    """The slabs of a launch whose student takes the series path (any class in the teacher modes)."""
+    return m.series if cell.opts.teacher else m.series & (m.cls == sp.FREE)
+
+
+def test_slab_classes_hold_exactly_the_special_elements():
+    """The model's classes against the kernel's geometry (test_protocol_model's slab-class test on the 16 x 32 slabs):
+    every element past the matrix lies in an edge slab and only edge slabs hold one; every own positional positive lies
+    in a diag slab, which only a diagonal 128 x 128 tile holds; positives and excluded pairs never lie in a free slab."""
+    g = np.random.default_rng(3)
+    for M, N in [(300, 337), (128, 128), (136, 200), (520, 600), (40, 24), (257, 129)]:
+        for own in (False, True):
+            y = np.where(g.random((M, N)) < 0.002, 1, np.where(g.random((M, N)) < 0.002, 0, -1))
+            cls = sp.classes(M, N, own, y)
+            nb, nc = cls.shape
+            assert (nb, nc) == (-(-M // 16), -(-N // 32))
+            for b in range(nb):
+                for c in range(nc):
+                    masked = b * 16 + 16 > M or c * 32 + 32 > N
+                    assert (cls[b, c] == sp.EDGE) == masked
+                    on_diag = own and any(b * 16 + i == c * 32 + j for i in range(16) for j in range(32)
+                                          if b * 16 + i < M and c * 32 + j < N)
+                    if on_diag and not masked:
+                        assert cls[b, c] == sp.DIAG and (b * 16) // 128 == (c * 32) // 128
+                    if cls[b, c] == sp.DIAG:
+                        assert on_diag
+                    blk = y[b * 16:b * 16 + 16, c * 32:c * 32 + 32]
+                    if (blk >= 0).any():
+                        assert cls[b, c] != sp.FREE
+
+
+def test_slab_votes_are_the_kernels_fp32_votes():
+    """fmaf(max s, t_eff, bias) in fp32 with t_eff = expf(t') (bf16) or expf(t') / 256 on 256 s (fp16(16 x)): the same
+    value; a slab's elements past the matrix read s = 0 (z = bias); the series path iff the vote is below kFastZ."""
+    s = np.full((20, 40), 23 / 64.0)
+    s[3, 5] = 24 / 64.0
+    m = sp.slab_map(s, -np.ones_like(s), False, om.TP, om.BIAS)
+    assert m.z[0, 0] == np.float32(np.float32(5.0) * np.float32(24 / 64.0) + np.float32(-6.0))
+    assert m.z[0, 0] > sp.FAST_Z and m.z[0, 1] < sp.FAST_Z and m.z[0, 1] == np.float32(5 * 23 / 64 - 6)
+    assert np.array_equal(m.z, sp.slab_map(s, -np.ones_like(s), False, om.TP, om.BIAS, f16=True).z)
+    assert m.cls[1, 0] == sp.EDGE and m.cls[0, 1] == sp.EDGE and m.cls[0, 0] == sp.FREE
+    t = sp.slab_map(-np.ones((20, 40)), -np.ones((20, 40)), False, om.TP, om.BIAS)
+    assert t.z[1, 1] == np.float32(om.BIAS) and t.z[0, 0] == np.float32(-11.0)
+    assert list(m.student_path(False)[0]) == ["general", "general"] and list(t.student_path(True)[0]) == ["series"] * 2
+
+
+def test_slab_fast_fraction_of_the_trained_regime_is_the_models():
+    """trained_regime.slab_fast_fraction counts the free slabs of slab_paths, the same as a direct float64 count."""
+    from trained_regime import REGIMES, make_batch, pair_terms, slab_fast_fraction
+
+    R = REGIMES["trained"]
+    imgs, texts, _, _ = make_batch(R, (160, 96), (40, 0), 64, 5, "hn")
+    fast = total = 0
+    for r, row in enumerate(pair_terms(imgs, texts, R.t_prime, R.bias)):
+        for c, x in enumerate(row):
+            z = math.exp(R.t_prime) * x["s"] + R.bias
+            M, N = z.shape
+            for b in range(0, M - 15, 16):
+                for c0 in range(0, N - 31, 32):
+                    if r == c and b < c0 + 32 and c0 < b + 16 or (x["y"][b:b + 16, c0:c0 + 32] > 0).any():
+                        continue
+                    total += 1
+                    fast += z[b:b + 16, c0:c0 + 32].max() < -4.2
+    assert slab_fast_fraction(imgs, texts, R.t_prime, R.bias) == (fast / total, total)
+    assert 0 < fast < total
+
+
+def test_row_panel_windows_tile_the_step():
+    """slab_paths.windows restates run_fwd_bwd's loss launches: every element of every chunk is scored once, the own
+    chunk's positional diagonal only in launches that carry own_chunk, and a window's origin is a multiple of 128."""
+    for cell in [c for c in om.TABLE + om.COLD if c.panels][:12] + om.COLD[:6]:
+        Bs, Rs, Ts = cell.shapes()
+        r = cell.r
+        for c in range(cell.W):
+            seen = np.zeros((Rs[r], Ts[c]), int)
+            diag = np.zeros(Rs[r], bool)
+            for r0, rows, c0, cols, own in sp.windows(Rs[r], Bs[r], Ts[c], c == r, om.own_pos_ids(cell),
+                                                      cell.panel_rows()):
+                assert r0 % 128 == 0 and c0 % 128 == 0
+                seen[r0:r0 + rows, c0:c0 + cols] += 1
+                if own:
+                    i = np.arange(r0, r0 + rows)
+                    diag[i[(i >= c0) & (i < c0 + cols)]] = True
+            assert (seen == 1).all(), cell.name
+            assert diag[:Bs[r]].all() == (c == r and not om.own_pos_ids(cell)), cell.name
+        assert cell.panel_rows() < Rs[r] if cell.panels else cell.panel_rows() == Rs[r]
+
+
+def test_warm_cells_run_no_series_slab():
+    """The planted data of the table's cells (t = 5, bias = -6, group centres and duplicate ids) never votes the
+    student's series path: what the cold family is for. (The teacher's vote does go either way there.)"""
+    series = {}
+    for cell in om.TABLE:
+        for _, m in _slabs(cell):
+            series[cell.mode] = series.get(cell.mode, 0) + int((m.series & (m.cls == sp.FREE)).sum())
+    assert series == {m: 0 for m in om.MODES}, series
+
+
+def _cold_items(cell):
+    """What a cold cell covers, each only where its launches run series slabs and general slabs off the diagonal:
+    its instantiations and runtime combinations (iota ids and a teacher's context apart: the coverage's fine items),
+    the student x teacher vote pairs of its free slabs, and its schedule, row panels, INPUT_F16 and peer chunks."""
+    out = set()
+    by_route = {}
+    for rt, m in _slabs(cell):
+        free = m.cls == sp.FREE
+        a = by_route.setdefault(rt, np.zeros(2, int))
+        a += [int(_student_series(cell, m).sum()), int((free & ~m.series).sum())]
+        if cell.opts.teacher:
+            for sv in (False, True):
+                for tv in (False, True):
+                    if (free & (m.series == sv) & (m.tseries == tv)).any():
+                        out.add(("votes", cell.mode, sv, tv))
+        if m.chunk != cell.r and _student_series(cell, m).any() and (free & ~m.series).any():
+            out.add(("peer chunk", cell.W))
+    for (inst, rt), (n_series, n_general) in by_route.items():
+        if n_series and n_general:
+            out.add(("instantiation", inst))
+            out.add(("branch", inst[0], rt))
+            out.update([("sched", cell.sched), ("panels", cell.panels), ("f16", cell.f16)])
+    return out
+
+
+def test_cold_cells_cover_every_instantiation_and_branch_in_series_slabs():
+    """Every loss-kernel instantiation and every runtime combination runs in a cold cell whose launches of it hold
+    series slabs and general slabs off the diagonal; the teacher modes run every student x teacher vote pair in free
+    slabs; the cold cells run each schedule, row panels, INPUT_F16 and peer chunks at W = 2 and 3 that way; every vote
+    is at least slab_paths.MARGIN from kFastZ, and some series slabs have their max z just below it, some general slabs
+    just above. pytest -s prints how many cold-cell slabs take each path, per mode."""
+    items = set().union(*(_cold_items(c) for c in om.COLD))
+    inst = {x[1] for x in items if x[0] == "instantiation"}
+    inst = {tuple(bool(v) if k == 3 else v for k, v in enumerate(i)) for i in inst}
+    combos = {(x[1], _branch(x[1], x[2], False)) for x in items if x[0] == "branch"}
+    need_i, need_c, _ = _required()
+    assert need_i <= inst, f"instantiations without series slabs: {sorted(need_i - inst)}"
+    assert need_c <= combos, f"runtime combinations without series slabs: {sorted(need_c - combos)}"
+    for mode in ("distill", "distill_opts"):
+        for sv in (False, True):
+            for tv in (False, True):
+                assert ("votes", mode, sv, tv) in items, (mode, sv, tv)
+    for x in [("sched", s) for s in om.SCHEDS] + [("panels", True), ("f16", True), ("peer chunk", 2),
+                                                   ("peer chunk", 3)]:
+        assert x in items, x
+    counts, near = {}, [0, 0]
+    for cell in om.COLD:
+        for _, m in _slabs(cell):
+            assert m.min_margin(cell.opts.teacher) >= sp.MARGIN, cell.name
+            ser = _student_series(cell, m)
+            gen = (m.cls == sp.FREE) & ~m.series
+            near[0] += int((ser & (m.z > sp.FAST_Z - 0.01)).sum())
+            near[1] += int((gen & (m.z < sp.FAST_Z + 0.1)).sum())
+            c = counts.setdefault(cell.mode, {k: 0 for k in ("series", "general off the diagonal") + sp.CLASSES[:-1]})
+            c["series"] += int(ser.sum())
+            c["general off the diagonal"] += int(gen.sum())
+            for k in sp.CLASSES[:-1]:
+                c[k] += int((m.cls == k).sum())
+    assert near[0] > 0 and near[1] > 0, near
+    for mode, c in counts.items():
+        print(f"cold cells, {mode}: " + ", ".join(f"{k} {v}" for k, v in c.items()))
+
+
+def test_no_cold_cell_is_redundant():
+    """Each cold cell is the only one that covers some item of _cold_items (iota ids apart from sample ids, a teacher's
+    context apart): removing one from the family loses series-path coverage."""
+    per = [_cold_items(c) for c in om.COLD]
+    for k, cell in enumerate(om.COLD):
+        rest = set().union(*(per[:k] + per[k + 1:]))
+        assert per[k] - rest, f"{cell.name} covers nothing no other cold cell covers"
+
+
+def _series_variants(cell):
+    """The variants of the sensitivity test: the step with one thing done wrong in its series slabs only. 'series terms':
+    the slabs' terms dropped; 'row weight' / 'column weight': a unit image / text weight; 'row sums' / 'column sums': the
+    slabs' terms left out of the per-sample losses; 'gamma' / 'alpha': the focal terms without gamma / alpha; 'target':
+    the teacher's soft target q replaced by the hard label; 'INPUT_F16 scale': t_eff off by 2^1."""
+    o = cell.opts
+    out = ["series terms"]
+    out += ["row weight", "column weight"] if o.weights else []
+    out += ["row sums", "column sums"] if o.losses else []
+    out += ["gamma"] + (["alpha"] if o.focal[1] is not None else []) if o.focal else []
+    out += ["target"] if o.teacher else []
+    out += ["INPUT_F16 scale"] if cell.f16 else []
+    return out
+
+
+def _rank_outputs(cell, P, S, res):
+    """Rank r's checked outputs by float64 autograd of its pair terms over the whole text set, with a variant applied to
+    the elements in S ([R_r, sum T] bool): a function of the variant (None: the step as it is) giving loss, dimg, dt',
+    dbias, contrib<c>, image_loss and text_loss (every rank's column sums of the own chunk: the other ranks' parts from
+    the oracle's res)."""
+    o, r = cell.opts, cell.r
+    Bs, Rs, Ts, imgs, txts = P.view(o)
+    T64 = functools.partial(torch.tensor, dtype=torch.float64)
+    F = torch.nn.functional
+    y = torch.from_numpy(np.concatenate(om.labels(P, o)[r], axis=1))
+    txt = np.concatenate(txts)
+    s0 = imgs[r] @ txt.T
+    one = torch.ones(1, dtype=torch.float64)
+    iw = T64(P.iw[r][:Rs[r]]) if o.weights else one
+    tw = T64(np.concatenate([x[:n] for x, n in zip(P.tw, Ts)])) if o.weights else one
+    p = None
+    if o.teacher:
+        timgs, ttxts = P.teacher(o)
+        p = torch.sigmoid(math.exp(om.TTP) * T64(timgs[r] @ np.concatenate(ttxts).T) + om.TBIAS)
+    Sm = torch.from_numpy(S)
+    lo = np.cumsum([0] + list(Ts))
+    gamma, alpha = o.focal if o.focal else (0.0, None)
+
+    def evaluate(variant=None):
+        s = T64(s0, requires_grad=True)
+        tp, b = T64(om.TP, requires_grad=True), T64(om.BIAS, requires_grad=True)
+
+        def terms(tp_=tp, iw_=iw, tw_=tw, gamma=gamma, alpha=alpha, teacher=o.teacher):
+            z = torch.exp(tp_) * s + b
+            w = y.abs() * iw_[:, None] * tw_[None, :]
+            if o.focal is not None:
+                m = torch.where(y > 0, -z, z)
+                a = 1.0 if alpha is None else torch.where(y > 0, alpha, 1.0 - alpha).to(z.dtype)
+                return w * a * torch.exp(-gamma * F.softplus(-m)) * F.softplus(m)
+            if teacher:
+                return w * (F.softplus(z) - ((1.0 - om.LAM) * (y > 0).double() + om.LAM * p) * z)
+            return w * F.softplus(-torch.where(y == 0, -torch.ones_like(y), y) * z)
+
+        full = terms()
+        wrong = {"series terms": lambda: torch.zeros_like(full), "row weight": lambda: terms(iw_=one),
+                 "column weight": lambda: terms(tw_=one), "gamma": lambda: terms(gamma=0.0),
+                 "alpha": lambda: terms(alpha=None), "target": lambda: terms(teacher=False),
+                 "INPUT_F16 scale": lambda: terms(tp_=tp + math.log(2.0))}
+        summed = torch.where(Sm, wrong[variant](), full) if variant in wrong else full
+        loss = summed.sum() / Bs[r]
+        gs, gt, gb = torch.autograd.grad(loss, [s, tp, b])
+        gs = gs.numpy()
+        out = {"loss": loss.item(), "dimg": gs @ txt, "dt_prime": float(gt), "dbias": float(gb)}
+        out.update({f"contrib{c}": gs[:, lo[c]:lo[c + 1]].T @ imgs[r] for c in range(cell.W)})
+        t = summed.detach()   # the per-sample sums add the same terms (lrow / lcol)
+        rows = torch.where(Sm, 0.0, t) if variant == "row sums" else t
+        cols = torch.where(Sm, 0.0, t) if variant == "column sums" else t
+        out["image_loss"] = rows.sum(axis=1).numpy()
+        out["text_loss"] = res[r]["text_loss"] - res[r]["text_part"][r] + cols[:, lo[r]:lo[r + 1]].sum(axis=0).numpy()
+        return out
+
+    return evaluate
+
+
+def _moved(cell, key, a, b):
+    """How far a variant moves an output, in units of what the GPU test allows: the norm-and-max error over 1e-3; for
+    the per-sample losses the largest per-sample error past the fixed-point words' resolution, over 1e-3 relative."""
+    if key not in ("image_loss", "text_loss"):
+        return om.rel(a, b) / om.TOL
+    Bs, Rs, Ts = cell.shapes()
+    words = sum((t + 127) // 128 + 1 for t in Ts) if key == "image_loss" else (Rs[cell.r] + 15) // 16 + cell.W
+    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
+    return float(np.max((np.abs(a - b) - words * 2.0 ** -32) / (om.TOL * np.abs(b) + 1e-300)))
+
+
+@pytest.mark.parametrize("cell", om.COLD, ids=lambda c: c.name)
+def test_a_series_path_bug_moves_what_the_cell_checks(cell):
+    """For each thing the series path computes in the cell (its terms, each weight, each per-sample sum, the focal
+    gamma and alpha, a teacher's target, the INPUT_F16 scale), the step with that done wrong in its series slabs only
+    moves an output the GPU test checks by more than 20x its tolerance. The restatement here is the composed oracle
+    (the same outputs to 1e-10), so a bug local to the series path of any instantiation fails the GPU test. One
+    exception: a teacher cell that checks its loss alone sees the INPUT_F16 scale off by 2 at 8x its tolerance or more
+    only (its soft targets' -q z terms move little), which the cells with gradients cover; and a text's loss holds the
+    terms of every rank, so at W > 1 a column-sum bug of this rank's series slabs moves it by 10x or more."""
+    P = om.planted(cell)
+    Bs, Rs, Ts, _, _ = P.view(cell.opts)
+    S = [np.zeros((Rs[cell.r], t), bool) for t in Ts]
+    for _, m in _slabs(cell):
+        S[m.chunk][m.r0:m.r0 + m.rows, m.c0:m.c0 + m.cols] |= m.elements(_student_series(cell, m))
+    S = np.concatenate(S, axis=1)
+    assert S.any()
+    res = om.oracle(P, cell.opts)
+    checked = list(_outputs(cell, res, cell.r))
+    evaluate = _rank_outputs(cell, P, S, res)
+    full = evaluate()
+    for k in ("loss", "dimg", "dt_prime", "dbias", "image_loss", "text_loss"):
+        assert om.rel(full[k], res[cell.r][k]) < 1e-10, k
+    weak = []
+    for v in _series_variants(cell):
+        got = evaluate(v)
+        moved = max(_moved(cell, k, got[k], full[k]) for k in checked)
+        if moved <= (10 if v == "column sums" and cell.W > 1 else 20):
+            weak.append(f"{v}: {moved:.1f}x")
+    if cell.opts.teacher and cell.sched == "fwd":
+        weak = [w for w in weak if not w.startswith("INPUT_F16")]
+    assert not weak, f"{cell.name}: a series-path bug moves its checked outputs by {weak} of the tolerance only"

@@ -31,8 +31,6 @@ import torch
 
 from oracle.siglip_oracle import _sigmoid
 
-SLAB_ROWS, SLAB_COLS = 16, 32      # the loss kernel's epilogue slab: a warp's 16-row band x 32 columns
-FAST_Z = -4.2                      # kFastZ: a slab whose every z is below it takes the series path
 SIGMA_NORMAL_MIN = 2.0 ** -28      # 3.7e-9: sigma * 2^14 below fp16's smallest normal 2^-14 (z < -19.4)
 
 
@@ -284,23 +282,18 @@ def split_own_diagonal(imgs, texts, t_prime: float, bias: float, iws=None, tws=N
 
 def slab_fast_fraction(imgs, texts, t_prime: float, bias: float, labels=None) -> Tuple[float, int]:
     """Fraction of the 16x32 slabs (kernel geometry: 16-row bands x 32 columns of each rank-by-chunk block) whose max z
-    is below FAST_Z, i.e. that take the series path, among the slabs whose path depends on z at all: slabs touching the
+    is below kFastZ, i.e. that take the series path, among the slabs whose path depends on z at all: slabs touching the
     own diagonal, crossing the border of the block, or holding a positive pair take the label-applying path whatever z
-    is and are left out. Returns (fraction, number of slabs counted)."""
-    t = math.exp(t_prime)
+    is and are left out (tests/slab_paths.py's free slabs). Returns (fraction, number of slabs counted)."""
+    from slab_paths import FREE, slab_map
+
     fast = total = 0
     for r, row in enumerate(pair_terms(imgs, texts, t_prime, bias, labels=labels)):
         for c, x in enumerate(row):
-            z, y = t * x["s"] + bias, x["y"]
-            M, N = z.shape
-            for r0 in range(0, M - SLAB_ROWS + 1, SLAB_ROWS):
-                for c0 in range(0, N - SLAB_COLS + 1, SLAB_COLS):
-                    if r == c and r0 < c0 + SLAB_COLS and c0 < r0 + SLAB_ROWS:
-                        continue
-                    if (y[r0:r0 + SLAB_ROWS, c0:c0 + SLAB_COLS] > 0).any():
-                        continue
-                    total += 1
-                    fast += int(z[r0:r0 + SLAB_ROWS, c0:c0 + SLAB_COLS].max() < FAST_Z)
+            m = slab_map(x["s"], x["y"], r == c, t_prime, bias)
+            free = m.cls == FREE
+            total += int(free.sum())
+            fast += int((free & m.series).sum())
     return fast / max(total, 1), total
 
 
