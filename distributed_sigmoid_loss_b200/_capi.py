@@ -79,6 +79,7 @@ EXPORTED_SYMBOLS = (
     "siglip_debug_set_chunk_label_sets",
     "siglip_debug_set_peer_extra_image_label_sets",
     "siglip_debug_set_mailbox",
+    "siglip_debug_set_peer_contribution",
     "siglip_debug_set_peer_metric_keys",
     "siglip_debug_set_peer_sample_loss_partials",
     "siglip_debug_set_peer_sample_loss_poison",
@@ -212,6 +213,8 @@ def lib() -> ctypes.CDLL:
     L.siglip_host_submit_grads.restype = ci
     L.siglip_debug_set_mailbox.argtypes = [vp, ci, ctypes.c_float, ctypes.c_float]
     L.siglip_debug_set_mailbox.restype = ci
+    L.siglip_debug_set_peer_contribution.argtypes = [vp, ci, vp, vp]
+    L.siglip_debug_set_peer_contribution.restype = ci
     L.siglip_ctx_aux_trace.argtypes = [vp, vp, ci, ctypes.POINTER(ci)]
     L.siglip_ctx_aux_trace.restype = ci
     L.siglip_fwd.argtypes = [vp] * 7

@@ -312,7 +312,8 @@ struct siglip_ctx {
   unsigned int* flags = nullptr;         // [kFlagKinds][kMaxWorld]
   unsigned int* sync_words = nullptr;    // [kSyncWords] local tickets / flags
   float* loop_mailboxes = nullptr;       // loopback only: [world][2] stand-ins for the peers' (dt', dbias) mailboxes
-  float* loop_zero = nullptr;            // loopback only: [world][Tmax, D] zeros standing in for the peers' contribution slots
+  float* loop_contrib = nullptr;         // loopback only: [world][Tmax, D] peer p's contribution to my chunk at block p
+  __nv_bfloat16* loop_txt = nullptr;     // loopback only: the peers' exported text allocation (text, ids, weights, teacher)
   unsigned long long* loop_keys = nullptr;  // loopback only: [world][Tmax] the peers' column partials of my chunk
   unsigned long long* loop_lsums = nullptr;  // loopback only: [world] blocks standing in for the peers' loss partials
   unsigned long long* loop_topk = nullptr;   // loopback only: [world][Tmax][kTopKMax] the peers' column lists of my chunk
@@ -389,7 +390,7 @@ int timing_mark(siglip_ctx* c, std::vector<cudaEvent_t>& evs, size_t& used, cuda
   return 0;
 }
 
-// elements between consecutive text chunks of txt_all / slots / loop_zero (and the size of a txt16 copy)
+// elements between consecutive text chunks of txt_all / slots / loop_contrib (and the size of a txt16 copy)
 inline size_t chunk_stride(const siglip_ctx* c) { return static_cast<size_t>(c->Tmax) * c->D; }
 
 // Sample ids of text chunk `cidx` as the loss kernel reads them (null outside SIGLIP_OPT_SAMPLE_IDS): the caller's ids
@@ -545,6 +546,15 @@ inline size_t teacher_offset(const siglip_ctx* c) {
 inline const __nv_bfloat16* peer_teacher(const siglip_ctx* c, int o) {
   return reinterpret_cast<const __nv_bfloat16*>(reinterpret_cast<const char*>(c->peer_txt[o]) + teacher_offset(c)) +
          static_cast<size_t>(o) * teacher_stride(c);
+}
+// Where a siglip_debug_set_*chunk* hook writes chunk `chunk`'s published data, given its place in my gathered buffers:
+// in a loopback context, for a peer's chunk, the same offset in the stand-in of the owner's exported allocation
+// (peer_txt), from where the step's pulls copy it; otherwise (my own chunk, or no loopback) in place
+template <typename T>
+T* seed_at(const siglip_ctx* c, int chunk, T* gathered) {
+  if (!c->loopback || chunk == c->rank) return gathered;
+  const ptrdiff_t off = reinterpret_cast<char*>(gathered) - reinterpret_cast<char*>(c->txt_all);
+  return reinterpret_cast<T*>(reinterpret_cast<char*>(c->peer_txt[chunk]) + off);
 }
 // teacher text of chunk `cidx` as the loss kernel reads it: the caller's for the own chunk, the gathered copy otherwise
 inline const void* teacher_chunk(const siglip_ctx* c, int cidx) {
@@ -3063,12 +3073,19 @@ int siglip_debug_loopback(siglip_ctx* c) {
   if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "ctx is null");
   if (c->world == 1) return fail(SIGLIP_ERR_STATE, "loopback needs world > 1");
   CK(cudaSetDevice(c->device));
-  // the "peers'" contributions to my text gradient: a zero buffer, so that the step's dtxt output is exactly this
-  // rank's own-chunk contribution; the "peers'" scalar mailboxes: separate words a test can seed
+  // The "peers'" contributions to my text gradient: one [Tmax, D] block per peer, zero until
+  // siglip_debug_set_peer_contribution seeds it (unseeded, the step's dtxt output is exactly this rank's own-chunk
+  // contribution). Every fold and reduction reads peer_slots[p] + rank * stride, so peer_slots[p] is offset to land on
+  // block p. The "peers'" exported text allocation: one stand-in with its layout up to the per-sample-loss blocks
+  // (text, ids / groups / sets, metric keys, weights, teacher text), peer o's chunk at slot o, where the
+  // siglip_debug_set_*chunk* hooks write it: every pull then copies real data from it into my gathered buffers. The
+  // "peers'" scalar mailboxes, key blocks, partials, top-K lists and extra-image ids: separate words a test can seed.
   const size_t stride = chunk_stride(c);
-  if (c->loop_zero == nullptr) {
-    CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_zero), stride * c->world * sizeof(float)));
-    CK(cudaMemset(c->loop_zero, 0, stride * c->world * sizeof(float)));
+  if (c->loop_contrib == nullptr) {
+    CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_contrib), stride * c->world * sizeof(float)));
+    CK(cudaMemset(c->loop_contrib, 0, stride * c->world * sizeof(float)));
+    CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_txt), lsum_offset(c)));
+    CK(cudaMemset(c->loop_txt, 0, lsum_offset(c)));
     CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_mailboxes), 2 * kMaxWorld * sizeof(float)));
     CK(cudaMemset(c->loop_mailboxes, 0, 2 * kMaxWorld * sizeof(float)));
     CK(cudaMalloc(reinterpret_cast<void**>(&c->loop_keys), static_cast<size_t>(c->world) * c->Tmax * 8));
@@ -3083,8 +3100,10 @@ int siglip_debug_loopback(siglip_ctx* c) {
     }
   }
   for (int p = 0; p < c->world; ++p) {
-    c->peer_txt[p] = c->txt_all;
-    c->peer_slots[p] = (p == c->rank) ? c->slots : c->loop_zero;
+    c->peer_txt[p] = (p == c->rank) ? c->txt_all : c->loop_txt;
+    c->peer_slots[p] = (p == c->rank) ? c->slots
+                                      : c->loop_contrib + (static_cast<ptrdiff_t>(p) - c->rank) *
+                                                              static_cast<ptrdiff_t>(stride);
     c->peer_flags[p] = c->flags;
   }
   c->loopback = true;   // every signal then raises the flag entry of EVERY rank in the local table
@@ -3094,7 +3113,7 @@ int siglip_debug_loopback(siglip_ctx* c) {
 int siglip_debug_set_text_chunk(siglip_ctx* c, int chunk, const void* txt_dev, void* cuda_stream) {
   if (c == nullptr || txt_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
-  CK(cudaMemcpyAsync(c->txt_all + chunk * chunk_stride(c), txt_dev,
+  CK(cudaMemcpyAsync(seed_at(c, chunk, c->txt_all + chunk * chunk_stride(c)), txt_dev,
                      static_cast<size_t>(c->Ts[chunk]) * c->D * sizeof(__nv_bfloat16), cudaMemcpyDeviceToDevice,
                      static_cast<cudaStream_t>(cuda_stream)));
   return 0;
@@ -3104,8 +3123,8 @@ int siglip_debug_set_teacher_text_chunk(siglip_ctx* c, int chunk, const void* tt
   if (c == nullptr || ttxt_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (c->DT == 0) return fail(SIGLIP_ERR_STATE, "not a distillation context (siglip_ctx_create_distill)");
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
-  CK(cudaMemcpyAsync(c->ttxt_all + chunk * teacher_stride(c), ttxt_dev, teacher_chunk_bytes(c, chunk),
-                     cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
+  CK(cudaMemcpyAsync(seed_at(c, chunk, c->ttxt_all + chunk * teacher_stride(c)), ttxt_dev,
+                     teacher_chunk_bytes(c, chunk), cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
 
@@ -3141,8 +3160,8 @@ int siglip_teacher_normalize_fwd(siglip_ctx* c, int rows, const void* x, int in_
 int siglip_debug_set_chunk_ids(siglip_ctx* c, int chunk, const int64_t* ids_dev, void* cuda_stream) {
   if (c == nullptr || ids_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
-  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * ids_slot(c), ids_dev, chunk_ids_bytes(c, chunk),
-                     cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
+  CK(cudaMemcpyAsync(seed_at(c, chunk, c->ids_all + static_cast<size_t>(chunk) * ids_slot(c)), ids_dev,
+                     chunk_ids_bytes(c, chunk), cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
 
@@ -3150,8 +3169,8 @@ int siglip_debug_set_chunk_groups(siglip_ctx* c, int chunk, const int64_t* group
   if (c == nullptr || groups_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
   // the group half of the chunk's slot, where its owner's ids publish puts them
-  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * ids_slot(c) + set_words(c), groups_dev,
-                     static_cast<size_t>(c->Ts[chunk]) * sizeof(int64_t), cudaMemcpyDeviceToDevice,
+  CK(cudaMemcpyAsync(seed_at(c, chunk, c->ids_all + static_cast<size_t>(chunk) * ids_slot(c) + set_words(c)),
+                     groups_dev, static_cast<size_t>(c->Ts[chunk]) * sizeof(int64_t), cudaMemcpyDeviceToDevice,
                      static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
@@ -3161,7 +3180,7 @@ int siglip_debug_set_chunk_label_sets(siglip_ctx* c, int chunk, const int64_t* s
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
   if (c->LM == 0) return fail(SIGLIP_ERR_STATE, "siglip_debug_set_chunk_label_sets needs a context with label sets");
   // the set half of the chunk's slot, where its owner's ids publish puts them
-  CK(cudaMemcpyAsync(c->ids_all + static_cast<size_t>(chunk) * ids_slot(c), sets_dev,
+  CK(cudaMemcpyAsync(seed_at(c, chunk, c->ids_all + static_cast<size_t>(chunk) * ids_slot(c)), sets_dev,
                      static_cast<size_t>(c->Ts[chunk]) * c->LM * sizeof(int64_t), cudaMemcpyDeviceToDevice,
                      static_cast<cudaStream_t>(cuda_stream)));
   return 0;
@@ -3171,8 +3190,8 @@ int siglip_debug_set_chunk_weights(siglip_ctx* c, int chunk, const float* text_w
   if (c == nullptr) return fail(SIGLIP_ERR_INVALID, "ctx is null");
   if (c->world == 1 || chunk < 0 || chunk >= c->world) return fail(SIGLIP_ERR_INVALID, "chunk out of range");
   // clamped like the owner's siglip_set_sample_weights (NULL = ones)
-  CKI(siglip::launch_clamp_weights(text_w_dev, c->w_all + static_cast<size_t>(chunk) * c->w_stride, c->Ts[chunk],
-                                   nullptr, nullptr, 0, static_cast<cudaStream_t>(cuda_stream)));
+  CKI(siglip::launch_clamp_weights(text_w_dev, seed_at(c, chunk, c->w_all + static_cast<size_t>(chunk) * c->w_stride),
+                                   c->Ts[chunk], nullptr, nullptr, 0, static_cast<cudaStream_t>(cuda_stream)));
   c->launches++;
   return 0;
 }
@@ -3193,6 +3212,18 @@ int siglip_debug_set_mailbox(siglip_ctx* c, int peer, float dt_prime, float dbia
   CK(cudaSetDevice(c->device));
   const float v[2] = {dt_prime, dbias};
   CK(cudaMemcpy(c->loop_mailboxes + 2 * peer, v, sizeof(v), cudaMemcpyHostToDevice));
+  return 0;
+}
+
+int siglip_debug_set_peer_contribution(siglip_ctx* c, int peer, const float* contrib_dev, void* cuda_stream) {
+  if (c == nullptr || contrib_dev == nullptr) return fail(SIGLIP_ERR_INVALID, "null argument");
+  if (!c->loopback || peer < 0 || peer >= c->world || peer == c->rank)
+    return fail(SIGLIP_ERR_INVALID,
+                "siglip_debug_set_peer_contribution needs a loopback context and a peer rank != own rank");
+  // block `peer` of the stand-in, where every fold of that peer's contribution reads (peer_slots[peer] + rank * stride)
+  CK(cudaMemcpyAsync(c->peer_slots[peer] + c->rank * chunk_stride(c), contrib_dev,
+                     static_cast<size_t>(c->T) * c->D * sizeof(float), cudaMemcpyDeviceToDevice,
+                     static_cast<cudaStream_t>(cuda_stream)));
   return 0;
 }
 
@@ -3463,7 +3494,8 @@ void free_ctx(siglip_ctx* c) {
   cudaFree(c->flags);
   cudaFree(c->sync_words);
   cudaFree(c->loop_mailboxes);
-  cudaFree(c->loop_zero);
+  cudaFree(c->loop_contrib);
+  cudaFree(c->loop_txt);
   cudaFree(c->loop_keys);
   if (c->world == 1) cudaFree(c->mkeys[0]);   // world > 1: part of txt_all
   cudaFree(c->mkey_ptrs_dev);

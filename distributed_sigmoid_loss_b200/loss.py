@@ -496,6 +496,15 @@ class SigmoidLossEngine:
     def debug_set_mailbox(self, peer: int, dt_prime: float, dbias: float) -> None:
         _capi.check(self._L.siglip_debug_set_mailbox(self._h, peer, float(dt_prime), float(dbias)))
 
+    def debug_set_peer_contribution(self, peer: int, contrib: torch.Tensor) -> None:
+        """Loopback: the contribution to this rank's text gradient ([texts, dim] fp32, contiguous, already scaled by the
+        upstream gradient) standing in for peer `peer`'s; the step's dtxt adds it to this rank's own contribution."""
+        if contrib.dtype != torch.float32 or tuple(contrib.shape) != (self.texts, self.dim) or \
+                not contrib.is_contiguous() or contrib.device != self.device:
+            raise RuntimeError(f"peer contribution must be a contiguous fp32 [{self.texts}, {self.dim}] tensor on "
+                               f"{self.device}")
+        _capi.check(self._L.siglip_debug_set_peer_contribution(self._h, peer, contrib.data_ptr(), self._stream()))
+
     def aux_trace(self, max_launches: int = 4096):
         """Per launch since the last call, globaltimer ns: (aux start, flags seen, aux jobs done, launch end, kernel
         entry, set-up done, first operands landed, last MMA issued, first CTA finished, latest / earliest "last MMA issued"

@@ -649,13 +649,22 @@ int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, cons
 
 /*
  * Test hooks for exercising the multi-chunk schedule of ONE rank on ONE GPU (world > 1 context, no peers):
- * loopback wires every "peer" pointer to the context's own buffers (the peers' contribution slots to a zero buffer);
- * the test preloads the text chunks of the other ranks, runs the step, and reads this rank's per-owner dtxt
- * contributions back: slot c for c != rank, and the dtxt OUTPUT of the step for the own chunk (own contribution + the
- * zero "peer" contributions). Chunks and slots hold T_chunk rows (its batch plus its hard negatives).
+ * loopback wires every "peer" pointer to stand-in buffers of the context. The peers' exported text allocations are
+ * one stand-in with the same layout, peer o's chunk at slot o: siglip_debug_set_text_chunk and its twins below write a
+ * peer's chunk (text, ids, groups, label sets, weights, teacher text) there, and every step pulls it into the gathered
+ * buffers the kernels read, as from a real owner (the own chunk is written in place, and the step overwrites it with
+ * its own inputs). The peers' contribution slots are one [T of this rank, D] fp32 block per peer, zero until
+ * siglip_debug_set_peer_contribution seeds it: the step folds each peer's block into the dtxt OUTPUT, which is then this
+ * rank's own-chunk contribution plus the seeded blocks. The test runs the step and reads this rank's per-owner dtxt
+ * contributions back: slot c for c != rank (siglip_debug_get_slot), the dtxt output for the own chunk. Chunks and
+ * slots hold T_chunk rows (its batch plus its hard negatives).
  */
 int siglip_debug_loopback(siglip_ctx* ctx);
 int siglip_debug_set_text_chunk(siglip_ctx* ctx, int chunk, const void* txt_dev, void* cuda_stream);
+/* Loopback only: the contribution to this rank's text gradient standing in for peer rank `peer`'s ([T of this rank, D]
+ * fp32 device buffer, already scaled by the upstream gradient as a peer's gradient kernel writes it). It stays until
+ * seeded again, and the step's dtxt output adds it to g x (own contribution). */
+int siglip_debug_set_peer_contribution(siglip_ctx* ctx, int peer, const float* contrib_dev, void* cuda_stream);
 
 /* The teacher twin of siglip_debug_set_text_chunk (SIGLIP_OPT_DISTILL): the teacher text of chunk `chunk`
  * ([T of that rank, D_teacher] in the teacher's format: paired texts, then extras) as its owner would have published

@@ -60,7 +60,11 @@ FOCALS = tuple((g, a) for g in (0.5, 2.0, 5.0) for a in (None, 0.25))
 
 # per-rank paired batches, extra texts and extra images of each world size (uneven, ragged past 256 at W = 1); the
 # panel cells use larger batches so that a budget of a few MiB splits the rows into several panels
-SHAPES = {1: ((300,), (37,), (23,)), 2: ((200, 136), (29, 41), (17, 30)), 3: ((136, 200, 160), (19, 0, 33), (9, 27, 13))}
+SHAPES = {1: ((300,), (37,), (23,)), 2: ((200, 136), (29, 41), (17, 30)),
+          3: ((136, 200, 160), (19, 0, 33), (9, 27, 13)),
+          # W = 4: the loopback exchange cells (tests/loopback_exchange.py), where the bidirectional schedule first
+          # reads other owners than the ring
+          4: ((136, 120, 160, 104), (19, 0, 33, 8), (9, 27, 0, 13))}
 PANEL_SHAPES = {1: ((700,), (60,), (48,)), 2: ((600, 520), (40, 72), (24, 36)),
                 3: ((520, 456, 600), (8, 40, 0), (36, 12, 20))}
 

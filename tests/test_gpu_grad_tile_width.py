@@ -107,14 +107,16 @@ def test_hard_negatives_and_extra_texts():
 
 def test_two_rank_loopback_with_in_kernel_fold():
     """Rank 1 of a 2-rank step on one GPU: two gradient launches, the second adds the folded peer contribution
-    (p1_wait_flag) and the running dimg of the first."""
+    (p1_wait_flag), seeded non-zero through the loopback stand-in, and the running dimg of the first."""
     B, D = 1024, 768
     out = {}
+    peer = _emb(B, D, 22).float() * 1e-3
     for tn in (128, 256):
         eng = _engine(B, D, rank_world=(1, 2), loopback=True)
         _set_width(eng, tn)
         for k in range(2):
             eng.debug_set_text_chunk(k, _emb(B, D, 20 + k))
+        eng.debug_set_peer_contribution(0, peer)
         _, dimg, dtxt, dtp, db = eng.fwd_bwd(_emb(B, D, 30), _emb(B, D, 21), _scal(math.log(10.0)), _scal(-10.0))
         torch.cuda.synchronize()
         out[tn] = (dimg.clone(), torch.cat([dtxt.float(), eng.debug_get_slot(0)]), dtp.clone(), db.clone())
