@@ -2835,9 +2835,18 @@ int siglip_debug_set_peer_extra_image_label_sets(siglip_ctx* c, int peer, const 
   return 0;
 }
 
+// A request is for the next step only, whether that step runs or is refused: a refused step (an argument, the budget,
+// take_ids) returns before take_metrics / take_sample_losses / take_topk consume it, and a request left armed would
+// write the next step's results into buffers its caller may have released already.
+static int disarm_on_error(siglip_ctx* c, int rc) {
+  if (rc != 0 && c != nullptr) c->metrics_armed = c->losses_armed = c->topk_armed = false;
+  return rc;
+}
+
 int siglip_forward(siglip_ctx* c, const void* img, const void* txt, const float* t_prime, const float* bias,
                    float* loss, int save_for_backward, void* cuda_stream) {
-  return forward_impl(c, img, txt, t_prime, bias, loss, save_for_backward != 0, static_cast<cudaStream_t>(cuda_stream));
+  return disarm_on_error(c, forward_impl(c, img, txt, t_prime, bias, loss, save_for_backward != 0,
+                                         static_cast<cudaStream_t>(cuda_stream)));
 }
 
 unsigned long long siglip_ctx_saved_generation(const siglip_ctx* c) { return c ? c->gen : 0ull; }
@@ -2851,18 +2860,18 @@ int siglip_backward(siglip_ctx* c, const void* img, const void* txt, const float
 int siglip_fwd_bwd(siglip_ctx* c, const void* img, const void* txt, const float* t_prime, const float* bias,
                    float* loss, void* dimg, void* dtxt, float* dt_prime, float* dbias, void* cuda_stream) {
   if (dimg == nullptr || dtxt == nullptr || dt_prime == nullptr || dbias == nullptr)
-    return fail(SIGLIP_ERR_INVALID, "null gradient pointer");
-  return fused_impl(c, img, txt, t_prime, bias, loss, nullptr, dimg, dtxt, dt_prime, dbias,
-                    static_cast<cudaStream_t>(cuda_stream));
+    return disarm_on_error(c, fail(SIGLIP_ERR_INVALID, "null gradient pointer"));
+  return disarm_on_error(c, fused_impl(c, img, txt, t_prime, bias, loss, nullptr, dimg, dtxt, dt_prime, dbias,
+                                       static_cast<cudaStream_t>(cuda_stream)));
 }
 
 int siglip_fwd_bwd_scaled(siglip_ctx* c, const void* img, const void* txt, const float* t_prime, const float* bias,
                           const float* grad_out, float* loss, void* dimg, void* dtxt, float* dt_prime, float* dbias,
                           void* cuda_stream) {
   if (dimg == nullptr || dtxt == nullptr || dt_prime == nullptr || dbias == nullptr)
-    return fail(SIGLIP_ERR_INVALID, "null gradient pointer");
-  return fused_impl(c, img, txt, t_prime, bias, loss, grad_out, dimg, dtxt, dt_prime, dbias,
-                    static_cast<cudaStream_t>(cuda_stream));
+    return disarm_on_error(c, fail(SIGLIP_ERR_INVALID, "null gradient pointer"));
+  return disarm_on_error(c, fused_impl(c, img, txt, t_prime, bias, loss, grad_out, dimg, dtxt, dt_prime, dbias,
+                                       static_cast<cudaStream_t>(cuda_stream)));
 }
 
 int siglip_fwd(siglip_ctx* c, const void* img, const void* txt, const float* t_prime, const float* bias, float* loss,

@@ -12,6 +12,7 @@ the stream and the process group used to exchange CUDA-IPC handles once. No CPU 
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import math
 from typing import Dict, Optional, Tuple
@@ -535,12 +536,14 @@ class SigmoidLossEngine:
         1-element fp32 device tensor, multiplied in by the kernel epilogues); scalars are fp32, dimg/dtxt are
         `grad_dtype` (fp32, or bf16 written directly by the kernel epilogue). txt is [T, D]: T = B plus this rank's hard
         negatives (texts_per_rank)."""
-        self._check(img, txt)
-        self._set_grad_dtype(grad_dtype)
+        with self._refusal_disarms():
+            self._check(img, txt)
+            self._set_grad_dtype(grad_dtype)
+            f64 = self._set_tprime_f64(t_prime)
         opts = dict(device=self.device, dtype=torch.float32)
         scal = torch.empty(3, **opts)                 # loss, dt', dbias in one allocation
         loss, dtp, db = scal[0:1], scal[1:2], scal[2:3]
-        if self._set_tprime_f64(t_prime):
+        if f64:
             dtp = torch.empty(1, device=self.device, dtype=torch.float64)
         dimg = torch.empty(self.images, self.dim, device=self.device, dtype=grad_dtype)
         dtxt = torch.empty(self.texts, self.dim, device=self.device, dtype=grad_dtype)
@@ -551,6 +554,17 @@ class SigmoidLossEngine:
                 dtxt.data_ptr(), dtp.data_ptr(), db.data_ptr(), self._stream()))
         return loss, dimg, dtxt, dtp, db
 
+    @contextlib.contextmanager
+    def _refusal_disarms(self):
+        """A step this engine refuses before it reaches the library consumes the requests armed for it, as a step the
+        library refuses does (include/siglip_b200.h, siglip_request_metrics): siglip_fwd with null operands is such a
+        refusal, and disarms them."""
+        try:
+            yield
+        except Exception:
+            self._L.siglip_fwd(self._h, None, None, None, None, None, None)
+            raise
+
     # -- the two halves autograd uses ----------------------------------------------------------------------
     @property
     def saved_generation(self) -> int:
@@ -559,8 +573,9 @@ class SigmoidLossEngine:
     def forward(self, img: torch.Tensor, txt: torch.Tensor, t_prime: torch.Tensor, bias: torch.Tensor,
                 save_for_backward: bool) -> torch.Tensor:
         """The W loss kernels. Returns loss[1] (fp32). With save_for_backward the context keeps the sigma operands."""
-        self._check(img, txt)
-        self._set_tprime_f64(t_prime)
+        with self._refusal_disarms():
+            self._check(img, txt)
+            self._set_tprime_f64(t_prime)
         loss = torch.empty(1, device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.device):
             _capi.check(self._L.siglip_forward(self._h, img.data_ptr(), txt.data_ptr(), t_prime.data_ptr(),
@@ -644,8 +659,9 @@ class SigmoidLossEngine:
         return dst
 
     def fwd(self, img: torch.Tensor, txt: torch.Tensor, t_prime: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
-        self._check(img, txt)
-        self._set_tprime_f64(t_prime)
+        with self._refusal_disarms():
+            self._check(img, txt)
+            self._set_tprime_f64(t_prime)
         loss = torch.empty(1, device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.device):
             _capi.check(self._L.siglip_fwd(self._h, img.data_ptr(), txt.data_ptr(), t_prime.data_ptr(),

@@ -527,6 +527,11 @@ int siglip_set_focal(siglip_ctx* ctx, float gamma, float alpha);
  * single-rank context the first call allocates the key buffers (4 x B 64-bit words; also allowed inside a capture), so a
  * context that never asks for metrics holds exactly the workspace it held before.
  * Collective: every rank arms the same steps. The host-buffer entries return SIGLIP_ERR_STATE while armed.
+ * A step entry (siglip_fwd_bwd(_scaled) / siglip_forward / siglip_fwd) that returns an error disarms every request
+ * (metrics, per-sample losses, top-K). A call refused before the step starts (an argument, the sigma budget, a missing
+ * input) writes none of the buffers, and no later step does; an error after the step has started (a launch, a
+ * workspace allocation, a peer wait) may leave the buffers written in part. siglip_backward takes no request: a
+ * refused backward leaves the requests armed for the next forward.
  */
 int siglip_request_metrics(siglip_ctx* ctx, float* top1, int64_t* i2t_index, int64_t* t2i_index);
 
@@ -550,7 +555,8 @@ int siglip_request_metrics(siglip_ctx* ctx, float* top1, int64_t* i2t_index, int
  * exported text allocation from creation. This call only records the pointers, so a single-rank step stays capturable.
  * Collective: every rank arms the same steps. Under SIGLIP_OPT_DISTILL the sums are those of the distillation
  * terms; a siglip_ctx_create_distill context returns SIGLIP_ERR_STATE there (siglip_ctx_create_distill_extras takes
- * them). The host-buffer entries return SIGLIP_ERR_STATE while armed. */
+ * them). The host-buffer entries return SIGLIP_ERR_STATE while armed. A refused step disarms the request, as for
+ * siglip_request_metrics. */
 int siglip_request_sample_losses(siglip_ctx* ctx, float* image_loss, float* text_loss);
 
 /* Largest K of siglip_request_topk. */
@@ -576,7 +582,8 @@ int siglip_request_sample_losses(siglip_ctx* ctx, float* image_loss, float* text
  * allocation from creation. This call only records the pointers.
  * Collective: every rank arms the same steps with the same k. Returns SIGLIP_ERR_INVALID for k out of range or a null
  * recall, SIGLIP_ERR_STATE under SIGLIP_OPT_DISTILL on a siglip_ctx_create_distill context (a
- * siglip_ctx_create_distill_extras context takes it); the host-buffer entries return SIGLIP_ERR_STATE while armed. */
+ * siglip_ctx_create_distill_extras context takes it); the host-buffer entries return SIGLIP_ERR_STATE while armed.
+ * A refused step disarms the request, as for siglip_request_metrics. */
 int siglip_request_topk(siglip_ctx* ctx, int k, float* recall, int64_t* i2t_topk, int64_t* t2i_topk);
 
 /* Forward only (torch.no_grad / evaluation): siglip_forward with save_for_backward = 0. */

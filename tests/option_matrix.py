@@ -67,6 +67,9 @@ SHAPES = {1: ((300,), (37,), (23,)), 2: ((200, 136), (29, 41), (17, 30)),
           4: ((136, 120, 160, 104), (19, 0, 33, 8), (9, 27, 0, 13))}
 PANEL_SHAPES = {1: ((700,), (60,), (48,)), 2: ((600, 520), (40, 72), (24, 36)),
                 3: ((520, 456, 600), (8, 40, 0), (36, 12, 20))}
+# one rank with more than 960 images and texts: the gradient kernel's split-K splits (launch_impl cuts K into slices of
+# at least 8 k-blocks of 64), which the shapes above never reach (the step sequences' split-K steps run these)
+SPLIT_SHAPES = {1: ((1040,), (37,), (23,))}
 
 
 @dataclass(frozen=True)
@@ -161,6 +164,7 @@ class Cell:
     mcast: int
     seed: int
     cold: bool = False   # planted_cold's data: the series path's family
+    splitk: bool = False  # SPLIT_SHAPES instead of SHAPES / PANEL_SHAPES
 
     @property
     def mode(self) -> str:
@@ -181,11 +185,11 @@ class Cell:
         return (f"{self.seed:03d}-{self.mode}-{o.context}-{'+'.join(on) or 'none'}-W{self.W}r{self.r}"
                 f"{'-bidir' if self.bidir else ''}-{self.sched}{'-panels' if self.panels else ''}"
                 f"{'-f16' if self.f16 else ''}-t{self.tile_n}-s{self.stages}-cg{self.cg}m{self.mcast}"
-                f"{'-cold' if self.cold else ''}")
+                f"{'-cold' if self.cold else ''}{'-splitk' if self.splitk else ''}")
 
     def shapes(self):
         """(Bs, Rs, Ts) of every rank, as the step sees them."""
-        Bs, K, E = (PANEL_SHAPES if self.panels else SHAPES)[self.W]
+        Bs, K, E = shape_table(self)[self.W]
         Ts = tuple(b + (k if self.opts.xtexts else 0) for b, k in zip(Bs, K))
         Rs = tuple(b + (e if self.opts.ximages else 0) for b, e in zip(Bs, E))
         return Bs, Rs, Ts
@@ -212,6 +216,10 @@ class Cell:
         unit = 128 * self.cluster
         P = self.budget_mib() * 2 ** 20 // ((2 if self.W > 1 else 1) * _round_up(max(Ts), 256) * 2) // unit * unit
         return min(P, Rs[self.r])
+
+
+def shape_table(cell: Cell):
+    return SPLIT_SHAPES if cell.splitk else PANEL_SHAPES if cell.panels else SHAPES
 
 
 def _round_up(x, m):
@@ -484,7 +492,7 @@ class Problem:
 def planted(cell: Cell) -> Problem:
     if cell.cold:
         return planted_cold(cell)
-    Bs, K, E = (PANEL_SHAPES if cell.panels else SHAPES)[cell.W]
+    Bs, K, E = shape_table(cell)[cell.W]
     Rs = tuple(b + e for b, e in zip(Bs, E))
     Ts = tuple(b + k for b, k in zip(Bs, K))
     g = np.random.default_rng(1000 + cell.seed)
@@ -561,7 +569,7 @@ def planted_cold(cell: Cell) -> Problem:
     max z lies 3e-3 below kFastZ, where the series truncation is largest. The teacher's rows are a signature of 6 entries
     +-4 (z_T = -1 on pairs of one id, below -5.5 elsewhere) and, on some whole slabs of rank r, U_T + COLD_TEACHER_U:
     a teacher that knows matches the labels do not, in slabs whose student votes either way. Weights as planted's."""
-    Bs, K, E = (PANEL_SHAPES if cell.panels else SHAPES)[cell.W]
+    Bs, K, E = shape_table(cell)[cell.W]
     Rs = tuple(b + e for b, e in zip(Bs, E))
     Ts = tuple(b + k for b, k in zip(Bs, K))
     g = np.random.default_rng(1000 + cell.seed)
@@ -691,19 +699,20 @@ def labels(P: Problem, o: Options):
     return lab
 
 
-def oracle(P: Problem, o: Options) -> List[Dict]:
+def oracle(P: Problem, o: Options, tp: float = TP, bias: float = BIAS, lam: float = LAM) -> List[Dict]:
     """Per rank: loss, dimg [R_r, D], contrib[c] [T_c, D], dt_prime, dbias, image_loss [R_r], text_part[c] (this rank's
-    column sums over chunk c) and text_loss [T_r] (every rank's column sums of its chunk)."""
+    column sums over chunk c) and text_loss [T_r] (every rank's column sums of its chunk), at t' = tp, bias and the
+    distillation weight lam (the cells' TP, BIAS and LAM by default)."""
     Bs, Rs, Ts, imgs, txts = P.view(o)
     iw = [x[:n].astype(np.float64) for x, n in zip(P.iw, Rs)] if o.weights else None
     tw = [x[:n].astype(np.float64) for x, n in zip(P.tw, Ts)] if o.weights else None
     lab = labels(P, o)
     if o.teacher:
-        res = closed_form_distill_options(imgs, txts, TP, BIAS, *P.teacher(o), TTP, TBIAS, LAM, lab, Bs, iw, tw)
+        res = closed_form_distill_options(imgs, txts, tp, bias, *P.teacher(o), TTP, TBIAS, lam, lab, Bs, iw, tw)
     elif o.focal is not None:
-        res = closed_form_focal(imgs, txts, TP, BIAS, lab, o.focal[0], o.focal[1], Bs, iw, tw)
+        res = closed_form_focal(imgs, txts, tp, bias, lab, o.focal[0], o.focal[1], Bs, iw, tw)
     else:
-        res = closed_form_groups(imgs, txts, TP, BIAS, lab, Bs, iw, tw)
+        res = closed_form_groups(imgs, txts, tp, bias, lab, Bs, iw, tw)
     for r, x in enumerate(res):
         x["text_loss"] = text_loss_of(res, r)
     return res
