@@ -14,6 +14,7 @@ from __future__ import annotations
 
 import contextlib
 import ctypes
+import dataclasses
 import math
 from typing import Dict, Optional, Tuple
 
@@ -786,6 +787,44 @@ def _aligned(x: torch.Tensor) -> torch.Tensor:
     return x if x.data_ptr() % 16 == 0 else x.clone()
 
 
+@dataclasses.dataclass
+class _StepInputs:
+    """The per-step inputs of one forward (_step_inputs), each None when the module's options take none. The engine
+    copies them for the NEXT step, so they are applied before every step it runs for the call.
+    ids: [B] int64 sample ids (SIGLIP_OPT_SAMPLE_IDS engines).
+    extra_text_ids: [T - B] int64 ids of the extra texts (SIGLIP_OPT_EXTRA_TEXT_IDS engines).
+    extra_image_ids: [R - B] int64 ids of the extra images (SIGLIP_OPT_EXTRA_IMAGE_IDS engines).
+    weights: (image_weights [R] or None, text_weights [T] or None) fp32 (SIGLIP_OPT_SAMPLE_WEIGHTS engines).
+    groups: (image_groups [R], text_groups [T]) int64 (SIGLIP_OPT_EXCLUDE_GROUPS engines).
+    label_sets: (sample_labels [B, M], extra_text_labels [T - B, M] or None, extra_image_labels [R - B, M] or None) int64
+    (SIGLIP_OPT_LABEL_SETS engines).
+    teacher: (teacher_image, teacher_text, teacher_t_prime, teacher_bias, lambda) of a distillation step
+    (SIGLIP_OPT_DISTILL engines): constants, no gradient flows to them."""
+    ids: Optional[torch.Tensor] = None
+    extra_text_ids: Optional[torch.Tensor] = None
+    extra_image_ids: Optional[torch.Tensor] = None
+    weights: Optional[tuple] = None
+    groups: Optional[tuple] = None
+    label_sets: Optional[tuple] = None
+    teacher: Optional[tuple] = None
+
+    def apply(self, engine: SigmoidLossEngine) -> None:
+        if self.teacher is not None:
+            engine.set_teacher(*self.teacher)
+        if self.ids is not None:
+            engine.set_sample_ids(self.ids)
+        if self.extra_text_ids is not None:
+            engine.set_extra_text_ids(self.extra_text_ids)
+        if self.extra_image_ids is not None:
+            engine.set_extra_image_ids(self.extra_image_ids)
+        if self.weights is not None:
+            engine.set_sample_weights(*self.weights)
+        if self.groups is not None:
+            engine.set_groups(*self.groups)
+        if self.label_sets is not None:
+            engine.set_label_sets(*self.label_sets)
+
+
 class _SigmoidLossFn(torch.autograd.Function):
     """loss = sum_chunks(-logsigmoid(labels * (img @ txt_chunk.T * exp(t') + b))).sum() / B.
 
@@ -797,27 +836,16 @@ class _SigmoidLossFn(torch.autograd.Function):
         operands, every cross-rank flag handled inside the kernels) which leaves the gradients for an upstream gradient
         of 1; backward = one multiply by grad_output per tensor (siglip_scale). O(B^2) workspace.
     normalize=True additionally fuses F.normalize of both inputs (forward) and its backward around the loss.
-    ids: [B] int64 sample ids (SIGLIP_OPT_SAMPLE_IDS engines), set before every step the engine runs for this call.
-    extra_ids: [T - B] int64 ids of the extra texts (SIGLIP_OPT_EXTRA_TEXT_IDS engines), set along with ids.
+    inputs: the call's _StepInputs, applied to the engine before every step it runs for this call; the teacher's
+    embeddings are converted to the kernels' operand format here (teacher_operand) and kept in that form.
     metrics: (top1, i2t_index, t2i_index) output buffers: the retrieval metrics of this call's step are armed. A re-run
     of the forward by the backward's generation guard does not arm them again (they belong to the first run).
-    weights: (image_weights [R] or None, text_weights [T] or None) fp32 (SIGLIP_OPT_SAMPLE_WEIGHTS engines), set before
-    every step the engine runs for this call, like the ids.
-    extra_img_ids: [R - B] int64 ids of the extra images (SIGLIP_OPT_EXTRA_IMAGE_IDS engines), set along with ids.
-    teacher: (teacher_image, teacher_text, teacher_t_prime, teacher_bias, lambda) of a distillation step
-    (SIGLIP_OPT_DISTILL engines): constants, no gradient flows to them; set before every step like the ids.
     sample_losses: (image_loss [R], text_loss [T]) fp32 output buffers: the per-sample losses of this call's step are
-    armed. Like the metrics, a re-run of the forward by the backward's generation guard does not arm them again.
-    groups: (image_groups [R], text_groups [T]) int64 (SIGLIP_OPT_EXCLUDE_GROUPS engines), set before every step the
-    engine runs for this call, like the ids.
-    label_sets: (sample_labels [B, M], extra_text_labels [T - B, M] or None, extra_image_labels [R - B, M] or None) int64
-    (SIGLIP_OPT_LABEL_SETS engines), set before every step the engine runs for this call, like the ids."""
+    armed. Like the metrics, a re-run of the forward by the backward's generation guard does not arm them again."""
 
     @staticmethod
-    def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool = False, fused: bool = False,
-                ids: Optional[torch.Tensor] = None, metrics=None, extra_ids: Optional[torch.Tensor] = None, weights=None,
-                extra_img_ids: Optional[torch.Tensor] = None, teacher=None, sample_losses=None, groups=None,
-                label_sets=None):
+    def forward(ctx, img, txt, t_prime, bias, engine: SigmoidLossEngine, normalize: bool, fused: bool,
+                inputs: _StepInputs, metrics, sample_losses):
         need_grad = any(ctx.needs_input_grad[:4])
         raw = None
         # bf16 callers: bf16 operands (what autograd would multiply). Anything wider (the reference's own test feeds
@@ -851,29 +879,15 @@ class _SigmoidLossFn(torch.autograd.Function):
             b = b.to(device=img.device, dtype=torch.float32)
         b = b.reshape(1)
         ctx.fused = bool(fused and need_grad)
-        if teacher is not None:
-            timg, ttxt, ttp, tbias, lam = teacher
-            teacher = (engine.teacher_operand(timg.detach(), normalize), engine.teacher_operand(ttxt.detach(), normalize),
-                       ttp.detach().to(device=img.device, dtype=torch.float32).reshape(1),
-                       tbias.detach().to(device=img.device, dtype=torch.float32).reshape(1), lam)
-            engine.set_teacher(*teacher)
-        ctx.ids, ctx.extra_ids, ctx.weights, ctx.extra_img_ids = ids, extra_ids, weights, extra_img_ids
-        ctx.groups = groups
-        ctx.label_sets = label_sets
-        # the split schedule's backward may have to re-run the forward with the same teacher; the fused one never does
-        ctx.teacher = None if ctx.fused else teacher
-        if ids is not None:
-            engine.set_sample_ids(ids)
-        if extra_ids is not None:
-            engine.set_extra_text_ids(extra_ids)
-        if extra_img_ids is not None:
-            engine.set_extra_image_ids(extra_img_ids)
-        if weights is not None:
-            engine.set_sample_weights(*weights)
-        if groups is not None:
-            engine.set_groups(*groups)
-        if label_sets is not None:
-            engine.set_label_sets(*label_sets)
+        if inputs.teacher is not None:
+            timg, ttxt, ttp, tbias, lam = inputs.teacher
+            inputs = dataclasses.replace(inputs, teacher=(
+                engine.teacher_operand(timg.detach(), normalize), engine.teacher_operand(ttxt.detach(), normalize),
+                ttp.detach().to(device=img.device, dtype=torch.float32).reshape(1),
+                tbias.detach().to(device=img.device, dtype=torch.float32).reshape(1), lam))
+        inputs.apply(engine)
+        # the split schedule's backward may have to re-run the forward with the same inputs; the fused one never does
+        ctx.inputs = None if ctx.fused else inputs
         if metrics is not None:
             engine.request_metrics(*metrics[:3])
             if len(metrics) > 3:   # metrics_topk = K > 1: (K, recall, i2t_topk, t2i_topk) follow
@@ -926,21 +940,8 @@ class _SigmoidLossFn(torch.autograd.Function):
             img_b, txt_b, tp, b = saved[:4]
             if eng.saved_generation != ctx.gen:
                 # another forward of the same module ran in between: rebuild the saved state (every rank takes this
-                # branch together, so the collective stays matched); the re-run takes this call's ids and weights again
-                if ctx.ids is not None:
-                    eng.set_sample_ids(ctx.ids)
-                if ctx.extra_ids is not None:
-                    eng.set_extra_text_ids(ctx.extra_ids)
-                if ctx.extra_img_ids is not None:
-                    eng.set_extra_image_ids(ctx.extra_img_ids)
-                if ctx.weights is not None:
-                    eng.set_sample_weights(*ctx.weights)
-                if ctx.groups is not None:
-                    eng.set_groups(*ctx.groups)
-                if ctx.label_sets is not None:
-                    eng.set_label_sets(*ctx.label_sets)
-                if ctx.teacher is not None:
-                    eng.set_teacher(*ctx.teacher)
+                # branch together, so the collective stays matched) with this call's inputs
+                ctx.inputs.apply(eng)
                 eng.forward(img_b, txt_b, tp, b, True)
                 ctx.gen = eng.saved_generation
             if ctx.normalize:
@@ -957,85 +958,97 @@ class _SigmoidLossFn(torch.autograd.Function):
                 gt = dtxt.to(tdt) if ctx.needs_input_grad[1] else None
         gp = dtp.reshape(pshape).to(device=pdev, dtype=pdt) if ctx.needs_input_grad[2] else None
         gb = db.reshape(bshape).to(device=bdev, dtype=bdt) if ctx.needs_input_grad[3] else None
-        return gi, gt, gp, gb, None, None, None, None, None, None, None, None, None, None, None, None
+        return gi, gt, gp, gb, None, None, None, None, None, None
+
+
+@dataclasses.dataclass(frozen=True)
+class _LossOptions:
+    """The loss options DDPSigmoidLoss and SigLipLoss share, checked together by _loss_options; each is also a
+    read-only attribute of the module (see the class docstring of DDPSigmoidLoss for what they do)."""
+    multi_positive: bool
+    hard_negatives: int
+    extra_texts: int
+    sample_weights: bool
+    extra_images: int
+    distill: Optional[float]
+    distill_options: bool
+    # distill=lambda without distill_options (None otherwise): what the checks of the other options refuse
+    distill_closed: Optional[float]
+    exclude_groups: bool
+    multi_label: int   # labels per set, 0: off
+    focal: Optional[Tuple[float, Optional[float]]]   # (gamma, alpha or None), or None
+    sigma_budget_bytes: Optional[int]
+    ranks_per_node: Optional[int]
+
+
+def _with_option_attributes(cls):
+    """Each field of _LossOptions as a read-only attribute of the module class (loss.multi_label, loss.focal, ...)."""
+    for f in dataclasses.fields(_LossOptions):
+        setattr(cls, f.name, property(lambda self, name=f.name: getattr(self._options, name)))
+    return cls
 
 
 class _EngineCache:
-    def __init__(self, group=None, cta_group: int = 2, overlap_pull: bool = True, sync_scalar_grads: bool = False,
-                 bidir: bool = False, batch_per_rank=None, multi_positive: bool = False, hard_negatives: int = 0,
-                 extra_texts: int = 0, sample_weights: bool = False, extra_images: int = 0,
-                 distill: Optional[float] = None, sigma_budget_bytes: Optional[int] = None,
-                 exclude_groups: bool = False, multi_label: int = 0, focal=None, distill_options: bool = False,
-                 ranks_per_node: Optional[int] = None):
+    def __init__(self, group, cta_group: int, overlap_pull: bool, sync_scalar_grads: bool, bidir: bool, batch_per_rank,
+                 options: _LossOptions):
         self.group, self.cta_group, self.overlap_pull = group, cta_group, overlap_pull
-        self.ranks_per_node = ranks_per_node
+        self.sync_scalar_grads, self.bidir, self.batch_per_rank = sync_scalar_grads, bidir, batch_per_rank
+        self.options = options
         self._topology = None   # cross_node.Topology of a group that spans nodes, found when the first engine is built
         self._topology_known = False
-        self.distill_options = distill_options
-        self.focal = focal   # (gamma, alpha or None), or None
-        self.exclude_groups = exclude_groups
-        self.multi_label = multi_label
-        self.sigma_budget_bytes = sigma_budget_bytes
-        self.distill = distill
-        self.extra_images = extra_images
-        self.sample_weights = sample_weights
-        self.sync_scalar_grads, self.bidir = sync_scalar_grads, bidir
-        self.multi_positive = multi_positive
-        self.batch_per_rank = batch_per_rank
-        self.hard_negatives = hard_negatives
-        self.extra_texts = extra_texts
         self._engines: Dict[Tuple[int, int, int, int], SigmoidLossEngine] = {}
 
     def get(self, batch: int, dim: int, device: torch.device, teacher_dim: int = 0) -> SigmoidLossEngine:
         key = (device.index if device.index is not None else torch.cuda.current_device(), batch, dim, teacher_dim)
         eng = self._engines.get(key)
         if eng is None:
+            o = self.options
             dev = torch.device("cuda", key[0])
             if not self._topology_known:
-                self._topology = cross_node.topology(self.group, self.ranks_per_node)
+                self._topology = cross_node.topology(self.group, o.ranks_per_node)
                 self._topology_known = True
             topo = self._topology
             tpr = ipr = None
-            extras = self.hard_negatives + self.extra_texts   # at most one of the two is non-zero
+            extras = o.hard_negatives + o.extra_texts   # at most one of the two is non-zero
             rank, world = _group_rank_world(self.group)
             bpr = self.batch_per_rank if self.batch_per_rank is not None else [batch] * world
             if extras:
                 # every rank scores the same number K of extras: T_p = B_p + K
                 tpr = [int(b) + extras for b in bpr]
-            if self.extra_images:
+            if o.extra_images:
                 # every rank holds the same number K of extra images: R_p = B_p + K
-                ipr = [int(b) + self.extra_images for b in bpr]
+                ipr = [int(b) + o.extra_images for b in bpr]
             if topo is None:
                 eng = SigmoidLossEngine(batch, dim, dev, self.group, self.cta_group, self.overlap_pull,
                                         batch_per_rank=self.batch_per_rank, texts_per_rank=tpr, images_per_rank=ipr,
-                                        teacher_dim=teacher_dim, labels=self.multi_label,
-                                        distill_options=self.distill_options and teacher_dim > 0)
+                                        teacher_dim=teacher_dim, labels=o.multi_label,
+                                        distill_options=o.distill_options and teacher_dim > 0)
             else:
                 eng = self._node_engine(topo, batch, dim, dev, [int(b) for b in bpr], extras, teacher_dim)
             if self.sync_scalar_grads:
                 eng.set_option(_capi.SIGLIP_OPT_SYNC_SCALAR_GRADS, 1)
             if self.bidir:
                 eng.set_option(_capi.SIGLIP_OPT_BIDIR, 1)
-            if self.multi_positive:
+            if o.multi_positive:
                 eng.set_option(_capi.SIGLIP_OPT_SAMPLE_IDS, 1)
-            if self.multi_label:
+            if o.multi_label:
                 eng.set_option(_capi.SIGLIP_OPT_LABEL_SETS, 1)
-            if (self.extra_texts and not self.multi_label) or (topo is not None and self.multi_positive):
+            if (o.extra_texts and not o.multi_label) or (topo is not None and o.multi_positive):
                 # needs the sample ids on first; across nodes the remote rows carry their owners' ids
                 eng.set_option(_capi.SIGLIP_OPT_EXTRA_TEXT_IDS, 1)
-            if self.extra_images and self.multi_positive:
+            if o.extra_images and o.multi_positive:
                 eng.set_option(_capi.SIGLIP_OPT_EXTRA_IMAGE_IDS, 1)
-            if self.sample_weights:
+            if o.sample_weights:
                 eng.set_option(_capi.SIGLIP_OPT_SAMPLE_WEIGHTS, 1)
-            if self.distill is not None:
+            if o.distill is not None:
                 eng.set_option(_capi.SIGLIP_OPT_DISTILL, 1)
-            if self.exclude_groups:
+            if o.exclude_groups:
                 eng.set_option(_capi.SIGLIP_OPT_EXCLUDE_GROUPS, 1)
-            if self.focal is not None:
+            if o.focal is not None:
                 eng.set_option(_capi.SIGLIP_OPT_FOCAL, 1)
-                eng.set_focal(*self.focal)
-            if self.sigma_budget_bytes:
-                eng.set_sigma_budget(self.sigma_budget_bytes)
+                eng.set_focal(*o.focal)
+            if o.sigma_budget_bytes:
+                eng.set_sigma_budget(o.sigma_budget_bytes)
             self._engines[key] = eng
         return eng
 
@@ -1043,17 +1056,18 @@ class _EngineCache:
                      teacher_dim: int) -> SigmoidLossEngine:
         """The context of this rank's node in a group that spans nodes: local rank l of L, every local rank holding its
         own texts and those of its counterparts on the other nodes (cross_node)."""
-        cross_node.check_options(self.distill, self.multi_positive, self.hard_negatives)
+        o = self.options
+        cross_node.check_options(o.distill, o.multi_positive, o.hard_negatives)
         if len(bpr) != topo.world:
             raise RuntimeError(f"batch_per_rank {bpr} must list one batch per rank of the group ({topo.world})")
         group_tpr = [b + extras for b in bpr]
         base, L = topo.node_base, topo.ranks_per_node
         node_bpr = bpr[base:base + L]
-        ipr = [b + self.extra_images for b in node_bpr] if self.extra_images else None
+        ipr = [b + o.extra_images for b in node_bpr] if o.extra_images else None
         eng = SigmoidLossEngine(batch, dim, dev, self.group, self.cta_group, self.overlap_pull,
                                 rank_world=(topo.local, L), batch_per_rank=node_bpr,
                                 texts_per_rank=topo.node_texts_per_rank(group_tpr), images_per_rank=ipr,
-                                teacher_dim=teacher_dim, labels=self.multi_label, node_base=base)
+                                teacher_dim=teacher_dim, labels=o.multi_label, node_base=base)
         eng.topology, eng.group_texts_per_rank = topo, group_tpr
         return eng
 
@@ -1086,24 +1100,34 @@ def _fused_under_budget(eng, fused_step: Optional[bool]) -> bool:
 _ID_DTYPES = (torch.int8, torch.uint8, torch.int16, torch.int32, torch.int64)
 
 
+def _int_tensor(x, name: str, shape: Tuple, per: str, like: torch.Tensor, whose: str) -> torch.Tensor:
+    """An integer input of a forward (ids, groups, label sets): an integer tensor of `shape` (`per`: what its rows are,
+    for the message) on the device of `like` (`whose`: what `like` holds). Returns it as contiguous int64, what the
+    kernels compare."""
+    if not isinstance(x, torch.Tensor) or x.dtype not in _ID_DTYPES:
+        raise RuntimeError(f"{name} must be an integer tensor, got "
+                           f"{x.dtype if isinstance(x, torch.Tensor) else type(x)}")
+    if tuple(x.shape) != shape:
+        raise RuntimeError(f"{name} must have shape [{', '.join(map(str, shape))}] ({per}), got {tuple(x.shape)}")
+    if x.device != like.device:
+        raise RuntimeError(f"{name} are on {x.device}, the {whose} on {like.device}")
+    return x.to(torch.int64).contiguous()
+
+
+def _rows(x: torch.Tensor) -> Optional[int]:
+    return x.shape[0] if x.dim() >= 1 else None
+
+
 def _validate_ids(sample_ids, multi_positive: bool, embeddings: torch.Tensor) -> Optional[torch.Tensor]:
     """sample_ids of a forward: required ([B] integers on the embeddings' device) with multi_positive, refused without.
-    Returns them as contiguous int64 (what the kernels compare), or None. Raises before any GPU work."""
+    Returns them as contiguous int64, or None. Raises before any GPU work."""
     if not multi_positive:
         if sample_ids is not None:
             raise RuntimeError("sample_ids given, but the loss was built without multi_positive=True")
         return None
     if sample_ids is None:
         raise RuntimeError("multi_positive=True: forward needs sample_ids ([batch] integer tensor, one id per sample)")
-    if not isinstance(sample_ids, torch.Tensor) or sample_ids.dtype not in _ID_DTYPES:
-        raise RuntimeError(f"sample_ids must be an integer tensor, got "
-                           f"{sample_ids.dtype if isinstance(sample_ids, torch.Tensor) else type(sample_ids)}")
-    batch = embeddings.shape[0] if embeddings.dim() >= 1 else None
-    if sample_ids.dim() != 1 or sample_ids.shape[0] != batch:
-        raise RuntimeError(f"sample_ids must have shape [{batch}] (one id per sample), got {tuple(sample_ids.shape)}")
-    if sample_ids.device != embeddings.device:
-        raise RuntimeError(f"sample_ids are on {sample_ids.device}, the embeddings on {embeddings.device}")
-    return sample_ids.to(torch.int64).contiguous()
+    return _int_tensor(sample_ids, "sample_ids", (_rows(embeddings),), "one id per sample", embeddings, "embeddings")
 
 
 def _validate_hard_negatives(hard_negatives, name: str = "hard_negatives") -> int:
@@ -1156,15 +1180,8 @@ def _validate_extra_text_ids(extra_text_ids, extra_texts: int, text_embeddings: 
         return None
     if extra_text_ids is None:
         raise RuntimeError(f"extra_texts={extra_texts}: forward needs extra_text_ids ([{extra_texts}] integer tensor)")
-    if not isinstance(extra_text_ids, torch.Tensor) or extra_text_ids.dtype not in _ID_DTYPES:
-        raise RuntimeError(f"extra_text_ids must be an integer tensor, got "
-                           f"{extra_text_ids.dtype if isinstance(extra_text_ids, torch.Tensor) else type(extra_text_ids)}")
-    if extra_text_ids.dim() != 1 or extra_text_ids.shape[0] != extra_texts:
-        raise RuntimeError(f"extra_text_ids must have shape [{extra_texts}] (one id per extra text), got "
-                           f"{tuple(extra_text_ids.shape)}")
-    if extra_text_ids.device != text_embeddings.device:
-        raise RuntimeError(f"extra_text_ids are on {extra_text_ids.device}, the texts on {text_embeddings.device}")
-    return extra_text_ids.to(torch.int64).contiguous()
+    return _int_tensor(extra_text_ids, "extra_text_ids", (extra_texts,), "one id per extra text", text_embeddings,
+                       "texts")
 
 
 def _validate_extra_image_ids(extra_image_ids, extra_images: int, multi_positive: bool,
@@ -1180,15 +1197,8 @@ def _validate_extra_image_ids(extra_image_ids, extra_images: int, multi_positive
     if extra_image_ids is None:
         raise RuntimeError(f"extra_images={extra_images} with multi_positive=True: forward needs extra_image_ids "
                            f"([{extra_images}] integer tensor)")
-    if not isinstance(extra_image_ids, torch.Tensor) or extra_image_ids.dtype not in _ID_DTYPES:
-        raise RuntimeError(f"extra_image_ids must be an integer tensor, got "
-                           f"{extra_image_ids.dtype if isinstance(extra_image_ids, torch.Tensor) else type(extra_image_ids)}")
-    if extra_image_ids.dim() != 1 or extra_image_ids.shape[0] != extra_images:
-        raise RuntimeError(f"extra_image_ids must have shape [{extra_images}] (one id per extra image), got "
-                           f"{tuple(extra_image_ids.shape)}")
-    if extra_image_ids.device != image_embeddings.device:
-        raise RuntimeError(f"extra_image_ids are on {extra_image_ids.device}, the images on {image_embeddings.device}")
-    return extra_image_ids.to(torch.int64).contiguous()
+    return _int_tensor(extra_image_ids, "extra_image_ids", (extra_images,), "one id per extra image", image_embeddings,
+                       "images")
 
 
 def _validate_sample_weights(sample_weights) -> bool:
@@ -1227,11 +1237,10 @@ def _weights_of(sample_weights: bool, image_weights, text_weights, image_embeddi
     """Both weight arguments checked; (image_weights, text_weights) for the step, or None without sample_weights. The
     texts are the paired ones followed by the K extras, so text_weights has B + K entries; the images likewise, so
     image_weights has B + K_img entries."""
-    rows = lambda x: x.shape[0] if x.dim() >= 1 else None  # noqa: E731
-    ni = rows(image_embeddings)
+    ni = _rows(image_embeddings)
     iw = _validate_weights(image_weights, sample_weights, ni + extra_images if ni is not None else None,
                            "image_weights", image_embeddings.device)
-    nt = rows(text_embeddings)
+    nt = _rows(text_embeddings)
     tw = _validate_weights(text_weights, sample_weights, nt + extras if nt is not None else None, "text_weights",
                            text_embeddings.device)
     return (iw, tw) if sample_weights else None
@@ -1248,17 +1257,10 @@ def _validate_exclude_groups(exclude_groups, distill) -> bool:
     return exclude_groups
 
 
-def _validate_group_ids(groups, n: Optional[int], name: str, what: str, device: torch.device) -> torch.Tensor:
+def _validate_group_ids(groups, n: Optional[int], name: str, what: str, embeddings: torch.Tensor) -> torch.Tensor:
     if groups is None:
         raise RuntimeError(f"exclude_groups=True: forward needs {name} ([{n}] integer tensor, one group per {what[:-1]})")
-    if not isinstance(groups, torch.Tensor) or groups.dtype not in _ID_DTYPES:
-        raise RuntimeError(f"{name} must be an integer tensor, got "
-                           f"{groups.dtype if isinstance(groups, torch.Tensor) else type(groups)}")
-    if groups.dim() != 1 or groups.shape[0] != n:
-        raise RuntimeError(f"{name} must have shape [{n}] (one group per {what[:-1]}), got {tuple(groups.shape)}")
-    if groups.device != device:
-        raise RuntimeError(f"{name} are on {groups.device}, the {what} on {device}")
-    return groups.to(torch.int64).contiguous()
+    return _int_tensor(groups, name, (n,), f"one group per {what[:-1]}", embeddings, what)
 
 
 def _groups_of(exclude_groups: bool, image_groups, text_groups, image_embeddings: torch.Tensor,
@@ -1271,12 +1273,11 @@ def _groups_of(exclude_groups: bool, image_groups, text_groups, image_embeddings
             if v is not None:
                 raise RuntimeError(f"{name} given, but the loss was built without exclude_groups=True")
         return None
-    ni = image_embeddings.shape[0] if image_embeddings.dim() >= 1 else None
-    nt = text_embeddings.shape[0] if text_embeddings.dim() >= 1 else None
+    ni, nt = _rows(image_embeddings), _rows(text_embeddings)
     gi = _validate_group_ids(image_groups, ni + extra_images if ni is not None else None, "image_groups", "images",
-                             image_embeddings.device)
+                             image_embeddings)
     gt = _validate_group_ids(text_groups, nt + extras if nt is not None else None, "text_groups", "texts",
-                             text_embeddings.device)
+                             text_embeddings)
     return gi, gt
 
 
@@ -1297,19 +1298,12 @@ def _validate_multi_label(multi_label, multi_positive: bool, distill) -> int:
     return multi_label
 
 
-def _validate_label_set(labels, n: Optional[int], m: int, name: str, what: str, device: torch.device) -> torch.Tensor:
+def _validate_label_set(labels, n: Optional[int], m: int, name: str, what: str,
+                        embeddings: torch.Tensor) -> torch.Tensor:
     if labels is None:
         raise RuntimeError(f"multi_label={m}: forward needs {name} ([{n}, {m}] integer tensor, one label set per "
                            f"{what})")
-    if not isinstance(labels, torch.Tensor) or labels.dtype not in _ID_DTYPES:
-        raise RuntimeError(f"{name} must be an integer tensor, got "
-                           f"{labels.dtype if isinstance(labels, torch.Tensor) else type(labels)}")
-    if labels.dim() != 2 or tuple(labels.shape) != (n, m):
-        raise RuntimeError(f"{name} must have shape [{n}, {m}] (one set of {m} labels per {what}), got "
-                           f"{tuple(labels.shape)}")
-    if labels.device != device:
-        raise RuntimeError(f"{name} are on {labels.device}, the embeddings on {device}")
-    return labels.to(torch.int64).contiguous()
+    return _int_tensor(labels, name, (n, m), f"one set of {m} labels per {what}", embeddings, "embeddings")
 
 
 def _label_sets_of(multi_label: int, sample_labels, extra_text_labels, extra_image_labels,
@@ -1331,13 +1325,12 @@ def _label_sets_of(multi_label: int, sample_labels, extra_text_labels, extra_ima
                            "empty label sets)")
     if extra_images == 0 and extra_image_labels is not None:
         raise RuntimeError("extra_image_labels given, but the loss was built without extra_images=K")
-    dev = image_embeddings.device
-    nb = image_embeddings.shape[0] if image_embeddings.dim() >= 1 else None
-    ls = _validate_label_set(sample_labels, nb, multi_label, "sample_labels", "sample", dev)
+    emb = image_embeddings
+    ls = _validate_label_set(sample_labels, _rows(emb), multi_label, "sample_labels", "sample", emb)
     lt = _validate_label_set(extra_text_labels, extra_texts, multi_label, "extra_text_labels", "extra text",
-                             dev) if extra_texts else None
+                             emb) if extra_texts else None
     li = _validate_label_set(extra_image_labels, extra_images, multi_label, "extra_image_labels", "extra image",
-                             dev) if extra_images else None
+                             emb) if extra_images else None
     return ls, lt, li
 
 
@@ -1442,13 +1435,6 @@ def _teacher_of(distill: Optional[float], image_embeddings: torch.Tensor, names,
     return (_pad_dim(timg), _pad_dim(ttxt), tscale, tbias, distill)
 
 
-def _teacher_extras(mod, negative_text, extra_text, extra_image):
-    """The teacher-extras argument of _teacher_of for a module (DDPSigmoidLoss or SigLipLoss)."""
-    return (("teacher_negative_text", negative_text, mod.hard_negatives, "text"),
-            ("teacher_extra_text", extra_text, mod.extra_texts, "text"),
-            ("teacher_extra_image", extra_image, mod.extra_images, "image"))
-
-
 def _validate_return_metrics(return_metrics) -> None:
     if not isinstance(return_metrics, bool):
         raise RuntimeError(f"return_metrics must be a bool, got {type(return_metrics).__name__}")
@@ -1537,17 +1523,110 @@ def _validate(image_embeddings: torch.Tensor, text_embeddings: torch.Tensor, exp
         raise RuntimeError("distributed_sigmoid_loss_b200 runs on CUDA (sm_90a) tensors only; there is no CPU path")
 
 
-def _node_step(mod, eng, text, t_prime, bias, sync_scalars: bool, ids, extra_ids, weights, groups, label_sets):
+# the teacher's image, text, scale and bias arguments of each module's forward
+_DDP_TEACHER = ("teacher_image", "teacher_text", "teacher_t_prime", "teacher_bias")
+_SIGLIP_TEACHER = ("teacher_image", "teacher_text", "teacher_logit_scale", "teacher_logit_bias")
+
+
+def _loss_options(multi_positive, hard_negatives, extra_texts, sample_weights, extra_images, distill,
+                  sigma_budget_bytes, exclude_groups, multi_label, focal_gamma, focal_alpha, distill_options,
+                  ranks_per_node) -> _LossOptions:
+    """The shared options of a module's constructor, checked in this order. Raises before any GPU work."""
+    _sigma_budget_mib(sigma_budget_bytes)
+    ranks_per_node = cross_node.validate_ranks_per_node(ranks_per_node)
+    hard_negatives = _validate_hard_negatives(hard_negatives)
+    extra_images = _validate_hard_negatives(extra_images, "extra_images")
+    closed = None if distill_options is True else distill
+    multi_label = _validate_multi_label(multi_label, multi_positive, closed)
+    # extra texts carry ids under multi_positive, label sets under multi_label
+    extra_texts = _validate_extra_texts(extra_texts, multi_positive or bool(multi_label), hard_negatives)
+    sample_weights = _validate_sample_weights(sample_weights)
+    distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images, distill_options)
+    closed = None if distill_options else distill
+    exclude_groups = _validate_exclude_groups(exclude_groups, closed)
+    focal = _validate_focal(focal_gamma, focal_alpha, distill)
+    return _LossOptions(multi_positive, hard_negatives, extra_texts, sample_weights, extra_images, distill,
+                        distill_options, closed, exclude_groups, multi_label, focal, sigma_budget_bytes, ranks_per_node)
+
+
+def _step_inputs(o: _LossOptions, args, image_embeddings, text_embeddings, expect_batch: Optional[int],
+                 teacher_names) -> Tuple[_StepInputs, int]:
+    """A forward's arguments (args: by name) checked against the options, in this order: (the step's inputs, top-K's
+    K). teacher_names: the forward's names of the teacher's image, text, scale and bias. Raises before any GPU work."""
+    return_metrics = args["return_metrics"]
+    _validate_return_metrics(return_metrics)
+    _validate_return_sample_losses(args["return_sample_losses"], o.distill_closed)
+    topk = _validate_metrics_topk(args["metrics_topk"], return_metrics, o.distill_closed)
+    teacher = _teacher_of(o.distill, image_embeddings, teacher_names, [args[n] for n in teacher_names],
+                          (("teacher_negative_text", args["teacher_negative_text"], o.hard_negatives, "text"),
+                           ("teacher_extra_text", args["teacher_extra_text"], o.extra_texts, "text"),
+                           ("teacher_extra_image", args["teacher_extra_image"], o.extra_images, "image")))
+    ids = _validate_ids(args["sample_ids"], o.multi_positive, image_embeddings)
+    _validate_negatives(text_embeddings, args["negative_text"], o.hard_negatives)
+    _validate_negatives(text_embeddings, args["extra_text"], o.extra_texts, "extra_text", "extra_texts")
+    extra_ids = _validate_extra_text_ids(args["extra_text_ids"], 0 if o.multi_label else o.extra_texts,
+                                         text_embeddings)
+    _validate_negatives(image_embeddings, args["extra_image"], o.extra_images, "extra_image", "extra_images", "images")
+    ximg_ids = _validate_extra_image_ids(args["extra_image_ids"], o.extra_images, o.multi_positive, image_embeddings)
+    extras = o.hard_negatives + o.extra_texts
+    weights = _weights_of(o.sample_weights, args["image_weights"], args["text_weights"], image_embeddings,
+                          text_embeddings, extras, o.extra_images)
+    groups = _groups_of(o.exclude_groups, args["image_groups"], args["text_groups"], image_embeddings, text_embeddings,
+                        extras, o.extra_images)
+    label_sets = _label_sets_of(o.multi_label, args["sample_labels"], args["extra_text_labels"],
+                                args["extra_image_labels"], image_embeddings, o.extra_texts, o.extra_images)
+    _validate(image_embeddings, text_embeddings, expect_batch)
+    return _StepInputs(ids, extra_ids, ximg_ids, weights, groups, label_sets, teacher), topk
+
+
+def _loss_forward(mod, args, image_embeddings, text_embeddings, t_prime, bias, expect_batch: Optional[int],
+                  normalize: bool, sync_scalar_grads: bool, rank_world: Optional[Tuple[int, int]], teacher_names):
+    """The forward of DDPSigmoidLoss and SigLipLoss: the checks, the extras appended to their embeddings, the engine,
+    the exchange across nodes and the step. args: the forward's arguments by name (its locals() on entry: one dict,
+    not two dozen keyword arguments passed on per step). rank_world: SigLipLoss's (rank, world_size), checked against
+    the group. Returns (loss, metric buffers or None, per-sample-loss buffers or None)."""
+    inputs, topk = _step_inputs(mod._options, args, image_embeddings, text_embeddings, expect_batch, teacher_names)
+    batch = image_embeddings.shape[0]
+    text_embeddings = _with_negatives(_with_negatives(text_embeddings, args["negative_text"]), args["extra_text"])
+    image_embeddings = _with_negatives(image_embeddings, args["extra_image"])
+    image_embeddings, text_embeddings = _pad_dim(image_embeddings), _pad_dim(text_embeddings)
+    eng = mod._cache.get(batch, image_embeddings.shape[1], image_embeddings.device,
+                         inputs.teacher[0].shape[1] if inputs.teacher is not None else 0)
+    topo = eng.topology
+    if rank_world is not None:
+        have = (eng.rank, eng.world) if topo is None else (topo.rank, topo.world)
+        if have != rank_world:
+            raise RuntimeError(
+                f"SigLipLoss(rank={rank_world[0]}, world_size={rank_world[1]}) does not match the process group "
+                f"(rank={have[0]}, world_size={have[1]})")
+    rows = text_embeddings.shape[0]
+    if topo is not None:
+        cross_node.check_forward(args["return_metrics"])
+        text_embeddings, t_prime, bias, inputs = _node_step(eng, text_embeddings, t_prime, bias, sync_scalar_grads,
+                                                            inputs)
+    fused = _fused_under_budget(eng, mod.fused_step)
+    bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if args["return_metrics"] \
+        else None
+    bufs = _topk_buffers(eng, topk, bufs)
+    lbufs = _sample_loss_buffers(eng) if args["return_sample_losses"] else None
+    loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, t_prime, bias, eng, normalize, fused, inputs, bufs,
+                                lbufs)
+    return loss, bufs, _fold_text_loss(eng, lbufs, rows)
+
+
+def _node_step(eng, text, t_prime, bias, sync_scalars: bool, inputs: _StepInputs):
     """The inputs of a node context's step in a group that spans nodes (eng.topology set): this rank's text rows
     [T, D] (captions, then extras) followed by its counterparts' rows, and the per-text data that rides with them:
     the owners' ids (captions' sample ids, extra texts' ids) as extra-text ids, their text weights, text groups and
     label sets (hard negatives: empty sets). Images and their data stay on their rank. Returns (text, t_prime, bias,
-    extra_ids, weights, groups, label_sets) for _SigmoidLossFn; t_prime / bias pass through the exchange so that
-    sync_scalar_grads averages their gradients over the nodes."""
+    inputs) for _SigmoidLossFn; t_prime / bias pass through the exchange so that sync_scalar_grads averages their
+    gradients over the nodes."""
     topo, tpr, group = eng.topology, eng.group_texts_per_rank, eng.group
     rows, B = text.shape[0], eng.batch
+    ids, extra_ids, weights, groups, label_sets = (inputs.ids, inputs.extra_text_ids, inputs.weights, inputs.groups,
+                                                   inputs.label_sets)
     cols = []
-    if mod.multi_positive:
+    if ids is not None:   # multi_positive
         cols.append(ids if extra_ids is None else torch.cat([ids, extra_ids]))
     if weights is not None:
         tw = weights[1] if weights[1] is not None else torch.ones(rows, device=text.device, dtype=torch.float32)
@@ -1565,7 +1644,7 @@ def _node_step(mod, eng, text, t_prime, bias, sync_scalars: bool, ids, extra_ids
         own = torch.cat(cols, dim=1)
         both = torch.cat([own, cross_node.send_rows(own, topo, tpr, group)])
         c = 0
-        if mod.multi_positive:
+        if ids is not None:
             extra_ids = both[B:, 0].contiguous()
             c += 1
         if weights is not None:
@@ -1576,7 +1655,9 @@ def _node_step(mod, eng, text, t_prime, bias, sync_scalars: bool, ids, extra_ids
             c += 1
         if label_sets is not None:
             label_sets = (label_sets[0], both[B:, c:].contiguous(), label_sets[2])
-    return text, t_prime, bias, extra_ids, weights, groups, label_sets
+        inputs = dataclasses.replace(inputs, extra_text_ids=extra_ids, weights=weights, groups=groups,
+                                     label_sets=label_sets)
+    return text, t_prime, bias, inputs
 
 
 def _fold_text_loss(eng, lbufs, rows: int):
@@ -1594,6 +1675,7 @@ def _pad_dim(x: torch.Tensor) -> torch.Tensor:
     return x if d % 8 == 0 else torch.nn.functional.pad(x, (0, 8 - d % 8))
 
 
+@_with_option_attributes
 class DDPSigmoidLoss(nn.Module):
     """Drop-in for the reference ``DDPSigmoidLoss`` (distributed_sigmoid_loss.py:8-48).
 
@@ -1749,20 +1831,9 @@ class DDPSigmoidLoss(nn.Module):
                  focal_gamma: Optional[float] = None, focal_alpha: Optional[float] = None,
                  distill_options: bool = False, ranks_per_node: Optional[int] = None) -> None:
         super().__init__()
-        _sigma_budget_mib(sigma_budget_bytes)
-        ranks_per_node = cross_node.validate_ranks_per_node(ranks_per_node)
-        hard_negatives = _validate_hard_negatives(hard_negatives)
-        extra_images = _validate_hard_negatives(extra_images, "extra_images")
-        # distill_closed: what the option checks refuse, distill=lambda without distill_options (None otherwise)
-        closed = None if distill_options is True else distill
-        multi_label = _validate_multi_label(multi_label, multi_positive, closed)
-        # extra texts carry ids under multi_positive, label sets under multi_label
-        extra_texts = _validate_extra_texts(extra_texts, multi_positive or bool(multi_label), hard_negatives)
-        sample_weights = _validate_sample_weights(sample_weights)
-        distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images, distill_options)
-        self.distill_closed = None if distill_options else distill
-        exclude_groups = _validate_exclude_groups(exclude_groups, self.distill_closed)
-        focal = _validate_focal(focal_gamma, focal_alpha, distill)
+        self._options = _loss_options(multi_positive, hard_negatives, extra_texts, sample_weights, extra_images,
+                                      distill, sigma_budget_bytes, exclude_groups, multi_label, focal_gamma,
+                                      focal_alpha, distill_options, ranks_per_node)
         self.t_prime = nn.Parameter(torch.tensor(math.log(10), dtype=torch.float64))
         self.bias = nn.Parameter(torch.tensor(-10.0))
         self.gpu_batch_size = gpu_batch_size
@@ -1776,32 +1847,8 @@ class DDPSigmoidLoss(nn.Module):
         # rank, the split forward / backward otherwise (one operand either way; saves the multiply by grad_output)
         self.fused_step = fused_step
         # extension (SURVEY.md §8f-4): per-rank batch sizes may differ; every rank passes the same list
-        # extension: labels from per-sample ids (positive iff same id, across ranks too)
-        self.multi_positive = multi_positive
-        # extension: hard-negative captions, K extra texts per rank scored against every image
-        self.hard_negatives = hard_negatives
-        # extension: extra captions with ids of their own (several captions per image)
-        self.extra_texts = extra_texts
-        # extension: per-sample loss weights (weight 0 drops a sample at a fixed batch shape)
-        self.sample_weights = sample_weights
-        # extension: extra images per rank (hard-negative images, or with ids several images per caption)
-        self.extra_images = extra_images
-        # extension: distillation from a frozen teacher (soft targets from the teacher's embeddings)
-        self.distill = distill
-        # extension: same-group pairs excluded from the loss (in-batch false negatives made neutral)
-        self.exclude_groups = exclude_groups
-        # extension: multi-label positives from per-sample label sets (0: off)
-        self.multi_label = multi_label
-        # extension: the focal pair loss (torchvision's sigmoid_focal_loss), (gamma, alpha) or None
-        self.focal = focal
-        self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, batch_per_rank=batch_per_rank,
-                                   multi_positive=multi_positive, hard_negatives=hard_negatives,
-                                   extra_texts=extra_texts, sample_weights=sample_weights, extra_images=extra_images,
-                                   distill=distill, sigma_budget_bytes=sigma_budget_bytes,
-                                   exclude_groups=exclude_groups, multi_label=multi_label, focal=focal,
-                                   distill_options=distill_options, ranks_per_node=ranks_per_node)
-        # extension: bound of the 16-bit sigma operands; steps then run in row panels (memory O(budget), not O(B^2))
-        self.sigma_budget_bytes = sigma_budget_bytes
+        self._cache = _EngineCache(group, cta_group, overlap_pull, sync_scalar_grads, False, batch_per_rank,
+                                   self._options)
 
     def engine_for(self, batch: int, dim: int, device: torch.device, teacher_dim: int = 0) -> SigmoidLossEngine:
         """The engine forward() uses for these shapes. A module built with distill=lambda needs the teacher's width
@@ -1824,51 +1871,15 @@ class DDPSigmoidLoss(nn.Module):
                 teacher_negative_text: Optional[torch.Tensor] = None,
                 teacher_extra_text: Optional[torch.Tensor] = None,
                 teacher_extra_image: Optional[torch.Tensor] = None):
-        _validate_return_metrics(return_metrics)
-        _validate_return_sample_losses(return_sample_losses, self.distill_closed)
-        topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill_closed)
-        teacher = _teacher_of(self.distill, image_embeddings,
-                              ("teacher_image", "teacher_text", "teacher_t_prime", "teacher_bias"),
-                              (teacher_image, teacher_text, teacher_t_prime, teacher_bias),
-                              _teacher_extras(self, teacher_negative_text, teacher_extra_text, teacher_extra_image))
-        ids = _validate_ids(sample_ids, self.multi_positive, image_embeddings)
-        _validate_negatives(text_embeddings, negative_text, self.hard_negatives)
-        _validate_negatives(text_embeddings, extra_text, self.extra_texts, "extra_text", "extra_texts")
-        extra_ids = _validate_extra_text_ids(extra_text_ids, 0 if self.multi_label else self.extra_texts,
-                                             text_embeddings)
-        _validate_negatives(image_embeddings, extra_image, self.extra_images, "extra_image", "extra_images", "images")
-        ximg_ids = _validate_extra_image_ids(extra_image_ids, self.extra_images, self.multi_positive, image_embeddings)
-        weights = _weights_of(self.sample_weights, image_weights, text_weights, image_embeddings, text_embeddings,
-                              self.hard_negatives + self.extra_texts, self.extra_images)
-        groups = _groups_of(self.exclude_groups, image_groups, text_groups, image_embeddings, text_embeddings,
-                            self.hard_negatives + self.extra_texts, self.extra_images)
-        label_sets = _label_sets_of(self.multi_label, sample_labels, extra_text_labels, extra_image_labels,
-                                    image_embeddings, self.extra_texts, self.extra_images)
-        _validate(image_embeddings, text_embeddings, self.gpu_batch_size)
-        text_embeddings = _with_negatives(_with_negatives(text_embeddings, negative_text), extra_text)
-        image_embeddings = _with_negatives(image_embeddings, extra_image)
-        image_embeddings, text_embeddings = _pad_dim(image_embeddings), _pad_dim(text_embeddings)
-        eng = self._cache.get(self.gpu_batch_size, image_embeddings.shape[1], image_embeddings.device,
-                              teacher[0].shape[1] if teacher is not None else 0)
-        t_prime, bias, rows = self.t_prime, self.bias, text_embeddings.shape[0]
-        if eng.topology is not None:
-            cross_node.check_forward(return_metrics)
-            text_embeddings, t_prime, bias, extra_ids, weights, groups, label_sets = _node_step(
-                self, eng, text_embeddings, t_prime, bias, self.sync_scalar_grads, ids, extra_ids, weights, groups,
-                label_sets)
-        fused = _fused_under_budget(eng, self.fused_step)
-        bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
-        bufs = _topk_buffers(eng, topk, bufs)
-        lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
-        loss = _SigmoidLossFn.apply(image_embeddings, text_embeddings, t_prime, bias, eng,
-                                    self.normalize_inputs, fused, ids, bufs, extra_ids, weights, ximg_ids, teacher,
-                                    lbufs, groups, label_sets)
-        return _with_outputs(loss, bufs, _fold_text_loss(eng, lbufs, rows))
+        return _with_outputs(*_loss_forward(self, locals(), image_embeddings, text_embeddings, self.t_prime, self.bias,
+                                            self.gpu_batch_size, self.normalize_inputs, self.sync_scalar_grads, None,
+                                            _DDP_TEACHER))
 
 
 SigmoidLoss = DDPSigmoidLoss
 
 
+@_with_option_attributes
 class SigLipLoss(nn.Module):
     """open_clip-signature adapter (rwightman_sigmoid_loss.py:12-124): scale and bias are passed in, the ring
     exchange of the original is replaced by the direct NVSwitch pulls of the fused path. ``bidir`` selects the
@@ -1906,38 +1917,14 @@ class SigLipLoss(nn.Module):
                  focal_alpha: Optional[float] = None, distill_options: bool = False,
                  ranks_per_node: Optional[int] = None):
         super().__init__()
-        _sigma_budget_mib(sigma_budget_bytes)
-        ranks_per_node = cross_node.validate_ranks_per_node(ranks_per_node)
         assert not use_horovod  # same restriction as the reference (rwightman_sigmoid_loss.py:35)
-        hard_negatives = _validate_hard_negatives(hard_negatives)
-        extra_images = _validate_hard_negatives(extra_images, "extra_images")
-        closed = None if distill_options is True else distill   # as on DDPSigmoidLoss
-        multi_label = _validate_multi_label(multi_label, multi_positive, closed)
-        extra_texts = _validate_extra_texts(extra_texts, multi_positive or bool(multi_label), hard_negatives)
-        sample_weights = _validate_sample_weights(sample_weights)
-        distill = _validate_distill(distill, hard_negatives, extra_texts, extra_images, distill_options)
-        self.distill_closed = None if distill_options else distill
-        exclude_groups = _validate_exclude_groups(exclude_groups, self.distill_closed)
-        focal = _validate_focal(focal_gamma, focal_alpha, distill)
-        self.focal = focal
-        self.distill = distill
-        self.exclude_groups = exclude_groups
-        self.multi_label = multi_label
+        self._options = _loss_options(multi_positive, hard_negatives, extra_texts, sample_weights, extra_images,
+                                      distill, sigma_budget_bytes, exclude_groups, multi_label, focal_gamma,
+                                      focal_alpha, distill_options, ranks_per_node)
         self.cache_labels, self.rank, self.world_size, self.bidir = cache_labels, rank, world_size, bidir
         self.use_horovod = use_horovod
         self.fused_step = fused_step
-        self.multi_positive = multi_positive
-        self.hard_negatives = hard_negatives
-        self.extra_texts = extra_texts
-        self.sample_weights = sample_weights
-        self.extra_images = extra_images
-        self._cache = _EngineCache(group, cta_group, bidir=bidir, multi_positive=multi_positive,
-                                   hard_negatives=hard_negatives, extra_texts=extra_texts, sample_weights=sample_weights,
-                                   extra_images=extra_images, distill=distill, sigma_budget_bytes=sigma_budget_bytes,
-                                   exclude_groups=exclude_groups, multi_label=multi_label, focal=focal,
-                                   distill_options=distill_options, ranks_per_node=ranks_per_node)
-        # bound of the 16-bit sigma operands; steps then run in row panels (as on DDPSigmoidLoss)
-        self.sigma_budget_bytes = sigma_budget_bytes
+        self._cache = _EngineCache(group, cta_group, True, False, bidir, None, self._options)
 
     def forward(self, image_features, text_features, logit_scale, logit_bias, output_dict: bool = False, *,
                 negative_text: Optional[torch.Tensor] = None, sample_ids: Optional[torch.Tensor] = None,
@@ -1953,50 +1940,9 @@ class SigLipLoss(nn.Module):
                 teacher_negative_text: Optional[torch.Tensor] = None,
                 teacher_extra_text: Optional[torch.Tensor] = None,
                 teacher_extra_image: Optional[torch.Tensor] = None):
-        _validate_return_metrics(return_metrics)
-        _validate_return_sample_losses(return_sample_losses, self.distill_closed)
-        topk = _validate_metrics_topk(metrics_topk, return_metrics, self.distill_closed)
-        teacher = _teacher_of(self.distill, image_features,
-                              ("teacher_image", "teacher_text", "teacher_logit_scale", "teacher_logit_bias"),
-                              (teacher_image, teacher_text, teacher_logit_scale, teacher_logit_bias),
-                              _teacher_extras(self, teacher_negative_text, teacher_extra_text, teacher_extra_image))
-        ids = _validate_ids(sample_ids, self.multi_positive, image_features)
-        _validate_negatives(text_features, negative_text, self.hard_negatives)
-        _validate_negatives(text_features, extra_text, self.extra_texts, "extra_text", "extra_texts")
-        extra_ids = _validate_extra_text_ids(extra_text_ids, 0 if self.multi_label else self.extra_texts, text_features)
-        _validate_negatives(image_features, extra_image, self.extra_images, "extra_image", "extra_images", "images")
-        ximg_ids = _validate_extra_image_ids(extra_image_ids, self.extra_images, self.multi_positive, image_features)
-        weights = _weights_of(self.sample_weights, image_weights, text_weights, image_features, text_features,
-                              self.hard_negatives + self.extra_texts, self.extra_images)
-        groups = _groups_of(self.exclude_groups, image_groups, text_groups, image_features, text_features,
-                            self.hard_negatives + self.extra_texts, self.extra_images)
-        label_sets = _label_sets_of(self.multi_label, sample_labels, extra_text_labels, extra_image_labels,
-                                    image_features, self.extra_texts, self.extra_images)
-        _validate(image_features, text_features, None)
-        batch = image_features.shape[0]
-        text_features = _with_negatives(_with_negatives(text_features, negative_text), extra_text)
-        image_features = _with_negatives(image_features, extra_image)
-        image_features, text_features = _pad_dim(image_features), _pad_dim(text_features)
-        eng = self._cache.get(batch, image_features.shape[1], image_features.device,
-                              teacher[0].shape[1] if teacher is not None else 0)
-        topo = eng.topology
-        rank_world = (eng.rank, eng.world) if topo is None else (topo.rank, topo.world)
-        if rank_world != (self.rank, self.world_size):
-            raise RuntimeError(
-                f"SigLipLoss(rank={self.rank}, world_size={self.world_size}) does not match the process group "
-                f"(rank={rank_world[0]}, world_size={rank_world[1]})")
+        args = locals()
         if logit_bias is None:
             logit_bias = torch.zeros((), device=image_features.device)
-        rows = text_features.shape[0]
-        if topo is not None:
-            cross_node.check_forward(return_metrics)
-            text_features, logit_scale, logit_bias, extra_ids, weights, groups, label_sets = _node_step(
-                self, eng, text_features, logit_scale, logit_bias, False, ids, extra_ids, weights, groups, label_sets)
-        fused = _fused_under_budget(eng, self.fused_step)
-        bufs = _metric_buffers(eng.batch, eng.device, eng.metric_texts, eng.metric_images) if return_metrics else None
-        bufs = _topk_buffers(eng, topk, bufs)
-        lbufs = _sample_loss_buffers(eng) if return_sample_losses else None
-        loss = _SigmoidLossFn.apply(image_features, text_features, logit_scale, logit_bias, eng, False, fused, ids, bufs,
-                                    extra_ids, weights, ximg_ids, teacher, lbufs, groups, label_sets)
-        out = {"contrastive_loss": loss} if output_dict else loss
-        return _with_outputs(out, bufs, _fold_text_loss(eng, lbufs, rows))
+        loss, bufs, lbufs = _loss_forward(self, args, image_features, text_features, logit_scale, logit_bias, None,
+                                          False, False, (self.rank, self.world_size), _SIGLIP_TEACHER)
+        return _with_outputs({"contrastive_loss": loss} if output_dict else loss, bufs, lbufs)
