@@ -70,6 +70,7 @@ EXPORTED_SYMBOLS = (
     "siglip_debug_gemm",
     "siglip_debug_gemm_timed",
     "siglip_debug_max_active_clusters",
+    "siglip_debug_loss_max_active_clusters",
     "siglip_debug_loopback",
     "siglip_debug_set_text_chunk",
     "siglip_debug_get_slot",
@@ -301,6 +302,8 @@ def lib() -> ctypes.CDLL:
     L.siglip_debug_gemm_timed.restype = ci
     L.siglip_debug_max_active_clusters.argtypes = [ci, ci, ci, ci, ci]
     L.siglip_debug_max_active_clusters.restype = ci
+    L.siglip_debug_loss_max_active_clusters.argtypes = [ci, ci, ci, ci, ci]
+    L.siglip_debug_loss_max_active_clusters.restype = ci
     L.siglip_ctx_destroy.argtypes = [vp]
     L.siglip_ctx_destroy.restype = None
     _lib = L
@@ -319,6 +322,20 @@ def check(code: int) -> None:
 def max_active_clusters(cta_group: int, mcast: int, tile_n: int, stages: int = 0, device: int = 0) -> int:
     """Clusters of the persistent grid of a gradient-kernel launch on `device` (siglip_debug_max_active_clusters)."""
     n = lib().siglip_debug_max_active_clusters(device, cta_group, mcast, tile_n, stages)
+    if n < 0:
+        raise SiglipError(-n, last_error())
+    return n
+
+
+# the loss kernel's modes by number (csrc/siglip_kernels.cuh KernelMode)
+LOSS_MODES = {"loss": 0, "distill": 2, "sample_loss": 3, "topk": 4, "groups": 5, "labels": 6, "focal": 7,
+              "distill_opts": 8}
+
+
+def loss_max_active_clusters(mode: str, cta_group: int, mcast: int, stages: int = 0, device: int = 0) -> int:
+    """Clusters of the persistent grid of a loss-kernel launch of `mode` (a LOSS_MODES name) on `device`
+    (siglip_debug_loss_max_active_clusters)."""
+    n = lib().siglip_debug_loss_max_active_clusters(device, cta_group, mcast, LOSS_MODES[mode], stages)
     if n < 0:
         raise SiglipError(-n, last_error())
     return n

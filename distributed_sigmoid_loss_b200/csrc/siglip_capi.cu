@@ -3334,6 +3334,20 @@ int siglip_debug_max_active_clusters(int device, int cta_group, int mcast, int t
   return n;
 }
 
+int siglip_debug_loss_max_active_clusters(int device, int cta_group, int mcast, int mode, int stages) {
+  if (cta_group != 1 && cta_group != 2) return -fail(SIGLIP_ERR_INVALID, "cta_group must be 1 or 2");
+  if (mcast != 1 && mcast != 2) return -fail(SIGLIP_ERR_INVALID, "mcast must be 1 or 2");
+  if (mode < 0 || mode > siglip::kModeDistillOpts || mode == siglip::kModeOut)
+    return -fail(SIGLIP_ERR_INVALID, "mode must be a loss-kernel mode");
+  if (stages != 0 && stages != 4 && stages != 6) return -fail(SIGLIP_ERR_INVALID, "stages must be 0 (default), 4 or 6");
+  if (siglip_device_count() == 0) return -fail(SIGLIP_ERR_NO_DEVICE, "no sm_90 device; no CPU fallback");
+  if (cudaSetDevice(device) != cudaSuccess) return -fail(SIGLIP_ERR_CUDA, "cudaSetDevice failed");
+  const int n = siglip::query_loss_max_active_clusters(mode, siglip::cluster_size(cta_group, mcast),
+                                                       stages > 0 ? stages : siglip::default_stages(mode));
+  if (n < 1) return -fail(SIGLIP_ERR_CUDA, "cannot read the device's multiprocessor count");
+  return n;
+}
+
 int siglip_debug_gemm(int device, int cta_group, int M, int N, int K, const void* A, long long lda, int a_mn,
                       const void* Bm, long long ldb, int b_mn, float* C, long long ldc, void* cuda_stream) {
   return siglip_debug_gemm_timed(device, cta_group, M, N, K, A, lda, a_mn, Bm, ldb, b_mn, C, ldc, 1, nullptr,

@@ -2853,12 +2853,13 @@ int launch_impl(const CUtensorMap* tmA0, const CUtensorMap* tmB0, const CUtensor
 }  // namespace
 
 namespace {
-// The persistent grid's cluster count of one out-kernel instantiation, as launch_impl derives it: the runtime's
-// co-resident clusters (num_sms / kCS when the query fails), at most num_sms / kCS.
-template <int kStages, int kCS, int kTileNT = kTileN>
-int out_kernel_clusters(int num_sms) {
-  auto kern = siglip_gemm_kernel<kModeOut, kStages, kCS, false, false, false, false, kTileNT>;
-  const int smem = Cfg<kModeOut, kStages, kTileNT>::kSmemBytes;
+// The persistent grid's cluster count of one kernel instantiation, as launch_impl derives it: the runtime's
+// co-resident clusters (num_sms / kCS when the query fails), at most num_sms / kCS. kModeLoss's ids / metrics / weights
+// variants share one shared-memory size and one block of threads with its plain instantiation, which answers for them.
+template <int kMode, int kStages, int kCS, int kTileNT = kTileN>
+int kernel_clusters(int num_sms) {
+  auto kern = siglip_gemm_kernel<kMode, kStages, kCS, false, false, false, false, kTileNT>;
+  const int smem = Cfg<kMode, kStages, kTileNT>::kSmemBytes;
   cudaLaunchConfig_t cfg{};
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -2886,18 +2887,18 @@ int query_max_active_clusters(int cluster, int tile_n, int stages) {
       cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
     return -1;
   if (tile_n == kWideTileN) {   // every stage request maps to kWideStages, as in launch_gemm
-    if (cluster == 4) return out_kernel_clusters<kWideStages, 4, kWideTileN>(num_sms);
-    if (cluster == 2) return out_kernel_clusters<kWideStages, 2, kWideTileN>(num_sms);
-    return out_kernel_clusters<kWideStages, 1, kWideTileN>(num_sms);
+    if (cluster == 4) return kernel_clusters<kModeOut, kWideStages, 4, kWideTileN>(num_sms);
+    if (cluster == 2) return kernel_clusters<kModeOut, kWideStages, 2, kWideTileN>(num_sms);
+    return kernel_clusters<kModeOut, kWideStages, 1, kWideTileN>(num_sms);
   }
   if (stages == 4) {
-    if (cluster == 4) return out_kernel_clusters<4, 4>(num_sms);
-    if (cluster == 2) return out_kernel_clusters<4, 2>(num_sms);
-    return out_kernel_clusters<4, 1>(num_sms);
+    if (cluster == 4) return kernel_clusters<kModeOut, 4, 4>(num_sms);
+    if (cluster == 2) return kernel_clusters<kModeOut, 4, 2>(num_sms);
+    return kernel_clusters<kModeOut, 4, 1>(num_sms);
   }
-  if (cluster == 4) return out_kernel_clusters<6, 4>(num_sms);
-  if (cluster == 2) return out_kernel_clusters<6, 2>(num_sms);
-  return out_kernel_clusters<6, 1>(num_sms);
+  if (cluster == 4) return kernel_clusters<kModeOut, 6, 4>(num_sms);
+  if (cluster == 2) return kernel_clusters<kModeOut, 6, 2>(num_sms);
+  return kernel_clusters<kModeOut, 6, 1>(num_sms);
 }
 
 int default_stages(int /*mode*/) { return 6; }
@@ -3170,6 +3171,40 @@ static int launch_distill_opts(int cluster, const CUtensorMap* tmA0, const CUten
     case 4: return launch_impl<kModeDistillOpts, kDistillStages, 4>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
     case 2: return launch_impl<kModeDistillOpts, kDistillStages, 2>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
     default: return launch_impl<kModeDistillOpts, kDistillStages, 1>(tmA0, tmB0, tmA1, tmB1, tmG, p, num_sms, stream);
+  }
+}
+
+// The loss-kernel twin of query_max_active_clusters: the grid of a loss launch of `mode` before launch_impl caps it at
+// the launch's tiles. Defined last, behind launch_distill_opts, so that no kernel of the module moves.
+template <int kMode>
+static int loss_clusters(int cluster, int stages, int num_sms) {
+  constexpr int kS4 = teacher_mode(kMode) ? kDistillStages : 4;
+  constexpr int kS6 = teacher_mode(kMode) ? kDistillStages : 6;
+  if (stages == 4 || teacher_mode(kMode)) {
+    if (cluster == 4) return kernel_clusters<kMode, kS4, 4>(num_sms);
+    if (cluster == 2) return kernel_clusters<kMode, kS4, 2>(num_sms);
+    return kernel_clusters<kMode, kS4, 1>(num_sms);
+  }
+  if (cluster == 4) return kernel_clusters<kMode, kS6, 4>(num_sms);
+  if (cluster == 2) return kernel_clusters<kMode, kS6, 2>(num_sms);
+  return kernel_clusters<kMode, kS6, 1>(num_sms);
+}
+
+int query_loss_max_active_clusters(int mode, int cluster, int stages) {
+  int dev = 0, num_sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return -1;
+  switch (mode) {
+    case kModeLoss: return loss_clusters<kModeLoss>(cluster, stages, num_sms);
+    case kModeDistill: return loss_clusters<kModeDistill>(cluster, stages, num_sms);
+    case kModeSampleLoss: return loss_clusters<kModeSampleLoss>(cluster, stages, num_sms);
+    case kModeTopK: return loss_clusters<kModeTopK>(cluster, stages, num_sms);
+    case kModeGroups: return loss_clusters<kModeGroups>(cluster, stages, num_sms);
+    case kModeLabels: return loss_clusters<kModeLabels>(cluster, stages, num_sms);
+    case kModeFocal: return loss_clusters<kModeFocal>(cluster, stages, num_sms);
+    case kModeDistillOpts: return loss_clusters<kModeDistillOpts>(cluster, stages, num_sms);
+    default: return -2;
   }
 }
 

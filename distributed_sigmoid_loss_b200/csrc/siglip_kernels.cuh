@@ -260,6 +260,9 @@ int default_stages(int mode);
 // kWideTileCols) and `stages` (4, else 6; the wide tiles always have kWideStages): what launch_impl launches
 // (diagnostics and tests). -1 without a device.
 int query_max_active_clusters(int cluster, int tile_n = kTileCols, int stages = 6);
+// The same for the loss kernel of `mode` (kModeLoss or one of its twins; stages 4, else 6; the teacher modes always have
+// kDistillStages). -1 without a device, -2 for a mode that is not a loss mode.
+int query_loss_max_active_clusters(int mode, int cluster, int stages);
 
 // Launch the warp-specialised persistent kernel. `stages` <= 0 selects the default pipeline depth (4 or 6).
 // tmG: store map of the sigma operand (loss mode; 16-bit [B, B], box {32, 16}, 64B swizzle) — any valid map in out mode.

@@ -648,6 +648,13 @@ int siglip_debug_gemm(int device, int cta_group, int M, int N, int K, const void
  */
 int siglip_debug_max_active_clusters(int device, int cta_group, int mcast, int tile_n, int stages);
 
+/* Test hook: the same for the loss kernel of one mode (0 the plain loss kernel, whatever its ids, metrics and weights;
+ * 2 distillation, 3 per-sample losses, 4 top-K, 5 excluded groups, 6 label sets, 7 focal terms, 8 distillation with
+ * options) at SIGLIP_OPT_STAGES_LOSS stages = 0, 4 or 6 (the distillation modes always run 4): the clusters of its
+ * persistent grid before a launch caps them at its tiles. Returns the count, or minus the status code.
+ */
+int siglip_debug_loss_max_active_clusters(int device, int cta_group, int mcast, int mode, int stages);
+
 /* Same contraction launched `iters` times back to back (after one warm-up when iters > 1); *ms_per_iter receives
  * the CUDA-event time per launch. Used to tune the mainloop apart from the loss epilogue. */
 int siglip_debug_gemm_timed(int device, int cta_group, int M, int N, int K, const void* A, long long lda, int a_mn,

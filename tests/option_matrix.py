@@ -70,6 +70,14 @@ PANEL_SHAPES = {1: ((700,), (60,), (48,)), 2: ((600, 520), (40, 72), (24, 36)),
 # one rank with more than 960 images and texts: the gradient kernel's split-K splits (launch_impl cuts K into slices of
 # at least 8 k-blocks of 64), which the shapes above never reach (the step sequences' split-K steps run these)
 SPLIT_SHAPES = {1: ((1040,), (37,), (23,))}
+# the multi-tile family (MULTI, MULTI_COLD): every launch over a chunk with its extra texts runs several tiles per
+# cluster at every cluster size, on an H100 SXM's co-resident cluster counts (tests/tile_schedule.py). 17 520 texts are
+# 137 column blocks, more than the 132 clusters of size 1: consecutive tiles of a cluster keep their row block; 520
+# images are 5 row blocks, 3 row panels of 2 blocks (the last one a phantom) and 2 panels of 4 (three phantoms). At W = 2
+# the family runs rank 1, whose own chunk is narrow: its launches keep the wide chunk's grid (grid_n) and leave most
+# clusters without a tile. D = 136 and D_T = 72 make a tile 3 k-blocks, 5 with the teacher's: a multiple of neither 4
+# nor 6 stages.
+MULTI_SHAPES = {1: ((520,), (17000,), (40,)), 2: ((520, 520), (17000, 60), (40, 20))}
 
 
 @dataclass(frozen=True)
@@ -165,6 +173,7 @@ class Cell:
     seed: int
     cold: bool = False   # planted_cold's data: the series path's family
     splitk: bool = False  # SPLIT_SHAPES instead of SHAPES / PANEL_SHAPES
+    multi: bool = False   # MULTI_SHAPES: the multi-tile family
 
     @property
     def mode(self) -> str:
@@ -185,7 +194,7 @@ class Cell:
         return (f"{self.seed:03d}-{self.mode}-{o.context}-{'+'.join(on) or 'none'}-W{self.W}r{self.r}"
                 f"{'-bidir' if self.bidir else ''}-{self.sched}{'-panels' if self.panels else ''}"
                 f"{'-f16' if self.f16 else ''}-t{self.tile_n}-s{self.stages}-cg{self.cg}m{self.mcast}"
-                f"{'-cold' if self.cold else ''}{'-splitk' if self.splitk else ''}")
+                f"{'-cold' if self.cold else ''}{'-splitk' if self.splitk else ''}{'-multi' if self.multi else ''}")
 
     def shapes(self):
         """(Bs, Rs, Ts) of every rank, as the step sees them."""
@@ -219,7 +228,7 @@ class Cell:
 
 
 def shape_table(cell: Cell):
-    return SPLIT_SHAPES if cell.splitk else PANEL_SHAPES if cell.panels else SHAPES
+    return MULTI_SHAPES if cell.multi else SPLIT_SHAPES if cell.splitk else PANEL_SHAPES if cell.panels else SHAPES
 
 
 def _round_up(x, m):
@@ -379,10 +388,13 @@ def _lru_pick(order, ok):
     return v
 
 
-def build_table(cold: bool = False) -> List[Cell]:
+def build_table(cold: bool = False, multi: bool = False) -> List[Cell]:
     """The cells of every row of _mode_rows. cold: the same rows on planted_cold's data (seeds from COLD_SEED), without
     kModeDistill's rows for the other contexts: they run its branches again, and the cold family is the minimal cover of
-    the instantiations and runtime combinations."""
+    the instantiations and runtime combinations. multi: the multi-tile family on MULTI_SHAPES (seeds from MULTI_SEED),
+    every cell with extra texts (the wide chunk), at W = 1 and 2 without row panels, and only the rows that add an item
+    of multi_items to the rows before them and to the rows after them (the minimal cover of what the tile schedule has
+    to reach)."""
     cells, counters = [], {}
     for seed, (mode, f, stages, cs) in enumerate(_mode_rows()):
         j = counters.setdefault(mode, [0, {}])
@@ -392,14 +404,19 @@ def build_table(cold: bool = False) -> List[Cell]:
             continue
         ids = f.get("ids", False)
         sets = mode == "labels" or f.get("sets", False)
-        W = (1, 2, 3)[i % 3]
+        W = (1, 2)[i // 2 % 2] if multi else (1, 2, 3)[i % 3]
         # xt / xi: extras with ids or sets of their own; both at W = 1 under positional labels would run iota ids only
-        if mode == "distill":   # its runtime combinations without extras, then every other context once
+        # (which the multi-tile family wants of every mode with an ids option: every context of it has the wide chunk's
+        # extra texts; a kModeLoss row would run the kIds instantiation instead of its own)
+        if multi:
+            ctx = _lru_pick(cyc.setdefault("ctx", list(MULTI_CONTEXTS)),
+                            lambda c: ids or sets or (c != "xt" and not (c == "both" and W == 1 and mode == "loss")))
+        elif mode == "distill":   # its runtime combinations without extras, then every other context once
             ctx = "plain" if i < len(runtime_combos(mode)) else CONTEXTS[1 + i - len(runtime_combos(mode))]
         else:
             ctx = _lru_pick(cyc.setdefault("ctx", list(CONTEXTS)),
                             lambda c: (ids or sets or c not in ("xt", "xi")) and (ids or sets or W > 1 or c != "both"))
-        panels = i % 4 == 3
+        panels = i % 4 == 3 and not multi
         # the loss alone can move by less than 20x the tolerance when a label-set step has extras (the tag positives
         # raise it, the same-id positives lower it, and the extras' pairs are few) or a teacher's step has sets or
         # extras with ids (its soft targets): those cells check gradients too
@@ -426,14 +443,84 @@ def build_table(cold: bool = False) -> List[Cell]:
                     topk=(5 if mode == "topk" else 3 if f.get("topk") else
                           1 if metrics and mode in ("loss", "sample_loss") and i % 2 else 0))
         assert o.valid() and mode_of(o) == mode, o
-        cells.append(Cell(o, W, i % W, W > 1 and (i // 3) % 2 == 1, sched, panels, (i + i // 4) % 2 == 1,
-                          (128, 256)[(i // 2 + i // 8) % 2], stages, cg, mcast, seed + COLD_SEED * cold, cold))
-    return cells
+        cells.append(Cell(o, W, W - 1 if multi else i % W, W > 1 and (i // 3) % 2 == 1, sched, panels, (i + i // 4) % 2 == 1,
+                          (128, 256)[(i // 2 + i // 8) % 2], stages, cg, mcast,
+                          seed + COLD_SEED * cold + MULTI_SEED * multi, cold, multi=multi))
+    if not multi:
+        return cells
+    items = [multi_items(c) for c in cells]
+    keep, seen = [], set()
+    for k in range(len(cells)):   # forward: the rows that add something; backward: drop the ones the rest cover
+        if items[k] - seen:
+            keep.append(k)
+            seen |= items[k]
+    for k in reversed(list(keep)):
+        rest = set().union(*(items[j] for j in keep if j != k))
+        if items[k] <= rest:
+            keep.remove(k)
+    return [cells[k] for k in keep]
 
 
 COLD_SEED = 500
+MULTI_SEED = 1000
+MULTI_CONTEXTS = ("hn", "xt", "both")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the tile schedule of a cell's loss launches (tests/tile_schedule.py)
+# ---------------------------------------------------------------------------------------------------------------------
+def cell_launches(cell: Cell, clusters=None, num_sms: Optional[int] = None):
+    """(chunk_route, chunk, window, tile_schedule.Launch) of every loss launch of rank r's step (slab_paths.windows), on
+    clusters[(mode, stages, cluster size)] co-resident clusters of each instantiation and num_sms SMs (an H100 SXM's by
+    default). The
+    grid counts the step's widest chunk (grid_n = Tmax); a tile is D / 64 k-blocks, plus D_T / 64 under a teacher."""
+    import slab_paths
+    import tile_schedule as ts
+
+    Bs, Rs, Ts = cell.shapes()
+    r = cell.r
+    kb = ts.num_kb(D, DT if cell.opts.teacher else 0)
+    out = []
+    for c in range(cell.W):
+        rt = chunk_route(cell, c)
+        mode, stages, cs = rt[0][:3]
+        n = ts.H100_CLUSTERS[cs] if clusters is None else clusters[(mode, stages, cs)]
+        for win in slab_paths.windows(Rs[r], Bs[r], Ts[c], c == r, own_pos_ids(cell), cell.panel_rows()):
+            out.append((rt, c, win, ts.launch(win[1], win[3], cs, stages, kb, n, max(Ts), num_sms or ts.NUM_SMS)))
+    return out
+
+
+def multi_items(cell: Cell, clusters=None, num_sms: Optional[int] = None) -> set:
+    """What a cell's launches reach of the tile schedule: per instantiation a launch where some cluster runs 3 tiles or
+    more and the last wave is ragged ("waves"), and consecutive tiles that keep / change the row block, a tile that
+    starts mid-ring and one at phase 1; per mode every runtime option on in such a multi-wave launch (ids "iota" apart);
+    per cluster size > 1 a CTA that scores a real block and then a phantom, in a cluster that goes on after a phantom;
+    and at W > 1 chunks that give a cluster different tile counts (the grid_n grid)."""
+    out = set()
+    counts = {}
+    for (inst, rt), _, _, L in cell_launches(cell, clusters, num_sms):
+        mode = inst[0]
+        opts = dict(ids=inst[3], metrics=inst[4], weights=inst[5]) if mode == "loss" else dict(rt)
+        inst = tuple(bool(v) if k >= 3 else v for k, v in enumerate(inst))
+        if L.max_tiles() >= 3 and L.ragged():
+            out.add(("waves", inst))
+            out.update(("option", mode, k if v is True else f"{k}={v}") for k, v in opts.items() if v)
+        for what, ok in (("keep", L.keeps_row_block()), ("change", L.changes_row_block()), ("stage", L.mid_ring()),
+                         ("phase", L.phase_one())):
+            if ok:
+                out.add((what, inst))
+        if L.cs > 1 and L.phantom_after_real() and L.phantom_then_more():
+            out.add(("phantom", L.cs))
+        counts.setdefault(L.clusters, set()).add(tuple(len(x) for x in L.per_cluster))
+    if cell.W > 1 and any(len(v) > 1 for v in counts.values()):
+        out.add(("grid_n",))
+    return out
+
+
 TABLE = build_table()
 COLD = build_table(cold=True)
+MULTI = build_table(multi=True)
+MULTI_COLD = build_table(cold=True, multi=True)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -547,7 +634,15 @@ def planted(cell: Cell) -> Problem:
         P["ttags"].append(np.concatenate([ti[:b], tags(t_ - b)]))
         P["timgs"].append(np.concatenate([tnear(ids), tnear(xi_content)]))
         P["ttxts"].append(np.concatenate([tnear(ids), tnear(xt)]))
+    if cell.multi and cell.opts.topk > 1:
+        # rank r's first row block at 8x (integers, still exact): its rows' K-th best over any one tile lies above the
+        # top-K keys of the next row blocks, so a CTA whose next tile kept the previous rows' top-K floor would lose
+        # keys of its new rows' lists
+        P["imgs"][cell.r][:TOPK_FLOOR_ROWS] *= TOPK_FLOOR_SCALE
     return Problem(Bs, Rs, Ts, **P)
+
+
+TOPK_FLOOR_ROWS, TOPK_FLOOR_SCALE = 128, 8
 
 
 # Cold data: integer rows / 8, so U = 64 <img, txt> is an integer and z = 5 U / 64 - 6 (U < 23.04: z < kFastZ).

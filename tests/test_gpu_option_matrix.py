@@ -47,7 +47,10 @@ def _report():
 
 
 def _note(kind, err, tag=""):
-    kind = ("cold cells: " if tag.endswith("-cold") or "-cold " in tag else "") + kind
+    cold = tag.endswith("-cold") or "-cold " in tag or "-cold-" in tag
+    multi = tag.endswith("-multi") or "-multi " in tag
+    kind = ("multi-tile " if multi and cold else "") + ("cold cells: " if cold else "multi-tile cells: " if multi
+                                                          else "") + kind
     OBSERVED[kind] = max(OBSERVED.get(kind, 0.0), err)
 
 
@@ -303,7 +306,34 @@ def _run(cell, **variant):
     return RESULTS[key]
 
 
-@pytest.mark.parametrize("cell", om.TABLE + om.COLD, ids=lambda c: c.name)
+def test_coverage_holds_with_the_device_cluster_counts():
+    """The multi-tile families' coverage (test_option_matrix_cpu._multi_missing) derived again from this device's
+    co-resident clusters of every loss-kernel instantiation: if a count differs from an H100 SXM's and a cluster no
+    longer runs several tiles somewhere, this fails and names what is missing."""
+    from distributed_sigmoid_loss_b200 import _capi
+    from test_option_matrix_cpu import _multi_missing
+
+    props = torch.cuda.get_device_properties(0)
+    counts = {}
+    for mode in om.MODES:
+        for st in sorted({i[1] for i in om.instantiations(mode)}):
+            for cs, shapes in om.CLUSTERS.items():
+                got = {_capi.loss_max_active_clusters(mode, cg, mc, st) for cg, mc in shapes}
+                assert len(got) == 1, f"{mode} {st} stages: cluster shapes of {cs} CTAs differ: {got}"
+                counts[(mode, st, cs)] = got.pop()
+                assert 1 <= counts[(mode, st, cs)] <= props.multi_processor_count // cs
+    print(f"\n{props.name}, {props.multi_processor_count} SMs: co-resident clusters of the loss kernel "
+          "(mode, stages, cluster size)")
+    for k in sorted(counts):
+        print(f"  {k}: {counts[k]}")
+    with pytest.raises(_capi.SiglipError):   # mode 1 is the gradient kernel
+        _capi.check(-_capi.lib().siglip_debug_loss_max_active_clusters(0, 1, 1, 1, 6))
+    for name in ("MULTI", "MULTI_COLD"):
+        missing = _multi_missing(getattr(om, name), counts, props.multi_processor_count)
+        assert not missing, f"{name} with this device's cluster counts: " + "; ".join(missing)
+
+
+@pytest.mark.parametrize("cell", om.TABLE + om.COLD + om.MULTI + om.MULTI_COLD, ids=lambda c: c.name)
 def test_cell_matches_the_composed_oracle(cell):
     _run(cell)
 

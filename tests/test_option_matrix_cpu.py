@@ -4,7 +4,9 @@ but the focal terms; its reduction to the single-feature oracles; every cell's s
 the table's coverage of the loss kernel's instantiations and runtime branches; the table's modes against the loss modes
 launch_gemm dispatches to; the exactness of the planted logits; and the series path: the slab model of
 tests/slab_paths.py, the cold family's coverage of every instantiation and runtime combination in series slabs, and
-each cold cell's sensitivity to a bug local to its series slabs."""
+each cold cell's sensitivity to a bug local to its series slabs; the loss kernel's tile schedule (tests/tile_schedule.py),
+the multi-tile families' coverage of the state a CTA carries from one tile into the next, and each family's
+sensitivity to a leak of that state."""
 import dataclasses
 import functools
 import math
@@ -17,6 +19,7 @@ import torch
 
 import option_matrix as om
 import slab_paths as sp
+import tile_schedule as ts
 from distill_oracle import closed_form_distill
 from distill_options_oracle import closed_form_distill_options
 from exclude_groups_oracle import closed_form_groups, group_labels, torch_loss, torch_terms
@@ -702,3 +705,376 @@ def test_a_series_path_bug_moves_what_the_cell_checks(cell):
     if cell.opts.teacher and cell.sched == "fwd":
         weak = [w for w in weak if not w.startswith("INPUT_F16")]
     assert not weak, f"{cell.name}: a series-path bug moves its checked outputs by {weak} of the tolerance only"
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# several tiles per CTA: the tile schedule (tests/tile_schedule.py) and the multi-tile family
+# ---------------------------------------------------------------------------------------------------------------------
+def test_tile_schedule_by_hand():
+    """Schedules worked out by hand from launch_impl and decode_tile."""
+    # 300 x 640 at cluster size 1 on 4 clusters, 3 k-blocks, 4 stages: 3 x 5 tiles in row-panel order
+    L = ts.launch(300, 640, 1, 4, 3, 4)
+    assert (L.clusters, L.tiles_m, L.tiles_n) == (4, 3, 5)
+    assert L.per_cluster[0] == [ts.Tile(0, 0, 0, 0), ts.Tile(0, 4, 3, 0), ts.Tile(1, 3, 2, 1), ts.Tile(2, 2, 1, 0)]
+    assert [(t.mrow, t.n_blk) for t in L.per_cluster[3]] == [(0, 3), (1, 2), (2, 1)]
+    assert L.ragged() and L.max_tiles() == 4 and L.keeps_row_block() and L.changes_row_block()
+    assert L.mid_ring() and L.phase_one()
+    # 6 stages: the third tile starts at stage 0 again, on phase 1
+    assert [(t.stage, t.phase) for t in ts.launch(300, 640, 1, 6, 3, 4).per_cluster[0]] == [(0, 0), (3, 0), (0, 1),
+                                                                                           (3, 1)]
+    # a teacher tile of 2 + 3 k-blocks on 4 stages: the second tile starts at stage 1, phase 1
+    assert ts.num_kb(om.D, om.DT) == 5 and ts.num_kb(om.D) == 3
+    assert [(t.stage, t.phase) for t in ts.launch(128, 256, 1, 4, 5, 1).per_cluster[0]] == [(0, 0), (1, 1)]
+    # cluster size 2, 300 rows: row blocks 0 and 1, then 2 (rows 256..299) and 3, a phantom past row 300
+    L = ts.launch(300, 256, 2, 6, 3, 66)
+    assert (L.clusters, L.tiles_m, L.tiles_n) == (4, 2, 2) and L.max_tiles() == 1 and not L.ragged()
+    assert L.cta_tiles(2, 0) == [(2, 0, 0, 0, False)] and L.cta_tiles(2, 1) == [(3, 0, 0, 0, True)]
+    # on 3 clusters: cluster 0 runs tiles 0 and 3; its second CTA scores block 1, then the phantom block 3
+    L = ts.launch(300, 256, 2, 6, 3, 3)
+    assert L.cta_tiles(0, 1) == [(1, 0, 0, 0, False), (3, 1, 3, 0, True)]
+    assert L.phantom_after_real() and not L.phantom_then_more() and not L.phantom_before_real()
+    # the grid of the step's widest chunk: 8 clusters for a one-tile chunk, 7 of them without a tile
+    L = ts.launch(128, 128, 1, 6, 3, 132, grid_n=1000)
+    assert L.clusters == 8 and [len(x) for x in L.per_cluster] == [1] + [0] * 7
+    # at most num_sms / cluster size clusters, whatever the co-resident count says
+    assert ts.launch(4096, 4096, 4, 6, 3, 40).clusters == 33
+
+
+@pytest.mark.parametrize("rows,cols,cs", [(520, 17520, 1), (520, 17520, 2), (520, 17520, 4), (2100, 300, 4),
+                                          (1000, 5000, 2)])
+def test_a_phantom_block_is_never_followed_by_a_real_one(rows, cols, cs):
+    """The last row panel is the last in the tile order, so a CTA that scores a phantom block scores only phantom blocks
+    after it; what a phantom hands on is the ring position, to its own later phantoms and to its siblings' real tiles."""
+    L = ts.launch(rows, cols, cs, 4, 3, ts.H100_CLUSTERS[cs])
+    assert not L.phantom_before_real()
+    for c in range(L.clusters):
+        for k in range(cs):
+            ph = [x[4] for x in L.cta_tiles(c, k)]
+            assert ph == sorted(ph)
+
+
+def _multi_missing(families, clusters=None, num_sms=ts.NUM_SMS):
+    """What the families' launches do not reach of the tile schedule (om.multi_items), one line per kind, naming the
+    instantiations, modes and cluster sizes left out."""
+    items = set().union(*(om.multi_items(c, clusters, num_sms) for c in families))
+    need_i, _, _ = _required()
+    need_i = {tuple(bool(v) if k >= 3 else v for k, v in enumerate(i)) for i in need_i}
+    missing = []
+    for what, text in (("waves", "no cluster runs 3 tiles or more in a ragged last wave"),
+                       ("keep", "no cluster's consecutive tiles keep the row block"),
+                       ("change", "no cluster's consecutive tiles change the row block"),
+                       ("stage", "no tile starts mid-ring"), ("phase", "no tile starts at phase 1")):
+        lost = sorted(i for i in need_i if (what, i) not in items)
+        if lost:
+            missing.append(f"{text}: {lost}")
+    lost = [cs for cs in (2, 4) if ("phantom", cs) not in items]
+    if lost:
+        missing.append(f"no CTA scores a real block then a phantom, in a cluster that goes on, at cluster size {lost}")
+    need_o = {("option", m, o) for m in om.MODES for o in (["ids", "metrics", "weights"] if m == "loss" else
+                                                            om.runtime_options(m))}
+    need_o |= {("option", m, "ids=iota") for m in om.MODES if "ids" in om.runtime_options(m)}
+    need_o |= {("option", m, "extras_ctx") for m in ("distill", "distill_opts")}
+    lost = sorted(need_o - items)
+    if lost:
+        missing.append(f"runtime options never on in a multi-wave launch: {[x[1:] for x in lost]}")
+    if ("grid_n",) not in items:
+        missing.append("no cell at W > 1 whose chunks give a cluster different tile counts")
+    return missing
+
+
+@pytest.mark.parametrize("family", ["MULTI", "MULTI_COLD"])
+def test_multi_tile_family_reaches_the_cross_tile_state(family):
+    """With an H100 SXM's co-resident clusters (132, 66, 30), every loss-kernel instantiation runs, in a cell of the
+    family, a launch where some cluster scores 3 tiles or more and the last wave is ragged; consecutive tiles that keep
+    and that change the row block; a tile that starts mid-ring and one at phase 1. At cluster sizes 2 and 4 a CTA scores
+    a real block and then a phantom; every runtime option of every mode (iota ids and a teacher's extras context
+    included) is on in a multi-wave launch; and a cell at W = 2 has chunks that give a cluster different tile counts."""
+    missing = _multi_missing(getattr(om, family))
+    assert not missing, f"{family}: " + "; ".join(missing)
+
+
+def test_the_other_families_do_not_reach_it():
+    """The option matrix and the cold family never give a cluster a second tile: the multi-tile family is what does."""
+    for c in om.TABLE + om.COLD:
+        assert all(L.max_tiles() <= 1 for _, _, _, L in om.cell_launches(c)), c.name
+    assert len(_multi_missing(om.TABLE + om.COLD)) >= 6
+
+
+def test_no_multi_cell_is_redundant():
+    """Each cell of a family is the only one that reaches some item of om.multi_items, and the family does not repeat a
+    cell of the option matrix or the cold family."""
+    for fam in (om.MULTI, om.MULTI_COLD):
+        per = [om.multi_items(c) for c in fam]
+        for k, cell in enumerate(fam):
+            rest = set().union(*(per[:k] + per[k + 1:]))
+            assert per[k] - rest, f"{cell.name} reaches nothing no other cell of its family reaches"
+    names = [c.name for c in om.TABLE + om.COLD + om.MULTI + om.MULTI_COLD]
+    assert len(set(names)) == len(names)
+    for c in om.MULTI + om.MULTI_COLD:
+        assert c.opts.valid() and not c.panels and not (c.bidir and c.W == 1) and 0 <= c.r < c.W, c.name
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# a cross-tile leak moves what a multi-tile cell checks
+# ---------------------------------------------------------------------------------------------------------------------
+def _later_tiles(cell):
+    """(chunk, launch window, ordinal, previous (m_blk, n_blk), (m_blk, n_blk)) of every real tile after a CTA's first
+    in rank r's launches, global rows and the chunk's columns: what the CTA scored before it, and what it scores."""
+    out = []
+    for _, chunk, (r0, rows, c0, cols, own), L in om.cell_launches(cell):
+        for cl in range(L.clusters):
+            for k in range(L.cs):
+                t = L.cta_tiles(cl, k)
+                for j in range(1, len(t)):
+                    if not t[j][4]:
+                        out.append((chunk, (r0, rows, c0, cols), j, t[j - 1][:2], t[j][:2], L))
+    return out
+
+
+def _block(win, m, n, lo):
+    """Rows and global columns (lo: the chunks' offsets) of tile (m, n) of a launch window, clipped to the window."""
+    r0, rows, c0, cols = win
+    return (np.arange(m * 128, min(m * 128 + 128, rows)) + r0,
+            np.arange(n * 128, min(n * 128 + 128, cols)) + c0)
+
+
+def _leak_eval(cell, P, res):
+    """Rank r's checked outputs by float64 autograd of its pair terms, from the labels y [R_r, sum T], element weights
+    w, logits s and the teacher's p: a function of (y, w, s, p) overrides (None: the step's own)."""
+    o, r = cell.opts, cell.r
+    Bs, Rs, Ts, imgs, txts = P.view(o)
+    F = torch.nn.functional
+    txt = np.concatenate(txts)
+    y0 = np.concatenate(om.labels(P, o)[r], axis=1)
+    iw = P.iw[r][:Rs[r]].astype(np.float64) if o.weights else np.ones(Rs[r])
+    tw = np.concatenate([x[:n] for x, n in zip(P.tw, Ts)]).astype(np.float64) if o.weights else np.ones(len(txt))
+    w0 = iw[:, None] * tw[None, :]
+    s0 = imgs[r] @ txt.T
+    ts0 = None
+    if o.teacher:
+        timgs, ttxts = P.teacher(o)
+        ts0 = timgs[r] @ np.concatenate(ttxts).T
+    lo = np.cumsum([0] + list(Ts))
+    gamma, alpha = o.focal if o.focal else (0.0, None)
+
+    def evaluate(y=None, w=None, s=None, ts_=None, row_extra=None):
+        y = torch.from_numpy(y0 if y is None else y)
+        s = torch.tensor(s0 if s is None else s, dtype=torch.float64, requires_grad=True)
+        tp = torch.tensor(om.TP, dtype=torch.float64, requires_grad=True)
+        b = torch.tensor(om.BIAS, dtype=torch.float64, requires_grad=True)
+        z = torch.exp(tp) * s + b
+        wt = y.abs() * torch.from_numpy(w0 if w is None else w)
+        if o.focal is not None:
+            m = torch.where(y > 0, -z, z)
+            a = 1.0 if alpha is None else torch.where(y > 0, alpha, 1.0 - alpha).to(z.dtype)
+            terms = wt * a * torch.exp(-gamma * F.softplus(-m)) * F.softplus(m)
+        elif o.teacher:
+            p = torch.sigmoid(math.exp(om.TTP) * torch.from_numpy(ts0 if ts_ is None else ts_) + om.TBIAS)
+            terms = wt * (F.softplus(z) - ((1.0 - om.LAM) * (y > 0).double() + om.LAM * p) * z)
+        else:
+            terms = wt * F.softplus(-torch.where(y == 0, -torch.ones_like(y), y) * z)
+        loss = terms.sum() / Bs[r]
+        gs, gt, gb = torch.autograd.grad(loss, [s, tp, b])
+        gs = gs.numpy()
+        out = {"loss": loss.item(), "dimg": gs @ txt, "dt_prime": float(gt), "dbias": float(gb)}
+        out.update({f"contrib{c}": gs[:, lo[c]:lo[c + 1]].T @ imgs[r] for c in range(cell.W)})
+        t = terms.detach().numpy()
+        out["image_loss"] = t.sum(axis=1) + (0 if row_extra is None else row_extra)
+        out["text_loss"] = res[r]["text_loss"] - res[r]["text_part"][r] + t[:, lo[r]:lo[r + 1]].sum(axis=0)
+        return out, t
+
+    return evaluate, y0, w0, s0, ts0, lo
+
+
+def _row_swap(cell, lo, y0):
+    """(rows, columns, previous rows) of every later tile whose row block differs from the CTA's previous one."""
+    out = []
+    for chunk, win, j, prev, cur, L in _later_tiles(cell):
+        if prev[0] != cur[0]:
+            rows, cols = _block(win, *cur, 0)
+            prow = np.arange(len(rows)) + prev[0] * 128 + win[0]
+            out.append((rows, cols + lo[chunk], prow))
+    return out
+
+
+def _leak_applies(cell, leak):
+    """The cell has what the leak touches: row-side labels (ids, sets, groups, iota ids), weights, per-sample losses,
+    a teacher."""
+    o = cell.opts
+    return {"row labels": o.ids or o.labels or o.groups or om.own_pos_ids(cell), "row weights": o.weights,
+            "row partials": o.losses, "student k-block": True, "teacher k-block": o.teacher}[leak]
+
+
+def _leak_moves(cell, leak):
+    """How far the leak moves the cell's checked outputs, in units of the tolerance (_moved)."""
+    o = cell.opts
+    P = om.planted(cell)
+    res = om.oracle(P, o)
+    evaluate, y0, w0, s0, ts0, lo = _leak_eval(cell, P, res)
+    checked = list(_outputs(cell, res, cell.r))
+    full, terms = evaluate()
+    for k in ("loss", "dimg", "dt_prime", "dbias", "image_loss", "text_loss"):
+        assert om.rel(full[k], res[cell.r][k]) < 1e-10, k
+    Bs, Rs, Ts = cell.shapes()
+    own = np.zeros_like(y0, bool)   # the own chunk's positional positives: geometry, not a row-side value
+    if not om.own_pos_ids(cell):
+        i = np.arange(Bs[cell.r])
+        own[i, lo[cell.r] + i] = True
+    if leak == "row labels":   # ids, sets and groups of the previous row block
+        y = y0.copy()
+        for rows, cols, prow in _row_swap(cell, lo, y0):
+            y[np.ix_(rows, cols)] = np.where(own[np.ix_(rows, cols)], y0[np.ix_(rows, cols)], y0[np.ix_(prow, cols)])
+        got, _ = evaluate(y=y)
+    elif leak == "row weights":
+        w = w0.copy()
+        for rows, cols, prow in _row_swap(cell, lo, y0):
+            w[np.ix_(rows, cols)] = w0[np.ix_(prow, cols)]
+        got, _ = evaluate(w=w)
+    elif leak == "row partials":   # a tile's row sums start from the previous tile's
+        extra = np.zeros(Rs[cell.r])
+        for chunk, win, j, prev, cur, L in _later_tiles(cell):
+            rows, cols = _block(win, *cur, 0)
+            prows, pcols = _block(win, *prev, 0)
+            part = np.zeros(len(rows))
+            if prev[0] * 128 + win[0] < win[0] + win[1]:
+                n = min(len(rows), len(prows))
+                part[:n] = terms[np.ix_(prows[:n], pcols + lo[chunk])].sum(axis=1)
+            extra[rows] += part
+        got, _ = evaluate(row_extra=extra)
+    else:   # a stale k-block: the first k-block of the student's (or the teacher's) pass in one later tile
+        return _stale_kblock(cell, P, evaluate, checked, full, s0, ts0, lo, leak == "teacher k-block")
+    return max(_moved(cell, k, got[k], full[k]) for k in checked)
+
+
+def _stale_kblock(cell, P, evaluate, checked, full, s0, ts0, lo, teacher):
+    """The largest move over a few later tiles (those with the most positives) of reading, in place of the pass's first
+    k-block, what the same stage held one ring lap before (tile_schedule: ring position j kb - stages)."""
+    o, r = cell.opts, cell.r
+    Bs, Rs, Ts, imgs, txts = P.view(o)
+    timgs, ttxts = P.teacher(o) if o.teacher else (None, None)
+    kbt = ts.num_kb(om.DT) if o.teacher else 0
+    y = np.concatenate(om.labels(P, o)[r], axis=1)
+    # a later tile whose pass starts at least one ring lap in: its stage then holds an earlier k-block of the CTA
+    cands = [x for x in _later_tiles(cell) if x[2] * x[5].num_kb + (0 if teacher else kbt) >= x[5].stages]
+    cands.sort(key=lambda x: -int((y[np.ix_(*_block(x[1], *x[4], lo[x[0]]))] > 0).sum()))
+    best = 0.0
+    for chunk, win, j, prev, cur, L in cands[:3]:
+        g = j * L.num_kb + (0 if teacher else kbt)
+        gp = g - L.stages
+        assert gp >= 0
+        jp, kp = gp // L.num_kb, gp % L.num_kb
+        cl = next(c for c in range(L.clusters) for k in range(L.cs)
+                  if len(L.cta_tiles(c, k)) > j and L.cta_tiles(c, k)[j][:2] == cur and L.cta_tiles(c, k)[j - 1][:2] == prev)
+        crank = next(k for k in range(L.cs) if L.cta_tiles(cl, k)[j][:2] == cur)
+        src = L.cta_tiles(cl, crank)[jp][:2]
+
+        def operands(tile, k, as_teacher):
+            rows = np.arange(tile[0] * 128, tile[0] * 128 + 128) + win[0]
+            cols = np.arange(tile[1] * 128, tile[1] * 128 + 128) + win[2]
+            A = (timgs[r] if as_teacher else imgs[r])
+            B = (ttxts[chunk] if as_teacher else txts[chunk])
+            a, bm = np.zeros((128, 64)), np.zeros((128, 64))
+            rr, cc = rows[rows < win[0] + win[1]], cols[cols < win[2] + win[3]]
+            ks = slice(k * 64, k * 64 + 64)
+            a[:len(rr), :A[:, ks].shape[1]] = A[rr, ks]
+            bm[:len(cc), :B[:, ks].shape[1]] = B[cc, ks]
+            return a @ bm.T, len(rr), len(cc)
+
+        cur_prod, nr, nc = operands(cur, 0, teacher)
+        src_prod, _, _ = operands(src, kp if kp < kbt else kp - kbt, kp < kbt)
+        rows, cols = _block(win, *cur, lo[chunk])
+        delta = (src_prod - cur_prod)[:nr, :nc]
+        if teacher:
+            t2 = ts0.copy()
+            t2[np.ix_(rows, cols)] += delta
+            got, _ = evaluate(ts_=t2)
+        else:
+            s2 = s0.copy()
+            s2[np.ix_(rows, cols)] += delta
+            got, _ = evaluate(s=s2)
+        best = max(best, max(_moved(cell, k, got[k], full[k]) for k in checked))
+    return best
+
+
+LEAKS = ("row labels", "row weights", "row partials", "student k-block", "teacher k-block")
+
+
+@pytest.mark.parametrize("leak", LEAKS)
+@pytest.mark.parametrize("mode", om.MODES)
+def test_a_cross_tile_leak_moves_what_a_multi_tile_cell_checks(mode, leak):
+    """For each leak from one tile of a CTA into its next that the tile schedule allows, some multi-tile cell of each
+    mode the leak applies to moves an output the GPU test checks by more than 20x its tolerance: a tile that labels its
+    rows with the previous row block's ids, sets and groups (the own positional positives stay: geometry), or weights
+    them with its weights; per-sample row sums that start from the previous tile's; and one k-block of one tile (the
+    student's first, or the teacher's) that reads what its stage held one ring lap before."""
+    cells = sorted([c for c in om.MULTI if c.mode == mode and _leak_applies(c, leak)], key=lambda c: c.W)
+    if not cells:
+        pytest.skip(f"no {mode} cell has what the leak touches")
+    moved = {}
+    for cell in cells[:3]:
+        moved[cell.name] = _leak_moves(cell, leak)
+        if moved[cell.name] > 20:
+            return
+    pytest.fail(f"{mode}: a {leak} leak moves its cells' checked outputs by {moved} of the tolerance only")
+
+
+
+@pytest.mark.parametrize("mode", [m for m in om.MODES if m == "topk" or "topk" in om.runtime_options(m)])
+def test_a_stale_topk_floor_changes_a_multi_tile_cells_lists(mode):
+    """A tile that keeps the top-K floor of the CTA's previous row block offers only the keys above the previous rows'
+    floor. That floor is at least the previous row's K-th best over the previous tile (a list holds the top K of every
+    key offered so far), so a row whose top-K list holds a key of this tile below that bound loses it whatever the
+    stale floor was, and the GPU test compares the lists exactly. The top-K cells of the family scale rank r's first
+    row block (om.TOPK_FLOOR_SCALE): the CTAs that move on from it carry a floor above their new rows' lists."""
+    cells = sorted([c for c in om.MULTI if c.mode == mode and c.opts.topk > 1], key=lambda c: c.W)
+    assert cells
+    lost = {}
+    for cell in cells[:3]:
+        o, r = cell.opts, cell.r
+        P = om.planted(cell)
+        Bs, Rs, Ts, imgs, txts = P.view(o)
+        S = imgs[r] @ np.concatenate(txts).T
+        lo = np.cumsum([0] + list(Ts))
+        lists = om.retrieval(P, o, o.topk)[r]["i2t_topk"]
+        rows_hit = set()
+        for chunk, win, j, prev, cur, L in _later_tiles(cell):
+            if prev[0] == cur[0]:
+                continue
+            rows, cols = _block(win, *cur, lo[chunk])
+            prows, pcols = _block(win, *prev, lo[chunk])
+            for k, i in enumerate(rows):
+                if i >= len(lists) or k >= len(prows) or len(pcols) < o.topk:
+                    continue
+                floor = np.sort(S[prows[k], pcols])[::-1][o.topk - 1]
+                if any(S[i, g] < floor for g in lists[i] if cols[0] <= g <= cols[-1]):
+                    rows_hit.add(int(i))
+        lost[cell.name] = len(rows_hit)
+        if rows_hit:
+            return
+    pytest.fail(f"{mode}: a stale top-K floor changes no row's list: {lost}")
+
+
+def test_cold_multi_tile_cells_run_both_paths_on_later_tiles():
+    """In a cold multi-tile cell of every mode, the tiles after a CTA's first hold series slabs and general slabs off
+    the diagonal (slab_paths): both epilogue paths run on state carried from an earlier tile."""
+    seen = {}
+    for mode in om.MODES:
+        for cell in [c for c in om.MULTI_COLD if c.mode == mode][:2]:
+            later = {}
+            for chunk, win, j, prev, cur, L in _later_tiles(cell):
+                later.setdefault((chunk, win), set()).add(cur)
+            n = np.zeros(2, int)
+            for _, m in _slabs(cell):
+                tiles = later.get((m.chunk, (m.r0, m.rows, m.c0, m.cols)), set())
+                if not tiles:
+                    continue
+                nb, nc = m.cls.shape
+                t = np.zeros((nb, nc), bool)
+                for mb, cb in tiles:
+                    t[mb * 8:mb * 8 + 8, cb * 4:cb * 4 + 4] = True
+                n += [int((t & _student_series(cell, m)).sum()), int((t & (m.cls == sp.FREE) & ~m.series).sum())]
+            seen[cell.name] = tuple(n)
+            if n.all():
+                break
+        else:
+            pytest.fail(f"{mode}: no cold multi-tile cell runs both paths on later tiles: {seen}")
